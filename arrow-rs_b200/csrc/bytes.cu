@@ -503,7 +503,7 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const Byte
 // ---- dictionary gather: take_bytes from a SMALL source (Dictionary<Int32,Utf8> -> Utf8, cast/dictionary.rs:310-317) ----
 // A gather of 32 random dictionary rows through global memory costs 32 L1 wavefronts per load instruction whatever its
 // width (one 128-byte line per lane): with two offset loads and the value bytes per row that alone is ~5 cycles per row
-// per SM, i.e. the 1.4 ms the generic kernels need for 1e8 rows. Here the dictionary is first re-laid out as a table of
+// per SM. Here the dictionary is first re-laid out as a table of
 // 16-byte zero-padded entries + one length byte per entry (k_dict_table; sources with an entry longer than 16 bytes keep
 // the generic path) and every CTA keeps that table in shared memory (D x 17 bytes: 70 KB for D = 4096): the gathers become
 // LDS.128 / LDS.U8.
@@ -515,8 +515,7 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const Byte
 //     the output's 16-byte alignment) by funnel shifts + predicated ATOMS.OR; the image leaves as coalesced 128-bit stores
 //     (only the first / last chunk of a CTA, shared with its neighbours, is written bytewise) and is re-zeroed on the way.
 //     All positions inside a round are 32-bit. The first version of this path (warp-private rings, 64-bit positions,
-//     bytewise head / tail per warp) needed 1047 warp instructions per 128 rows and was issue-bound (ncu: 67 % issue
-//     slots busy, 1.07 ms per 1e8 rows, profiles/r02_dict_notes.md).
+//     bytewise head / tail per warp) was issue-bound.
 #define DG_THREADS 512
 #define DG_WARPS (DG_THREADS / 32)
 #define DG_WROWS (BY_ROWS / DG_WARPS)   // 128 rows per warp and round
@@ -624,8 +623,7 @@ __device__ __forceinline__ void red_or(uint32_t saddr, uint32_t x) {
 
 // pass 2: new offsets + bytes. A CTA round is a dependent chain (keys -> lengths -> scan -> barrier -> image -> barrier ->
 // flush -> barrier) with only two CTAs per SM, so the NEXT round's keys, validity words and base offset are loaded at the
-// top of the current round (software prefetch): without it every round exposes a full DRAM latency (measured 0.78 ms vs
-// profiles/r02_dict_notes.md for 1e8 rows).
+// top of the current round (software prefetch): without it every round exposes a full DRAM latency.
 struct DictRound {
   uint32_t key[DG_ITERS];  // raw keys (~0 for rows past the end)
   uint32_t vw;             // lane i < 4: validity word of the warp's i-th 32-row group (all ones without a bitmap)

@@ -1,4 +1,4 @@
-// common.cuh — shared device/host helpers for the sm_100a arrow::compute kernels.
+// common.cuh — shared device/host helpers for the sm_90a arrow::compute kernels.
 //
 // Layout conventions (arrow-buffer, see include/arrow_cuda.h): LSB-first bitmaps with an
 // arbitrary bit offset on INPUT, bit offset 0 and whole-u64-word stores on OUTPUT.
@@ -166,8 +166,8 @@ static inline int acu_wave_grid(acu_ctx *ctx, K kernel, int block, size_t smem, 
   } else {
     per_sm = it->second;
   }
-  // 8 waves of CTAs: the hardware scheduler evens out per-SM imbalance (+3.5 % on the streaming
-  // add vs exactly one wave, tools/arith_sweep.cu)
+  // 8 waves of CTAs: the hardware scheduler evens out per-SM imbalance (tools/arith_sweep.cu compares
+  // waves and occupancy points on the streaming add)
   return acu_grid(ctx, work_blocks, per_sm * 8);
 }
 

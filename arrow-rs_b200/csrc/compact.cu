@@ -406,8 +406,7 @@ __global__ void __launch_bounds__(256, 6) k_filter_values_async(const FilterBatc
 
 // ---- one-pass filter: values + validity in the same kernel ---------------------------------
 // k_filter_fused<W>: the value compaction of k_filter_values_async with (a) the mask / rank bookkeeping strength-reduced
-// to 32-bit operations on lane-constant positions (the round-1 kernel was ISSUE-bound: 75 % issue-active, 0.77 warp
-// instructions per row; a lane's selection bits of a whole pass are packed into one register at issue time and reused
+// to 32-bit operations on lane-constant positions (the older value kernel was issue-bound; a lane's selection bits of a whole pass are packed into one register at issue time and reused
 // by the consume phase) and (b) FilterPredicate::filter_nulls (filter.rs:512-533) fused in: the warp that owns a 1024-row tile already holds the
 // tile's 16 mask words and their popcount prefix, so lanes 0..15 PEXT the source validity words with them, the bits are
 // assembled in a warp-private shared-memory window and leave as whole 32-bit words (atomicOr only on the two words a
@@ -754,7 +753,7 @@ CompressArgs compress_args(const acu_filter_plan *plan, const uint8_t *src, int6
 
 // The one-pass kernel (k_filter_fused: values + validity) is used for 16-byte aligned value buffers unless the predicate is
 // very sparse (< 4 % selected: almost no value bytes move, the per-tile validity work dominates and the round-1 pair
-// k_filter_values_async + k_compress_bits is ~20 % faster — measured, profiles/r02_filter_ab.md). ACU_FILTER_LEGACY=1 forces
+// k_filter_values_async + k_compress_bits is faster there). ACU_FILTER_LEGACY=1 forces
 // the round-1 kernels for A/B measurements.
 bool plan_uses_fused(const acu_filter_plan *plan) {
   static const bool legacy = getenv("ACU_FILTER_LEGACY") != nullptr;

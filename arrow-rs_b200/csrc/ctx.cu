@@ -229,8 +229,8 @@ acu_status acu_ctx_create(int32_t device, acu_ctx **out) {
     cudaMemPoolSetAttribute(pool, cudaMemPoolAttrReleaseThreshold, &thr);
   }
   // L2 fill granularity. Sparse kernels (filter at low selectivity, take) only need the 32-B
-  // sectors they touch; the default granularity fills whole 128-B lines from HBM (measured with
-  // ncu: dram__bytes_read = 81.5 % of the column at 10 % selectivity = 1 - 0.9^16).
+  // sectors they touch; the default granularity fills whole 128-B lines from HBM (at 10 % selectivity
+  // a 128-B line of 8-B values holds a selected row with probability 1 - 0.9^16 = 81.5 %).
   // ACU_L2_FETCH_GRANULARITY=32|64|128 overrides (tuning knob).
   {
     size_t gran = 32;

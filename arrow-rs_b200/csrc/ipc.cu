@@ -5,7 +5,7 @@
 // end), RecordBatchDecoder::create_primitive_array (:264-297: validity buffer used only when null_count > 0), and the
 // flatbuffers tables of arrow-ipc/src/gen/{Message,Schema}.rs (vtable slots cited below).
 //
-// B200 design: the reference copies every IPC buffer into its own host allocation; here a RecordBatch message costs ONE
+// Design: the reference copies every IPC buffer into its own host allocation; here a RecordBatch message costs ONE
 // host->device copy of its whole body, and the columns handed to the kernels are *views* into that device buffer (IPC
 // body buffers are 8-byte aligned and already in Arrow layout: values, LSB-first bitmaps, offsets — nothing to re-lay
 // out). The metadata (a few hundred bytes of flatbuffers) is walked on the host by the small reader below; no flatbuffers

@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py — Mrows/s of the arrow::compute hot path (filter + take + add) on B200.
+"""bench.py — Mrows/s of the arrow::compute hot path (filter + take + add) on H100.
 
 One "step" = one pass of the hot path over one synthetic 1e9-row table per GPU
 (BASELINE.json configs[1] + configs[2] shapes):
@@ -58,7 +58,7 @@ SELECTIVITY, NULL_DENSITY = 0.10, 0.05
 def so_sha16():
     """Identity of the kernel build: sha256 over the kernel SOURCES (csrc/*.cu, *.cuh, Makefile, the C header), in name order.
     (nvcc's output is not bit-reproducible from one build to the next, so the binary's own hash would call a clean rebuild of
-    the same sources a different build.) tools/gpu_profiles.sh records the same value beside every ncu capture."""
+    the same sources a different build.) A profiles/rNN_traffic.json capture records the same value as its so_sha16."""
     import glob
     import hashlib
     h = hashlib.sha256()
@@ -110,7 +110,7 @@ def peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "fallback (H100 SXM data sheet 3.35 TB/s)"
 
 
 class ClockSampler:
@@ -293,6 +293,68 @@ def gpu_checksums(ctx, abi, wl):
     return {"filter_rows": int(wl.out_filter.len), "filter_nulls": nulls(wl.out_filter), "filter_values_wsum": wsum(wl.out_filter),
             "take_nulls": nulls(wl.out_take), "take_values_wsum": wsum(wl.out_take), "add_nulls": nulls(wl.out_add),
             "add_bits_wsum": wsum(wl.out_add), "sum_valid_rows": int(cnt), "sum_bits": int(bits), "valid_rows": int(cnt)}
+
+
+DUMP_SAMPLE_ROWS = 1 << 19  # rows kept per output column: (2 x (8 + 16 + 4) + (8 + 8 + 4)) B x 2^19 = 38 MiB, under the 64 MB cap
+DUMP_CHUNK_ROWS = 1 << 24
+
+
+def sample_rows(n, seed):
+    """Ascending positions of a fixed, seeded sample of DUMP_SAMPLE_ROWS of n rows (every row when n is smaller)."""
+    if n <= DUMP_SAMPLE_ROWS:
+        return np.arange(n, dtype=np.int64)
+    return np.sort(np.random.default_rng(seed).choice(n, DUMP_SAMPLE_ROWS, replace=False)).astype(np.int64)
+
+
+def gather_device(ctx, dptr, width, pos):
+    """Elements `pos` (ascending) of a device buffer of `width`-byte elements, copied in chunks so that a
+    1e9-row column never needs a host copy of its own size."""
+    dt = np.dtype(f"u{width}")
+    out = np.empty(len(pos), dtype=dt)
+    i = 0
+    while i < len(pos):
+        lo = int(pos[i])
+        j = int(np.searchsorted(pos, lo + DUMP_CHUNK_ROWS))
+        buf = ctx.d2h(dptr + lo * width, (int(pos[j - 1]) + 1 - lo) * width, dt)
+        out[i:j] = buf[pos[i:j] - lo]
+        i = j
+    return out
+
+
+def int64_halves(v):
+    """An Int64 array as two float64 arrays that hold it exactly: the signed high 32 bits and the unsigned low 32 bits."""
+    v = np.asarray(v, dtype=np.int64)
+    return (v >> 32).astype(np.float64), (v & 0xFFFFFFFF).astype(np.float64)
+
+
+def dump_outputs(ctx, wl, total_bits, total_cnt, out_dir):
+    """What the last timed step handed its caller: the filter, take and add output columns and the sum.
+    For every column, at the positions <name>_rows (a seeded sample, the same on every run), <name>_valid holds the
+    validity as float32 (1 = valid) and the values are float64 with 0 where the slot is null (what lies under a null is
+    unspecified, and every array stays finite): add_values for the Float64 column; for the Int64 columns
+    <name>_values_hi / <name>_values_lo, the signed high and unsigned low 32 bits, so that they compare bit-exactly.
+    sum.npy = [high 32 bits, low 32 bits of the wrapping Int64 sum of the taken column, its valid-row count]."""
+    os.makedirs(out_dir, exist_ok=True)
+    arrays = {}
+    for name, out, dtype, seed in (("filter", wl.out_filter, np.int64, 1), ("take", wl.out_take, np.int64, 1), ("add", wl.out_add, np.float64, 2)):
+        pos = sample_rows(int(out.len), seed)
+        vals = gather_device(ctx, out.values, 8, pos).view(dtype).copy()
+        if out.has_validity:
+            bits = gather_device(ctx, out.validity, 1, pos >> 3)
+            valid = ((bits >> (pos & 7).astype(np.uint8)) & 1).astype(bool)
+        else:
+            valid = np.ones(len(pos), dtype=bool)
+        vals[~valid] = 0
+        arrays[f"{name}_rows"] = pos.astype(np.float64)
+        if dtype == np.int64:
+            arrays[f"{name}_values_hi"], arrays[f"{name}_values_lo"] = int64_halves(vals)
+        else:
+            arrays[f"{name}_values"] = vals
+        arrays[f"{name}_valid"] = valid.astype(np.float32)
+    hi, lo = int64_halves(np.array([total_bits], np.uint64).view(np.int64))
+    arrays["sum"] = np.array([hi[0], lo[0], total_cnt], dtype=np.float64)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), a)
 
 
 ALLREDUCE_WALL = [0.0, 0]  # host seconds spent inside the final-reduce call (includes waiting for the slowest rank), calls
@@ -525,8 +587,8 @@ class HostPipelined:
 
 def numa_bind(gpu_index):
     """Default for the e2e arm (ACU_BENCH_NUMA=0 disables): run this rank's host threads, and therefore allocate / first-touch
-    its pinned buffers, on the CPUs NVML reports as local to the GPU (round 1: 8 unbound ranks reached 0.41 of 8 x the
-    one-GPU e2e rate — half the GPUs streamed from the remote socket's memory). Returns the previous affinity (to restore) or
+    its pinned buffers, on the CPUs NVML reports as local to the GPU (unbound ranks stream half their data from the remote
+    socket's memory). Returns the previous affinity (to restore) or
     None when nothing was changed."""
     try:
         before = os.sched_getaffinity(0)
@@ -625,6 +687,8 @@ def run_gpu(args):
         if cnt.value:
             kstats[name] = {"ms_per_step": tot.value / args.steps, "launches_per_step": cnt.value / args.steps,
                             "share_of_step": tot.value / ms.value}
+    if args.dump_outputs and rank == 0:
+        dump_outputs(ctx, wl, total_bits, total_cnt, args.dump_outputs)
 
     # ---- e2e: host buffers, copies inside the timed region --------------------------------
     e2e = None
@@ -691,7 +755,7 @@ def run_gpu(args):
         "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "i64 (filter/take/sum) + f64 (add)", "data": "synthetic",
         "config": {"workload": WORKLOAD, "rows_per_gpu": n, "parallelism": f"row-range shards x{world}, NCCL all-reduce of the sum only",
-                   "l2": "inputs >> L2 (126 MB): no flush needed", "input_residency": "HBM"},
+                   "l2": "inputs >> L2 (50 MB): no flush needed", "input_residency": "HBM"},
         "selected_rows": wl.m,
         "roofline": {"bound": "hbm", "kernel": "k_arith<double> (Float64 add, fused validity AND + popcount)",
                      "achieved": dom.get("achieved_gbs"), "peak": peak, "unit": "GB/s", "frac": dom.get("frac"),
@@ -793,11 +857,12 @@ def config_subresults(ctx, abi, wl, args, peak, traffic):
                                                   "traffic": None}
     except Exception as e:  # sub-results never take the headline down
         out["error"] = repr(e)[:300]
-    # config #5: RecordBatch pipeline (tools/recordbatch_bench.py body), one GPU's share: 15 x 2^26-row 8-column batches
+    # config #5: RecordBatch pipeline (tools/recordbatch_bench.py body), one GPU's share: 6 x 2^26-row 8-column batches
+    # (about 5 GB of HBM per batch: six of them fit an 80 GB H100 beside the resident 1e9-row headline table)
     try:
         if n >= 1_000_000_000:
             import recordbatch_bench as rbb
-            tb = rbb.Table(ctx, abi, 0, 15, 1 << 26, SELECTIVITY, NULL_DENSITY)
+            tb = rbb.Table(ctx, abi, 0, rbb.BATCHES, 1 << 26, SELECTIVITY, NULL_DENSITY)
             import acu
             # extra lanes (ctx + stream + host thread each): the host gaps of one lane overlap the kernels of the others
             extra = [acu.Context(ctx.device) for _ in range(max(int(os.environ.get("ACU_RB_STREAMS", "3")), 1) - 1)]
@@ -829,12 +894,12 @@ def config_subresults(ctx, abi, wl, args, peak, traffic):
                     kcls[abi.KERNEL_CLASS_NAMES[cls]] = round(ms_c, 3)
             for c in extra:
                 c.close()
-            rows = 15 * (1 << 26)
+            rows = rbb.BATCHES * (1 << 26)
             out["cfg5"] = {"filter_record_batch -> take_record_batch -> 6 sums": {
                 "rows": rows, "ms_per_step": step_ms, "kernel_ms": ksum, "kernel_ms_by_class": kcls, "algorithmic_bytes": alg, "achieved_gbs": alg / (step_ms * 1e-3) / 1e9,
                 "frac": alg / (step_ms * 1e-3) / 1e9 / peak, "mrows_s": rows / (step_ms * 1e-3) / 1e6, "traffic": None,
                 "streams": len(lanes), "timer": "host clock around steps bracketed by a synchronisation of every stream",
-                "note": "one GPU's share of BASELINE configs[4]: 15 batches of 2^26 rows x {3 Int64, 3 Float64, 2 Utf8}, every batch resident in HBM; "
+                "note": f"one GPU's share of BASELINE configs[4]: {rbb.BATCHES} batches of 2^26 rows x {{3 Int64, 3 Float64, 2 Utf8}}, every batch resident in HBM; "
                         "frac is whole-pipeline algorithmic bytes / step time (host launch gaps included)"}}
     except Exception as e:
         out["cfg5_error"] = repr(e)[:300]
@@ -942,9 +1007,8 @@ def cpu_reference(args, steps, warmup, secondary=True, one_thread=True):
     calib = None
     threads_req = args.cpu_threads or 0
     if not threads_req and n >= 200_000_000:
-        # "all the host threads it can use" is not always the fastest way to run a memory-bound step: on the round-2 GPU box a
-        # plain Float64 add reaches 132 GB/s on 16 threads, 118 on 64 and 64 on all 128 hyperthreads (tools/experiments/membw.c).
-        # The arm therefore measures a 1e8-row sample at a few thread counts and runs the full table with the best one.
+        # "all the host threads it can use" is not always the fastest way to run a memory-bound step: past a point, more
+        # threads only contend for the same memory controllers. The arm therefore measures a 1e8-row sample at a few thread counts and runs the full table with the best one.
         ncpu = len(os.sched_getaffinity(0))
         calib = {}
         for t in sorted({ncpu, max(ncpu // 2, 1), max(ncpu // 4, 1), max(ncpu // 8, 1)}):
@@ -1006,7 +1070,7 @@ def run_reference(args):
         "ms_per_step": sec * 1e3, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "i64 (filter/take/sum) + f64 (add)", "data": "synthetic",
         "config": {"workload": WORKLOAD, "rows_per_gpu": args.rows, "parallelism": f"row-range shards x{args.gpus}, NCCL all-reduce of the sum only",
-                   "l2": "inputs >> L2 (126 MB): no flush needed", "input_residency": "HBM"},
+                   "l2": "inputs >> L2 (50 MB): no flush needed", "input_residency": "HBM"},
         "rows_per_step": n, "same_config": base["same_config"],
         "timing": {"seconds": secs, "median": sec, "min": base["seconds_min"], "spread": base["spread"]},
         "cpu_baseline": base,
@@ -1034,7 +1098,10 @@ def main():
     ap.add_argument("--cpu-steps", type=int, default=5, help="timed CPU steps of the cpu_baseline leg of the GPU arm")
     ap.add_argument("--no-configs", action="store_true", help="skip the per-config sub-results (configs #2-#5)")
     ap.add_argument("--cpu-threads", type=int, default=0)
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write a seeded sample of the last step's outputs as DIR/*.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     args.warmup = max(args.warmup, 3) if args.impl == "ours" else args.warmup
     if args.impl == "reference":
         run_reference(args)

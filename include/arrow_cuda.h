@@ -1,5 +1,5 @@
 /*
- * arrow_cuda.h — C ABI of the B200-native arrow::compute hot path.
+ * arrow_cuda.h — C ABI of the H100-native arrow::compute hot path.
  *
  * This is the drop-in boundary (SURVEY.md §8(b)): one extern "C" entry point per
  * reference kernel, taking raw DEVICE pointers + explicit lengths / bit offsets, so

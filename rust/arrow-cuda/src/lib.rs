@@ -1,4 +1,4 @@
-//! `arrow-cuda`: drop-in for the `arrow::compute` hot path, backed by hand-written sm_100a kernels
+//! `arrow-cuda`: drop-in for the `arrow::compute` hot path, backed by hand-written sm_90a kernels
 //! (libarrow_cuda.so, C ABI in include/arrow_cuda.h).
 //!
 //! SOURCE ONLY in this repository — there is no Rust toolchain in the build image, so this crate is written to be correct by

@@ -1,6 +1,6 @@
 // tools/arith_sweep.cu — standalone tuning harness (not part of the product library):
 // times variants of the streaming f64 add (2 loads + 1 store per 16 B) to pick the
-// bytes-in-flight / occupancy point for k_arith. Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o arith_sweep arith_sweep.cu
+// bytes-in-flight / occupancy point for k_arith. Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o arith_sweep arith_sweep.cu
 #include <cuda_runtime.h>
 #include <cstdio>
 #include <cstdint>

@@ -23,7 +23,7 @@ def peak():
     try:
         return float(json.load(open(os.path.join(REPO, "MEASURED_PEAKS.json")))["hbm_gbs"])
     except Exception:
-        return 6650.0
+        return 3350.0  # H100 SXM data sheet HBM3 bandwidth
 
 
 class Bench:
