@@ -235,6 +235,48 @@ class ViewColumn:
         return out
 
 
+class FixedSizeBinaryColumn:
+    """A FixedSizeBinary column on the host (FixedSizeBinaryArray, arrow-array/src/array/fixed_size_binary_array.rs): `values`
+    is an (n, width) uint8 array, `nulls` a HostArray carrying validity / length."""
+
+    def __init__(self, values, nulls):
+        self.values, self.nulls = np.ascontiguousarray(values, dtype=np.uint8), nulls
+
+    @property
+    def width(self):
+        return self.values.shape[1]
+
+    @property
+    def length(self):
+        return self.nulls.length
+
+    @staticmethod
+    def from_values(items, width):
+        """items: list of bytes (each exactly `width` long) / None."""
+        vals = np.zeros((len(items), width), dtype=np.uint8)
+        for i, it in enumerate(items):
+            if it is not None:
+                assert len(it) == width
+                vals[i] = np.frombuffer(bytes(it), dtype=np.uint8)
+        nulls = HostArray.from_list(U8, [0 if it is not None else None for it in items])
+        nulls.values = np.zeros(0, np.uint8)
+        return FixedSizeBinaryColumn(vals, nulls)
+
+
+def column_value(col, row):
+    """The bytes of logical row `row` of a Utf8Column / ViewColumn / FixedSizeBinaryColumn (`array.value(row)`)."""
+    if isinstance(col, Utf8Column):
+        return bytes(col.data[int(col.offsets[row]): int(col.offsets[row + 1])])
+    if isinstance(col, FixedSizeBinaryColumn):
+        return bytes(col.values[row])
+    v = col.views[row]
+    ln = int(np.frombuffer(v[:4].tobytes(), dtype=np.uint32)[0])
+    if ln <= 12:
+        return bytes(v[4:4 + ln])
+    bi, off = (int(x) for x in np.frombuffer(v[8:16].tobytes(), dtype=np.uint32))
+    return bytes(col.buffers[bi][off:off + ln])
+
+
 class DeviceArray:
     """A HostArray's buffers uploaded to HBM (DeviceBuffer pair) with the same offsets."""
 
@@ -881,6 +923,37 @@ class Context:
             d.validity = dn
         return d
 
+    def _upload_bytes_col(self, col, owned):
+        """acu_bytes_array of a Utf8Column uploaded to HBM (device pointers appended to `owned`)."""
+        d = abi.BytesArray()
+        d_off, d_data = self.malloc(col.offsets.nbytes + 16), self.malloc(col.data.nbytes + 16)
+        owned += [d_off, d_data]
+        self.h2d(d_off, col.offsets)
+        if col.data.nbytes:
+            self.h2d(d_data, col.data)
+        d.offsets, d.data, d.nulls = d_off, d_data, self._upload_nulls(col.nulls, owned)
+        return d
+
+    def _upload_view_col(self, col, owned, keep):
+        """acu_view_array of a ViewColumn uploaded to HBM; the host pointer table is appended to `keep`."""
+        d = abi.ViewArray()
+        views = np.ascontiguousarray(col.views)
+        d_views = self.malloc(views.nbytes + 16)
+        owned.append(d_views)
+        if views.nbytes:
+            self.h2d(d_views, views)
+        ptrs = []
+        for buf in col.buffers:
+            db = self.malloc(buf.nbytes + 16)
+            owned.append(db)
+            self.h2d(db, buf)
+            ptrs.append(db)
+        table = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
+        keep.append(table)
+        d.views, d.buffers, d.n_buffers = d_views, table, len(ptrs)
+        d.nulls = self._upload_nulls(col.nulls, owned)
+        return d
+
     def cmp_bytes(self, op, a, b):
         """a, b: Utf8Column (offsets, data, nulls); nulls.is_scalar marks a Datum scalar."""
         assert a.offsets.dtype == b.offsets.dtype
@@ -888,16 +961,7 @@ class Context:
         n = max(a.nulls.length if not a.nulls.is_scalar else 0, b.nulls.length if not b.nulls.is_scalar else 0, 1)
         out = self.alloc_out(bitmap_bytes(n), n)
         try:
-            descs = []
-            for col in (a, b):
-                d = abi.BytesArray()
-                d_off, d_data = self.malloc(col.offsets.nbytes + 16), self.malloc(col.data.nbytes + 16)
-                owned += [d_off, d_data]
-                self.h2d(d_off, col.offsets)
-                if col.data.nbytes:
-                    self.h2d(d_data, col.data)
-                d.offsets, d.data, d.nulls = d_off, d_data, self._upload_nulls(col.nulls, owned)
-                descs.append(d)
+            descs = [self._upload_bytes_col(col, owned) for col in (a, b)]
             self.check(self.lib.acu_cmp_bytes(self.h, a.offsets.dtype.itemsize, op, C.byref(descs[0]), C.byref(descs[1]), C.byref(out)))
             res, out = self.download_out(out, BOOL), None
             return res
@@ -913,25 +977,8 @@ class Context:
         n = max(a.length if not a.nulls.is_scalar else 0, b.length if not b.nulls.is_scalar else 0, 1)
         out = self.alloc_out(bitmap_bytes(n), n)
         try:
-            descs, keep = [], []
-            for col in (a, b):
-                d = abi.ViewArray()
-                views = np.ascontiguousarray(col.views)
-                d_views = self.malloc(views.nbytes + 16)
-                owned.append(d_views)
-                if views.nbytes:
-                    self.h2d(d_views, views)
-                ptrs = []
-                for buf in col.buffers:
-                    db = self.malloc(buf.nbytes + 16)
-                    owned.append(db)
-                    self.h2d(db, buf)
-                    ptrs.append(db)
-                table = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
-                keep.append(table)
-                d.views, d.buffers, d.n_buffers = d_views, table, len(ptrs)
-                d.nulls = self._upload_nulls(col.nulls, owned)
-                descs.append(d)
+            keep = []
+            descs = [self._upload_view_col(col, owned, keep) for col in (a, b)]
             self.check(self.lib.acu_cmp_byte_view(self.h, op, C.byref(descs[0]), C.byref(descs[1]), C.byref(out)))
             res, out = self.download_out(out, BOOL), None
             return res
@@ -1091,3 +1138,67 @@ class Context:
     def sum(self, a): return self.aggregate(SUM, a)
     def min(self, a): return self.aggregate(MIN, a)
     def max(self, a): return self.aggregate(MAX, a)
+
+    # -- min / max of byte columns, boolean min / max (aggregate.rs:372-568, :880-889) ----------
+    def min_max_row(self, op, col):
+        """(row, valid_count): the lowest logical row holding the minimum (op = MIN) / maximum (MAX) of a Utf8Column,
+        ViewColumn or FixedSizeBinaryColumn, -1 when there is none."""
+        owned, keep = [], []
+        row, cnt = C.c_int64(0), C.c_int64(0)
+        try:
+            if isinstance(col, Utf8Column):
+                d = self._upload_bytes_col(col, owned)
+                self.check(self.lib.acu_aggregate_bytes(self.h, col.offsets.dtype.itemsize, op, C.byref(d), C.byref(row), C.byref(cnt)))
+            elif isinstance(col, ViewColumn):
+                d = self._upload_view_col(col, owned, keep)
+                self.check(self.lib.acu_aggregate_byte_view(self.h, op, C.byref(d), C.byref(row), C.byref(cnt)))
+            else:
+                d = self._upload_nulls(col.nulls, owned)
+                dv = self.malloc(col.values.nbytes + 16)
+                owned.append(dv)
+                if col.values.nbytes:
+                    self.h2d(dv, col.values)
+                d.values = dv
+                self.check(self.lib.acu_aggregate_fixed_size_binary(self.h, col.width, op, C.byref(d), C.byref(row), C.byref(cnt)))
+            return row.value, cnt.value
+        finally:
+            for p in owned:
+                self.free(p)
+
+    def _min_max_value(self, op, col, as_str):
+        row, _ = self.min_max_row(op, col)
+        if row < 0:
+            return None
+        b = column_value(col, row)
+        return b.decode() if as_str else b
+
+    def min_string(self, col): return self._min_max_value(MIN, col, True)
+    def max_string(self, col): return self._min_max_value(MAX, col, True)
+    def min_binary(self, col): return self._min_max_value(MIN, col, False)
+    def max_binary(self, col): return self._min_max_value(MAX, col, False)
+    def min_string_view(self, col): return self._min_max_value(MIN, col, True)
+    def max_string_view(self, col): return self._min_max_value(MAX, col, True)
+    def min_binary_view(self, col): return self._min_max_value(MIN, col, False)
+    def max_binary_view(self, col): return self._min_max_value(MAX, col, False)
+    def min_fixed_size_binary(self, col): return self._min_max_value(MIN, col, False)
+    def max_fixed_size_binary(self, col): return self._min_max_value(MAX, col, False)
+
+    def aggregate_boolean(self, op, a):
+        """(value, valid_count) of min_boolean (op = MIN) / max_boolean (MAX): value 0 | 1, -1 = None."""
+        da = self.upload(a)
+        try:
+            val, cnt = C.c_int32(0), C.c_int64(0)
+            ad = da.descriptor()
+            self.check(self.lib.acu_aggregate_boolean(self.h, op, C.byref(ad), C.byref(val), C.byref(cnt)))
+            return val.value, cnt.value
+        finally:
+            da.free()
+
+    def _boolean_value(self, op, a):
+        v, _ = self.aggregate_boolean(op, a)
+        return None if v < 0 else bool(v)
+
+    def min_boolean(self, a): return self._boolean_value(MIN, a)
+    def max_boolean(self, a): return self._boolean_value(MAX, a)
+    def bool_and(self, a): return self._boolean_value(MIN, a)
+    def bool_or(self, a): return self._boolean_value(MAX, a)

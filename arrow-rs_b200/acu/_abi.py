@@ -206,6 +206,10 @@ PROTOTYPES = {
     "acu_boolean": (i32, [vp, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_aggregate": (i32, [vp, i32, i32, P(Array), P(u64), P(i64)]),
     "acu_sum_checked": (i32, [vp, i32, P(Array), P(u64), P(i64)]),
+    "acu_aggregate_bytes": (i32, [vp, i32, i32, P(BytesArray), P(i64), P(i64)]),
+    "acu_aggregate_byte_view": (i32, [vp, i32, P(ViewArray), P(i64), P(i64)]),
+    "acu_aggregate_fixed_size_binary": (i32, [vp, i32, i32, P(Array), P(i64), P(i64)]),
+    "acu_aggregate_boolean": (i32, [vp, i32, P(Array), P(i32), P(i64)]),
     "acu_filter_record_batch": (i32, [vp, vp, i32, P(Column), P(ColumnOut)]),
     "acu_take_record_batch": (i32, [vp, i32, P(Column), P(Array), i32, i32, P(ColumnOut)]),
     "acu_aggregate_columns": (i32, [vp, i32, P(i32), P(i32), P(Array), P(u64), P(i64)]),

@@ -11,6 +11,7 @@
 // lane 0 of each 32-row group owns the group's 32-bit value and validity words.
 // Roofline: 2 offsets + the compared bytes per side (byte arrays), 16 B per view (views); HBM-bound.
 #include "bitmap.cuh"
+#include "bytes_cmp.cuh"
 #include "internal.cuh"
 
 namespace {
@@ -29,80 +30,7 @@ struct RowCmpCommon {
   unsigned long long *res;
 };
 
-struct BytesOperand {
-  const void *offs;
-  const uint8_t *data;
-  int ob;
-};
-
-struct ViewOperand {
-  const uint4 *views;
-  const uint8_t *const *buffers;  // device array of device pointers
-  int n_buffers;
-};
-
-__device__ __forceinline__ int64_t ld_offset(const void *offs, int ob, int64_t i) {
-  return ob == 4 ? (int64_t)__ldg(static_cast<const int32_t *>(offs) + i) : __ldg(static_cast<const int64_t *>(offs) + i);
-}
-
-// Up to 8 bytes of p[0 .. nb) as a little-endian u64, zero above nb: aligned 8-byte loads that contain a requested byte.
-__device__ __forceinline__ uint64_t ld_upto8(const uint8_t *__restrict__ p, uint32_t nb) {
-  const uintptr_t addr = (uintptr_t)p;
-  const uint64_t *q = reinterpret_cast<const uint64_t *>(addr & ~(uintptr_t)7);
-  const uint32_t sh = (uint32_t)(addr & 7u) * 8u;
-  uint64_t lo = 0, hi = 0;
-  if (nb) lo = __ldg(q);
-  if (sh + nb * 8u > 64u) hi = __ldg(q + 1);
-  const uint64_t w = (lo >> sh) | ((hi << 1) << (63u - sh));
-  return w & (nb >= 8u ? ~0ull : ((1ull << (nb * 8u)) - 1ull));
-}
-
-__device__ __forceinline__ uint64_t bswap64(uint64_t x) {
-  const uint32_t lo = (uint32_t)x, hi = (uint32_t)(x >> 32);
-  return ((uint64_t)__byte_perm(lo, 0, 0x0123) << 32) | (uint64_t)__byte_perm(hi, 0, 0x0123);
-}
-
-// `&[u8]` equality / ordering of Rust (lexicographic on unsigned bytes, then length)
-__device__ __forceinline__ bool bytes_eq(const uint8_t *a, int64_t la, const uint8_t *b, int64_t lb) {
-  if (la != lb) return false;
-  for (int64_t k = 0; k < la; k += 8) {
-    const uint32_t nb = (uint32_t)((la - k) < 8 ? (la - k) : 8);
-    if (ld_upto8(a + k, nb) != ld_upto8(b + k, nb)) return false;
-  }
-  return true;
-}
-__device__ __forceinline__ bool bytes_lt(const uint8_t *a, int64_t la, const uint8_t *b, int64_t lb) {
-  const int64_t n = la < lb ? la : lb;
-  for (int64_t k = 0; k < n; k += 8) {
-    const uint32_t nb = (uint32_t)((n - k) < 8 ? (n - k) : 8);
-    const uint64_t x = ld_upto8(a + k, nb), y = ld_upto8(b + k, nb);
-    if (x != y) return bswap64(x) < bswap64(y);  // first differing byte decides
-  }
-  return la < lb;
-}
-
-struct BytesItem { const uint8_t *p; int64_t len; };
-__device__ __forceinline__ BytesItem bytes_item(const BytesOperand &s, int64_t i) {
-  const int64_t b = ld_offset(s.offs, s.ob, i), e = ld_offset(s.offs, s.ob, i + 1);
-  return BytesItem{s.data + b, e - b};
-}
-
-// ---- views (arrow-data/src/byte_view.rs): x = length, y = prefix / inline[0..4), z, w = inline[4..12) or (buffer index, offset)
-__device__ __forceinline__ BytesItem view_item(const ViewOperand &s, const uint4 &v, const uint4 *slot) {
-  if (v.x <= 12u) return BytesItem{reinterpret_cast<const uint8_t *>(slot) + 4, (int64_t)v.x};
-  return BytesItem{s.buffers[v.z] + v.w, (int64_t)v.x};
-}
 __device__ __forceinline__ bool view_bits_eq(const uint4 &a, const uint4 &b) { return a.x == b.x && a.y == b.y && a.z == b.z && a.w == b.w; }
-// GenericByteViewArray::inline_key_fast (byte_view_array.rs:872-874): (raw.swap_bytes() << 32) | len, compared as u128
-__device__ __forceinline__ bool inline_key_lt(const uint4 &a, const uint4 &b) {
-  // the key's 128 bits, most significant first: inline bytes 0..11 in order (big endian), then the length
-  const uint32_t ak[4] = {__byte_perm(a.y, 0, 0x0123), __byte_perm(a.z, 0, 0x0123), __byte_perm(a.w, 0, 0x0123), a.x};
-  const uint32_t bk[4] = {__byte_perm(b.y, 0, 0x0123), __byte_perm(b.z, 0, 0x0123), __byte_perm(b.w, 0, 0x0123), b.x};
-#pragma unroll
-  for (int k = 0; k < 4; ++k)
-    if (ak[k] != bk[k]) return ak[k] < bk[k];
-  return false;
-}
 __device__ __forceinline__ bool view_is_eq(const ViewOperand &L, const uint4 &l, const uint4 *lslot, const ViewOperand &R, const uint4 &r,
                                            const uint4 *rslot) {  // cmp.rs:810-862
   if (L.n_buffers == 0 && R.n_buffers == 0) return view_bits_eq(l, r);

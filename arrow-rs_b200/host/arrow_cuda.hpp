@@ -1246,6 +1246,66 @@ template <class T> Result<std::optional<T>> sum_checked(const PrimitiveArray<T> 
   return std::optional<T>(out);
 }
 
+// min_string / max_string, min_string_view / max_string_view (aggregate.rs:520-568): the device returns the lowest row
+// holding the extremal value; its bytes are copied out (an owned value where the reference borrows from the array).
+namespace detail {
+inline std::optional<std::string> string_extreme(acu_agg_op op, const StringArray &a) {
+  acu_bytes_array b{};
+  b.offsets = a.offsets().data();
+  b.data = static_cast<const uint8_t *>(a.value_data().data());
+  b.nulls = a.view();
+  int64_t row = -1, valid = 0;
+  Context &c = Context::get();
+  const acu_status st = acu_aggregate_bytes(c.raw(), 4, op, &b, &row, &valid);
+  if (st != ACU_OK) throw std::runtime_error(c.last_error(st).message);
+  if (row < 0) return std::nullopt;
+  int32_t se[2];
+  acu_memcpy_d2h(c.raw(), se, static_cast<const int32_t *>(a.offsets().data()) + row, sizeof se);
+  std::string out((size_t)(se[1] - se[0]), '\0');
+  if (!out.empty()) acu_memcpy_d2h(c.raw(), out.data(), static_cast<const uint8_t *>(a.value_data().data()) + se[0], out.size());
+  return out;
+}
+inline std::optional<std::string> string_view_extreme(acu_agg_op op, const StringViewArray &a) {
+  Context &c = Context::get();
+  std::vector<const uint8_t *> ptrs;
+  for (const auto &b : a.data_buffers()) ptrs.push_back(static_cast<const uint8_t *>(b.buffer.data()));
+  std::optional<NullBuffer> nulls = nulls_from_mask(a.valid());  // the mirror keeps view validity on the host
+  acu_view_array v{};
+  v.views = a.views_ptr();
+  v.buffers = ptrs.data();
+  v.n_buffers = (int32_t)ptrs.size();
+  v.nulls.len = a.len();
+  if (nulls) {
+    v.nulls.validity = static_cast<const uint8_t *>(nulls->buffer.data());
+    v.nulls.null_count = nulls->null_count;
+  }
+  int64_t row = -1, valid = 0;
+  const acu_status st = acu_aggregate_byte_view(c.raw(), op, &v, &row, &valid);
+  if (st != ACU_OK) throw std::runtime_error(c.last_error(st).message);
+  if (row < 0) return std::nullopt;
+  return a.slice(row, 1).to_vec()[0];
+}
+inline std::optional<bool> boolean_extreme(acu_agg_op op, const BooleanArray &a) {
+  acu_array v = a.view();
+  int32_t value = -1;
+  int64_t valid = 0;
+  Context &c = Context::get();
+  const acu_status st = acu_aggregate_boolean(c.raw(), op, &v, &value, &valid);
+  if (st != ACU_OK) throw std::runtime_error(c.last_error(st).message);
+  if (value < 0) return std::nullopt;
+  return value != 0;
+}
+}  // namespace detail
+inline std::optional<std::string> min_string(const StringArray &a) { return detail::string_extreme(ACU_MIN, a); }
+inline std::optional<std::string> max_string(const StringArray &a) { return detail::string_extreme(ACU_MAX, a); }
+inline std::optional<std::string> min_string_view(const StringViewArray &a) { return detail::string_view_extreme(ACU_MIN, a); }
+inline std::optional<std::string> max_string_view(const StringViewArray &a) { return detail::string_view_extreme(ACU_MAX, a); }
+// min_boolean / max_boolean (aggregate.rs:372-457); bool_and / bool_or are the same functions (:880-889)
+inline std::optional<bool> min_boolean(const BooleanArray &a) { return detail::boolean_extreme(ACU_MIN, a); }
+inline std::optional<bool> max_boolean(const BooleanArray &a) { return detail::boolean_extreme(ACU_MAX, a); }
+inline std::optional<bool> bool_and(const BooleanArray &a) { return min_boolean(a); }
+inline std::optional<bool> bool_or(const BooleanArray &a) { return max_boolean(a); }
+
 
 // ---- nullif / zip (arrow-select/src/nullif.rs:44-113, zip.rs:99-226) -------------------------------------------
 namespace detail {

@@ -442,6 +442,27 @@ acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu
 acu_status acu_sum_checked(acu_ctx *ctx, acu_dtype dtype, const acu_array *a, uint64_t *out_bits,
                            int64_t *out_valid_count);
 
+/* min / max of Utf8 / Binary (offset_bytes 4), LargeUtf8 / LargeBinary (8), Utf8View / BinaryView and FixedSizeBinary
+ * columns: min_max_helper / min_max_view_helper (aggregate.rs:460-518) behind min_string, max_binary_view,
+ * min_fixed_size_binary ... (:520-568). Values order like Rust's `&[u8]` (lexicographic on unsigned bytes, a proper prefix
+ * first). op = ACU_MIN | ACU_MAX (ACU_SUM => ACU_ERR_INVALID_ARGUMENT). *out_row = the LOWEST logical row holding the
+ * extremal value (the reference folds in row order and replaces only on a strict < / >), -1 = None (every row null, or
+ * len == 0); *out_valid_count = non-null rows. Null slots are never read. The column layouts are those of acu_cmp_bytes /
+ * acu_cmp_byte_view; a FixedSizeBinary column is an acu_array whose `values` holds len x byte_width bytes (byte_width >= 0,
+ * negative => ACU_ERR_INVALID_ARGUMENT). is_scalar inputs => ACU_ERR_INVALID_ARGUMENT. Synchronous (not available inside a
+ * stream-ordered section); kernel time is counted in ACU_K_REDUCE. */
+acu_status acu_aggregate_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_agg_op op, const acu_bytes_array *a,
+                               int64_t *out_row, int64_t *out_valid_count);
+acu_status acu_aggregate_byte_view(acu_ctx *ctx, acu_agg_op op, const acu_view_array *a, int64_t *out_row,
+                                   int64_t *out_valid_count);
+acu_status acu_aggregate_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, acu_agg_op op, const acu_array *a,
+                                           int64_t *out_row, int64_t *out_valid_count);
+/* min_boolean / bool_and (ACU_MIN), max_boolean / bool_or (ACU_MAX) (aggregate.rs:372-457, :880-889): *out_value 0 | 1,
+ * -1 = None; *out_valid_count = non-null rows. `values` is the value bitmap with bit offset values_offset. Synchronous, as
+ * above. */
+acu_status acu_aggregate_boolean(acu_ctx *ctx, acu_agg_op op, const acu_array *a, int32_t *out_value,
+                                 int64_t *out_valid_count);
+
 /* ------------------------------------------------------------------------- */
 /* RecordBatch level — filter_record_batch / take_record_batch / per-column   */
 /* aggregates with ONE stream synchronisation per call                        */

@@ -191,6 +191,12 @@ extern "C" {
     pub fn acu_aggregate_columns(ctx: *mut acu_ctx, n_columns: i32, dtypes: *const i32, ops: *const i32, arrays: *const acu_array,
                                  out_bits: *mut u64, out_valid_counts: *mut i64) -> acu_status;
     pub fn acu_sum_checked(ctx: *mut acu_ctx, dtype: i32, a: *const acu_array, out_bits: *mut u64, out_valid: *mut i64) -> acu_status;
+    pub fn acu_aggregate_bytes(ctx: *mut acu_ctx, offset_bytes: i32, op: i32, a: *const acu_bytes_array, out_row: *mut i64,
+                               out_valid: *mut i64) -> acu_status;
+    pub fn acu_aggregate_byte_view(ctx: *mut acu_ctx, op: i32, a: *const acu_view_array, out_row: *mut i64, out_valid: *mut i64) -> acu_status;
+    pub fn acu_aggregate_fixed_size_binary(ctx: *mut acu_ctx, byte_width: i32, op: i32, a: *const acu_array, out_row: *mut i64,
+                                           out_valid: *mut i64) -> acu_status;
+    pub fn acu_aggregate_boolean(ctx: *mut acu_ctx, op: i32, a: *const acu_array, out_value: *mut i32, out_valid: *mut i64) -> acu_status;
     pub fn acu_filter_plan_create_cmp(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array,
                                       out: *mut *mut acu_filter_plan) -> acu_status;
     pub fn acu_nullif(ctx: *mut acu_ctx, left: *const acu_array, right: *const acu_array, out: *mut acu_array_out) -> acu_status;

@@ -14,6 +14,8 @@
 //!   compute::kernels::boolean::{and .. is_not_null}                          arrow-arith/src/boolean.rs:60-354
 //!   compute::{cast, cast_with_options, CastOptions}                          arrow-cast/src/cast/mod.rs:347,790
 //!   compute::{sum, min, max, sum_checked}                                    arrow-arith/src/aggregate.rs:897-1027
+//!   compute::aggregate::{min_string .. max_fixed_size_binary, min_boolean,   arrow-arith/src/aggregate.rs:372-568, 880-889
+//!                        max_boolean, bool_and, bool_or}
 //!   compute::{nullif, zip, concat, concat_batches}                           arrow-select/src/{nullif,zip,concat}.rs
 //!
 //! The wrappers are reference-shaped: host `ArrayRef` in, host `ArrayRef` out, upload / download around every call. A
@@ -419,6 +421,94 @@ pub mod compute {
         let (mut bits, mut valid) = (0u64, 0i64);
         ctx.check(unsafe { ffi::acu_sum_checked(ctx.raw(), dtype, a.view(), &mut bits, &mut valid) })?;
         Ok((valid != 0).then(|| unsafe { std::ptr::read_unaligned(&bits as *const u64 as *const T::Native) }))
+    }
+
+    /// min / max of byte, view, fixed-size-binary and boolean arrays (aggregate.rs:372-568, :880-889). The device returns the
+    /// lowest row holding the extremal value; the result borrows that row from the host array, as the reference's does.
+    pub mod aggregate {
+        use super::super::{ffi, Context, DeviceArray, DeviceBuffer};
+        use arrow_array::types::{BinaryViewType, ByteViewType, StringViewType};
+        use arrow_array::{Array, BooleanArray, FixedSizeBinaryArray, GenericBinaryArray, GenericByteViewArray, GenericStringArray, OffsetSizeTrait};
+        use arrow_schema::ArrowError;
+
+        fn nulls_view(ctx: &Context, array: &dyn Array, bufs: &mut Vec<DeviceBuffer>) -> Result<ffi::acu_array, ArrowError> {
+            let (validity, validity_offset, null_count) = match array.nulls() {
+                Some(n) => {
+                    let b = DeviceBuffer::from_host(ctx, n.buffer().as_slice())?;
+                    let p = b.as_ptr() as *const u8;
+                    bufs.push(b);
+                    (p, n.offset() as i64, n.null_count() as i64)
+                }
+                None => (std::ptr::null(), 0, 0),
+            };
+            Ok(ffi::acu_array { values: std::ptr::null(), values_offset: 0, validity, validity_offset, len: array.len() as i64, null_count,
+                                is_scalar: 0, reserved: 0 })
+        }
+        fn bytes_row<O: OffsetSizeTrait>(op: i32, array: &dyn Array) -> Option<usize> {
+            let ctx = Context::current().ok()?;
+            let a = DeviceArray::upload(&ctx, array, false).ok()?;
+            let b = ffi::acu_bytes_array { offsets: a.column.array.values, data: a.column.data, nulls: a.column.array };
+            let (mut row, mut valid) = (-1i64, 0i64);
+            ctx.check(unsafe { ffi::acu_aggregate_bytes(ctx.raw(), std::mem::size_of::<O>() as i32, op, &b, &mut row, &mut valid) }).ok()?;
+            (row >= 0).then_some(row as usize)
+        }
+        fn view_row<T: ByteViewType + ?Sized>(op: i32, array: &GenericByteViewArray<T>) -> Option<usize> {
+            let ctx = Context::current().ok()?;
+            let mut bufs = Vec::new();
+            let nulls = nulls_view(&ctx, array, &mut bufs).ok()?;
+            let views = array.views();
+            let v = DeviceBuffer::from_host(&ctx, views.inner().as_slice()).ok()?;
+            let views_ptr = v.as_ptr();
+            bufs.push(v);
+            let mut ptrs = Vec::new();
+            for d in array.data_buffers() {
+                let b = DeviceBuffer::from_host(&ctx, d.as_slice()).ok()?;
+                ptrs.push(b.as_ptr() as *const u8);
+                bufs.push(b);
+            }
+            let a = ffi::acu_view_array { views: views_ptr, buffers: ptrs.as_ptr(), n_buffers: ptrs.len() as i32, reserved: 0, nulls };
+            let (mut row, mut valid) = (-1i64, 0i64);
+            ctx.check(unsafe { ffi::acu_aggregate_byte_view(ctx.raw(), op, &a, &mut row, &mut valid) }).ok()?;
+            (row >= 0).then_some(row as usize)
+        }
+        fn fixed_row(op: i32, array: &FixedSizeBinaryArray) -> Option<usize> {
+            let ctx = Context::current().ok()?;
+            let mut bufs = Vec::new();
+            let mut a = nulls_view(&ctx, array, &mut bufs).ok()?;
+            let w = array.value_length() as usize;
+            let d = array.to_data();
+            let bytes = &d.buffers()[0].as_slice()[d.offset() * w..(d.offset() + d.len()) * w];
+            let v = DeviceBuffer::from_host(&ctx, bytes).ok()?;
+            a.values = v.as_ptr();
+            bufs.push(v);
+            let (mut row, mut valid) = (-1i64, 0i64);
+            ctx.check(unsafe { ffi::acu_aggregate_fixed_size_binary(ctx.raw(), w as i32, op, &a, &mut row, &mut valid) }).ok()?;
+            (row >= 0).then_some(row as usize)
+        }
+        fn boolean(op: i32, array: &BooleanArray) -> Option<bool> {
+            let ctx = Context::current().ok()?;
+            let a = DeviceArray::upload(&ctx, array, false).ok()?;
+            let (mut value, mut valid) = (-1i32, 0i64);
+            ctx.check(unsafe { ffi::acu_aggregate_boolean(ctx.raw(), op, &a.column.array, &mut value, &mut valid) }).ok()?;
+            (value >= 0).then_some(value != 0)
+        }
+
+        /// aggregate.rs:520-568
+        pub fn max_binary<T: OffsetSizeTrait>(array: &GenericBinaryArray<T>) -> Option<&[u8]> { bytes_row::<T>(ffi::ACU_MAX, array).map(|i| array.value(i)) }
+        pub fn min_binary<T: OffsetSizeTrait>(array: &GenericBinaryArray<T>) -> Option<&[u8]> { bytes_row::<T>(ffi::ACU_MIN, array).map(|i| array.value(i)) }
+        pub fn max_string<T: OffsetSizeTrait>(array: &GenericStringArray<T>) -> Option<&str> { bytes_row::<T>(ffi::ACU_MAX, array).map(|i| array.value(i)) }
+        pub fn min_string<T: OffsetSizeTrait>(array: &GenericStringArray<T>) -> Option<&str> { bytes_row::<T>(ffi::ACU_MIN, array).map(|i| array.value(i)) }
+        pub fn max_binary_view(array: &GenericByteViewArray<BinaryViewType>) -> Option<&[u8]> { view_row(ffi::ACU_MAX, array).map(|i| array.value(i)) }
+        pub fn min_binary_view(array: &GenericByteViewArray<BinaryViewType>) -> Option<&[u8]> { view_row(ffi::ACU_MIN, array).map(|i| array.value(i)) }
+        pub fn max_string_view(array: &GenericByteViewArray<StringViewType>) -> Option<&str> { view_row(ffi::ACU_MAX, array).map(|i| array.value(i)) }
+        pub fn min_string_view(array: &GenericByteViewArray<StringViewType>) -> Option<&str> { view_row(ffi::ACU_MIN, array).map(|i| array.value(i)) }
+        pub fn max_fixed_size_binary(array: &FixedSizeBinaryArray) -> Option<&[u8]> { fixed_row(ffi::ACU_MAX, array).map(|i| array.value(i)) }
+        pub fn min_fixed_size_binary(array: &FixedSizeBinaryArray) -> Option<&[u8]> { fixed_row(ffi::ACU_MIN, array).map(|i| array.value(i)) }
+        /// aggregate.rs:372-457, :880-889
+        pub fn min_boolean(array: &BooleanArray) -> Option<bool> { boolean(ffi::ACU_MIN, array) }
+        pub fn max_boolean(array: &BooleanArray) -> Option<bool> { boolean(ffi::ACU_MAX, array) }
+        pub fn bool_and(array: &BooleanArray) -> Option<bool> { min_boolean(array) }
+        pub fn bool_or(array: &BooleanArray) -> Option<bool> { max_boolean(array) }
     }
 
     // ---- nullif / zip / concat (arrow-select) ----------------------------------------------------------------------------

@@ -185,10 +185,99 @@ def main():
         b.timed("cast dict<i32,utf8>->utf8", [abi.K_TAKE, abi.K_BYTES], 4 * ns + ns / 8 + 4 * (ns + 1) + 0.95 * ns * 8 + ns / 8, ns,
                 lambda: ctx.check(lib.acu_take_bytes(h, 4, d_off, d_data, C.byref(dict_nulls), C.byref(keys), abi.I32, 0, d_out_off, d_out_data, ns * 13, C.byref(total), C.byref(on))),
                 note="kernel_ms = validity + table + lengths + copy kernels (the three tiny scan kernels only show in call_ms)")
+        # ---------------- min / max of byte columns (arrow-arith/src/aggregate.rs:460-568), bool_and ----------------
+        if not b.only or any(t in "min_string max_string cmp_bytes bool_and" for t in b.only.split("|")):
+            agg_bytes_rows(b, ctx, ns, d_off, d_data, dkeys, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D, va, nva, n)
     print("\n| op | rows | kernel ms | GB/s (algorithmic) | % of measured HBM peak | Mrows/s |")
     print("|---|---|---|---|---|---|")
     for r in b.rows:
         print(f"| {r['op']} | {r['rows']:.3g} | {r['kernel_ms']} | {r['achieved_gbs']} | {100 * r['frac_of_measured_peak']:.1f} | {r['mrows_s']} |")
+
+
+def agg_bytes_rows(b, ctx, ns, d_off, d_data, dkeys, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D, va, nva, n):
+    """min_string / max_string on the dictionary-decoded Utf8 column (D = 4096 values of 4..12 bytes, 5 % nulls) and on the
+    same values as an all-inline view column; an adversarial Utf8 / view pair whose values share a 24-byte prefix; bool_and on
+    a 1e9-row bitmap with validity. acu_cmp_bytes lt on the same Utf8 column (it reads the same bytes twice) is the bar."""
+    lib, h = ctx.lib, ctx.h
+    total = C.c_int64(0)
+    ctx.check(lib.acu_take_bytes(h, 4, d_off, d_data, C.byref(dict_nulls), C.byref(keys), abi.I32, 0, d_out_off, d_out_data, ns * 13,
+                                 C.byref(total), C.byref(on)))
+    row, cnt = C.c_int64(0), C.c_int64(0)
+    U = abi.BytesArray()
+    U.offsets, U.data = d_out_off, d_out_data
+    U.nulls = b.arr(None, on.validity, ns, on.null_count)
+    ub = 4 * (ns + 1) + total.value + ns / 8  # offsets + value bytes + validity
+    for name, op in (("min_string utf8 dict-decoded", abi.MIN), ("max_string utf8 dict-decoded", abi.MAX)):
+        b.timed(name, [abi.K_REDUCE], ub, ns, lambda op=op: ctx.check(lib.acu_aggregate_bytes(h, 4, op, C.byref(U), C.byref(row), C.byref(cnt))),
+                note=f"D={D}, lengths 4..12, 5% nulls; {total.value} value bytes")
+    ob = ctx.malloc(abi.bitmap_bytes(ns) + 64)
+    ov = abi.ArrayOut()
+    ov.values, ov.validity = ob, ctx.malloc(abi.bitmap_bytes(ns) + 64)
+    b.timed("min_max bar: cmp_bytes lt utf8 dict-decoded", [abi.K_CMP], 2 * ub + ns / 8, ns,
+            lambda: ctx.check(lib.acu_cmp_bytes(h, 4, abi.LT, C.byref(U), C.byref(U), C.byref(ov))), note="reads the column twice")
+    ctx._free_out(ov)
+    # the same values as an all-inline view column: take(dictionary views, keys) with 16-byte elements
+    dict_views = np.zeros((D, 16), dtype=np.uint8)
+    for k in range(D):
+        ln = int(offs[k + 1] - offs[k])
+        dict_views[k, :4] = np.frombuffer(np.uint32(ln).tobytes(), np.uint8)
+        dict_views[k, 4:4 + ln] = data[offs[k]: offs[k + 1]]
+    d_dv = ctx.malloc(dict_views.nbytes + 64)
+    ctx.h2d(d_dv, dict_views)
+    ovw = b.out(ns * 16, ns)
+    ctx.check(lib.acu_take_primitive(h, 16, C.byref(b.arr(d_dv, None, D, 0)), C.byref(keys), abi.I32, 0, C.byref(ovw)))
+    V = abi.ViewArray()
+    V.views, V.buffers, V.n_buffers = ovw.values, (C.c_void_p * 1)(), 0
+    V.nulls = b.arr(None, ovw.validity, ns, ovw.null_count if ovw.has_validity else 0)
+    vb = 16 * ns + ns / 8
+    for name, op in (("min_string_view inline dict-decoded", abi.MIN), ("max_string_view inline dict-decoded", abi.MAX)):
+        b.timed(name, [abi.K_REDUCE], vb, ns, lambda op=op: ctx.check(lib.acu_aggregate_byte_view(h, op, C.byref(V), C.byref(row), C.byref(cnt))),
+                note="views only (all values inline)")
+    ctx._free_out(ovw)
+    ctx.free(d_dv)
+    # adversarial: every value = the same 24-byte prefix + an 8-byte tail (4096 distinct tails): every key ties
+    na = 10_000_000
+    rng = np.random.default_rng(3)
+    tails = rng.integers(97, 123, (D, 8)).astype(np.uint8)
+    vals = np.empty((na, 32), dtype=np.uint8)
+    vals[:, :24] = np.frombuffer(b"shared-prefix-of-24-byte", np.uint8)
+    vals[:, 24:] = tails[rng.integers(0, D, na)]
+    mask = rng.random(na) >= 0.05
+    nulls = acu.HostArray.from_numpy(abi.U8, np.zeros(na, np.uint8), mask)
+    d_vals, d_aoff, d_valid = ctx.malloc(vals.nbytes + 64), ctx.malloc(4 * (na + 1) + 64), ctx.malloc(nulls.validity.nbytes + 64)
+    ctx.h2d(d_vals, vals)
+    ctx.h2d(d_aoff, np.arange(na + 1, dtype=np.int32) * 32)
+    ctx.h2d(d_valid, nulls.validity)
+    views = np.zeros((na, 4), dtype=np.uint32)
+    views[:, 0] = 32
+    views[:, 1] = np.frombuffer(b"shar", np.uint32)[0]
+    views[:, 3] = np.arange(na, dtype=np.uint32) * 32  # buffer 0 = the Utf8 value bytes
+    d_views = ctx.malloc(views.nbytes + 64)
+    ctx.h2d(d_views, views)
+    UA = abi.BytesArray()
+    UA.offsets, UA.data, UA.nulls = d_aoff, d_vals, b.arr(None, d_valid, na, na - int(mask.sum()))
+    VA = abi.ViewArray()
+    VA.views, VA.buffers, VA.n_buffers = d_views, (C.c_void_p * 1)(d_vals), 1
+    VA.nulls = UA.nulls
+    for name, op in (("min_string utf8 24-byte shared prefix", abi.MIN), ("max_string utf8 24-byte shared prefix", abi.MAX)):
+        b.timed(name, [abi.K_REDUCE], 4 * (na + 1) + 32 * na + na / 8, na,
+                lambda op=op: ctx.check(lib.acu_aggregate_bytes(h, 4, op, C.byref(UA), C.byref(row), C.byref(cnt))), note="every key ties")
+    ov2 = b.out(abi.bitmap_bytes(na), na)
+    b.timed("min_max bar: cmp_bytes lt utf8 24-byte shared prefix", [abi.K_CMP], 2 * (4 * (na + 1) + 32 * na + na / 8) + na / 8, na,
+            lambda: ctx.check(lib.acu_cmp_bytes(h, 4, abi.LT, C.byref(UA), C.byref(UA), C.byref(ov2))), note="reads the column twice")
+    ctx._free_out(ov2)
+    for name, op in (("min_string_view 24-byte shared prefix", abi.MIN), ("max_string_view 24-byte shared prefix", abi.MAX)):
+        b.timed(name, [abi.K_REDUCE], 16 * na + 32 * na + na / 8, na,
+                lambda op=op: ctx.check(lib.acu_aggregate_byte_view(h, op, C.byref(VA), C.byref(row), C.byref(cnt))),
+                note="every key ties: algorithmic bytes count the value bytes as read once")
+    for p in (d_vals, d_aoff, d_valid, d_views):
+        ctx.free(p)
+    # bool_and on a 1e9-row bitmap with validity (values almost all true: the answer needs the whole pass)
+    bv, _ = b.bits(52, 0.999, n)
+    BA = b.arr(bv, va, n, n - nva)
+    val = C.c_int32(0)
+    b.timed("bool_and 1e9", [abi.K_REDUCE], 2 * n / 8, n, lambda: ctx.check(lib.acu_aggregate_boolean(h, abi.MIN, C.byref(BA), C.byref(val), C.byref(cnt))))
+    ctx.free(bv)
 
 
 if __name__ == "__main__":
