@@ -1034,17 +1034,6 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_gather_copy(const BytesArgs a
 // on the ctx stream without synchronising; gather_finalize reads the fetched result block:
 // RES_ERR_INDEX = lowest out-of-bounds row (detect_oob), RES_AUX0 = total value bytes,
 // RES_ERR2 = lowest row whose running total exceeds the offset type.
-struct GatherState {
-  BytesArgs a;
-  int64_t blocks = 0;
-  int64_t *block_tot = nullptr;
-  void *out_offsets = nullptr;
-  uint8_t *out_data = nullptr;
-  int64_t out_cap = 0;
-  int64_t limit = 0;
-  bool detect_oob = false;
-};
-
 size_t gather_block_bytes(int64_t m) {
   const int64_t blocks = (m + BY_ROWS - 1) / BY_ROWS;
   return (((size_t)(2 * blocks + blocks / SCAN_ELEMS + 4096) * 8) + 255) & ~(size_t)255;
@@ -1054,22 +1043,28 @@ size_t gather_scratch_bytes(int64_t m) { return gather_block_bytes(m) + (size_t)
 
 acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const uint8_t *data, const void *idx, int kind,
                          int64_t m, int64_t n_src, const uint8_t *out_valid, bool detect_oob, void *out_offsets,
-                         uint8_t *out_data, int64_t out_cap, void *scratch, unsigned long long *res, GatherState *gs) {
+                         uint8_t *out_data, int64_t out_cap, void *scratch, unsigned long long *res, acu_bytes_col_state *gs) {
   const int64_t blocks = (m + BY_ROWS - 1) / BY_ROWS;
   int64_t *block_tot = static_cast<int64_t *>(scratch);
   BytesArgs a{offsets, data, idx, kind, (int)ob, m, n_src, reinterpret_cast<const uint32_t *>(out_valid), detect_oob ? 1 : 0};
   const bool fast = ob == 4 && kind == 4 && ((uintptr_t)idx % 16 == 0) && ((uintptr_t)offsets % 4 == 0);
-  gs->a = a;
-  gs->blocks = blocks;
+  const int64_t limit = ob == 4 ? (int64_t)INT32_MAX : INT64_MAX;
+  gs->gathered = true;
+  gs->ob = ob;
+  gs->kind = kind;
+  gs->offsets = offsets;
+  gs->idx = idx;
+  gs->data = data;
+  gs->out_valid = out_valid;
+  gs->m = m;
+  gs->n_src = n_src;
+  gs->detect_oob = detect_oob;
   gs->block_tot = block_tot;
   gs->out_offsets = out_offsets;
   gs->out_data = out_data;
   gs->out_cap = out_cap;
-  gs->limit = ob == 4 ? (int64_t)INT32_MAX : INT64_MAX;
-  gs->detect_oob = detect_oob;
   // small source (a dictionary): table in shared memory, see k_dict_copy
-  static const bool no_dict = getenv("ACU_BYTES_NO_DICT") != nullptr;  // A/B measurements
-  if (fast && !no_dict && n_src <= DG_MAX_ENTRIES && n_src > 0 && m >= 65536 && ((uintptr_t)out_offsets % 4 == 0)) {
+  if (fast && n_src <= DG_MAX_ENTRIES && n_src > 0 && m >= 65536 && ((uintptr_t)out_offsets % 4 == 0)) {
     uint8_t *extra = static_cast<uint8_t *>(scratch) + gather_block_bytes(m);
     uint4 *table = reinterpret_cast<uint4 *>(extra);
     uint8_t *lens = extra + (size_t)DG_MAX_ENTRIES * 16;
@@ -1090,7 +1085,7 @@ acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const ui
       ACU_TRY(scan_inclusive(ctx, block_tot, blocks, block_tot + blocks));
       ACU_CUDA(ctx, cudaMemcpyAsync(res + RES_AUX0, block_tot + (blocks - 1), 8, cudaMemcpyDeviceToDevice, ctx->stream));
       da.detect_oob = 0;
-      ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_dict_copy, g2, DG_THREADS, smem2, da, block_tot, blocks, static_cast<int32_t *>(out_offsets), out_data, gs->limit, res,
+      ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_dict_copy, g2, DG_THREADS, smem2, da, block_tot, blocks, static_cast<int32_t *>(out_offsets), out_data, limit, res,
                        block_tot + (blocks - 1), out_cap);
       return ACU_OK;
     }
@@ -1101,28 +1096,27 @@ acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const ui
   ACU_CUDA(ctx, cudaMemcpyAsync(res + RES_AUX0, block_tot + (blocks - 1), 8, cudaMemcpyDeviceToDevice, ctx->stream));
   const int stage_cap = BY_STAGE_CAP;
   a.detect_oob = 0;
-  static const bool generic_v1 = getenv("ACU_BYTES_GENERIC_V1") != nullptr;  // A/B: the round-1 copy kernel
-  if (fast && !generic_v1 && ((uintptr_t)out_offsets % 4 == 0)) {
+  if (fast && ((uintptr_t)out_offsets % 4 == 0)) {
     const size_t smem = GC_IMG_BYTES + 32;
     ACU_CUDA(ctx, cudaFuncSetAttribute(k_gather_copy, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     int per_sm = 1;
     if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gather_copy, DG_THREADS, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_gather_copy, acu_grid(ctx, blocks, per_sm), DG_THREADS, smem, a, block_tot, blocks, static_cast<int32_t *>(out_offsets),
-                     out_data, gs->limit, res, block_tot + (blocks - 1), out_cap);
+                     out_data, limit, res, block_tot + (blocks - 1), out_cap);
   } else if (fast) {
     ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<true>, (unsigned)blocks, BY_THREADS, stage_cap, a, block_tot, (int64_t)0, out_offsets,
-                     out_data, gs->limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
+                     out_data, limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
   } else {
     ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<false>, (unsigned)blocks, BY_THREADS, stage_cap, a, block_tot, (int64_t)0, out_offsets,
-                     out_data, gs->limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
+                     out_data, limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
   }
   return ACU_OK;
 }
 
 // *oob_row >= 0: an out-of-bounds index at a valid slot (the caller raises the panic status).
-acu_status gather_finalize(acu_ctx *ctx, const GatherState &gs, const unsigned long long *hres, int64_t *out_len, int64_t *oob_row) {
+acu_status gather_finalize(acu_ctx *ctx, const acu_bytes_col_state &gs, const unsigned long long *hres, int64_t *out_len, int64_t *oob_row) {
   if (oob_row) *oob_row = -1;
   if (gs.detect_oob && hres[RES_ERR_INDEX] != ~0ull) {
     if (oob_row) *oob_row = (int64_t)hres[RES_ERR_INDEX];
@@ -1131,8 +1125,7 @@ acu_status gather_finalize(acu_ctx *ctx, const GatherState &gs, const unsigned l
   *out_len = (int64_t)hres[RES_AUX0];
   if (hres[RES_ERR2] != ~0ull) {  // T::Offset::from_usize(capacity) failed (take.rs:520-523)
     const int64_t j = (int64_t)hres[RES_ERR2];
-    BytesArgs a = gs.a;
-    a.detect_oob = 0;
+    const BytesArgs a{gs.offsets, gs.data, gs.idx, gs.kind, (int)gs.ob, gs.m, gs.n_src, reinterpret_cast<const uint32_t *>(gs.out_valid), 0};
     ACU_TRY(acu_res_reset(ctx));
     ACU_LAUNCH(ctx, k_bytes_offsets_copy<false>, 1, BY_THREADS, 0, a, gs.block_tot, j / BY_ROWS, gs.out_offsets, static_cast<uint8_t *>(nullptr),
                INT64_MAX, j, ctx->d_res, 0, static_cast<const int64_t *>(nullptr), (int64_t)0);
@@ -1264,54 +1257,31 @@ acu_status acu_plan_cached_indices(acu_ctx *ctx, const acu_filter_plan *plan, co
 size_t acu_bytes_col_scratch(int64_t out_rows) { return gather_scratch_bytes(out_rows); }
 
 // ---- one variable-width column of take / take_record_batch ------------------------------------
-struct acu_bytes_col_state {
-  GatherState gs;
-  int take_mode = 0;     // acu_take_col_launch's mode (nulls via the take kernel)
-  int nulls_kind = 0;    // 0 none, 1 = copy of indices.nulls (count in RES_COUNT), 2 = take kernel, 3 = filter_col (mode in take_mode)
-  bool gathered = false;
-};
-acu_bytes_col_state *acu_bytes_col_state_new() { return new acu_bytes_col_state(); }
-void acu_bytes_col_state_free(acu_bytes_col_state *s) { delete s; }
-
 acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const uint8_t *data, const acu_array *nulls_of,
                                      bool val_nulls, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls,
                                      void *out_offsets, uint8_t *out_data, int64_t out_cap, acu_array_out *out_nulls, void *scratch,
-                                     unsigned long long *res, acu_bytes_col_state *st, int nulls_mode) {
+                                     unsigned long long *res, acu_bytes_col_state *st) {
   *st = acu_bytes_col_state();
   if (ob != 4 && ob != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
-  const int kind = index_kind(index_dtype);
-  if (kind < 0)  // take.rs:103
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Take only supported for integers, got %s", acu_dtype_name(index_dtype));
   const int64_t m = indices->len;
-  if (nulls_mode < 0) {
-    out_nulls->len = m;
-    out_nulls->has_validity = 0;
-    out_nulls->null_count = 0;
-  }
+  out_nulls->len = m;
+  out_nulls->has_validity = 0;
+  out_nulls->null_count = 0;
   if (m == 0) return zero_first_offset(ctx, out_offsets, ob);
   const uint8_t *ov = nullptr;
-  bool detect_oob;
-  if (!val_nulls) {
+  if (val_nulls) {
+    ov = out_nulls->validity;  // take_bits(values.nulls), gathered by acu_take_cols_launch
+  } else if (indices->validity) {
     // values without nulls: take_nulls = indices.nulls().cloned() (take.rs:429) is a bitmap copy, and the
     // out-of-bounds check rides in the first bytes pass — no separate gather pass.
-    if (indices->validity) {
-      ACU_TRY(acu_bitmap_and_launch(ctx, indices->validity, indices->validity_offset, nullptr, 0, m,
-                                    reinterpret_cast<uint64_t *>(out_nulls->validity), true, res));
-      st->nulls_kind = 1;
-      if (idx_nulls) ov = out_nulls->validity;
-    }
-    detect_oob = true;
-  } else {
-    if (nulls_mode >= 0) st->take_mode = nulls_mode;  // the validity gather was queued by the record-batch driver
-    else ACU_TRY(acu_take_col_launch(ctx, 0, nulls_of, false, true, indices, index_dtype, idx_nulls, out_nulls, res, &st->take_mode));
-    st->nulls_kind = 2;
-    if (st->take_mode & 1) ov = out_nulls->validity;
-    detect_oob = false;  // the take kernel reports it
+    ACU_TRY(acu_bitmap_and_launch(ctx, indices->validity, indices->validity_offset, nullptr, 0, m,
+                                  reinterpret_cast<uint64_t *>(out_nulls->validity), true, res));
+    st->idx_nulls_copied = true;
+    if (idx_nulls) ov = out_nulls->validity;
   }
-  ACU_TRY(gather_launch(ctx, ob, offsets, data, indices->values, kind, m, nulls_of->len, ov, detect_oob, out_offsets, out_data, out_cap,
-                        scratch, res, &st->gs));
-  st->gathered = true;
-  return ACU_OK;
+  // with value nulls the take kernel of the validity gather reports an out-of-bounds index
+  return gather_launch(ctx, ob, offsets, data, indices->values, index_kind(index_dtype), m, nulls_of->len, ov, !val_nulls, out_offsets,
+                       out_data, out_cap, scratch, res, st);
 }
 
 acu_status acu_take_bytes_col_finalize(acu_ctx *ctx, const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype,
@@ -1320,9 +1290,8 @@ acu_status acu_take_bytes_col_finalize(acu_ctx *ctx, const acu_array *nulls_of, 
   *out_data_len = 0;
   const int64_t m = indices->len;
   if (!st->gathered) return ACU_OK;
-  if (st->nulls_kind == 2) ACU_TRY(acu_take_col_finalize(ctx, nulls_of, indices, index_dtype, st->take_mode, hres, out_nulls));
   int64_t oob_row = -1;
-  ACU_TRY(gather_finalize(ctx, st->gs, hres, out_data_len, &oob_row));
+  ACU_TRY(gather_finalize(ctx, *st, hres, out_data_len, &oob_row));
   if (oob_row >= 0) {  // the reference panics on a bounds-checked slice index (take.rs:517)
     uint64_t raw = 0;
     const int sz = acu_dtype_size(index_dtype);
@@ -1335,83 +1304,32 @@ acu_status acu_take_bytes_col_finalize(acu_ctx *ctx, const acu_array *nulls_of, 
     return acu_fail(ctx, ACU_ERR_PANIC_OUT_OF_BOUNDS, oob_row, widened, 0, (uint64_t)nulls_of->len, "Out-of-bounds index %llu",
                     (unsigned long long)widened);
   }
-  if (st->nulls_kind == 1) {
+  if (st->idx_nulls_copied) {
     out_nulls->has_validity = 1;
     out_nulls->null_count = m - (int64_t)hres[RES_COUNT];
   }
   return ACU_OK;
 }
 
-extern "C" acu_status acu_take_bytes(acu_ctx *ctx, int32_t offset_bytes, const void *offsets, const uint8_t *data,
-                                     const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype,
-                                     int32_t check_bounds, void *out_offsets, uint8_t *out_data,
-                                     int64_t out_data_capacity, int64_t *out_data_len, acu_array_out *out_nulls) {
-  ACU_ENTER(ctx);
-  *out_data_len = 0;
-  if (index_kind(index_dtype) < 0)  // take.rs:103
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Take only supported for integers, got %s", acu_dtype_name(index_dtype));
-  acu_status s;
-  const int64_t vnc = acu_resolve_null_count(ctx, nulls_of, &s);
-  ACU_TRY(s);
-  const int64_t inc = acu_resolve_null_count(ctx, indices, &s);
-  ACU_TRY(s);
-  const bool idx_nulls = indices->validity && inc > 0;
-  if (check_bounds) ACU_TRY(acu_take_check_bounds(ctx, indices, index_dtype, idx_nulls, nulls_of->len));
-  void *scratch;
-  ACU_TRY(acu_scratch(ctx, gather_scratch_bytes(indices->len), &scratch));
-  acu_bytes_col_state st;
-  ACU_TRY(acu_res_reset(ctx));
-  ACU_TRY(acu_take_bytes_col_launch(ctx, offset_bytes, offsets, data, nulls_of, nulls_of->validity && vnc > 0, indices, index_dtype, idx_nulls,
-                                    out_offsets, out_data, out_data_capacity, out_nulls, scratch, acu_dres(ctx, 0), &st, -1));
-  ACU_TRY(acu_res_fetch(ctx));
-  return acu_take_bytes_col_finalize(ctx, nulls_of, indices, index_dtype, &st, acu_hres(ctx, 0), out_data_len, out_nulls);
-}
-
 // ---- one variable-width column of filter / filter_record_batch ---------------------------------
 acu_status acu_filter_bytes_col_launch(acu_ctx *ctx, const acu_filter_plan *plan, int32_t ob, const void *offsets, const uint8_t *data,
-                                       const acu_array *nulls_of, void *out_offsets, uint8_t *out_data, int64_t out_cap,
-                                       acu_array_out *out_nulls, void *scratch, unsigned long long *res, acu_bytes_col_state *st,
-                                       int nulls_mode) {
+                                       const acu_array *nulls_of, void *out_offsets, uint8_t *out_data, int64_t out_cap, void *scratch,
+                                       unsigned long long *res, acu_bytes_col_state *st) {
   *st = acu_bytes_col_state();
   if (ob != 4 && ob != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
   const int64_t count = acu_filter_plan_count(plan);
-  // nulls first (FilterPredicate::filter_nulls); also validates the predicate length. nulls_mode >= 0: already queued by
-  // the record-batch driver together with the other columns' validity compactions.
-  if (nulls_mode >= 0) st->take_mode = nulls_mode;
-  else ACU_TRY(acu_filter_col_launch(ctx, plan, 2, 0, nulls_of, out_nulls, res, &st->take_mode));
-  st->nulls_kind = 3;
   if (count == 0) return zero_first_offset(ctx, out_offsets, ob);
   const void *idx;
   int kind;
   ACU_TRY(acu_plan_cached_indices(ctx, plan, &idx, &kind));
   // null slots are copied too (filter.rs:891-892): no output-validity masking of the lengths
-  ACU_TRY(gather_launch(ctx, ob, offsets, data, idx, kind, count, nulls_of->len, nullptr, false, out_offsets, out_data, out_cap, scratch,
-                        res, &st->gs));
-  st->gathered = true;
-  return ACU_OK;
+  return gather_launch(ctx, ob, offsets, data, idx, kind, count, nulls_of->len, nullptr, false, out_offsets, out_data, out_cap, scratch,
+                       res, st);
 }
 
-acu_status acu_filter_bytes_col_finalize(acu_ctx *ctx, const acu_filter_plan *plan, const acu_array *nulls_of,
-                                         const acu_bytes_col_state *st, const unsigned long long *hres, int64_t *out_data_len,
-                                         acu_array_out *out_nulls) {
+acu_status acu_filter_bytes_col_finalize(acu_ctx *ctx, const acu_bytes_col_state *st, const unsigned long long *hres,
+                                         int64_t *out_data_len) {
   *out_data_len = 0;
-  if (st->nulls_kind == 3) acu_filter_col_finalize(plan, nulls_of, st->take_mode, hres, out_nulls);
   if (!st->gathered) return ACU_OK;
-  return gather_finalize(ctx, st->gs, hres, out_data_len, nullptr);
-}
-
-extern "C" acu_status acu_filter_bytes(acu_ctx *ctx, const acu_filter_plan *plan, int32_t offset_bytes,
-                                       const void *offsets, const uint8_t *data, const acu_array *nulls_of,
-                                       void *out_offsets, uint8_t *out_data, int64_t out_data_capacity,
-                                       int64_t *out_data_len, acu_array_out *out_nulls) {
-  ACU_ENTER(ctx);
-  *out_data_len = 0;
-  void *scratch;
-  ACU_TRY(acu_scratch(ctx, gather_scratch_bytes(acu_filter_plan_count(plan)), &scratch));
-  acu_bytes_col_state st;
-  ACU_TRY(acu_res_reset(ctx));
-  ACU_TRY(acu_filter_bytes_col_launch(ctx, plan, offset_bytes, offsets, data, nulls_of, out_offsets, out_data, out_data_capacity, out_nulls,
-                                      scratch, acu_dres(ctx, 0), &st, -1));
-  ACU_TRY(acu_res_fetch(ctx));
-  return acu_filter_bytes_col_finalize(ctx, plan, nulls_of, &st, acu_hres(ctx, 0), out_data_len, out_nulls);
+  return gather_finalize(ctx, *st, hres, out_data_len, nullptr);
 }

@@ -244,12 +244,14 @@ acu_status acu_aggregate_allreduce(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op,
   const int64_t nc = deferred_nc ? -1 : (a->len ? acu_resolve_null_count(ctx, a, &st) : 0);
   ACU_TRY(st);
   const int64_t valid = deferred_nc ? -1 : a->len - nc;
+  const size_t scratch_bytes = acu_reduce_col_scratch(ctx);
   void *scratch;
-  ACU_TRY(acu_scratch(ctx, acu_reduce_col_scratch(ctx), &scratch));
+  ACU_TRY(acu_scratch(ctx, scratch_bytes, &scratch));
   int launched = 0;
   const int blk = acu_call_begin(ctx, &st);
   ACU_TRY(st);
-  ACU_TRY(acu_reduce_col_launch(ctx, dtype, op, a, nc, scratch, acu_dres(ctx, blk), &launched));
+  unsigned long long *res = acu_dres(ctx, blk);
+  ACU_TRY(acu_reduce_cols_launch(ctx, 1, &dtype, &op, a, &nc, static_cast<uint8_t *>(scratch), scratch_bytes, &res, &launched));
   constexpr int SLOT = 8;  // slots 8..9 of the block: {combined value, combined valid count}
   uint64_t *buf = reinterpret_cast<uint64_t *>(acu_dres(ctx, blk) + SLOT);
   ACU_LAUNCH(ctx, k_stage_partial, 1, 32, 0, acu_dres(ctx, blk), launched, (long long)valid, (int)dtype, (int)op, buf);

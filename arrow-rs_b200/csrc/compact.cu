@@ -22,7 +22,6 @@
 //             window assembles output words (atomicOr only on the two boundary words), and
 //             the popcount gives filter_nulls' null count. Also used for boolean VALUES
 //             (filter_bits / filter_boolean).
-#include <cstdlib>
 #include <vector>
 
 #include "bitmap.cuh"
@@ -691,7 +690,7 @@ template <int W>
 acu_status launch_filter(acu_ctx *ctx, const FilterBatch &fb, int n_cols, bool fused) {
   const FilterArgs &fa = fb.col[0];
   if (fa.aligned16) {
-    if (!fused) {  // sparse predicates (and ACU_FILTER_LEGACY=1): the round-1 value kernel; validity goes through k_compress_bits
+    if (!fused) {  // sparse predicates: the round-1 value kernel; validity goes through k_compress_bits
       constexpr size_t smem = 8 * (size_t)AsyncCfg<W>::PASS_BYTES;  // 8 warps x per-warp landing buffer
       if (ctx->occupancy.find(reinterpret_cast<const void *>(k_filter_values_async<W>)) == ctx->occupancy.end())  // first use on this device
         ACU_CUDA(ctx, cudaFuncSetAttribute(k_filter_values_async<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
@@ -704,7 +703,7 @@ acu_status launch_filter(acu_ctx *ctx, const FilterBatch &fb, int n_cols, bool f
       ACU_CUDA(ctx, cudaFuncSetAttribute(k_filter_fused<W>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     // every warp should own several tiles (the next tile's mask / offsets are prefetched while the current one is in
     // flight): with the columns of a record batch in blockIdx.y the x-grid is divided by the column count
-    static const int tiles_per_warp = getenv("ACU_FILTER_TILES_PER_WARP") ? atoi(getenv("ACU_FILTER_TILES_PER_WARP")) : 4;
+    constexpr int tiles_per_warp = 4;
     const int64_t want = (fa.n_tiles + 8 * (int64_t)tiles_per_warp - 1) / (8 * (int64_t)tiles_per_warp);
     int gx = acu_wave_grid(ctx, k_filter_fused<W>, 256, smem, (fa.n_tiles + 7) / 8);
     gx = (gx + n_cols - 1) / n_cols;
@@ -753,11 +752,9 @@ CompressArgs compress_args(const acu_filter_plan *plan, const uint8_t *src, int6
 
 // The one-pass kernel (k_filter_fused: values + validity) is used for 16-byte aligned value buffers unless the predicate is
 // very sparse (< 4 % selected: almost no value bytes move, the per-tile validity work dominates and the round-1 pair
-// k_filter_values_async + k_compress_bits is faster there). ACU_FILTER_LEGACY=1 forces
-// the round-1 kernels for A/B measurements.
+// k_filter_values_async + k_compress_bits is faster there).
 bool plan_uses_fused(const acu_filter_plan *plan) {
-  static const bool legacy = getenv("ACU_FILTER_LEGACY") != nullptr;
-  return !legacy && (plan->count < 0 || plan->count * 25 >= plan->len);  // count < 0: not fetched yet (async section)
+  return plan->count < 0 || plan->count * 25 >= plan->len;  // count < 0: not fetched yet (async section)
 }
 bool fuses_validity(const acu_filter_plan *plan, const acu_array *values) {
   return plan_uses_fused(plan) && ((uintptr_t)values->values % 16) == 0;
@@ -904,97 +901,55 @@ int64_t acu_filter_plan_count(const acu_filter_plan *plan) { return plan->count;
 int64_t acu_filter_plan_len(const acu_filter_plan *plan) { return plan->len; }
 int32_t acu_filter_plan_strategy(const acu_filter_plan *plan) { return plan->strategy; }
 
-acu_status acu_filter_primitive(acu_ctx *ctx, const acu_filter_plan *plan, int32_t elem_bytes,
-                                const acu_array *values, acu_array_out *out) {
+// filter of one primitive (kind 0) or boolean (kind 1) array: the record-batch launcher on one column.
+static acu_status filter_array(acu_ctx *ctx, const acu_filter_plan *plan, int kind, int32_t elem_bytes, const acu_array *values,
+                               acu_array_out *out) {
   ACU_ENTER(ctx);
   int mode = 0;
   acu_status st = ACU_OK;
   const int blk = acu_call_begin(ctx, &st);
   ACU_TRY(st);
-  ACU_TRY(acu_filter_col_launch(ctx, plan, 0, elem_bytes, values, out, acu_dres(ctx, blk), &mode));
+  unsigned long long *res = acu_dres(ctx, blk);
+  ACU_TRY(acu_filter_cols_launch(ctx, plan, 1, &kind, &elem_bytes, &values, &out, &res, &mode));
   return acu_call_end(ctx, blk, [plan, mode, out](const unsigned long long *h) -> acu_status {
-    acu_filter_col_finalize(plan, nullptr, mode, h, out);
+    acu_filter_col_finalize(plan, mode, h, out);
     return ACU_OK;
   });
+}
+
+acu_status acu_filter_primitive(acu_ctx *ctx, const acu_filter_plan *plan, int32_t elem_bytes,
+                                const acu_array *values, acu_array_out *out) {
+  return filter_array(ctx, plan, 0, elem_bytes, values, out);
 }
 
 acu_status acu_filter_boolean(acu_ctx *ctx, const acu_filter_plan *plan, const acu_array *values,
                               acu_array_out *out) {
-  ACU_ENTER(ctx);
-  int mode = 0;
-  acu_status st = ACU_OK;
-  const int blk = acu_call_begin(ctx, &st);
-  ACU_TRY(st);
-  ACU_TRY(acu_filter_col_launch(ctx, plan, 1, 0, values, out, acu_dres(ctx, blk), &mode));
-  return acu_call_end(ctx, blk, [plan, mode, out](const unsigned long long *h) -> acu_status {
-    acu_filter_col_finalize(plan, nullptr, mode, h, out);
-    return ACU_OK;
-  });
+  return filter_array(ctx, plan, 1, 0, values, out);
 }
 
 }  // extern "C"
 
-// One column of filter / filter_record_batch: queue the value kernel (kind 0 = primitive of
-// elem_bytes, 1 = boolean, 2 = validity only) and the validity compaction on the ctx stream
-// WITHOUT synchronising. *mode tells acu_filter_col_finalize how to read the result block:
-// 0 = no validity work, 1 = compacted validity + popcount, 2 = IterationStrategy::All slice.
-acu_status acu_filter_col_launch(acu_ctx *ctx, const acu_filter_plan *plan, int kind, int32_t elem_bytes,
-                                 const acu_array *values, acu_array_out *out, unsigned long long *res, int *mode) {
-  *mode = 0;
-  ACU_TRY(check_len(ctx, plan, values->len));
-  out->len = plan->count;
-  out->has_validity = 0;
-  out->null_count = 0;
-  const bool pending = plan->count < 0;  // async section: the count is still on the device, outputs are sized for plan->len
-  if (!pending && (plan->strategy == ACU_FILTER_NONE || plan->count == 0)) return ACU_OK;
-  // a validity buffer with a cached null_count of 0 is dropped (filter.rs:513-516); an unknown
-  // null_count (-1) is compacted and counted: the result is the same, NullBuffer-wise
-  // (a pending plan may turn out to select everything, where the reference slices and KEEPS the NullBuffer even without
-  // nulls: the validity is then compacted whenever it exists and the finaliser decides, mode 3)
-  const bool has_nulls = values->validity != nullptr && (values->null_count != 0 || pending);
-  if (plan->strategy == ACU_FILTER_ALL) {  // values.slice(0, count) (filter.rs:546)
-    if (kind == 0)
-      ACU_CUDA(ctx, cudaMemcpyAsync(out->values, values->values, (size_t)plan->count * elem_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
-    else if (kind == 1)
-      ACU_TRY(acu_bitmap_and_launch(ctx, static_cast<const uint8_t *>(values->values), values->values_offset, nullptr, 0,
-                                    plan->count, static_cast<uint64_t *>(out->values), false));
-    if (values->validity) {
-      ACU_TRY(acu_bitmap_and_launch(ctx, values->validity, values->validity_offset, nullptr, 0, plan->count,
-                                    reinterpret_cast<uint64_t *>(out->validity), true, res));
-      *mode = 2;
-    }
-    return ACU_OK;
+// IterationStrategy::All: values.slice(0, count) (filter.rs:546) of one column; the slice keeps its NullBuffer (mode 2).
+static acu_status filter_slice_col(acu_ctx *ctx, const acu_filter_plan *plan, int kind, int32_t elem_bytes, const acu_array *values,
+                                   acu_array_out *out, unsigned long long *res, int *mode) {
+  if (kind == 0)
+    ACU_CUDA(ctx, cudaMemcpyAsync(out->values, values->values, (size_t)plan->count * elem_bytes, cudaMemcpyDeviceToDevice, ctx->stream));
+  else if (kind == 1)
+    ACU_TRY(acu_bitmap_and_launch(ctx, static_cast<const uint8_t *>(values->values), values->values_offset, nullptr, 0,
+                                  plan->count, static_cast<uint64_t *>(out->values), false));
+  if (values->validity) {
+    ACU_TRY(acu_bitmap_and_launch(ctx, values->validity, values->validity_offset, nullptr, 0, plan->count,
+                                  reinterpret_cast<uint64_t *>(out->validity), true, res));
+    *mode = 2;
   }
-  bool fused = false;
-  if (kind == 0) {
-    FilterBatch fb{};
-    fb.col[0] = filter_args(plan, values, out, has_nulls, res);
-    fused = fb.col[0].vsrc != nullptr;
-    if (fused) {  // the kernel ORs boundary words into the bitmap
-      if (pending)
-        ACU_LAUNCH(ctx, k_zero_bitmap_dev, acu_grid(ctx, (plan->len / 64 + 255) / 256, 2), 256, 0, reinterpret_cast<uint64_t *>(out->validity),
-                   plan->tile_off + plan->n_tiles);
-      else
-        ACU_CUDA(ctx, cudaMemsetAsync(out->validity, 0, acu_bitmap_bytes(plan->count), ctx->stream));
-      *mode = pending ? 3 : 1;
-    }
-    ACU_TRY(launch_filter_width(ctx, elem_bytes, fb, 1, plan_uses_fused(plan)));
-  }
-  CompressBatch cb{};
-  int nc = 0;
-  if (kind == 1)
-    cb.col[nc++] = compress_args(plan, static_cast<const uint8_t *>(values->values), values->values_offset, out->values, nullptr);
-  if (has_nulls && !fused) {  // FilterPredicate::filter_nulls (filter.rs:512-533)
-    cb.col[nc++] = compress_args(plan, values->validity, values->validity_offset, out->validity, res);
-    *mode = pending ? 3 : 1;
-  }
-  if (nc) ACU_TRY(launch_compress(ctx, plan, cb, nc));
   return ACU_OK;
 }
 
-// All columns of a record batch (kinds[c]: 0 primitive, 1 boolean, 2 validity only): the same work as
-// acu_filter_col_launch per column, but the value kernels of equal-width columns and all the bit compactions
-// share launches (blockIdx.y = column). res_block(c) = result block of column c.
+// The columns of filter / filter_record_batch (kinds[c]: 0 primitive of widths[c] bytes, 1 boolean, 2 validity only):
+// queue the value kernels and the validity compactions on the ctx stream WITHOUT synchronising. The value kernels of
+// equal-width columns and all the bit compactions share launches (blockIdx.y = column); res[c] = result block of column c.
+// modes[c] tells acu_filter_col_finalize how to read that block: 0 = no validity work, 1 = compacted validity + popcount,
+// 2 = IterationStrategy::All slice, 3 = compacted with a pending plan.
 acu_status acu_filter_cols_launch(acu_ctx *ctx, const acu_filter_plan *plan, int n, const int *kinds, const int32_t *widths,
                                   const acu_array *const *values, acu_array_out *const *outs, unsigned long long *const *res, int *modes) {
   for (int c = 0; c < n; ++c) {
@@ -1004,11 +959,18 @@ acu_status acu_filter_cols_launch(acu_ctx *ctx, const acu_filter_plan *plan, int
     outs[c]->has_validity = 0;
     outs[c]->null_count = 0;
   }
-  if (plan->strategy == ACU_FILTER_NONE || plan->count == 0) return ACU_OK;
-  if (plan->strategy == ACU_FILTER_ALL) {  // slices: per column
-    for (int c = 0; c < n; ++c) ACU_TRY(acu_filter_col_launch(ctx, plan, kinds[c], widths[c], values[c], outs[c], res[c], &modes[c]));
+  const bool pending = plan->count < 0;  // async section: the count is still on the device, outputs are sized for plan->len
+  if (!pending && (plan->strategy == ACU_FILTER_NONE || plan->count == 0)) return ACU_OK;
+  if (plan->strategy == ACU_FILTER_ALL) {
+    for (int c = 0; c < n; ++c) ACU_TRY(filter_slice_col(ctx, plan, kinds[c], widths[c], values[c], outs[c], res[c], &modes[c]));
     return ACU_OK;
   }
+  // a validity buffer with a cached null_count of 0 is dropped (filter.rs:513-516); an unknown
+  // null_count (-1) is compacted and counted: the result is the same, NullBuffer-wise
+  // (a pending plan may turn out to select everything, where the reference slices and KEEPS the NullBuffer even without
+  // nulls: the validity is then compacted whenever it exists and the finaliser decides, mode 3)
+  auto has_nulls = [&](int c) { return values[c]->validity != nullptr && (values[c]->null_count != 0 || pending); };
+  const int compacted_mode = pending ? 3 : 1;
   // value kernels grouped by (element width, alignment class)
   std::vector<char> done(n, 0);
   for (int c = 0; c < n; ++c) {
@@ -1018,18 +980,22 @@ acu_status acu_filter_cols_launch(acu_ctx *ctx, const acu_filter_plan *plan, int
     const int al = ((uintptr_t)values[c]->values % 16) == 0;
     for (int d = c; d < n && k < BATCH_COLS; ++d) {
       if (kinds[d] != 0 || done[d] || widths[d] != widths[c] || (((uintptr_t)values[d]->values % 16) == 0) != al) continue;
-      const bool has_nulls = values[d]->validity != nullptr && values[d]->null_count != 0;
-      fb.col[k] = filter_args(plan, values[d], outs[d], has_nulls, res[d]);
-      if (fb.col[k].vsrc) {
-        ACU_CUDA(ctx, cudaMemsetAsync(outs[d]->validity, 0, acu_bitmap_bytes(plan->count), ctx->stream));
-        modes[d] = 1;
+      fb.col[k] = filter_args(plan, values[d], outs[d], has_nulls(d), res[d]);
+      if (fb.col[k].vsrc) {  // the kernel ORs boundary words into the bitmap
+        if (pending)
+          ACU_LAUNCH(ctx, k_zero_bitmap_dev, acu_grid(ctx, (plan->len / 64 + 255) / 256, 2), 256, 0,
+                     reinterpret_cast<uint64_t *>(outs[d]->validity), plan->tile_off + plan->n_tiles);
+        else
+          ACU_CUDA(ctx, cudaMemsetAsync(outs[d]->validity, 0, acu_bitmap_bytes(plan->count), ctx->stream));
+        modes[d] = compacted_mode;
       }
       ++k;
       done[d] = 1;
     }
     ACU_TRY(launch_filter_width(ctx, widths[c], fb, k, plan_uses_fused(plan)));
   }
-  // bit compactions: boolean values and every validity buffer that may hold nulls
+  // bit compactions: boolean values and every validity buffer that may hold nulls (FilterPredicate::filter_nulls,
+  // filter.rs:512-533) unless the value kernel compacted it
   CompressBatch cb{};
   int k = 0;
   auto flush = [&]() -> acu_status {
@@ -1042,18 +1008,16 @@ acu_status acu_filter_cols_launch(acu_ctx *ctx, const acu_filter_plan *plan, int
       cb.col[k++] = compress_args(plan, static_cast<const uint8_t *>(values[c]->values), values[c]->values_offset, outs[c]->values, nullptr);
       if (k == BATCH_COLS) ACU_TRY(flush());
     }
-    if (values[c]->validity != nullptr && values[c]->null_count != 0 && !(kinds[c] == 0 && fuses_validity(plan, values[c]))) {
+    if (has_nulls(c) && !(kinds[c] == 0 && fuses_validity(plan, values[c]))) {
       cb.col[k++] = compress_args(plan, values[c]->validity, values[c]->validity_offset, outs[c]->validity, res[c]);
-      modes[c] = 1;
+      modes[c] = compacted_mode;
       if (k == BATCH_COLS) ACU_TRY(flush());
     }
   }
   return flush();
 }
 
-void acu_filter_col_finalize(const acu_filter_plan *plan, const acu_array *values, int mode,
-                             const unsigned long long *hres, acu_array_out *out) {
-  (void)values;
+void acu_filter_col_finalize(const acu_filter_plan *plan, int mode, const unsigned long long *hres, acu_array_out *out) {
   out->len = plan->count;  // (known only now when the call was queued in an async section)
   out->has_validity = 0;
   out->null_count = 0;
@@ -1069,20 +1033,8 @@ void acu_filter_col_finalize(const acu_filter_plan *plan, const acu_array *value
   }
 }
 
-// FilterPredicate::filter_nulls for any array kind (bytes.cu). Synchronises the stream.
-acu_status acu_filter_nulls_internal(acu_ctx *ctx, const acu_filter_plan *plan, const acu_array *a,
-                                     acu_array_out *out) {
-  int mode = 0;
-  ACU_TRY(acu_res_reset(ctx));
-  ACU_TRY(acu_filter_col_launch(ctx, plan, 2, 0, a, out, acu_dres(ctx, 0), &mode));
-  ACU_TRY(acu_res_fetch(ctx));
-  acu_filter_col_finalize(plan, a, mode, acu_hres(ctx, 0), out);
-  return ACU_OK;
-}
-
 // Internal accessors for bytes.cu (filter_bytes materialises the selected row indices).
 const uint64_t *acu_plan_mask(const acu_filter_plan *p) { return p->mask; }
 const uint64_t *acu_plan_tile_off(const acu_filter_plan *p) { return p->tile_off; }
-int64_t acu_plan_n_tiles(const acu_filter_plan *p) { return p->n_tiles; }
 void **acu_plan_index_cache(const acu_filter_plan *p) { return &p->index_cache; }
 int64_t acu_plan_n_words_padded(const acu_filter_plan *p) { return ((p->n_tiles * TILE_WORDS + 31) / 32) * 32; }

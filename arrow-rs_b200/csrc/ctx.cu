@@ -231,13 +231,8 @@ acu_status acu_ctx_create(int32_t device, acu_ctx **out) {
   // L2 fill granularity. Sparse kernels (filter at low selectivity, take) only need the 32-B
   // sectors they touch; the default granularity fills whole 128-B lines from HBM (at 10 % selectivity
   // a 128-B line of 8-B values holds a selected row with probability 1 - 0.9^16 = 81.5 %).
-  // ACU_L2_FETCH_GRANULARITY=32|64|128 overrides (tuning knob).
-  {
-    size_t gran = 32;
-    if (const char *e = getenv("ACU_L2_FETCH_GRANULARITY")) gran = (size_t)atoi(e);
-    if (gran == 32 || gran == 64 || gran == 128) cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, gran);
-    cudaGetLastError();
-  }
+  cudaDeviceSetLimit(cudaLimitMaxL2FetchGranularity, 32);
+  cudaGetLastError();
   ctx->err.status = ACU_OK;
   ctx->err.index = -1;
   *out = ctx;

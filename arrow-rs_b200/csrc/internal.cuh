@@ -5,73 +5,62 @@
 struct acu_filter_plan;
 const uint64_t *acu_plan_mask(const acu_filter_plan *p);      // normalised mask words (padded to x32)
 const uint64_t *acu_plan_tile_off(const acu_filter_plan *p);  // exclusive output offset per 1024-row tile
-int64_t acu_plan_n_tiles(const acu_filter_plan *p);
 int64_t acu_plan_n_words_padded(const acu_filter_plan *p);
 void **acu_plan_index_cache(const acu_filter_plan *p);        // lazily materialised selected-row ids (bytes.cu)
 
-// FilterPredicate::filter_nulls (filter.rs:512-533) for any array kind.
-acu_status acu_filter_nulls_internal(acu_ctx *ctx, const acu_filter_plan *plan, const acu_array *a,
-                                     acu_array_out *out);
-
-// One column of filter / filter_record_batch, split so that several columns share one stream
-// synchronisation: launch queues the kernels (popcounts land in `res`, a device result block),
-// finalize turns the fetched block into the NullBuffer decision. kind: 0 primitive, 1 boolean,
-// 2 validity only.
-acu_status acu_filter_col_launch(acu_ctx *ctx, const acu_filter_plan *plan, int kind, int32_t elem_bytes,
-                                 const acu_array *values, acu_array_out *out, unsigned long long *res, int *mode);
-void acu_filter_col_finalize(const acu_filter_plan *plan, const acu_array *values, int mode,
-                             const unsigned long long *hres, acu_array_out *out);
-
-// Shared front end of take_primitive / take_boolean / take_bytes (take.cu).
-acu_status acu_take_common(acu_ctx *ctx, int32_t elem_bytes, const acu_array *values, bool boolean_values,
-                           const acu_array *indices, acu_dtype index_dtype, int32_t check_bounds,
-                           acu_array_out *out);
-
-// One column of take / take_record_batch (see acu_filter_col_launch for the split).
-acu_status acu_take_col_launch(acu_ctx *ctx, int32_t elem_bytes, const acu_array *values, bool boolean_values, bool val_nulls,
-                               const acu_array *indices, acu_dtype index_dtype, bool idx_nulls, acu_array_out *out,
-                               unsigned long long *res, int *mode);
+// The columns of filter / take / sum-min-max, split so that several columns share one stream synchronisation: launch
+// queues the kernels of every column, like columns sharing launches (blockIdx.y = column), with popcounts and results
+// landing in res[c], column c's device result block; finalize turns the fetched block into the NullBuffer decision.
+// The single-array calls are these launchers on one column.
+// filter kinds[c]: 0 primitive, 1 boolean, 2 validity only.
+acu_status acu_filter_cols_launch(acu_ctx *ctx, const acu_filter_plan *plan, int n, const int *kinds, const int32_t *widths,
+                                  const acu_array *const *values, acu_array_out *const *outs, unsigned long long *const *res, int *modes);
+void acu_filter_col_finalize(const acu_filter_plan *plan, int mode, const unsigned long long *hres, acu_array_out *out);
+acu_status acu_take_cols_launch(acu_ctx *ctx, int n, const int32_t *elem_bytes, const acu_array *const *values, const char *boolean,
+                                const char *val_nulls, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls,
+                                acu_array_out *const *outs, unsigned long long *const *res, int *modes);
 acu_status acu_take_col_finalize(acu_ctx *ctx, const acu_array *values, const acu_array *indices, acu_dtype index_dtype, int mode,
                                  const unsigned long long *hres, acu_array_out *out);
 acu_status acu_take_check_bounds(acu_ctx *ctx, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls, int64_t values_len);
 int acu_take_index_kind(acu_dtype t);  // -1 for non-integer index types
+// sum / min / max: nc[c] = resolved null count; result bits in res[c][RES_AUX0].
+size_t acu_reduce_col_scratch(const acu_ctx *ctx);
+acu_status acu_reduce_cols_launch(acu_ctx *ctx, int n, const acu_dtype *dtypes, const acu_agg_op *ops, const acu_array *arrays,
+                                  const int64_t *nc, uint8_t *scratch, size_t scratch_per_col, unsigned long long *const *res, int *launched);
 
-// Variable-width columns (bytes.cu), same launch / finalize split. nulls_mode < 0: the column's validity work is queued
-// here; >= 0: it was queued by the record-batch driver (acu_filter_cols_launch / acu_take_cols_launch) with that mode. `scratch` must hold
-// acu_bytes_col_scratch(output rows) bytes and stay untouched until the stream has drained.
-struct acu_bytes_col_state;
-acu_bytes_col_state *acu_bytes_col_state_new();
-void acu_bytes_col_state_free(acu_bytes_col_state *s);
+// Variable-width columns (bytes.cu), same launch / finalize split for the offsets and value bytes. The column's validity
+// is queued and finalised by the driver through acu_filter_cols_launch / acu_take_cols_launch, except take's copy of the
+// indices' validity when the values have no nulls. `scratch` must hold acu_bytes_col_scratch(output rows) bytes and
+// stay untouched until the stream has drained.
+struct acu_bytes_col_state {
+  bool gathered = false;          // the offsets / bytes gather was queued (output rows > 0)
+  bool idx_nulls_copied = false;  // take: the output validity is a copy of the indices' (valid count in RES_COUNT)
+  // the gather's arguments, for the finaliser's offset-overflow diagnosis and capacity check
+  int32_t ob = 0;
+  int kind = 0;
+  const void *offsets = nullptr, *idx = nullptr;
+  const uint8_t *data = nullptr, *out_valid = nullptr;
+  int64_t m = 0, n_src = 0;
+  bool detect_oob = false;
+  int64_t *block_tot = nullptr;
+  void *out_offsets = nullptr;
+  uint8_t *out_data = nullptr;
+  int64_t out_cap = 0;
+};
 size_t acu_bytes_col_scratch(int64_t out_rows);
 acu_status acu_plan_cached_indices(acu_ctx *ctx, const acu_filter_plan *plan, const void **out_idx, int *out_kind);
 acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const uint8_t *data, const acu_array *nulls_of,
                                      bool val_nulls, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls,
                                      void *out_offsets, uint8_t *out_data, int64_t out_cap, acu_array_out *out_nulls, void *scratch,
-                                     unsigned long long *res, acu_bytes_col_state *st, int nulls_mode);
+                                     unsigned long long *res, acu_bytes_col_state *st);
 acu_status acu_take_bytes_col_finalize(acu_ctx *ctx, const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype,
                                        const acu_bytes_col_state *st, const unsigned long long *hres, int64_t *out_data_len,
                                        acu_array_out *out_nulls);
 acu_status acu_filter_bytes_col_launch(acu_ctx *ctx, const acu_filter_plan *plan, int32_t ob, const void *offsets, const uint8_t *data,
-                                       const acu_array *nulls_of, void *out_offsets, uint8_t *out_data, int64_t out_cap,
-                                       acu_array_out *out_nulls, void *scratch, unsigned long long *res, acu_bytes_col_state *st,
-                                       int nulls_mode);
-acu_status acu_filter_bytes_col_finalize(acu_ctx *ctx, const acu_filter_plan *plan, const acu_array *nulls_of,
-                                         const acu_bytes_col_state *st, const unsigned long long *hres, int64_t *out_data_len,
-                                         acu_array_out *out_nulls);
-
-// One column of sum / min / max (reduce.cu): nc = resolved null count; result bits in res[RES_AUX0].
-size_t acu_reduce_col_scratch(const acu_ctx *ctx);
-acu_status acu_reduce_col_launch(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a, int64_t nc, void *scratch,
-                                 unsigned long long *res, int *launched);
-
-// Record-batch variants: the same per-column work with kernels of like columns sharing launches (blockIdx.y = column).
-acu_status acu_filter_cols_launch(acu_ctx *ctx, const acu_filter_plan *plan, int n, const int *kinds, const int32_t *widths,
-                                  const acu_array *const *values, acu_array_out *const *outs, unsigned long long *const *res, int *modes);
-acu_status acu_take_cols_launch(acu_ctx *ctx, int n, const int32_t *elem_bytes, const acu_array *const *values, const char *boolean,
-                                const char *val_nulls, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls,
-                                acu_array_out *const *outs, unsigned long long *const *res, int *modes);
-acu_status acu_reduce_cols_launch(acu_ctx *ctx, int n, const acu_dtype *dtypes, const acu_agg_op *ops, const acu_array *arrays,
-                                  const int64_t *nc, uint8_t *scratch, size_t scratch_per_col, unsigned long long *const *res, int *launched);
+                                       const acu_array *nulls_of, void *out_offsets, uint8_t *out_data, int64_t out_cap, void *scratch,
+                                       unsigned long long *res, acu_bytes_col_state *st);
+acu_status acu_filter_bytes_col_finalize(acu_ctx *ctx, const acu_bytes_col_state *st, const unsigned long long *hres,
+                                         int64_t *out_data_len);
 
 // Fused compare -> filter plan (elementwise.cu): the cmp kernels write the plan's mask words and per-tile counts.
 acu_status acu_cmp_result_len(acu_ctx *ctx, const acu_array *l, const acu_array *r, int64_t *out_len);

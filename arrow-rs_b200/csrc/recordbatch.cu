@@ -1,12 +1,12 @@
 // recordbatch.cu — RecordBatch-level entry points: every column of a batch goes through the
 // same per-column launch code as the single-array calls, but all kernels of all columns are
 // queued back to back on the ctx stream and the host synchronises ONCE (each column owns one
-// result block of ctx->d_res), instead of once or twice per column.
+// result block of ctx->d_res), instead of once or twice per column. filter_bytes / take_bytes
+// are these drivers on one variable-width column.
 //
 //   filter_record_batch   arrow-select/src/filter.rs:225-244, :459-478 (one predicate, all columns)
 //   take_record_batch     arrow-select/src/take.rs:1123-1133 (take_arrays :155-164)
 //   sum/min/max           arrow-arith/src/aggregate.rs:943,1012,1027 (one call per column in the reference)
-#include <memory>
 #include <vector>
 
 #include "bitmap.cuh"
@@ -14,20 +14,9 @@
 
 namespace {
 
-struct StateDeleter {
-  void operator()(acu_bytes_col_state *s) const { acu_bytes_col_state_free(s); }
-};
-using StatePtr = std::unique_ptr<acu_bytes_col_state, StateDeleter>;
-
 acu_status bad_columns(acu_ctx *ctx, int32_t n) {
   return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, (uint64_t)n, "record batch of %d columns: 0..%d supported per call", n,
                   ACU_MAX_BATCH_COLUMNS);
-}
-
-acu_status column_failed(acu_ctx *ctx, acu_status st, int32_t c) {
-  (void)ctx;
-  (void)c;  // like the reference, the error is the failing column's own ArrowError
-  return st;
 }
 
 acu_status bad_kind(acu_ctx *ctx, int32_t c, int32_t kind) {
@@ -35,11 +24,16 @@ acu_status bad_kind(acu_ctx *ctx, int32_t c, int32_t kind) {
   return ACU_ERR_INVALID_ARGUMENT;
 }
 
-}  // namespace
+// A failed launch may leave work queued: wait for it before returning the error (like the reference, the failing
+// column's own ArrowError).
+acu_status drain(acu_ctx *ctx, acu_status st) {
+  cudaStreamSynchronize(ctx->stream);
+  acu_kstats_drain(ctx);
+  return st;
+}
 
-extern "C" acu_status acu_filter_record_batch(acu_ctx *ctx, const acu_filter_plan *plan, int32_t n_columns,
-                                              const acu_column *columns, acu_column_out *outs) {
-  ACU_ENTER(ctx);
+acu_status filter_columns(acu_ctx *ctx, const acu_filter_plan *plan, int32_t n_columns, const acu_column *columns,
+                          acu_column_out *outs) {
   if (n_columns < 0 || n_columns > ACU_MAX_BATCH_COLUMNS) return bad_columns(ctx, n_columns);
   if (n_columns == 0) return ACU_OK;  // RecordBatch with no columns keeps only its row count (filter.rs:236-243)
   const int64_t count = acu_filter_plan_count(plan);
@@ -54,7 +48,7 @@ extern "C" acu_status acu_filter_record_batch(acu_ctx *ctx, const acu_filter_pla
   std::vector<const acu_array *> vals(n_columns);
   std::vector<acu_array_out *> outp(n_columns);
   std::vector<unsigned long long *> resp(n_columns);
-  std::vector<StatePtr> bstate(n_columns);
+  std::vector<acu_bytes_col_state> bstate(n_columns);
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
     if (col.kind != ACU_COL_PRIMITIVE && col.kind != ACU_COL_BOOLEAN && col.kind != ACU_COL_BYTES) return bad_kind(ctx, c, col.kind);
@@ -65,41 +59,29 @@ extern "C" acu_status acu_filter_record_batch(acu_ctx *ctx, const acu_filter_pla
     resp[c] = acu_dres(ctx, c);
   }
   ACU_TRY(acu_res_reset_n(ctx, n_columns));
-  auto drain = [&](acu_status st, int32_t c) {
-    cudaStreamSynchronize(ctx->stream);
-    acu_kstats_drain(ctx);
-    return column_failed(ctx, st, c);
-  };
   {  // values of fixed-width columns + every validity compaction, like columns sharing launches
     acu_status st = acu_filter_cols_launch(ctx, plan, n_columns, kinds.data(), widths.data(), vals.data(), outp.data(), resp.data(), mode.data());
-    if (st != ACU_OK) return drain(st, 0);
+    if (st != ACU_OK) return drain(ctx, st);
   }
   size_t k = 0;
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
     if (col.kind != ACU_COL_BYTES) continue;
-    bstate[c].reset(acu_bytes_col_state_new());
     acu_status st = acu_filter_bytes_col_launch(ctx, plan, col.width, col.array.values, col.data, &col.array, outs[c].array.values, outs[c].data,
-                                                outs[c].data_capacity, &outs[c].array, scratch + per_col * k++, acu_dres(ctx, c), bstate[c].get(), mode[c]);
-    if (st != ACU_OK) return drain(st, c);
+                                                outs[c].data_capacity, scratch + per_col * k++, acu_dres(ctx, c), &bstate[c]);
+    if (st != ACU_OK) return drain(ctx, st);
   }
   ACU_TRY(acu_res_fetch_n(ctx, n_columns));
   for (int32_t c = 0; c < n_columns; ++c) {
-    const acu_column &col = columns[c];
-    if (col.kind == ACU_COL_BYTES) {
-      acu_status st = acu_filter_bytes_col_finalize(ctx, plan, &col.array, bstate[c].get(), acu_hres(ctx, c), &outs[c].data_len, &outs[c].array);
-      if (st != ACU_OK) return column_failed(ctx, st, c);
-    } else {
-      acu_filter_col_finalize(plan, &col.array, mode[c], acu_hres(ctx, c), &outs[c].array);
-      outs[c].data_len = 0;
-    }
+    acu_filter_col_finalize(plan, mode[c], acu_hres(ctx, c), &outs[c].array);
+    outs[c].data_len = 0;
+    if (columns[c].kind == ACU_COL_BYTES) ACU_TRY(acu_filter_bytes_col_finalize(ctx, &bstate[c], acu_hres(ctx, c), &outs[c].data_len));
   }
   return ACU_OK;
 }
 
-extern "C" acu_status acu_take_record_batch(acu_ctx *ctx, int32_t n_columns, const acu_column *columns, const acu_array *indices,
-                                            acu_dtype index_dtype, int32_t check_bounds, acu_column_out *outs) {
-  ACU_ENTER(ctx);
+acu_status take_columns(acu_ctx *ctx, int32_t n_columns, const acu_column *columns, const acu_array *indices, acu_dtype index_dtype,
+                        int32_t check_bounds, acu_column_out *outs) {
   if (n_columns < 0 || n_columns > ACU_MAX_BATCH_COLUMNS) return bad_columns(ctx, n_columns);
   if (n_columns == 0) return ACU_OK;
   if (acu_take_index_kind(index_dtype) < 0)  // take.rs:103
@@ -113,11 +95,10 @@ extern "C" acu_status acu_take_record_batch(acu_ctx *ctx, int32_t n_columns, con
   int64_t checked_len = -1;
   for (int32_t c = 0; c < n_columns; ++c) {  // host-visible facts first: anything that needs its own sync
     const int64_t vnc = acu_resolve_null_count(ctx, &columns[c].array, &st);
-    if (st != ACU_OK) return column_failed(ctx, st, c);
+    ACU_TRY(st);
     val_nulls[c] = columns[c].array.validity && vnc > 0;
     if (check_bounds && columns[c].array.len != checked_len) {  // the columns of a RecordBatch share one length: normally once
-      st = acu_take_check_bounds(ctx, indices, index_dtype, idx_nulls, columns[c].array.len);
-      if (st != ACU_OK) return column_failed(ctx, st, c);
+      ACU_TRY(acu_take_check_bounds(ctx, indices, index_dtype, idx_nulls, columns[c].array.len));
       checked_len = columns[c].array.len;
     }
   }
@@ -126,8 +107,8 @@ extern "C" acu_status acu_take_record_batch(acu_ctx *ctx, int32_t n_columns, con
   for (int32_t c = 0; c < n_columns; ++c) n_bytes_cols += columns[c].kind == ACU_COL_BYTES;
   uint8_t *scratch = nullptr;
   if (n_bytes_cols) ACU_TRY(acu_scratch(ctx, per_col * n_bytes_cols, reinterpret_cast<void **>(&scratch)));
-  std::vector<int> mode(n_columns, -1);
-  std::vector<StatePtr> bstate(n_columns);
+  std::vector<int> mode(n_columns, -1);  // -1: no validity gather queued for the column
+  std::vector<acu_bytes_col_state> bstate(n_columns);
   // fixed-width / boolean columns, and the validity gather of variable-width columns whose values have nulls:
   // like columns share launches
   std::vector<int32_t> eb;
@@ -149,40 +130,96 @@ extern "C" acu_status acu_take_record_batch(acu_ctx *ctx, int32_t n_columns, con
     who.push_back(c);
   }
   ACU_TRY(acu_res_reset_n(ctx, n_columns));
-  auto drain = [&](acu_status s, int32_t c) {
-    cudaStreamSynchronize(ctx->stream);
-    acu_kstats_drain(ctx);
-    return column_failed(ctx, s, c);
-  };
   if (!who.empty()) {
     std::vector<int> modes(who.size(), 0);
     st = acu_take_cols_launch(ctx, (int)who.size(), eb.data(), vals.data(), isbool.data(), vnulls.data(), indices, index_dtype, idx_nulls,
                               outp.data(), resp.data(), modes.data());
-    if (st != ACU_OK) return drain(st, who[0]);
+    if (st != ACU_OK) return drain(ctx, st);
     for (size_t i = 0; i < who.size(); ++i) mode[who[i]] = modes[i];
   }
   size_t k = 0;
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
     if (col.kind != ACU_COL_BYTES) continue;
-    bstate[c].reset(acu_bytes_col_state_new());
     st = acu_take_bytes_col_launch(ctx, col.width, col.array.values, col.data, &col.array, val_nulls[c], indices, index_dtype, idx_nulls,
                                    outs[c].array.values, outs[c].data, outs[c].data_capacity, &outs[c].array, scratch + per_col * k++,
-                                   acu_dres(ctx, c), bstate[c].get(), val_nulls[c] ? mode[c] : -1);
-    if (st != ACU_OK) return drain(st, c);
+                                   acu_dres(ctx, c), &bstate[c]);
+    if (st != ACU_OK) return drain(ctx, st);
   }
   ACU_TRY(acu_res_fetch_n(ctx, n_columns));
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
+    outs[c].data_len = 0;
+    if (mode[c] >= 0) ACU_TRY(acu_take_col_finalize(ctx, &col.array, indices, index_dtype, mode[c], acu_hres(ctx, c), &outs[c].array));
     if (col.kind == ACU_COL_BYTES)
-      st = acu_take_bytes_col_finalize(ctx, &col.array, indices, index_dtype, bstate[c].get(), acu_hres(ctx, c), &outs[c].data_len, &outs[c].array);
-    else {
-      st = acu_take_col_finalize(ctx, &col.array, indices, index_dtype, mode[c], acu_hres(ctx, c), &outs[c].array);
-      outs[c].data_len = 0;
-    }
-    if (st != ACU_OK) return column_failed(ctx, st, c);
+      ACU_TRY(acu_take_bytes_col_finalize(ctx, &col.array, indices, index_dtype, &bstate[c], acu_hres(ctx, c), &outs[c].data_len, &outs[c].array));
   }
   return ACU_OK;
+}
+
+// One Utf8 / Binary array as an ACU_COL_BYTES column: `array` carries the nulls, its values the offsets.
+acu_column bytes_column(int32_t offset_bytes, const void *offsets, const uint8_t *data, const acu_array *nulls_of) {
+  acu_column col{};
+  col.kind = ACU_COL_BYTES;
+  col.width = offset_bytes;
+  col.array = *nulls_of;
+  col.array.values = offsets;
+  col.data = data;
+  return col;
+}
+
+acu_column_out bytes_column_out(void *out_offsets, uint8_t *out_data, int64_t out_data_capacity, const acu_array_out *out_nulls) {
+  acu_column_out out{};
+  out.array = *out_nulls;
+  out.array.values = out_offsets;
+  out.data = out_data;
+  out.data_capacity = out_data_capacity;
+  return out;
+}
+
+// What the single-array byte calls return: the data length and the NullBuffer decision.
+acu_status bytes_result(const acu_column_out &out, acu_status st, int64_t *out_data_len, acu_array_out *out_nulls) {
+  *out_data_len = out.data_len;
+  out_nulls->len = out.array.len;
+  out_nulls->null_count = out.array.null_count;
+  out_nulls->has_validity = out.array.has_validity;
+  return st;
+}
+
+}  // namespace
+
+extern "C" acu_status acu_filter_record_batch(acu_ctx *ctx, const acu_filter_plan *plan, int32_t n_columns,
+                                              const acu_column *columns, acu_column_out *outs) {
+  ACU_ENTER(ctx);
+  return filter_columns(ctx, plan, n_columns, columns, outs);
+}
+
+extern "C" acu_status acu_take_record_batch(acu_ctx *ctx, int32_t n_columns, const acu_column *columns, const acu_array *indices,
+                                            acu_dtype index_dtype, int32_t check_bounds, acu_column_out *outs) {
+  ACU_ENTER(ctx);
+  return take_columns(ctx, n_columns, columns, indices, index_dtype, check_bounds, outs);
+}
+
+extern "C" acu_status acu_filter_bytes(acu_ctx *ctx, const acu_filter_plan *plan, int32_t offset_bytes,
+                                       const void *offsets, const uint8_t *data, const acu_array *nulls_of,
+                                       void *out_offsets, uint8_t *out_data, int64_t out_data_capacity,
+                                       int64_t *out_data_len, acu_array_out *out_nulls) {
+  ACU_ENTER(ctx);
+  const acu_column col = bytes_column(offset_bytes, offsets, data, nulls_of);
+  acu_column_out out = bytes_column_out(out_offsets, out_data, out_data_capacity, out_nulls);
+  const acu_status st = filter_columns(ctx, plan, 1, &col, &out);
+  return bytes_result(out, st, out_data_len, out_nulls);
+}
+
+extern "C" acu_status acu_take_bytes(acu_ctx *ctx, int32_t offset_bytes, const void *offsets, const uint8_t *data,
+                                     const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype,
+                                     int32_t check_bounds, void *out_offsets, uint8_t *out_data,
+                                     int64_t out_data_capacity, int64_t *out_data_len, acu_array_out *out_nulls) {
+  ACU_ENTER(ctx);
+  const acu_column col = bytes_column(offset_bytes, offsets, data, nulls_of);
+  acu_column_out out = bytes_column_out(out_offsets, out_data, out_data_capacity, out_nulls);
+  const acu_status st = take_columns(ctx, 1, &col, indices, index_dtype, check_bounds, &out);
+  return bytes_result(out, st, out_data_len, out_nulls);
 }
 
 extern "C" acu_status acu_aggregate_columns(acu_ctx *ctx, int32_t n_columns, const acu_dtype *dtypes, const acu_agg_op *ops,
@@ -195,7 +232,7 @@ extern "C" acu_status acu_aggregate_columns(acu_ctx *ctx, int32_t n_columns, con
   for (int32_t c = 0; c < n_columns; ++c) {
     out_bits[c] = 0;
     nc[c] = acu_resolve_null_count(ctx, &arrays[c], &st);
-    if (st != ACU_OK) return column_failed(ctx, st, c);
+    ACU_TRY(st);
     out_valid_counts[c] = arrays[c].len - nc[c];
   }
   const size_t per_col = (acu_reduce_col_scratch(ctx) + 255) & ~(size_t)255;
@@ -206,11 +243,7 @@ extern "C" acu_status acu_aggregate_columns(acu_ctx *ctx, int32_t n_columns, con
   for (int32_t c = 0; c < n_columns; ++c) resp[c] = acu_dres(ctx, c);
   ACU_TRY(acu_res_reset_n(ctx, n_columns));
   st = acu_reduce_cols_launch(ctx, n_columns, dtypes, ops, arrays, nc.data(), scratch, per_col, resp.data(), launched.data());
-  if (st != ACU_OK) {
-    cudaStreamSynchronize(ctx->stream);
-    acu_kstats_drain(ctx);
-    return st;
-  }
+  if (st != ACU_OK) return drain(ctx, st);
   ACU_TRY(acu_res_fetch_n(ctx, n_columns));
   for (int32_t c = 0; c < n_columns; ++c)
     if (launched[c]) out_bits[c] = acu_hres(ctx, c)[RES_AUX0];

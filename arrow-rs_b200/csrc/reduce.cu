@@ -218,28 +218,16 @@ ReduceArgs reduce_args(const acu_array *a, int64_t nc, void *scratch, unsigned l
 // per-column scratch of one queued reduction: one partial per CTA of the widest grid
 size_t acu_reduce_col_scratch(const acu_ctx *ctx) { return (size_t)ctx->sm_count * 8 * 8 * 16 + 4096; }
 
-// Queue sum / min / max of one column on the ctx stream (no sync). The caller has resolved the
-// null count (nc < 0: unknown, the kernel consults the validity and counts): nc == len (or len == 0) means None and
-// nothing is launched (*launched = 0). The
-// result lands in res[RES_AUX0] as the native bit pattern.
-acu_status acu_reduce_col_launch(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a, int64_t nc, void *scratch,
-                                 unsigned long long *res, int *launched) {
-  *launched = 0;
-  if (a->len == 0 || nc == a->len) return ACU_OK;  // aggregate.rs:320-323
-  ReduceBatch rb{};
-  rb.col[0] = reduce_args(a, nc, scratch, res);
-  ACU_TRY(reduce_dispatch(ctx, dtype, op, rb, 1, a->len));
-  *launched = 1;
-  return ACU_OK;
-}
-
-// Several columns: those with the same (dtype, op) share a launch (blockIdx.y = column).
+// Queue sum / min / max of columns on the ctx stream (no sync); those with the same (dtype, op) share a launch
+// (blockIdx.y = column). The caller has resolved the null counts (nc[c] < 0: unknown, the kernel consults the validity
+// and counts): nc[c] == len (or len == 0) means None and nothing is launched for the column (launched[c] = 0). The
+// result lands in res[c][RES_AUX0] as the native bit pattern.
 acu_status acu_reduce_cols_launch(acu_ctx *ctx, int n, const acu_dtype *dtypes, const acu_agg_op *ops, const acu_array *arrays,
                                   const int64_t *nc, uint8_t *scratch, size_t scratch_per_col, unsigned long long *const *res, int *launched) {
   char done[ACU_MAX_BATCH_COLUMNS] = {0};
   for (int c = 0; c < n; ++c) {
     launched[c] = 0;
-    if (arrays[c].len == 0 || nc[c] == arrays[c].len) done[c] = 1;  // None
+    if (arrays[c].len == 0 || nc[c] == arrays[c].len) done[c] = 1;  // None (aggregate.rs:320-323)
   }
   for (int c = 0; c < n; ++c) {
     if (done[c]) continue;
@@ -271,12 +259,14 @@ extern "C" acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op
   const int64_t nc = deferred_nc ? -1 : acu_resolve_null_count(ctx, a, &st);
   ACU_TRY(st);
   if (!deferred_nc) *out_valid_count = a->len - nc;
+  const size_t scratch_bytes = acu_reduce_col_scratch(ctx);
   void *scratch;
-  ACU_TRY(acu_scratch(ctx, acu_reduce_col_scratch(ctx), &scratch));
+  ACU_TRY(acu_scratch(ctx, scratch_bytes, &scratch));
   int launched = 0;
   const int blk = acu_call_begin(ctx, &st);
   ACU_TRY(st);
-  ACU_TRY(acu_reduce_col_launch(ctx, dtype, op, a, nc, scratch, acu_dres(ctx, blk), &launched));
+  unsigned long long *res = acu_dres(ctx, blk);
+  ACU_TRY(acu_reduce_cols_launch(ctx, 1, &dtype, &op, a, &nc, static_cast<uint8_t *>(scratch), scratch_bytes, &res, &launched));
   if (!launched && !ctx->async_on) return ACU_OK;
   return acu_call_end(ctx, blk, [launched, deferred_nc, out_bits, out_valid_count](const unsigned long long *h) -> acu_status {
     if (!launched) return ACU_OK;

@@ -314,11 +314,9 @@ acu_status fetch_index(acu_ctx *ctx, const acu_array *indices, acu_dtype t, int6
 
 }  // namespace
 
-// Shared front end of take_primitive / take_boolean / take_bytes' null handling.
-// `elem_bytes` == 0: no value gather (bits / nulls only).
-acu_status acu_take_common(acu_ctx *ctx, int32_t elem_bytes, const acu_array *values, bool boolean_values,
-                           const acu_array *indices, acu_dtype index_dtype, int32_t check_bounds,
-                           acu_array_out *out) {
+// take_primitive / take_boolean: the record-batch launcher on one column.
+static acu_status take_array(acu_ctx *ctx, int32_t elem_bytes, const acu_array *values, bool boolean_values,
+                             const acu_array *indices, acu_dtype index_dtype, int32_t check_bounds, acu_array_out *out) {
   ACU_ENTER(ctx);
   const int kind = index_kind(index_dtype);
   if (kind < 0)  // take.rs:103
@@ -335,21 +333,19 @@ acu_status acu_take_common(acu_ctx *ctx, int32_t elem_bytes, const acu_array *va
   if (m == 0) return ACU_OK;  // take_impl: new_empty_array (take.rs:216-218)
   const int64_t vnc = acu_resolve_null_count(ctx, values, &st);
   ACU_TRY(st);
-  const bool val_nulls = values->validity && vnc > 0;  // take_nulls (take.rs:419-430)
+  const char val_nulls = values->validity && vnc > 0;  // take_nulls (take.rs:419-430)
+  const char is_bool = boolean_values;
   int mode = 0;
   const int blk = acu_call_begin(ctx, &st);
   ACU_TRY(st);
-  ACU_TRY(acu_take_col_launch(ctx, elem_bytes, values, boolean_values, val_nulls, indices, index_dtype, idx_nulls, out, acu_dres(ctx, blk), &mode));
+  unsigned long long *res = acu_dres(ctx, blk);
+  ACU_TRY(acu_take_cols_launch(ctx, 1, &elem_bytes, &values, &is_bool, &val_nulls, indices, index_dtype, idx_nulls, &out, &res, &mode));
   const acu_array v = *values, ix = *indices;  // the finaliser may run later (acu_results_fetch): keep copies of the descriptors
   return acu_call_end(ctx, blk, [ctx, v, ix, index_dtype, mode, out](const unsigned long long *h) -> acu_status {
     return acu_take_col_finalize(ctx, &v, &ix, index_dtype, mode, h, out);
   });
 }
 
-// One column of take / take_record_batch: queue the gather on the ctx stream without
-// synchronising. val_nulls / idx_nulls = "has a validity buffer with at least one null"
-// (exact, the NullBuffer decision depends on it). *mode: bit 0 = an output validity was
-// produced, bit 1 = it came from take_bits(values.nulls) (None when it has no nulls).
 static TakeArgs take_args(int32_t elem_bytes, const acu_array *values, bool boolean_values, bool val_nulls, const acu_array *indices,
                           acu_dtype /*index_dtype*/, bool idx_nulls, acu_array_out *out, unsigned long long *res) {
   TakeArgs ta{};
@@ -368,25 +364,11 @@ static TakeArgs take_args(int32_t elem_bytes, const acu_array *values, bool bool
   return ta;
 }
 
-acu_status acu_take_col_launch(acu_ctx *ctx, int32_t elem_bytes, const acu_array *values, bool boolean_values, bool val_nulls,
-                               const acu_array *indices, acu_dtype index_dtype, bool idx_nulls, acu_array_out *out,
-                               unsigned long long *res, int *mode) {
-  *mode = 0;
-  const int kind = index_kind(index_dtype);
-  out->len = indices->len;
-  out->has_validity = 0;
-  out->null_count = 0;
-  if (indices->len == 0) return ACU_OK;
-  TakeBatch tb{};
-  tb.col[0] = take_args(elem_bytes, values, boolean_values, val_nulls, indices, index_dtype, idx_nulls, out, res);
-  ACU_TRY(launch_take(ctx, tb.col[0].values ? elem_bytes : 1, kind, tb, 1));
-  *mode = (tb.col[0].out_valid ? 1 : 0) | (val_nulls ? 2 : 0);
-  return ACU_OK;
-}
-
-// All columns of a take_record_batch: columns that run the same kernel instantiation (element width / boolean /
-// validity-only) share a launch. elem_bytes[c] == 0 with boolean[c] == 0 is the validity-only gather of a
-// variable-width column.
+// The columns of take / take_record_batch: queue the gathers on the ctx stream without synchronising. Columns that run
+// the same kernel instantiation (element width / boolean / validity-only) share a launch. elem_bytes[c] == 0 with
+// boolean[c] == 0 is the validity-only gather of a variable-width column. val_nulls / idx_nulls = "has a validity
+// buffer with at least one null" (exact, the NullBuffer decision depends on it). modes[c]: bit 0 = an output validity
+// was produced, bit 1 = it came from take_bits(values.nulls) (None when it has no nulls).
 acu_status acu_take_cols_launch(acu_ctx *ctx, int n, const int32_t *elem_bytes, const acu_array *const *values, const char *boolean,
                                 const char *val_nulls, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls,
                                 acu_array_out *const *outs, unsigned long long *const *res, int *modes) {
@@ -398,7 +380,8 @@ acu_status acu_take_cols_launch(acu_ctx *ctx, int n, const int32_t *elem_bytes, 
     outs[c]->null_count = 0;
   }
   if (indices->len == 0) return ACU_OK;
-  auto klass = [&](int c) { return boolean[c] ? -1 : (elem_bytes[c] > 0 ? elem_bytes[c] : 0); };  // kernel instantiation of column c
+  // kernel instantiation of column c: a column without a value buffer gathers its validity only
+  auto klass = [&](int c) { return boolean[c] ? -1 : (elem_bytes[c] > 0 && values[c]->values ? elem_bytes[c] : 0); };
   char done[ACU_MAX_BATCH_COLUMNS] = {0};
   for (int c = 0; c < n; ++c) {
     if (done[c]) continue;
@@ -481,10 +464,10 @@ int acu_take_index_kind(acu_dtype t) { return index_kind(t); }
 extern "C" acu_status acu_take_primitive(acu_ctx *ctx, int32_t elem_bytes, const acu_array *values,
                                          const acu_array *indices, acu_dtype index_dtype,
                                          int32_t check_bounds, acu_array_out *out) {
-  return acu_take_common(ctx, elem_bytes, values, false, indices, index_dtype, check_bounds, out);
+  return take_array(ctx, elem_bytes, values, false, indices, index_dtype, check_bounds, out);
 }
 
 extern "C" acu_status acu_take_boolean(acu_ctx *ctx, const acu_array *values, const acu_array *indices,
                                        acu_dtype index_dtype, int32_t check_bounds, acu_array_out *out) {
-  return acu_take_common(ctx, 0, values, true, indices, index_dtype, check_bounds, out);
+  return take_array(ctx, 0, values, true, indices, index_dtype, check_bounds, out);
 }

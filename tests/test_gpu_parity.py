@@ -378,18 +378,21 @@ def test_take_wide_elements(gpu, oracle, width):
     import ctypes as C
     rng = np.random.default_rng(90 + width)
     lanes = width // 8
-    for n, m in [(1, 5), (100, 0), (4097, 9000), (9000, 4097)]:
+    for n, m in [(1, 5), (100, 0), (4097, 9000), (9000, 4097), (0, 6)]:
         raw = rng.integers(0, 2**63, n * lanes, dtype=np.uint64)
         mask = rng.random(n) >= 0.2
         col, owned = _wide_column(gpu, raw, n, width, mask)
-        idx_h = HostArray.from_numpy(abi.U32, rng.integers(0, n, m).astype(np.uint32), rng.random(m) >= 0.1)
+        if n == 0:  # an empty column without a value buffer, taken at null indices only
+            col.values = None
+        idx_h = HostArray.from_numpy(abi.U32, rng.integers(0, max(n, 1), m).astype(np.uint32),
+                                     rng.random(m) >= 0.1 if n else np.zeros(m, dtype=bool))
         di = gpu.upload(idx_h)
         out = gpu.alloc_out(m * width, m)
         idd = di.descriptor()
         gpu.check(gpu.lib.acu_take_primitive(gpu.h, width, C.byref(col), C.byref(idd), abi.U32, 0, C.byref(out)))
         vals, valid = _wide_result(gpu, out, width)
         ix, iv = idx_h.value_array(), idx_h.valid_mask()
-        assert np.array_equal(valid, mask[ix] & iv)
+        assert np.array_equal(valid, (mask[ix] if n else False) & iv)
         assert np.array_equal(vals[iv], raw.reshape(n, lanes)[ix[iv]])  # the value is gathered wherever the index is valid
         gpu._free_out(out)
         di.free()
