@@ -874,7 +874,7 @@ acu_status acu_filter_plan_create_cmp(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op 
   *out_plan = nullptr;
   ACU_ENTER(ctx);
   int64_t len = 0;
-  ACU_TRY(acu_cmp_result_len(ctx, a, b, &len));
+  ACU_TRY(acu_cmp_len(ctx, a, b, &len));
   acu_filter_plan *plan = nullptr;
   ACU_TRY(plan_alloc(ctx, len, &plan));
   if (len == 0) { *out_plan = plan; return ACU_OK; }

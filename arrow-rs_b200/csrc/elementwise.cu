@@ -16,6 +16,7 @@
 #include <type_traits>
 
 #include "bitmap.cuh"
+#include "internal.cuh"
 
 namespace {
 
@@ -315,17 +316,6 @@ acu_status arith_error(acu_ctx *ctx, acu_arith_op op, bool is_neg, const acu_arr
                   "Overflow happened on: %s %s %s", ls, op_symbol(op), rs);
 }
 
-acu_status set_new_null(acu_ctx *ctx, int64_t len, size_t value_bytes, acu_array_out *out) {
-  // PrimitiveArray::new_null / BooleanArray::new_null: zeroed values, all-null bitmap
-  if (value_bytes) ACU_CUDA(ctx, cudaMemsetAsync(out->values, 0, value_bytes, ctx->stream));
-  if (len) ACU_CUDA(ctx, cudaMemsetAsync(out->validity, 0, acu_bitmap_bytes(len), ctx->stream));
-  ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  out->len = len;
-  out->has_validity = 1;
-  out->null_count = len;
-  return ACU_OK;
-}
-
 template <class T>
 acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const acu_array *b, acu_array_out *out) {
   const bool checked = !is_fp<T>::value && (op == ACU_ADD || op == ACU_SUB || op == ACU_MUL || op == ACU_DIV || op == ACU_REM);
@@ -353,7 +343,7 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
     len = arr->len;
     int64_t snc = acu_resolve_null_count(ctx, s, &st);
     ACU_TRY(st);
-    if (snc != 0) return set_new_null(ctx, len, (size_t)len * sizeof(T), out);
+    if (snc != 0) return acu_new_null(ctx, len, (size_t)len * sizeof(T), out);
     out->len = len;
     if (len == 0) { out->has_validity = arr->validity != nullptr; return ACU_OK; }
     if (arr->validity) {  // nulls().cloned()
@@ -449,8 +439,6 @@ acu_status neg_typed(acu_ctx *ctx, int32_t checked_in, const acu_array *a, acu_a
 // ---------------------------------------------------------------------------------------
 // cmp — one result bit per row (collect_bool, cmp.rs:580-611)
 // ---------------------------------------------------------------------------------------
-enum { FOLD_NONE = 0, FOLD_DISTINCT = 1, FOLD_NOT_DISTINCT = 2 };
-
 template <class T>
 struct CmpParams {
   const T *a, *b;
@@ -634,70 +622,50 @@ template <class T>
 acu_status cmp_typed(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_array *r, acu_array_out *out, const CmpFuse *fuse = nullptr) {
   acu_array_out scratch_out{};
   if (fuse) out = &scratch_out;
-  const bool ls = l->is_scalar != 0, rs = r->is_scalar != 0;
-  if (l->len != r->len && !ls && !rs)  // cmp.rs:228-232
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0,
-                    "Cannot compare arrays of different lengths, got %lld vs %lld", (long long)l->len, (long long)r->len);
-  const int64_t len = ls ? r->len : l->len;
-  out->len = len;
-  out->has_validity = 0;
-  out->null_count = 0;
+  acu_cmp_decision d;
+  ACU_TRY(acu_cmp_decide(ctx, op, l, r, out, &d));
+  const int64_t len = d.len;
   if (len == 0) return ACU_OK;
-  acu_status st;
-  const int64_t lnc = acu_resolve_null_count(ctx, l, &st);
-  ACU_TRY(st);
-  const int64_t rnc = acu_resolve_null_count(ctx, r, &st);
-  ACU_TRY(st);
-  const bool ln = lnc > 0, rn = rnc > 0;  // logical_nulls().filter(null_count > 0)
-  const bool fold = op == ACU_DISTINCT || op == ACU_NOT_DISTINCT;
-  const bool l_null_scalar = ls && ln, r_null_scalar = rs && rn;
   if (fuse) {  // words past the data (the plan pads its mask to a multiple of 32 words) select nothing
     const int64_t used = (len + 63) / 64;
     if (fuse->n_words_padded > used)
       ACU_CUDA(ctx, cudaMemsetAsync(fuse->mask + used, 0, (size_t)(fuse->n_words_padded - used) * 8, ctx->stream));
   }
-  if (!fold && (l_null_scalar || r_null_scalar) && !(ls && rs)) {
-    // a null scalar against an array: BooleanArray::new_null(len) (cmp.rs:353, :364)
+  if (d.all_null) {
     if (fuse) {  // an all-null predicate selects nothing
       ACU_CUDA(ctx, cudaMemsetAsync(fuse->mask, 0, (size_t)fuse->n_words_padded * 8, ctx->stream));
       ACU_CUDA(ctx, cudaMemsetAsync(fuse->tile_count, 0, (size_t)fuse->n_tiles * 4, ctx->stream));
       return ACU_OK;
     }
-    ACU_CUDA(ctx, cudaMemsetAsync(out->values, 0, acu_bitmap_bytes(len), ctx->stream));
-    return set_new_null(ctx, len, 0, out);
+    return acu_new_null(ctx, len, acu_bitmap_bytes(len), out);
   }
   CmpParams<T> p{};
+  p.a = static_cast<const T *>((d.swap ? r : l)->values);
+  p.b = static_cast<const T *>((d.swap ? l : r)->values);
   p.n = len;
-  p.res = ctx->d_res;
+  p.av = d.av; p.aoff = d.aoff;
+  p.bv = d.bv; p.boff = d.boff;
+  p.a_scalar = d.a_scalar; p.a_null_scalar = d.a_null_scalar;
+  p.b_scalar = d.b_scalar; p.b_null_scalar = d.b_null_scalar;
+  p.neg = d.neg;
+  p.fold = d.fold;
   p.out_bits = fuse ? fuse->mask : static_cast<uint64_t *>(out->values);
+  if (d.has_validity && !fuse) p.out_valid = reinterpret_cast<uint64_t *>(out->validity);
+  p.res = ctx->d_res;
   if (fuse) { p.fuse = 1; p.tile_count = fuse->tile_count; }
-  // Less / Greater family: gt and lt_eq swap the operands (cmp.rs:481-488)
-  const bool swap = (op == ACU_GT || op == ACU_LT_EQ);
-  const acu_array *x = swap ? r : l, *y = swap ? l : r;
-  const bool xs = x->is_scalar != 0, ys = y->is_scalar != 0;
-  const bool xn = swap ? rn : ln, yn = swap ? ln : rn;
-  p.a = static_cast<const T *>(x->values);
-  p.b = static_cast<const T *>(y->values);
-  p.a_scalar = xs && !(xs && ys);
-  p.b_scalar = ys && !(xs && ys);
-  p.neg = (op == ACU_NEQ || op == ACU_DISTINCT || op == ACU_LT_EQ || op == ACU_GT_EQ);
-  p.fold = op == ACU_DISTINCT ? FOLD_DISTINCT : op == ACU_NOT_DISTINCT ? FOLD_NOT_DISTINCT : FOLD_NONE;
-  if (xn) { if (xs && !(xs && ys)) p.a_null_scalar = 1; else { p.av = x->validity; p.aoff = x->validity_offset; } }
-  if (yn) { if (ys && !(xs && ys)) p.b_null_scalar = 1; else { p.bv = y->validity; p.boff = y->validity_offset; } }
-  if (!fold && (xn || yn) && !fuse) p.out_valid = reinterpret_cast<uint64_t *>(out->validity);
   int blk = 0;
   if (!fuse) {
+    acu_status st;
     blk = acu_call_begin(ctx, &st);
     ACU_TRY(st);
     p.res = acu_dres(ctx, blk);
   }
-  const bool lt = !(op == ACU_EQ || op == ACU_NEQ || fold);
   // streaming head over whole 2048-row super-groups when the value pointers are 16-B aligned
   const bool aligned = (p.a_scalar || (uintptr_t)p.a % 16 == 0) && (p.b_scalar || (uintptr_t)p.b % 16 == 0);
   const int64_t sgroups = aligned ? len / 2048 : 0;
   if (sgroups > 0) {
     const int64_t blocks = (sgroups + 7) / 8;
-    if (lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp_v2<T, true>), acu_wave_grid(ctx, k_cmp_v2<T, true>, 256, 0, blocks), 256, 0, p, sgroups);
+    if (d.lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp_v2<T, true>), acu_wave_grid(ctx, k_cmp_v2<T, true>, 256, 0, blocks), 256, 0, p, sgroups);
     else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp_v2<T, false>), acu_wave_grid(ctx, k_cmp_v2<T, false>, 256, 0, blocks), 256, 0, p, sgroups);
   }
   const int64_t head = sgroups * 2048;
@@ -712,7 +680,7 @@ acu_status cmp_typed(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_
     if (q.out_valid) q.out_valid += head >> 6;
     const int64_t strips = (q.n + 63) >> 6;
     const int64_t blocks = (strips + 31) / 32;
-    if (lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, true>), acu_wave_grid(ctx, k_cmp<T, true>, 256, 0, blocks), 256, 0, q);
+    if (d.lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, true>), acu_wave_grid(ctx, k_cmp<T, true>, 256, 0, blocks), 256, 0, q);
     else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, false>), acu_wave_grid(ctx, k_cmp<T, false>, 256, 0, blocks), 256, 0, q);
     if (fuse) {  // the tail's tiles (head is a multiple of 2048 rows = 2 tiles)
       const int64_t first_tile = head >> 10, rest = fuse->n_tiles - first_tile;
@@ -720,12 +688,8 @@ acu_status cmp_typed(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_
     }
   }
   if (fuse) return ACU_OK;  // stream-ordered: the plan's scan kernels follow on the same stream
-  const bool has_valid = p.out_valid != nullptr;
-  return acu_call_end(ctx, blk, [has_valid, len, out](const unsigned long long *h) -> acu_status {
-    if (has_valid) {
-      out->has_validity = 1;
-      out->null_count = len - (int64_t)h[RES_COUNT];
-    }
+  return acu_call_end(ctx, blk, [d, out](const unsigned long long *h) -> acu_status {
+    acu_cmp_finalize(d, h, out);
     return ACU_OK;
   });
 }
@@ -970,16 +934,66 @@ extern "C" acu_status acu_cmp(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, cons
   return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid comparison operation: dtype %d", (int)dtype);
 }
 
-// The comparison of acu_cmp written straight into a filter plan's mask / tile counts (compact.cu: acu_filter_plan_create_cmp).
-// Stream-ordered, no synchronisation. *out_len = the result length (cmp.rs:228-235).
-acu_status acu_cmp_result_len(acu_ctx *ctx, const acu_array *l, const acu_array *r, int64_t *out_len) {
+acu_status acu_cmp_len(acu_ctx *ctx, const acu_array *l, const acu_array *r, int64_t *len) {
   const bool ls = l->is_scalar != 0, rs = r->is_scalar != 0;
-  if (l->len != r->len && !ls && !rs)
+  if (l->len != r->len && !ls && !rs)  // cmp.rs:228-232
     return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0,
                     "Cannot compare arrays of different lengths, got %lld vs %lld", (long long)l->len, (long long)r->len);
-  *out_len = ls ? r->len : l->len;
+  *len = ls ? r->len : l->len;
   return ACU_OK;
 }
+
+acu_status acu_cmp_decide(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_array *r, acu_array_out *out,
+                          acu_cmp_decision *d) {
+  *d = acu_cmp_decision{};
+  ACU_TRY(acu_cmp_len(ctx, l, r, &d->len));
+  out->len = d->len;
+  out->has_validity = 0;
+  out->null_count = 0;
+  if (d->len == 0) return ACU_OK;
+  acu_status st;
+  const int64_t lnc = acu_resolve_null_count(ctx, l, &st);
+  ACU_TRY(st);
+  const int64_t rnc = acu_resolve_null_count(ctx, r, &st);
+  ACU_TRY(st);
+  const bool ls = l->is_scalar != 0, rs = r->is_scalar != 0;
+  const bool ln = lnc > 0, rn = rnc > 0;  // logical_nulls().filter(null_count > 0)
+  const bool fold = op == ACU_DISTINCT || op == ACU_NOT_DISTINCT;
+  d->all_null = !fold && ((ls && ln) || (rs && rn)) && !(ls && rs);
+  if (d->all_null) return ACU_OK;
+  d->swap = op == ACU_GT || op == ACU_LT_EQ;
+  const acu_array *x = d->swap ? r : l, *y = d->swap ? l : r;
+  const bool xs = d->swap ? rs : ls, ys = d->swap ? ls : rs;
+  const bool xn = d->swap ? rn : ln, yn = d->swap ? ln : rn;
+  d->lt = !(op == ACU_EQ || op == ACU_NEQ || fold);
+  d->neg = op == ACU_NEQ || op == ACU_DISTINCT || op == ACU_LT_EQ || op == ACU_GT_EQ;
+  d->fold = op == ACU_DISTINCT ? FOLD_DISTINCT : op == ACU_NOT_DISTINCT ? FOLD_NOT_DISTINCT : FOLD_NONE;
+  d->a_scalar = xs && !ys;
+  d->b_scalar = ys && !xs;
+  if (xn) { if (d->a_scalar) d->a_null_scalar = 1; else { d->av = x->validity; d->aoff = x->validity_offset; } }
+  if (yn) { if (d->b_scalar) d->b_null_scalar = 1; else { d->bv = y->validity; d->boff = y->validity_offset; } }
+  d->has_validity = !fold && (xn || yn);
+  return ACU_OK;
+}
+
+void acu_cmp_finalize(const acu_cmp_decision &d, const unsigned long long *hres, acu_array_out *out) {
+  if (!d.has_validity) return;
+  out->has_validity = 1;
+  out->null_count = d.len - (int64_t)hres[RES_COUNT];
+}
+
+acu_status acu_new_null(acu_ctx *ctx, int64_t len, size_t value_bytes, acu_array_out *out) {
+  if (value_bytes) ACU_CUDA(ctx, cudaMemsetAsync(out->values, 0, value_bytes, ctx->stream));
+  if (len) ACU_CUDA(ctx, cudaMemsetAsync(out->validity, 0, acu_bitmap_bytes(len), ctx->stream));
+  ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  out->len = len;
+  out->has_validity = 1;
+  out->null_count = len;
+  return ACU_OK;
+}
+
+// The comparison of acu_cmp written straight into a filter plan's mask / tile counts (compact.cu: acu_filter_plan_create_cmp).
+// Stream-ordered, no synchronisation.
 acu_status acu_cmp_into_plan(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, const acu_array *a, const acu_array *b, uint64_t *mask,
                              int64_t n_words_padded, uint32_t *tile_count, int64_t n_tiles) {
   CmpFuse f{mask, n_words_padded, tile_count, n_tiles};

@@ -62,8 +62,34 @@ acu_status acu_filter_bytes_col_launch(acu_ctx *ctx, const acu_filter_plan *plan
 acu_status acu_filter_bytes_col_finalize(acu_ctx *ctx, const acu_bytes_col_state *st, const unsigned long long *hres,
                                          int64_t *out_data_len);
 
+// compare_op (arrow-ord/src/cmp.rs:220-382), elementwise.cu: the host-side decisions of every comparison, whatever the
+// operand type (primitive, Utf8 / Binary, view). The kernels compute is_lt(a, b) or is_eq(a, b) of the swapped operands
+// (a, b) at every slot, negate, then fold the validity into the values (distinct / not_distinct) or write it beside them.
+enum { FOLD_NONE = 0, FOLD_DISTINCT = 1, FOLD_NOT_DISTINCT = 2 };
+struct acu_cmp_decision {
+  int64_t len;
+  bool all_null;  // a null scalar against an array: BooleanArray::new_null(len), no kernel (cmp.rs:353, :364)
+  bool swap;      // gt / lt_eq: a = r, b = l (cmp.rs:481-488)
+  int lt, neg, fold;
+  int a_scalar, b_scalar;             // a scalar against an array (two scalars compare as arrays of length 1)
+  int a_null_scalar, b_null_scalar;   // that scalar's single slot is null
+  const uint8_t *av, *bv;             // validity bitmaps the kernel reads, NULL = no nulls
+  int64_t aoff, boff;
+  bool has_validity;                  // the result carries a NullBuffer (valid count in RES_COUNT)
+};
+// The length check (cmp.rs:228-232) and the result length.
+acu_status acu_cmp_len(acu_ctx *ctx, const acu_array *l, const acu_array *r, int64_t *len);
+// acu_cmp_len, then out = an empty result of that length; for len > 0 the operands' null counts are resolved and the
+// rest of *d is decided. Issues no device work unless a null count is unknown.
+acu_status acu_cmp_decide(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_array *r, acu_array_out *out,
+                          acu_cmp_decision *d);
+// has_validity / null_count of the result from its fetched result block
+void acu_cmp_finalize(const acu_cmp_decision &d, const unsigned long long *hres, acu_array_out *out);
+// PrimitiveArray::new_null / BooleanArray::new_null: `value_bytes` zeroed value bytes, an all-null bitmap, one
+// synchronisation.
+acu_status acu_new_null(acu_ctx *ctx, int64_t len, size_t value_bytes, acu_array_out *out);
+
 // Fused compare -> filter plan (elementwise.cu): the cmp kernels write the plan's mask words and per-tile counts.
-acu_status acu_cmp_result_len(acu_ctx *ctx, const acu_array *l, const acu_array *r, int64_t *out_len);
 acu_status acu_cmp_into_plan(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, const acu_array *a, const acu_array *b, uint64_t *mask,
                              int64_t n_words_padded, uint32_t *tile_count, int64_t n_tiles);
 

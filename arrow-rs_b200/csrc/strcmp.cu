@@ -5,18 +5,16 @@
 //     GenericByteViewArray  (Utf8View, BinaryView)                                      ArrayOrd cmp.rs:803-898
 //   and the short-constant fast path of views, eq_inline_scalar                          cmp.rs:282-300, :405-435
 //
-// compare_op's null handling (cmp.rs:319-381) is the same as for primitives (elementwise.cu): value bits are computed at
-// every slot, validity = union of the inputs' (folded into the values for distinct / not_distinct), a null scalar makes
-// the result all-null. One thread per row, 4 rows per lane in flight, result bits packed with a warp ballot (lane == bit),
-// lane 0 of each 32-row group owns the group's 32-bit value and validity words.
+// compare_op's host-side decisions (length check, null scalars, operand swap, negation, fold, NullBuffer) are made by
+// acu_cmp_decide (internal.cuh), as for primitives. Value bits are computed at every slot. One thread per row, 4 rows per
+// lane in flight, result bits packed with a warp ballot (lane == bit), lane 0 of each 32-row group owns the group's
+// 32-bit value and validity words.
 // Roofline: 2 offsets + the compared bytes per side (byte arrays), 16 B per view (views); HBM-bound.
 #include "bitmap.cuh"
 #include "bytes_cmp.cuh"
 #include "internal.cuh"
 
 namespace {
-
-enum { SFOLD_NONE = 0, SFOLD_DISTINCT = 1, SFOLD_NOT_DISTINCT = 2 };
 
 struct RowCmpCommon {
   int64_t n;
@@ -61,8 +59,8 @@ __device__ __forceinline__ void finish_group(const RowCmpCommon &p, int64_t row0
   uint32_t l = p.a_null_scalar ? 0u : m, r = p.b_null_scalar ? 0u : m;
   if (p.av) l &= ld_bits32(p.av, p.aoff + row0, p.aoff + p.n);
   if (p.bv) r &= ld_bits32(p.bv, p.boff + row0, p.boff + p.n);
-  if (p.fold == SFOLD_DISTINCT) v = (l ^ r) | (l & r & v);                  // cmp.rs:331
-  else if (p.fold == SFOLD_NOT_DISTINCT) v = (~(l | r) & m) | (l & r & v);  // cmp.rs:341
+  if (p.fold == FOLD_DISTINCT) v = (l ^ r) | (l & r & v);                  // cmp.rs:331
+  else if (p.fold == FOLD_NOT_DISTINCT) v = (~(l | r) & m) | (l & r & v);  // cmp.rs:341
   p.out_bits[row0 >> 5] = v;
   if (p.out_valid) {
     p.out_valid[row0 >> 5] = l & r;
@@ -167,72 +165,11 @@ __global__ void __launch_bounds__(256) k_view_eq_inline(const uint4 *__restrict_
   }
 }
 
-// ---- host side: compare_op (cmp.rs:220-382), the part that does not depend on the operand kind -----------------------
-struct CmpPlan {
-  RowCmpCommon p;
-  bool swap;
-  bool done;  // the result was produced without a comparison kernel (all-null)
-};
-
-acu_status new_null_bool(acu_ctx *ctx, int64_t len, acu_array_out *out) {  // BooleanArray::new_null(len)
-  ACU_CUDA(ctx, cudaMemsetAsync(out->values, 0, acu_bitmap_bytes(len), ctx->stream));
-  ACU_CUDA(ctx, cudaMemsetAsync(out->validity, 0, acu_bitmap_bytes(len), ctx->stream));
-  ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  out->has_validity = 1;
-  out->null_count = len;
-  return ACU_OK;
-}
-
-acu_status cmp_prepare(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_array *r, acu_array_out *out, CmpPlan *plan) {
-  plan->done = false;
-  const bool ls = l->is_scalar != 0, rs = r->is_scalar != 0;
-  if (l->len != r->len && !ls && !rs)  // cmp.rs:228-232
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Cannot compare arrays of different lengths, got %lld vs %lld",
-                    (long long)l->len, (long long)r->len);
-  const int64_t len = ls ? r->len : l->len;
-  out->len = len;
-  out->has_validity = 0;
-  out->null_count = 0;
-  if (len == 0) { plan->done = true; return ACU_OK; }
-  acu_status st;
-  const int64_t lnc = acu_resolve_null_count(ctx, l, &st);
-  ACU_TRY(st);
-  const int64_t rnc = acu_resolve_null_count(ctx, r, &st);
-  ACU_TRY(st);
-  const bool ln = lnc > 0, rn = rnc > 0;
-  const bool fold = op == ACU_DISTINCT || op == ACU_NOT_DISTINCT;
-  const bool l_null_scalar = ls && ln, r_null_scalar = rs && rn;
-  if (!fold && (l_null_scalar || r_null_scalar) && !(ls && rs)) {  // cmp.rs:353, :364
-    plan->done = true;
-    return new_null_bool(ctx, len, out);
-  }
-  RowCmpCommon &p = plan->p;
-  p = RowCmpCommon{};
-  p.n = len;
-  p.res = ctx->d_res;
-  p.out_bits = static_cast<uint32_t *>(out->values);
-  plan->swap = (op == ACU_GT || op == ACU_LT_EQ);  // cmp.rs:481-488
-  const bool xs = plan->swap ? rs : ls, ys = plan->swap ? ls : rs;
-  const bool xn = plan->swap ? rn : ln, yn = plan->swap ? ln : rn;
-  const acu_array *x = plan->swap ? r : l, *y = plan->swap ? l : r;
-  p.a_scalar = xs && !(xs && ys);
-  p.b_scalar = ys && !(xs && ys);
-  p.neg = (op == ACU_NEQ || op == ACU_DISTINCT || op == ACU_LT_EQ || op == ACU_GT_EQ);
-  p.fold = op == ACU_DISTINCT ? SFOLD_DISTINCT : op == ACU_NOT_DISTINCT ? SFOLD_NOT_DISTINCT : SFOLD_NONE;
-  p.lt = !(op == ACU_EQ || op == ACU_NEQ || fold);
-  if (xn) { if (p.a_scalar) p.a_null_scalar = 1; else { p.av = x->validity; p.aoff = x->validity_offset; } }
-  if (yn) { if (p.b_scalar) p.b_null_scalar = 1; else { p.bv = y->validity; p.boff = y->validity_offset; } }
-  if (!fold && (xn || yn)) p.out_valid = reinterpret_cast<uint32_t *>(out->validity);
-  return ACU_OK;
-}
-
-acu_status cmp_finish(acu_ctx *ctx, const CmpPlan &plan, acu_array_out *out) {
-  ACU_TRY(acu_res_fetch(ctx));
-  if (plan.p.out_valid) {
-    out->has_validity = 1;
-    out->null_count = plan.p.n - (int64_t)ctx->h_res[RES_COUNT];
-  }
-  return ACU_OK;
+// ---- host side -------------------------------------------------------------------------------------------------------
+RowCmpCommon row_cmp_params(acu_ctx *ctx, const acu_cmp_decision &d, acu_array_out *out) {
+  return RowCmpCommon{d.len, d.av, d.bv, d.aoff, d.boff, d.a_scalar, d.b_scalar, d.a_null_scalar, d.b_null_scalar, d.lt, d.neg, d.fold,
+                      static_cast<uint32_t *>(out->values), d.has_validity ? reinterpret_cast<uint32_t *>(out->validity) : nullptr,
+                      ctx->d_res};
 }
 
 int cmp_grid(acu_ctx *ctx, int64_t n, int rows_per_lane) {
@@ -246,14 +183,17 @@ extern "C" acu_status acu_cmp_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_cmp_
                                     acu_array_out *out) {
   ACU_ENTER(ctx);
   if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
-  CmpPlan plan;
-  ACU_TRY(cmp_prepare(ctx, op, &l->nulls, &r->nulls, out, &plan));
-  if (plan.done) return ACU_OK;
-  const acu_bytes_array *x = plan.swap ? r : l, *y = plan.swap ? l : r;
+  acu_cmp_decision d;
+  ACU_TRY(acu_cmp_decide(ctx, op, &l->nulls, &r->nulls, out, &d));
+  if (d.len == 0) return ACU_OK;
+  if (d.all_null) return acu_new_null(ctx, d.len, acu_bitmap_bytes(d.len), out);
+  const acu_bytes_array *x = d.swap ? r : l, *y = d.swap ? l : r;
   const BytesOperand A{x->offsets, x->data, offset_bytes}, B{y->offsets, y->data, offset_bytes};
   ACU_TRY(acu_res_reset(ctx));
-  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_bytes, cmp_grid(ctx, plan.p.n, ROWS_PER_LANE), 256, 0, plan.p, A, B);
-  return cmp_finish(ctx, plan, out);
+  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_bytes, cmp_grid(ctx, d.len, ROWS_PER_LANE), 256, 0, row_cmp_params(ctx, d, out), A, B);
+  ACU_TRY(acu_res_fetch(ctx));
+  acu_cmp_finalize(d, ctx->h_res, out);
+  return ACU_OK;
 }
 
 extern "C" acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_view_array *l, const acu_view_array *r, acu_array_out *out) {
@@ -293,10 +233,11 @@ extern "C" acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_v
       }
     }
   }
-  CmpPlan plan;
-  ACU_TRY(cmp_prepare(ctx, op, &l->nulls, &r->nulls, out, &plan));
-  if (plan.done) return ACU_OK;
-  const acu_view_array *x = plan.swap ? r : l, *y = plan.swap ? l : r;
+  acu_cmp_decision d;
+  ACU_TRY(acu_cmp_decide(ctx, op, &l->nulls, &r->nulls, out, &d));
+  if (d.len == 0) return ACU_OK;
+  if (d.all_null) return acu_new_null(ctx, d.len, acu_bitmap_bytes(d.len), out);
+  const acu_view_array *x = d.swap ? r : l, *y = d.swap ? l : r;
   // the data-buffer pointer tables go to the device (scratch): [x buffers][y buffers]
   const int nx = x->n_buffers, ny = y->n_buffers;
   const uint8_t **table = nullptr;
@@ -309,6 +250,8 @@ extern "C" acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_v
   }
   const ViewOperand A{static_cast<const uint4 *>(x->views), table, nx}, B{static_cast<const uint4 *>(y->views), table ? table + nx : nullptr, ny};
   ACU_TRY(acu_res_reset(ctx));
-  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_views, cmp_grid(ctx, plan.p.n, ROWS_PER_LANE), 256, 0, plan.p, A, B);
-  return cmp_finish(ctx, plan, out);
+  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_views, cmp_grid(ctx, d.len, ROWS_PER_LANE), 256, 0, row_cmp_params(ctx, d, out), A, B);
+  ACU_TRY(acu_res_fetch(ctx));
+  acu_cmp_finalize(d, ctx->h_res, out);
+  return ACU_OK;
 }

@@ -10,9 +10,10 @@ import pytest
 
 import acu
 from acu import _abi as abi
-from acu import BOOL, ArrowError, HostArray
+from acu import BOOL, ArrowError, HostArray, ViewColumn, bitmap_bytes
 
 from test_gpu_parity import assert_same, rand_array, rand_bool
+from test_oracle_cmp_bytes import rand_strings, utf8_column
 
 pytestmark = pytest.mark.gpu
 
@@ -162,3 +163,28 @@ def test_section_rules(gpu):
     # and the synchronous ABI works as before
     got = gpu.arith(acu.ADD_WRAPPING, x, x)
     assert got.null_count == x.null_count
+
+
+def test_comparison_brackets_in_section(gpu):
+    """Primitive comparisons only enqueue inside a section; Utf8 / view comparisons synchronise, so there they refuse."""
+    lib, h = gpu.lib, gpu.h
+    rng = np.random.default_rng(8)
+    n = 5000
+    x, y = rand_array(rng, abi.I64, n, 0.1, 0), rand_array(rng, abi.I64, n, 0.05, 0)
+    expected = gpu.cmp(acu.LT_EQ, x, y)
+    sa, sb = utf8_column(rand_strings(rng, 100, 0.1)), utf8_column(rand_strings(rng, 100, 0.2))
+    va, vb = ViewColumn.from_values(rand_strings(rng, 100, 0.1)), ViewColumn.from_values(rand_strings(rng, 100, 0.2))
+    dx, dy = gpu.upload(x), gpu.upload(y)
+    out = gpu.alloc_out(bitmap_bytes(n), n)
+    xd, yd = dx.descriptor(), dy.descriptor()
+    gpu.async_begin()
+    assert lib.acu_cmp(h, abi.I64, acu.LT_EQ, C.byref(xd), C.byref(yd), C.byref(out)) == abi.OK
+    for call in (lambda: gpu.cmp_bytes(acu.LT_EQ, sa, sb), lambda: gpu.cmp_view(acu.LT_EQ, va, vb)):
+        with pytest.raises(ArrowError) as e:
+            call()
+        assert e.value.status == abi.ERR_INVALID_ARGUMENT
+        assert "not available between acu_async_begin" in str(e.value)
+    gpu.results_fetch()
+    assert_same(gpu.download_out(out, BOOL), expected, "acu_cmp queued in a section")
+    dx.free()
+    dy.free()
