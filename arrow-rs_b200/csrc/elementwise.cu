@@ -6,10 +6,12 @@
 //
 // All kernels are single-pass and HBM-bound: each input byte is read once, each output
 // byte written once, and the validity AND + popcount ride along in the same pass.
-// Work unit = a "strip" of R rows handled by one warp: R = max(64, 32*EPL) where EPL =
-// elements per 128-bit lane access. Lane l owns elements [l*EPL, (l+1)*EPL) of each
-// 32*EPL-row load, so every warp access is a fully coalesced 512-B (EPL>1) request, and a
-// strip always spans whole 64-bit validity words (lanes 0..R/64-1 own one word each).
+// Every kernel here has one shape: a warp owns 2048-row super-groups = 32 validity words,
+// lane l owning word l (one coalesced 256-B bitmap access per super-group). Lane l reads
+// elements [l*EPL, (l+1)*EPL) of each 32*EPL-row load: EPL = 16 / sizeof(T) (128-bit
+// accesses, 512-B warp requests) when the value pointers are 16-B aligned, EPL = 1 for
+// unaligned slices. Warp 0 finishes the ragged tail (< 2048 rows) in 64-row strips after
+// its super-groups, so each call is one launch.
 #include <stdio.h>
 
 #include <limits>
@@ -451,7 +453,7 @@ struct CmpParams {
   uint64_t *out_bits, *out_valid;
   unsigned long long *res;
   // fused compare -> filter plan (acu_filter_plan_create_cmp): out_bits is the plan's mask and receives result & validity;
-  // tile_count[t] = selected rows of 1024-row tile t (written by the streaming kernel; the tail's tiles are counted separately)
+  // tile_count[t] = selected rows of 1024-row tile t
   int fuse;
   uint32_t *tile_count;
 };
@@ -466,82 +468,42 @@ template <class T> __device__ __forceinline__ bool pred_lt(T l, T r) {
   else return l < r;
 }
 
-// Lane l of a warp owns rows l and l+32 of each 64-row strip: two ballots give the low and
-// high halves of the packed u64, and the loads are coalesced 32*sizeof(T)-byte requests.
-template <class T, bool LT>
-__global__ void __launch_bounds__(256) k_cmp(const CmpParams<T> p) {
-  constexpr int U = 4;
+// A super-group's 2048 rows are read as 2048 / (32*EPL) warp-wide loads; lane l holds rows [l*EPL, (l+1)*EPL) of
+// each. `bits` has one bit per such row (bit e = row l*EPL + e). The rows of load `load` fill EPL 32-bit halves of the
+// super-group's bit string, and each half is ONE warp OR-reduction (redux.sync) of the lanes' shifted bits. Half h goes
+// to lane h/2, so lane l ends up owning word l of the super-group (rows [l*64, l*64+64)) as (lo, hi).
+template <int EPL>
+__device__ __forceinline__ void pack_lane_bits(uint32_t bits, int load, uint32_t &lo, uint32_t &hi) {
   const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int64_t n = p.n;
-  const int64_t strips = (n + 63) >> 6;
-  T sa = T(), sb = T();
-  if (p.a_scalar) sa = __ldg(p.a);
-  if (p.b_scalar) sb = __ldg(p.b);
-  unsigned valid_cnt = 0;
-  for (int64_t s0 = warp * U; s0 < strips; s0 += nwarps * U) {
-    T va[U][2], vb[U][2];
+  bits <<= (lane * EPL) & 31;              // where this lane's EPL bits land inside their 32-bit half
+  const int my_half = (lane * EPL) >> 5;   // which half of the load's bit string they belong to
 #pragma unroll
-    for (int u = 0; u < U; ++u) {
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t i = (s0 + u) * 64 + h * 32 + lane;
-        va[u][h] = (!p.a_scalar && i < n) ? __ldg(p.a + i) : sa;
-        vb[u][h] = (!p.b_scalar && i < n) ? __ldg(p.b + i) : sb;
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int64_t row = (s0 + u) * 64;
-      if (row >= n) break;
-      bool r0 = LT ? pred_lt(va[u][0], vb[u][0]) : pred_eq(va[u][0], vb[u][0]);
-      bool r1 = LT ? pred_lt(va[u][1], vb[u][1]) : pred_eq(va[u][1], vb[u][1]);
-      uint64_t v = (uint64_t)__ballot_sync(ACU_FULL_MASK, r0) | ((uint64_t)__ballot_sync(ACU_FULL_MASK, r1) << 32);
-      if (p.neg) v = ~v;
-      if (lane == 0) {
-        const uint64_t m = ones_to(row, n);
-        v &= m;
-        uint64_t l = p.a_null_scalar ? 0ull : m, r = p.b_null_scalar ? 0ull : m;
-        if (p.av) l &= ld_bits64(p.av, p.aoff + row, p.aoff + n);
-        if (p.bv) r &= ld_bits64(p.bv, p.boff + row, p.boff + n);
-        if (p.fold == FOLD_DISTINCT) v = (l ^ r) | (l & r & v);              // cmp.rs:331
-        else if (p.fold == FOLD_NOT_DISTINCT) v = (~(l | r) & m) | (l & r & v);  // cmp.rs:341
-        else if (p.fuse) v &= l & r;  // a null result selects nothing (filter.rs:167-171)
-        p.out_bits[row >> 6] = v;
-        if (p.out_valid) {
-          p.out_valid[row >> 6] = l & r;
-          valid_cnt += __popcll(l & r);
-        }
-      }
-    }
+  for (int hh = 0; hh < EPL; ++hh) {
+    const uint32_t half = __reduce_or_sync(ACU_FULL_MASK, my_half == hh ? bits : 0u);
+    const int h = load * EPL + hh;         // 32-bit half inside the super-group
+    if (lane == (h >> 1)) { if (h & 1) hi = half; else lo = half; }
   }
-  if (p.out_valid && lane == 0 && valid_cnt) atomicAdd(p.res + RES_COUNT, (unsigned long long)valid_cnt);
 }
 
-// Streaming variant for 16-B aligned operands: a warp owns 2048-row super-groups = 32 result
-// words. Every lane reads 128-bit vectors (EPL elements), 4 vector pairs in flight; a lane's
-// EPL result bits sit at bit position lane*EPL of the load's bit string, so each 32-bit half
-// of a result word is ONE warp OR-reduction (redux.sync) of the shifted groups. Lane l ends up
-// owning result word l and validity word l: one coalesced 256-B store each per super-group.
-// The ragged tail (< 2048 rows) is finished by k_cmp on offset pointers.
-template <class T, bool LT>
-__global__ void __launch_bounds__(256, 4) k_cmp_v2(const CmpParams<T> p, const int64_t sgroups) {
-  constexpr int EPL = 16 / sizeof(T);
-  constexpr int RPL = 32 * EPL;          // rows per warp-wide vector load
-  constexpr int HPL = RPL / 32;          // 32-bit result halves per load (= EPL)
-  constexpr int LOADS = 2048 / RPL;      // vector loads per super-group (32 / 16 / 8 / 4)
+// A warp owns 2048-row super-groups = 32 result words. Every lane reads EPL elements per warp-wide load (128-bit
+// vectors when the value pointers are 16-B aligned, one element otherwise), 4 loads in flight, and ends up owning
+// result word l and validity word l: one coalesced 256-B store each per super-group. The ragged tail (< 2048 rows) is
+// finished by warp 0 in 64-row strips: lane l compares rows l and l+32, two ballots give the packed word. In fuse mode
+// it also writes the tail's (at most two) tile counts.
+template <class T, bool LT, int EPL>
+__global__ void __launch_bounds__(256, 4) k_cmp(const CmpParams<T> p) {
+  constexpr int RPL = 32 * EPL;          // rows per warp-wide load
+  constexpr int LOADS = 2048 / RPL;      // loads per super-group
   constexpr int U = LOADS < 4 ? LOADS : 4;
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t n = p.n;
+  const int64_t sgroups = n >> 11;
   T sa = T(), sb = T();
   if (p.a_scalar) sa = __ldg(p.a);
   if (p.b_scalar) sb = __ldg(p.b);
   unsigned valid_cnt = 0;
-  const int grp_shift = (lane * EPL) & 31;   // where this lane's EPL bits land inside their 32-bit half
-  const int grp_half = (lane * EPL) >> 5;    // which half of the load's bit string they belong to
   for (int64_t sg = warp; sg < sgroups; sg += nwarps) {
     const int64_t sbase = sg << 11;
     uint64_t lw = ~0ull, rw = ~0ull;  // lane-owned validity words
@@ -569,13 +531,7 @@ __global__ void __launch_bounds__(256, 4) k_cmp_v2(const CmpParams<T> p, const i
           const T r = p.b_scalar ? sb : vb[u].v[e];
           x |= (uint32_t)(LT ? pred_lt(l, r) : pred_eq(l, r)) << e;
         }
-        x <<= grp_shift;
-#pragma unroll
-        for (int hh = 0; hh < HPL; ++hh) {
-          const uint32_t half = __reduce_or_sync(ACU_FULL_MASK, grp_half == hh ? x : 0u);
-          const int widx = ((l0 + u) * HPL + hh) >> 1;  // result word inside the super-group
-          if (lane == widx) { if (hh & 1) my_hi = half; else my_lo = half; }
-        }
+        pack_lane_bits<EPL>(x, l0 + u, my_lo, my_hi);
       }
     }
     uint64_t v = (uint64_t)my_lo | ((uint64_t)my_hi << 32);
@@ -595,20 +551,52 @@ __global__ void __launch_bounds__(256, 4) k_cmp_v2(const CmpParams<T> p, const i
       valid_cnt += __popcll(lw & rw);
     }
   }
+
+  if (warp == 0) {
+    unsigned tile_cnt = 0;
+    for (int64_t row = sgroups << 11; row < n; row += 64) {
+      uint64_t v = 0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t i = row + h * 32 + lane;
+        const T l = (!p.a_scalar && i < n) ? __ldg(p.a + i) : sa;
+        const T r = (!p.b_scalar && i < n) ? __ldg(p.b + i) : sb;
+        v |= (uint64_t)__ballot_sync(ACU_FULL_MASK, LT ? pred_lt(l, r) : pred_eq(l, r)) << (h * 32);
+      }
+      if (p.neg) v = ~v;
+      if (lane == 0) {
+        const uint64_t m = ones_to(row, n);
+        v &= m;
+        uint64_t lw = p.a_null_scalar ? 0ull : m, rw = p.b_null_scalar ? 0ull : m;
+        if (p.av) lw &= ld_bits64(p.av, p.aoff + row, p.aoff + n);
+        if (p.bv) rw &= ld_bits64(p.bv, p.boff + row, p.boff + n);
+        if (p.fold == FOLD_DISTINCT) v = (lw ^ rw) | (lw & rw & v);              // cmp.rs:331
+        else if (p.fold == FOLD_NOT_DISTINCT) v = (~(lw | rw) & m) | (lw & rw & v);  // cmp.rs:341
+        else if (p.fuse) v &= lw & rw;  // a null result selects nothing (filter.rs:167-171)
+        p.out_bits[row >> 6] = v;
+        if (p.out_valid) {
+          p.out_valid[row >> 6] = lw & rw;
+          valid_cnt += __popcll(lw & rw);
+        }
+        if (p.fuse) {  // a tile ends every 16 words and at the last word
+          tile_cnt += __popcll(v);
+          if (row + 64 >= n || ((row + 64) & 1023) == 0) { p.tile_count[row >> 10] = tile_cnt; tile_cnt = 0; }
+        }
+      }
+    }
+  }
   if (p.out_valid) {
     valid_cnt = warp_sum(valid_cnt);
     if (lane == 0 && valid_cnt) atomicAdd(p.res + RES_COUNT, (unsigned long long)valid_cnt);
   }
 }
 
-// popcount of the 1024-row tiles [first_tile, n_tiles) of a plan mask (the ragged tail of a fused compare)
-__global__ void __launch_bounds__(256) k_tile_counts(const uint64_t *__restrict__ mask, int64_t first_tile, int64_t n_tiles,
-                                                     uint32_t *__restrict__ tile_count) {
-  const int64_t t = first_tile + (int64_t)blockIdx.x * blockDim.x + threadIdx.x;
-  if (t >= n_tiles) return;
-  unsigned c = 0;
-  for (int k = 0; k < 16; ++k) c += __popcll(mask[t * 16 + k]);
-  tile_count[t] = c;
+template <class T, int EPL>
+acu_status launch_cmp(acu_ctx *ctx, bool lt, const CmpParams<T> &p) {
+  const int64_t blocks = (p.n / 2048 + 1 + 7) / 8;  // 8 warps per CTA; a column shorter than 2048 rows still gets warp 0
+  if (lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, true, EPL>), acu_wave_grid(ctx, k_cmp<T, true, EPL>, 256, 0, blocks), 256, 0, p);
+  else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, false, EPL>), acu_wave_grid(ctx, k_cmp<T, false, EPL>, 256, 0, blocks), 256, 0, p);
+  return ACU_OK;
 }
 
 struct CmpFuse {  // destination of a fused compare -> filter plan
@@ -660,33 +648,10 @@ acu_status cmp_typed(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_
     ACU_TRY(st);
     p.res = acu_dres(ctx, blk);
   }
-  // streaming head over whole 2048-row super-groups when the value pointers are 16-B aligned
+  // 128-bit loads when both non-scalar value pointers are 16-B aligned, one element per lane otherwise
   const bool aligned = (p.a_scalar || (uintptr_t)p.a % 16 == 0) && (p.b_scalar || (uintptr_t)p.b % 16 == 0);
-  const int64_t sgroups = aligned ? len / 2048 : 0;
-  if (sgroups > 0) {
-    const int64_t blocks = (sgroups + 7) / 8;
-    if (d.lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp_v2<T, true>), acu_wave_grid(ctx, k_cmp_v2<T, true>, 256, 0, blocks), 256, 0, p, sgroups);
-    else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp_v2<T, false>), acu_wave_grid(ctx, k_cmp_v2<T, false>, 256, 0, blocks), 256, 0, p, sgroups);
-  }
-  const int64_t head = sgroups * 2048;
-  if (head < len) {  // ragged tail (or everything, for unaligned slices)
-    CmpParams<T> q = p;
-    q.n = len - head;
-    if (!q.a_scalar) q.a += head;
-    if (!q.b_scalar) q.b += head;
-    q.aoff += head;
-    q.boff += head;
-    q.out_bits += head >> 6;
-    if (q.out_valid) q.out_valid += head >> 6;
-    const int64_t strips = (q.n + 63) >> 6;
-    const int64_t blocks = (strips + 31) / 32;
-    if (d.lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, true>), acu_wave_grid(ctx, k_cmp<T, true>, 256, 0, blocks), 256, 0, q);
-    else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, false>), acu_wave_grid(ctx, k_cmp<T, false>, 256, 0, blocks), 256, 0, q);
-    if (fuse) {  // the tail's tiles (head is a multiple of 2048 rows = 2 tiles)
-      const int64_t first_tile = head >> 10, rest = fuse->n_tiles - first_tile;
-      if (rest > 0) ACU_LAUNCH(ctx, k_tile_counts, (unsigned)((rest + 255) / 256), 256, 0, fuse->mask, first_tile, fuse->n_tiles, fuse->tile_count);
-    }
-  }
+  if (aligned) ACU_TRY((launch_cmp<T, 16 / sizeof(T)>(ctx, d.lt, p)));
+  else ACU_TRY((launch_cmp<T, 1>(ctx, d.lt, p)));
   if (fuse) return ACU_OK;  // stream-ordered: the plan's scan kernels follow on the same stream
   return acu_call_end(ctx, blk, [d, out](const unsigned long long *h) -> acu_status {
     acu_cmp_finalize(d, h, out);
@@ -731,63 +696,7 @@ __device__ __forceinline__ bool num_cast(I v, O &o) {
   }
 }
 
-template <class I, class O>
-__global__ void __launch_bounds__(256) k_cast(const I *__restrict__ in, O *__restrict__ out, int64_t n,
-                                              const uint8_t *__restrict__ iv, int64_t ioff, uint64_t *out_valid,
-                                              int safe, unsigned long long *res) {
-  constexpr int U = 4;
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int64_t strips = (n + 63) >> 6;
-  unsigned valid_cnt = 0;
-  unsigned long long err = ~0ull;
-  for (int64_t s0 = warp * U; s0 < strips; s0 += nwarps * U) {
-    I v[U][2];
-    uint64_t vw[U];
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int64_t row = (s0 + u) * 64;
-      vw[u] = ones_to(row, n);
-      if (iv) vw[u] &= ld_bits64(iv, ioff + row, ioff + n);
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t i = row + h * 32 + lane;
-        v[u][h] = i < n ? __ldg(in + i) : I();
-      }
-    }
-#pragma unroll
-    for (int u = 0; u < U; ++u) {
-      const int64_t row = (s0 + u) * 64;
-      if (row >= n) break;
-      uint32_t failed[2];
-#pragma unroll
-      for (int h = 0; h < 2; ++h) {
-        const int64_t i = row + h * 32 + lane;
-        const bool live = (vw[u] >> (h * 32 + lane)) & 1ull;  // unary_opt / try_unary: valid slots only
-        O o = O();
-        bool ok = true;
-        if (live) {
-          ok = num_cast<I, O>(v[u][h], o);
-          if (!ok) { o = O(); if (!safe) { unsigned long long e = (unsigned long long)i; err = e < err ? e : err; } }
-        }
-        failed[h] = __ballot_sync(ACU_FULL_MASK, live && !ok);
-        if (i < n) out[i] = o;
-      }
-      if (lane == 0 && out_valid) {
-        uint64_t w = vw[u];
-        if (safe) w &= ~((uint64_t)failed[0] | ((uint64_t)failed[1] << 32));  // unrepresentable => null
-        out_valid[row >> 6] = w;
-        valid_cnt += __popcll(w);
-      }
-    }
-  }
-  if (out_valid && lane == 0 && valid_cnt) atomicAdd(res + RES_COUNT, (unsigned long long)valid_cnt);
-  if (err != ~0ull) atomicMin(res + RES_ERR_INDEX, err);
-}
-
-// Streaming variant for casts that cannot fail (anything -> float, widening integer casts):
-// 2048-row super-groups, 128-bit input vectors, lane-owned validity words, zero under nulls.
+// Casts that cannot fail (anything -> float, widening integer casts) compile without the failure bookkeeping.
 template <class I, class O> struct cast_infallible {
   static constexpr bool value = is_fp<O>::value ||
       (!is_fp<I>::value && ((std::is_signed<I>::value == std::is_signed<O>::value && sizeof(O) >= sizeof(I)) ||
@@ -795,23 +704,29 @@ template <class I, class O> struct cast_infallible {
 };
 template <class O, int EPL> struct alignas((sizeof(O) * EPL >= 16) ? 16 : sizeof(O) * EPL) OutPack { O v[EPL]; };
 
-template <class I, class O>
-__global__ void __launch_bounds__(256, 4) k_cast_v2(const I *__restrict__ in, O *__restrict__ out, const int64_t n,
-                                                    const int64_t sgroups, const uint8_t *__restrict__ iv, const int64_t ioff,
-                                                    uint64_t *__restrict__ out_valid, unsigned long long *__restrict__ res) {
-  constexpr int EPL = 16 / sizeof(I);
+// The layout of k_cmp: 2048-row super-groups, EPL input elements per lane and load (128-bit vectors when both pointers
+// are 16-B aligned, one element otherwise), lane-owned validity words, ragged tail finished by warp 0. unary_opt /
+// try_unary: the cast runs at valid slots only, zero elsewhere. A valid slot whose value does not fit O becomes null
+// (`safe`) or reports its row, the lowest one winning (atomicMin).
+template <class I, class O, int EPL>
+__global__ void __launch_bounds__(256, 4) k_cast(const I *__restrict__ in, O *__restrict__ out, const int64_t n,
+                                                 const uint8_t *__restrict__ iv, const int64_t ioff, uint64_t *__restrict__ out_valid,
+                                                 const int safe, unsigned long long *__restrict__ res) {
+  constexpr bool fallible = !cast_infallible<I, O>::value;
   constexpr int RPL = 32 * EPL;
   constexpr int LOADS = 2048 / RPL;
   constexpr int U = LOADS < 4 ? LOADS : 4;
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int64_t sgroups = n >> 11;
   unsigned valid_cnt = 0;
+  unsigned long long err = ~0ull;
   for (int64_t sg = warp; sg < sgroups; sg += nwarps) {
     const int64_t sbase = sg << 11;
     uint64_t vw = ~0ull;
     if (iv) vw = ld_bits64(iv, ioff + sbase + lane * 64, ioff + n);
-    if (out_valid) { out_valid[(sbase >> 6) + lane] = vw; valid_cnt += __popcll(vw); }
+    uint32_t bad_lo = 0, bad_hi = 0;  // lane-owned word: valid slots whose value does not fit O
 #pragma unroll 1
     for (int l0 = 0; l0 < LOADS; l0 += U) {
       Pack<I, EPL> v[U];
@@ -823,20 +738,50 @@ __global__ void __launch_bounds__(256, 4) k_cast_v2(const I *__restrict__ in, O 
         const uint64_t w = __shfl_sync(ACU_FULL_MASK, vw, pos >> 6);
         const uint32_t bits = (uint32_t)(w >> (pos & 63));
         OutPack<O, EPL> o;
+        uint32_t bad = 0;
 #pragma unroll
         for (int e = 0; e < EPL; ++e) {
           O x = O();
-          if ((bits >> e) & 1u) num_cast<I, O>(v[u].v[e], x);  // unary_opt / try_unary: valid slots only, zero elsewhere
+          if (((bits >> e) & 1u) && !num_cast<I, O>(v[u].v[e], x)) bad |= 1u << e;
           o.v[e] = x;
         }
         *reinterpret_cast<OutPack<O, EPL> *>(out + sbase + pos) = o;
+        if (fallible && __any_sync(ACU_FULL_MASK, bad)) pack_lane_bits<EPL>(bad, l0 + u, bad_lo, bad_hi);  // failures are rare
       }
+    }
+    const uint64_t bad = (uint64_t)bad_lo | ((uint64_t)bad_hi << 32);
+    if (fallible && bad) {
+      if (safe) vw &= ~bad;  // unrepresentable => null
+      else err = min(err, (unsigned long long)(sbase + lane * 64 + __ffsll((long long)bad) - 1));
+    }
+    if (out_valid) { out_valid[(sbase >> 6) + lane] = vw; valid_cnt += __popcll(vw); }
+  }
+
+  if (warp == 0) {
+    for (int64_t row = sgroups << 11; row < n; row += 64) {
+      uint64_t vw = ones_to(row, n);
+      if (iv) vw &= ld_bits64(iv, ioff + row, ioff + n);
+      uint64_t bad = 0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t i = row + h * 32 + lane;
+        O x = O();
+        const bool b = ((vw >> (h * 32 + lane)) & 1ull) && !num_cast<I, O>(__ldg(in + i), x);
+        if (i < n) out[i] = x;
+        if constexpr (fallible) bad |= (uint64_t)__ballot_sync(ACU_FULL_MASK, b) << (h * 32);
+      }
+      if (fallible && bad) {
+        if (safe) vw &= ~bad;
+        else err = min(err, (unsigned long long)(row + __ffsll((long long)bad) - 1));
+      }
+      if (out_valid && lane == 0) { out_valid[row >> 6] = vw; valid_cnt += __popcll(vw); }
     }
   }
   if (out_valid) {
     valid_cnt = warp_sum(valid_cnt);
     if (lane == 0 && valid_cnt) atomicAdd(res + RES_COUNT, (unsigned long long)valid_cnt);
   }
+  if (fallible && err != ~0ull) atomicMin(res + RES_ERR_INDEX, err);
 }
 
 template <class I, class O>
@@ -849,22 +794,18 @@ acu_status cast_typed(acu_ctx *ctx, acu_dtype to, int32_t safe, const acu_array 
   if (len == 0) return ACU_OK;
   uint64_t *ov = out->has_validity ? reinterpret_cast<uint64_t *>(out->validity) : nullptr;
   ACU_TRY(acu_res_reset(ctx));
-  int64_t head = 0;
-  if constexpr (cast_infallible<I, O>::value) {
-    if ((uintptr_t)a->values % 16 == 0 && (uintptr_t)out->values % 16 == 0 && len >= 2048) {
-      const int64_t sgroups = len / 2048;
-      head = sgroups * 2048;
-      ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast_v2<I, O>), acu_wave_grid(ctx, k_cast_v2<I, O>, 256, 0, (sgroups + 7) / 8), 256, 0,
-                       static_cast<const I *>(a->values), static_cast<O *>(out->values), len, sgroups, a->validity,
-                       a->validity_offset, ov, ctx->d_res);
-    }
-  }
-  if (head < len) {
-    const int64_t strips = (len - head + 63) >> 6;
-    ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast<I, O>), acu_wave_grid(ctx, k_cast<I, O>, 256, 0, (strips + 31) / 32), 256, 0,
-                     static_cast<const I *>(a->values) + head, static_cast<O *>(out->values) + head, len - head, a->validity,
-                     a->validity_offset + head, ov ? ov + (head >> 6) : nullptr, safe, ctx->d_res);
-  }
+  const I *in = static_cast<const I *>(a->values);
+  O *o = static_cast<O *>(out->values);
+  // An 8-byte input read one element per lane is already one coalesced 256-B warp request; on an H100 that beats 16-B
+  // vectors for these casts (f64 -> i32 and i64 -> f64 at 1e8 and 1e9 rows), so only narrower inputs are vectorised.
+  constexpr int EPLV = sizeof(I) == 8 ? 1 : 16 / sizeof(I);
+  const int64_t blocks = (len / 2048 + 1 + 7) / 8;
+  if ((uintptr_t)in % 16 == 0 && (uintptr_t)o % 16 == 0)
+    ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast<I, O, EPLV>), acu_wave_grid(ctx, k_cast<I, O, EPLV>, 256, 0, blocks), 256, 0,
+                     in, o, len, a->validity, a->validity_offset, ov, safe, ctx->d_res);
+  else
+    ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast<I, O, 1>), acu_wave_grid(ctx, k_cast<I, O, 1>, 256, 0, blocks), 256, 0,
+                     in, o, len, a->validity, a->validity_offset, ov, safe, ctx->d_res);
   ACU_TRY(acu_res_fetch(ctx));
   if (!safe && ctx->h_res[RES_ERR_INDEX] != ~0ull) {
     const int64_t idx = (int64_t)ctx->h_res[RES_ERR_INDEX];

@@ -55,6 +55,11 @@ class Bench:
         self.ctx.check(self.lib.acu_bitmap_count(self.h, d, 0, None, 0, n, C.byref(c)))
         return d, c.value
 
+    def nulls(self, validity, offset, n):
+        c = C.c_int64(0)
+        self.ctx.check(self.lib.acu_bitmap_count(self.h, validity, offset, None, 0, n, C.byref(c)))
+        return n - c.value
+
     def timed(self, name, classes, alg_bytes, rows, fn, note=""):
         if self.only and not any(t in name for t in self.only.split("|")):
             return
@@ -104,6 +109,11 @@ def main():
             b.timed(name, [abi.K_ARITH], 24 * n + 3 * n / 8, n, lambda op=op: ctx.check(lib.acu_arith(h, abi.F64, op, C.byref(A), C.byref(Bv), C.byref(o))))
         for name, op in [("lt f64", abi.LT), ("eq f64", abi.EQ)]:
             b.timed(name, [abi.K_CMP], 16 * n + 4 * n / 8, n, lambda op=op: ctx.check(lib.acu_cmp(h, abi.F64, op, C.byref(A), C.byref(Bv), C.byref(o))))
+        # the same columns one element in: value pointers 8 bytes past a 16-byte boundary run the one-element-per-lane kernel
+        Au, Bu = b.arr(da + 8, va, n - 1, b.nulls(va, 1, n - 1)), b.arr(dbv + 8, vb, n - 1, b.nulls(vb, 1, n - 1))
+        Au.validity_offset = Bu.validity_offset = 1
+        b.timed("lt f64 unaligned", [abi.K_CMP], 16 * (n - 1) + 4 * (n - 1) / 8, n - 1,
+                lambda: ctx.check(lib.acu_cmp(h, abi.F64, abi.LT, C.byref(Au), C.byref(Bu), C.byref(o))))
         sc = b.arr(dbv, None, 1, 0, scalar=1)
         b.timed("add f64 array+scalar", [abi.K_ARITH], 16 * n + 2 * n / 8, n, lambda: ctx.check(lib.acu_arith(h, abi.F64, abi.ADD, C.byref(A), C.byref(sc), C.byref(o))))
         # Int64 checked add on the same buffers reinterpreted (values in [-2^61, 2^61) -> no overflow)
@@ -164,6 +174,13 @@ def main():
         Is = b.arr(di, va, ns, -1)
         oc = b.out(ns * 8, ns)
         b.timed("cast i64->f64", [abi.K_CAST], 16 * ns + 2 * ns / 8, ns, lambda: ctx.check(lib.acu_cast_numeric(h, abi.I64, abi.F64, 1, C.byref(Is), C.byref(oc))))
+        Iu = b.arr(di + 8, va, ns, -1)
+        Iu.validity_offset = 1
+        b.timed("cast i64->f64 unaligned", [abi.K_CAST], 16 * ns + 2 * ns / 8, ns,
+                lambda: ctx.check(lib.acu_cast_numeric(h, abi.I64, abi.F64, 1, C.byref(Iu), C.byref(oc))), note="input one element in")
+        Fs = b.arr(da, va, ns, -1)
+        b.timed("cast f64->i32 safe", [abi.K_CAST], 12 * ns + 2 * ns / 8, ns,
+                lambda: ctx.check(lib.acu_cast_numeric(h, abi.F64, abi.I32, 1, C.byref(Fs), C.byref(oc))), note="narrowing: out-of-range values become null")
         D = 4096
         rng = np.random.default_rng(1)
         lens = rng.integers(4, 13, D)
