@@ -46,7 +46,9 @@ def rand_values(rng, dtype, n, small=False):
 
 
 def rand_array(rng, dtype, n, null_p, offset=0, small=False):
-    """Random primitive array; `offset` > 0 builds a longer buffer and slices it (bit + element offsets)."""
+    """Random primitive array; `offset` > 0 builds a longer buffer and slices it. `Context.upload` copies the sliced values
+    into a fresh aligned allocation, so only the validity bit offset reaches the device; shifted device pointers are built
+    in test_gpu_elementwise_shapes.py and test_gpu_device_slices.py."""
     total = n + offset
     vals = rand_values(rng, dtype, total, small)
     mask = None if null_p is None else rng.random(total) >= null_p
