@@ -4,8 +4,8 @@ status / text / index).
 
 `Array::slice` moves the values pointer by offset * width, and every producer of device columns passes such pointers on
 (acu_import_column, the IPC reader's views into one body, the C++ mirror's slices). Several launchers pick another kernel
-or another staging path when a buffer is not 16-byte aligned: filter (k_filter_values + k_compress_bits instead of
-k_filter_fused / k_filter_values_async), take (per-lane index staging instead of cp.async.bulk), the Utf8 gathers with
+or another staging path when a buffer is not 16-byte aligned: filter (8-, 4- or 1-byte loads instead of cp.async in
+k_filter_fused, also below 4 % selectivity, where aligned values take k_filter_values_async), take (per-lane index staging instead of cp.async.bulk), the Utf8 gathers with
 32-bit indices (the generic kernels instead of FAST / k_dict_*) and zip (k_zip_elem instead of k_zip). `Context.upload`
 re-aligns every column, so the tests here build the shifted descriptors themselves, and every helper asserts that the
 pointer it produces is not 16-byte aligned. Shifts are whole elements at the element's natural alignment.
@@ -251,7 +251,8 @@ def validity_column(gpu, rng, dtype, n, shift, validity):
 @pytest.mark.parametrize("dtype", [abi.I8, abi.I16, abi.I32, abi.I64, abi.F64])
 @pytest.mark.parametrize("true_p", SELECTIVITIES)
 def test_filter_shifted_column(gpu, oracle, dtype, true_p):
-    """k_filter_values<W> with its 8-byte / 4-byte / byte loads, and the validity through k_compress_bits."""
+    """k_filter_fused<W, false> with its 8-byte / 4-byte / byte loads, the validity compacted in the same pass or, below
+    4 % selectivity, through k_compress_bits."""
     rng = np.random.default_rng(20_000 + dtype * 100 + int(true_p * 100))
     shifts = unaligned_shifts(abi.DTYPE_SIZE[dtype])
     k = 0
@@ -289,20 +290,38 @@ def test_filter_shifted_column_multi_round(gpu, oracle, dtype, shift):
         col.free()
 
 
-def test_shifted_filter_takes_the_unfused_kernels(gpu):
-    """At 50 % selectivity a column with nulls is filtered by k_filter_fused (values and validity in one launch) when its
-    base is 16-byte aligned, and by k_filter_values + k_zero_outputs + k_compress_bits when it is not."""
+def filter_launches(gpu, fn):
+    """(all launches, launches of the filter's value and bit-compaction kernels) of fn, after a warm call."""
+    fn()
+    gpu.check(gpu.lib.acu_kernel_stats_reset(gpu.h))
+    before = gpu.launch_count()
+    fn()
+    gpu.check(gpu.lib.acu_ctx_sync(gpu.h))
+    ms, n = C.c_double(0), C.c_int64(0)
+    gpu.check(gpu.lib.acu_kernel_stats(gpu.h, abi.K_FILTER, C.byref(ms), C.byref(n)))
+    return gpu.launch_count() - before, n.value
+
+
+def test_shifted_filter_takes_the_aligned_launches(gpu):
+    """A column with nulls is filtered by as many launches whether its values base is 16-byte aligned or not: at 50 %
+    selectivity one value launch that also compacts the validity (no k_compress_bits), and below 4 % the value launch
+    plus k_zero_outputs + k_compress_bits for the validity."""
     rng = np.random.default_rng(20_600)
     n = 70001
     col, _, aligned = column(gpu, abi.I64, rng.integers(-9, 9, n + 1 + PAD), rng.random(n + 1 + PAD) >= 0.05, 0, n, exact_count=True)
     _, shifted = at(col, 1, n, exact_count=True)
     assert aligned.values % 16 == 0 and aligned.null_count > 0 and shifted.null_count > 0
-    plan = Plan(gpu, rand_bool(rng, n, 0.5, 0.05))
+    dense, sparse = Plan(gpu, rand_bool(rng, n, 0.5, 0.05)), Plan(gpu, rand_bool(rng, n, 0.02, 0.05))
     try:
-        assert plan.count * 25 >= n  # not the sparse (< 4 %) path, where aligned columns also compact the validity apart
-        assert launches(gpu, lambda: plan.filter(abi.I64, shifted)) > launches(gpu, lambda: plan.filter(abi.I64, aligned))
+        assert dense.count * 25 >= n and sparse.count * 25 < n
+        d_al, d_sh = (filter_launches(gpu, lambda: dense.filter(abi.I64, d)) for d in (aligned, shifted))
+        s_al, s_sh = (filter_launches(gpu, lambda: sparse.filter(abi.I64, d)) for d in (aligned, shifted))
+        assert d_al == d_sh and s_al == s_sh
+        assert d_al[1] == 1 and s_al[1] == 2  # timed filter kernels: the value kernel, + k_compress_bits when sparse
+        assert s_al[0] == d_al[0] + 2  # + k_zero_outputs and k_compress_bits
     finally:
-        plan.free()
+        dense.free()
+        sparse.free()
         col.free()
 
 

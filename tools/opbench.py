@@ -138,19 +138,32 @@ def main():
             b.timed(name, [abi.K_REDUCE], 8 * n + n / 8, n, lambda dt=dt, arr_=arr_, op=op: ctx.check(lib.acu_aggregate(h, dt, op, C.byref(arr_), C.byref(bits_), C.byref(cnt_))))
         ctx.free(dj)
         # ---------------- config 2: filter + take Int64 1e9 ----------------
-        for sel in (0.01, 0.1, 0.5, 0.9):
+        # the same Int64 column one element in (values 8 bytes past a 16-byte boundary, validity offset 1), and its first n
+        # bytes as an Int8 column: the workloads on each side of the kernel's alignment and < 4 % validity choices
+        Iu = b.arr(di + 8, va, n - 1, b.nulls(va, 1, n - 1))
+        Iu.validity_offset = 1
+        I8 = b.arr(di, va, n, n - nva)
+        for sel in (0.001, 0.01, 0.1, 0.5, 0.9):
             dp, m = b.bits(46, sel, n)
             pred = b.arr(dp, None, n, 0)
+            pred_u = b.arr(dp, None, n - 1, 0)
             of = b.out(m * 8, m)
             plan = C.c_void_p()
 
-            def run_filter():
+            def run_filter(pred=pred, width=8, col=I):
                 p = C.c_void_p()
                 ctx.check(lib.acu_filter_plan_create(h, C.byref(pred), C.byref(p)))
-                ctx.check(lib.acu_filter_primitive(h, p, 8, C.byref(I), C.byref(of)))
+                ctx.check(lib.acu_filter_primitive(h, p, width, C.byref(col), C.byref(of)))
                 lib.acu_filter_plan_destroy(h, p)
 
-            b.timed(f"filter i64 s={sel}", [abi.K_FILTER, abi.K_FILTER_PLAN], 8 * n + 2 * n / 8 + 8 * m + m / 8, n, run_filter, note=f"selected {m}; plan + values + validity kernels")
+            note = f"selected {m}; plan + values + validity kernels"
+            b.timed(f"filter i64 s={sel}", [abi.K_FILTER, abi.K_FILTER_PLAN], 8 * n + 2 * n / 8 + 8 * m + m / 8, n, run_filter, note=note)
+            if sel in (0.01, 0.5):
+                b.timed(f"filter i64 s={sel} unaligned", [abi.K_FILTER, abi.K_FILTER_PLAN], 8 * n + 2 * n / 8 + 8 * m + m / 8, n - 1,
+                        lambda: run_filter(pred=pred_u, col=Iu), note=note + "; values one element in")
+            if sel == 0.01:
+                b.timed(f"filter i8 s={sel}", [abi.K_FILTER, abi.K_FILTER_PLAN], n + 2 * n / 8 + m + m / 8, n,
+                        lambda: run_filter(width=1, col=I8), note=note)
             if sel in (0.1, 0.5):
                 didx = ctx.malloc(m * 4 + 64)
                 ctx.check(lib.acu_filter_plan_create(h, C.byref(pred), C.byref(plan)))
