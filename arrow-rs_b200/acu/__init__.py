@@ -988,6 +988,42 @@ class Context:
             for p in owned:
                 self.free(p)
 
+    # -- like / ilike / contains / starts_with / ends_with / eq_ignore_ascii_case (arrow-string/src/like.rs) -------
+    def like_bytes(self, op, a, b, is_utf8=True):
+        """a (haystack), b (pattern / needle): Utf8Column; is_utf8=False for Binary / LargeBinary."""
+        assert a.offsets.dtype == b.offsets.dtype
+        owned = []
+        n = max(a.nulls.length if not a.nulls.is_scalar else 0, b.nulls.length if not b.nulls.is_scalar else 0, 1)
+        out = self.alloc_out(bitmap_bytes(n), n)
+        try:
+            descs = [self._upload_bytes_col(col, owned) for col in (a, b)]
+            self.check(self.lib.acu_like_bytes(self.h, a.offsets.dtype.itemsize, int(is_utf8), op, C.byref(descs[0]), C.byref(descs[1]),
+                                               C.byref(out)))
+            res, out = self.download_out(out, BOOL), None
+            return res
+        finally:
+            if out is not None:
+                self._free_out(out)
+            for p in owned:
+                self.free(p)
+
+    def like_view(self, op, a, b, is_utf8=True):
+        """a (haystack), b (pattern / needle): ViewColumn; is_utf8=False for BinaryView."""
+        owned = []
+        n = max(a.length if not a.nulls.is_scalar else 0, b.length if not b.nulls.is_scalar else 0, 1)
+        out = self.alloc_out(bitmap_bytes(n), n)
+        try:
+            keep = []
+            descs = [self._upload_view_col(col, owned, keep) for col in (a, b)]
+            self.check(self.lib.acu_like_byte_view(self.h, int(is_utf8), op, C.byref(descs[0]), C.byref(descs[1]), C.byref(out)))
+            res, out = self.download_out(out, BOOL), None
+            return res
+        finally:
+            if out is not None:
+                self._free_out(out)
+            for p in owned:
+                self.free(p)
+
     # -- fused compare -> filter (cmp.rs:220-382 feeding filter.rs:254-273) -------------------
     def filter_cmp(self, values, op, a, b):
         """filter(values, &cmp::op(a, b)?) with the predicate never materialised: the comparison writes the filter plan."""

@@ -34,6 +34,8 @@ ADD_WRAPPING, ADD, SUB_WRAPPING, SUB, MUL_WRAPPING, MUL, DIV, REM = range(8)
 EQ, NEQ, LT, LT_EQ, GT, GT_EQ, DISTINCT, NOT_DISTINCT = range(8)
 # acu_agg_op
 SUM, MIN, MAX = range(3)
+# acu_like_op (arrow-string/src/like.rs `enum Op`)
+LIKE, NLIKE, ILIKE, NILIKE, CONTAINS, STARTS_WITH, ENDS_WITH, EQ_IGNORE_ASCII_CASE = range(8)
 # acu_filter_strategy
 FILTER_NONE, FILTER_ALL, FILTER_INDEX, FILTER_SLICES = range(4)
 
@@ -202,6 +204,8 @@ PROTOTYPES = {
     "acu_cmp": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_cmp_bytes": (i32, [vp, i32, i32, P(BytesArray), P(BytesArray), P(ArrayOut)]),
     "acu_cmp_byte_view": (i32, [vp, i32, P(ViewArray), P(ViewArray), P(ArrayOut)]),
+    "acu_like_bytes": (i32, [vp, i32, i32, i32, P(BytesArray), P(BytesArray), P(ArrayOut)]),
+    "acu_like_byte_view": (i32, [vp, i32, i32, P(ViewArray), P(ViewArray), P(ArrayOut)]),
     "acu_cast_numeric": (i32, [vp, i32, i32, i32, P(Array), P(ArrayOut)]),
     "acu_boolean": (i32, [vp, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_aggregate": (i32, [vp, i32, i32, P(Array), P(u64), P(i64)]),

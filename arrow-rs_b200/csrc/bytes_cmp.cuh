@@ -1,5 +1,5 @@
 // bytes_cmp.cuh — device helpers that read and order variable-width values (Utf8 / Binary, Utf8View / BinaryView),
-// shared by the comparison kernels (strcmp.cu) and the min / max reductions (aggregate_bytes.cu).
+// shared by the comparison kernels (strcmp.cu), the min / max reductions (aggregate_bytes.cu) and the LIKE family (like.cu).
 //
 // Order: Rust's `Ord` for `&[u8]` (lexicographic on unsigned bytes, a proper prefix sorts first); `&str` orders the same.
 #pragma once
@@ -38,14 +38,29 @@ __device__ __forceinline__ uint64_t bswap64(uint64_t x) {
   return ((uint64_t)__byte_perm(lo, 0, 0x0123) << 32) | (uint64_t)__byte_perm(hi, 0, 0x0123);
 }
 
-// `&[u8]` equality / ordering of Rust (lexicographic on unsigned bytes, then length)
-__device__ __forceinline__ bool bytes_eq(const uint8_t *a, int64_t la, const uint8_t *b, int64_t lb) {
-  if (la != lb) return false;
-  for (int64_t k = 0; k < la; k += 8) {
-    const uint32_t nb = (uint32_t)((la - k) < 8 ? (la - k) : 8);
-    if (ld_upto8(a + k, nb) != ld_upto8(b + k, nb)) return false;
+// u8::to_ascii_lowercase on each of 8 bytes: 'A'..='Z' gain 0x20, every other byte (non-ASCII included) stays
+__device__ __forceinline__ uint64_t ascii_lower8(uint64_t x) {
+  const uint64_t h = x & 0x7f7f7f7f7f7f7f7full;
+  const uint64_t ge_a = h + 0x3f3f3f3f3f3f3f3full;  // bit 7 set where h >= 'A'
+  const uint64_t gt_z = h + 0x2525252525252525ull;  // bit 7 set where h > 'Z'
+  return x | (((ge_a & ~gt_z & ~x) & 0x8080808080808080ull) >> 2);
+}
+
+// n bytes of a and b equal; ICASE: u8::eq_ignore_ascii_case per byte
+template <bool ICASE>
+__device__ __forceinline__ bool bytes_range_eq(const uint8_t *a, const uint8_t *b, int64_t n) {
+  for (int64_t k = 0; k < n; k += 8) {
+    const uint32_t nb = (uint32_t)((n - k) < 8 ? (n - k) : 8);
+    uint64_t x = ld_upto8(a + k, nb), y = ld_upto8(b + k, nb);
+    if (ICASE) x = ascii_lower8(x), y = ascii_lower8(y);
+    if (x != y) return false;
   }
   return true;
+}
+
+// `&[u8]` equality / ordering of Rust (lexicographic on unsigned bytes, then length)
+__device__ __forceinline__ bool bytes_eq(const uint8_t *a, int64_t la, const uint8_t *b, int64_t lb) {
+  return la == lb && bytes_range_eq<false>(a, b, la);
 }
 __device__ __forceinline__ bool bytes_lt(const uint8_t *a, int64_t la, const uint8_t *b, int64_t lb) {
   const int64_t n = la < lb ? la : lb;

@@ -1306,6 +1306,64 @@ inline std::optional<bool> max_boolean(const BooleanArray &a) { return detail::b
 inline std::optional<bool> bool_and(const BooleanArray &a) { return min_boolean(a); }
 inline std::optional<bool> bool_or(const BooleanArray &a) { return max_boolean(a); }
 
+// ---- like (arrow-string/src/like.rs) --------------------------------------------------------------------------
+// like / nlike / ilike / nilike / contains / starts_with / ends_with / eq_ignore_ascii_case on Utf8 and Utf8View arrays
+// and scalars (the haystack first), through acu_like_bytes / acu_like_byte_view.
+namespace like {
+namespace detail {
+inline Result<BooleanArray> like_strings(acu_like_op op, const StringArray &l, bool ls, const StringArray &r, bool rs) {
+  Context &c = Context::get();
+  const int64_t n = ls ? r.len() : l.len();
+  Buffer vb, nb;
+  acu_bytes_array a = kernels::cmp::bytes_view(l, ls), b = kernels::cmp::bytes_view(r, rs);
+  acu_array_out o = compute::detail::make_out(vb, nb, acu_bitmap_bytes(std::max<int64_t>(n, 1)), std::max<int64_t>(n, 1));
+  const acu_status st = acu_like_bytes(c.raw(), 4, 1, op, &a, &b, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return BooleanArray(vb, 0, o.len, compute::detail::out_nulls(o, nb));
+}
+struct ViewDesc {  // an acu_view_array with the buffer pointer table and the validity it points at
+  std::vector<const uint8_t *> ptrs;
+  std::optional<NullBuffer> nulls;
+  acu_view_array v{};
+  ViewDesc(const StringViewArray &a, bool scalar) : nulls(nulls_from_mask(a.valid())) {
+    for (const auto &b : a.data_buffers()) ptrs.push_back(static_cast<const uint8_t *>(b.buffer.data()));
+    v.views = a.views_ptr();
+    v.buffers = ptrs.data();
+    v.n_buffers = (int32_t)ptrs.size();
+    v.nulls.len = a.len();
+    v.nulls.is_scalar = scalar ? 1 : 0;
+    if (nulls) {
+      v.nulls.validity = static_cast<const uint8_t *>(nulls->buffer.data());
+      v.nulls.null_count = nulls->null_count;
+    }
+  }
+};
+inline Result<BooleanArray> like_views(acu_like_op op, const StringViewArray &l, bool ls, const StringViewArray &r, bool rs) {
+  Context &c = Context::get();
+  const int64_t n = ls ? r.len() : l.len();
+  Buffer vb, nb;
+  const ViewDesc a(l, ls), b(r, rs);
+  acu_array_out o = compute::detail::make_out(vb, nb, acu_bitmap_bytes(std::max<int64_t>(n, 1)), std::max<int64_t>(n, 1));
+  const acu_status st = acu_like_byte_view(c.raw(), 1, op, &a.v, &b.v, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return BooleanArray(vb, 0, o.len, compute::detail::out_nulls(o, nb));
+}
+}  // namespace detail
+#define ACU_LIKE_FN(NAME, OP)                                                                                                     \
+  inline Result<BooleanArray> NAME(const StringArray &l, const StringArray &r) { return detail::like_strings(OP, l, false, r, false); } \
+  inline Result<BooleanArray> NAME(const StringArray &l, const Scalar<StringArray> &r) { return detail::like_strings(OP, l, false, r.array, true); } \
+  inline Result<BooleanArray> NAME(const Scalar<StringArray> &l, const StringArray &r) { return detail::like_strings(OP, l.array, true, r, false); } \
+  inline Result<BooleanArray> NAME(const Scalar<StringArray> &l, const Scalar<StringArray> &r) { return detail::like_strings(OP, l.array, true, r.array, true); } \
+  inline Result<BooleanArray> NAME(const StringViewArray &l, const StringViewArray &r) { return detail::like_views(OP, l, false, r, false); } \
+  inline Result<BooleanArray> NAME(const StringViewArray &l, const Scalar<StringViewArray> &r) { return detail::like_views(OP, l, false, r.array, true); } \
+  inline Result<BooleanArray> NAME(const Scalar<StringViewArray> &l, const StringViewArray &r) { return detail::like_views(OP, l.array, true, r, false); } \
+  inline Result<BooleanArray> NAME(const Scalar<StringViewArray> &l, const Scalar<StringViewArray> &r) { return detail::like_views(OP, l.array, true, r.array, true); }
+ACU_LIKE_FN(like, ACU_LIKE) ACU_LIKE_FN(nlike, ACU_NLIKE) ACU_LIKE_FN(ilike, ACU_ILIKE) ACU_LIKE_FN(nilike, ACU_NILIKE)
+ACU_LIKE_FN(contains, ACU_CONTAINS) ACU_LIKE_FN(starts_with, ACU_STARTS_WITH) ACU_LIKE_FN(ends_with, ACU_ENDS_WITH)
+ACU_LIKE_FN(eq_ignore_ascii_case, ACU_EQ_IGNORE_ASCII_CASE)
+#undef ACU_LIKE_FN
+}  // namespace like
+
 
 // ---- nullif / zip (arrow-select/src/nullif.rs:44-113, zip.rs:99-226) -------------------------------------------
 namespace detail {

@@ -372,6 +372,40 @@ acu_status acu_cmp_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_cmp_op op, cons
 acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_view_array *l, const acu_view_array *r,
                              acu_array_out *out);
 
+/* ------------------------------------------------------------------------- */
+/* like — arrow-string/src/like.rs                                           */
+/* ------------------------------------------------------------------------- */
+/* arrow-string/src/like.rs `enum Op` */
+typedef enum acu_like_op {
+  ACU_LIKE = 0, ACU_NLIKE = 1, ACU_ILIKE = 2, ACU_NILIKE = 3,
+  ACU_CONTAINS = 4, ACU_STARTS_WITH = 5, ACU_ENDS_WITH = 6, ACU_EQ_IGNORE_ASCII_CASE = 7
+} acu_like_op;
+/* like / nlike / ilike / nilike / contains / starts_with / ends_with / eq_ignore_ascii_case (like.rs:83-216, like_op
+ * :218-296). l = the haystack, r = the pattern / needle; either may be a scalar (nulls.is_scalar), with the column layouts
+ * of acu_cmp_bytes / acu_cmp_byte_view. is_utf8 = 1 for Utf8 / LargeUtf8 / Utf8View, 0 for Binary / LargeBinary /
+ * BinaryView, which accept only contains / starts_with / ends_with (binary_like.rs:34-47).
+ * Result (a boolean array, as acu_cmp):
+ *   - r a null scalar: every row null (BooleanArray::new_null);
+ *   - r a non-null scalar (op_scalar): the predicate runs at every slot of l, null slots included, and the result carries
+ *     l's NullBuffer as it is (present iff l->nulls.validity != NULL);
+ *   - otherwise (op_binary, l an array or a scalar): a row with a null side is null with value bit 0, and the result has a
+ *     NullBuffer iff some row is null.
+ * LIKE patterns: `\x` is a literal x (a trailing `\` a literal backslash), `%` any run of characters, `_` one character
+ * (one UTF-8 scalar), anchored at both ends; ilike folds like the reference's regex (simple case folding: an ASCII letter
+ * matches both cases, k / K also U+212A and s / S also U+017F). Errors: lengths differ => ACU_ERR_INVALID_ARGUMENT "Cannot
+ * compare arrays of different lengths, got {l} vs {r}"; a binary column with another op => ACU_ERR_INVALID_ARGUMENT
+ * "Invalid binary operation: {OP}" (LIKE, NILIKE, EQ_IGNORE_ASCII_CASE, ...).
+ * Not reproduced:
+ *   - an ilike / nilike pattern with a non-ASCII character fails with ACU_ERR_NOT_YET_IMPLEMENTED wherever the reference
+ *     would compile it: a non-null scalar pattern (detail.index = -1), or a per-row pattern in a row whose two sides are
+ *     non-null (detail.index = the lowest such row);
+ *   - the reference fails to compile the regex of a huge pattern (its regex size limit); the device matches it.
+ * Synchronous (not available inside a stream-ordered section); kernel time is counted in ACU_K_CMP. */
+acu_status acu_like_bytes(acu_ctx *ctx, int32_t offset_bytes, int32_t is_utf8, acu_like_op op, const acu_bytes_array *l,
+                          const acu_bytes_array *r, acu_array_out *out);
+acu_status acu_like_byte_view(acu_ctx *ctx, int32_t is_utf8, acu_like_op op, const acu_view_array *l,
+                              const acu_view_array *r, acu_array_out *out);
+
 /* Utf8View / BinaryView buffer management for BatchCoalescer (InProgressByteViewArray, arrow-select/src/coalesce/
  * byte_view.rs). The reference decides per source array whether its data buffers are compacted ("gc": when they hold more
  * than twice the bytes its views use, :366-381) and how output buffers are sized (BufferSource, :526-559); that policy stays

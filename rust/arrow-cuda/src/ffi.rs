@@ -48,6 +48,15 @@ pub const ACU_GT: i32 = 4;
 pub const ACU_GT_EQ: i32 = 5;
 pub const ACU_DISTINCT: i32 = 6;
 pub const ACU_NOT_DISTINCT: i32 = 7;
+// acu_like_op (arrow-string/src/like.rs `enum Op`)
+pub const ACU_LIKE: i32 = 0;
+pub const ACU_NLIKE: i32 = 1;
+pub const ACU_ILIKE: i32 = 2;
+pub const ACU_NILIKE: i32 = 3;
+pub const ACU_CONTAINS: i32 = 4;
+pub const ACU_STARTS_WITH: i32 = 5;
+pub const ACU_ENDS_WITH: i32 = 6;
+pub const ACU_EQ_IGNORE_ASCII_CASE: i32 = 7;
 pub const ACU_SUM: i32 = 0;
 pub const ACU_MIN: i32 = 1;
 pub const ACU_MAX: i32 = 2;
@@ -205,6 +214,10 @@ extern "C" {
     pub fn acu_cmp_bytes(ctx: *mut acu_ctx, offset_bytes: i32, op: i32, l: *const acu_bytes_array, r: *const acu_bytes_array,
                          out: *mut acu_array_out) -> acu_status;
     pub fn acu_cmp_byte_view(ctx: *mut acu_ctx, op: i32, l: *const acu_view_array, r: *const acu_view_array, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_like_bytes(ctx: *mut acu_ctx, offset_bytes: i32, is_utf8: i32, op: i32, l: *const acu_bytes_array, r: *const acu_bytes_array,
+                          out: *mut acu_array_out) -> acu_status;
+    pub fn acu_like_byte_view(ctx: *mut acu_ctx, is_utf8: i32, op: i32, l: *const acu_view_array, r: *const acu_view_array,
+                              out: *mut acu_array_out) -> acu_status;
     pub fn acu_concat(ctx: *mut acu_ctx, n_arrays: i32, arrays: *const acu_column, out: *mut acu_column_out) -> acu_status;
     pub fn acu_concat_batches(ctx: *mut acu_ctx, n_batches: i32, n_columns: i32, columns: *const acu_column, outs: *mut acu_column_out,
                               out_rows: *mut i64) -> acu_status;

@@ -425,6 +425,87 @@ pub mod compute {
 
     /// min / max of byte, view, fixed-size-binary and boolean arrays (aggregate.rs:372-568, :880-889). The device returns the
     /// lowest row holding the extremal value; the result borrows that row from the host array, as the reference's does.
+    /// `arrow::compute::like` (arrow-string/src/like.rs:83-216): the haystack first; Utf8 / LargeUtf8 / Utf8View take all eight,
+    /// Binary / LargeBinary / BinaryView contains / starts_with / ends_with. Dictionary operands are not accepted.
+    pub mod like {
+        use super::super::{ffi, ColumnOut, Context, DeviceArray, DeviceBuffer};
+        use arrow_array::types::ByteViewType;
+        use arrow_array::{Array, BooleanArray, Datum, GenericByteViewArray};
+        use arrow_array::cast::AsArray;
+        use arrow_schema::{ArrowError, DataType};
+
+        const OP_NAMES: [&str; 8] = ["LIKE", "NLIKE", "ILIKE", "NILIKE", "CONTAINS", "STARTS_WITH", "ENDS_WITH", "EQ_IGNORE_ASCII_CASE"];
+
+        fn view_operand<T: ByteViewType + ?Sized>(ctx: &Context, a: &GenericByteViewArray<T>, scalar: bool, bufs: &mut Vec<DeviceBuffer>,
+                                                  ptrs: &mut Vec<*const u8>) -> Result<ffi::acu_view_array, ArrowError> {
+            let (validity, validity_offset, null_count) = match a.nulls() {
+                Some(n) => {
+                    let b = DeviceBuffer::from_host(ctx, n.buffer().as_slice())?;
+                    let p = b.as_ptr() as *const u8;
+                    bufs.push(b);
+                    (p, n.offset() as i64, n.null_count() as i64)
+                }
+                None => (std::ptr::null(), 0, 0),
+            };
+            let v = DeviceBuffer::from_host(ctx, a.views().inner().as_slice())?;
+            let views = v.as_ptr();
+            bufs.push(v);
+            for d in a.data_buffers() {
+                let b = DeviceBuffer::from_host(ctx, d.as_slice())?;
+                ptrs.push(b.as_ptr() as *const u8);
+                bufs.push(b);
+            }
+            let nulls = ffi::acu_array { values: std::ptr::null(), values_offset: 0, validity, validity_offset, len: a.len() as i64, null_count,
+                                         is_scalar: scalar as i32, reserved: 0 };
+            Ok(ffi::acu_view_array { views, buffers: ptrs.as_ptr(), n_buffers: ptrs.len() as i32, reserved: 0, nulls })
+        }
+
+        /// like_op (like.rs:218-296)
+        fn like_op(op: i32, lhs: &dyn Datum, rhs: &dyn Datum) -> Result<BooleanArray, ArrowError> {
+            use DataType::*;
+            let (l, l_s) = lhs.get();
+            let (r, r_s) = rhs.get();
+            let ctx = Context::current()?;
+            let n = if l_s { r.len() } else { l.len() };
+            let mut out = ColumnOut::new(&ctx, &DataType::Boolean, n, 0)?;
+            let is_utf8 = matches!(l.data_type(), Utf8 | LargeUtf8 | Utf8View) as i32;
+            let st = match (l.data_type(), r.data_type()) {
+                (Utf8, Utf8) | (LargeUtf8, LargeUtf8) | (Binary, Binary) | (LargeBinary, LargeBinary) => {
+                    let ob = if matches!(l.data_type(), LargeUtf8 | LargeBinary) { 8 } else { 4 };
+                    let (a, b) = (DeviceArray::upload(&ctx, l, l_s)?, DeviceArray::upload(&ctx, r, r_s)?);
+                    let (x, y) = (ffi::acu_bytes_array { offsets: a.view().values, data: a.column.data, nulls: *a.view() },
+                                  ffi::acu_bytes_array { offsets: b.view().values, data: b.column.data, nulls: *b.view() });
+                    unsafe { ffi::acu_like_bytes(ctx.raw(), ob, is_utf8, op, &x, &y, out.array_out()) }
+                }
+                (Utf8View, Utf8View) | (BinaryView, BinaryView) => {
+                    let (mut bufs, mut lp, mut rp) = (Vec::new(), Vec::new(), Vec::new());
+                    let (x, y) = if is_utf8 != 0 {
+                        (view_operand(&ctx, l.as_string_view(), l_s, &mut bufs, &mut lp)?, view_operand(&ctx, r.as_string_view(), r_s, &mut bufs, &mut rp)?)
+                    } else {
+                        (view_operand(&ctx, l.as_binary_view(), l_s, &mut bufs, &mut lp)?, view_operand(&ctx, r.as_binary_view(), r_s, &mut bufs, &mut rp)?)
+                    };
+                    unsafe { ffi::acu_like_byte_view(ctx.raw(), is_utf8, op, &x, &y, out.array_out()) }
+                }
+                (l_t, r_t) => {
+                    return Err(ArrowError::InvalidArgumentError(format!("Invalid string/binary operation: {l_t} {} {r_t}", OP_NAMES[op as usize])))
+                }
+            };
+            ctx.check(st)?;
+            let r = out.finish(&DataType::Boolean)?;
+            Ok(r.as_any().downcast_ref::<BooleanArray>().unwrap().clone())
+        }
+        pub fn like(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> { like_op(ffi::ACU_LIKE, left, right) }
+        pub fn ilike(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> { like_op(ffi::ACU_ILIKE, left, right) }
+        pub fn nlike(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> { like_op(ffi::ACU_NLIKE, left, right) }
+        pub fn nilike(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> { like_op(ffi::ACU_NILIKE, left, right) }
+        pub fn starts_with(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> { like_op(ffi::ACU_STARTS_WITH, left, right) }
+        pub fn ends_with(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> { like_op(ffi::ACU_ENDS_WITH, left, right) }
+        pub fn contains(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> { like_op(ffi::ACU_CONTAINS, left, right) }
+        pub fn eq_ignore_ascii_case(left: &dyn Datum, right: &dyn Datum) -> Result<BooleanArray, ArrowError> {
+            like_op(ffi::ACU_EQ_IGNORE_ASCII_CASE, left, right)
+        }
+    }
+
     pub mod aggregate {
         use super::super::{ffi, Context, DeviceArray, DeviceBuffer};
         use arrow_array::types::{BinaryViewType, ByteViewType, StringViewType};

@@ -218,10 +218,31 @@ def main():
         # ---------------- min / max of byte columns (arrow-arith/src/aggregate.rs:460-568), bool_and ----------------
         if not b.only or any(t in "min_string max_string cmp_bytes bool_and" for t in b.only.split("|")):
             agg_bytes_rows(b, ctx, ns, d_off, d_data, dkeys, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D, va, nva, n)
+        # ---------------- like family (arrow-string/src/like.rs) ----------------
+        if not b.only or any(t in "like starts_with ends_with contains cmp_bytes cmp_byte_view" for t in b.only.split("|")):
+            like_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D)
     print("\n| op | rows | kernel ms | GB/s (algorithmic) | % of measured HBM peak | Mrows/s |")
     print("|---|---|---|---|---|---|")
     for r in b.rows:
         print(f"| {r['op']} | {r['rows']:.3g} | {r['kernel_ms']} | {r['achieved_gbs']} | {100 * r['frac_of_measured_peak']:.1f} | {r['mrows_s']} |")
+
+
+def dict_view_column(b, ctx, keys, offs, data, D, ns):
+    """The dictionary-decoded column as all-inline views: take(dictionary views, keys) with 16-byte elements."""
+    dict_views = np.zeros((D, 16), dtype=np.uint8)
+    for k in range(D):
+        ln = int(offs[k + 1] - offs[k])
+        dict_views[k, :4] = np.frombuffer(np.uint32(ln).tobytes(), np.uint8)
+        dict_views[k, 4:4 + ln] = data[offs[k]: offs[k + 1]]
+    d_dv = ctx.malloc(dict_views.nbytes + 64)
+    ctx.h2d(d_dv, dict_views)
+    ovw = b.out(ns * 16, ns)
+    ctx.check(ctx.lib.acu_take_primitive(ctx.h, 16, C.byref(b.arr(d_dv, None, D, 0)), C.byref(keys), abi.I32, 0, C.byref(ovw)))
+    ctx.free(d_dv)
+    V = abi.ViewArray()
+    V.views, V.buffers, V.n_buffers = ovw.values, (C.c_void_p * 1)(), 0
+    V.nulls = b.arr(None, ovw.validity, ns, ovw.null_count if ovw.has_validity else 0)
+    return V, ovw
 
 
 def agg_bytes_rows(b, ctx, ns, d_off, d_data, dkeys, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D, va, nva, n):
@@ -246,25 +267,13 @@ def agg_bytes_rows(b, ctx, ns, d_off, d_data, dkeys, keys, dict_nulls, d_out_off
     b.timed("min_max bar: cmp_bytes lt utf8 dict-decoded", [abi.K_CMP], 2 * ub + ns / 8, ns,
             lambda: ctx.check(lib.acu_cmp_bytes(h, 4, abi.LT, C.byref(U), C.byref(U), C.byref(ov))), note="reads the column twice")
     ctx._free_out(ov)
-    # the same values as an all-inline view column: take(dictionary views, keys) with 16-byte elements
-    dict_views = np.zeros((D, 16), dtype=np.uint8)
-    for k in range(D):
-        ln = int(offs[k + 1] - offs[k])
-        dict_views[k, :4] = np.frombuffer(np.uint32(ln).tobytes(), np.uint8)
-        dict_views[k, 4:4 + ln] = data[offs[k]: offs[k + 1]]
-    d_dv = ctx.malloc(dict_views.nbytes + 64)
-    ctx.h2d(d_dv, dict_views)
-    ovw = b.out(ns * 16, ns)
-    ctx.check(lib.acu_take_primitive(h, 16, C.byref(b.arr(d_dv, None, D, 0)), C.byref(keys), abi.I32, 0, C.byref(ovw)))
-    V = abi.ViewArray()
-    V.views, V.buffers, V.n_buffers = ovw.values, (C.c_void_p * 1)(), 0
-    V.nulls = b.arr(None, ovw.validity, ns, ovw.null_count if ovw.has_validity else 0)
+    # the same values as an all-inline view column
+    V, ovw = dict_view_column(b, ctx, keys, offs, data, D, ns)
     vb = 16 * ns + ns / 8
     for name, op in (("min_string_view inline dict-decoded", abi.MIN), ("max_string_view inline dict-decoded", abi.MAX)):
         b.timed(name, [abi.K_REDUCE], vb, ns, lambda op=op: ctx.check(lib.acu_aggregate_byte_view(h, op, C.byref(V), C.byref(row), C.byref(cnt))),
                 note="views only (all values inline)")
     ctx._free_out(ovw)
-    ctx.free(d_dv)
     # adversarial: every value = the same 24-byte prefix + an 8-byte tail (4096 distinct tails): every key ties
     na = 10_000_000
     rng = np.random.default_rng(3)
@@ -308,6 +317,69 @@ def agg_bytes_rows(b, ctx, ns, d_off, d_data, dkeys, keys, dict_nulls, d_out_off
     val = C.c_int32(0)
     b.timed("bool_and 1e9", [abi.K_REDUCE], 2 * n / 8, n, lambda: ctx.check(lib.acu_aggregate_boolean(h, abi.MIN, C.byref(BA), C.byref(val), C.byref(cnt))))
     ctx.free(bv)
+
+
+def like_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D):
+    """like / starts_with / ends_with / contains / ilike against a scalar on the dictionary-decoded Utf8 column of config 4
+    (D = 4096 values of 4..12 bytes, mean 8, 5 % nulls) and on the same values as all-inline views, with acu_cmp_bytes /
+    acu_cmp_byte_view EQ against the same scalar as the same-traffic yardstick. Algorithmic bytes (DESIGN.md §3): Utf8 =
+    offsets + validity + result bits + the value bytes the op must read (eq: rows whose length equals the needle's, prefix /
+    suffix: the needle's length in rows at least that long, substring / glob: every value byte); views = 16 B per view +
+    validity + result bits (every value is inline)."""
+    lib, h = ctx.lib, ctx.h
+    total = C.c_int64(0)
+    ctx.check(lib.acu_take_bytes(h, 4, d_off, d_data, C.byref(dict_nulls), C.byref(keys), abi.I32, 0, d_out_off, d_out_data, ns * 13,
+                                 C.byref(total), C.byref(on)))
+    lens = np.diff(ctx.d2h(d_out_off, 4 * (ns + 1), np.int32))
+    U = abi.BytesArray()
+    U.offsets, U.data = d_out_off, d_out_data
+    U.nulls = b.arr(None, on.validity, ns, on.null_count)
+    base = 4 * (ns + 1) + ns / 8 + ns / 8
+    V, ovw = dict_view_column(b, ctx, keys, offs, data, D, ns)
+    vbytes = 16 * ns + ns / 8 + ns / 8
+    ov = b.out(abi.bitmap_bytes(ns), ns)
+    keep = []
+
+    def scalars(pat):
+        """A one-row Utf8 scalar and view scalar holding `pat` (<= 12 bytes)."""
+        raw = pat.encode()
+        so, sd, sv = ctx.malloc(64), ctx.malloc(64), ctx.malloc(64)
+        ctx.h2d(so, np.array([0, len(raw)], np.int32))
+        ctx.h2d(sd, np.frombuffer(raw + b"\0" * 8, np.uint8))
+        v = np.zeros(16, np.uint8)
+        v[:4] = np.frombuffer(np.uint32(len(raw)).tobytes(), np.uint8)
+        v[4:4 + len(raw)] = np.frombuffer(raw, np.uint8)
+        ctx.h2d(sv, v)
+        keep.extend([so, sd, sv])
+        S = abi.BytesArray()
+        S.offsets, S.data, S.nulls = so, sd, b.arr(None, None, 1, 0, scalar=1)
+        SV = abi.ViewArray()
+        SV.views, SV.buffers, SV.n_buffers, SV.nulls = sv, (C.c_void_p * 1)(), 0, b.arr(None, None, 1, 0, scalar=1)
+        return S, SV
+
+    rows = [("like 'abc'", abi.LIKE, "abc", int((lens == 3).sum()) * 3),
+            ("starts_with 'ab'", abi.STARTS_WITH, "ab", int((lens >= 2).sum()) * 2),
+            ("ends_with 'ab'", abi.ENDS_WITH, "ab", int((lens >= 2).sum()) * 2),
+            ("contains 'abc'", abi.CONTAINS, "abc", total.value),
+            ("like '%a_c%'", abi.LIKE, "%a_c%", total.value),
+            ("ilike '%abc%'", abi.ILIKE, "%abc%", total.value)]
+    note = f"D={D}, lengths 4..12, 5% nulls; {total.value} value bytes"
+    for name, op, pat, value_bytes in rows:
+        S, SV = scalars(pat)
+        b.timed(f"like: {name} utf8 dict-decoded", [abi.K_CMP], base + value_bytes, ns,
+                lambda op=op, S=S: ctx.check(lib.acu_like_bytes(h, 4, 1, op, C.byref(U), C.byref(S), C.byref(ov))), note=note)
+        b.timed(f"like: {name} view inline dict-decoded", [abi.K_CMP], vbytes, ns,
+                lambda op=op, SV=SV: ctx.check(lib.acu_like_byte_view(h, 1, op, C.byref(V), C.byref(SV), C.byref(ov))), note="views only (all values inline)")
+    S, SV = scalars("abc")
+    b.timed("like bar: cmp_bytes eq 'abc' utf8 dict-decoded", [abi.K_CMP], base + int((lens == 3).sum()) * 3, ns,
+            lambda: ctx.check(lib.acu_cmp_bytes(h, 4, abi.EQ, C.byref(U), C.byref(S), C.byref(ov))), note=note)
+    b.timed("like bar: cmp_byte_view eq 'abc' view inline dict-decoded", [abi.K_CMP], 8 * ns + ns / 8 + ns / 8, ns,
+            lambda: ctx.check(lib.acu_cmp_byte_view(h, abi.EQ, C.byref(V), C.byref(SV), C.byref(ov))),
+            note="eq_inline_scalar: reads the low 8 bytes of each view")
+    for p in keep:
+        ctx.free(p)
+    ctx._free_out(ov)
+    ctx._free_out(ovw)
 
 
 if __name__ == "__main__":
