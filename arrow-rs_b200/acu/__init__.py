@@ -145,6 +145,105 @@ class HostArray:
         return 1 if self.dtype == BOOL else abi.DTYPE_SIZE[self.dtype]
 
 
+DECIMAL_MAX_PRECISION = {4: 9, 8: 18, 16: 38}  # = MAX_SCALE
+_DECIMAL_NATIVE = {4: abi.I32, 8: abi.I64, 16: abi.I128}
+CMP_OP_TEXT = ["==", "!=", "<", "<=", ">", ">=", "IS DISTINCT FROM", "IS NOT DISTINCT FROM"]  # arrow-ord/src/cmp.rs:51-63
+
+
+def i128_to_halves(ints):
+    """Python ints (two's complement in 128 bits) -> an (n, 2) uint64 array of (low, high) halves."""
+    out = np.zeros((len(ints), 2), dtype=np.uint64)
+    for i, v in enumerate(ints):
+        v &= (1 << 128) - 1
+        out[i, 0], out[i, 1] = v & 0xFFFFFFFFFFFFFFFF, v >> 64
+    return out
+
+
+def halves_to_i128(halves):
+    """(n, 2) uint64 (low, high) -> list of Python ints."""
+    lo, hi = halves[:, 0].tolist(), halves[:, 1].view(np.int64).tolist()
+    return [(h << 64) | l for l, h in zip(lo, hi)]
+
+
+class DecimalArray(HostArray):
+    """Decimal32 / Decimal64 / Decimal128(precision, scale) in host memory (PrimitiveArray<Decimal*Type>): `values` is an
+    int32 / int64 array, or for Decimal128 an (n, 2) uint64 array of (low, high) halves; validity, bit offset, null_count and
+    scalar-ness as HostArray. `dtype` is the native the C ABI sees (ACU_I32 / ACU_I64 / ACU_I128)."""
+
+    def __init__(self, byte_width, precision, scale, values, length, validity=None, validity_offset=0, null_count=0,
+                 is_scalar=False):
+        super().__init__(_DECIMAL_NATIVE[byte_width], values, length, validity, validity_offset, 0, null_count, is_scalar)
+        self.byte_width, self.precision, self.scale = byte_width, precision, scale
+
+    @staticmethod
+    def from_ints(byte_width, precision, scale, items, force_validity=False, bit_offset=0, scalar=False):
+        """items: Python ints / None (None = null, value 0 under it)."""
+        ints = [0 if x is None else int(x) for x in items]
+        if byte_width == 16:
+            vals = i128_to_halves(ints)
+        else:
+            bits = 8 * byte_width
+            vals = np.array([((v + (1 << (bits - 1))) % (1 << bits)) - (1 << (bits - 1)) for v in ints],
+                            dtype=np.int32 if byte_width == 4 else np.int64)
+        mask = np.array([x is not None for x in items], dtype=bool)
+        validity, nc = None, 0
+        if force_validity or not mask.all():
+            validity, nc = pack_bits(mask, bit_offset), int(len(items) - mask.sum())
+        return DecimalArray(byte_width, precision, scale, vals, len(items), validity, bit_offset if validity is not None else 0,
+                            nc, scalar)
+
+    @staticmethod
+    def from_int64(byte_width, precision, scale, ints, mask=None, bit_offset=0):
+        """Vectorised constructor from an int64 numpy array (sign-extended for Decimal128)."""
+        ints = np.asarray(ints, dtype=np.int64)
+        if byte_width == 16:
+            vals = np.empty((len(ints), 2), dtype=np.uint64)
+            vals[:, 0] = ints.view(np.uint64)
+            vals[:, 1] = (ints >> 63).view(np.uint64)
+        else:
+            vals = ints.astype(np.int32 if byte_width == 4 else np.int64)
+        validity, nc = None, 0
+        if mask is not None:
+            mask = np.asarray(mask, dtype=bool)
+            validity, nc = pack_bits(mask, bit_offset), int(len(mask) - mask.sum())
+        return DecimalArray(byte_width, precision, scale, vals, len(ints), validity, bit_offset if validity is not None else 0, nc)
+
+    def data_type(self):
+        """Display of DataType::Decimal*(p, s)."""
+        return f"Decimal{8 * self.byte_width}({self.precision}, {self.scale})"
+
+    def like(self, h, precision=None, scale=None):
+        """The HostArray `h` (a result with this array's native) as a DecimalArray of this / the given type."""
+        return DecimalArray(self.byte_width, self.precision if precision is None else precision, self.scale if scale is None else scale,
+                            h.values, h.length, h.validity, h.validity_offset, h.null_count, h.is_scalar)
+
+    def width(self):
+        return self.byte_width
+
+    def raw_ints(self):
+        """Python ints of every slot, nulls included."""
+        if self.byte_width == 16:
+            return halves_to_i128(np.asarray(self.values[: self.length]).reshape(-1, 2))
+        return [int(v) for v in np.asarray(self.values[: self.length])]
+
+    def value_array(self):
+        return self.raw_ints()
+
+    def to_list(self):
+        return [v if m else None for v, m in zip(self.raw_ints(), self.valid_mask())]
+
+    def scalar(self):
+        assert self.length == 1
+        d = self.like(self)
+        d.is_scalar = True
+        return d
+
+    def slice(self, offset, length):
+        nc = -1 if self.validity is not None else 0
+        return DecimalArray(self.byte_width, self.precision, self.scale, self.values[offset:], length, self.validity,
+                            self.validity_offset + offset if self.validity is not None else 0, nc, False)
+
+
 def _np_ptr(a):
     return a.ctypes.data if a is not None else None
 
@@ -398,6 +497,8 @@ class Context:
         n = out.len
         if dtype == BOOL:
             vals = self.d2h(out.values, bitmap_bytes(n))
+        elif dtype == abi.I128:
+            vals = self.d2h(out.values, n * 16, np.uint64).reshape(-1, 2)
         else:
             vals = self.d2h(out.values, n * abi.DTYPE_SIZE[dtype], NP_DTYPES[dtype])
         validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
@@ -427,7 +528,7 @@ class Context:
             else:
                 self.check(self.lib.acu_filter_primitive(self.h, plan, values.width(), C.byref(vd), C.byref(out)))
             res, out = self.download_out(out, values.dtype), None
-            return res
+            return values.like(res) if isinstance(values, DecimalArray) else res
         finally:
             if out is not None:
                 self._free_out(out)
@@ -562,7 +663,7 @@ class Context:
                 self.check(self.lib.acu_take_primitive(self.h, values.width(), C.byref(vd), C.byref(idd), indices.dtype,
                                                        int(check_bounds), C.byref(out)))
             res, out = self.download_out(out, values.dtype), None
-            return res
+            return values.like(res) if isinstance(values, DecimalArray) else res
         finally:
             if out is not None:
                 self._free_out(out)
@@ -893,8 +994,53 @@ class Context:
 
     def neg_wrapping(self, a): return self.neg(a, checked=False)
 
+    # -- decimal arithmetic (decimal_op, arrow-arith/src/numeric.rs:970-1107) -----------------------------
+    def decimal_arith(self, op, a, b):
+        """add / sub / mul / div / rem (acu_arith_op) of two DecimalArrays (either may be a scalar): a DecimalArray of the
+        reference's result type; raises ArrowError with the reference's text."""
+        n = b.length if a.is_scalar and not b.is_scalar else a.length
+        da, db = self.upload(a), self.upload(b)
+        out = self.alloc_out(n * a.byte_width, n)
+        try:
+            lt, rt, ot = (abi.DecimalType(x.byte_width, x.precision, x.scale) for x in (a, b, a))
+            ad, bd = da.descriptor(), db.descriptor()
+            self.check(self.lib.acu_decimal_arith(self.h, op, C.byref(lt), C.byref(ad), C.byref(rt), C.byref(bd), C.byref(ot),
+                                                  C.byref(out)))
+            res, out = self.download_out(out, a.dtype), None
+            return a.like(res, ot.precision, ot.scale)
+        finally:
+            if out is not None:
+                self._free_out(out)
+            da.free()
+            db.free()
+
+    def decimal_add(self, a, b): return self.decimal_arith(ADD, a, b)
+    def decimal_sub(self, a, b): return self.decimal_arith(SUB, a, b)
+    def decimal_mul(self, a, b): return self.decimal_arith(MUL, a, b)
+    def decimal_div(self, a, b): return self.decimal_arith(DIV, a, b)
+    def decimal_rem(self, a, b): return self.decimal_arith(REM, a, b)
+
+    def decimal_neg(self, a):
+        """neg / neg_wrapping of a DecimalArray: neg_checked at every width (numeric.rs:116-136, :181-186)."""
+        return a.like(self.neg(a, checked=True))
+
+    @staticmethod
+    def check_decimal_cmp(op, a, b):
+        """compare_op's type check (arrow-ord/src/cmp.rs:228-263): after the length check, decimal operands must have equal
+        DataTypes, precision included. The C ABI carries natives only, so the check lives here."""
+        if not (isinstance(a, DecimalArray) and isinstance(b, DecimalArray)):
+            return
+        if a.data_type() == b.data_type():
+            return
+        if not a.is_scalar and not b.is_scalar and a.length != b.length:
+            raise ArrowError(abi.ERR_INVALID_ARGUMENT,
+                             f"Invalid argument error: Cannot compare arrays of different lengths, got {a.length} vs {b.length}")
+        raise ArrowError(abi.ERR_INVALID_ARGUMENT,
+                         f"Invalid argument error: Invalid comparison operation: {a.data_type()} {CMP_OP_TEXT[op]} {b.data_type()}")
+
     # -- cmp (arrow-ord/src/cmp.rs) -----------------------------------------------------------
     def cmp(self, op, a, b):
+        self.check_decimal_cmp(op, a, b)
         assert a.dtype == b.dtype
         n = b.length if a.is_scalar else a.length
         da, db = self.upload(a), self.upload(b)
@@ -1027,6 +1173,7 @@ class Context:
     # -- fused compare -> filter (cmp.rs:220-382 feeding filter.rs:254-273) -------------------
     def filter_cmp(self, values, op, a, b):
         """filter(values, &cmp::op(a, b)?) with the predicate never materialised: the comparison writes the filter plan."""
+        self.check_decimal_cmp(op, a, b)
         assert a.dtype == b.dtype
         dv, da, db = self.upload(values), self.upload(a), self.upload(b)
         plan = C.c_void_p()
@@ -1043,7 +1190,7 @@ class Context:
                 self.check(self.lib.acu_filter_primitive(self.h, plan, values.width(), C.byref(vd), C.byref(out)))
             strategy = self.lib.acu_filter_plan_strategy(plan)
             res, out = self.download_out(out, values.dtype), None
-            return res, (count, strategy)
+            return (values.like(res) if isinstance(values, DecimalArray) else res), (count, strategy)
         finally:
             if out is not None:
                 self._free_out(out)
@@ -1145,6 +1292,8 @@ class Context:
 
     # -- aggregate (arrow-arith/src/aggregate.rs) ----------------------------------------------
     def aggregate(self, op, a):
+        if a.dtype == abi.I128:
+            return self.aggregate_i128(op, a)
         da = self.upload(a)
         try:
             bits, cnt = C.c_uint64(0), C.c_int64(0)
@@ -1154,6 +1303,19 @@ class Context:
                 return None
             return np.array([bits.value], dtype=np.uint64).view(NP_DTYPES[a.dtype])[0].item() if abi.DTYPE_SIZE[a.dtype] == 8 \
                 else np.array([bits.value], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[a.dtype]].view(NP_DTYPES[a.dtype])[0].item()
+        finally:
+            da.free()
+
+    def aggregate_i128(self, op, a):
+        """sum (wrapping) / min / max of a Decimal128 column as a Python int, None without valid rows."""
+        da = self.upload(a)
+        try:
+            bits, cnt = (C.c_uint64 * 2)(), C.c_int64(0)
+            ad = da.descriptor()
+            self.check(self.lib.acu_aggregate_i128(self.h, op, C.byref(ad), bits, C.byref(cnt)))
+            if cnt.value == 0:
+                return None
+            return halves_to_i128(np.array([[bits[0], bits[1]]], dtype=np.uint64))[0]
         finally:
             da.free()
 

@@ -27,6 +27,9 @@ ERR_OUT_OF_MEMORY = 102
 I8, I16, I32, I64, U8, U16, U32, U64, F32, F64 = range(10)
 DTYPE_NAMES = ["int8", "int16", "int32", "int64", "uint8", "uint16", "uint32", "uint64", "float32", "float64"]
 DTYPE_SIZE = [1, 2, 4, 8, 1, 2, 4, 8, 4, 8]
+# Decimal128's native (16-byte two's complement); accepted only by acu_cmp / acu_filter_plan_create_cmp / acu_neg, so it
+# stays out of the per-dtype lists above
+I128 = 10
 
 # acu_arith_op (arrow-arith/src/numeric.rs:181-190)
 ADD_WRAPPING, ADD, SUB_WRAPPING, SUB, MUL_WRAPPING, MUL, DIV, REM = range(8)
@@ -79,6 +82,11 @@ class ArrayOut(C.Structure):
         ("has_validity", C.c_int32),
         ("reserved", C.c_int32),
     ]
+
+
+class DecimalType(C.Structure):
+    """acu_decimal_type: DataType::Decimal32 / 64 / 128(precision, scale) as byte_width 4 / 8 / 16."""
+    _fields_ = [("byte_width", C.c_int32), ("precision", C.c_uint8), ("scale", C.c_int8), ("reserved", C.c_uint8 * 2)]
 
 
 class BytesArray(C.Structure):
@@ -201,6 +209,7 @@ PROTOTYPES = {
     "acu_take_bytes": (i32, [vp, i32, vp, vp, P(Array), P(Array), i32, i32, vp, vp, i64, P(i64), P(ArrayOut)]),
     "acu_arith": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_neg": (i32, [vp, i32, i32, P(Array), P(ArrayOut)]),
+    "acu_decimal_arith": (i32, [vp, i32, P(DecimalType), P(Array), P(DecimalType), P(Array), P(DecimalType), P(ArrayOut)]),
     "acu_cmp": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_cmp_bytes": (i32, [vp, i32, i32, P(BytesArray), P(BytesArray), P(ArrayOut)]),
     "acu_cmp_byte_view": (i32, [vp, i32, P(ViewArray), P(ViewArray), P(ArrayOut)]),
@@ -209,6 +218,7 @@ PROTOTYPES = {
     "acu_cast_numeric": (i32, [vp, i32, i32, i32, P(Array), P(ArrayOut)]),
     "acu_boolean": (i32, [vp, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_aggregate": (i32, [vp, i32, i32, P(Array), P(u64), P(i64)]),
+    "acu_aggregate_i128": (i32, [vp, i32, P(Array), P(u64), P(i64)]),
     "acu_sum_checked": (i32, [vp, i32, P(Array), P(u64), P(i64)]),
     "acu_aggregate_bytes": (i32, [vp, i32, i32, P(BytesArray), P(i64), P(i64)]),
     "acu_aggregate_byte_view": (i32, [vp, i32, P(ViewArray), P(i64), P(i64)]),

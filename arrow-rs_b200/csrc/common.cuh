@@ -139,8 +139,8 @@ static inline int acu_dtype_size(acu_dtype t) {
 static inline bool acu_dtype_is_float(acu_dtype t) { return t == ACU_F32 || t == ACU_F64; }
 static inline bool acu_dtype_is_signed(acu_dtype t) { return t <= ACU_I64; }
 static inline const char *acu_dtype_name(acu_dtype t) {
-  static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64"};
-  return n[(int)t];
+  static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64", "Int128"};
+  return (int)t >= 0 && (int)t <= (int)ACU_I128 ? n[(int)t] : "unknown";
 }
 
 // Persistent-style grid: enough CTAs to fill every SM `per_sm` times, never more than the work.
@@ -227,6 +227,18 @@ __device__ __forceinline__ uint64_t ld_stream8(const void *p) {
 }
 __device__ __forceinline__ void st_stream8(void *p, uint64_t v) {
   asm volatile("st.global.cs.u64 [%0], %1;" ::"l"(p), "l"(v) : "memory");
+}
+
+// __ldg of one element of any native width; __int128 (Decimal128, 16-byte aligned) has no __ldg overload.
+template <class T> __device__ __forceinline__ T ldg_elem(const T *p) {
+  if constexpr (sizeof(T) == 16) {
+    const longlong2 v = __ldg(reinterpret_cast<const longlong2 *>(p));
+    T r;
+    memcpy(&r, &v, 16);
+    return r;
+  } else {
+    return __ldg(p);
+  }
 }
 
 template <class T> __device__ __forceinline__ T warp_sum(T v) {

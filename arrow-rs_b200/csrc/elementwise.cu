@@ -14,6 +14,7 @@
 // its super-groups, so each call is one launch.
 #include <stdio.h>
 
+#include <algorithm>
 #include <limits>
 #include <type_traits>
 
@@ -56,7 +57,7 @@ __device__ __forceinline__ uint64_t ones_to(int64_t row, int64_t n) {  // bits [
 // ---------------------------------------------------------------------------------------
 // Per-element arithmetic (ArrowNativeTypeOp, arithmetic.rs:148-437)
 // ---------------------------------------------------------------------------------------
-enum { CLS_WRAP = 0, CLS_CHECKED = 1, CLS_DIVREM = 2 };
+enum { CLS_WRAP = 0, CLS_CHECKED = 1, CLS_DIVREM = 2, CLS_DECIMAL = 3 };
 enum { OP_ADD = 0, OP_SUB = 1, OP_MUL = 2, OP_DIV = 3, OP_REM = 4, OP_NEG = 5 };
 
 template <class T> struct is_fp { static constexpr bool value = std::is_floating_point<T>::value; };
@@ -141,6 +142,113 @@ __device__ __forceinline__ bool apply_op(int op, T l, T r, T &o) {
 }
 
 // ---------------------------------------------------------------------------------------
+// Decimal rows (decimal_op, numeric.rs:970-1107) on the natives int32_t / int64_t / __int128. Every step is checked
+// (arithmetic.rs:148-300). Under strict C++17 std::is_signed / make_unsigned do not cover __int128, hence own traits.
+// Host and device share these functions: the error finaliser replays the failing row with them.
+// ---------------------------------------------------------------------------------------
+template <class T> struct dec_unsigned;
+template <> struct dec_unsigned<int32_t> { using type = uint32_t; };
+template <> struct dec_unsigned<int64_t> { using type = uint64_t; };
+template <> struct dec_unsigned<__int128> { using type = unsigned __int128; };
+template <class T> __host__ __device__ __forceinline__ T dec_min() {
+  return (T)((typename dec_unsigned<T>::type)1 << (8 * sizeof(T) - 1));
+}
+
+__host__ __device__ __forceinline__ uint64_t umul64hi(uint64_t a, uint64_t b) {
+#ifdef __CUDA_ARCH__
+  return __umul64hi(a, b);
+#else
+  return (uint64_t)(((unsigned __int128)a * b) >> 64);
+#endif
+}
+__host__ __device__ __forceinline__ int64_t mul64hi(int64_t a, int64_t b) {
+#ifdef __CUDA_ARCH__
+  return __mul64hi(a, b);
+#else
+  return (int64_t)(((__int128)a * b) >> 64);
+#endif
+}
+
+// each returns true when the checked op overflows
+template <class T> __host__ __device__ __forceinline__ bool add_ovf(T a, T b, T &o) {
+  using U = typename dec_unsigned<T>::type;
+  const T s = (T)((U)a + (U)b);
+  o = s;
+  return ((a ^ s) & (b ^ s)) < 0;
+}
+template <class T> __host__ __device__ __forceinline__ bool sub_ovf(T a, T b, T &o) {
+  using U = typename dec_unsigned<T>::type;
+  const T s = (T)((U)a - (U)b);
+  o = s;
+  return ((a ^ b) & (a ^ s)) < 0;
+}
+__host__ __device__ __forceinline__ bool mul_ovf(int32_t a, int32_t b, int32_t &o) {
+  const int64_t w = (int64_t)a * b;
+  o = (int32_t)w;
+  return w != (int64_t)o;
+}
+__host__ __device__ __forceinline__ bool mul_ovf(int64_t a, int64_t b, int64_t &o) {
+  const int64_t lo = (int64_t)((uint64_t)a * (uint64_t)b);
+  o = lo;
+  return mul64hi(a, b) != (lo >> 63);
+}
+// i128 x i128 with 64-bit limbs. Two operands that fit in i64 cannot overflow (one 64 x 64 -> 128 product);
+// otherwise the magnitudes are multiplied and range-checked for the sign of the result.
+__host__ __device__ __forceinline__ bool mul_ovf(__int128 a, __int128 b, __int128 &o) {
+  const int64_t a64 = (int64_t)a, b64 = (int64_t)b;
+  if ((__int128)a64 == a && (__int128)b64 == b) {
+    const uint64_t lo = (uint64_t)a64 * (uint64_t)b64;
+    o = (__int128)(((unsigned __int128)(uint64_t)mul64hi(a64, b64) << 64) | lo);
+    return false;
+  }
+  using U = unsigned __int128;
+  const bool neg = (a < 0) != (b < 0);
+  const U ua = a < 0 ? (U)0 - (U)a : (U)a, ub = b < 0 ? (U)0 - (U)b : (U)b;
+  const uint64_t ah = (uint64_t)(ua >> 64), al = (uint64_t)ua, bh = (uint64_t)(ub >> 64), bl = (uint64_t)ub;
+  if (ah && bh) return true;
+  const uint64_t x = ah ? ah : bh, y = ah ? bl : al;  // the one cross term that can be non-zero
+  if (umul64hi(x, y)) return true;
+  const uint64_t cross = x * y;
+  const uint64_t hi = umul64hi(al, bl) + cross;
+  if (hi < cross) return true;
+  const U m = ((U)hi << 64) | (U)(al * bl);
+  if (m > ((U)1 << 127) - (neg ? 0 : 1)) return true;
+  o = neg ? (__int128)((U)0 - m) : (__int128)m;
+  return false;
+}
+// div_checked / mod_checked: zero divisor, MIN / -1 and MIN % -1 fail; div truncates toward zero
+template <class T> __host__ __device__ __forceinline__ bool divrem_ovf(bool is_div, T l, T r, T &o) {
+  o = T();
+  if (r == T()) return true;
+  if (r == (T)-1) {
+    if (l == dec_min<T>()) return true;
+    if (is_div) o = (T)(T() - l);
+    return false;
+  }
+  if constexpr (sizeof(T) == 16) {  // 64-bit division when both operands allow it; __int128 `/` is a software routine
+    const int64_t l64 = (int64_t)l, r64 = (int64_t)r;
+    if ((__int128)l64 == l && (__int128)r64 == r) {
+      o = is_div ? l64 / r64 : l64 % r64;
+      return false;
+    }
+  }
+  o = is_div ? (T)(l / r) : (T)(l % r);
+  return false;
+}
+// One row: add / sub / div / rem = l.mul_checked(l_mul)?.op(r.mul_checked(r_mul)?) (a multiplier of 1 is skipped: it
+// cannot fail), mul = l.mul_checked(r), neg = r.neg_checked().
+template <class T> __host__ __device__ __forceinline__ bool dec_apply(int op, T l, T r, T l_mul, T r_mul, T &o) {
+  o = T();
+  if (op == OP_NEG) return sub_ovf<T>(T(), r, o);
+  if (op == OP_MUL) return mul_ovf(l, r, o);
+  if (l_mul != (T)1 && mul_ovf(l, l_mul, l)) return true;
+  if (r_mul != (T)1 && mul_ovf(r, r_mul, r)) return true;
+  if (op == OP_ADD) return add_ovf<T>(l, r, o);
+  if (op == OP_SUB) return sub_ovf<T>(l, r, o);
+  return divrem_ovf<T>(op == OP_DIV, l, r, o);
+}
+
+// ---------------------------------------------------------------------------------------
 // Binary / unary arithmetic kernel
 // ---------------------------------------------------------------------------------------
 template <class T>
@@ -155,17 +263,28 @@ struct ArithParams {
   int op;
   int a_scalar, b_scalar;
   int zero_nulls;          // try_binary / try_unary: zero under nulls, op only at valid slots
+  T l_mul, r_mul;          // CLS_DECIMAL: rescale multipliers of add / sub / div / rem
 };
+
+template <class T, int CLS>
+__device__ __forceinline__ bool row_op(const ArithParams<T> &p, T l, T r, T &o) {
+  if constexpr (CLS == CLS_DECIMAL) return dec_apply<T>(p.op, l, r, p.l_mul, p.r_mul, o);
+  else return apply_op<T, CLS>(p.op, l, r, o);
+}
 
 // Steady state: a warp owns "super-groups" of 2048 rows = 32 validity words (lane l <-> word
 // l: ONE coalesced 256-B bitmap access per operand per super-group), processed as groups of
 // U strips whose loads are all issued before any use. The ragged remainder (< 2048 rows) is
 // finished element-wise by warp 0 so that bounds-checked code stays out of the streaming loop.
+// Decimal128 rows are 16 B per operand: U = 4 strips keep 128 B per operand and lane in flight, two CTAs per SM give
+// the checked i128 steps their registers.
 template <class T, int CLS, int EPL>
-__global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : 3)) k_arith(const ArithParams<T> p) {
+__global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : (CLS == CLS_DECIMAL && sizeof(T) == 16) ? 2 : 3))
+    k_arith(const ArithParams<T> p) {
+  constexpr bool WIDE = CLS == CLS_DECIMAL && sizeof(T) == 16;
   constexpr int R = (32 * EPL > 64) ? 32 * EPL : 64;  // rows per strip
   constexpr int LPS = R / (32 * EPL);                 // loads per lane per strip
-  constexpr int U = (LPS >= 2) ? 2 : 4;               // strips in flight per warp
+  constexpr int U = (LPS >= 2 && !WIDE) ? 2 : 4;      // strips in flight per warp
   constexpr int GROUP = U * R;                        // rows per group
   constexpr int SG = 2048;                            // rows per super-group
   constexpr int GPS = SG / GROUP;                     // groups per super-group
@@ -177,8 +296,8 @@ __global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : 3)) k_arith(const 
   const int64_t sgroups = n / SG;
   const bool has_valid = p.out_valid != nullptr;
   T sa = T(), sb = T();
-  if (p.a_scalar) sa = __ldg(p.a);
-  if (p.b_scalar) sb = __ldg(p.b);
+  if (p.a_scalar) sa = ldg_elem(p.a);
+  if (p.b_scalar) sb = ldg_elem(p.b);
   unsigned valid_cnt = 0;
   unsigned long long err = ~0ull;
 
@@ -220,7 +339,7 @@ __global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : 3)) k_arith(const 
           const T l = p.a_scalar ? sa : va[k].v[e];
           const T r = p.b_scalar ? sb : vb[k].v[e];
           T x;
-          const bool bad = apply_op<T, CLS>(p.op, l, r, x);
+          const bool bad = row_op<T, CLS>(p, l, r, x);
           if (fallible) {
             if (!((bits >> e) & 1u)) x = T();
             else if (bad) {
@@ -248,10 +367,10 @@ __global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : 3)) k_arith(const 
       for (int h = 0; h < 2; ++h) {
         const int64_t i = row + h * 32 + lane;
         if (i >= n) continue;
-        const T l = p.a_scalar ? sa : __ldg(p.a + i);
-        const T r = p.b_scalar ? sb : __ldg(p.b + i);
+        const T l = p.a_scalar ? sa : ldg_elem(p.a + i);
+        const T r = p.b_scalar ? sb : ldg_elem(p.b + i);
         T x;
-        const bool bad = apply_op<T, CLS>(p.op, l, r, x);
+        const bool bad = row_op<T, CLS>(p, l, r, x);
         if (fallible) {
           const bool live = !p.zero_nulls || ((vw >> (h * 32 + lane)) & 1ull);
           if (!live) x = T();
@@ -293,34 +412,93 @@ const char *op_symbol(acu_arith_op op) {  // numeric.rs:192-202
   }
 }
 
+// Rust {:?} of i128: snprintf has no 128-bit conversion
+void fmt_i128(char *buf, size_t n, __int128 v) {
+  char tmp[48];
+  int k = 0;
+  unsigned __int128 m = v < 0 ? (unsigned __int128)0 - (unsigned __int128)v : (unsigned __int128)v;
+  do { tmp[k++] = (char)('0' + (int)(m % 10)); m /= 10; } while (m);
+  size_t j = 0;
+  if (v < 0 && j + 1 < n) buf[j++] = '-';
+  while (k && j + 1 < n) buf[j++] = tmp[--k];
+  buf[j] = 0;
+}
 template <class T> void fmt_native(char *buf, size_t n, T v) {  // Rust {:?} of integers
-  if constexpr (std::is_floating_point<T>::value) snprintf(buf, n, "%.17g", (double)v);
+  if constexpr (sizeof(T) == 16) fmt_i128(buf, n, v);
+  else if constexpr (std::is_floating_point<T>::value) snprintf(buf, n, "%.17g", (double)v);
   else if constexpr (std::is_signed<T>::value) snprintf(buf, n, "%lld", (long long)v);
   else snprintf(buf, n, "%llu", (unsigned long long)v);
 }
-template <class T> uint64_t bits_of(T v) { uint64_t b = 0; memcpy(&b, &v, sizeof(T)); return b; }
+// bit pattern for acu_error_detail (the low 64 bits of an i128)
+template <class T> uint64_t bits_of(T v) { uint64_t b = 0; memcpy(&b, &v, sizeof(T) < 8 ? sizeof(T) : 8); return b; }
 
-// Fetch the operands at the lowest failing row and rebuild the reference's error.
+// The rescale multipliers and result type of one decimal_op call (numeric.rs:991-1104).
+template <class T> struct DecArgs {
+  T l_mul, r_mul;
+  int max_precision, max_scale;
+  uint8_t precision;
+  int8_t scale;
+};
+
+// with_precision_and_scale / validate_decimal_precision_and_scale (arrow-array/src/types.rs:1442-1472)
+acu_status decimal_validate(acu_ctx *ctx, int max_precision, int max_scale, int precision, int scale) {
+  if (precision == 0)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "precision cannot be 0, has to be between [1, %d]", max_precision);
+  if (precision > max_precision)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "precision %d is greater than max %d", precision, max_precision);
+  if (scale > max_scale)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "scale %d is greater than max %d", scale, max_scale);
+  if (scale > 0 && scale > precision)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "scale %d is greater than precision %d", scale, precision);
+  return ACU_OK;
+}
+
+// Fetch the operands at the lowest failing row and rebuild the reference's error. Decimal rows are replayed step by
+// step with the device's own checked ops, so the message names the step that failed and its (rescaled) operands.
 template <class T>
-acu_status arith_error(acu_ctx *ctx, acu_arith_op op, bool is_neg, const acu_array *a, const acu_array *b, int64_t idx) {
+acu_status arith_error(acu_ctx *ctx, acu_arith_op op, bool is_neg, const acu_array *a, const acu_array *b, int64_t idx,
+                       const DecArgs<T> *dec = nullptr) {
   T l = T(), r = T();
   if (a) ACU_CUDA(ctx, cudaMemcpyAsync(&l, static_cast<const T *>(a->values) + (a->is_scalar ? 0 : idx), sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
   ACU_CUDA(ctx, cudaMemcpyAsync(&r, static_cast<const T *>(b->values) + (b->is_scalar ? 0 : idx), sizeof(T), cudaMemcpyDeviceToHost, ctx->stream));
   ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  char ls[40], rs[40];
-  fmt_native(ls, sizeof ls, l);
-  fmt_native(rs, sizeof rs, r);
+  const uint64_t lb = bits_of(l), rb = bits_of(r);
+  T x = l, y = r;  // the operands of the failing step
+  const char *sym = op_symbol(op);
+  bool rescale_failed = false;
+  if constexpr (std::is_same<T, int32_t>::value || std::is_same<T, int64_t>::value || sizeof(T) == 16) {
+    if (dec && !is_neg && op != ACU_MUL && op != ACU_MUL_WRAPPING) {
+      T t;
+      if (dec->l_mul != (T)1 && mul_ovf(l, dec->l_mul, t)) {
+        y = dec->l_mul, rescale_failed = true;
+      } else {
+        if (dec->l_mul != (T)1) x = t;
+        if (dec->r_mul != (T)1 && mul_ovf(r, dec->r_mul, t)) x = r, y = dec->r_mul, rescale_failed = true;
+        else if (dec->r_mul != (T)1) y = t;
+      }
+      if (rescale_failed) sym = "*";
+    }
+  }
+  if ((op == ACU_DIV || op == ACU_REM) && !is_neg && !rescale_failed && y == T())
+    return acu_fail(ctx, ACU_ERR_DIVIDE_BY_ZERO, idx, lb, rb, 0, "Divide by zero error");
+  char ls[48], rs[48];
+  fmt_native(ls, sizeof ls, x);
+  fmt_native(rs, sizeof rs, y);
   if (is_neg)
-    return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, bits_of(r), 0, 0, "Overflow happened on: - %s", rs);
-  if ((op == ACU_DIV || op == ACU_REM) && r == T())
-    return acu_fail(ctx, ACU_ERR_DIVIDE_BY_ZERO, idx, bits_of(l), bits_of(r), 0, "Divide by zero error");
-  return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, bits_of(l), bits_of(r), 0,
-                  "Overflow happened on: %s %s %s", ls, op_symbol(op), rs);
+    return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, rb, 0, 0, "Overflow happened on: - %s", rs);
+  return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, lb, rb, 0, "Overflow happened on: %s %s %s", ls, sym, rs);
 }
 
-template <class T>
-acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const acu_array *b, acu_array_out *out) {
-  const bool checked = !is_fp<T>::value && (op == ACU_ADD || op == ACU_SUB || op == ACU_MUL || op == ACU_DIV || op == ACU_REM);
+// DEC: decimal_op rows (every op checked, CLS_DECIMAL) with dec's multipliers, then its result-type validation.
+template <class T, bool DEC = false>
+acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const acu_array *b, acu_array_out *out,
+                       const DecArgs<T> *dec = nullptr) {
+  const bool checked = DEC || (!is_fp<T>::value && (op == ACU_ADD || op == ACU_SUB || op == ACU_MUL || op == ACU_DIV || op == ACU_REM));
+  DecArgs<T> dv{};
+  if constexpr (DEC) dv = *dec;
+  auto validate = [ctx, dv]() -> acu_status {
+    return DEC ? decimal_validate(ctx, dv.max_precision, dv.max_scale, dv.precision, dv.scale) : ACU_OK;
+  };
   const bool a_s = a->is_scalar != 0, b_s = b->is_scalar != 0;
   acu_status st;
   ArithParams<T> p{};
@@ -337,6 +515,8 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
     case ACU_DIV: p.op = OP_DIV; break;
     default: p.op = OP_REM; break;
   }
+  p.l_mul = DEC ? dv.l_mul : T();
+  p.r_mul = DEC ? dv.r_mul : T();
   out->has_validity = 0;
   out->null_count = 0;
   int64_t len;
@@ -345,9 +525,12 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
     len = arr->len;
     int64_t snc = acu_resolve_null_count(ctx, s, &st);
     ACU_TRY(st);
-    if (snc != 0) return acu_new_null(ctx, len, (size_t)len * sizeof(T), out);
+    if (snc != 0) {
+      ACU_TRY(acu_new_null(ctx, len, (size_t)len * sizeof(T), out));
+      return validate();
+    }
     out->len = len;
-    if (len == 0) { out->has_validity = arr->validity != nullptr; return ACU_OK; }
+    if (len == 0) { out->has_validity = arr->validity != nullptr; return validate(); }
     if (arr->validity) {  // nulls().cloned()
       (a_s ? p.bv : p.av) = arr->validity;
       (a_s ? p.boff : p.aoff) = arr->validity_offset;
@@ -361,7 +544,7 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
                               : "Cannot perform binary operation on arrays of different length");
     len = a->len;
     out->len = len;
-    if (len == 0) return ACU_OK;
+    if (len == 0) return validate();
     int64_t an = acu_resolve_null_count(ctx, a, &st);
     ACU_TRY(st);
     int64_t bn = acu_resolve_null_count(ctx, b, &st);
@@ -384,7 +567,9 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
   const int blk = acu_call_begin(ctx, &st);
   ACU_TRY(st);
   p.res = acu_dres(ctx, blk);
-  if (is_fp<T>::value) {
+  if constexpr (DEC) {
+    ACU_TRY((launch_arith<T, CLS_DECIMAL>(ctx, p)));
+  } else if (is_fp<T>::value) {
     if (op == ACU_DIV || op == ACU_REM) ACU_TRY((launch_arith<T, CLS_DIVREM>(ctx, p)));
     else ACU_TRY((launch_arith<T, CLS_WRAP>(ctx, p)));
   } else if (op == ACU_DIV || op == ACU_REM) {
@@ -396,19 +581,21 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
   }
   const acu_array ca = *a, cb = *b;  // the finaliser may run later (acu_results_fetch)
   const bool has_valid = p.out_valid != nullptr;
-  return acu_call_end(ctx, blk, [ctx, op, checked, ca, cb, has_valid, len, out](const unsigned long long *h) -> acu_status {
-    if (checked && h[RES_ERR_INDEX] != ~0ull) return arith_error<T>(ctx, op, false, &ca, &cb, (int64_t)h[RES_ERR_INDEX]);
+  return acu_call_end(ctx, blk, [ctx, op, checked, ca, cb, has_valid, len, out, dv, validate](const unsigned long long *h) -> acu_status {
+    if (checked && h[RES_ERR_INDEX] != ~0ull) return arith_error<T>(ctx, op, false, &ca, &cb, (int64_t)h[RES_ERR_INDEX], DEC ? &dv : nullptr);
     if (has_valid) {
       out->has_validity = 1;
       out->null_count = len - (int64_t)h[RES_COUNT];
     }
-    return ACU_OK;
+    return validate();
   });
 }
 
+// Decimal128 (T = __int128) is always neg_checked, on the decimal class, and stream-ordered inside sections.
 template <class T>
 acu_status neg_typed(acu_ctx *ctx, int32_t checked_in, const acu_array *a, acu_array_out *out) {
-  const bool checked = checked_in && !is_fp<T>::value;
+  constexpr bool DEC = sizeof(T) == 16;
+  const bool checked = DEC || (checked_in && !is_fp<T>::value);
   int64_t len = a->len;
   out->len = len;
   out->has_validity = a->validity != nullptr;
@@ -428,14 +615,30 @@ acu_status neg_typed(acu_ctx *ctx, int32_t checked_in, const acu_array *a, acu_a
     p.out_valid = reinterpret_cast<uint64_t *>(out->validity);
     p.zero_nulls = checked;
   }
-  ACU_TRY(acu_res_reset(ctx));
-  if (checked) ACU_TRY((launch_arith<T, CLS_CHECKED>(ctx, p)));
-  else ACU_TRY((launch_arith<T, CLS_WRAP>(ctx, p)));
-  ACU_TRY(acu_res_fetch(ctx));
-  if (checked && ctx->h_res[RES_ERR_INDEX] != ~0ull)
-    return arith_error<T>(ctx, ACU_SUB, true, nullptr, a, (int64_t)ctx->h_res[RES_ERR_INDEX]);
-  if (p.out_valid) out->null_count = len - (int64_t)ctx->h_res[RES_COUNT];
-  return ACU_OK;
+  if constexpr (DEC) {
+    acu_status st;
+    const int blk = acu_call_begin(ctx, &st);
+    ACU_TRY(st);
+    p.res = acu_dres(ctx, blk);
+    p.l_mul = p.r_mul = 1;
+    ACU_TRY((launch_arith<T, CLS_DECIMAL>(ctx, p)));
+    const acu_array ca = *a;
+    const bool has_valid = p.out_valid != nullptr;
+    return acu_call_end(ctx, blk, [ctx, ca, has_valid, len, out](const unsigned long long *h) -> acu_status {
+      if (h[RES_ERR_INDEX] != ~0ull) return arith_error<T>(ctx, ACU_SUB, true, nullptr, &ca, (int64_t)h[RES_ERR_INDEX]);
+      if (has_valid) out->null_count = len - (int64_t)h[RES_COUNT];
+      return ACU_OK;
+    });
+  } else {
+    ACU_TRY(acu_res_reset(ctx));
+    if (checked) ACU_TRY((launch_arith<T, CLS_CHECKED>(ctx, p)));
+    else ACU_TRY((launch_arith<T, CLS_WRAP>(ctx, p)));
+    ACU_TRY(acu_res_fetch(ctx));
+    if (checked && ctx->h_res[RES_ERR_INDEX] != ~0ull)
+      return arith_error<T>(ctx, ACU_SUB, true, nullptr, a, (int64_t)ctx->h_res[RES_ERR_INDEX]);
+    if (p.out_valid) out->null_count = len - (int64_t)ctx->h_res[RES_COUNT];
+    return ACU_OK;
+  }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -501,8 +704,8 @@ __global__ void __launch_bounds__(256, 4) k_cmp(const CmpParams<T> p) {
   const int64_t n = p.n;
   const int64_t sgroups = n >> 11;
   T sa = T(), sb = T();
-  if (p.a_scalar) sa = __ldg(p.a);
-  if (p.b_scalar) sb = __ldg(p.b);
+  if (p.a_scalar) sa = ldg_elem(p.a);
+  if (p.b_scalar) sb = ldg_elem(p.b);
   unsigned valid_cnt = 0;
   for (int64_t sg = warp; sg < sgroups; sg += nwarps) {
     const int64_t sbase = sg << 11;
@@ -559,8 +762,8 @@ __global__ void __launch_bounds__(256, 4) k_cmp(const CmpParams<T> p) {
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         const int64_t i = row + h * 32 + lane;
-        const T l = (!p.a_scalar && i < n) ? __ldg(p.a + i) : sa;
-        const T r = (!p.b_scalar && i < n) ? __ldg(p.b + i) : sb;
+        const T l = (!p.a_scalar && i < n) ? ldg_elem(p.a + i) : sa;
+        const T r = (!p.b_scalar && i < n) ? ldg_elem(p.b + i) : sb;
         v |= (uint64_t)__ballot_sync(ACU_FULL_MASK, LT ? pred_lt(l, r) : pred_eq(l, r)) << (h * 32);
       }
       if (p.neg) v = ~v;
@@ -837,6 +1040,98 @@ acu_status cast_from(acu_ctx *ctx, acu_dtype to, int32_t safe, const acu_array *
   return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast to dtype %d", (int)to);
 }
 
+// ACU_I128 values are read and written as 16-byte vectors: the pointers must have the alignment of i128.
+acu_status i128_aligned(acu_ctx *ctx, const void *x, const void *y) {
+  if (((uintptr_t)x | (uintptr_t)y) % 16 != 0)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Int128 values must be 16-byte aligned");
+  return ACU_OK;
+}
+
+// ---------------------------------------------------------------------------------------
+// decimal_op's result type and multipliers (numeric.rs:991-1104), in Rust's i8 / u8 arithmetic. Where the reference's
+// i8 subtractions overflow (debug builds panic) this wraps, as a release build does.
+// ---------------------------------------------------------------------------------------
+int8_t i8_wrap(int v) { return (int8_t)(uint8_t)(v & 0xff); }
+int8_t i8_sat(int v) { return (int8_t)(v < -128 ? -128 : v > 127 ? 127 : v); }
+uint8_t u8_sat(int v) { return (uint8_t)(v > 255 ? 255 : v); }
+uint8_t u8_of(int8_t v) { return (uint8_t)v; }                  // `as u8`
+uint32_t u32_of(int8_t v) { return (uint32_t)(int32_t)v; }      // `as u32` (sign-extending)
+
+template <class T> bool pow10_checked(uint32_t exp, T *out) {  // 10.checked_pow(exp)
+  T v = 1;
+  for (uint32_t i = 0; i < exp; ++i)
+    if (mul_ovf(v, (T)10, v)) return false;
+  *out = v;
+  return true;
+}
+template <class T> T pow10_wrapping(uint32_t exp) {  // 10.wrapping_pow(exp): 2^exp divides 10^exp, so 0 from exp = bits
+  using U = typename dec_unsigned<T>::type;
+  if (exp >= 8 * sizeof(T)) return T();
+  U v = 1;
+  for (uint32_t i = 0; i < exp; ++i) v *= 10;
+  return (T)v;
+}
+
+const char *decimal_name(int width) { return width == 4 ? "Decimal32" : width == 8 ? "Decimal64" : "Decimal128"; }
+
+template <class T>
+acu_status decimal_typed(acu_ctx *ctx, acu_arith_op op, const acu_decimal_type &lt, const acu_array *a, const acu_decimal_type &rt,
+                         const acu_array *b, acu_decimal_type *out_type, acu_array_out *out) {
+  constexpr int MP = sizeof(T) == 4 ? 9 : sizeof(T) == 8 ? 18 : 38;  // MAX_PRECISION = MAX_SCALE
+  const int p1 = lt.precision, p2 = rt.precision, s1 = lt.scale, s2 = rt.scale;
+  DecArgs<T> d{};
+  d.l_mul = d.r_mul = 1;
+  d.max_precision = d.max_scale = MP;
+  uint32_t le = 0, re = 0;  // exponents of the checked multipliers
+  bool pow_l = false, pow_r = false;
+  switch (op) {
+    case ACU_ADD: case ACU_ADD_WRAPPING: case ACU_SUB: case ACU_SUB_WRAPPING: case ACU_REM: {
+      const int8_t rs = (int8_t)(s1 > s2 ? s1 : s2);
+      const int8_t d1 = i8_wrap(p1 - s1), d2 = i8_wrap(p2 - s2);
+      if (op == ACU_REM) {
+        d.precision = (uint8_t)std::min<int>(u8_of(i8_sat(rs + std::min(d1, d2))), MP);
+        d.l_mul = pow10_wrapping<T>(u32_of(i8_wrap(rs - s1)));
+        d.r_mul = pow10_wrapping<T>(u32_of(i8_wrap(rs - s2)));
+      } else {
+        d.precision = (uint8_t)std::min<int>(u8_sat(u8_of(i8_sat(rs + std::max(d1, d2))) + 1), MP);
+        le = u32_of(i8_wrap(rs - s1));
+        re = u32_of(i8_wrap(rs - s2));
+        pow_l = pow_r = true;
+      }
+      d.scale = rs;
+      break;
+    }
+    case ACU_MUL: case ACU_MUL_WRAPPING: {
+      d.precision = (uint8_t)std::min<int>(u8_sat(p1 + p2 + 1), MP);
+      d.scale = i8_sat(s1 + s2);
+      if (d.scale > MP)
+        return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Output scale of %s(%d, %d) * %s(%d, %d) would exceed max scale of %d",
+                        decimal_name(lt.byte_width), p1, s1, decimal_name(rt.byte_width), p2, s2, MP);
+      break;
+    }
+    case ACU_DIV: {
+      const int8_t rs = (int8_t)std::min<int>(i8_sat(s1 + 4), MP);
+      const int8_t mul_pow = i8_wrap(i8_wrap(rs - s1) + s2);
+      d.precision = (uint8_t)std::min<int>(u8_of(i8_sat(mul_pow + p1)), MP);
+      d.scale = rs;
+      if (mul_pow > 0) { le = u32_of(mul_pow); pow_l = true; }
+      else if (mul_pow < 0) { re = u32_of(i8_wrap(-mul_pow)); pow_r = true; }
+      break;
+    }
+    default:
+      return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: op %d", (int)op);
+  }
+  if (pow_l && !pow10_checked<T>(le, &d.l_mul))
+    return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, -1, 0, 0, 0, "Overflow happened on: 10 ^ %u", le);
+  if (pow_r && !pow10_checked<T>(re, &d.r_mul))
+    return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, -1, 0, 0, 0, "Overflow happened on: 10 ^ %u", re);
+  out_type->byte_width = lt.byte_width;
+  out_type->precision = d.precision;
+  out_type->scale = d.scale;
+  out_type->reserved[0] = out_type->reserved[1] = 0;
+  return arith_typed<T, true>(ctx, op, a, b, out, &d);
+}
+
 }  // namespace
 
 #define ACU_DISPATCH(dt, F, ...)                         \
@@ -865,6 +1160,10 @@ extern "C" acu_status acu_neg(acu_ctx *ctx, acu_dtype dtype, int32_t checked, co
   if (checked && (dtype == ACU_U8 || dtype == ACU_U16 || dtype == ACU_U32 || dtype == ACU_U64))  // numeric.rs:174-176
     return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: !%s", acu_dtype_name(dtype));
   ACU_DISPATCH(dtype, neg_typed, ctx, checked, a, out)
+  if (dtype == ACU_I128) {
+    ACU_TRY(i128_aligned(ctx, a->values, out->values));
+    return neg_typed<__int128>(ctx, 1, a, out);
+  }
   return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: dtype %d", (int)dtype);
 }
 
@@ -872,6 +1171,10 @@ extern "C" acu_status acu_cmp(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, cons
                               const acu_array *b, acu_array_out *out) {
   ACU_ENTER(ctx);
   ACU_DISPATCH(dtype, cmp_typed, ctx, op, a, b, out)
+  if (dtype == ACU_I128) {
+    ACU_TRY(i128_aligned(ctx, a->values, b->values));
+    return cmp_typed<__int128>(ctx, op, a, b, out);
+  }
   return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid comparison operation: dtype %d", (int)dtype);
 }
 
@@ -941,6 +1244,10 @@ acu_status acu_cmp_into_plan(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, const
   const CmpFuse *fuse = &f;
   acu_array_out *out = nullptr;
   ACU_DISPATCH(dtype, cmp_typed, ctx, op, a, b, out, fuse)
+  if (dtype == ACU_I128) {
+    ACU_TRY(i128_aligned(ctx, a->values, b->values));
+    return cmp_typed<__int128>(ctx, op, a, b, out, fuse);
+  }
   return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid comparison operation: dtype %d", (int)dtype);
 }
 
@@ -949,4 +1256,21 @@ extern "C" acu_status acu_cast_numeric(acu_ctx *ctx, acu_dtype from, acu_dtype t
   ACU_ENTER(ctx);
   ACU_DISPATCH(from, cast_from, ctx, to, safe, a, out)
   return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from dtype %d", (int)from);
+}
+
+extern "C" acu_status acu_decimal_arith(acu_ctx *ctx, acu_arith_op op, const acu_decimal_type *lt, const acu_array *a,
+                                        const acu_decimal_type *rt, const acu_array *b, acu_decimal_type *out_type,
+                                        acu_array_out *out) {
+  ACU_ENTER(ctx);
+  const int w = lt->byte_width;
+  if ((w != 4 && w != 8 && w != 16) || rt->byte_width != w)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid decimal operation: byte widths %d and %d", (int)w, (int)rt->byte_width);
+  const int mp = w == 4 ? 9 : w == 8 ? 18 : 38;
+  ACU_TRY(decimal_validate(ctx, mp, mp, lt->precision, lt->scale));
+  ACU_TRY(decimal_validate(ctx, mp, mp, rt->precision, rt->scale));
+  if (w == 4) return decimal_typed<int32_t>(ctx, op, *lt, a, *rt, b, out_type, out);
+  if (w == 8) return decimal_typed<int64_t>(ctx, op, *lt, a, *rt, b, out_type, out);
+  ACU_TRY(i128_aligned(ctx, a->values, b->values));
+  ACU_TRY(i128_aligned(ctx, out->values, nullptr));
+  return decimal_typed<__int128>(ctx, op, *lt, a, *rt, b, out_type, out);
 }

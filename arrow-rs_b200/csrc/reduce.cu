@@ -45,6 +45,7 @@ template <class A, int OP> __device__ __forceinline__ A acc_merge(A a, A b) {
   if constexpr (OP == ACU_SUM) {
     if constexpr (std::is_same<A, double>::value) return __dadd_rn(a, b);
     else if constexpr (std::is_same<A, float>::value) return __fadd_rn(a, b);
+    else if constexpr (sizeof(A) == 16) return (A)((unsigned __int128)a + (unsigned __int128)b);  // i128 add_wrapping
     else return (A)((typename std::make_unsigned<A>::type)a + (typename std::make_unsigned<A>::type)b);  // add_wrapping
   } else if constexpr (OP == ACU_MIN) {
     return b < a ? b : a;
@@ -58,7 +59,14 @@ template <class T, int OP> __device__ __forceinline__ typename AccOf<T, OP>::typ
 }
 
 template <class A> __device__ __forceinline__ A shfl_down_any(A v, int o) {
-  if constexpr (sizeof(A) == 8) {
+  if constexpr (sizeof(A) == 16) {  // Decimal128: two 64-bit halves
+    long long x[2];
+    memcpy(x, &v, 16);
+    x[0] = __shfl_down_sync(ACU_FULL_MASK, x[0], o);
+    x[1] = __shfl_down_sync(ACU_FULL_MASK, x[1], o);
+    memcpy(&v, x, 16);
+    return v;
+  } else if constexpr (sizeof(A) == 8) {
     long long x;
     memcpy(&x, &v, 8);
     x = __shfl_down_sync(ACU_FULL_MASK, x, o);
@@ -121,7 +129,7 @@ __global__ void __launch_bounds__(256) k_reduce(const ReduceBatch batch) {
 #pragma unroll
         for (int h = 0; h < 2; ++h) {
           const int64_t i = sbase + (s0 + u) * 64 + h * 32 + lane;
-          x[u][h] = i < n ? __ldg(v + i) : T();
+          x[u][h] = i < n ? ldg_elem(v + i) : T();
         }
       }
 #pragma unroll
@@ -159,9 +167,10 @@ __global__ void __launch_bounds__(256) k_reduce(const ReduceBatch batch) {
       T r;
       if constexpr (OP == ACU_SUM) r = f;
       else r = from_key<T>(f);
-      unsigned long long bits = 0;
-      memcpy(&bits, &r, sizeof(T));
-      res[RES_AUX0] = bits;
+      unsigned long long bits[2] = {0, 0};  // an i128 result fills RES_AUX0 (low) and RES_AUX1 (high)
+      memcpy(bits, &r, sizeof(T));
+      res[RES_AUX0] = bits[0];
+      if (sizeof(T) == 16) res[RES_AUX1] = bits[1];
       *ticket = 0;
     }
   }
@@ -246,10 +255,9 @@ acu_status acu_reduce_cols_launch(acu_ctx *ctx, int n, const acu_dtype *dtypes, 
   return ACU_OK;
 }
 
-extern "C" acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a,
-                                    uint64_t *out_bits, int64_t *out_valid_count) {
-  ACU_ENTER(ctx);
-  *out_bits = 0;
+// acu_aggregate / acu_aggregate_i128 (wide: out_bits[0..1] of an __int128 result)
+static acu_status aggregate_one(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a, bool wide, uint64_t *out_bits,
+                                int64_t *out_valid_count) {
   *out_valid_count = 0;
   if (a->len == 0) return ACU_OK;  // None
   acu_status st = ACU_OK;
@@ -266,15 +274,41 @@ extern "C" acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op
   const int blk = acu_call_begin(ctx, &st);
   ACU_TRY(st);
   unsigned long long *res = acu_dres(ctx, blk);
-  ACU_TRY(acu_reduce_cols_launch(ctx, 1, &dtype, &op, a, &nc, static_cast<uint8_t *>(scratch), scratch_bytes, &res, &launched));
+  if (!wide) {
+    ACU_TRY(acu_reduce_cols_launch(ctx, 1, &dtype, &op, a, &nc, static_cast<uint8_t *>(scratch), scratch_bytes, &res, &launched));
+  } else if (nc != a->len) {  // Decimal128: the same launch on __int128, kept out of the dtype dispatch of acu_aggregate*
+    ReduceBatch rb{};
+    rb.col[0] = reduce_args(a, nc, scratch, res);
+    ACU_TRY(reduce_typed<__int128>(ctx, op, rb, 1, a->len));
+    launched = 1;
+  }
   if (!launched && !ctx->async_on) return ACU_OK;
-  return acu_call_end(ctx, blk, [launched, deferred_nc, out_bits, out_valid_count](const unsigned long long *h) -> acu_status {
+  return acu_call_end(ctx, blk, [launched, deferred_nc, wide, out_bits, out_valid_count](const unsigned long long *h) -> acu_status {
     if (!launched) return ACU_OK;
     if (deferred_nc) {
       *out_valid_count = (int64_t)h[RES_COUNT];
       if (*out_valid_count == 0) return ACU_OK;  // every row null: None (aggregate.rs:320-323)
     }
-    *out_bits = h[RES_AUX0];
+    out_bits[0] = h[RES_AUX0];
+    if (wide) out_bits[1] = h[RES_AUX1];
     return ACU_OK;
   });
+}
+
+extern "C" acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a,
+                                    uint64_t *out_bits, int64_t *out_valid_count) {
+  ACU_ENTER(ctx);
+  *out_bits = 0;
+  return aggregate_one(ctx, dtype, op, a, false, out_bits, out_valid_count);
+}
+
+extern "C" acu_status acu_aggregate_i128(acu_ctx *ctx, acu_agg_op op, const acu_array *a, uint64_t out_bits[2],
+                                         int64_t *out_valid_count) {
+  ACU_ENTER(ctx);
+  out_bits[0] = out_bits[1] = 0;
+  if (op != ACU_SUM && op != ACU_MIN && op != ACU_MAX)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "aggregate: op %d", (int)op);
+  if (a->len && (uintptr_t)a->values % 16 != 0)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Int128 values must be 16-byte aligned");
+  return aggregate_one(ctx, ACU_I128, op, a, true, out_bits, out_valid_count);
 }

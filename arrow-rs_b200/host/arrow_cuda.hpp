@@ -141,7 +141,7 @@ inline std::vector<uint8_t> pack_bits(const std::vector<bool> &bits) {
 // ---------------------------------------------------------------------------------------
 // DataType / native type traits (arrow-array/src/types.rs:67-80)
 // ---------------------------------------------------------------------------------------
-enum class DataType { Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Boolean, Utf8 };
+enum class DataType { Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Boolean, Utf8, Decimal32, Decimal64, Decimal128 };
 
 template <class T> struct NativeOf;
 #define ACU_NATIVE(T, DT, CODE) \
@@ -279,6 +279,99 @@ using UInt32Array = PrimitiveArray<uint32_t>;
 using UInt64Array = PrimitiveArray<uint64_t>;
 using Float32Array = PrimitiveArray<float>;
 using Float64Array = PrimitiveArray<double>;
+
+// Decimal32 / Decimal64 / Decimal128 (arrow-array/src/types.rs DecimalType): natives int32_t / int64_t / __int128, with the
+// type's precision and scale. Decimal256 is not supported.
+template <class T> struct DecimalTraits;
+template <> struct DecimalTraits<int32_t> {
+  static constexpr DataType data_type = DataType::Decimal32; static constexpr acu_dtype code = ACU_I32;
+  static constexpr uint8_t max_precision = 9; static constexpr int8_t default_scale = 2; static constexpr const char *prefix = "Decimal32";
+};
+template <> struct DecimalTraits<int64_t> {
+  static constexpr DataType data_type = DataType::Decimal64; static constexpr acu_dtype code = ACU_I64;
+  static constexpr uint8_t max_precision = 18; static constexpr int8_t default_scale = 6; static constexpr const char *prefix = "Decimal64";
+};
+template <> struct DecimalTraits<__int128> {
+  static constexpr DataType data_type = DataType::Decimal128; static constexpr acu_dtype code = ACU_I128;
+  static constexpr uint8_t max_precision = 38; static constexpr int8_t default_scale = 10; static constexpr const char *prefix = "Decimal128";
+};
+
+// validate_decimal_precision_and_scale (arrow-array/src/types.rs:1442-1472): the error's Display text, empty when valid
+inline std::string decimal_type_error(int max_precision, int precision, int scale) {
+  const std::string p = "Invalid argument error: ";
+  if (precision == 0) return p + "precision cannot be 0, has to be between [1, " + std::to_string(max_precision) + "]";
+  if (precision > max_precision) return p + "precision " + std::to_string(precision) + " is greater than max " + std::to_string(max_precision);
+  if (scale > max_precision) return p + "scale " + std::to_string(scale) + " is greater than max " + std::to_string(max_precision);
+  if (scale > 0 && scale > precision) return p + "scale " + std::to_string(scale) + " is greater than precision " + std::to_string(precision);
+  return "";
+}
+
+template <class T>
+class DecimalArray : public Array {
+ public:
+  using Native = T;
+  using Traits = DecimalTraits<T>;
+  DecimalArray() = default;
+  DecimalArray(Buffer values, int64_t len, std::optional<NullBuffer> nulls, int64_t elem_offset = 0,
+               uint8_t precision = Traits::max_precision, int8_t scale = Traits::default_scale)
+      : values_(std::move(values)), elem_offset_(elem_offset), precision_(precision), scale_(scale) { len_ = len; nulls_ = std::move(nulls); }
+  // From<Vec<T>> / From<Vec<Option<T>>>: the default type Decimal*(MAX_PRECISION, DEFAULT_SCALE)
+  static DecimalArray from(const std::vector<T> &v) {
+    return DecimalArray(Buffer::from_host(v.data(), v.size() * sizeof(T)), (int64_t)v.size(), std::nullopt);
+  }
+  static DecimalArray from(const std::vector<std::optional<T>> &v) {
+    std::vector<T> vals(v.size(), T());
+    std::vector<bool> valid(v.size(), true);
+    for (size_t i = 0; i < v.size(); ++i) { if (v[i]) vals[i] = *v[i]; else valid[i] = false; }
+    return DecimalArray(Buffer::from_host(vals.data(), vals.size() * sizeof(T)), (int64_t)v.size(), nulls_from_mask(valid));
+  }
+  // PrimitiveArray::with_precision_and_scale (primitive_array.rs:1665-1671)
+  Result<DecimalArray> with_precision_and_scale(uint8_t precision, int8_t scale) const {
+    const std::string e = decimal_type_error(Traits::max_precision, precision, scale);
+    if (!e.empty()) return ArrowError{ACU_ERR_INVALID_ARGUMENT, e};
+    return DecimalArray(values_, len_, nulls_, elem_offset_, precision, scale);
+  }
+  DataType data_type() const override { return Traits::data_type; }
+  uint8_t precision() const { return precision_; }
+  int8_t scale() const { return scale_; }
+  acu_decimal_type decimal_type() const { return acu_decimal_type{(int32_t)sizeof(T), precision_, scale_, {0, 0}}; }
+  std::string type_display() const {  // Display of DataType::Decimal*(p, s)
+    return std::string(Traits::prefix) + "(" + std::to_string((int)precision_) + ", " + std::to_string((int)scale_) + ")";
+  }
+  DecimalArray slice(int64_t offset, int64_t length) const {
+    DecimalArray out(values_, length, nulls_, elem_offset_ + offset, precision_, scale_);
+    if (out.nulls_) {
+      out.nulls_->offset += offset;
+      out.nulls_->len = length;
+      out.nulls_->null_count = -1;
+    }
+    return out;
+  }
+  std::vector<T> values() const {
+    std::vector<T> v((size_t)len_);
+    if (len_) acu_memcpy_d2h(Context::get().raw(), v.data(), values_ptr(), (size_t)len_ * sizeof(T));
+    return v;
+  }
+  std::vector<std::optional<T>> to_vec() const {
+    auto vals = values();
+    auto valid = valid_mask();
+    std::vector<std::optional<T>> out((size_t)len_);
+    for (size_t i = 0; i < out.size(); ++i) if (valid[i]) out[i] = vals[i];
+    return out;
+  }
+ protected:
+  const void *values_ptr() const override { return static_cast<const T *>(values_.data()) + elem_offset_; }
+ private:
+  Buffer values_;
+  int64_t elem_offset_ = 0;
+  uint8_t precision_ = Traits::max_precision;
+  int8_t scale_ = Traits::default_scale;
+};
+using Decimal32Array = DecimalArray<int32_t>;
+using Decimal64Array = DecimalArray<int64_t>;
+using Decimal128Array = DecimalArray<__int128>;
+template <class A> struct is_decimal_array : std::false_type {};
+template <class T> struct is_decimal_array<DecimalArray<T>> : std::true_type {};
 
 class BooleanArray : public Array {
  public:
@@ -422,6 +515,9 @@ class RecordBatch {
 namespace compute {
 namespace detail {
 
+// DataType Display of an operand (decimals carry their precision and scale)
+template <class A> std::string type_text(const A &a);
+
 inline acu_array_out make_out(Buffer &values, Buffer &validity, size_t value_bytes, int64_t rows) {
   values = Buffer::allocate(value_bytes);
   validity = Buffer::allocate(acu_bitmap_bytes(rows));
@@ -455,8 +551,13 @@ inline ArrayRef make_primitive(DataType dt, Buffer values, int64_t len, std::opt
   }
 }
 inline const char *dtype_display(DataType t) {
-  static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64", "Boolean", "Utf8"};
+  static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64", "Boolean", "Utf8",
+                            "Decimal32", "Decimal64", "Decimal128"};
   return n[(int)t];
+}
+template <class A> std::string type_text(const A &a) {
+  if constexpr (is_decimal_array<A>::value) return a.type_display();
+  else return dtype_display(a.data_type());
 }
 // One acu_column per column of a RecordBatch (include/arrow_cuda.h: acu_column)
 inline acu_column column_view(const Array &a) {
@@ -1078,11 +1179,41 @@ class InProgressByteViewArray {
 namespace kernels {
 namespace numeric {
 namespace detail2 {
+// decimal_op (numeric.rs:970-1107): the result type comes from the device call
+template <class T>
+Result<ArrayRef> decimal_arith(acu_arith_op op, const DecimalArray<T> &l, bool ls, const DecimalArray<T> &r, bool rs) {
+  Context &c = Context::get();
+  const int64_t n = ls && !rs ? r.len() : l.len();
+  Buffer vb, nb;
+  acu_array a = l.view(ls), b = r.view(rs);
+  acu_decimal_type lt = l.decimal_type(), rt = r.decimal_type(), ot{};
+  acu_array_out o = compute::detail::make_out(vb, nb, (size_t)std::max<int64_t>(n, 1) * sizeof(T), n);
+  acu_status st = acu_decimal_arith(c.raw(), op, &lt, &a, &rt, &b, &ot, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return ArrayRef(std::make_shared<DecimalArray<T>>(vb, o.len, compute::detail::out_nulls(o, nb), 0, ot.precision, ot.scale));
+}
+template <class T> Result<ArrayRef> decimal_neg(const DecimalArray<T> &a) {  // neg_checked at every width (numeric.rs:116-136)
+  Context &c = Context::get();
+  Buffer vb, nb;
+  acu_array v = a.view();
+  acu_array_out o = compute::detail::make_out(vb, nb, (size_t)std::max<int64_t>(a.len(), 1) * sizeof(T), a.len());
+  acu_status st = acu_neg(c.raw(), DecimalTraits<T>::code, 1, &v, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return ArrayRef(std::make_shared<DecimalArray<T>>(vb, o.len, compute::detail::out_nulls(o, nb), 0, a.precision(), a.scale()));
+}
+
 template <class L, class R>
 Result<ArrayRef> arithmetic_op(acu_arith_op op, const char *sym, const L &lhs, const R &rhs) {
   const auto &l = datum_array(lhs);
   const auto &r = datum_array(rhs);
   const bool ls = datum_is_scalar(lhs), rs = datum_is_scalar(rhs);
+  using LA = std::decay_t<decltype(l)>;
+  using RA = std::decay_t<decltype(r)>;
+  if constexpr (is_decimal_array<LA>::value || is_decimal_array<RA>::value) {  // (Decimal*, Decimal*) arms, numeric.rs:257-260
+    if constexpr (std::is_same<LA, RA>::value) return decimal_arith(op, l, ls, r, rs);
+    else return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: Invalid arithmetic operation: " + compute::detail::type_text(l) +
+                                                         " " + sym + " " + compute::detail::type_text(r)};
+  } else {
   if (l.data_type() != r.data_type() || dtype_width(l.data_type()) == 0)  // numeric.rs:270-272
     return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Invalid arithmetic operation: ") +
                                                      compute::detail::dtype_display(l.data_type()) + " " + sym + " " +
@@ -1095,6 +1226,7 @@ Result<ArrayRef> arithmetic_op(acu_arith_op op, const char *sym, const L &lhs, c
   acu_status st = acu_arith(c.raw(), (acu_dtype)dtype_code(l.data_type()), op, &a, &b, &o);
   if (st != ACU_OK) return c.last_error(st);
   return compute::detail::make_primitive(l.data_type(), vb, o.len, compute::detail::out_nulls(o, nb));
+  }
 }
 }  // namespace detail2
 #define ACU_NUMERIC(NAME, OP, SYM) \
@@ -1105,6 +1237,10 @@ ACU_NUMERIC(div, ACU_DIV, "/") ACU_NUMERIC(rem, ACU_REM, "%")
 #undef ACU_NUMERIC
 
 inline Result<ArrayRef> neg_impl(const Array &a, int checked) {
+  // decimals: neg_wrapping falls back to neg (numeric.rs:181-186)
+  if (auto d = dynamic_cast<const Decimal32Array *>(&a)) return detail2::decimal_neg(*d);
+  if (auto d = dynamic_cast<const Decimal64Array *>(&a)) return detail2::decimal_neg(*d);
+  if (auto d = dynamic_cast<const Decimal128Array *>(&a)) return detail2::decimal_neg(*d);
   Context &c = Context::get();
   Buffer vb, nb;
   acu_array v = a.view();
@@ -1125,6 +1261,17 @@ Result<BooleanArray> compare_op(acu_cmp_op op, const char *sym, const L &lhs, co
   const auto &l = datum_array(lhs);
   const auto &r = datum_array(rhs);
   const bool ls = datum_is_scalar(lhs), rs = datum_is_scalar(rhs);
+  using LA = std::decay_t<decltype(l)>;
+  acu_dtype code = (acu_dtype)dtype_code(l.data_type());
+  if constexpr (is_decimal_array<LA>::value) {  // decimals compare as their natives; the DataTypes must be equal, precision included
+    if (!ls && !rs && l.len() != r.len())  // cmp.rs:228-232 comes first
+      return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: Cannot compare arrays of different lengths, got " +
+                                                      std::to_string(l.len()) + " vs " + std::to_string(r.len())};
+    if (compute::detail::type_text(l) != compute::detail::type_text(r))
+      return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: Invalid comparison operation: " + compute::detail::type_text(l) +
+                                                      " " + sym + " " + compute::detail::type_text(r)};
+    code = DecimalTraits<typename LA::Native>::code;
+  }
   if (l.data_type() != r.data_type())  // cmp.rs:260-264
     return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Invalid comparison operation: ") +
                                                      compute::detail::dtype_display(l.data_type()) + " " + sym + " " +
@@ -1134,7 +1281,7 @@ Result<BooleanArray> compare_op(acu_cmp_op op, const char *sym, const L &lhs, co
   Buffer vb, nb;
   acu_array a = l.view(ls), b = r.view(rs);
   acu_array_out o = compute::detail::make_out(vb, nb, acu_bitmap_bytes(std::max<int64_t>(n, 1)), std::max<int64_t>(n, 1));
-  acu_status st = acu_cmp(c.raw(), (acu_dtype)dtype_code(l.data_type()), op, &a, &b, &o);
+  acu_status st = acu_cmp(c.raw(), code, op, &a, &b, &o);
   if (st != ACU_OK) return c.last_error(st);
   return BooleanArray(vb, 0, o.len, compute::detail::out_nulls(o, nb));
 }
@@ -1229,7 +1376,24 @@ std::optional<T> aggregate(acu_agg_op op, const PrimitiveArray<T> &a) {
   std::memcpy(&out, &bits, sizeof(T));
   return out;
 }
+// decimals: sum wraps in the native, min / max in its order (acu_aggregate_i128 for Decimal128)
+template <class T>
+std::optional<T> aggregate_decimal(acu_agg_op op, const DecimalArray<T> &a) {
+  uint64_t bits[2] = {0, 0};
+  int64_t valid = 0;
+  acu_array v = a.view();
+  acu_status st = sizeof(T) == 16 ? acu_aggregate_i128(Context::get().raw(), op, &v, bits, &valid)
+                                  : acu_aggregate(Context::get().raw(), DecimalTraits<T>::code, op, &v, bits, &valid);
+  if (st != ACU_OK) throw std::runtime_error(Context::get().last_error(st).message);
+  if (valid == 0) return std::nullopt;
+  T out;
+  std::memcpy(&out, bits, sizeof(T));
+  return out;
+}
 }  // namespace detail
+template <class T> std::optional<T> sum(const DecimalArray<T> &a) { return detail::aggregate_decimal(ACU_SUM, a); }
+template <class T> std::optional<T> min(const DecimalArray<T> &a) { return detail::aggregate_decimal(ACU_MIN, a); }
+template <class T> std::optional<T> max(const DecimalArray<T> &a) { return detail::aggregate_decimal(ACU_MAX, a); }
 template <class T> std::optional<T> sum(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_SUM, a); }
 template <class T> std::optional<T> min(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_MIN, a); }
 template <class T> std::optional<T> max(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_MAX, a); }

@@ -82,11 +82,18 @@ typedef struct acu_error_detail {
 
 typedef struct acu_ctx acu_ctx;
 
-/* Native types (arrow-array/src/types.rs:67-80, ArrowPrimitiveType::Native). */
+/* Native types (arrow-array/src/types.rs:67-80, ArrowPrimitiveType::Native).
+ * ACU_I128 is the native of Decimal128: 16-byte little-endian two's complement values whose pointer must be 16-byte
+ * aligned (the alignment of i128; a misaligned pointer => ACU_ERR_INVALID_ARGUMENT). Only acu_cmp (and through it
+ * acu_filter_plan_create_cmp) and acu_neg accept it; every other entry point taking an acu_dtype rejects it as it
+ * rejects an unknown dtype. Decimal32 / Decimal64 columns ARE Int32 / Int64 columns to acu_cmp, acu_filter_plan_create_cmp,
+ * acu_aggregate and acu_aggregate_columns: the reference compares and aggregates decimals as their native integers, so
+ * ACU_I32 / ACU_I64 give Decimal32 / Decimal64 exactly the reference's results. */
 typedef enum acu_dtype {
   ACU_I8 = 0, ACU_I16 = 1, ACU_I32 = 2, ACU_I64 = 3,
   ACU_U8 = 4, ACU_U16 = 5, ACU_U32 = 6, ACU_U64 = 7,
-  ACU_F32 = 8, ACU_F64 = 9
+  ACU_F32 = 8, ACU_F64 = 9,
+  ACU_I128 = 10
 } acu_dtype;
 
 /* arrow-arith/src/numeric.rs:181-190 `enum Op` — same order. */
@@ -178,8 +185,9 @@ int64_t acu_bytes_allocated(const acu_ctx *ctx);
  * aggregate bits), fills acu_filter_plan count / strategy, and returns the FIRST error in call order with its exact
  * reference text (the outputs of the calls after a failed one are unspecified, as after any failed call).
  *   - stream-ordered inside a section: acu_filter_plan_create, acu_filter_plan_create_cmp, acu_filter_primitive,
- *     acu_filter_boolean, acu_take_primitive / acu_take_boolean (check_bounds = 0), acu_arith, acu_cmp, acu_aggregate,
- *     acu_aggregate_allreduce. Any other entry point fails with ACU_ERR_INVALID_ARGUMENT (it would synchronise).
+ *     acu_filter_boolean, acu_take_primitive / acu_take_boolean (check_bounds = 0), acu_arith, acu_decimal_arith, acu_cmp
+ *     (ACU_I128 included), acu_neg (ACU_I128 only), acu_aggregate, acu_aggregate_i128, acu_aggregate_allreduce. Any other
+ *     entry point fails with ACU_ERR_INVALID_ARGUMENT (it would synchronise).
  *   - every output descriptor, scalar output pointer and plan passed to a queued call must stay alive until the fetch;
  *     input arrays must carry their cached null_count (-1 would need a device count = a synchronisation), except for
  *     acu_aggregate*, which then counts the valid rows on the device (an array produced earlier in the same section);
@@ -333,16 +341,65 @@ acu_status acu_take_bytes(acu_ctx *ctx, int32_t offset_bytes, const void *offset
  * try_binary_mut consumes its input as well). */
 acu_status acu_arith(acu_ctx *ctx, acu_dtype dtype, acu_arith_op op, const acu_array *a,
                      const acu_array *b, acu_array_out *out);
-/* neg (checked != 0) / neg_wrapping (numeric.rs:103-186). */
+/* neg (checked != 0) / neg_wrapping (numeric.rs:103-186). ACU_I128 (Decimal128) is always neg_checked, whatever
+ * `checked` says: the reference's neg_wrapping falls back to neg for every non-integer type (numeric.rs:181-186). For the
+ * same reason a Decimal32 / Decimal64 negation is acu_neg(ACU_I32 / ACU_I64, checked = 1). */
 acu_status acu_neg(acu_ctx *ctx, acu_dtype dtype, int32_t checked, const acu_array *a,
                    acu_array_out *out);
+
+/* ------------------------------------------------------------------------- */
+/* decimal arithmetic — decimal_op (arrow-arith/src/numeric.rs:970-1107)     */
+/* ------------------------------------------------------------------------- */
+/* DataType::Decimal32 / 64 / 128(precision, scale): byte_width 4 / 8 / 16 (values ACU_I32 / ACU_I64 / ACU_I128).
+ * Decimal256 is not supported. */
+typedef struct acu_decimal_type {
+  int32_t byte_width;
+  uint8_t precision;
+  int8_t scale;
+  uint8_t reserved[2];
+} acu_decimal_type;
+
+/* add / sub / mul / div / rem of two decimal operands of the same width, with the reference's Hive precision / scale rules
+ * (MAX_PRECISION = MAX_SCALE = 9 / 18 / 38 for widths 4 / 8 / 16). *out_type receives the result type; out->values holds
+ * byte_width bytes per row.
+ *   - add, sub (s = max(s1, s2)): l * 10^(s - s1) +/- r * 10^(s - s2), each multiplication checked, left before right;
+ *     mul: l * r checked, scale s1 + s2; div (scale min(s1 + 4, MAX_SCALE)): l * l_mul / r * r_mul, truncated toward zero;
+ *     rem: l * l_mul % r * r_mul with the multipliers of add computed WRAPPING (pow_wrapping), and MIN % -1 an overflow
+ *     (mod_checked, not the integer rem's 0). The wrapping ops are checked like the others.
+ *   - rows are evaluated only where both sides are valid (try_binary / try_unary: zero under nulls); a scalar (is_scalar)
+ *     is rescaled per row, so its overflow is reported at the lowest valid row of the array and not at all when no row is
+ *     valid; a null scalar gives an all-null result. The error of the lowest failing valid row is returned:
+ *     ACU_ERR_ARITHMETIC_OVERFLOW "Overflow happened on: {a} {op} {b}" with the operands of the failing step (a rescale
+ *     prints the rescaled operand and its multiplier, "10 * 100000000000000000000000000000000000000"), or
+ *     ACU_ERR_DIVIDE_BY_ZERO "Divide by zero error". detail.index = that row, lhs_bits / rhs_bits = the low 64 bits of
+ *     the row's raw operands.
+ *   - before any row is read, also for empty arrays: ACU_ERR_ARITHMETIC_OVERFLOW "Overflow happened on: 10 ^ {exp}" when
+ *     a multiplier does not fit the native type; ACU_ERR_INVALID_ARGUMENT "Output scale of Decimal128(3, 3) *
+ *     Decimal128(37, 37) would exceed max scale of 38" for mul. After the rows (a row error wins), the result type is
+ *     validated like with_precision_and_scale: ACU_ERR_INVALID_ARGUMENT "precision cannot be 0, has to be between [1,
+ *     {MAX}]", "scale {s} is greater than max {MAX}", "scale {s} is greater than precision {p}".
+ *   - The result type follows Rust's i8 / u8 arithmetic (saturating_add, `as u8`, .min(MAX_PRECISION)). Where the
+ *     reference's `p as i8 - s` or a scale difference leaves the i8 range (a scale below -89), the reference panics in
+ *     debug builds and wraps in release builds; this library wraps, like a release build: the difference is taken
+ *     modulo 256 and a negative exponent reads as a huge u32 (so the multiplier overflows, or is 0 for rem).
+ *   - an operand type that validate_decimal_precision_and_scale rejects (precision 0 or above MAX_PRECISION, scale above
+ *     MAX_SCALE or above a positive precision), byte widths that differ or are not 4 / 8 / 16, an ACU_I128 pointer that is
+ *     not 16-byte aligned, or op outside acu_arith_op => ACU_ERR_INVALID_ARGUMENT at call time; lengths that differ =>
+ *     ACU_ERR_COMPUTE "Cannot perform a binary operation on arrays of different length".
+ * Stream-ordered inside a section (the result-type validation then reports at the fetch); kernel time counts in
+ * ACU_K_ARITH. In place as acu_arith. */
+acu_status acu_decimal_arith(acu_ctx *ctx, acu_arith_op op, const acu_decimal_type *lt, const acu_array *a,
+                             const acu_decimal_type *rt, const acu_array *b, acu_decimal_type *out_type,
+                             acu_array_out *out);
 
 /* ------------------------------------------------------------------------- */
 /* cmp — arrow-ord/src/cmp.rs                                                */
 /* ------------------------------------------------------------------------- */
 /* eq/neq/lt/lt_eq/gt/gt_eq/distinct/not_distinct (cmp.rs:79-202). Result is a boolean
  * array: out->values = bit-packed results. Floats compare by IEEE-754 totalOrder
- * (arrow-array/src/arithmetic.rs:400-410). */
+ * (arrow-array/src/arithmetic.rs:400-410). ACU_I128 (Decimal128) compares as signed i128; decimals compare as their
+ * native integers, so the reference's refusal of operands whose decimal types differ ("Invalid comparison operation:
+ * {l_t} {op} {r_t}", cmp.rs:260-263) belongs to the caller, which knows the logical types. */
 acu_status acu_cmp(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, const acu_array *a,
                    const acu_array *b, acu_array_out *out);
 
@@ -468,6 +525,11 @@ acu_status acu_boolean(acu_ctx *ctx, acu_bool_op op, const acu_array *a, const a
  * returns None iff out_valid_count == 0 (aggregate.rs:320-323). */
 acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a,
                          uint64_t *out_bits, int64_t *out_valid_count);
+/* sum / min / max of a Decimal128 (ACU_I128) column: out_bits[0] = low, out_bits[1] = high 64 bits of the i128 result;
+ * sum wraps (add_wrapping in i128), min / max use the signed i128 order; None iff *out_valid_count == 0. Decimal32 /
+ * Decimal64 columns use acu_aggregate with ACU_I32 / ACU_I64. Stream-ordered inside a section like acu_aggregate. */
+acu_status acu_aggregate_i128(acu_ctx *ctx, acu_agg_op op, const acu_array *a, uint64_t out_bits[2],
+                              int64_t *out_valid_count);
 
 /* sum_checked (aggregate.rs:897-937): the in-order checked fold. Integers:
  * ACU_ERR_ARITHMETIC_OVERFLOW "Overflow happened on: {acc} + {value}" at the first valid

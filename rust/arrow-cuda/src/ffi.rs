@@ -30,6 +30,8 @@ pub const ACU_U32: i32 = 6;
 pub const ACU_U64: i32 = 7;
 pub const ACU_F32: i32 = 8;
 pub const ACU_F64: i32 = 9;
+// Decimal128's native (16-byte two's complement, 16-byte aligned): acu_cmp, acu_filter_plan_create_cmp and acu_neg only
+pub const ACU_I128: i32 = 10;
 // acu_arith_op == arrow-arith/src/numeric.rs:181-190 `enum Op`
 pub const ACU_ADD_WRAPPING: i32 = 0;
 pub const ACU_ADD: i32 = 1;
@@ -87,6 +89,16 @@ pub struct acu_error_detail {
     pub rhs_bits: u64,
     pub len: u64,
     pub message: [c_char; 256],
+}
+
+/// acu_decimal_type: DataType::Decimal32 / 64 / 128(precision, scale) as byte_width 4 / 8 / 16
+#[repr(C)]
+#[derive(Clone, Copy, Debug, Default)]
+pub struct acu_decimal_type {
+    pub byte_width: i32,
+    pub precision: u8,
+    pub scale: i8,
+    pub reserved: [u8; 2],
 }
 
 #[repr(C)]
@@ -189,9 +201,13 @@ extern "C" {
                           out_data: *mut u8, out_data_capacity: i64, out_data_len: *mut i64, out_nulls: *mut acu_array_out) -> acu_status;
     pub fn acu_arith(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_neg(ctx: *mut acu_ctx, dtype: i32, checked: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_decimal_arith(ctx: *mut acu_ctx, op: i32, lt: *const acu_decimal_type, a: *const acu_array, rt: *const acu_decimal_type,
+                             b: *const acu_array, out_type: *mut acu_decimal_type, out: *mut acu_array_out) -> acu_status;
     pub fn acu_cmp(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_cast_numeric(ctx: *mut acu_ctx, from: i32, to: i32, safe: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_aggregate(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, out_bits: *mut u64, out_valid: *mut i64) -> acu_status;
+    /// out_bits: 2 words (low, high) of the i128 result
+    pub fn acu_aggregate_i128(ctx: *mut acu_ctx, op: i32, a: *const acu_array, out_bits: *mut u64, out_valid: *mut i64) -> acu_status;
     pub fn acu_boolean(ctx: *mut acu_ctx, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_filter_record_batch(ctx: *mut acu_ctx, plan: *const acu_filter_plan, n_columns: i32, columns: *const acu_column,
                                    outs: *mut acu_column_out) -> acu_status;

@@ -120,6 +120,28 @@ fn dtype_code(t: &DataType) -> Option<i32> {
     })
 }
 
+/// acu_dtype of a type's native for acu_cmp / acu_neg / the aggregates: the numeric types, and decimals as their integers
+/// (the reference compares and aggregates decimals as their natives). acu_arith takes only `dtype_code`.
+fn native_code(t: &DataType) -> Option<i32> {
+    match t {
+        DataType::Decimal32(_, _) => Some(ffi::ACU_I32),
+        DataType::Decimal64(_, _) => Some(ffi::ACU_I64),
+        DataType::Decimal128(_, _) => Some(ffi::ACU_I128),
+        t => dtype_code(t),
+    }
+}
+
+/// acu_decimal_type of Decimal32 / 64 / 128 (Decimal256 is not supported on the device)
+fn decimal_type(t: &DataType) -> Option<ffi::acu_decimal_type> {
+    let (byte_width, precision, scale) = match t {
+        DataType::Decimal32(p, s) => (4, *p, *s),
+        DataType::Decimal64(p, s) => (8, *p, *s),
+        DataType::Decimal128(p, s) => (16, *p, *s),
+        _ => return None,
+    };
+    Some(ffi::acu_decimal_type { byte_width, precision, scale, reserved: [0; 2] })
+}
+
 enum Kind { Primitive(usize), Boolean, Bytes(usize) }
 fn kind_of(t: &DataType) -> Result<Kind, ArrowError> {
     match t {
@@ -401,13 +423,18 @@ pub mod compute {
 
     // ---- aggregate (arrow-arith/src/aggregate.rs) ------------------------------------------------------------------------
     fn aggregate<T: ArrowPrimitiveType>(op: i32, array: &PrimitiveArray<T>) -> Option<T::Native> {
-        let dtype = dtype_code(&T::DATA_TYPE)?; // derived from T: a caller cannot pass a mismatching code
+        let dtype = native_code(&T::DATA_TYPE)?; // derived from T: a caller cannot pass a mismatching code
         let ctx = Context::current().ok()?;
         let a = DeviceArray::upload(&ctx, array, false).ok()?;
-        let (mut bits, mut valid) = (0u64, 0i64);
-        ctx.check(unsafe { ffi::acu_aggregate(ctx.raw(), dtype, op, a.view(), &mut bits, &mut valid) }).ok()?;
+        let (mut bits, mut valid) = ([0u64; 2], 0i64);
+        let st = if dtype == ffi::ACU_I128 { // Decimal128: sum wraps in i128, min / max in i128 order
+            unsafe { ffi::acu_aggregate_i128(ctx.raw(), op, a.view(), bits.as_mut_ptr(), &mut valid) }
+        } else {
+            unsafe { ffi::acu_aggregate(ctx.raw(), dtype, op, a.view(), bits.as_mut_ptr(), &mut valid) }
+        };
+        ctx.check(st).ok()?;
         if valid == 0 { return None; }
-        Some(unsafe { std::ptr::read_unaligned(&bits as *const u64 as *const T::Native) }) // native bit pattern, zero-extended, little endian
+        Some(unsafe { std::ptr::read_unaligned(bits.as_ptr() as *const T::Native) }) // native bit pattern, zero-extended, little endian
     }
     /// aggregate.rs:943 / :1012 / :1027 — `None` iff no valid row.
     pub fn sum<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_SUM, array) }
@@ -676,9 +703,30 @@ pub mod compute {
         /// `arrow::compute::kernels::numeric` (arrow-arith/src/numeric.rs:36-186)
         pub mod numeric {
             use super::*;
+            /// decimal_op (numeric.rs:970-1107): the result DataType comes back from the device call
+            fn decimal_op(op: i32, l: &dyn Array, l_s: bool, r: &dyn Array, r_s: bool) -> Result<ArrayRef, ArrowError> {
+                let (lt, rt) = (decimal_type(l.data_type()).unwrap(), decimal_type(r.data_type()).unwrap());
+                let ctx = Context::current()?;
+                let (a, b) = (DeviceArray::upload(&ctx, l, l_s)?, DeviceArray::upload(&ctx, r, r_s)?);
+                let n = if l_s && !r_s { r.len() } else { l.len() };
+                let mut out = ColumnOut::new(&ctx, l.data_type(), n, 0)?;
+                let mut ot = ffi::acu_decimal_type::default();
+                ctx.check(unsafe { ffi::acu_decimal_arith(ctx.raw(), op, &lt, a.view(), &rt, b.view(), &mut ot, out.array_out()) })?;
+                out.finish(&match ot.byte_width {
+                    4 => DataType::Decimal32(ot.precision, ot.scale),
+                    8 => DataType::Decimal64(ot.precision, ot.scale),
+                    _ => DataType::Decimal128(ot.precision, ot.scale),
+                })
+            }
             fn arithmetic_op(op: i32, sym: &str, lhs: &dyn Datum, rhs: &dyn Datum) -> Result<ArrayRef, ArrowError> {
                 let (l, l_s) = lhs.get();
                 let (r, r_s) = rhs.get();
+                match (l.data_type(), r.data_type()) { // the (Decimal*, Decimal*) arms of numeric.rs:257-259
+                    (DataType::Decimal32(_, _), DataType::Decimal32(_, _))
+                    | (DataType::Decimal64(_, _), DataType::Decimal64(_, _))
+                    | (DataType::Decimal128(_, _), DataType::Decimal128(_, _)) => return decimal_op(op, l, l_s, r, r_s),
+                    _ => {}
+                }
                 let dtype = match (dtype_code(l.data_type()), l.data_type() == r.data_type()) { // numeric.rs:270-272
                     (Some(c), true) => c,
                     _ => return Err(ArrowError::InvalidArgumentError(format!("Invalid arithmetic operation: {} {sym} {}", l.data_type(), r.data_type()))),
@@ -699,7 +747,11 @@ pub mod compute {
             pub fn div(lhs: &dyn Datum, rhs: &dyn Datum) -> Result<ArrayRef, ArrowError> { arithmetic_op(ffi::ACU_DIV, "/", lhs, rhs) }
             pub fn rem(lhs: &dyn Datum, rhs: &dyn Datum) -> Result<ArrayRef, ArrowError> { arithmetic_op(ffi::ACU_REM, "%", lhs, rhs) }
             fn neg_op(array: &dyn Array, checked: i32) -> Result<ArrayRef, ArrowError> {
-                let dtype = numeric_dtype("arithmetic", array.data_type())?;
+                // decimals: neg_checked at every width (numeric.rs:116-136); neg_wrapping falls back to neg (:181-186)
+                let (dtype, checked) = match (decimal_type(array.data_type()), native_code(array.data_type())) {
+                    (Some(_), Some(code)) => (code, 1),
+                    _ => (numeric_dtype("arithmetic", array.data_type())?, checked),
+                };
                 let ctx = Context::current()?;
                 let a = DeviceArray::upload(&ctx, array, false)?;
                 let mut out = ColumnOut::new(&ctx, array.data_type(), array.len(), 0)?;
@@ -730,7 +782,7 @@ pub mod compute {
                         unsafe { ffi::acu_cmp_bytes(ctx.raw(), ob as i32, op, &x, &y, out.array_out()) }
                     }
                     _ => {
-                        let dtype = dtype_code(l.data_type())
+                        let dtype = native_code(l.data_type()) // decimals compare as their natives
                             .ok_or_else(|| ArrowError::InvalidArgumentError(format!("Invalid comparison operation: {} {sym} {}", l.data_type(), r.data_type())))?;
                         unsafe { ffi::acu_cmp(ctx.raw(), dtype, op, a.view(), b.view(), out.array_out()) }
                     }
