@@ -64,6 +64,14 @@ def rand_bool(rng, n, true_p, null_p, offset=0):
     return h.slice(offset, n) if offset else h
 
 
+def word_aligned_bool(rng, n, true_p, null_p):
+    """A boolean array whose values and validity each start at bit 0, 64 or 128 of their buffers: the word-aligned variant
+    of the boolean kernels."""
+    voff, noff = (int(x) for x in rng.choice([0, 64, 128], 2))
+    mask = None if null_p is None else rng.random(n) >= null_p
+    return HostArray.bool_from_numpy(rng.random(n) < true_p, mask, bit_offset=voff, mask_offset=noff)
+
+
 def same_bits(a, b):
     return np.array_equal(np.ascontiguousarray(a).view(np.uint8), np.ascontiguousarray(b).view(np.uint8))
 
@@ -566,20 +574,27 @@ def test_cast_fuzz(gpu, oracle, frm, to):
 @pytest.mark.parametrize("op", ["and_", "or_", "and_not", "and_kleene", "or_kleene"])
 def test_boolean_binary_fuzz(gpu, oracle, op):
     rng = np.random.default_rng(6000 + len(op))
+    arng = np.random.default_rng(6500 + len(op))
     for n in SIZES:
         for an, bn in [(None, None), (0.2, None), (None, 0.2), (0.3, 0.3), (0.0, None)]:
             a, b = rand_bool(rng, n, 0.5, an, offset=int(rng.integers(0, 70))), rand_bool(rng, n, 0.4, bn, offset=int(rng.integers(0, 9)))
             assert_same(getattr(gpu, op)(a, b), getattr(oracle, op)(a, b), f"{op} n={n} nulls=({an},{bn})")
+            a, b = word_aligned_bool(arng, n, 0.5, an), word_aligned_bool(arng, n, 0.4, bn)
+            assert_same(getattr(gpu, op)(a, b), getattr(oracle, op)(a, b), f"{op} word-aligned n={n} nulls=({an},{bn})")
     got, exp = expect_same_error(gpu, oracle, lambda be: getattr(be, op)(rand_bool(np.random.default_rng(1), 5, 0.5, None), rand_bool(np.random.default_rng(2), 6, 0.5, None)))
     assert got is None and exp is None
 
 
 def test_boolean_unary_fuzz(gpu, oracle):
     rng = np.random.default_rng(6100)
+    arng = np.random.default_rng(6600)
     for n in SIZES:
         for null_p in (None, 0.25, 1.0):
             a = rand_bool(rng, n, 0.5, null_p, offset=int(rng.integers(0, 70)))
             assert_same(gpu.not_(a), oracle.not_(a), f"not n={n}")
+            w = word_aligned_bool(arng, n, 0.5, null_p)
+            for op in ("not_", "is_null", "is_not_null"):
+                assert_same(getattr(gpu, op)(w), getattr(oracle, op)(w), f"{op} word-aligned n={n}")
             for src in (a, rand_array(rng, abi.I64, n, null_p, offset=3), rand_array(rng, abi.I8, n, null_p)):
                 assert_same(gpu.is_null(src), oracle.is_null(src), f"is_null n={n}")
                 assert_same(gpu.is_not_null(src), oracle.is_not_null(src), f"is_not_null n={n}")
