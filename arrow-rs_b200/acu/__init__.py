@@ -1170,6 +1170,123 @@ class Context:
             for p in owned:
                 self.free(p)
 
+    # -- length / bit_length / substring / substring_by_char (arrow-string/src/length.rs, substring.rs) ------
+    def _upload_fsb(self, col, owned):
+        d = self._upload_nulls(col.nulls, owned)
+        dv = self.malloc(col.values.nbytes + 16)
+        owned.append(dv)
+        if col.values.nbytes:
+            self.h2d(dv, col.values)
+        d.values = dv
+        return d
+
+    def _length(self, op, col):
+        owned, keep = [], []
+        n = col.length
+        wide = isinstance(col, Utf8Column) and col.offsets.dtype == np.int64
+        out = self.alloc_out(n * (8 if wide else 4), n)
+        try:
+            if isinstance(col, Utf8Column):
+                d = self._upload_bytes_col(col, owned)
+                self.check(self.lib.acu_length_bytes(self.h, col.offsets.dtype.itemsize, op, C.byref(d), C.byref(out)))
+            elif isinstance(col, ViewColumn):
+                d = self._upload_view_col(col, owned, keep)
+                self.check(self.lib.acu_length_byte_view(self.h, op, C.byref(d), C.byref(out)))
+            else:
+                d = self._upload_fsb(col, owned)
+                self.check(self.lib.acu_length_fixed_size_binary(self.h, col.width, op, C.byref(d), C.byref(out)))
+            res, out = self.download_out(out, I64 if wide else I32), None
+            return res
+        finally:
+            if out is not None:
+                self._free_out(out)
+            for p in owned:
+                self.free(p)
+
+    def length(self, col):
+        """arrow_string::length::length of a Utf8Column, ViewColumn or FixedSizeBinaryColumn: an Int32 (Int64 for i64 offsets)
+        HostArray carrying the input's NullBuffer."""
+        return self._length(abi.LENGTH, col)
+
+    def bit_length(self, col):
+        return self._length(abi.BIT_LENGTH, col)
+
+    def _substring_offsets(self, fn, col, data_capacity):
+        """Two-phase byte-array substring: the sizing call (no data buffer), then the copy into `data_capacity` bytes
+        (default: exactly the size). fn(d_out_off, d_out_data, capacity, total_ref, out) calls the entry point."""
+        n, ob = col.length, col.offsets.dtype.itemsize
+        d_out_off = self.malloc((n + 1) * ob + 16)
+        out = self.alloc_out(0, n)
+        d_out_data = None
+        try:
+            total = C.c_int64(0)
+            self.check(fn(d_out_off, None, 0, C.byref(total), C.byref(out)))
+            cap = total.value if data_capacity is None else data_capacity
+            d_out_data = self.malloc(cap + 16)
+            self.check(fn(d_out_off, d_out_data, cap, C.byref(total), C.byref(out)))
+            o = self.d2h(d_out_off, (n + 1) * ob, col.offsets.dtype)
+            b = self.d2h(d_out_data, total.value)
+            validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+            return Utf8Column(o, b, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
+        finally:
+            self._free_out(out)
+            for p in (d_out_off, d_out_data):
+                self.free(p)
+
+    def substring(self, col, start, length=None, is_utf8=True, data_capacity=None):
+        """arrow_string::substring::substring(col, start, length) of a Utf8Column (is_utf8=False: Binary / LargeBinary),
+        ViewColumn (is_utf8=False: BinaryView) or FixedSizeBinaryColumn. A view result shares the input's data buffers."""
+        owned, keep = [], []
+        has_len, ln = (0, 0) if length is None else (1, int(length))
+        try:
+            if isinstance(col, Utf8Column):
+                d = self._upload_bytes_col(col, owned)
+                ob = col.offsets.dtype.itemsize
+                return self._substring_offsets(
+                    lambda oo, od, cap, tot, out: self.lib.acu_substring_bytes(self.h, ob, int(is_utf8), int(start), has_len, ln, C.byref(d),
+                                                                              col.data.nbytes, oo, od, cap, tot, out), col, data_capacity)
+            n = col.length
+            if isinstance(col, ViewColumn):
+                d = self._upload_view_col(col, owned, keep)
+                d_views = self.malloc(n * 16 + 16)
+                owned.append(d_views)
+                out = self.alloc_out(0, n)
+                try:
+                    self.check(self.lib.acu_substring_byte_view(self.h, int(is_utf8), int(start), has_len, ln, C.byref(d), d_views, C.byref(out)))
+                    views = self.d2h(d_views, n * 16).reshape(n, 16)
+                    validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+                finally:
+                    self._free_out(out)
+                nulls = HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0)
+                return ViewColumn(views, col.buffers, nulls)
+            d = self._upload_fsb(col, owned)
+            out = self.alloc_out(n * col.width, n)
+            try:
+                w = C.c_int32(0)
+                self.check(self.lib.acu_substring_fixed_size_binary(self.h, col.width, int(start), has_len, ln, C.byref(d), C.byref(w), C.byref(out)))
+                vals = self.d2h(out.values, n * w.value).reshape(n, w.value)
+                validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+            finally:
+                self._free_out(out)
+            return FixedSizeBinaryColumn(vals, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
+        finally:
+            for p in owned:
+                self.free(p)
+
+    def substring_by_char(self, col, start, length=None, data_capacity=None):
+        """arrow_string::substring::substring_by_char of a Utf8Column (Utf8 / LargeUtf8)."""
+        owned = []
+        has_len, ln = (0, 0) if length is None else (1, int(length))
+        try:
+            d = self._upload_bytes_col(col, owned)
+            ob = col.offsets.dtype.itemsize
+            return self._substring_offsets(
+                lambda oo, od, cap, tot, out: self.lib.acu_substring_by_char(self.h, ob, int(start), has_len, ln, C.byref(d), oo, od, cap, tot, out),
+                col, data_capacity)
+        finally:
+            for p in owned:
+                self.free(p)
+
     # -- fused compare -> filter (cmp.rs:220-382 feeding filter.rs:254-273) -------------------
     def filter_cmp(self, values, op, a, b):
         """filter(values, &cmp::op(a, b)?) with the predicate never materialised: the comparison writes the filter plan."""

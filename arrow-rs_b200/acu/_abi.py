@@ -39,6 +39,8 @@ EQ, NEQ, LT, LT_EQ, GT, GT_EQ, DISTINCT, NOT_DISTINCT = range(8)
 SUM, MIN, MAX = range(3)
 # acu_like_op (arrow-string/src/like.rs `enum Op`)
 LIKE, NLIKE, ILIKE, NILIKE, CONTAINS, STARTS_WITH, ENDS_WITH, EQ_IGNORE_ASCII_CASE = range(8)
+# acu_length_op (arrow-string/src/length.rs length / bit_length)
+LENGTH, BIT_LENGTH = range(2)
 # acu_filter_strategy
 FILTER_NONE, FILTER_ALL, FILTER_INDEX, FILTER_SLICES = range(4)
 
@@ -215,6 +217,13 @@ PROTOTYPES = {
     "acu_cmp_byte_view": (i32, [vp, i32, P(ViewArray), P(ViewArray), P(ArrayOut)]),
     "acu_like_bytes": (i32, [vp, i32, i32, i32, P(BytesArray), P(BytesArray), P(ArrayOut)]),
     "acu_like_byte_view": (i32, [vp, i32, i32, P(ViewArray), P(ViewArray), P(ArrayOut)]),
+    "acu_length_bytes": (i32, [vp, i32, i32, P(BytesArray), P(ArrayOut)]),
+    "acu_length_byte_view": (i32, [vp, i32, P(ViewArray), P(ArrayOut)]),
+    "acu_length_fixed_size_binary": (i32, [vp, i32, i32, P(Array), P(ArrayOut)]),
+    "acu_substring_bytes": (i32, [vp, i32, i32, i64, i32, u64, P(BytesArray), i64, vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_substring_by_char": (i32, [vp, i32, i64, i32, u64, P(BytesArray), vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_substring_byte_view": (i32, [vp, i32, i64, i32, u64, P(ViewArray), vp, P(ArrayOut)]),
+    "acu_substring_fixed_size_binary": (i32, [vp, i32, i64, i32, u64, P(Array), P(i32), P(ArrayOut)]),
     "acu_cast_numeric": (i32, [vp, i32, i32, i32, P(Array), P(ArrayOut)]),
     "acu_boolean": (i32, [vp, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_aggregate": (i32, [vp, i32, i32, P(Array), P(u64), P(i64)]),

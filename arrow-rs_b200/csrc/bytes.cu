@@ -16,12 +16,10 @@
 #include <stdlib.h>
 
 #include "bitmap.cuh"
+#include "bytes_engine.cuh"
 #include "internal.cuh"
 
 #define SCAN_ELEMS 4096
-#define BY_THREADS 512                 // CTA of the bytes kernels: 512 threads x 4 consecutive rows,
-#define BY_ROWS (BY_THREADS * 4)       // two CTAs resident per SM so that one loads while the other assembles
-#define BY_STAGE_CAP (48 * 1024)
 #define PLAN_TILE_WORDS 64
 #define PLAN_SCAN_CHUNK 4096
 
@@ -229,276 +227,14 @@ __device__ __forceinline__ void rows4(const BytesArgs &a, int64_t j0, int64_t be
   }
 }
 
-// CTA-wide exclusive scan of one u64 per thread (up to 1024 threads); returns the thread's exclusive
-// prefix, *total = the CTA total. Two barriers.
-__device__ __forceinline__ uint64_t cta_scan_excl(uint64_t v, uint64_t *warp_tot /* [33] shared */, uint64_t *total) {
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  uint64_t incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    const uint64_t y = __shfl_up_sync(ACU_FULL_MASK, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) warp_tot[wid] = incl;
-  __syncthreads();
-  if (wid == 0) {
-    const uint64_t w = lane < (int)(blockDim.x >> 5) ? warp_tot[lane] : 0ull;
-    uint64_t wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint64_t y = __shfl_up_sync(ACU_FULL_MASK, wi, o);
-      if (lane >= o) wi += y;
-    }
-    warp_tot[lane] = wi - w;
-    if (lane == 31) warp_tot[32] = wi;
-  }
-  __syncthreads();
-  *total = warp_tot[32];
-  return warp_tot[wid] + incl - v;
-}
-
-// pass 1: total value bytes of each CTA's 4096 rows (+ out-of-bounds detection)
+// The take / filter producer of bytes_engine.cuh.
 template <bool FAST>
-__global__ void __launch_bounds__(BY_THREADS) k_bytes_block_totals(const BytesArgs a, int64_t *__restrict__ block_tot,
-                                                             unsigned long long *__restrict__ res) {
-  __shared__ uint64_t warp_tot[32];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t j0 = (int64_t)blockIdx.x * BY_ROWS + (int64_t)threadIdx.x * 4;
-  int64_t begin[4];
-  uint64_t len[4];
-  unsigned long long err = ~0ull;
-  rows4<FAST>(a, j0, begin, len, &err);
-  uint64_t sum = len[0] + len[1] + len[2] + len[3];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(ACU_FULL_MASK, sum, o);
-  if (lane == 0) warp_tot[wid] = sum;
-  __syncthreads();
-  if (wid == 0) {
-    uint64_t t = lane < BY_THREADS / 32 ? warp_tot[lane] : 0ull;
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(ACU_FULL_MASK, t, o);
-    if (lane == 0) block_tot[blockIdx.x] = (int64_t)t;
-  }
-  if (a.detect_oob && err != ~0ull) atomicMin(res + RES_ERR_INDEX, err);
-}
-
-// Byte stream of one thread into the CTA's staging buffer: bytes are queued in a small
-// accumulator (fewer than 4 pending bytes between pushes) and leave as whole aligned 32-bit
-// words. A word shared with a neighbouring thread (the first one when the thread's output does
-// not start on a word boundary, and the last partial one) is merged with atomicOr into the
-// zero-initialised buffer; every other word is exclusively this thread's and is stored plainly.
-// push8 is branch-free apart from the two predicated stores.
-struct WordEmitter {
-  uint32_t *w;
-  uint32_t acc;   // pending bytes (low nacc bytes valid, rest zero)
-  uint32_t nacc;  // 0..3
-  bool shared_first;
-  __device__ __forceinline__ void init(uint8_t *stage, uint32_t pos) {
-    w = reinterpret_cast<uint32_t *>(stage) + (pos >> 2);
-    nacc = pos & 3u;
-    acc = 0;
-    shared_first = nacc != 0;
-  }
-  __device__ __forceinline__ void store(uint32_t v) {
-    if (shared_first) { atomicOr(w, v); shared_first = false; }
-    else *w = v;
-    ++w;
-  }
-  // v: up to 8 bytes (bytes at positions >= nb are zero), nb in 0..8
-  __device__ __forceinline__ void push8(uint64_t v, uint32_t nb) {
-    const uint32_t sh = nacc * 8u;                       // 0, 8, 16, 24
-    const uint32_t vlo = (uint32_t)v, vhi = (uint32_t)(v >> 32);
-    const uint32_t x0 = acc | (vlo << sh);
-    const uint32_t x1 = __funnelshift_l(vlo, vhi, sh);   // (vhi:vlo << sh) >> 32
-    const uint32_t x2 = __funnelshift_l(vhi, 0u, sh);    // bytes pushed past 64 bits (zero when sh == 0)
-    const uint32_t t = nacc + nb;                        // 0..11 bytes available
-    if (t >= 4u) store(x0);
-    if (t >= 8u) store(x1);
-    acc = t >= 8u ? x2 : (t >= 4u ? x1 : x0);
-    nacc = t & 3u;
-  }
-  // EXPERIMENT (off by default, -DACU_BYTES_PUSH16; DESIGN.md §9): a whole <= 16-byte row in one step — one 5-word
-  // shift instead of two 3-word ones. v = (w1:w0), bytes at positions >= nb are zero, nb in 0..16.
-  __device__ __forceinline__ void push16(uint64_t w0, uint64_t w1, uint32_t nb) {
-    const uint32_t sh = nacc * 8u;
-    const uint32_t v0 = (uint32_t)w0, v1 = (uint32_t)(w0 >> 32), v2 = (uint32_t)w1, v3 = (uint32_t)(w1 >> 32);
-    const uint32_t x0 = acc | (v0 << sh);
-    const uint32_t x1 = __funnelshift_l(v0, v1, sh);
-    const uint32_t x2 = __funnelshift_l(v1, v2, sh);
-    const uint32_t x3 = __funnelshift_l(v2, v3, sh);
-    const uint32_t x4 = __funnelshift_l(v3, 0u, sh);
-    const uint32_t t = nacc + nb;  // 0..19 bytes available
-    if (t >= 4u) store(x0);
-    if (t >= 8u) store(x1);
-    if (t >= 12u) store(x2);
-    if (t >= 16u) store(x3);
-    const uint32_t k = t >> 2;     // words that left
-    acc = k == 0u ? x0 : k == 1u ? x1 : k == 2u ? x2 : k == 3u ? x3 : x4;
-    nacc = t & 3u;
-  }
-  __device__ __forceinline__ void finish() {
-    if (acc != 0u) atomicOr(w, acc);
+struct GatherRows : BytesArgs {
+  static constexpr bool kVec4 = FAST;
+  __device__ __forceinline__ void ranges4(int64_t j0, int64_t begin[4], uint64_t len[4], unsigned long long *err) const {
+    rows4<FAST>(*this, j0, begin, len, err);
   }
 };
-
-// Up to 8 bytes of data[pos .. pos+nb) (nb in 0..8) as a little-endian u64, zero above nb. Only
-// aligned 8-byte words that contain at least one requested byte are read.
-__device__ __forceinline__ uint64_t load_upto8(const uint8_t *__restrict__ data, int64_t pos, uint32_t nb) {
-  const uintptr_t addr = (uintptr_t)data + (uintptr_t)pos;
-  const uint64_t *p = reinterpret_cast<const uint64_t *>(addr & ~(uintptr_t)7);
-  const uint32_t sh = (uint32_t)(addr & 7u) * 8u;
-  uint64_t lo = 0, hi = 0;
-  if (nb) lo = __ldg(p);
-  if (sh + nb * 8u > 64u) hi = __ldg(p + 1);
-  uint64_t w = (lo >> sh) | ((hi << 1) << (63u - sh));
-  const uint64_t mask = nb >= 8u ? ~0ull : ((1ull << (nb * 8u)) - 1ull);
-  return w & mask;
-}
-
-// The first nb (0..16) bytes of data[pos ..) as two little-endian u64 (zero above nb): three aligned
-// 8-byte loads, each predicated on containing a requested byte, shared by both halves.
-__device__ __forceinline__ void load_upto16(const uint8_t *__restrict__ data, int64_t pos, uint32_t nb, uint64_t *w0, uint64_t *w1) {
-  const uintptr_t addr = (uintptr_t)data + (uintptr_t)pos;
-  const uint64_t *p = reinterpret_cast<const uint64_t *>(addr & ~(uintptr_t)7);
-  const uint32_t sh = (uint32_t)(addr & 7u) * 8u, bits = sh + nb * 8u;
-  uint64_t x = 0, y = 0, z = 0;
-  if (nb) x = __ldg(p);
-  if (bits > 64u) y = __ldg(p + 1);
-  if (bits > 128u) z = __ldg(p + 2);
-  const uint64_t lo = (x >> sh) | ((y << 1) << (63u - sh));
-  const uint64_t hi = (y >> sh) | ((z << 1) << (63u - sh));
-  const uint32_t n0 = nb < 8u ? nb : 8u, n1 = nb - n0;
-  *w0 = lo & (n0 >= 8u ? ~0ull : ((1ull << (n0 * 8u)) - 1ull));
-  *w1 = hi & (n1 >= 8u ? ~0ull : ((1ull << (n1 * 8u)) - 1ull));
-}
-
-template <bool STAGED>
-__device__ __forceinline__ void copy_row_direct(uint8_t *__restrict__ dst, const uint8_t *__restrict__ data, int64_t src, uint64_t len) {
-  for (uint64_t c = 0; c < len; c += 8) {
-    const uint64_t w = ld_bits64(data, (src + (int64_t)c) << 3, (src + (int64_t)len) << 3);
-    const int nb = (int)((len - c) < 8 ? (len - c) : 8);
-#pragma unroll
-    for (int bidx = 0; bidx < 8; ++bidx)
-      if (bidx < nb) dst[c + bidx] = (uint8_t)(w >> (8 * bidx));
-  }
-}
-
-// pass 2 (after the inclusive scan of the CTA totals): offsets + byte copy. Source bytes are
-// fetched 8 at a time with two aligned loads + funnel shift (ld_bits64 on a byte position). The
-// CTA's output bytes [cta_begin, cta_end) are assembled in shared memory laid out relative to the
-// 16-B aligned global address and written back as whole 128-bit stores (STAGED); CTAs whose
-// output does not fit the staging buffer store bytes directly.
-template <bool FAST>
-__global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const BytesArgs a, const int64_t *__restrict__ block_incl,
-                                                             int64_t first_block, void *out_offs, uint8_t *__restrict__ out_data,
-                                                             int64_t limit, int64_t probe_row, unsigned long long *res,
-                                                             int stage_cap, const int64_t *__restrict__ total_ptr, int64_t out_cap) {
-  extern __shared__ __align__(16) uint8_t s_out[];
-  __shared__ uint64_t warp_tot[33];
-  // the byte copy is skipped (grid-uniformly) when the total does not fit the caller's buffer or
-  // the offset type: decided on the device so that no host round trip sits between the sizing
-  // pass and this one
-  if (out_data != nullptr && total_ptr != nullptr) {
-    const int64_t total = __ldg(total_ptr);
-    if (total > out_cap || total > limit) out_data = nullptr;
-  }
-  const int64_t blk = first_block + blockIdx.x;
-  const int64_t cta_begin = blk ? block_incl[blk - 1] : 0, cta_end = block_incl[blk];
-  const int64_t stage_origin = cta_begin - (int64_t)((uintptr_t)(out_data + cta_begin) & 15);  // global byte that maps to s_out[0]
-  const bool staged = out_data != nullptr && probe_row < 0 && (cta_end - stage_origin) <= (int64_t)stage_cap;
-  const uint32_t nbytes = staged ? (uint32_t)(cta_end - stage_origin) : 0u;  // staged span, starts 16-B aligned in global memory
-  const uint32_t lead = (uint32_t)(cta_begin - stage_origin);                // bytes of the first chunk owned by the previous CTA
-  if (staged) {  // zero the words the emitters OR into
-    const uint32_t chunks = (nbytes + 15) >> 4;
-    for (uint32_t c = threadIdx.x; c < chunks; c += BY_THREADS) reinterpret_cast<uint4 *>(s_out)[c] = make_uint4(0, 0, 0, 0);
-  }
-  const int64_t j0 = blk * BY_ROWS + (int64_t)threadIdx.x * 4;
-  int64_t begin[4];
-  uint64_t len[4];
-  unsigned long long oob = ~0ull;
-  rows4<FAST>(a, j0, begin, len, &oob);
-  uint64_t cta_total;
-  const uint64_t rel = cta_scan_excl(len[0] + len[1] + len[2] + len[3], warp_tot, &cta_total);  // also orders the zeroing before the emitters
-  int64_t end[4];
-  end[0] = cta_begin + (int64_t)(rel + len[0]);
-  end[1] = end[0] + (int64_t)len[1];
-  end[2] = end[1] + (int64_t)len[2];
-  end[3] = end[2] + (int64_t)len[3];
-  unsigned long long err = ~0ull;
-#pragma unroll
-  for (int k = 3; k >= 0; --k)
-    if (j0 + k < a.m && end[k] > limit) err = (unsigned long long)(j0 + k);
-  if (probe_row >= 0) {
-#pragma unroll
-    for (int k = 0; k < 4; ++k)
-      if (probe_row == j0 + k) res[RES_AUX1] = (unsigned long long)end[k];
-    return;
-  }
-  if (err != ~0ull) atomicMin(res + RES_ERR2, err);
-  // new offsets: out[j0] = end of the previous row, out[j0+1..j0+3] = the first three ends (one aligned 128-bit store);
-  // the thread holding the last row also writes out[m]
-  if (j0 <= a.m) {
-    const int64_t first = cta_begin + (int64_t)rel;
-    if (FAST && j0 + 3 <= a.m && ((uintptr_t)out_offs & 15) == 0) {
-      *reinterpret_cast<int4 *>(static_cast<int32_t *>(out_offs) + j0) = make_int4((int32_t)first, (int32_t)end[0], (int32_t)end[1], (int32_t)end[2]);
-    } else {
-#pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (j0 + k <= a.m) {
-          const int64_t v = k == 0 ? first : end[k - 1];
-          if (a.ob == 4) static_cast<int32_t *>(out_offs)[j0 + k] = (int32_t)v;
-          else static_cast<int64_t *>(out_offs)[j0 + k] = v;
-        }
-    }
-    if (j0 + 4 == a.m) {
-      if (a.ob == 4) static_cast<int32_t *>(out_offs)[a.m] = (int32_t)end[3];
-      else static_cast<int64_t *>(out_offs)[a.m] = end[3];
-    }
-  }
-  if (out_data == nullptr) return;  // grid-uniform
-  if (staged) {
-    WordEmitter em;
-    em.init(s_out, lead + (uint32_t)rel);
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      // the first 16 bytes of every row without branches (short strings are the common case) ...
-      const uint32_t l32 = len[k] > 16 ? 16u : (uint32_t)len[k];
-      const uint32_t n0 = l32 < 8u ? l32 : 8u, n1 = l32 - n0;
-      uint64_t w0, w1;
-      load_upto16(a.data, begin[k], l32, &w0, &w1);
-#ifdef ACU_BYTES_PUSH16
-      em.push16(w0, w1, l32);
-#else
-      em.push8(w0, n0);
-      em.push8(w1, n1);
-#endif
-      // ... the rest of a long row 8 bytes at a time
-      for (uint64_t c = 16; c < len[k]; c += 8) {
-        const uint32_t nb = (uint32_t)((len[k] - c) < 8 ? (len[k] - c) : 8);
-        em.push8(load_upto8(a.data, begin[k] + (int64_t)c, nb), nb);
-      }
-    }
-    em.finish();
-    __syncthreads();
-    uint8_t *g = out_data + stage_origin;
-    const uint32_t chunks = (nbytes + 15) >> 4;
-    for (uint32_t c = threadIdx.x; c < chunks; c += BY_THREADS) {
-      const uint32_t b0 = c << 4;
-      if (b0 >= lead && b0 + 16 <= nbytes) {
-        *reinterpret_cast<uint4 *>(g + b0) = *reinterpret_cast<const uint4 *>(s_out + b0);
-      } else {  // partial first / last chunk: only this CTA's bytes
-        for (uint32_t x = b0 < lead ? lead : b0; x < b0 + 16 && x < nbytes; ++x) g[x] = s_out[x];
-      }
-    }
-  } else {
-    int64_t pos = cta_begin + (int64_t)rel;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      if (len[k]) copy_row_direct<false>(out_data + pos, a.data, begin[k], len[k]);
-      pos += (int64_t)len[k];
-    }
-  }
-}
 
 // ---- dictionary gather: take_bytes from a SMALL source (Dictionary<Int32,Utf8> -> Utf8, cast/dictionary.rs:310-317) ----
 // A gather of 32 random dictionary rows through global memory costs 32 L1 wavefronts per load instruction whatever its
@@ -1090,8 +826,8 @@ acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const ui
       return ACU_OK;
     }
   }
-  if (fast) ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_block_totals<true>, (unsigned)blocks, BY_THREADS, 0, a, block_tot, res);
-  else ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_block_totals<false>, (unsigned)blocks, BY_THREADS, 0, a, block_tot, res);
+  if (fast) ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_block_totals<GatherRows<true>>, (unsigned)blocks, BY_THREADS, 0, GatherRows<true>{a}, block_tot, res);
+  else ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_block_totals<GatherRows<false>>, (unsigned)blocks, BY_THREADS, 0, GatherRows<false>{a}, block_tot, res);
   ACU_TRY(scan_inclusive(ctx, block_tot, blocks, block_tot + blocks));
   ACU_CUDA(ctx, cudaMemcpyAsync(res + RES_AUX0, block_tot + (blocks - 1), 8, cudaMemcpyDeviceToDevice, ctx->stream));
   const int stage_cap = BY_STAGE_CAP;
@@ -1104,12 +840,12 @@ acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const ui
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_gather_copy, acu_grid(ctx, blocks, per_sm), DG_THREADS, smem, a, block_tot, blocks, static_cast<int32_t *>(out_offsets),
                      out_data, limit, res, block_tot + (blocks - 1), out_cap);
   } else if (fast) {
-    ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
-    ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<true>, (unsigned)blocks, BY_THREADS, stage_cap, a, block_tot, (int64_t)0, out_offsets,
+    ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<GatherRows<true>>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
+    ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<GatherRows<true>>, (unsigned)blocks, BY_THREADS, stage_cap, GatherRows<true>{a}, block_tot, (int64_t)0, out_offsets,
                      out_data, limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
   } else {
-    ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
-    ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<false>, (unsigned)blocks, BY_THREADS, stage_cap, a, block_tot, (int64_t)0, out_offsets,
+    ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<GatherRows<false>>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
+    ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<GatherRows<false>>, (unsigned)blocks, BY_THREADS, stage_cap, GatherRows<false>{a}, block_tot, (int64_t)0, out_offsets,
                      out_data, limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
   }
   return ACU_OK;
@@ -1127,7 +863,7 @@ acu_status gather_finalize(acu_ctx *ctx, const acu_bytes_col_state &gs, const un
     const int64_t j = (int64_t)hres[RES_ERR2];
     const BytesArgs a{gs.offsets, gs.data, gs.idx, gs.kind, (int)gs.ob, gs.m, gs.n_src, reinterpret_cast<const uint32_t *>(gs.out_valid), 0};
     ACU_TRY(acu_res_reset(ctx));
-    ACU_LAUNCH(ctx, k_bytes_offsets_copy<false>, 1, BY_THREADS, 0, a, gs.block_tot, j / BY_ROWS, gs.out_offsets, static_cast<uint8_t *>(nullptr),
+    ACU_LAUNCH(ctx, k_bytes_offsets_copy<GatherRows<false>>, 1, BY_THREADS, 0, GatherRows<false>{a}, gs.block_tot, j / BY_ROWS, gs.out_offsets, static_cast<uint8_t *>(nullptr),
                INT64_MAX, j, ctx->d_res, 0, static_cast<const int64_t *>(nullptr), (int64_t)0);
     ACU_TRY(acu_res_fetch(ctx));
     const long long cap = (long long)ctx->h_res[RES_AUX1];

@@ -1,0 +1,293 @@
+// bytes_engine.cuh — the offsets-and-copy stage of the variable-width kernels: a producer gives each row's source byte
+// range, the engine sums them per CTA (k_bytes_block_totals), and after a device-wide scan of the CTA totals writes the new
+// offsets and copies the bytes (k_bytes_offsets_copy). take / filter (bytes.cu) and substring (substring.cu) differ only in
+// the producer.
+//
+// A producer `R` is a trivially copyable struct with
+//   static constexpr bool kVec4;  // i32 offsets whose new offsets may leave as one 128-bit store per thread
+//   int ob; int64_t m;            // offset width, output rows
+//   const uint8_t *data;          // the source value bytes the ranges point into
+//   int detect_oob;               // k_bytes_block_totals: *err of the first pass goes to res[RES_ERR_INDEX] (atomicMin)
+//   void ranges4(int64_t j0, int64_t begin[4], uint64_t len[4], unsigned long long *err) const;
+// where ranges4 gives the byte ranges of rows j0 .. j0+3 (zero length past m) and lowers *err to a failing row's key.
+#pragma once
+#include "common.cuh"
+
+#define BY_THREADS 512                 // CTA of the bytes kernels: 512 threads x 4 consecutive rows,
+#define BY_ROWS (BY_THREADS * 4)       // two CTAs resident per SM so that one loads while the other assembles
+#define BY_STAGE_CAP (48 * 1024)
+
+namespace {
+
+// CTA-wide exclusive scan of one u64 per thread (up to 1024 threads); returns the thread's exclusive
+// prefix, *total = the CTA total. Two barriers.
+__device__ __forceinline__ uint64_t cta_scan_excl(uint64_t v, uint64_t *warp_tot /* [33] shared */, uint64_t *total) {
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  uint64_t incl = v;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint64_t y = __shfl_up_sync(ACU_FULL_MASK, incl, o);
+    if (lane >= o) incl += y;
+  }
+  if (lane == 31) warp_tot[wid] = incl;
+  __syncthreads();
+  if (wid == 0) {
+    const uint64_t w = lane < (int)(blockDim.x >> 5) ? warp_tot[lane] : 0ull;
+    uint64_t wi = w;
+#pragma unroll
+    for (int o = 1; o < 32; o <<= 1) {
+      const uint64_t y = __shfl_up_sync(ACU_FULL_MASK, wi, o);
+      if (lane >= o) wi += y;
+    }
+    warp_tot[lane] = wi - w;
+    if (lane == 31) warp_tot[32] = wi;
+  }
+  __syncthreads();
+  *total = warp_tot[32];
+  return warp_tot[wid] + incl - v;
+}
+
+// pass 1: total value bytes of each CTA's 4096 rows (+ out-of-bounds detection)
+template <class R>
+__global__ void __launch_bounds__(BY_THREADS) k_bytes_block_totals(const R a, int64_t *__restrict__ block_tot,
+                                                             unsigned long long *__restrict__ res) {
+  __shared__ uint64_t warp_tot[32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int64_t j0 = (int64_t)blockIdx.x * BY_ROWS + (int64_t)threadIdx.x * 4;
+  int64_t begin[4];
+  uint64_t len[4];
+  unsigned long long err = ~0ull;
+  a.ranges4(j0, begin, len, &err);
+  uint64_t sum = len[0] + len[1] + len[2] + len[3];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sum += __shfl_xor_sync(ACU_FULL_MASK, sum, o);
+  if (lane == 0) warp_tot[wid] = sum;
+  __syncthreads();
+  if (wid == 0) {
+    uint64_t t = lane < BY_THREADS / 32 ? warp_tot[lane] : 0ull;
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(ACU_FULL_MASK, t, o);
+    if (lane == 0) block_tot[blockIdx.x] = (int64_t)t;
+  }
+  if (a.detect_oob && err != ~0ull) atomicMin(res + RES_ERR_INDEX, err);
+}
+
+// Byte stream of one thread into the CTA's staging buffer: bytes are queued in a small
+// accumulator (fewer than 4 pending bytes between pushes) and leave as whole aligned 32-bit
+// words. A word shared with a neighbouring thread (the first one when the thread's output does
+// not start on a word boundary, and the last partial one) is merged with atomicOr into the
+// zero-initialised buffer; every other word is exclusively this thread's and is stored plainly.
+// push8 is branch-free apart from the two predicated stores.
+struct WordEmitter {
+  uint32_t *w;
+  uint32_t acc;   // pending bytes (low nacc bytes valid, rest zero)
+  uint32_t nacc;  // 0..3
+  bool shared_first;
+  __device__ __forceinline__ void init(uint8_t *stage, uint32_t pos) {
+    w = reinterpret_cast<uint32_t *>(stage) + (pos >> 2);
+    nacc = pos & 3u;
+    acc = 0;
+    shared_first = nacc != 0;
+  }
+  __device__ __forceinline__ void store(uint32_t v) {
+    if (shared_first) { atomicOr(w, v); shared_first = false; }
+    else *w = v;
+    ++w;
+  }
+  // v: up to 8 bytes (bytes at positions >= nb are zero), nb in 0..8
+  __device__ __forceinline__ void push8(uint64_t v, uint32_t nb) {
+    const uint32_t sh = nacc * 8u;                       // 0, 8, 16, 24
+    const uint32_t vlo = (uint32_t)v, vhi = (uint32_t)(v >> 32);
+    const uint32_t x0 = acc | (vlo << sh);
+    const uint32_t x1 = __funnelshift_l(vlo, vhi, sh);   // (vhi:vlo << sh) >> 32
+    const uint32_t x2 = __funnelshift_l(vhi, 0u, sh);    // bytes pushed past 64 bits (zero when sh == 0)
+    const uint32_t t = nacc + nb;                        // 0..11 bytes available
+    if (t >= 4u) store(x0);
+    if (t >= 8u) store(x1);
+    acc = t >= 8u ? x2 : (t >= 4u ? x1 : x0);
+    nacc = t & 3u;
+  }
+  // EXPERIMENT (off by default, -DACU_BYTES_PUSH16; DESIGN.md §9): a whole <= 16-byte row in one step — one 5-word
+  // shift instead of two 3-word ones. v = (w1:w0), bytes at positions >= nb are zero, nb in 0..16.
+  __device__ __forceinline__ void push16(uint64_t w0, uint64_t w1, uint32_t nb) {
+    const uint32_t sh = nacc * 8u;
+    const uint32_t v0 = (uint32_t)w0, v1 = (uint32_t)(w0 >> 32), v2 = (uint32_t)w1, v3 = (uint32_t)(w1 >> 32);
+    const uint32_t x0 = acc | (v0 << sh);
+    const uint32_t x1 = __funnelshift_l(v0, v1, sh);
+    const uint32_t x2 = __funnelshift_l(v1, v2, sh);
+    const uint32_t x3 = __funnelshift_l(v2, v3, sh);
+    const uint32_t x4 = __funnelshift_l(v3, 0u, sh);
+    const uint32_t t = nacc + nb;  // 0..19 bytes available
+    if (t >= 4u) store(x0);
+    if (t >= 8u) store(x1);
+    if (t >= 12u) store(x2);
+    if (t >= 16u) store(x3);
+    const uint32_t k = t >> 2;     // words that left
+    acc = k == 0u ? x0 : k == 1u ? x1 : k == 2u ? x2 : k == 3u ? x3 : x4;
+    nacc = t & 3u;
+  }
+  __device__ __forceinline__ void finish() {
+    if (acc != 0u) atomicOr(w, acc);
+  }
+};
+
+// Up to 8 bytes of data[pos .. pos+nb) (nb in 0..8) as a little-endian u64, zero above nb. Only
+// aligned 8-byte words that contain at least one requested byte are read.
+__device__ __forceinline__ uint64_t load_upto8(const uint8_t *__restrict__ data, int64_t pos, uint32_t nb) {
+  const uintptr_t addr = (uintptr_t)data + (uintptr_t)pos;
+  const uint64_t *p = reinterpret_cast<const uint64_t *>(addr & ~(uintptr_t)7);
+  const uint32_t sh = (uint32_t)(addr & 7u) * 8u;
+  uint64_t lo = 0, hi = 0;
+  if (nb) lo = __ldg(p);
+  if (sh + nb * 8u > 64u) hi = __ldg(p + 1);
+  uint64_t w = (lo >> sh) | ((hi << 1) << (63u - sh));
+  const uint64_t mask = nb >= 8u ? ~0ull : ((1ull << (nb * 8u)) - 1ull);
+  return w & mask;
+}
+
+// The first nb (0..16) bytes of data[pos ..) as two little-endian u64 (zero above nb): three aligned
+// 8-byte loads, each predicated on containing a requested byte, shared by both halves.
+__device__ __forceinline__ void load_upto16(const uint8_t *__restrict__ data, int64_t pos, uint32_t nb, uint64_t *w0, uint64_t *w1) {
+  const uintptr_t addr = (uintptr_t)data + (uintptr_t)pos;
+  const uint64_t *p = reinterpret_cast<const uint64_t *>(addr & ~(uintptr_t)7);
+  const uint32_t sh = (uint32_t)(addr & 7u) * 8u, bits = sh + nb * 8u;
+  uint64_t x = 0, y = 0, z = 0;
+  if (nb) x = __ldg(p);
+  if (bits > 64u) y = __ldg(p + 1);
+  if (bits > 128u) z = __ldg(p + 2);
+  const uint64_t lo = (x >> sh) | ((y << 1) << (63u - sh));
+  const uint64_t hi = (y >> sh) | ((z << 1) << (63u - sh));
+  const uint32_t n0 = nb < 8u ? nb : 8u, n1 = nb - n0;
+  *w0 = lo & (n0 >= 8u ? ~0ull : ((1ull << (n0 * 8u)) - 1ull));
+  *w1 = hi & (n1 >= 8u ? ~0ull : ((1ull << (n1 * 8u)) - 1ull));
+}
+
+template <bool STAGED>
+__device__ __forceinline__ void copy_row_direct(uint8_t *__restrict__ dst, const uint8_t *__restrict__ data, int64_t src, uint64_t len) {
+  for (uint64_t c = 0; c < len; c += 8) {
+    const uint64_t w = ld_bits64(data, (src + (int64_t)c) << 3, (src + (int64_t)len) << 3);
+    const int nb = (int)((len - c) < 8 ? (len - c) : 8);
+#pragma unroll
+    for (int bidx = 0; bidx < 8; ++bidx)
+      if (bidx < nb) dst[c + bidx] = (uint8_t)(w >> (8 * bidx));
+  }
+}
+
+// pass 2 (after the inclusive scan of the CTA totals): offsets + byte copy. Source bytes are
+// fetched 8 at a time with two aligned loads + funnel shift (ld_bits64 on a byte position). The
+// CTA's output bytes [cta_begin, cta_end) are assembled in shared memory laid out relative to the
+// 16-B aligned global address and written back as whole 128-bit stores (STAGED); CTAs whose
+// output does not fit the staging buffer store bytes directly.
+template <class R>
+__global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a, const int64_t *__restrict__ block_incl,
+                                                             int64_t first_block, void *out_offs, uint8_t *__restrict__ out_data,
+                                                             int64_t limit, int64_t probe_row, unsigned long long *res,
+                                                             int stage_cap, const int64_t *__restrict__ total_ptr, int64_t out_cap) {
+  extern __shared__ __align__(16) uint8_t s_out[];
+  __shared__ uint64_t warp_tot[33];
+  // the byte copy is skipped (grid-uniformly) when the total does not fit the caller's buffer or
+  // the offset type: decided on the device so that no host round trip sits between the sizing
+  // pass and this one
+  if (out_data != nullptr && total_ptr != nullptr) {
+    const int64_t total = __ldg(total_ptr);
+    if (total > out_cap || total > limit) out_data = nullptr;
+  }
+  const int64_t blk = first_block + blockIdx.x;
+  const int64_t cta_begin = blk ? block_incl[blk - 1] : 0, cta_end = block_incl[blk];
+  const int64_t stage_origin = cta_begin - (int64_t)((uintptr_t)(out_data + cta_begin) & 15);  // global byte that maps to s_out[0]
+  const bool staged = out_data != nullptr && probe_row < 0 && (cta_end - stage_origin) <= (int64_t)stage_cap;
+  const uint32_t nbytes = staged ? (uint32_t)(cta_end - stage_origin) : 0u;  // staged span, starts 16-B aligned in global memory
+  const uint32_t lead = (uint32_t)(cta_begin - stage_origin);                // bytes of the first chunk owned by the previous CTA
+  if (staged) {  // zero the words the emitters OR into
+    const uint32_t chunks = (nbytes + 15) >> 4;
+    for (uint32_t c = threadIdx.x; c < chunks; c += BY_THREADS) reinterpret_cast<uint4 *>(s_out)[c] = make_uint4(0, 0, 0, 0);
+  }
+  const int64_t j0 = blk * BY_ROWS + (int64_t)threadIdx.x * 4;
+  int64_t begin[4];
+  uint64_t len[4];
+  unsigned long long oob = ~0ull;
+  a.ranges4(j0, begin, len, &oob);
+  uint64_t cta_total;
+  const uint64_t rel = cta_scan_excl(len[0] + len[1] + len[2] + len[3], warp_tot, &cta_total);  // also orders the zeroing before the emitters
+  int64_t end[4];
+  end[0] = cta_begin + (int64_t)(rel + len[0]);
+  end[1] = end[0] + (int64_t)len[1];
+  end[2] = end[1] + (int64_t)len[2];
+  end[3] = end[2] + (int64_t)len[3];
+  unsigned long long err = ~0ull;
+#pragma unroll
+  for (int k = 3; k >= 0; --k)
+    if (j0 + k < a.m && end[k] > limit) err = (unsigned long long)(j0 + k);
+  if (probe_row >= 0) {
+#pragma unroll
+    for (int k = 0; k < 4; ++k)
+      if (probe_row == j0 + k) res[RES_AUX1] = (unsigned long long)end[k];
+    return;
+  }
+  if (err != ~0ull) atomicMin(res + RES_ERR2, err);
+  // new offsets: out[j0] = end of the previous row, out[j0+1..j0+3] = the first three ends (one aligned 128-bit store);
+  // the thread holding the last row also writes out[m]
+  if (j0 <= a.m) {
+    const int64_t first = cta_begin + (int64_t)rel;
+    if (R::kVec4 && j0 + 3 <= a.m && ((uintptr_t)out_offs & 15) == 0) {
+      *reinterpret_cast<int4 *>(static_cast<int32_t *>(out_offs) + j0) = make_int4((int32_t)first, (int32_t)end[0], (int32_t)end[1], (int32_t)end[2]);
+    } else {
+#pragma unroll
+      for (int k = 0; k < 4; ++k)
+        if (j0 + k <= a.m) {
+          const int64_t v = k == 0 ? first : end[k - 1];
+          if (a.ob == 4) static_cast<int32_t *>(out_offs)[j0 + k] = (int32_t)v;
+          else static_cast<int64_t *>(out_offs)[j0 + k] = v;
+        }
+    }
+    if (j0 + 4 == a.m) {
+      if (a.ob == 4) static_cast<int32_t *>(out_offs)[a.m] = (int32_t)end[3];
+      else static_cast<int64_t *>(out_offs)[a.m] = end[3];
+    }
+  }
+  if (out_data == nullptr) return;  // grid-uniform
+  if (staged) {
+    WordEmitter em;
+    em.init(s_out, lead + (uint32_t)rel);
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      // the first 16 bytes of every row without branches (short strings are the common case) ...
+      const uint32_t l32 = len[k] > 16 ? 16u : (uint32_t)len[k];
+      const uint32_t n0 = l32 < 8u ? l32 : 8u, n1 = l32 - n0;
+      uint64_t w0, w1;
+      load_upto16(a.data, begin[k], l32, &w0, &w1);
+#ifdef ACU_BYTES_PUSH16
+      em.push16(w0, w1, l32);
+#else
+      em.push8(w0, n0);
+      em.push8(w1, n1);
+#endif
+      // ... the rest of a long row 8 bytes at a time
+      for (uint64_t c = 16; c < len[k]; c += 8) {
+        const uint32_t nb = (uint32_t)((len[k] - c) < 8 ? (len[k] - c) : 8);
+        em.push8(load_upto8(a.data, begin[k] + (int64_t)c, nb), nb);
+      }
+    }
+    em.finish();
+    __syncthreads();
+    uint8_t *g = out_data + stage_origin;
+    const uint32_t chunks = (nbytes + 15) >> 4;
+    for (uint32_t c = threadIdx.x; c < chunks; c += BY_THREADS) {
+      const uint32_t b0 = c << 4;
+      if (b0 >= lead && b0 + 16 <= nbytes) {
+        *reinterpret_cast<uint4 *>(g + b0) = *reinterpret_cast<const uint4 *>(s_out + b0);
+      } else {  // partial first / last chunk: only this CTA's bytes
+        for (uint32_t x = b0 < lead ? lead : b0; x < b0 + 16 && x < nbytes; ++x) g[x] = s_out[x];
+      }
+    }
+  } else {
+    int64_t pos = cta_begin + (int64_t)rel;
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+      if (len[k]) copy_row_direct<false>(out_data + pos, a.data, begin[k], len[k]);
+      pos += (int64_t)len[k];
+    }
+  }
+}
+
+}  // namespace

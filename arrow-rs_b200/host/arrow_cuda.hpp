@@ -1528,6 +1528,76 @@ ACU_LIKE_FN(eq_ignore_ascii_case, ACU_EQ_IGNORE_ASCII_CASE)
 #undef ACU_LIKE_FN
 }  // namespace like
 
+// ---- length / substring (arrow-string/src/length.rs, substring.rs) ----------------------------------------------
+// length / bit_length / substring on Utf8 (StringArray) and Utf8View (StringViewArray) arrays, substring_by_char on Utf8,
+// through acu_length_bytes / acu_length_byte_view / acu_substring_bytes / acu_substring_by_char / acu_substring_byte_view.
+// A view result shares the input's data buffers (a long value keeps its buffer index with an advanced offset); the
+// reference's StringViewBuilder copies it into new buffers, and the logical values are equal.
+namespace detail {
+inline Result<Int32Array> length_strings(acu_length_op op, const StringArray &a) {
+  Context &c = Context::get();
+  Buffer vb, nb;
+  const acu_bytes_array x = kernels::cmp::bytes_view(a, false);
+  acu_array_out o = make_out(vb, nb, (size_t)std::max<int64_t>(a.len(), 1) * 4, a.len());
+  const acu_status st = acu_length_bytes(c.raw(), 4, op, &x, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return Int32Array(vb, o.len, out_nulls(o, nb));
+}
+inline Result<Int32Array> length_views(acu_length_op op, const StringViewArray &a) {
+  Context &c = Context::get();
+  Buffer vb, nb;
+  const like::detail::ViewDesc x(a, false);
+  acu_array_out o = make_out(vb, nb, (size_t)std::max<int64_t>(a.len(), 1) * 4, a.len());
+  const acu_status st = acu_length_byte_view(c.raw(), op, &x.v, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return Int32Array(vb, o.len, out_nulls(o, nb));
+}
+// The two-phase byte-array call: the offsets and the byte count, then the bytes.
+template <class F>
+inline Result<StringArray> substring_two_phase(const StringArray &a, F call) {
+  Context &c = Context::get();
+  const acu_bytes_array x = kernels::cmp::bytes_view(a, false);
+  Buffer offs = Buffer::allocate((size_t)(a.len() + 1) * 4), nb = Buffer::allocate(acu_bitmap_bytes(std::max<int64_t>(a.len(), 1)));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  int64_t total = 0;
+  acu_status st = call(&x, offs.data(), nullptr, 0, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  Buffer data = Buffer::allocate((size_t)total);
+  st = call(&x, offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return StringArray(offs, data, o.len, out_nulls(o, nb));
+}
+}  // namespace detail
+inline Result<Int32Array> length(const StringArray &a) { return detail::length_strings(ACU_LENGTH, a); }
+inline Result<Int32Array> bit_length(const StringArray &a) { return detail::length_strings(ACU_BIT_LENGTH, a); }
+inline Result<Int32Array> length(const StringViewArray &a) { return detail::length_views(ACU_LENGTH, a); }
+inline Result<Int32Array> bit_length(const StringViewArray &a) { return detail::length_views(ACU_BIT_LENGTH, a); }
+
+// substring(array, start, length) (substring.rs:73-118); start / length count bytes.
+inline Result<StringArray> substring(const StringArray &a, int64_t start, std::optional<uint64_t> length = std::nullopt) {
+  const int64_t data_len = (int64_t)a.value_data().len();
+  return detail::substring_two_phase(a, [&](const acu_bytes_array *x, void *offs, uint8_t *data, int64_t cap, int64_t *total, acu_array_out *o) {
+    return acu_substring_bytes(Context::get().raw(), 4, 1, start, length.has_value(), length.value_or(0), x, data_len, offs, data, cap, total, o);
+  });
+}
+inline Result<StringViewArray> substring(const StringViewArray &a, int64_t start, std::optional<uint64_t> length = std::nullopt) {
+  Context &c = Context::get();
+  const like::detail::ViewDesc x(a, false);
+  Buffer views = Buffer::allocate((size_t)std::max<int64_t>(a.len(), 1) * 16), nb = Buffer::allocate(acu_bitmap_bytes(std::max<int64_t>(a.len(), 1)));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  const acu_status st = acu_substring_byte_view(c.raw(), 1, start, length.has_value(), length.value_or(0), &x.v, views.data(), &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return StringViewArray(views, 0, a.len(), a.data_buffers(), a.valid());  // null slots stay null
+}
+// substring_by_char(array, start, length) (substring.rs:144-165); start / length count chars.
+inline Result<StringArray> substring_by_char(const StringArray &a, int64_t start, std::optional<uint64_t> length = std::nullopt) {
+  return detail::substring_two_phase(a, [&](const acu_bytes_array *x, void *offs, uint8_t *data, int64_t cap, int64_t *total, acu_array_out *o) {
+    return acu_substring_by_char(Context::get().raw(), 4, start, length.has_value(), length.value_or(0), x, offs, data, cap, total, o);
+  });
+}
+
 
 // ---- nullif / zip (arrow-select/src/nullif.rs:44-113, zip.rs:99-226) -------------------------------------------
 namespace detail {

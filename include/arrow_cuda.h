@@ -463,6 +463,71 @@ acu_status acu_like_bytes(acu_ctx *ctx, int32_t offset_bytes, int32_t is_utf8, a
 acu_status acu_like_byte_view(acu_ctx *ctx, int32_t is_utf8, acu_like_op op, const acu_view_array *l,
                               const acu_view_array *r, acu_array_out *out);
 
+/* ------------------------------------------------------------------------- */
+/* length / substring — arrow-string/src/length.rs, substring.rs             */
+/* ------------------------------------------------------------------------- */
+typedef enum acu_length_op { ACU_LENGTH = 0, ACU_BIT_LENGTH = 1 } acu_length_op;
+/* length / bit_length (length.rs:26-200). The value is computed at EVERY slot, null slots included, and the result carries
+ * the input's NullBuffer as it is (nulls.cloned(): present iff nulls.validity != NULL, even without nulls), normalised to
+ * bit offset 0.
+ *   - acu_length_bytes: Utf8 / Binary (offset_bytes 4) give Int32, LargeUtf8 / LargeBinary (8) give Int64:
+ *     offsets[i+1] - offsets[i], wrapping; bit_length multiplies by 8, wrapping. out->values: len x offset_bytes bytes.
+ *   - acu_length_byte_view: Int32, the low 32 bits of each view (`*view as i32`; also for null views, whose bytes may be
+ *     anything); bit_length wrapping_mul(8). out->values: len x 4 bytes.
+ *   - acu_length_fixed_size_binary: Int32, byte_width (bit_length byte_width * 8, wrapping) at every slot; byte_width < 0
+ *     => ACU_ERR_INVALID_ARGUMENT.
+ * A scalar input or an op outside acu_length_op => ACU_ERR_INVALID_ARGUMENT. */
+acu_status acu_length_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_length_op op, const acu_bytes_array *a, acu_array_out *out);
+acu_status acu_length_byte_view(acu_ctx *ctx, acu_length_op op, const acu_view_array *a, acu_array_out *out);
+acu_status acu_length_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, acu_length_op op, const acu_array *a, acu_array_out *out);
+
+/* substring(array, start, length) (substring.rs:73-459): has_length = 0 is `None`, else `Some(length)`.
+ *
+ * acu_substring_bytes — byte_substring (:319-397) for Utf8 / LargeUtf8 (is_utf8 = 1) and Binary / LargeBinary (0).
+ *   `data_len` is the length of the whole value-data buffer `a->data` points at (value_data().len(), also for a slice).
+ *   - i32 offsets take `start as i32` and `length as i32` and add in i32, wrapping as in a release build; i64 offsets take
+ *     `length as i64`. Row i: new_start = min(offsets[i] + start, offsets[i+1]) for start > 0, offsets[i] for start == 0,
+ *     max(offsets[i+1] + start, offsets[i]) for start < 0; new_end = min(length + new_start, offsets[i+1]), or offsets[i+1].
+ *   - the rule runs at every slot, null slots included (a null slot keeps the substring of the bytes under it).
+ *   - Utf8 checks each new offset with is_char_boundary against the whole value-data buffer (offsets are absolute; the end
+ *     of the buffer is a boundary; a negative offset reads as its huge usize): new_start when start != 0, new_end when a
+ *     length is given, rows in order, start before end. The first failure is ACU_ERR_COMPUTE "The offset {offset} is at an
+ *     invalid utf-8 boundary." (detail.index = the row, lhs_bits = the offset).
+ *   - otherwise, where wrapping leaves a row whose slice data[new_start..new_end] is out of order or out of the buffer, the
+ *     reference panics: ACU_ERR_PANIC_OUT_OF_BOUNDS at the lowest such row, "slice index starts at {s} but ends at {e}" or
+ *     "range end index {e} out of range for slice of length {data_len}" (lhs_bits = s, rhs_bits = e as usize).
+ *   - out_offsets: len + 1 entries starting at 0 (also for a sliced input). Two-phase like acu_filter_bytes: out_data == NULL
+ *     writes only the offsets and *out_data_len; otherwise the bytes go to out_data (capacity out_data_capacity; too small
+ *     => ACU_ERR_INVALID_ARGUMENT, no byte written).
+ *   - out_nulls (validity capacity acu_bitmap_bytes(len)): NullBuffer::from_unsliced_buffer, so has_validity = 0 when the
+ *     input has no null (unlike length).
+ * acu_substring_by_char — substring_by_char (:144-251) for Utf8 / LargeUtf8: start and length count chars (utf8_bounds:
+ *   nth / nth_back for the start, nth for the end); null slots become empty; never fails. Output as acu_substring_bytes.
+ *   Both two-phase calls compute every row's range and run the offsets pass, the sizing call as well as the copy call.
+ * acu_substring_byte_view — string_view_substring / binary_view_substring (:254-317): null slots become all-zero views (as
+ *   append_null writes them); offsets are relative to the value (view_substring_range, length as i64); Utf8View
+ *   (is_utf8 = 1) checks both ends of every non-null row, and its error message gives the RELATIVE offset. A row whose slice
+ *   panics (length >= 2^63) => ACU_ERR_PANIC_OUT_OF_BOUNDS as above, relative to the value. out_views: 16 bytes per row,
+ *   16-byte aligned; out_nulls as the builder's: has_validity = 0 when the result has no null.
+ *   Buffer layout (differs on purpose from the reference's StringViewBuilder; the logical values are equal): a result of at
+ *   most 12 bytes is an inline view, zero padded; a longer one points into the INPUT's data buffers (same buffer_index,
+ *   offset advanced by new_start, the new 4-byte prefix), so the result shares a->buffers and no byte is copied.
+ * acu_substring_fixed_size_binary — fixed_size_binary_substring (:399-459): one output width *out_byte_width = new_len for
+ *   the whole column; row i = data[i*byte_width + new_start ..][..new_len], null rows too (out->values: len x new_len
+ *   bytes). Nulls as from_unsliced_buffer, except that new_len == 0 without nulls gives an all-valid NullBuffer.
+ * A scalar input, a negative byte_width or data_len, or an offset width other than 4 / 8 => ACU_ERR_INVALID_ARGUMENT.
+ * Synchronous (not available inside a stream-ordered section); kernel time is counted in ACU_K_BYTES. */
+acu_status acu_substring_bytes(acu_ctx *ctx, int32_t offset_bytes, int32_t is_utf8, int64_t start, int32_t has_length, uint64_t length,
+                               const acu_bytes_array *a, int64_t data_len, void *out_offsets, uint8_t *out_data,
+                               int64_t out_data_capacity, int64_t *out_data_len, acu_array_out *out_nulls);
+acu_status acu_substring_by_char(acu_ctx *ctx, int32_t offset_bytes, int64_t start, int32_t has_length, uint64_t length,
+                                 const acu_bytes_array *a, void *out_offsets, uint8_t *out_data, int64_t out_data_capacity,
+                                 int64_t *out_data_len, acu_array_out *out_nulls);
+acu_status acu_substring_byte_view(acu_ctx *ctx, int32_t is_utf8, int64_t start, int32_t has_length, uint64_t length,
+                                   const acu_view_array *a, void *out_views, acu_array_out *out_nulls);
+acu_status acu_substring_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, int64_t start, int32_t has_length, uint64_t length,
+                                           const acu_array *a, int32_t *out_byte_width, acu_array_out *out);
+
 /* Utf8View / BinaryView buffer management for BatchCoalescer (InProgressByteViewArray, arrow-select/src/coalesce/
  * byte_view.rs). The reference decides per source array whether its data buffers are compacted ("gc": when they hold more
  * than twice the bytes its views use, :366-381) and how output buffers are sized (BufferSource, :526-559); that policy stays

@@ -59,6 +59,9 @@ pub const ACU_CONTAINS: i32 = 4;
 pub const ACU_STARTS_WITH: i32 = 5;
 pub const ACU_ENDS_WITH: i32 = 6;
 pub const ACU_EQ_IGNORE_ASCII_CASE: i32 = 7;
+// acu_length_op (arrow-string/src/length.rs)
+pub const ACU_LENGTH: i32 = 0;
+pub const ACU_BIT_LENGTH: i32 = 1;
 pub const ACU_SUM: i32 = 0;
 pub const ACU_MIN: i32 = 1;
 pub const ACU_MAX: i32 = 2;
@@ -234,6 +237,19 @@ extern "C" {
                           out: *mut acu_array_out) -> acu_status;
     pub fn acu_like_byte_view(ctx: *mut acu_ctx, is_utf8: i32, op: i32, l: *const acu_view_array, r: *const acu_view_array,
                               out: *mut acu_array_out) -> acu_status;
+    pub fn acu_length_bytes(ctx: *mut acu_ctx, offset_bytes: i32, op: i32, a: *const acu_bytes_array, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_length_byte_view(ctx: *mut acu_ctx, op: i32, a: *const acu_view_array, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_length_fixed_size_binary(ctx: *mut acu_ctx, byte_width: i32, op: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_substring_bytes(ctx: *mut acu_ctx, offset_bytes: i32, is_utf8: i32, start: i64, has_length: i32, length: u64,
+                               a: *const acu_bytes_array, data_len: i64, out_offsets: *mut c_void, out_data: *mut u8, out_data_capacity: i64,
+                               out_data_len: *mut i64, out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_substring_by_char(ctx: *mut acu_ctx, offset_bytes: i32, start: i64, has_length: i32, length: u64, a: *const acu_bytes_array,
+                                 out_offsets: *mut c_void, out_data: *mut u8, out_data_capacity: i64, out_data_len: *mut i64,
+                                 out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_substring_byte_view(ctx: *mut acu_ctx, is_utf8: i32, start: i64, has_length: i32, length: u64, a: *const acu_view_array,
+                                   out_views: *mut c_void, out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_substring_fixed_size_binary(ctx: *mut acu_ctx, byte_width: i32, start: i64, has_length: i32, length: u64, a: *const acu_array,
+                                           out_byte_width: *mut i32, out: *mut acu_array_out) -> acu_status;
     pub fn acu_concat(ctx: *mut acu_ctx, n_arrays: i32, arrays: *const acu_column, out: *mut acu_column_out) -> acu_status;
     pub fn acu_concat_batches(ctx: *mut acu_ctx, n_batches: i32, n_columns: i32, columns: *const acu_column, outs: *mut acu_column_out,
                               out_rows: *mut i64) -> acu_status;

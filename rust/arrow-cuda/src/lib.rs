@@ -533,6 +533,186 @@ pub mod compute {
         }
     }
 
+    /// `arrow::compute::{length, bit_length}` (arrow-string/src/length.rs:26-200) and `substring`, `substring_by_char`
+    /// (arrow-string/src/substring.rs:73-251) on Utf8 / LargeUtf8 / Binary / LargeBinary, Utf8View / BinaryView and
+    /// FixedSizeBinary (`substring_by_char`: Utf8 / LargeUtf8). A view result shares the input's data buffers (long values keep
+    /// their buffer index with an advanced offset); the reference's builder copies them into new buffers, and the logical
+    /// values are equal. Dictionary and run-end-encoded inputs are not accepted here: apply to their values.
+    pub mod substring {
+        use super::super::{ffi, kind_of, ColumnOut, Context, DeviceArray, DeviceBuffer, Kind};
+        use arrow_array::cast::AsArray;
+        use arrow_array::types::ByteViewType;
+        use arrow_array::{make_array, Array, ArrayRef, GenericByteViewArray};
+        use arrow_buffer::{BooleanBuffer, NullBuffer, ScalarBuffer};
+        use arrow_data::ArrayData;
+        use arrow_schema::{ArrowError, DataType};
+        use std::sync::Arc;
+
+        fn bytes_operand(a: &DeviceArray) -> ffi::acu_bytes_array {
+            ffi::acu_bytes_array { offsets: a.view().values, data: a.column.data, nulls: *a.view() }
+        }
+
+        fn view_operand<T: ByteViewType + ?Sized>(ctx: &Context, a: &GenericByteViewArray<T>, bufs: &mut Vec<DeviceBuffer>,
+                                                  ptrs: &mut Vec<*const u8>) -> Result<ffi::acu_view_array, ArrowError> {
+            let (validity, validity_offset, null_count) = match a.nulls() {
+                Some(n) => {
+                    let b = DeviceBuffer::from_host(ctx, n.buffer().as_slice())?;
+                    let p = b.as_ptr() as *const u8;
+                    bufs.push(b);
+                    (p, n.offset() as i64, n.null_count() as i64)
+                }
+                None => (std::ptr::null(), 0, 0),
+            };
+            let v = DeviceBuffer::from_host(ctx, a.views().inner().as_slice())?;
+            let views = v.as_ptr();
+            bufs.push(v);
+            for d in a.data_buffers() {
+                let b = DeviceBuffer::from_host(ctx, d.as_slice())?;
+                ptrs.push(b.as_ptr() as *const u8);
+                bufs.push(b);
+            }
+            let nulls = ffi::acu_array { values: std::ptr::null(), values_offset: 0, validity, validity_offset, len: a.len() as i64, null_count,
+                                         is_scalar: 0, reserved: 0 };
+            Ok(ffi::acu_view_array { views, buffers: ptrs.as_ptr(), n_buffers: ptrs.len() as i32, reserved: 0, nulls })
+        }
+
+        fn fsb_operand(ctx: &Context, a: &dyn Array, width: usize, bufs: &mut Vec<DeviceBuffer>) -> Result<ffi::acu_array, ArrowError> {
+            let d = a.to_data();
+            let (validity, validity_offset, null_count) = match d.nulls() {
+                Some(n) => {
+                    let b = DeviceBuffer::from_host(ctx, n.buffer().as_slice())?;
+                    let p = b.as_ptr() as *const u8;
+                    bufs.push(b);
+                    (p, n.offset() as i64, n.null_count() as i64)
+                }
+                None => (std::ptr::null(), 0, 0),
+            };
+            let vals = DeviceBuffer::from_host(ctx, &d.buffers()[0].as_slice()[d.offset() * width..(d.offset() + d.len()) * width])?;
+            let values = vals.as_ptr();
+            bufs.push(vals);
+            Ok(ffi::acu_array { values, values_offset: 0, validity, validity_offset, len: d.len() as i64, null_count, is_scalar: 0, reserved: 0 })
+        }
+
+        fn length_op(op: i32, array: &dyn Array) -> Result<ArrayRef, ArrowError> {
+            use DataType::*;
+            let ctx = Context::current()?;
+            let out_type = if matches!(array.data_type(), LargeUtf8 | LargeBinary) { Int64 } else { Int32 };
+            let mut out = ColumnOut::new(&ctx, &out_type, array.len(), 0)?;
+            let st = match array.data_type() {
+                Utf8 | LargeUtf8 | Binary | LargeBinary => {
+                    let ob = if out_type == Int64 { 8 } else { 4 };
+                    let a = DeviceArray::upload(&ctx, array, false)?;
+                    unsafe { ffi::acu_length_bytes(ctx.raw(), ob, op, &bytes_operand(&a), out.array_out()) }
+                }
+                Utf8View | BinaryView => {
+                    let (mut bufs, mut ptrs) = (Vec::new(), Vec::new());
+                    let v = if array.data_type() == &Utf8View { view_operand(&ctx, array.as_string_view(), &mut bufs, &mut ptrs)? }
+                            else { view_operand(&ctx, array.as_binary_view(), &mut bufs, &mut ptrs)? };
+                    unsafe { ffi::acu_length_byte_view(ctx.raw(), op, &v, out.array_out()) }
+                }
+                FixedSizeBinary(w) => {
+                    let mut bufs = Vec::new();
+                    let a = fsb_operand(&ctx, array, *w as usize, &mut bufs)?;
+                    unsafe { ffi::acu_length_fixed_size_binary(ctx.raw(), *w, op, &a, out.array_out()) }
+                }
+                other => {
+                    let name = if op == ffi::ACU_LENGTH { "length" } else { "bit_length" };
+                    return Err(ArrowError::ComputeError(format!("{name} not supported for {other:?}")));
+                }
+            };
+            ctx.check(st)?;
+            out.finish(&out_type)
+        }
+        pub fn length(array: &dyn Array) -> Result<ArrayRef, ArrowError> { length_op(ffi::ACU_LENGTH, array) }
+        pub fn bit_length(array: &dyn Array) -> Result<ArrayRef, ArrowError> { length_op(ffi::ACU_BIT_LENGTH, array) }
+
+        /// The two-phase byte-array call: offsets and the byte count, then the bytes into a buffer of exactly that size.
+        fn two_phase(ctx: &Context, array: &dyn Array,
+                     call: &dyn Fn(&ffi::acu_bytes_array, *mut std::os::raw::c_void, *mut u8, i64, &mut i64, &mut ffi::acu_array_out) -> i32)
+                     -> Result<ArrayRef, ArrowError> {
+            let a = DeviceArray::upload(ctx, array, false)?;
+            let x = bytes_operand(&a);
+            let mut sizing = ColumnOut::new(ctx, array.data_type(), array.len(), 0)?;
+            let mut total = 0i64;
+            ctx.check(call(&x, sizing.out.array.values, std::ptr::null_mut(), 0, &mut total, &mut sizing.out.array))?;
+            let mut out = ColumnOut::new(ctx, array.data_type(), array.len(), total as usize)?;
+            let (offs, data, cap) = (out.out.array.values, out.out.data, out.out.data_capacity);
+            ctx.check(call(&x, offs, data, cap, &mut out.out.data_len, &mut out.out.array))?;
+            out.finish(array.data_type())
+        }
+
+        fn view_substring<T: ByteViewType + ?Sized>(ctx: &Context, a: &GenericByteViewArray<T>, is_utf8: i32, start: i64, has_len: i32,
+                                                    len: u64) -> Result<ArrayRef, ArrowError> {
+            let (mut bufs, mut ptrs) = (Vec::new(), Vec::new());
+            let v = view_operand(ctx, a, &mut bufs, &mut ptrs)?;
+            let out_views = DeviceBuffer::allocate(ctx, a.len().max(1) * 16)?;
+            let validity = DeviceBuffer::allocate(ctx, super::super::bitmap_bytes(a.len().max(1)))?;
+            let mut o = ffi::acu_array_out { values: out_views.as_ptr(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0,
+                                             has_validity: 0, reserved: 0 };
+            ctx.check(unsafe { ffi::acu_substring_byte_view(ctx.raw(), is_utf8, start, has_len, len, &v, out_views.as_ptr(), &mut o) })?;
+            let n = a.len();
+            let nulls = if o.has_validity != 0 {
+                let bits = BooleanBuffer::new(validity.to_host(super::super::bitmap_bytes(n))?, 0, n);
+                Some(unsafe { NullBuffer::new_unchecked(bits, o.null_count as usize) })
+            } else { None };
+            let views = ScalarBuffer::<u128>::new(out_views.to_host(n * 16)?, 0, n);
+            // long results point into the input's buffers: the result keeps them
+            Ok(Arc::new(unsafe { GenericByteViewArray::<T>::new_unchecked(views, a.data_buffers().to_vec(), nulls) }))
+        }
+
+        /// `substring(array, start, length)` (substring.rs:73-118).
+        pub fn substring(array: &dyn Array, start: i64, length: Option<u64>) -> Result<ArrayRef, ArrowError> {
+            use DataType::*;
+            let ctx = Context::current()?;
+            let (has_len, len) = (length.is_some() as i32, length.unwrap_or(0));
+            match array.data_type() {
+                Utf8 | LargeUtf8 | Binary | LargeBinary => {
+                    let ob = match kind_of(array.data_type())? { Kind::Bytes(ob) => ob as i32, _ => unreachable!() };
+                    let is_utf8 = matches!(array.data_type(), Utf8 | LargeUtf8) as i32;
+                    let data_len = array.to_data().buffers()[1].len() as i64;
+                    two_phase(&ctx, array, &|x, offs, data, cap, total, nulls| unsafe {
+                        ffi::acu_substring_bytes(ctx.raw(), ob, is_utf8, start, has_len, len, x, data_len, offs, data, cap, total, nulls)
+                    })
+                }
+                Utf8View => view_substring(&ctx, array.as_string_view(), 1, start, has_len, len),
+                BinaryView => view_substring(&ctx, array.as_binary_view(), 0, start, has_len, len),
+                FixedSizeBinary(w) => {
+                    let mut bufs = Vec::new();
+                    let a = fsb_operand(&ctx, array, *w as usize, &mut bufs)?;
+                    let n = array.len();
+                    let values = DeviceBuffer::allocate(&ctx, (n * *w as usize).max(1))?;
+                    let validity = DeviceBuffer::allocate(&ctx, super::super::bitmap_bytes(n.max(1)))?;
+                    let mut o = ffi::acu_array_out { values: values.as_ptr(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0,
+                                                     has_validity: 0, reserved: 0 };
+                    let mut new_len = 0i32;
+                    ctx.check(unsafe { ffi::acu_substring_fixed_size_binary(ctx.raw(), *w, start, has_len, len, &a, &mut new_len, &mut o) })?;
+                    let nulls = if o.has_validity != 0 {
+                        let bits = BooleanBuffer::new(validity.to_host(super::super::bitmap_bytes(n))?, 0, n);
+                        Some(unsafe { NullBuffer::new_unchecked(bits, o.null_count as usize) })
+                    } else { None };
+                    let d = ArrayData::builder(FixedSizeBinary(new_len)).len(n).nulls(nulls)
+                        .add_buffer(values.to_host(n * new_len as usize)?);
+                    Ok(make_array(unsafe { d.build_unchecked() }))
+                }
+                other => Err(ArrowError::ComputeError(format!("substring does not support type {other:?}"))),
+            }
+        }
+
+        /// `substring_by_char(array, start, length)` (substring.rs:144-165) for Utf8 / LargeUtf8.
+        pub fn substring_by_char(array: &dyn Array, start: i64, length: Option<u64>) -> Result<ArrayRef, ArrowError> {
+            let ctx = Context::current()?;
+            let ob = match array.data_type() {
+                DataType::Utf8 => 4,
+                DataType::LargeUtf8 => 8,
+                other => return Err(ArrowError::ComputeError(format!("substring_by_char does not support type {other:?}"))),
+            };
+            let (has_len, len) = (length.is_some() as i32, length.unwrap_or(0));
+            two_phase(&ctx, array, &|x, offs, data, cap, total, nulls| unsafe {
+                ffi::acu_substring_by_char(ctx.raw(), ob, start, has_len, len, x, offs, data, cap, total, nulls)
+            })
+        }
+    }
+
     pub mod aggregate {
         use super::super::{ffi, Context, DeviceArray, DeviceBuffer};
         use arrow_array::types::{BinaryViewType, ByteViewType, StringViewType};

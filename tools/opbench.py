@@ -225,6 +225,9 @@ def main():
         # ---------------- like family (arrow-string/src/like.rs) ----------------
         if not b.only or any(t in "like starts_with ends_with contains cmp_bytes cmp_byte_view" for t in b.only.split("|")):
             like_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D)
+        # ---------------- length / substring (arrow-string/src/length.rs, substring.rs) ----------------
+        if not b.only or any(t in "substring length" for t in b.only.split("|")):
+            substring_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D)
     print("\n| op | rows | kernel ms | GB/s (algorithmic) | % of measured HBM peak | Mrows/s |")
     print("|---|---|---|---|---|---|")
     for r in b.rows:
@@ -373,6 +376,53 @@ def agg_bytes_rows(b, ctx, ns, d_off, d_data, dkeys, keys, dict_nulls, d_out_off
     val = C.c_int32(0)
     b.timed("bool_and 1e9", [abi.K_REDUCE], 2 * n / 8, n, lambda: ctx.check(lib.acu_aggregate_boolean(h, abi.MIN, C.byref(BA), C.byref(val), C.byref(cnt))))
     ctx.free(bv)
+
+
+def substring_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D):
+    """length, substring(s, 1, 3), substring(s, -4, None), substring_by_char(s, 1, 3) on the dictionary-decoded Utf8 column of
+    config 4 (D = 4096 values of 4..12 bytes, 5 % nulls) and the view forms on the same values as all-inline views.
+    Algorithmic bytes (DESIGN.md §3): length = 4(N+1) + 4N + 2N/8; byte substring = 4(N+1) + 4(N+1) + 2S + 2N/8 with S the
+    selected bytes (the Utf8 boundary bytes are not counted); view substring = 16N + 16N + 2N/8 (every value is inline).
+    A byte substring is timed as the two calls a caller makes: the sizing call, then the copy."""
+    lib, h = ctx.lib, ctx.h
+    total = C.c_int64(0)
+    ctx.check(lib.acu_take_bytes(h, 4, d_off, d_data, C.byref(dict_nulls), C.byref(keys), abi.I32, 0, d_out_off, d_out_data, ns * 13,
+                                 C.byref(total), C.byref(on)))
+    U = abi.BytesArray()
+    U.offsets, U.data = d_out_off, d_out_data
+    U.nulls = b.arr(None, on.validity, ns, on.null_count)
+    data_len = total.value
+    V, ovw = dict_view_column(b, ctx, keys, offs, data, D, ns)
+    ol = b.out(ns * 4, ns)
+    b.timed("substring: length utf8 dict-decoded", [abi.K_BYTES], 4 * (ns + 1) + 4 * ns + 2 * ns / 8, ns,
+            lambda: ctx.check(lib.acu_length_bytes(h, 4, abi.LENGTH, C.byref(U), C.byref(ol))), note=f"D={D}, lengths 4..12, 5% nulls")
+    b.timed("substring: length view inline dict-decoded", [abi.K_BYTES], 16 * ns + 4 * ns + 2 * ns / 8, ns,
+            lambda: ctx.check(lib.acu_length_byte_view(h, abi.LENGTH, C.byref(V), C.byref(ol))), note="reads the length word of each view")
+    so_off, so_data = ctx.malloc((ns + 1) * 4 + 64), ctx.malloc(data_len + 64)
+    onn = abi.ArrayOut()
+    onn.validity = ctx.malloc(abi.bitmap_bytes(ns) + 64)
+    sel = C.c_int64(0)
+    for name, by_char, start, has_len, ln in [("substring(s, 1, 3)", False, 1, 1, 3), ("substring(s, -4, None)", False, -4, 0, 0),
+                                              ("substring_by_char(s, 1, 3)", True, 1, 1, 3)]:
+        def call(cap, out, by_char=by_char, start=start, has_len=has_len, ln=ln):
+            if by_char:
+                ctx.check(lib.acu_substring_by_char(h, 4, start, has_len, ln, C.byref(U), so_off, out, cap, C.byref(sel), C.byref(onn)))
+            else:
+                ctx.check(lib.acu_substring_bytes(h, 4, 1, start, has_len, ln, C.byref(U), data_len, so_off, out, cap, C.byref(sel), C.byref(onn)))
+        call(0, None)
+        s_bytes = sel.value
+        b.timed(f"substring: {name} utf8 dict-decoded", [abi.K_BYTES], 8 * (ns + 1) + 2 * s_bytes + 2 * ns / 8, ns,
+                lambda call=call: (call(0, None), call(data_len, so_data)), note=f"sizing + copy call; S = {s_bytes} selected bytes")
+    ovs = b.out(ns * 16, ns)
+    for name, start, has_len, ln in [("substring(s, 1, 3)", 1, 1, 3), ("substring(s, -4, None)", -4, 0, 0)]:
+        b.timed(f"substring: {name} view inline dict-decoded", [abi.K_BYTES], 32 * ns + 2 * ns / 8, ns,
+                lambda start=start, has_len=has_len, ln=ln: ctx.check(lib.acu_substring_byte_view(h, 1, start, has_len, ln, C.byref(V), ovs.values, C.byref(ovs))),
+                note="views only (all values inline)")
+    for p in (so_off, so_data, onn.validity):
+        ctx.free(p)
+    ctx._free_out(ol)
+    ctx._free_out(ovs)
+    ctx._free_out(ovw)
 
 
 def like_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D):
