@@ -102,13 +102,14 @@ def shapes():
 
 
 # ---- acu_cmp and acu_filter_plan_create_cmp ------------------------------------------------------------------------------
-def gpu_filter_cmp(gpu, dtype, op, ad, bd, vd):
+def gpu_filter_cmp(gpu, dtype, op, ad, bd, vd, vdtype=abi.I64):
     plan = C.c_void_p()
     gpu.check(gpu.lib.acu_filter_plan_create_cmp(gpu.h, dtype, op, C.byref(ad), C.byref(bd), C.byref(plan)))
     try:
         count = gpu.lib.acu_filter_plan_count(plan)
-        res = call_out(gpu, count * 8, count, abi.I64,
-                       lambda out: gpu.lib.acu_filter_primitive(gpu.h, plan, 8, C.byref(vd), C.byref(out)))
+        w = abi.DTYPE_SIZE[vdtype]
+        res = call_out(gpu, count * w, count, vdtype,
+                       lambda out: gpu.lib.acu_filter_primitive(gpu.h, plan, w, C.byref(vd), C.byref(out)))
         return res, (count, gpu.lib.acu_filter_plan_strategy(plan))
     finally:
         gpu.lib.acu_filter_plan_destroy(gpu.h, plan)
