@@ -1407,6 +1407,39 @@ class Context:
                 self._free_out(out)
             da.free()
 
+    # -- decimal casts (arrow-cast/src/cast/decimal.rs) -------------------------------------------
+    def cast_decimal(self, a, byte_width, precision, scale, safe=True):
+        """cast(DecimalArray, Decimal{32,64,128}(precision, scale)) -> DecimalArray."""
+        ft, tt = abi.DecimalType(a.byte_width, a.precision, a.scale), abi.DecimalType(byte_width, precision, scale)
+        res = self._cast_call(a, byte_width, lambda ad, out: self.lib.acu_cast_decimal(self.h, C.byref(ft), C.byref(tt), int(safe),
+                                                                                     C.byref(ad), C.byref(out)), _DECIMAL_NATIVE[byte_width])
+        return DecimalArray(byte_width, precision, scale, res.values, res.length, res.validity, res.validity_offset, res.null_count)
+
+    def cast_to_decimal(self, a, byte_width, precision, scale, safe=True):
+        """cast(Int8..UInt64 / Float32 / Float64 HostArray, Decimal{32,64,128}(precision, scale)) -> DecimalArray."""
+        tt = abi.DecimalType(byte_width, precision, scale)
+        res = self._cast_call(a, byte_width, lambda ad, out: self.lib.acu_cast_to_decimal(self.h, a.dtype, C.byref(tt), int(safe),
+                                                                                        C.byref(ad), C.byref(out)), _DECIMAL_NATIVE[byte_width])
+        return DecimalArray(byte_width, precision, scale, res.values, res.length, res.validity, res.validity_offset, res.null_count)
+
+    def cast_from_decimal(self, a, to_dtype, safe=True):
+        """cast(DecimalArray, Int8..UInt64 / Float32 / Float64) -> HostArray."""
+        ft = abi.DecimalType(a.byte_width, a.precision, a.scale)
+        return self._cast_call(a, abi.DTYPE_SIZE[to_dtype], lambda ad, out: self.lib.acu_cast_from_decimal(
+            self.h, C.byref(ft), to_dtype, int(safe), C.byref(ad), C.byref(out)), to_dtype)
+
+    def _cast_call(self, a, out_width, call, out_dtype):
+        da = self.upload(a)
+        out = self.alloc_out(a.length * out_width, a.length)
+        try:
+            self.check(call(da.descriptor(), out))
+            res, out = self.download_out(out, out_dtype), None
+            return res
+        finally:
+            if out is not None:
+                self._free_out(out)
+            da.free()
+
     # -- aggregate (arrow-arith/src/aggregate.rs) ----------------------------------------------
     def aggregate(self, op, a):
         if a.dtype == abi.I128:

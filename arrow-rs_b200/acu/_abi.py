@@ -225,6 +225,9 @@ PROTOTYPES = {
     "acu_substring_byte_view": (i32, [vp, i32, i64, i32, u64, P(ViewArray), vp, P(ArrayOut)]),
     "acu_substring_fixed_size_binary": (i32, [vp, i32, i64, i32, u64, P(Array), P(i32), P(ArrayOut)]),
     "acu_cast_numeric": (i32, [vp, i32, i32, i32, P(Array), P(ArrayOut)]),
+    "acu_cast_decimal": (i32, [vp, P(DecimalType), P(DecimalType), i32, P(Array), P(ArrayOut)]),
+    "acu_cast_to_decimal": (i32, [vp, i32, P(DecimalType), i32, P(Array), P(ArrayOut)]),
+    "acu_cast_from_decimal": (i32, [vp, P(DecimalType), i32, i32, P(Array), P(ArrayOut)]),
     "acu_boolean": (i32, [vp, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_aggregate": (i32, [vp, i32, i32, P(Array), P(u64), P(i64)]),
     "acu_aggregate_i128": (i32, [vp, i32, P(Array), P(u64), P(i64)]),

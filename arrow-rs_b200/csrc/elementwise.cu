@@ -13,9 +13,13 @@
 // unaligned slices. Warp 0 finishes the ragged tail (< 2048 rows) in 64-row strips after
 // its super-groups, so each call is one launch.
 #include <stdio.h>
+#include <stdlib.h>
+#include <string.h>
 
 #include <algorithm>
+#include <cmath>
 #include <limits>
+#include <string>
 #include <type_traits>
 
 #include "bitmap.cuh"
@@ -146,9 +150,7 @@ __device__ __forceinline__ bool apply_op(int op, T l, T r, T &o) {
 // (arithmetic.rs:148-300). Under strict C++17 std::is_signed / make_unsigned do not cover __int128, hence own traits.
 // Host and device share these functions: the error finaliser replays the failing row with them.
 // ---------------------------------------------------------------------------------------
-template <class T> struct dec_unsigned;
-template <> struct dec_unsigned<int32_t> { using type = uint32_t; };
-template <> struct dec_unsigned<int64_t> { using type = uint64_t; };
+template <class T> struct dec_unsigned { using type = typename std::make_unsigned<T>::type; };
 template <> struct dec_unsigned<__int128> { using type = unsigned __int128; };
 template <class T> __host__ __device__ __forceinline__ T dec_min() {
   return (T)((typename dec_unsigned<T>::type)1 << (8 * sizeof(T) - 1));
@@ -865,9 +867,30 @@ acu_status cmp_typed(acu_ctx *ctx, acu_cmp_op op, const acu_array *l, const acu_
 // ---------------------------------------------------------------------------------------
 // cast (numeric): unary_opt / try_unary over num_traits::cast (num-traits 0.2.19)
 // ---------------------------------------------------------------------------------------
+__host__ __device__ __forceinline__ int clz64(uint64_t x) {
+#ifdef __CUDA_ARCH__
+  return __clzll((long long)x);
+#else
+  return x ? __builtin_clzll(x) : 64;
+#endif
+}
+// An integral double with |v| < 2^127 as i128 (exact: the value has at most 53 significant bits).
+__host__ __device__ __forceinline__ __int128 f64_to_i128(double v) {
+  if (v > -9.2e18 && v < 9.2e18) return (__int128)(int64_t)v;
+  int e;
+  const double fr = frexp(fabs(v), &e);  // |v| = fr * 2^e, fr in [0.5, 1), e >= 63 > 53
+  const unsigned __int128 m = (unsigned __int128)(uint64_t)ldexp(fr, 53) << (e - 53);
+  return v < 0 ? (__int128)((unsigned __int128)0 - m) : (__int128)m;
+}
+
 template <class I, class O>
-__device__ __forceinline__ bool num_cast(I v, O &o) {
-  if constexpr (is_fp<O>::value) {
+__host__ __device__ __forceinline__ bool num_cast(I v, O &o) {
+  if constexpr (sizeof(O) == 16) {  // f64 -> i128 (num_traits to_i128): -2^127 <= v < 2^127
+    static_assert(is_fp<I>::value, "integer -> i128 is a widening, not a num_cast");
+    if (!(v >= -1.7014118346046923e38 && v < 1.7014118346046923e38)) return false;
+    o = f64_to_i128((double)v);
+    return true;
+  } else if constexpr (is_fp<O>::value) {
     o = (O)v;  // cvt.rn: int->float RNE, f64->f32 RNE (overflow -> inf), always Some
     return true;
   } else if constexpr (is_fp<I>::value) {
@@ -1132,6 +1155,567 @@ acu_status decimal_typed(acu_ctx *ctx, acu_arith_op op, const acu_decimal_type &
   return arith_typed<T, true>(ctx, op, a, b, out, &d);
 }
 
+// ---------------------------------------------------------------------------------------
+// Decimal casts (arrow-cast/src/cast/decimal.rs:161-529, :836-1004; mod.rs:86-92, :366-444). One row function per kind,
+// shared by the device and the host replay of a failing row. Every per-call constant (10^k, the rounding half, the output
+// precision's bounds, the powi multiplier) is computed once on the host.
+// ---------------------------------------------------------------------------------------
+enum { DK_DEC = 0, DK_INT = 1, DK_FLOAT = 2, DK_TO_INT = 3, DK_TO_FLOAT = 4 };  // decimal / integer / float -> decimal, decimal -> integer / float
+enum { DM_UNARY = 0, DM_OPT = 1, DM_TRY = 2 };  // unary (every slot; a failure is the unwrap panic), unary_opt / builder (valid slots; failure -> null), try_unary (valid slots; failure -> error)
+enum { DR_OK = 0, DR_NONE = 1, DR_MUL = 2, DR_PRECISION = 3 };  // row outcome: the conversion returned None / the checked multiply failed / outside the output precision
+
+struct DcastArgs {
+  __int128 k;       // 10^delta: the multiplier or divisor, in the native that applies it
+  __int128 half;    // k / 2 (downscale rounding)
+  __int128 lo, hi;  // MIN / MAX_FOR_EACH_PRECISION[p_out]; lo > hi when p_out exceeds MAX_PRECISION (nothing fits)
+  double fk;        // 10_f64.powi(scale)
+  uint32_t chunk[5];  // k = product of these powers of ten (each <= 10^9): the full-width i128 division
+  int nchunk;
+  int down;   // DK_DEC: divide by k and round; DK_INT / DK_TO_INT: divide by k (else multiply)
+  int zero;   // the all-zero shortcuts
+  int wrap;   // the infallible upscale multiplies wrapping
+  int check;  // is_valid_decimal_precision after the conversion
+};
+
+// O::from_decimal / NumCast / integer_to_decimal_native: does the (integral) value fit O?
+template <class O, class T> __host__ __device__ __forceinline__ bool fits_in(T v) {
+  if constexpr (sizeof(O) == 16) return true;  // every source native fits i128
+  else if constexpr (sizeof(T) == 16) {
+    if constexpr (std::is_signed<O>::value)
+      return v >= (__int128)std::numeric_limits<O>::min() && v <= (__int128)std::numeric_limits<O>::max();
+    else return v >= 0 && v <= (__int128)std::numeric_limits<O>::max();
+  } else {
+    O o;
+    return num_cast<T, O>(v, o);
+  }
+}
+
+// u128 / d for d < 2^32: long division over 32-bit limbs, three 64-bit divisions.
+__host__ __device__ __forceinline__ unsigned __int128 udiv_u32(unsigned __int128 x, uint32_t d) {
+  const uint64_t hi = (uint64_t)(x >> 64), lo = (uint64_t)x;
+  const uint64_t qh = hi / d;
+  uint64_t t = ((hi % d) << 32) | (lo >> 32);
+  const uint64_t q1 = t / d;
+  t = ((t % d) << 32) | (lo & 0xffffffffull);
+  return ((unsigned __int128)qh << 64) | (q1 << 32) | (t / d);
+}
+
+// Magnitude quotient and remainder by k = 10^delta. A value below 2^64 with k below 2^64 takes one 64-bit division; a
+// full-width i128 is divided by k's <= 10^9 factors in turn (floor(floor(x / a) / b) = floor(x / ab)).
+template <class I>
+__host__ __device__ __forceinline__ void udivmod_k(typename dec_unsigned<I>::type m, const DcastArgs &a, typename dec_unsigned<I>::type &q,
+                                                   typename dec_unsigned<I>::type &r) {
+  using U = typename dec_unsigned<I>::type;
+  const U k = (U)a.k;
+  if constexpr (sizeof(I) == 16) {
+    if ((m >> 64) == 0 && (k >> 64) == 0) {
+      q = (uint64_t)m / (uint64_t)k;
+    } else {
+      q = m;
+      for (int c = 0; c < a.nchunk; ++c) q = udiv_u32(q, a.chunk[c]);
+    }
+  } else {
+    q = m / k;
+  }
+  r = m - q * k;
+}
+
+__host__ __device__ __forceinline__ double i128_to_f64(__int128 v) {  // `as f64`: round to nearest, ties to even
+  const int64_t v64 = (int64_t)v;
+  if ((__int128)v64 == v) return (double)v64;
+  using U = unsigned __int128;
+  const U m = v < 0 ? (U)0 - (U)v : (U)v;
+  const int bits = 128 - clz64((uint64_t)(m >> 64));  // >= 64
+  const int sh = bits - 64;
+  // the top 64 bits with every lower bit folded into a sticky bit 0: one RNE conversion rounds exactly as the whole value
+  uint64_t top = (uint64_t)(m >> sh);
+  if (sh > 0 && (m & ((U(1) << sh) - 1)) != 0) top |= 1;
+  const double d = ldexp((double)top, sh);
+  return v < 0 ? -d : d;
+}
+__host__ __device__ __forceinline__ double dmul_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __dmul_rn(a, b);
+#else
+  return a * b;
+#endif
+}
+__host__ __device__ __forceinline__ double ddiv_rn(double a, double b) {
+#ifdef __CUDA_ARCH__
+  return __ddiv_rn(a, b);
+#else
+  return a / b;
+#endif
+}
+
+// One row. `mid` receives the value a message prints: the narrowed value whose multiply failed (DK_INT), the scaled
+// value (DK_TO_INT), the value outside the output precision.
+template <class I, class O, int KIND>
+__host__ __device__ __forceinline__ int dcast_row(const DcastArgs &a, I v, O &o, __int128 &mid) {
+  if (a.zero) { o = O(); return DR_OK; }
+  if constexpr (KIND == DK_DEC || KIND == DK_INT) {
+    if (a.down) {
+      // decimal downscale: div_wrapping / mod_wrapping in I, rounded half away from zero (decimal.rs:237-249);
+      // integer to a negative scale: div_checked in I (mod.rs:398-401)
+      using U = typename dec_unsigned<I>::type;
+      const bool neg = v < I();
+      const U m = neg ? (U)0 - (U)v : (U)v;
+      U q, r;
+      udivmod_k<I>(m, a, q, r);
+      if (KIND == DK_DEC && r >= (U)a.half) q += 1;
+      const I d = neg ? (I)((U)0 - q) : (I)q;
+      if (!fits_in<O>(d)) return DR_NONE;
+      o = (O)d;
+    } else {
+      if (!fits_in<O>(v)) return DR_NONE;  // from_decimal / integer_to_decimal_native
+      const O x = (O)v, k = (O)a.k;
+      using U = typename dec_unsigned<O>::type;
+      if (a.wrap) { o = (O)((U)x * (U)k); return DR_OK; }  // infallible: mul_wrapping
+      if (k != (O)1 && mul_ovf(x, k, o)) { mid = (__int128)x; return KIND == DK_INT ? DR_MUL : DR_NONE; }
+      if (k == (O)1) o = x;
+    }
+  } else if constexpr (KIND == DK_FLOAT) {
+    // single_float_to_decimal: (mul * v).round() (one IEEE multiply, round half away from zero), then to_i32 / i64 / i128
+    const double x = round(dmul_rn(a.fk, (double)v));
+    if (!num_cast<double, O>(x, o)) return DR_NONE;
+  } else if constexpr (KIND == DK_TO_INT) {
+    I s;
+    if (a.down) {  // div_checked by 10^scale: truncates toward zero
+      using U = typename dec_unsigned<I>::type;
+      const bool neg = v < I();
+      const U m = neg ? (U)0 - (U)v : (U)v;
+      U q, r;
+      udivmod_k<I>(m, a, q, r);
+      s = neg ? (I)((U)0 - q) : (I)q;
+    } else if (mul_ovf(v, (I)a.k, s)) {
+      mid = (__int128)v;
+      return DR_MUL;
+    }
+    mid = (__int128)s;
+    if (!fits_in<O>(s)) return DR_NONE;
+    o = (O)s;
+    return DR_OK;
+  } else {  // DK_TO_FLOAT: (x as f64) / 10_f64.powi(scale), `as f32` after for Float32
+    double x;
+    if constexpr (sizeof(I) == 16) x = i128_to_f64(v);
+    else x = (double)v;
+    o = (O)ddiv_rn(x, a.fk);
+    return DR_OK;
+  }
+  if constexpr (KIND != DK_TO_INT && KIND != DK_TO_FLOAT) {
+    if (a.check && !((O)a.lo <= o && o <= (O)a.hi)) { mid = (__int128)o; return DR_PRECISION; }
+  }
+  return DR_OK;
+}
+
+template <class I, class O>
+struct DcastParams {
+  const I *in;
+  O *out;
+  int64_t n;
+  const uint8_t *iv;
+  int64_t ioff;
+  uint64_t *out_valid;
+  unsigned long long *res;
+  int mode;
+  DcastArgs a;
+};
+
+// k_cast's layout, one element per lane and load (rows are 4-16 B, so a warp-wide load is already one coalesced
+// 128-512 B request): 2048-row super-groups, lane-owned validity words, the ragged tail finished by warp 0, the lowest
+// failing row by atomicMin. A sibling of k_cast rather than k_cast over a row functor: the decimal rows carry a 112-byte
+// parameter block and 128-bit steps that k_cast's numeric instantiations should not pay for in registers.
+template <class I, class O, int KIND>
+__global__ void __launch_bounds__(256, (sizeof(I) == 16 || sizeof(O) == 16) ? 2 : 4) k_dcast(const DcastParams<I, O> p) {
+  constexpr int U = 4;  // loads in flight per lane
+  const int lane = threadIdx.x & 31;
+  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
+  const int64_t n = p.n;
+  const int64_t sgroups = n >> 11;
+  const bool every = p.mode == DM_UNARY;
+  unsigned valid_cnt = 0;
+  unsigned long long err = ~0ull;
+  for (int64_t sg = warp; sg < sgroups; sg += nwarps) {
+    const int64_t sbase = sg << 11;
+    uint64_t vw = ~0ull;
+    if (p.iv) vw = ld_bits64(p.iv, p.ioff + sbase + lane * 64, p.ioff + n);
+    const uint64_t live = every ? ~0ull : vw;  // rows the cast runs at
+    uint32_t bad_lo = 0, bad_hi = 0;
+#pragma unroll 1
+    for (int l0 = 0; l0 < 64; l0 += U) {
+      I v[U];
+#pragma unroll
+      for (int u = 0; u < U; ++u) v[u] = ldg_elem(p.in + sbase + (int64_t)(l0 + u) * 32 + lane);
+#pragma unroll
+      for (int u = 0; u < U; ++u) {
+        const int pos = (l0 + u) * 32 + lane;
+        const uint64_t w = __shfl_sync(ACU_FULL_MASK, live, pos >> 6);
+        O x = O();
+        bool bad = false;
+        if ((w >> (pos & 63)) & 1ull) {
+          __int128 mid;
+          bad = dcast_row<I, O, KIND>(p.a, v[u], x, mid) != DR_OK;
+          if (bad) x = O();
+        }
+        p.out[sbase + pos] = x;
+        if (__any_sync(ACU_FULL_MASK, bad)) pack_lane_bits<1>(bad, l0 + u, bad_lo, bad_hi);  // failures are rare
+      }
+    }
+    const uint64_t bad = (uint64_t)bad_lo | ((uint64_t)bad_hi << 32);
+    if (bad) {
+      if (p.mode == DM_OPT) vw &= ~bad;
+      else err = min(err, (unsigned long long)(sbase + lane * 64 + __ffsll((long long)bad) - 1));
+    }
+    if (p.out_valid) { p.out_valid[(sbase >> 6) + lane] = vw; valid_cnt += __popcll(vw); }
+  }
+
+  if (warp == 0) {
+    for (int64_t row = sgroups << 11; row < n; row += 64) {
+      uint64_t vw = ones_to(row, n);
+      if (p.iv) vw &= ld_bits64(p.iv, p.ioff + row, p.ioff + n);
+      const uint64_t live = every ? ones_to(row, n) : vw;
+      uint64_t bad = 0;
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int64_t i = row + h * 32 + lane;
+        O x = O();
+        bool b = false;
+        if ((live >> (h * 32 + lane)) & 1ull) {
+          __int128 mid;
+          b = dcast_row<I, O, KIND>(p.a, ldg_elem(p.in + i), x, mid) != DR_OK;
+          if (b) x = O();
+        }
+        if (i < n) p.out[i] = x;
+        bad |= (uint64_t)__ballot_sync(ACU_FULL_MASK, b) << (h * 32);
+      }
+      if (bad) {
+        if (p.mode == DM_OPT) vw &= ~bad;
+        else err = min(err, (unsigned long long)(row + __ffsll((long long)bad) - 1));
+      }
+      if (p.out_valid && lane == 0) { p.out_valid[row >> 6] = vw; valid_cnt += __popcll(vw); }
+    }
+  }
+  if (p.out_valid) {
+    valid_cnt = warp_sum(valid_cnt);
+    if (lane == 0 && valid_cnt) atomicAdd(p.res + RES_COUNT, (unsigned long long)valid_cnt);
+  }
+  if (err != ~0ull) atomicMin(p.res + RES_ERR_INDEX, err);
+}
+
+int dec_max_precision(int width) { return width == 4 ? 9 : width == 8 ? 18 : 38; }
+__int128 pow10_i128(int k) {
+  __int128 v = 1;
+  for (int i = 0; i < k; ++i) v *= 10;
+  return v;
+}
+// O::MIN / MAX_FOR_EACH_PRECISION[p] (arrow-data/src/decimal.rs), or an empty range when p is past the table
+void precision_bounds(int width, int p, DcastArgs &a) {
+  if (p > dec_max_precision(width)) { a.lo = 1; a.hi = 0; return; }
+  a.hi = pow10_i128(p) - 1;
+  a.lo = -a.hi;
+}
+// 10^k as factors of at most 10^9, for the full-width division
+void set_k(DcastArgs &a, int k) {
+  a.k = pow10_i128(k);
+  a.half = a.k / 2;
+  a.nchunk = 0;
+  for (int left = k; left > 0; left -= 9) a.chunk[a.nchunk++] = (uint32_t)pow10_i128(left < 9 ? left : 9);
+}
+// 10_f64.powi(e): compiler-builtins' `pow` (what llvm.powi calls for a runtime exponent): repeated squaring, then 1 / r
+// for a negative exponent. Not always the correctly rounded 10^e (it differs at e = 33, 34, 37 and most e <= -23).
+double powi10(int e) {
+  double a = 10.0, r = 1.0;
+  const bool recip = e < 0;
+  uint32_t k = recip ? (uint32_t)0 - (uint32_t)e : (uint32_t)e;
+  for (;;) {
+    if (k & 1) r *= a;
+    k >>= 1;
+    if (!k) break;
+    a *= a;
+  }
+  return recip ? 1.0 / r : r;
+}
+
+// format_decimal_str_internal (arrow-data/src/decimal.rs:1137-1167), truncation quirk included
+void fmt_decimal_str(char *buf, size_t n, const char *value, int precision, int scale, bool safe) {
+  const bool neg = value[0] == '-';
+  const char *rest = neg ? value + 1 : value;
+  const size_t rlen = strlen(rest);
+  const size_t bound = safe ? std::min<size_t>((size_t)precision, rlen) + (neg ? 1 : 0) : strlen(value);
+  char v[64];
+  snprintf(v, sizeof v, "%.*s", (int)bound, value);
+  const size_t vlen = strlen(v);
+  const std::string zeros(scale < 0 ? (size_t)-scale : (size_t)scale - std::min<size_t>(rlen, (size_t)scale), '0');
+  if (scale == 0) snprintf(buf, n, "%s", v);
+  else if (scale < 0) snprintf(buf, n, "%s%s", v, zeros.c_str());
+  else if (rlen > (size_t)scale) snprintf(buf, n, "%.*s.%s", (int)(vlen - scale), v, v + vlen - scale);
+  else snprintf(buf, n, "%s0.%s%s", neg ? "-" : "", zeros.c_str(), rest);
+}
+// validate_decimal{32,64,}_precision's error (arrow-data/src/decimal.rs:1030ff)
+acu_status precision_error(acu_ctx *ctx, int width, __int128 v, int p, int s, int64_t idx, uint64_t bits) {
+  const char *name = decimal_name(width);
+  const int mp = dec_max_precision(width);
+  if (p > mp) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, idx, bits, 0, 0, "Max precision of a %s is %d, but got %d", name, mp, p);
+  const __int128 hi = p ? pow10_i128(p) - 1 : 0;
+  char vs[48], bs[48], a[96], b[96];
+  fmt_i128(vs, sizeof vs, v);
+  fmt_i128(bs, sizeof bs, v > hi ? hi : -hi);
+  fmt_decimal_str(a, sizeof a, vs, p, s, false);
+  fmt_decimal_str(b, sizeof b, bs, p, s, true);
+  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, idx, bits, 0, 0, "%s is too %s to store in a %s of precision %d. %s is %s", a,
+                  v > hi ? "large" : "small", name, p, v > hi ? "Max" : "Min", b);
+}
+
+// Rust's `{:?}` of f32 / f64: the shortest digits that round-trip in the value's own type; plain notation with at least one
+// fractional digit when 1e-4 <= |v| < 1e16 or v == 0, else `1e40` / `1.5e-7`.
+void fmt_float_debug(char *buf, size_t n, double v, bool f32) {
+  if (v != v) { snprintf(buf, n, "NaN"); return; }
+  if (std::isinf(v)) { snprintf(buf, n, v < 0 ? "-inf" : "inf"); return; }
+  if (v == 0) { snprintf(buf, n, std::signbit(v) ? "-0.0" : "0.0"); return; }
+  char t[64];
+  for (int prec = 0; prec <= 17; ++prec) {
+    snprintf(t, sizeof t, "%.*e", prec, v);
+    if (f32 ? strtof(t, nullptr) == (float)v : strtod(t, nullptr) == v) break;
+  }
+  char digits[32];
+  int nd = 0;
+  const char *c = t + (t[0] == '-');
+  for (; *c != 'e'; ++c) if (*c != '.') digits[nd++] = *c;
+  const int e = atoi(c + 1);
+  while (nd > 1 && digits[nd - 1] == '0') --nd;
+  digits[nd] = 0;
+  const double a = fabs(v);
+  const bool expo = f32 ? (a < (double)1e-4f || a >= (double)1e16f) : (a < 1e-4 || a >= 1e16);
+  char out[96];
+  int k = 0;
+  if (v < 0) out[k++] = '-';
+  if (expo) {
+    out[k++] = digits[0];
+    if (nd > 1) { out[k++] = '.'; for (int i = 1; i < nd; ++i) out[k++] = digits[i]; }
+    k += snprintf(out + k, sizeof out - k, "e%d", e);
+  } else if (e >= 0) {
+    for (int i = 0; i <= e; ++i) out[k++] = i < nd ? digits[i] : '0';
+    out[k++] = '.';
+    if (nd > e + 1) for (int i = e + 1; i < nd; ++i) out[k++] = digits[i];
+    else out[k++] = '0';
+  } else {
+    out[k++] = '0';
+    out[k++] = '.';
+    for (int i = 0; i < -e - 1; ++i) out[k++] = '0';
+    for (int i = 0; i < nd; ++i) out[k++] = digits[i];
+  }
+  out[k] = 0;
+  snprintf(buf, n, "%s", out);
+}
+
+template <class T> void fmt_value(char *buf, size_t n, T v) {
+  if constexpr (std::is_floating_point<T>::value) fmt_float_debug(buf, n, (double)v, sizeof(T) == 4);
+  else fmt_native(buf, n, v);
+}
+
+// What a failing row turns into; `what` names the output type of the messages ("Decimal32(9, 2)").
+struct DcastCall {
+  int kind;
+  int mode;
+  int safe;
+  int out_width;        // decimal outputs: 4 / 8 / 16
+  uint8_t precision;    // decimal outputs
+  int8_t scale;
+  acu_dtype out_dtype;  // integer / float outputs
+  bool builder;         // decimal -> integer: a NullBuffer only when some row is null
+};
+
+template <class I, class O, int KIND>
+acu_status dcast_launch(acu_ctx *ctx, const DcastCall &c, const DcastArgs &args, const acu_array *a, acu_array_out *out) {
+  const int64_t len = a->len;
+  out->len = len;
+  out->null_count = 0;
+  // unary_opt always carries a NullBuffer; unary / try_unary clone the input's; the builder decides after the rows
+  out->has_validity = c.mode == DM_OPT || (a->validity != nullptr);
+  if (len == 0) {
+    if (c.builder) out->has_validity = 0;
+    return ACU_OK;
+  }
+  DcastParams<I, O> p{};
+  p.in = static_cast<const I *>(a->values);
+  p.out = static_cast<O *>(out->values);
+  p.n = len;
+  p.iv = a->validity;
+  p.ioff = a->validity_offset;
+  p.out_valid = out->has_validity ? reinterpret_cast<uint64_t *>(out->validity) : nullptr;
+  p.res = ctx->d_res;
+  p.mode = c.mode;
+  p.a = args;
+  ACU_TRY(acu_res_reset(ctx));
+  const int64_t blocks = (len / 2048 + 1 + 7) / 8;
+  ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_dcast<I, O, KIND>), acu_wave_grid(ctx, k_dcast<I, O, KIND>, 256, 0, blocks), 256, 0, p);
+  ACU_TRY(acu_res_fetch(ctx));
+  if (ctx->h_res[RES_ERR_INDEX] != ~0ull) {
+    const int64_t idx = (int64_t)ctx->h_res[RES_ERR_INDEX];
+    I v;
+    ACU_CUDA(ctx, cudaMemcpyAsync(&v, p.in + idx, sizeof(I), cudaMemcpyDeviceToHost, ctx->stream));
+    ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    const uint64_t bits = bits_of(v);
+    if (c.mode == DM_UNARY)  // from_decimal(x).unwrap() / f_fallible(x).unwrap() on a slot that does not convert
+      return acu_fail(ctx, ACU_ERR_PANIC_OUT_OF_BOUNDS, idx, bits, 0, 0, "called `Option::unwrap()` on a `None` value");
+    O o;
+    __int128 mid = 0;
+    const int r = dcast_row<I, O, KIND>(args, v, o, mid);
+    char vs[64], ms[48], ks[48];
+    fmt_value(vs, sizeof vs, v);
+    fmt_i128(ms, sizeof ms, mid);
+    fmt_i128(ks, sizeof ks, args.k);
+    if (r == DR_PRECISION) return precision_error(ctx, c.out_width, mid, c.precision, c.scale, idx, bits);
+    if (r == DR_MUL) return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, bits, 0, 0, "Overflow happened on: %s * %s", ms, ks);
+    if (KIND == DK_TO_INT)
+      return acu_fail(ctx, ACU_ERR_CAST, idx, bits, 0, 0, "value of %s is out of range %s", ms, acu_dtype_name(c.out_dtype));
+    return acu_fail(ctx, ACU_ERR_CAST, idx, bits, 0, 0, "Cannot cast to %s(%d, %d). Overflowing on %s", decimal_name(c.out_width),
+                    (int)c.precision, (int)c.scale, vs);
+  }
+  if (p.out_valid) out->null_count = len - (int64_t)ctx->h_res[RES_COUNT];
+  if (c.builder && out->null_count == 0) out->has_validity = 0;
+  return ACU_OK;
+}
+
+template <class I, class O, int KIND>
+acu_status dcast_to_decimal(acu_ctx *ctx, const DcastCall &c, const DcastArgs &args, const acu_array *a, acu_array_out *out) {
+  ACU_TRY((dcast_launch<I, O, KIND>(ctx, c, args, a, out)));
+  const int mp = dec_max_precision(c.out_width);
+  return decimal_validate(ctx, mp, mp, c.precision, c.scale);  // with_precision_and_scale, after the rows
+}
+
+template <class I, int KIND>
+acu_status dcast_to_width(acu_ctx *ctx, const DcastCall &c, const DcastArgs &args, const acu_array *a, acu_array_out *out) {
+  if (c.out_width == 4) return dcast_to_decimal<I, int32_t, KIND>(ctx, c, args, a, out);
+  if (c.out_width == 8) return dcast_to_decimal<I, int64_t, KIND>(ctx, c, args, a, out);
+  return dcast_to_decimal<I, __int128, KIND>(ctx, c, args, a, out);
+}
+
+// decimal -> decimal: cast_decimal_to_decimal(_same_type), decimal.rs:448-529 with make_upscaler / make_downscaler
+template <class I>
+acu_status cast_decimal_typed(acu_ctx *ctx, const acu_decimal_type &from, const acu_decimal_type &to, int32_t safe,
+                              const acu_array *a, acu_array_out *out) {
+  const int p_in = from.precision, s_in = from.scale, p_out = to.precision, s_out = to.scale;
+  DcastCall c{DK_DEC, DM_UNARY, safe, to.byte_width, to.precision, to.scale, ACU_I8, false};
+  DcastArgs args{};
+  precision_bounds(to.byte_width, p_out, args);
+  if (from.byte_width == to.byte_width && s_in == s_out && p_in <= p_out) {
+    // array.clone() (decimal.rs:461), decided in u8 before any i8 arithmetic: the same bytes, the input's nulls. Run as the
+    // identity unary (multiply by 1), which reproduces them exactly.
+    set_k(args, 0);
+    c.mode = DM_UNARY, args.wrap = 1;
+  } else if (s_in <= s_out) {
+    const int8_t delta = i8_wrap(s_out - s_in);
+    if (delta < 0 || delta > dec_max_precision(to.byte_width))  // O::MAX_FOR_EACH_PRECISION.get(delta as usize) misses
+      return acu_fail(ctx, ACU_ERR_CAST, -1, 0, 0, 0, "Cannot cast to %s(%d, %d). Value overflows for output scale",
+                      decimal_name(to.byte_width), p_out, s_out);
+    set_k(args, delta);
+    if (i8_wrap((int8_t)p_in + delta) <= (int8_t)p_out) c.mode = DM_UNARY, args.wrap = 1;
+    else c.mode = safe ? DM_OPT : DM_TRY, args.check = 1;
+  } else {
+    const int8_t delta = i8_wrap(s_in - s_out);
+    if (delta < 0 || delta > dec_max_precision(from.byte_width)) {  // past I's table: every value rounds to zero
+      args.zero = 1;
+    } else {
+      set_k(args, delta);
+      args.down = 1;
+      if (i8_wrap((int8_t)p_in - delta) < (int8_t)p_out) c.mode = DM_UNARY;
+      else c.mode = safe ? DM_OPT : DM_TRY, args.check = 1;
+    }
+  }
+  return dcast_to_width<I, DK_DEC>(ctx, c, args, a, out);
+}
+
+// integer -> decimal: cast_integer_to_decimal, mod.rs:366-444
+template <class I>
+acu_status cast_int_to_decimal(acu_ctx *ctx, const acu_decimal_type &to, int32_t safe, const acu_array *a, acu_array_out *out) {
+  DcastCall c{DK_INT, safe ? DM_OPT : DM_TRY, safe, to.byte_width, to.precision, to.scale, ACU_I8, false};
+  DcastArgs args{};
+  precision_bounds(to.byte_width, to.precision, args);
+  args.check = 1;
+  const uint32_t e = to.scale < 0 ? (uint32_t)(-(int)to.scale) : (uint32_t)to.scale;
+  if (to.scale < 0) {  // 10^|scale| in the source type
+    if (!pow10_checked<__int128>(e, &args.k) || !fits_in<I>(args.k)) {
+      args.zero = 1, c.mode = DM_UNARY;  // a factor beyond the source type: every quotient is 0 (unary)
+    } else {
+      set_k(args, (int)e);
+      args.down = 1;
+    }
+  } else {
+    bool ok;
+    if (to.byte_width == 4) { int32_t k; ok = pow10_checked<int32_t>(e, &k); }
+    else if (to.byte_width == 8) { int64_t k; ok = pow10_checked<int64_t>(e, &k); }
+    else { __int128 k; ok = pow10_checked<__int128>(e, &k); }
+    if (!ok)
+      return acu_fail(ctx, ACU_ERR_CAST, -1, 0, 0, 0, "Cannot cast to \"%s\"(%d, %d). The scale causes overflow.",
+                      decimal_name(to.byte_width), (int)to.precision, (int)to.scale);
+    set_k(args, (int)e);
+  }
+  return dcast_to_width<I, DK_INT>(ctx, c, args, a, out);
+}
+
+// float -> decimal: cast_floating_point_to_decimal, decimal.rs:836-885
+template <class I>
+acu_status cast_float_to_decimal(acu_ctx *ctx, const acu_decimal_type &to, int32_t safe, const acu_array *a, acu_array_out *out) {
+  DcastCall c{DK_FLOAT, safe ? DM_OPT : DM_TRY, safe, to.byte_width, to.precision, to.scale, ACU_I8, false};
+  DcastArgs args{};
+  precision_bounds(to.byte_width, to.precision, args);
+  args.check = 1;
+  args.fk = powi10(to.scale);
+  return dcast_to_width<I, DK_FLOAT>(ctx, c, args, a, out);
+}
+
+// decimal -> integer / float: cast_decimal_to_integer / cast_decimal_to_float, decimal.rs:887-1004
+template <class I, class O>
+acu_status cast_from_decimal_typed(acu_ctx *ctx, const acu_decimal_type &from, acu_dtype to, int32_t safe, const acu_array *a,
+                                   acu_array_out *out) {
+  DcastArgs args{};
+  if constexpr (is_fp<O>::value) {
+    DcastCall c{DK_TO_FLOAT, DM_UNARY, safe, 0, 0, 0, to, false};
+    args.fk = powi10(from.scale);
+    return dcast_launch<I, O, DK_TO_FLOAT>(ctx, c, args, a, out);
+  } else {
+    DcastCall c{DK_TO_INT, safe ? DM_OPT : DM_TRY, safe, 0, 0, 0, to, true};
+    const uint32_t e = from.scale < 0 ? (uint32_t)(-(int)from.scale) : (uint32_t)from.scale;
+    I k;
+    if (!pow10_checked<I>(e, &k))
+      return acu_fail(ctx, ACU_ERR_CAST, -1, 0, 0, 0, "Cannot cast to \"%s\". The scale %d causes overflow.",
+                      decimal_name(from.byte_width), (int)from.scale);
+    set_k(args, (int)e);
+    args.down = from.scale >= 0;
+    return dcast_launch<I, O, DK_TO_INT>(ctx, c, args, a, out);
+  }
+}
+
+template <class I>
+acu_status cast_from_decimal_to(acu_ctx *ctx, const acu_decimal_type &from, acu_dtype to, int32_t safe, const acu_array *a,
+                                acu_array_out *out) {
+  switch (to) {
+    case ACU_I8: return cast_from_decimal_typed<I, int8_t>(ctx, from, to, safe, a, out);
+    case ACU_I16: return cast_from_decimal_typed<I, int16_t>(ctx, from, to, safe, a, out);
+    case ACU_I32: return cast_from_decimal_typed<I, int32_t>(ctx, from, to, safe, a, out);
+    case ACU_I64: return cast_from_decimal_typed<I, int64_t>(ctx, from, to, safe, a, out);
+    case ACU_U8: return cast_from_decimal_typed<I, uint8_t>(ctx, from, to, safe, a, out);
+    case ACU_U16: return cast_from_decimal_typed<I, uint16_t>(ctx, from, to, safe, a, out);
+    case ACU_U32: return cast_from_decimal_typed<I, uint32_t>(ctx, from, to, safe, a, out);
+    case ACU_U64: return cast_from_decimal_typed<I, uint64_t>(ctx, from, to, safe, a, out);
+    case ACU_F32: return cast_from_decimal_typed<I, float>(ctx, from, to, safe, a, out);
+    case ACU_F64: return cast_from_decimal_typed<I, double>(ctx, from, to, safe, a, out);
+    default: break;
+  }
+  return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from %s to dtype %d", decimal_name(from.byte_width), (int)to);
+}
+
+// the operand's decimal type is an array's: refused like an invalid type (with_precision_and_scale) at call time
+acu_status decimal_type_ok(acu_ctx *ctx, const acu_decimal_type *t) {
+  const int w = t->byte_width;
+  if (w != 4 && w != 8 && w != 16)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid decimal type: byte width %d", (int)w);
+  const int mp = dec_max_precision(w);
+  return decimal_validate(ctx, mp, mp, t->precision, t->scale);
+}
+
 }  // namespace
 
 #define ACU_DISPATCH(dt, F, ...)                         \
@@ -1273,4 +1857,49 @@ extern "C" acu_status acu_decimal_arith(acu_ctx *ctx, acu_arith_op op, const acu
   ACU_TRY(i128_aligned(ctx, a->values, b->values));
   ACU_TRY(i128_aligned(ctx, out->values, nullptr));
   return decimal_typed<__int128>(ctx, op, *lt, a, *rt, b, out_type, out);
+}
+
+extern "C" acu_status acu_cast_decimal(acu_ctx *ctx, const acu_decimal_type *from, const acu_decimal_type *to, int32_t safe,
+                                       const acu_array *a, acu_array_out *out) {
+  ACU_ENTER(ctx);
+  ACU_TRY(decimal_type_ok(ctx, from));
+  if (to->byte_width != 4 && to->byte_width != 8 && to->byte_width != 16)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid decimal type: byte width %d", (int)to->byte_width);
+  if (from->byte_width == 16) ACU_TRY(i128_aligned(ctx, a->values, nullptr));
+  if (to->byte_width == 16) ACU_TRY(i128_aligned(ctx, out->values, nullptr));
+  if (from->byte_width == 4) return cast_decimal_typed<int32_t>(ctx, *from, *to, safe, a, out);
+  if (from->byte_width == 8) return cast_decimal_typed<int64_t>(ctx, *from, *to, safe, a, out);
+  return cast_decimal_typed<__int128>(ctx, *from, *to, safe, a, out);
+}
+
+extern "C" acu_status acu_cast_to_decimal(acu_ctx *ctx, acu_dtype from, const acu_decimal_type *to, int32_t safe,
+                                          const acu_array *a, acu_array_out *out) {
+  ACU_ENTER(ctx);
+  if (to->byte_width != 4 && to->byte_width != 8 && to->byte_width != 16)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid decimal type: byte width %d", (int)to->byte_width);
+  if (to->byte_width == 16) ACU_TRY(i128_aligned(ctx, out->values, nullptr));
+  switch (from) {
+    case ACU_I8: return cast_int_to_decimal<int8_t>(ctx, *to, safe, a, out);
+    case ACU_I16: return cast_int_to_decimal<int16_t>(ctx, *to, safe, a, out);
+    case ACU_I32: return cast_int_to_decimal<int32_t>(ctx, *to, safe, a, out);
+    case ACU_I64: return cast_int_to_decimal<int64_t>(ctx, *to, safe, a, out);
+    case ACU_U8: return cast_int_to_decimal<uint8_t>(ctx, *to, safe, a, out);
+    case ACU_U16: return cast_int_to_decimal<uint16_t>(ctx, *to, safe, a, out);
+    case ACU_U32: return cast_int_to_decimal<uint32_t>(ctx, *to, safe, a, out);
+    case ACU_U64: return cast_int_to_decimal<uint64_t>(ctx, *to, safe, a, out);
+    case ACU_F32: return cast_float_to_decimal<float>(ctx, *to, safe, a, out);
+    case ACU_F64: return cast_float_to_decimal<double>(ctx, *to, safe, a, out);
+    default: break;
+  }
+  return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from dtype %d to %s", (int)from, decimal_name(to->byte_width));
+}
+
+extern "C" acu_status acu_cast_from_decimal(acu_ctx *ctx, const acu_decimal_type *from, acu_dtype to, int32_t safe,
+                                            const acu_array *a, acu_array_out *out) {
+  ACU_ENTER(ctx);
+  ACU_TRY(decimal_type_ok(ctx, from));
+  if (from->byte_width == 4) return cast_from_decimal_to<int32_t>(ctx, *from, to, safe, a, out);
+  if (from->byte_width == 8) return cast_from_decimal_to<int64_t>(ctx, *from, to, safe, a, out);
+  ACU_TRY(i128_aligned(ctx, a->values, nullptr));
+  return cast_from_decimal_to<__int128>(ctx, *from, to, safe, a, out);
 }

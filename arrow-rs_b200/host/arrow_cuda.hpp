@@ -1344,8 +1344,52 @@ inline Result<BooleanArray> is_not_null(const Array &a) { return detail4::boolea
 
 // ---- cast (arrow-cast/src/cast/mod.rs) -------------------------------------------------------
 struct CastOptions { bool safe = true; };  // mod.rs:96-111
+// A decimal cast target: DataType::Decimal32 / Decimal64 / Decimal128(precision, scale)
+struct DecimalDataType { DataType data_type; uint8_t precision; int8_t scale; };
+
+namespace detail {
+inline bool decimal_type_of(const Array &a, acu_decimal_type *t) {
+  if (auto d = dynamic_cast<const DecimalArray<int32_t> *>(&a)) { *t = d->decimal_type(); return true; }
+  if (auto d = dynamic_cast<const DecimalArray<int64_t> *>(&a)) { *t = d->decimal_type(); return true; }
+  if (auto d = dynamic_cast<const DecimalArray<__int128> *>(&a)) { *t = d->decimal_type(); return true; }
+  return false;
+}
+inline int decimal_width(DataType t) { return t == DataType::Decimal32 ? 4 : t == DataType::Decimal64 ? 8 : t == DataType::Decimal128 ? 16 : 0; }
+}  // namespace detail
+
+// The decimal arms of cast_with_options (mod.rs:980-1219): decimal -> decimal, integer / float -> decimal. The result is
+// Decimal*Array::with_precision_and_scale(precision, scale) of the cast values.
+inline Result<ArrayRef> cast_with_options(const Array &array, const DecimalDataType &to, const CastOptions &opt) {
+  const int w = detail::decimal_width(to.data_type);
+  acu_decimal_type from{}, tt{w, to.precision, to.scale, {0, 0}};
+  const bool from_decimal = detail::decimal_type_of(array, &from);
+  if (w == 0 || (!from_decimal && dtype_width(array.data_type()) == 0))
+    return ArrowError{ACU_ERR_CAST, std::string("Cast error: Casting from ") + detail::dtype_display(array.data_type()) + " to " +
+                                        detail::dtype_display(to.data_type) + " not supported"};
+  Context &c = Context::get();
+  Buffer vb, nb;
+  acu_array v = array.view();
+  acu_array_out o = detail::make_out(vb, nb, (size_t)std::max<int64_t>(array.len(), 1) * w, array.len());
+  acu_status st = from_decimal ? acu_cast_decimal(c.raw(), &from, &tt, opt.safe ? 1 : 0, &v, &o)
+                               : acu_cast_to_decimal(c.raw(), (acu_dtype)dtype_code(array.data_type()), &tt, opt.safe ? 1 : 0, &v, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  auto nulls = detail::out_nulls(o, nb);
+  if (w == 4) return ArrayRef(std::make_shared<DecimalArray<int32_t>>(vb, o.len, nulls, 0, to.precision, to.scale));
+  if (w == 8) return ArrayRef(std::make_shared<DecimalArray<int64_t>>(vb, o.len, nulls, 0, to.precision, to.scale));
+  return ArrayRef(std::make_shared<DecimalArray<__int128>>(vb, o.len, nulls, 0, to.precision, to.scale));
+}
 
 inline Result<ArrayRef> cast_with_options(const Array &array, DataType to_type, const CastOptions &opt) {
+  acu_decimal_type from{};
+  if (detail::decimal_type_of(array, &from) && dtype_width(to_type) != 0) {  // decimal -> integer / float
+    Context &c = Context::get();
+    Buffer vb, nb;
+    acu_array v = array.view();
+    acu_array_out o = detail::make_out(vb, nb, (size_t)std::max<int64_t>(array.len(), 1) * dtype_width(to_type), array.len());
+    acu_status st = acu_cast_from_decimal(c.raw(), &from, (acu_dtype)dtype_code(to_type), opt.safe ? 1 : 0, &v, &o);
+    if (st != ACU_OK) return c.last_error(st);
+    return detail::make_primitive(to_type, vb, o.len, detail::out_nulls(o, nb));
+  }
   if (dtype_width(array.data_type()) == 0 || dtype_width(to_type) == 0)
     return ArrowError{ACU_ERR_CAST, std::string("Cast error: Casting from ") + detail::dtype_display(array.data_type()) + " to " +
                                         detail::dtype_display(to_type) + " not supported"};

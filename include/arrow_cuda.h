@@ -560,6 +560,68 @@ acu_status acu_view_rebase(acu_ctx *ctx, const void *views, int64_t n, uint32_t 
 acu_status acu_cast_numeric(acu_ctx *ctx, acu_dtype from, acu_dtype to, int32_t safe,
                             const acu_array *a, acu_array_out *out);
 
+/* Decimal casts (arrow-cast/src/cast/decimal.rs, the decimal arms of cast_with_options in mod.rs), under
+ * CastOptions{safe: safe != 0}. Decimal32 / 64 / 128 values are ACU_I32 / ACU_I64 / ACU_I128 natives (acu_decimal_type);
+ * out->values holds the output native per row. Synchronous, like acu_cast_numeric (not stream-ordered inside a section);
+ * kernel time counts in ACU_K_CAST. Decimal128 pointers, input and output, must be 16-byte aligned, and the input decimal
+ * type must pass validate_decimal_precision_and_scale (ACU_ERR_INVALID_ARGUMENT otherwise, at call time).
+ *
+ * Which array the reference builds decides values under nulls and the NullBuffer:
+ *   - unary (the infallible casts): the value is computed at EVERY slot, null slots included; the input's nulls are kept.
+ *   - unary_opt (safe, fallible): valid slots only, 0 under nulls and where the cast fails (-> null); the result ALWAYS has
+ *     a NullBuffer.
+ *   - try_unary (unsafe, fallible): valid slots only, 0 under nulls, the input's nulls kept; the lowest failing valid row
+ *     is the error (detail.index, detail.lhs_bits = the low 64 bits of its raw input).
+ *   - decimal -> integer (PrimitiveBuilder): 0 under nulls, a NullBuffer only when some row is null.
+ *
+ * acu_cast_decimal, decimal -> decimal (cast_decimal_to_decimal(_same_type), decimal.rs:161-529):
+ *   - delta = s_out - s_in (upscale, s_in <= s_out) or s_in - s_out (downscale), in i8 arithmetic that wraps like a release
+ *     build; a negative delta misses MAX_FOR_EACH_PRECISION. Upscale: x converted to the output native, times 10^delta.
+ *     Downscale: x / 10^delta in the INPUT native, rounded half away from zero, then converted.
+ *   - infallible (unary) when p_in + delta <= p_out (upscale) or p_in - delta < p_out (downscale), computed in i8: the
+ *     infallible upscale multiplies wrapping; a slot whose value does not convert to the output native (a valid value that
+ *     breaks its own precision, or bytes under a null) is the reference's `unwrap()` panic: ACU_ERR_PANIC_OUT_OF_BOUNDS
+ *     "called `Option::unwrap()` on a `None` value" at the lowest such slot. Same scale, same width and p_in <= p_out is
+ *     the reference's array.clone(), decided in u8 ahead of the i8 test (so p_out above 127 still clones and only the
+ *     closing type check fails): the same bytes, nulls and null slots included.
+ *   - otherwise fallible: a failed rescale or a value outside p_out is null (safe), or ACU_ERR_CAST "Cannot cast to
+ *     Decimal64(18, 18). Overflowing on {x}" (the input value) / the precision error below (unsafe).
+ *   - an upscale delta past the output's table: ACU_ERR_CAST "Cannot cast to Decimal128(p, s). Value overflows for output
+ *     scale", safe or not, also for an empty array. A downscale delta past the input's table: every value 0, the input's
+ *     nulls kept.
+ * acu_cast_to_decimal, from ACU_I8 .. ACU_U64, ACU_F32, ACU_F64:
+ *   - integers (cast_integer_to_decimal, mod.rs:366-444): scale < 0 divides by 10^-scale in the SOURCE type first (a
+ *     factor that overflows the source type gives all zeros, the input's nulls kept); scale >= 0 multiplies by 10^scale,
+ *     computed checked in the output native before any row (ACU_ERR_CAST "Cannot cast to \"Decimal32\"(9, 10). The scale
+ *     causes overflow."). A failing row (unsafe): the value does not fit the output native (or any failure at a negative
+ *     scale) => ACU_ERR_CAST "Cannot cast to Decimal32(9, 0). Overflowing on {v}" with the input; the checked multiply
+ *     fails => ACU_ERR_ARITHMETIC_OVERFLOW "Overflow happened on: {v} * {10^scale}" with the narrowed value.
+ *   - floats (cast_floating_point_to_decimal, decimal.rs:836-885): (mul * v).round() with mul = 10_f64.powi(scale), one
+ *     IEEE multiply (no FMA), rounded half away from zero, then to_i32 / to_i64 / to_i128 (NaN, +-inf or out of range =>
+ *     None). powi is repeated squaring with 1 / r for a negative exponent (the `pow` of Rust's compiler-builtins, which a
+ *     runtime-exponent llvm.powi calls), not the correctly rounded 10^scale. A failing row (unsafe): ACU_ERR_CAST
+ *     "Cannot cast to Decimal128(38, 10). Overflowing on {v:?}" with Rust's Debug of the f32 / f64 (shortest round-trip
+ *     digits; 1e-4 <= |v| < 1e16 or 0 in plain notation with a fractional digit, else "1e40"; NaN, inf, -inf).
+ * acu_cast_from_decimal, to ACU_I8 .. ACU_U64, ACU_F32, ACU_F64:
+ *   - integers (cast_decimal_to_integer, decimal.rs:887-987): 10^|scale| computed checked in the decimal native before any
+ *     row (ACU_ERR_CAST "Cannot cast to \"Decimal32\". The scale 10 causes overflow."); scale >= 0 divides truncating,
+ *     scale < 0 multiplies checked (unsafe: ACU_ERR_ARITHMETIC_OVERFLOW "Overflow happened on: {v} * {10^k}"); then
+ *     NumCast to the integer type (unsafe: ACU_ERR_CAST "value of {v} is out of range Int8", v scaled).
+ *   - floats (cast_decimal_to_float, mod.rs:86-92): unary (x as f64) / 10_f64.powi(scale); i128 -> f64 rounds to nearest,
+ *     ties to even; Float32 is that f64 `as f32` (two roundings, as the reference). Never fails.
+ * In every cast to a decimal, an unsafe row outside the output precision is validate_decimal{32,64,}_precision's
+ * ACU_ERR_INVALID_ARGUMENT "1234567.89 is too large to store in a Decimal128 of precision 6. Max is 9999.99" (or "too small
+ * ... Min is", or "Max precision of a Decimal128 is 38, but got 40"), the value formatted by format_decimal_str_internal
+ * with its truncation rule. Type-level errors come before any row, row errors before the closing with_precision_and_scale
+ * check of the output type (ACU_ERR_INVALID_ARGUMENT, as acu_decimal_arith's). Not reproduced: Decimal256, Float16,
+ * strings, temporal types, Null and dictionary inputs. */
+acu_status acu_cast_decimal(acu_ctx *ctx, const acu_decimal_type *from, const acu_decimal_type *to, int32_t safe,
+                            const acu_array *a, acu_array_out *out);
+acu_status acu_cast_to_decimal(acu_ctx *ctx, acu_dtype from, const acu_decimal_type *to, int32_t safe,
+                               const acu_array *a, acu_array_out *out);
+acu_status acu_cast_from_decimal(acu_ctx *ctx, const acu_decimal_type *from, acu_dtype to, int32_t safe,
+                                 const acu_array *a, acu_array_out *out);
+
 /* ------------------------------------------------------------------------- */
 /* boolean — arrow-arith/src/boolean.rs (predicate construction before filter) */
 /* ------------------------------------------------------------------------- */

@@ -208,6 +208,12 @@ extern "C" {
                              b: *const acu_array, out_type: *mut acu_decimal_type, out: *mut acu_array_out) -> acu_status;
     pub fn acu_cmp(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_cast_numeric(ctx: *mut acu_ctx, from: i32, to: i32, safe: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_cast_decimal(ctx: *mut acu_ctx, from: *const acu_decimal_type, to: *const acu_decimal_type, safe: i32, a: *const acu_array,
+                            out: *mut acu_array_out) -> acu_status;
+    pub fn acu_cast_to_decimal(ctx: *mut acu_ctx, from: i32, to: *const acu_decimal_type, safe: i32, a: *const acu_array,
+                               out: *mut acu_array_out) -> acu_status;
+    pub fn acu_cast_from_decimal(ctx: *mut acu_ctx, from: *const acu_decimal_type, to: i32, safe: i32, a: *const acu_array,
+                                 out: *mut acu_array_out) -> acu_status;
     pub fn acu_aggregate(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, out_bits: *mut u64, out_valid: *mut i64) -> acu_status;
     /// out_bits: 2 words (low, high) of the i128 result
     pub fn acu_aggregate_i128(ctx: *mut acu_ctx, op: i32, a: *const acu_array, out_bits: *mut u64, out_valid: *mut i64) -> acu_status;

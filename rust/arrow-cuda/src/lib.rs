@@ -410,6 +410,26 @@ pub mod compute {
                 return take(values.as_ref(), keys.as_ref(), None);
             }
         }
+        // the decimal arms (mod.rs:980-1219): decimal -> decimal, integer / float -> decimal, decimal -> integer / float
+        let (from_dec, to_dec) = (decimal_type(array.data_type()), decimal_type(to_type));
+        if from_dec.is_some() || to_dec.is_some() {
+            let (fc, tc) = (dtype_code(array.data_type()), dtype_code(to_type));
+            if !matches!((&from_dec, &to_dec, fc, tc), (Some(_), Some(_), _, _) | (None, Some(_), Some(_), _) | (Some(_), None, _, Some(_))) {
+                return Err(ArrowError::CastError(format!("Casting from {} to {} not supported", array.data_type(), to_type)));
+            }
+            let ctx = Context::current()?;
+            let a = DeviceArray::upload(&ctx, array, false)?;
+            let mut out = ColumnOut::new(&ctx, to_type, array.len(), 0)?;
+            let safe = options.safe as i32;
+            let st = match (from_dec, to_dec) {
+                (Some(f), Some(t)) => unsafe { ffi::acu_cast_decimal(ctx.raw(), &f, &t, safe, a.view(), out.array_out()) },
+                (None, Some(t)) => unsafe { ffi::acu_cast_to_decimal(ctx.raw(), fc.unwrap(), &t, safe, a.view(), out.array_out()) },
+                (Some(f), None) => unsafe { ffi::acu_cast_from_decimal(ctx.raw(), &f, tc.unwrap(), safe, a.view(), out.array_out()) },
+                (None, None) => unreachable!(),
+            };
+            ctx.check(st)?;
+            return out.finish(to_type);
+        }
         let (from, to) = match (dtype_code(array.data_type()), dtype_code(to_type)) {
             (Some(f), Some(t)) => (f, t),
             _ => return Err(ArrowError::CastError(format!("Casting from {} to {} not supported", array.data_type(), to_type))),

@@ -284,6 +284,51 @@ def decimal_rows(b, ctx, n):
             lambda: ctx.check(lib.acu_decimal_arith(h, abi.ADD, C.byref(L), C.byref(A64), C.byref(R), C.byref(B64), C.byref(ot), C.byref(o))))
     for d in (dx, dy, ds, va, vb, o.values, o.validity):
         ctx.free(d)
+    decimal_cast_rows(b, ctx, n, x)
+
+
+def decimal_cast_rows(b, ctx, n, x):
+    """The decimal casts (CastOptions{safe: true}) on n-row columns with 5 % nulls, from the 64-bit-sized values x
+    (|x| < 2^40), and for the Decimal128 sources also from full-width values (|v| ~ 2^100: the i128 division and conversion
+    slow paths). Algorithmic bytes: input + output values, input + output validity (n / 4)."""
+    lib, h = ctx.lib, ctx.h
+    rng = np.random.default_rng(6)
+    va, nva = b.bits(62, 0.95, n)
+    o = b.out(n * 16, n)
+
+    def col(vals):
+        d = ctx.malloc(vals.nbytes + 64)
+        ctx.h2d(d, vals)
+        return d
+
+    halves = np.empty((n, 2), dtype=np.uint64)
+    halves[:, 0] = x.view(np.uint64)
+    halves[:, 1] = (x >> 63).view(np.uint64)
+    wide = np.empty((n, 2), dtype=np.uint64)
+    wide[:, 0] = rng.integers(0, 2 ** 63, n).view(np.uint64) * np.uint64(2)
+    wide[:, 1] = rng.integers(-2 ** 36, 2 ** 36, n).view(np.uint64)
+    d128, d128w, d64, df = col(halves), col(wide), col(x), col(x.astype(np.float64) / 1000.0)
+    D = {k: abi.DecimalType(*t) for k, t in (("38,10", (16, 38, 10)), ("38,2", (16, 38, 2)), ("18,2", (8, 18, 2)), ("38,6", (16, 38, 6)))}
+    for label, d in (("64-bit values", d128), ("full-width values", d128w)):
+        A = b.arr(d, va, n, n - nva)
+        b.timed(f"decimal128 cast (38,10)->(38,2) {label}", [abi.K_CAST], 32 * n + n / 4, n,
+                lambda A=A: ctx.check(lib.acu_cast_decimal(h, C.byref(D["38,10"]), C.byref(D["38,2"]), 1, C.byref(A), C.byref(o))),
+                note="infallible downscale (38 - 8 < 38): unary, rounded half away from zero")
+        b.timed(f"decimal128 cast (38,10)->float64 {label}", [abi.K_CAST], 24 * n + n / 4, n,
+                lambda A=A: ctx.check(lib.acu_cast_from_decimal(h, C.byref(D["38,10"]), abi.F64, 1, C.byref(A), C.byref(o))))
+        b.timed(f"decimal128 cast (38,2)->int64 {label}", [abi.K_CAST], 24 * n + n / 4, n,
+                lambda A=A: ctx.check(lib.acu_cast_from_decimal(h, C.byref(D["38,2"]), abi.I64, 1, C.byref(A), C.byref(o))))
+    A64 = b.arr(d64, va, n, n - nva)
+    b.timed("decimal64 cast (18,2)->decimal128(38,6)", [abi.K_CAST], 24 * n + n / 4, n,
+            lambda: ctx.check(lib.acu_cast_decimal(h, C.byref(D["18,2"]), C.byref(D["38,6"]), 1, C.byref(A64), C.byref(o))),
+            note="infallible widening upscale")
+    b.timed("decimal cast int64->decimal128(38,2)", [abi.K_CAST], 24 * n + n / 4, n,
+            lambda: ctx.check(lib.acu_cast_to_decimal(h, abi.I64, C.byref(D["38,2"]), 1, C.byref(A64), C.byref(o))))
+    AF = b.arr(df, va, n, n - nva)
+    b.timed("decimal cast float64->decimal128(38,10)", [abi.K_CAST], 24 * n + n / 4, n,
+            lambda: ctx.check(lib.acu_cast_to_decimal(h, abi.F64, C.byref(D["38,10"]), 1, C.byref(AF), C.byref(o))))
+    for d in (d128, d128w, d64, df, va, o.values, o.validity):
+        ctx.free(d)
 
 
 def dict_view_column(b, ctx, keys, offs, data, D, ns):
