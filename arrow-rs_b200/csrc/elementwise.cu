@@ -1,4 +1,4 @@
-// elementwise.cu — numeric::{add,sub,mul,div,rem,neg}(_wrapping), cmp::*, cast (numeric).
+// elementwise.cu — numeric::{add,sub,mul,div,rem,neg}(_wrapping), cmp::*, cast (numeric and decimal).
 //
 // Reference: arrow-arith/src/numeric.rs:36-374, arrow-arith/src/arity.rs:104-135,254-299,
 // arrow-array/src/array/primitive_array.rs:916-1103, arrow-array/src/arithmetic.rs:148-437,
@@ -57,6 +57,10 @@ __device__ __forceinline__ uint64_t ones_to(int64_t row, int64_t n) {  // bits [
   int64_t k = n - row;
   return k >= 64 ? ~0ull : (k <= 0 ? 0ull : ((~0ull) >> (64 - k)));
 }
+
+// 256-thread CTAs for n rows: 8 warps per CTA, one 2048-row super-group per warp step; a column shorter than 2048 rows
+// still gets warp 0, which finishes the ragged tail.
+int64_t sg_blocks(int64_t n) { return (n / 2048 + 1 + 7) / 8; }
 
 // ---------------------------------------------------------------------------------------
 // Per-element arithmetic (ArrowNativeTypeOp, arithmetic.rs:148-437)
@@ -394,13 +398,11 @@ acu_status launch_arith(acu_ctx *ctx, const ArithParams<T> &p) {
   constexpr int EPLV = 16 / sizeof(T);
   bool aligned = ((uintptr_t)p.out % 16 == 0) && (p.a_scalar || (uintptr_t)p.a % 16 == 0) &&
                  (p.b_scalar || (uintptr_t)p.b % 16 == 0);
-  if (aligned) {
-    int64_t blocks = (p.n / 2048 + 1 + 7) / 8;  // 8 warps per CTA, one 2048-row super-group per warp step
+  const int64_t blocks = sg_blocks(p.n);
+  if (aligned)
     ACU_LAUNCH_TIMED(ctx, ACU_K_ARITH, (k_arith<T, CLS, EPLV>), acu_wave_grid(ctx, k_arith<T, CLS, EPLV>, 256, 0, blocks), 256, 0, p);
-  } else {
-    int64_t blocks = (p.n / 2048 + 1 + 7) / 8;
+  else
     ACU_LAUNCH_TIMED(ctx, ACU_K_ARITH, (k_arith<T, CLS, 1>), acu_wave_grid(ctx, k_arith<T, CLS, 1>, 256, 0, blocks), 256, 0, p);
-  }
   return ACU_OK;
 }
 
@@ -798,7 +800,7 @@ __global__ void __launch_bounds__(256, 4) k_cmp(const CmpParams<T> p) {
 
 template <class T, int EPL>
 acu_status launch_cmp(acu_ctx *ctx, bool lt, const CmpParams<T> &p) {
-  const int64_t blocks = (p.n / 2048 + 1 + 7) / 8;  // 8 warps per CTA; a column shorter than 2048 rows still gets warp 0
+  const int64_t blocks = sg_blocks(p.n);
   if (lt) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, true, EPL>), acu_wave_grid(ctx, k_cmp<T, true, EPL>, 256, 0, blocks), 256, 0, p);
   else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_cmp<T, false, EPL>), acu_wave_grid(ctx, k_cmp<T, false, EPL>, 256, 0, blocks), 256, 0, p);
   return ACU_OK;
@@ -1010,59 +1012,6 @@ __global__ void __launch_bounds__(256, 4) k_cast(const I *__restrict__ in, O *__
   if (fallible && err != ~0ull) atomicMin(res + RES_ERR_INDEX, err);
 }
 
-template <class I, class O>
-acu_status cast_typed(acu_ctx *ctx, acu_dtype to, int32_t safe, const acu_array *a, acu_array_out *out) {
-  const int64_t len = a->len;
-  out->len = len;
-  out->null_count = 0;
-  // numeric_cast (safe) always carries a NullBuffer; try_numeric_cast clones the input's
-  out->has_validity = safe ? 1 : (a->validity != nullptr);
-  if (len == 0) return ACU_OK;
-  uint64_t *ov = out->has_validity ? reinterpret_cast<uint64_t *>(out->validity) : nullptr;
-  ACU_TRY(acu_res_reset(ctx));
-  const I *in = static_cast<const I *>(a->values);
-  O *o = static_cast<O *>(out->values);
-  // An 8-byte input read one element per lane is already one coalesced 256-B warp request; on an H100 that beats 16-B
-  // vectors for these casts (f64 -> i32 and i64 -> f64 at 1e8 and 1e9 rows), so only narrower inputs are vectorised.
-  constexpr int EPLV = sizeof(I) == 8 ? 1 : 16 / sizeof(I);
-  const int64_t blocks = (len / 2048 + 1 + 7) / 8;
-  if ((uintptr_t)in % 16 == 0 && (uintptr_t)o % 16 == 0)
-    ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast<I, O, EPLV>), acu_wave_grid(ctx, k_cast<I, O, EPLV>, 256, 0, blocks), 256, 0,
-                     in, o, len, a->validity, a->validity_offset, ov, safe, ctx->d_res);
-  else
-    ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast<I, O, 1>), acu_wave_grid(ctx, k_cast<I, O, 1>, 256, 0, blocks), 256, 0,
-                     in, o, len, a->validity, a->validity_offset, ov, safe, ctx->d_res);
-  ACU_TRY(acu_res_fetch(ctx));
-  if (!safe && ctx->h_res[RES_ERR_INDEX] != ~0ull) {
-    const int64_t idx = (int64_t)ctx->h_res[RES_ERR_INDEX];
-    I v;
-    ACU_CUDA(ctx, cudaMemcpyAsync(&v, static_cast<const I *>(a->values) + idx, sizeof(I), cudaMemcpyDeviceToHost, ctx->stream));
-    ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-    char s[40];
-    fmt_native(s, sizeof s, v);
-    return acu_fail(ctx, ACU_ERR_CAST, idx, bits_of(v), 0, 0, "Can't cast value %s to type %s", s, acu_dtype_name(to));
-  }
-  if (ov) out->null_count = len - (int64_t)ctx->h_res[RES_COUNT];
-  return ACU_OK;
-}
-
-template <class I>
-acu_status cast_from(acu_ctx *ctx, acu_dtype to, int32_t safe, const acu_array *a, acu_array_out *out) {
-  switch (to) {
-    case ACU_I8: return cast_typed<I, int8_t>(ctx, to, safe, a, out);
-    case ACU_I16: return cast_typed<I, int16_t>(ctx, to, safe, a, out);
-    case ACU_I32: return cast_typed<I, int32_t>(ctx, to, safe, a, out);
-    case ACU_I64: return cast_typed<I, int64_t>(ctx, to, safe, a, out);
-    case ACU_U8: return cast_typed<I, uint8_t>(ctx, to, safe, a, out);
-    case ACU_U16: return cast_typed<I, uint16_t>(ctx, to, safe, a, out);
-    case ACU_U32: return cast_typed<I, uint32_t>(ctx, to, safe, a, out);
-    case ACU_U64: return cast_typed<I, uint64_t>(ctx, to, safe, a, out);
-    case ACU_F32: return cast_typed<I, float>(ctx, to, safe, a, out);
-    case ACU_F64: return cast_typed<I, double>(ctx, to, safe, a, out);
-  }
-  return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast to dtype %d", (int)to);
-}
-
 // ACU_I128 values are read and written as 16-byte vectors: the pointers must have the alignment of i128.
 acu_status i128_aligned(acu_ctx *ctx, const void *x, const void *y) {
   if (((uintptr_t)x | (uintptr_t)y) % 16 != 0)
@@ -1158,9 +1107,11 @@ acu_status decimal_typed(acu_ctx *ctx, acu_arith_op op, const acu_decimal_type &
 // ---------------------------------------------------------------------------------------
 // Decimal casts (arrow-cast/src/cast/decimal.rs:161-529, :836-1004; mod.rs:86-92, :366-444). One row function per kind,
 // shared by the device and the host replay of a failing row. Every per-call constant (10^k, the rounding half, the output
-// precision's bounds, the powi multiplier) is computed once on the host.
+// precision's bounds, the powi multiplier) is computed once on the host. cast_launch launches and finalises these and
+// the numeric casts (DK_NUM: k_cast over num_cast).
 // ---------------------------------------------------------------------------------------
-enum { DK_DEC = 0, DK_INT = 1, DK_FLOAT = 2, DK_TO_INT = 3, DK_TO_FLOAT = 4 };  // decimal / integer / float -> decimal, decimal -> integer / float
+// decimal / integer / float -> decimal, decimal -> integer / float, numeric -> numeric
+enum { DK_DEC = 0, DK_INT = 1, DK_FLOAT = 2, DK_TO_INT = 3, DK_TO_FLOAT = 4, DK_NUM = 5 };
 enum { DM_UNARY = 0, DM_OPT = 1, DM_TRY = 2 };  // unary (every slot; a failure is the unwrap panic), unary_opt / builder (valid slots; failure -> null), try_unary (valid slots; failure -> error)
 enum { DR_OK = 0, DR_NONE = 1, DR_MUL = 2, DR_PRECISION = 3 };  // row outcome: the conversion returned None / the checked multiply failed / outside the output precision
 
@@ -1323,8 +1274,10 @@ struct DcastParams {
 
 // k_cast's layout, one element per lane and load (rows are 4-16 B, so a warp-wide load is already one coalesced
 // 128-512 B request): 2048-row super-groups, lane-owned validity words, the ragged tail finished by warp 0, the lowest
-// failing row by atomicMin. A sibling of k_cast rather than k_cast over a row functor: the decimal rows carry a 112-byte
-// parameter block and 128-bit steps that k_cast's numeric instantiations should not pay for in registers.
+// failing row by atomicMin. A sibling of k_cast rather than k_cast over this row function: ptxas (CUDA 12.9, sm_90a) gives
+// the merged kernel more registers either way its parameters are passed. With one parameter struct, 95 of the 170
+// numeric casts grow (up to +6, e.g. i32 -> i8 48 -> 54); with k_cast's separate parameters, 15 of these 69 do
+// (i128 -> Decimal32 rescale 72 -> 96, i8 -> Decimal64 40 -> 48).
 template <class I, class O, int KIND>
 __global__ void __launch_bounds__(256, (sizeof(I) == 16 || sizeof(O) == 16) ? 2 : 4) k_dcast(const DcastParams<I, O> p) {
   constexpr int U = 4;  // loads in flight per lane
@@ -1527,60 +1480,73 @@ struct DcastCall {
 };
 
 template <class I, class O, int KIND>
-acu_status dcast_launch(acu_ctx *ctx, const DcastCall &c, const DcastArgs &args, const acu_array *a, acu_array_out *out) {
+acu_status cast_launch(acu_ctx *ctx, const DcastCall &c, const DcastArgs &args, const acu_array *a, acu_array_out *out) {
   const int64_t len = a->len;
   out->len = len;
   out->null_count = 0;
-  // unary_opt always carries a NullBuffer; unary / try_unary clone the input's; the builder decides after the rows
+  // unary_opt (numeric_cast when safe) always carries a NullBuffer; unary / try_unary clone the input's; the builder
+  // decides after the rows
   out->has_validity = c.mode == DM_OPT || (a->validity != nullptr);
   if (len == 0) {
     if (c.builder) out->has_validity = 0;
     return ACU_OK;
   }
-  DcastParams<I, O> p{};
-  p.in = static_cast<const I *>(a->values);
-  p.out = static_cast<O *>(out->values);
-  p.n = len;
-  p.iv = a->validity;
-  p.ioff = a->validity_offset;
-  p.out_valid = out->has_validity ? reinterpret_cast<uint64_t *>(out->validity) : nullptr;
-  p.res = ctx->d_res;
-  p.mode = c.mode;
-  p.a = args;
+  const I *in = static_cast<const I *>(a->values);
+  O *dst = static_cast<O *>(out->values);
+  uint64_t *ov = out->has_validity ? reinterpret_cast<uint64_t *>(out->validity) : nullptr;
   ACU_TRY(acu_res_reset(ctx));
-  const int64_t blocks = (len / 2048 + 1 + 7) / 8;
-  ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_dcast<I, O, KIND>), acu_wave_grid(ctx, k_dcast<I, O, KIND>, 256, 0, blocks), 256, 0, p);
+  const int64_t blocks = sg_blocks(len);
+  if constexpr (KIND == DK_NUM) {
+    // An 8-byte input read one element per lane is already one coalesced 256-B warp request; on an H100 that beats 16-B
+    // vectors for these casts (f64 -> i32 and i64 -> f64 at 1e8 and 1e9 rows), so only narrower inputs are vectorised.
+    constexpr int EPLV = sizeof(I) == 8 ? 1 : 16 / sizeof(I);
+    if ((uintptr_t)in % 16 == 0 && (uintptr_t)dst % 16 == 0)
+      ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast<I, O, EPLV>), acu_wave_grid(ctx, k_cast<I, O, EPLV>, 256, 0, blocks), 256, 0,
+                       in, dst, len, a->validity, a->validity_offset, ov, c.safe, ctx->d_res);
+    else
+      ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_cast<I, O, 1>), acu_wave_grid(ctx, k_cast<I, O, 1>, 256, 0, blocks), 256, 0,
+                       in, dst, len, a->validity, a->validity_offset, ov, c.safe, ctx->d_res);
+  } else {
+    const DcastParams<I, O> p{in, dst, len, a->validity, a->validity_offset, ov, ctx->d_res, c.mode, args};
+    ACU_LAUNCH_TIMED(ctx, ACU_K_CAST, (k_dcast<I, O, KIND>), acu_wave_grid(ctx, k_dcast<I, O, KIND>, 256, 0, blocks), 256, 0, p);
+  }
   ACU_TRY(acu_res_fetch(ctx));
   if (ctx->h_res[RES_ERR_INDEX] != ~0ull) {
     const int64_t idx = (int64_t)ctx->h_res[RES_ERR_INDEX];
     I v;
-    ACU_CUDA(ctx, cudaMemcpyAsync(&v, p.in + idx, sizeof(I), cudaMemcpyDeviceToHost, ctx->stream));
+    ACU_CUDA(ctx, cudaMemcpyAsync(&v, in + idx, sizeof(I), cudaMemcpyDeviceToHost, ctx->stream));
     ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     const uint64_t bits = bits_of(v);
-    if (c.mode == DM_UNARY)  // from_decimal(x).unwrap() / f_fallible(x).unwrap() on a slot that does not convert
-      return acu_fail(ctx, ACU_ERR_PANIC_OUT_OF_BOUNDS, idx, bits, 0, 0, "called `Option::unwrap()` on a `None` value");
-    O o;
-    __int128 mid = 0;
-    const int r = dcast_row<I, O, KIND>(args, v, o, mid);
-    char vs[64], ms[48], ks[48];
-    fmt_value(vs, sizeof vs, v);
-    fmt_i128(ms, sizeof ms, mid);
-    fmt_i128(ks, sizeof ks, args.k);
-    if (r == DR_PRECISION) return precision_error(ctx, c.out_width, mid, c.precision, c.scale, idx, bits);
-    if (r == DR_MUL) return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, bits, 0, 0, "Overflow happened on: %s * %s", ms, ks);
-    if (KIND == DK_TO_INT)
-      return acu_fail(ctx, ACU_ERR_CAST, idx, bits, 0, 0, "value of %s is out of range %s", ms, acu_dtype_name(c.out_dtype));
-    return acu_fail(ctx, ACU_ERR_CAST, idx, bits, 0, 0, "Cannot cast to %s(%d, %d). Overflowing on %s", decimal_name(c.out_width),
-                    (int)c.precision, (int)c.scale, vs);
+    if constexpr (KIND == DK_NUM) {  // try_numeric_cast: num_traits::cast returned None
+      char s[40];
+      fmt_native(s, sizeof s, v);
+      return acu_fail(ctx, ACU_ERR_CAST, idx, bits, 0, 0, "Can't cast value %s to type %s", s, acu_dtype_name(c.out_dtype));
+    } else {
+      if (c.mode == DM_UNARY)  // from_decimal(x).unwrap() / f_fallible(x).unwrap() on a slot that does not convert
+        return acu_fail(ctx, ACU_ERR_PANIC_OUT_OF_BOUNDS, idx, bits, 0, 0, "called `Option::unwrap()` on a `None` value");
+      O o;
+      __int128 mid = 0;
+      const int r = dcast_row<I, O, KIND>(args, v, o, mid);
+      char vs[64], ms[48], ks[48];
+      fmt_value(vs, sizeof vs, v);
+      fmt_i128(ms, sizeof ms, mid);
+      fmt_i128(ks, sizeof ks, args.k);
+      if (r == DR_PRECISION) return precision_error(ctx, c.out_width, mid, c.precision, c.scale, idx, bits);
+      if (r == DR_MUL) return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, bits, 0, 0, "Overflow happened on: %s * %s", ms, ks);
+      if (KIND == DK_TO_INT)
+        return acu_fail(ctx, ACU_ERR_CAST, idx, bits, 0, 0, "value of %s is out of range %s", ms, acu_dtype_name(c.out_dtype));
+      return acu_fail(ctx, ACU_ERR_CAST, idx, bits, 0, 0, "Cannot cast to %s(%d, %d). Overflowing on %s", decimal_name(c.out_width),
+                      (int)c.precision, (int)c.scale, vs);
+    }
   }
-  if (p.out_valid) out->null_count = len - (int64_t)ctx->h_res[RES_COUNT];
+  if (ov) out->null_count = len - (int64_t)ctx->h_res[RES_COUNT];
   if (c.builder && out->null_count == 0) out->has_validity = 0;
   return ACU_OK;
 }
 
 template <class I, class O, int KIND>
 acu_status dcast_to_decimal(acu_ctx *ctx, const DcastCall &c, const DcastArgs &args, const acu_array *a, acu_array_out *out) {
-  ACU_TRY((dcast_launch<I, O, KIND>(ctx, c, args, a, out)));
+  ACU_TRY((cast_launch<I, O, KIND>(ctx, c, args, a, out)));
   const int mp = dec_max_precision(c.out_width);
   return decimal_validate(ctx, mp, mp, c.precision, c.scale);  // with_precision_and_scale, after the rows
 }
@@ -1674,7 +1640,7 @@ acu_status cast_from_decimal_typed(acu_ctx *ctx, const acu_decimal_type &from, a
   if constexpr (is_fp<O>::value) {
     DcastCall c{DK_TO_FLOAT, DM_UNARY, safe, 0, 0, 0, to, false};
     args.fk = powi10(from.scale);
-    return dcast_launch<I, O, DK_TO_FLOAT>(ctx, c, args, a, out);
+    return cast_launch<I, O, DK_TO_FLOAT>(ctx, c, args, a, out);
   } else {
     DcastCall c{DK_TO_INT, safe ? DM_OPT : DM_TRY, safe, 0, 0, 0, to, true};
     const uint32_t e = from.scale < 0 ? (uint32_t)(-(int)from.scale) : (uint32_t)from.scale;
@@ -1684,27 +1650,18 @@ acu_status cast_from_decimal_typed(acu_ctx *ctx, const acu_decimal_type &from, a
                       decimal_name(from.byte_width), (int)from.scale);
     set_k(args, (int)e);
     args.down = from.scale >= 0;
-    return dcast_launch<I, O, DK_TO_INT>(ctx, c, args, a, out);
+    return cast_launch<I, O, DK_TO_INT>(ctx, c, args, a, out);
   }
 }
 
 template <class I>
 acu_status cast_from_decimal_to(acu_ctx *ctx, const acu_decimal_type &from, acu_dtype to, int32_t safe, const acu_array *a,
                                 acu_array_out *out) {
-  switch (to) {
-    case ACU_I8: return cast_from_decimal_typed<I, int8_t>(ctx, from, to, safe, a, out);
-    case ACU_I16: return cast_from_decimal_typed<I, int16_t>(ctx, from, to, safe, a, out);
-    case ACU_I32: return cast_from_decimal_typed<I, int32_t>(ctx, from, to, safe, a, out);
-    case ACU_I64: return cast_from_decimal_typed<I, int64_t>(ctx, from, to, safe, a, out);
-    case ACU_U8: return cast_from_decimal_typed<I, uint8_t>(ctx, from, to, safe, a, out);
-    case ACU_U16: return cast_from_decimal_typed<I, uint16_t>(ctx, from, to, safe, a, out);
-    case ACU_U32: return cast_from_decimal_typed<I, uint32_t>(ctx, from, to, safe, a, out);
-    case ACU_U64: return cast_from_decimal_typed<I, uint64_t>(ctx, from, to, safe, a, out);
-    case ACU_F32: return cast_from_decimal_typed<I, float>(ctx, from, to, safe, a, out);
-    case ACU_F64: return cast_from_decimal_typed<I, double>(ctx, from, to, safe, a, out);
-    default: break;
-  }
-  return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from %s to dtype %d", decimal_name(from.byte_width), (int)to);
+  return acu_with_native(
+      to, [&](auto o) { return cast_from_decimal_typed<I, decltype(o)>(ctx, from, to, safe, a, out); },
+      [&] {
+        return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from %s to dtype %d", decimal_name(from.byte_width), (int)to);
+      });
 }
 
 // the operand's decimal type is an array's: refused like an invalid type (with_precision_and_scale) at call time
@@ -1718,48 +1675,37 @@ acu_status decimal_type_ok(acu_ctx *ctx, const acu_decimal_type *t) {
 
 }  // namespace
 
-#define ACU_DISPATCH(dt, F, ...)                         \
-  switch (dt) {                                          \
-    case ACU_I8: return F<int8_t>(__VA_ARGS__);          \
-    case ACU_I16: return F<int16_t>(__VA_ARGS__);        \
-    case ACU_I32: return F<int32_t>(__VA_ARGS__);        \
-    case ACU_I64: return F<int64_t>(__VA_ARGS__);        \
-    case ACU_U8: return F<uint8_t>(__VA_ARGS__);         \
-    case ACU_U16: return F<uint16_t>(__VA_ARGS__);       \
-    case ACU_U32: return F<uint32_t>(__VA_ARGS__);       \
-    case ACU_U64: return F<uint64_t>(__VA_ARGS__);       \
-    case ACU_F32: return F<float>(__VA_ARGS__);          \
-    case ACU_F64: return F<double>(__VA_ARGS__);         \
-  }
-
 extern "C" acu_status acu_arith(acu_ctx *ctx, acu_dtype dtype, acu_arith_op op, const acu_array *a,
                                 const acu_array *b, acu_array_out *out) {
   ACU_ENTER(ctx);
-  ACU_DISPATCH(dtype, arith_typed, ctx, op, a, b, out)
-  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: dtype %d", (int)dtype);
+  return acu_with_native(
+      dtype, [&](auto t) { return arith_typed<decltype(t)>(ctx, op, a, b, out); },
+      [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: dtype %d", (int)dtype); });
 }
 
 extern "C" acu_status acu_neg(acu_ctx *ctx, acu_dtype dtype, int32_t checked, const acu_array *a, acu_array_out *out) {
   ACU_ENTER(ctx);
   if (checked && (dtype == ACU_U8 || dtype == ACU_U16 || dtype == ACU_U32 || dtype == ACU_U64))  // numeric.rs:174-176
     return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: !%s", acu_dtype_name(dtype));
-  ACU_DISPATCH(dtype, neg_typed, ctx, checked, a, out)
   if (dtype == ACU_I128) {
     ACU_TRY(i128_aligned(ctx, a->values, out->values));
     return neg_typed<__int128>(ctx, 1, a, out);
   }
-  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: dtype %d", (int)dtype);
+  return acu_with_native(
+      dtype, [&](auto t) { return neg_typed<decltype(t)>(ctx, checked, a, out); },
+      [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: dtype %d", (int)dtype); });
 }
 
 extern "C" acu_status acu_cmp(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, const acu_array *a,
                               const acu_array *b, acu_array_out *out) {
   ACU_ENTER(ctx);
-  ACU_DISPATCH(dtype, cmp_typed, ctx, op, a, b, out)
   if (dtype == ACU_I128) {
     ACU_TRY(i128_aligned(ctx, a->values, b->values));
     return cmp_typed<__int128>(ctx, op, a, b, out);
   }
-  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid comparison operation: dtype %d", (int)dtype);
+  return acu_with_native(
+      dtype, [&](auto t) { return cmp_typed<decltype(t)>(ctx, op, a, b, out); },
+      [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid comparison operation: dtype %d", (int)dtype); });
 }
 
 acu_status acu_cmp_len(acu_ctx *ctx, const acu_array *l, const acu_array *r, int64_t *len) {
@@ -1827,19 +1773,28 @@ acu_status acu_cmp_into_plan(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, const
   CmpFuse f{mask, n_words_padded, tile_count, n_tiles};
   const CmpFuse *fuse = &f;
   acu_array_out *out = nullptr;
-  ACU_DISPATCH(dtype, cmp_typed, ctx, op, a, b, out, fuse)
   if (dtype == ACU_I128) {
     ACU_TRY(i128_aligned(ctx, a->values, b->values));
     return cmp_typed<__int128>(ctx, op, a, b, out, fuse);
   }
-  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid comparison operation: dtype %d", (int)dtype);
+  return acu_with_native(
+      dtype, [&](auto t) { return cmp_typed<decltype(t)>(ctx, op, a, b, out, fuse); },
+      [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid comparison operation: dtype %d", (int)dtype); });
 }
 
 extern "C" acu_status acu_cast_numeric(acu_ctx *ctx, acu_dtype from, acu_dtype to, int32_t safe,
                                        const acu_array *a, acu_array_out *out) {
   ACU_ENTER(ctx);
-  ACU_DISPATCH(from, cast_from, ctx, to, safe, a, out)
-  return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from dtype %d", (int)from);
+  // numeric_cast (unary_opt: a value that does not fit O is null) / try_numeric_cast (try_unary: it is an error)
+  const DcastCall c{DK_NUM, safe ? DM_OPT : DM_TRY, safe, 0, 0, 0, to, false};
+  return acu_with_native(
+      from,
+      [&](auto i) {
+        return acu_with_native(
+            to, [&](auto o) { return cast_launch<decltype(i), decltype(o), DK_NUM>(ctx, c, DcastArgs{}, a, out); },
+            [&] { return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast to dtype %d", (int)to); });
+      },
+      [&] { return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from dtype %d", (int)from); });
 }
 
 extern "C" acu_status acu_decimal_arith(acu_ctx *ctx, acu_arith_op op, const acu_decimal_type *lt, const acu_array *a,
@@ -1878,20 +1833,16 @@ extern "C" acu_status acu_cast_to_decimal(acu_ctx *ctx, acu_dtype from, const ac
   if (to->byte_width != 4 && to->byte_width != 8 && to->byte_width != 16)
     return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid decimal type: byte width %d", (int)to->byte_width);
   if (to->byte_width == 16) ACU_TRY(i128_aligned(ctx, out->values, nullptr));
-  switch (from) {
-    case ACU_I8: return cast_int_to_decimal<int8_t>(ctx, *to, safe, a, out);
-    case ACU_I16: return cast_int_to_decimal<int16_t>(ctx, *to, safe, a, out);
-    case ACU_I32: return cast_int_to_decimal<int32_t>(ctx, *to, safe, a, out);
-    case ACU_I64: return cast_int_to_decimal<int64_t>(ctx, *to, safe, a, out);
-    case ACU_U8: return cast_int_to_decimal<uint8_t>(ctx, *to, safe, a, out);
-    case ACU_U16: return cast_int_to_decimal<uint16_t>(ctx, *to, safe, a, out);
-    case ACU_U32: return cast_int_to_decimal<uint32_t>(ctx, *to, safe, a, out);
-    case ACU_U64: return cast_int_to_decimal<uint64_t>(ctx, *to, safe, a, out);
-    case ACU_F32: return cast_float_to_decimal<float>(ctx, *to, safe, a, out);
-    case ACU_F64: return cast_float_to_decimal<double>(ctx, *to, safe, a, out);
-    default: break;
-  }
-  return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from dtype %d to %s", (int)from, decimal_name(to->byte_width));
+  return acu_with_native(
+      from,
+      [&](auto i) {
+        using I = decltype(i);
+        if constexpr (is_fp<I>::value) return cast_float_to_decimal<I>(ctx, *to, safe, a, out);
+        else return cast_int_to_decimal<I>(ctx, *to, safe, a, out);
+      },
+      [&] {
+        return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "cast from dtype %d to %s", (int)from, decimal_name(to->byte_width));
+      });
 }
 
 extern "C" acu_status acu_cast_from_decimal(acu_ctx *ctx, const acu_decimal_type *from, acu_dtype to, int32_t safe,

@@ -2,6 +2,25 @@
 #pragma once
 #include "common.cuh"
 
+// f(T()) for T the native type of a numeric dtype (ACU_I8 .. ACU_F64), otherwise(): one dtype -> C++ type mapping
+// for the typed entry points, each keeping its own failure for the dtypes it does not take.
+template <class F, class G>
+auto acu_with_native(acu_dtype dt, F &&f, G &&otherwise) -> decltype(otherwise()) {
+  switch (dt) {
+    case ACU_I8: return f(int8_t());
+    case ACU_I16: return f(int16_t());
+    case ACU_I32: return f(int32_t());
+    case ACU_I64: return f(int64_t());
+    case ACU_U8: return f(uint8_t());
+    case ACU_U16: return f(uint16_t());
+    case ACU_U32: return f(uint32_t());
+    case ACU_U64: return f(uint64_t());
+    case ACU_F32: return f(float());
+    case ACU_F64: return f(double());
+    default: return otherwise();
+  }
+}
+
 struct acu_filter_plan;
 const uint64_t *acu_plan_mask(const acu_filter_plan *p);      // normalised mask words (padded to x32)
 const uint64_t *acu_plan_tile_off(const acu_filter_plan *p);  // exclusive output offset per 1024-row tile

@@ -196,19 +196,9 @@ acu_status reduce_typed(acu_ctx *ctx, acu_agg_op op, const ReduceBatch &rb, int 
 }
 
 acu_status reduce_dispatch(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const ReduceBatch &rb, int n_cols, int64_t max_len) {
-  switch (dtype) {
-    case ACU_I8: return reduce_typed<int8_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_I16: return reduce_typed<int16_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_I32: return reduce_typed<int32_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_I64: return reduce_typed<int64_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_U8: return reduce_typed<uint8_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_U16: return reduce_typed<uint16_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_U32: return reduce_typed<uint32_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_U64: return reduce_typed<uint64_t>(ctx, op, rb, n_cols, max_len);
-    case ACU_F32: return reduce_typed<float>(ctx, op, rb, n_cols, max_len);
-    case ACU_F64: return reduce_typed<double>(ctx, op, rb, n_cols, max_len);
-  }
-  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "aggregate: dtype %d", (int)dtype);
+  return acu_with_native(
+      dtype, [&](auto t) { return reduce_typed<decltype(t)>(ctx, op, rb, n_cols, max_len); },
+      [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "aggregate: dtype %d", (int)dtype); });
 }
 
 ReduceArgs reduce_args(const acu_array *a, int64_t nc, void *scratch, unsigned long long *res) {

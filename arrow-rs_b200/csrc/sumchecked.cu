@@ -215,15 +215,13 @@ extern "C" acu_status acu_sum_checked(acu_ctx *ctx, acu_dtype dtype, const acu_a
   *out_valid_count = a->len - nc;
   if (nc == a->len) return ACU_OK;  // aggregate.rs:902-904
   const uint8_t *valid = (a->validity && nc > 0) ? a->validity : nullptr;
-  switch (dtype) {
-    case ACU_I8: return sum_checked_typed<int8_t>(ctx, a, valid, out_bits);
-    case ACU_I16: return sum_checked_typed<int16_t>(ctx, a, valid, out_bits);
-    case ACU_I32: return sum_checked_typed<int32_t>(ctx, a, valid, out_bits);
-    case ACU_I64: return sum_checked_typed<int64_t>(ctx, a, valid, out_bits);
-    case ACU_U8: return sum_checked_typed<uint8_t>(ctx, a, valid, out_bits);
-    case ACU_U16: return sum_checked_typed<uint16_t>(ctx, a, valid, out_bits);
-    case ACU_U32: return sum_checked_typed<uint32_t>(ctx, a, valid, out_bits);
-    case ACU_U64: return sum_checked_typed<uint64_t>(ctx, a, valid, out_bits);
-    default: return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "sum_checked: dtype %d", (int)dtype);
-  }
+  auto fail = [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "sum_checked: dtype %d", (int)dtype); };
+  return acu_with_native(
+      dtype,
+      [&](auto t) {
+        using T = decltype(t);
+        if constexpr (std::is_integral<T>::value) return sum_checked_typed<T>(ctx, a, valid, out_bits);
+        else return fail();
+      },
+      fail);
 }
