@@ -2,9 +2,8 @@
 against tests/oracle_decimal.py, bit for bit: values (0 under nulls), validity, null_count, NullBuffer presence, result
 type, status, message and error row.
 
-Sizes: the decimal kernels run at most 2 CTAs of 8 warps per SM (k_arith<__int128> and k_reduce<__int128> use 123-128
-registers a thread) in 8 waves, so multi_round() rows (1.2 x 8 x SMs x 16 warps x 2048-row super-groups) run them through
-two grid-stride rounds. Those sizes are checked with numpy on values below 2^40, where the exact result fits an int64."""
+The multi-round size is sized() of test_gpu_elementwise_rounds: at least 1.2 rounds of an acu_wave_grid launch at any
+occupancy, checked on periodic columns (test_gpu_decimal_edges)."""
 import ctypes as C
 
 import numpy as np
@@ -14,6 +13,8 @@ import acu
 import oracle_decimal as od
 from acu import _abi as abi
 from acu import ArrowError, DecimalArray, bitmap_bytes
+from test_gpu_decimal_edges import P, Exp, Periodic, check_out, exp_from, gpu_aggregate, raw_of, run_out
+from test_gpu_elementwise_rounds import SG, sized
 from test_oracle_decimal import CMP_OPS, OPS, golden
 
 pytestmark = pytest.mark.gpu
@@ -268,48 +269,46 @@ def test_invalid_types_and_dtypes_are_rejected(gpu):
         da.free()
 
 
-# ---- injected failures across CTAs and grid-stride rounds; multi-round sizes ----------------------------------------------
-def multi_round(gpu):
-    return int(1.2 * 8 * gpu.lib.acu_device_sm_count(gpu.h) * 16 * 2048)
-
-
-def halves_of(ints64):
-    h = np.empty((len(ints64), 2), dtype=np.uint64)
-    h[:, 0] = ints64.view(np.uint64)
-    h[:, 1] = (ints64 >> 63).view(np.uint64)
-    return h
-
-
+# ---- multi-round sizes ---------------------------------------------------------------------------------------------------
 def test_multi_round_add_sum_cmp(gpu):
-    n = multi_round(gpu)
+    """add (the right operand rescaled by 100), sum / min / max and a comparison with a scalar over more than one
+    grid-stride round, on the periodic columns of test_gpu_decimal_edges (which also places failing rows for every
+    occupancy)."""
+    n = sized(gpu, SG)
     rng = np.random.default_rng(7)
-    x = rng.integers(-2 ** 39, 2 ** 39, n)
-    y = rng.integers(-2 ** 39, 2 ** 39, n)
-    mask = rng.integers(0, 100, n) >= 3
-    a = DecimalArray.from_int64(16, 38, 4, x, mask)
-    b = DecimalArray.from_int64(16, 38, 2, y)
-    r = gpu.decimal_add(a, b)
-    exp = np.where(mask, x + y * 100, 0)
-    assert (r.precision, r.scale) == (38, 4) and r.null_count == int((~mask).sum())
-    assert np.array_equal(np.asarray(r.values).reshape(-1, 2), halves_of(exp))
-    assert np.array_equal(r.valid_mask(), mask)
-    assert gpu.sum(a) == int(x[mask].sum()) and gpu.min(a) == int(x[mask].min()) and gpu.max(a) == int(x[mask].max())
-    t = int(np.median(x))
-    got = gpu.cmp(abi.LT, a, DecimalArray.from_ints(16, 38, 4, [t], scalar=True))
-    assert np.array_equal(got.value_array(), x < t) and np.array_equal(got.valid_mask(), mask)
-    # the lowest failing row lies in the LAST CTA of the first round (super-group nwarps - 1), a higher one in CTA 0 of the
-    # second round (super-group nwarps): a "lowest CTA wins" policy would report the higher row
-    del r, exp, b
-    nwarps = 8 * gpu.lib.acu_device_sm_count(gpu.h) * 2 * 8  # 8 waves x SMs x 2 CTAs of 8 warps (k_arith<__int128>)
-    assert n > (nwarps + 1) * 2048
-    lo_row, hi_row = (nwarps - 1) * 2048 + 7, nwarps * 2048 + 5
-    xx = x.copy()
-    xx[[hi_row, lo_row]] = 2 ** 62
-    a2 = DecimalArray.from_int64(16, 38, 0, xx)
-    a2.values[[hi_row, lo_row], 1] = np.uint64(1 << 62)  # |l| ~ 2^126: l * l_mul overflows
-    with pytest.raises(ArrowError) as e:
-        gpu.decimal_add(a2, DecimalArray.from_int64(16, 38, 2, y))
-    assert e.value.index == lo_row and e.value.message.startswith("Arithmetic overflow: Overflow happened on: ") and e.value.message.endswith(" * 100")
+    x = [int(v) for v in rng.integers(-2 ** 39, 2 ** 39, P)]
+    y = [int(v) for v in rng.integers(-2 ** 39, 2 ** 39, P)]
+    mask = rng.integers(0, 100, P) >= 3
+    a = Periodic(gpu, abi.I128, raw_of(DecimalArray.from_ints(16, 38, 4, x)), mask, n)
+    b = Periodic(gpu, abi.I128, raw_of(DecimalArray.from_ints(16, 38, 2, y)), None, n)
+    t = DecimalArray.from_ints(16, 38, 4, [int(np.median(x))], scalar=True)
+    dt = gpu.upload(t)
+    try:
+        ad, bd, td = a.descriptor(), b.descriptor(), dt.descriptor()
+        ox = od.Operand(16, 38, 4, x, mask.tolist())
+        exp = od.decimal_op(abi.ADD, ox, od.Operand(16, 38, 2, y))
+        lt, rt, ot = abi.DecimalType(16, 38, 4), abi.DecimalType(16, 38, 2), abi.DecimalType()
+        st, out = run_out(gpu, n, n * 16, lambda o: gpu.lib.acu_decimal_arith(gpu.h, abi.ADD, C.byref(lt), C.byref(ad), C.byref(rt),
+                                                                              C.byref(bd), C.byref(ot), C.byref(o)))
+        try:
+            assert st == abi.OK and (ot.precision, ot.scale) == (38, 4)
+            check_out(gpu, out, n, abi.I128, exp_from(exp, abi.I128), "add")
+        finally:
+            gpu._free_out(out)
+        valid = [v for v, m in zip(x, mask) if m]
+        total = (n // P) * sum(valid) + sum(v for v, m in zip(x[: n % P], mask[: n % P]) if m)
+        assert gpu_aggregate(gpu, a) == (total, min(valid), max(valid))
+        vals, validity = od.cmp(od.LT, ox, od.Operand(16, 38, 4, t.raw_ints(), None, True))
+        st, out = run_out(gpu, n, bitmap_bytes(n), lambda o: gpu.lib.acu_cmp(gpu.h, abi.I128, abi.LT, C.byref(ad), C.byref(td), C.byref(o)))
+        try:
+            assert st == abi.OK
+            check_out(gpu, out, n, acu.BOOL, Exp(np.array(vals), np.array(validity)), "cmp LT scalar")
+        finally:
+            gpu._free_out(out)
+    finally:
+        a.free()
+        b.free()
+        dt.free()
 
 
 # ---- bit offsets and zero-copy unaligned slices ---------------------------------------------------------------------------

@@ -2,9 +2,8 @@
 tests/oracle_decimal_cast.py, bit for bit: values at every slot (the unary casts compute under nulls too; the others write
 0 there), validity, null_count, NullBuffer presence, status, message and error row.
 
-k_dcast runs 8 waves of its resident CTAs (8 warps each) per SM. From the ptxas register counts (76 for
-k_dcast<__int128, __int128>, 46 for k_dcast<int64_t, int32_t>) that is 3 and 5 CTAs per SM, so multi_round() sizes
-(1.2 x 8 x SMs x CTAs x 8 warps x 2048-row super-groups) take them through a second grid-stride round."""
+The multi-round size is sized() of test_gpu_elementwise_rounds: at least 1.2 rounds of an acu_wave_grid launch at any
+occupancy, with the first failing row placed for every occupancy (test_gpu_decimal_edges)."""
 import ctypes as C
 import math
 
@@ -16,6 +15,8 @@ import oracle_decimal as od
 import oracle_decimal_cast as oc
 from acu import _abi as abi
 from acu import ArrowError, DecimalArray, HostArray
+from test_gpu_decimal_edges import P, Call, Periodic, check_out, check_placements, exp_from, raw_of, raw_value
+from test_gpu_elementwise_rounds import SG, sized
 from test_oracle_decimal_cast import golden_cases
 
 pytestmark = pytest.mark.gpu
@@ -385,37 +386,43 @@ def test_empty_arrays_raise_type_level_errors(gpu):
     assert r.length == 0 and r.validity is None
 
 
-# ---- multi-round sizes: the lowest failing row in the last CTA of round one below one in CTA 0 of round two -----------------
-def multi_round(gpu, ctas_per_sm):
-    return int(1.2 * 8 * gpu.lib.acu_device_sm_count(gpu.h) * ctas_per_sm * 8 * 2048)
-
-
-@pytest.mark.parametrize("wi,wo,ctas", [(16, 16, 3), (8, 4, 5)])
-def test_multi_round_first_error_row(gpu, wi, wo, ctas):
-    n = multi_round(gpu, ctas)
+# ---- multi-round sizes: a rescale over more than one grid-stride round, and its first failing row at every placement -------
+@pytest.mark.parametrize("wi,wo", [(16, 16), (8, 4)])
+def test_multi_round_first_error_row(gpu, wi, wo):
+    """Decimal(18, 4) -> (9 or 38, 1) on a periodic column (test_gpu_decimal_edges) with safe = True against the oracle
+    on one period; then -> (9, 1) with safe = False and 10^17 at every placement of test_gpu_elementwise_rounds."""
+    n = sized(gpu, SG)
     rng = np.random.default_rng(wi + wo)
-    x = rng.integers(-10 ** 12, 10 ** 12, n)
-    mask = rng.integers(0, 100, n) >= 3
-    a = DecimalArray.from_int64(wi, 18, 4, x, mask)
-    r = gpu.cast_decimal(a, wo, 9 if wo == 4 else 38, 1, safe=True)
-    q = np.abs(x) // 1000 + ((np.abs(x) % 1000) >= 500)
-    q = np.where(x < 0, -q, q)
-    ok = mask & (np.abs(q) <= (10 ** (9 if wo == 4 else 38) - 1))
-    assert np.array_equal(r.valid_mask(), ok) and r.null_count == int((~ok).sum())
-    vals = np.asarray(r.values).reshape(-1, 2)[:, 0].view(np.int64) if wo == 16 else np.asarray(r.values).astype(np.int64)
-    assert np.array_equal(np.where(ok, vals, 0), np.where(ok, q, 0))
-    nwarps = 8 * gpu.lib.acu_device_sm_count(gpu.h) * ctas * 8
-    assert n > (nwarps + 1) * 2048
-    lo_row, hi_row = (nwarps - 1) * 2048 + 7, nwarps * 2048 + 5
-    xx = np.where(mask, x, 0) % 10 ** 5
-    xx[[hi_row, lo_row]] = 10 ** 17
-    m2 = mask.copy()
-    m2[[hi_row, lo_row]] = True
-    a2 = DecimalArray.from_int64(wi, 18, 4, xx, m2)
-    with pytest.raises(ArrowError) as e:
-        gpu.cast_decimal(a2, wo, 9, 1, safe=False)
-    assert e.value.index == lo_row
-    if wo == 4:  # 10^14 does not convert to i32: the rescale itself fails
-        assert e.value.message == f"Cast error: Cannot cast to Decimal32(9, 1). Overflowing on {10 ** 17}"
-    else:
-        assert e.value.message == f"Invalid argument error: {10 ** 13}.0 is too large to store in a Decimal128 of precision 9. Max is 99999999.9"
+    x = [int(v) for v in rng.integers(-2 * 10 ** 12, 2 * 10 ** 12, P)]
+    mask = rng.integers(0, 100, P) >= 3
+    src, dst = {8: abi.I64, 16: abi.I128}[wi], {4: abi.I32, 16: abi.I128}[wo]
+    p_out = 9 if wo == 4 else 38
+    col = Periodic(gpu, src, raw_of(DecimalArray.from_ints(wi, 18, 4, x)), mask, n)
+    try:
+        d = col.descriptor()
+        ft, tt, t9 = abi.DecimalType(wi, 18, 4), abi.DecimalType(wo, p_out, 1), abi.DecimalType(wo, 9, 1)
+        exp = oc.cast_decimal(od.Operand(wi, 18, 4, x, mask.tolist()), wo, p_out, 1, True)
+        assert (exp.null_count > int((~mask).sum())) == (wo == 4)  # quotients past 9 digits become nulls
+        st, out = Call(gpu, n, n * wo, lambda o: gpu.lib.acu_cast_decimal(gpu.h, C.byref(ft), C.byref(tt), 1, C.byref(d), C.byref(o)))()
+        try:
+            assert st == abi.OK
+            check_out(gpu, out, n, dst, exp_from(exp, dst), f"{wi}->{wo} safe")
+        finally:
+            gpu._free_out(out)
+        # values whose quotients all fit 9 digits, then 10^17 / 10^3 = 10^14: past Decimal32's i32 (the rescale itself
+        # fails) and past 9 digits of Decimal128(9, 1)
+        small = [v % 10 ** 11 - 5 * 10 ** 10 for v in x]
+        col.base = (raw_of(DecimalArray.from_ints(wi, 18, 4, small)), mask)
+        col.restore()
+        if wo == 4:
+            err = (abi.ERR_CAST, f"Cast error: Cannot cast to Decimal32(9, 1). Overflowing on {10 ** 17}")
+        else:
+            err = (abi.ERR_INVALID_ARGUMENT, f"Invalid argument error: {10 ** 13}.0 is too large to store in a Decimal128 of precision 9. "
+                                             "Max is 99999999.9")
+        call = Call(gpu, n, n * wo, lambda o: gpu.lib.acu_cast_decimal(gpu.h, C.byref(ft), C.byref(t9), 0, C.byref(d), C.byref(o)))
+        st, out = call()
+        gpu._free_out(out)
+        assert st == abi.OK
+        check_placements(gpu, n, [(col, raw_value(src, 10 ** 17))], call, lambda: err, f"{wi}->{wo}")
+    finally:
+        col.free()
