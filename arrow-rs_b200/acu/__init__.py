@@ -932,7 +932,8 @@ class Context:
             di.free()
 
     def aggregate_columns(self, ops, columns):
-        """[sum|min|max](column) for several primitive columns with one synchronisation -> [(value|None)]."""
+        """[sum|min|max|product|bit_and|bit_or|bit_xor](column) for several primitive columns with one synchronisation ->
+        [(value|None)]."""
         n = len(columns)
         das = [self.upload(c) for c in columns]
         try:
@@ -993,6 +994,35 @@ class Context:
             da.free()
 
     def neg_wrapping(self, a): return self.neg(a, checked=False)
+
+    # -- bitwise (arrow-arith/src/bitwise.rs) ------------------------------------------------------
+    def bitwise(self, op, a, b=None):
+        """bitwise_and / or / xor / and_not / shift_left / shift_right (acu_bitwise_op) of two integer HostArrays, their
+        _scalar forms (b a scalar HostArray) and bitwise_not (op = BITWISE_NOT, b None)."""
+        assert b is None or a.dtype == b.dtype
+        da = self.upload(a)
+        db = self.upload(b) if b is not None else None
+        out = self.alloc_out(a.length * a.width(), a.length)
+        try:
+            ad = da.descriptor()
+            bd = db.descriptor() if db is not None else None
+            self.check(self.lib.acu_bitwise(self.h, a.dtype, op, C.byref(ad), C.byref(bd) if bd is not None else None, C.byref(out)))
+            res, out = self.download_out(out, a.dtype), None
+            return res
+        finally:
+            if out is not None:
+                self._free_out(out)
+            da.free()
+            if db is not None:
+                db.free()
+
+    def bitwise_and(self, a, b): return self.bitwise(abi.BITWISE_AND, a, b)
+    def bitwise_or(self, a, b): return self.bitwise(abi.BITWISE_OR, a, b)
+    def bitwise_xor(self, a, b): return self.bitwise(abi.BITWISE_XOR, a, b)
+    def bitwise_and_not(self, a, b): return self.bitwise(abi.BITWISE_AND_NOT, a, b)
+    def bitwise_shift_left(self, a, b): return self.bitwise(abi.BITWISE_SHIFT_LEFT, a, b)
+    def bitwise_shift_right(self, a, b): return self.bitwise(abi.BITWISE_SHIFT_RIGHT, a, b)
+    def bitwise_not(self, a): return self.bitwise(abi.BITWISE_NOT, a)
 
     # -- decimal arithmetic (decimal_op, arrow-arith/src/numeric.rs:970-1107) -----------------------------
     def decimal_arith(self, op, a, b):
@@ -1471,11 +1501,19 @@ class Context:
 
     def sum_checked(self, a):
         """arrow::compute::sum_checked (aggregate.rs:897): the in-order checked fold; raises ArrowError on overflow."""
+        return self._checked_fold(self.lib.acu_sum_checked, a)
+
+    def product_checked(self, a):
+        """arrow::compute::product_checked (aggregate.rs:963): the in-order checked fold of mul_checked; raises ArrowError
+        on the first overflowing valid row."""
+        return self._checked_fold(self.lib.acu_product_checked, a)
+
+    def _checked_fold(self, fn, a):
         da = self.upload(a)
         try:
             bits, cnt = C.c_uint64(0), C.c_int64(0)
             ad = da.descriptor()
-            self.check(self.lib.acu_sum_checked(self.h, a.dtype, C.byref(ad), C.byref(bits), C.byref(cnt)))
+            self.check(fn(self.h, a.dtype, C.byref(ad), C.byref(bits), C.byref(cnt)))
             if cnt.value == 0:
                 return None
             raw = np.array([bits.value], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[a.dtype]]
@@ -1486,6 +1524,10 @@ class Context:
     def sum(self, a): return self.aggregate(SUM, a)
     def min(self, a): return self.aggregate(MIN, a)
     def max(self, a): return self.aggregate(MAX, a)
+    def product(self, a): return self.aggregate(abi.PRODUCT, a)
+    def bit_and(self, a): return self.aggregate(abi.BIT_AND, a)
+    def bit_or(self, a): return self.aggregate(abi.BIT_OR, a)
+    def bit_xor(self, a): return self.aggregate(abi.BIT_XOR, a)
 
     # -- min / max of byte columns, boolean min / max (aggregate.rs:372-568, :880-889) ----------
     def min_max_row(self, op, col):

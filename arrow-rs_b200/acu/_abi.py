@@ -36,7 +36,9 @@ ADD_WRAPPING, ADD, SUB_WRAPPING, SUB, MUL_WRAPPING, MUL, DIV, REM = range(8)
 # acu_cmp_op (arrow-ord/src/cmp.rs:40-60)
 EQ, NEQ, LT, LT_EQ, GT, GT_EQ, DISTINCT, NOT_DISTINCT = range(8)
 # acu_agg_op
-SUM, MIN, MAX = range(3)
+SUM, MIN, MAX, PRODUCT, BIT_AND, BIT_OR, BIT_XOR = range(7)
+# acu_bitwise_op (arrow-arith/src/bitwise.rs)
+BITWISE_AND, BITWISE_OR, BITWISE_XOR, BITWISE_AND_NOT, BITWISE_SHIFT_LEFT, BITWISE_SHIFT_RIGHT, BITWISE_NOT = range(7)
 # acu_like_op (arrow-string/src/like.rs `enum Op`)
 LIKE, NLIKE, ILIKE, NILIKE, CONTAINS, STARTS_WITH, ENDS_WITH, EQ_IGNORE_ASCII_CASE = range(8)
 # acu_length_op (arrow-string/src/length.rs length / bit_length)
@@ -210,6 +212,7 @@ PROTOTYPES = {
     "acu_take_boolean": (i32, [vp, P(Array), P(Array), i32, i32, P(ArrayOut)]),
     "acu_take_bytes": (i32, [vp, i32, vp, vp, P(Array), P(Array), i32, i32, vp, vp, i64, P(i64), P(ArrayOut)]),
     "acu_arith": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
+    "acu_bitwise": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_neg": (i32, [vp, i32, i32, P(Array), P(ArrayOut)]),
     "acu_decimal_arith": (i32, [vp, i32, P(DecimalType), P(Array), P(DecimalType), P(Array), P(DecimalType), P(ArrayOut)]),
     "acu_cmp": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
@@ -232,6 +235,7 @@ PROTOTYPES = {
     "acu_aggregate": (i32, [vp, i32, i32, P(Array), P(u64), P(i64)]),
     "acu_aggregate_i128": (i32, [vp, i32, P(Array), P(u64), P(i64)]),
     "acu_sum_checked": (i32, [vp, i32, P(Array), P(u64), P(i64)]),
+    "acu_product_checked": (i32, [vp, i32, P(Array), P(u64), P(i64)]),
     "acu_aggregate_bytes": (i32, [vp, i32, i32, P(BytesArray), P(i64), P(i64)]),
     "acu_aggregate_byte_view": (i32, [vp, i32, P(ViewArray), P(i64), P(i64)]),
     "acu_aggregate_fixed_size_binary": (i32, [vp, i32, i32, P(Array), P(i64), P(i64)]),

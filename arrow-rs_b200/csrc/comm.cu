@@ -110,6 +110,12 @@ __global__ void k_stage_partial(const unsigned long long *res, int launched, lon
   buf[0] = encode_partial(bits, valid_count == 0, (acu_dtype)dtype, (acu_agg_op)op);
   buf[1] = (uint64_t)valid_count;
 }
+
+// The partial encodings and NCCL ops above exist for sum / min / max only; NCCL has no product or bitwise reduction.
+acu_status allreduce_op_ok(acu_ctx *ctx, acu_agg_op op) {
+  if (op == ACU_SUM || op == ACU_MIN || op == ACU_MAX) return ACU_OK;
+  return acu_fail(ctx, ACU_ERR_NOT_YET_IMPLEMENTED, -1, 0, 0, 0, "all-reduce of aggregate op %d", (int)op);
+}
 }  // namespace
 
 extern "C" {
@@ -165,6 +171,7 @@ acu_status acu_comm_allreduce_i64_sum(acu_ctx *ctx, int64_t *values, int32_t n) 
 acu_status acu_comm_allreduce_aggregates(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, uint64_t *partial_bits,
                                          int64_t *valid_counts, int32_t n) {
   ACU_ENTER(ctx);
+  ACU_TRY(allreduce_op_ok(ctx, op));
   if (ctx->world <= 1 || !ctx->nccl_comm || n <= 0) return ACU_OK;
   NcclApi *api = nccl_api();
   if (n > 32) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "at most 32 aggregates per all-reduce");
@@ -234,6 +241,7 @@ acu_status acu_comm_allreduce_aggregates(acu_ctx *ctx, acu_dtype dtype, acu_agg_
 // the block (the call's fetch, or acu_results_fetch at the end of an async section): no host bounce.
 acu_status acu_aggregate_allreduce(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a, uint64_t *out_bits,
                                    int64_t *out_valid_count) {
+  ACU_TRY(allreduce_op_ok(ctx, op));
   if (ctx->world <= 1 || !ctx->nccl_comm) return acu_aggregate(ctx, dtype, op, a, out_bits, out_valid_count);
   ACU_ENTER(ctx);
   NcclApi *api = nccl_api();

@@ -1,6 +1,6 @@
-// elementwise.cu — numeric::{add,sub,mul,div,rem,neg}(_wrapping), cmp::*, cast (numeric and decimal).
+// elementwise.cu — numeric::{add,sub,mul,div,rem,neg}(_wrapping), bitwise::*, cmp::*, cast (numeric and decimal).
 //
-// Reference: arrow-arith/src/numeric.rs:36-374, arrow-arith/src/arity.rs:104-135,254-299,
+// Reference: arrow-arith/src/numeric.rs:36-374, arrow-arith/src/bitwise.rs, arrow-arith/src/arity.rs:104-135,254-299,
 // arrow-array/src/array/primitive_array.rs:916-1103, arrow-array/src/arithmetic.rs:148-437,
 // arrow-ord/src/cmp.rs:220-648, arrow-cast/src/cast/mod.rs:2550-2614.
 //
@@ -65,7 +65,7 @@ int64_t sg_blocks(int64_t n) { return (n / 2048 + 1 + 7) / 8; }
 // ---------------------------------------------------------------------------------------
 // Per-element arithmetic (ArrowNativeTypeOp, arithmetic.rs:148-437)
 // ---------------------------------------------------------------------------------------
-enum { CLS_WRAP = 0, CLS_CHECKED = 1, CLS_DIVREM = 2, CLS_DECIMAL = 3 };
+enum { CLS_WRAP = 0, CLS_CHECKED = 1, CLS_DIVREM = 2, CLS_DECIMAL = 3, CLS_BITWISE = 4 };
 enum { OP_ADD = 0, OP_SUB = 1, OP_MUL = 2, OP_DIV = 3, OP_REM = 4, OP_NEG = 5 };
 
 template <class T> struct is_fp { static constexpr bool value = std::is_floating_point<T>::value; };
@@ -147,6 +147,120 @@ __device__ __forceinline__ bool apply_op(int op, T l, T r, T &o) {
       return false;
     }
   }
+}
+
+// bitwise.rs rows (op = acu_bitwise_op), integer T only. Shifts are wrapping_shl / wrapping_shr by b's bit pattern modulo
+// the width (bitwise.rs:81-111, :176-207). Narrow values shift in 32 bits: a left shift of a negative signed value is
+// undefined, and a narrow unsigned one would be promoted to int.
+template <int OP, class T> __device__ __forceinline__ T bitwise_row(T l, T r) {
+  using U = typename std::make_unsigned<T>::type;
+  using W = typename std::conditional<(sizeof(T) < 4), uint32_t, U>::type;
+  using SW = typename std::conditional<(sizeof(T) < 4), int32_t, T>::type;
+  const unsigned amt = (unsigned)((U)r & (U)(8 * sizeof(T) - 1));
+  if constexpr (OP == ACU_BITWISE_AND) return l & r;
+  else if constexpr (OP == ACU_BITWISE_OR) return l | r;
+  else if constexpr (OP == ACU_BITWISE_XOR) return l ^ r;
+  else if constexpr (OP == ACU_BITWISE_AND_NOT) return l & (T)~r;
+  else if constexpr (OP == ACU_BITWISE_SHIFT_LEFT) return (T)((W)(U)l << amt);
+  else if constexpr (OP == ACU_BITWISE_SHIFT_RIGHT) {  // arithmetic for signed, logical for unsigned T
+    if constexpr (std::is_signed<T>::value) return (T)((SW)l >> amt);
+    else return (T)((W)l >> amt);
+  } else {
+    return (T)~l;  // not
+  }
+}
+// f(integral_constant<op>): one straight-line body per op, so that the op is decided once per strip group and not at
+// each of its (up to 64 narrow) elements, which would spill
+template <class F> __device__ __forceinline__ void bitwise_dispatch(int op, F &&f) {
+  switch (op) {
+    case ACU_BITWISE_AND: f(std::integral_constant<int, ACU_BITWISE_AND>()); break;
+    case ACU_BITWISE_OR: f(std::integral_constant<int, ACU_BITWISE_OR>()); break;
+    case ACU_BITWISE_XOR: f(std::integral_constant<int, ACU_BITWISE_XOR>()); break;
+    case ACU_BITWISE_AND_NOT: f(std::integral_constant<int, ACU_BITWISE_AND_NOT>()); break;
+    case ACU_BITWISE_SHIFT_LEFT: f(std::integral_constant<int, ACU_BITWISE_SHIFT_LEFT>()); break;
+    case ACU_BITWISE_SHIFT_RIGHT: f(std::integral_constant<int, ACU_BITWISE_SHIFT_RIGHT>()); break;
+    default: f(std::integral_constant<int, ACU_BITWISE_NOT>()); break;
+  }
+}
+// The rows of 16 bytes of values: the logical ops act on whole 32-bit words, the shifts on each element in turn, so that
+// 128-bit packs of narrow values are never unpacked into one register per element (they would spill).
+template <int OP, class T> __device__ __forceinline__ uint32_t bitwise_word(uint32_t a, uint32_t b) {
+  if constexpr (OP == ACU_BITWISE_SHIFT_LEFT || OP == ACU_BITWISE_SHIFT_RIGHT) {
+    constexpr int BITS = 8 * sizeof(T);
+    constexpr uint32_t MASK = BITS == 32 ? ~0u : (1u << (BITS & 31)) - 1u;
+    uint32_t o = 0;
+#pragma unroll
+    for (int i = 0; i < 4 / (int)sizeof(T); ++i) {  // element i: bits [BITS*i, BITS*(i+1)) of the word
+      const unsigned amt = (b >> (BITS * i)) & (BITS - 1);
+      uint32_t r;
+      if constexpr (OP == ACU_BITWISE_SHIFT_LEFT) r = (a >> (BITS * i)) << amt;
+      else if constexpr (std::is_signed<T>::value) r = (uint32_t)((int32_t)(a << (32 - BITS * (i + 1))) >> (32 - BITS + amt));
+      else r = ((a >> (BITS * i)) & MASK) >> amt;
+      o |= (r & MASK) << (BITS * i);
+    }
+    return o;
+  } else {
+    return bitwise_row<OP, uint32_t>(a, b);
+  }
+}
+template <int OP, class T> __device__ __forceinline__ uint4 bitwise_vec(uint4 a, uint4 b) {
+  uint4 o;
+  if constexpr (sizeof(T) == 8 && (OP == ACU_BITWISE_SHIFT_LEFT || OP == ACU_BITWISE_SHIFT_RIGHT)) {
+    const T r0 = bitwise_row<OP, T>((T)(((uint64_t)a.y << 32) | a.x), (T)(((uint64_t)b.y << 32) | b.x));
+    const T r1 = bitwise_row<OP, T>((T)(((uint64_t)a.w << 32) | a.z), (T)(((uint64_t)b.w << 32) | b.z));
+    o.x = (uint32_t)(uint64_t)r0; o.y = (uint32_t)((uint64_t)r0 >> 32);
+    o.z = (uint32_t)(uint64_t)r1; o.w = (uint32_t)((uint64_t)r1 >> 32);
+  } else {
+    o.x = bitwise_word<OP, T>(a.x, b.x);
+    o.y = bitwise_word<OP, T>(a.y, b.y);
+    o.z = bitwise_word<OP, T>(a.z, b.z);
+    o.w = bitwise_word<OP, T>(a.w, b.w);
+  }
+  return o;
+}
+
+// One strip group of k_arith's CLS_BITWISE steady state: NL warp-wide loads per operand, all issued before any use, then
+// the op decided once for the group. `a` is always an array (acu_bitwise).
+template <class T, int EPL, int NL>
+__device__ __forceinline__ void bitwise_group(int op, const T *__restrict__ pa, const T *__restrict__ pb, T *__restrict__ po,
+                                              int b_scalar, T sb) {
+  if constexpr (EPL * sizeof(T) == 16) {
+    uint4 va[NL], vb[NL];
+#pragma unroll
+    for (int k = 0; k < NL; ++k) {
+      va[k] = ld_stream16(pa + k * 32 * EPL);
+      if (!b_scalar) vb[k] = ld_stream16(pb + k * 32 * EPL);
+    }
+    uint4 sv;  // the scalar in every element
+    if constexpr (sizeof(T) == 8) {
+      sv.x = sv.z = (uint32_t)(uint64_t)sb;
+      sv.y = sv.w = (uint32_t)((uint64_t)sb >> 32);
+    } else {
+      sv.x = sv.y = sv.z = sv.w = (uint32_t)(typename std::make_unsigned<T>::type)sb * (sizeof(T) == 1 ? 0x01010101u : sizeof(T) == 2 ? 0x00010001u : 1u);
+    }
+    bitwise_dispatch(op, [&](auto c) {
+#pragma unroll
+      for (int k = 0; k < NL; ++k) st_stream16(po + k * 32 * EPL, bitwise_vec<decltype(c)::value, T>(va[k], b_scalar ? sv : vb[k]));
+    });
+  } else {
+    static_assert(EPL == 1, "scalar path");
+    T va[NL], vb[NL];
+#pragma unroll
+    for (int k = 0; k < NL; ++k) {
+      va[k] = __ldg(pa + k * 32);
+      if (!b_scalar) vb[k] = __ldg(pb + k * 32);
+    }
+    bitwise_dispatch(op, [&](auto c) {
+#pragma unroll
+      for (int k = 0; k < NL; ++k) po[k * 32] = bitwise_row<decltype(c)::value, T>(va[k], b_scalar ? sb : vb[k]);
+    });
+  }
+}
+
+template <class T> __device__ __forceinline__ T bitwise_apply(int op, T l, T r) {
+  T o;
+  bitwise_dispatch(op, [&](auto c) { o = bitwise_row<decltype(c)::value, T>(l, r); });
+  return o;
 }
 
 // ---------------------------------------------------------------------------------------
@@ -275,6 +389,7 @@ struct ArithParams {
 template <class T, int CLS>
 __device__ __forceinline__ bool row_op(const ArithParams<T> &p, T l, T r, T &o) {
   if constexpr (CLS == CLS_DECIMAL) return dec_apply<T>(p.op, l, r, p.l_mul, p.r_mul, o);
+  else if constexpr (CLS == CLS_BITWISE) { o = bitwise_apply<T>(p.op, l, r); return false; }
   else return apply_op<T, CLS>(p.op, l, r, o);
 }
 
@@ -285,7 +400,7 @@ __device__ __forceinline__ bool row_op(const ArithParams<T> &p, T l, T r, T &o) 
 // Decimal128 rows are 16 B per operand: U = 4 strips keep 128 B per operand and lane in flight, two CTAs per SM give
 // the checked i128 steps their registers.
 template <class T, int CLS, int EPL>
-__global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : (CLS == CLS_DECIMAL && sizeof(T) == 16) ? 2 : 3))
+__global__ void __launch_bounds__(256, ((CLS == CLS_WRAP || CLS == CLS_BITWISE) ? 4 : (CLS == CLS_DECIMAL && sizeof(T) == 16) ? 2 : 3))
     k_arith(const ArithParams<T> p) {
   constexpr bool WIDE = CLS == CLS_DECIMAL && sizeof(T) == 16;
   constexpr int R = (32 * EPL > 64) ? 32 * EPL : 64;  // rows per strip
@@ -294,7 +409,7 @@ __global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : (CLS == CLS_DECIMA
   constexpr int GROUP = U * R;                        // rows per group
   constexpr int SG = 2048;                            // rows per super-group
   constexpr int GPS = SG / GROUP;                     // groups per super-group
-  constexpr bool fallible = (CLS != CLS_WRAP) && !is_fp<T>::value;
+  constexpr bool fallible = (CLS != CLS_WRAP && CLS != CLS_BITWISE) && !is_fp<T>::value;
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
@@ -322,6 +437,11 @@ __global__ void __launch_bounds__(256, (CLS == CLS_WRAP ? 4 : (CLS == CLS_DECIMA
       const int64_t base = sbase + gi * GROUP;
       const T *__restrict__ pa = p.a + base + lane * EPL;
       const T *__restrict__ pb = p.b + base + lane * EPL;
+      if constexpr (CLS == CLS_BITWISE) {  // `a` is always an array here (acu_bitwise)
+        T *__restrict__ po = p.out + base + lane * EPL;
+        bitwise_group<T, EPL, U * LPS>(p.op, pa, pb, po, p.b_scalar, sb);
+        continue;
+      }
       Pack<T, EPL> va[U * LPS], vb[U * LPS];
       // ---- every load of the group is issued before any use (memory-level parallelism) ----
 #pragma unroll
@@ -493,11 +613,19 @@ acu_status arith_error(acu_ctx *ctx, acu_arith_op op, bool is_neg, const acu_arr
   return acu_fail(ctx, ACU_ERR_ARITHMETIC_OVERFLOW, idx, lb, rb, 0, "Overflow happened on: %s %s %s", ls, sym, rs);
 }
 
+template <class T> acu_status launch_bitwise(acu_ctx *ctx, const ArithParams<T> &p) {
+  if constexpr (std::is_integral<T>::value) return launch_arith<T, CLS_BITWISE>(ctx, p);
+  else return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "bitwise operation on a non-integer type");
+}
+
 // DEC: decimal_op rows (every op checked, CLS_DECIMAL) with dec's multipliers, then its result-type validation.
+// bitwise_op >= 0: a bitwise.rs op (acu_bitwise_op, CLS_BITWISE) through the same binary / unary rules as the wrapping ops;
+// `op` is then unused.
 template <class T, bool DEC = false>
 acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const acu_array *b, acu_array_out *out,
-                       const DecArgs<T> *dec = nullptr) {
-  const bool checked = DEC || (!is_fp<T>::value && (op == ACU_ADD || op == ACU_SUB || op == ACU_MUL || op == ACU_DIV || op == ACU_REM));
+                       const DecArgs<T> *dec = nullptr, int bitwise_op = -1) {
+  const bool bitwise = bitwise_op >= 0;
+  const bool checked = DEC || (!bitwise && !is_fp<T>::value && (op == ACU_ADD || op == ACU_SUB || op == ACU_MUL || op == ACU_DIV || op == ACU_REM));
   DecArgs<T> dv{};
   if constexpr (DEC) dv = *dec;
   auto validate = [ctx, dv]() -> acu_status {
@@ -519,6 +647,7 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
     case ACU_DIV: p.op = OP_DIV; break;
     default: p.op = OP_REM; break;
   }
+  if (bitwise) p.op = bitwise_op;
   p.l_mul = DEC ? dv.l_mul : T();
   p.r_mul = DEC ? dv.r_mul : T();
   out->has_validity = 0;
@@ -573,6 +702,8 @@ acu_status arith_typed(acu_ctx *ctx, acu_arith_op op, const acu_array *a, const 
   p.res = acu_dres(ctx, blk);
   if constexpr (DEC) {
     ACU_TRY((launch_arith<T, CLS_DECIMAL>(ctx, p)));
+  } else if (bitwise) {
+    ACU_TRY(launch_bitwise<T>(ctx, p));
   } else if (is_fp<T>::value) {
     if (op == ACU_DIV || op == ACU_REM) ACU_TRY((launch_arith<T, CLS_DIVREM>(ctx, p)));
     else ACU_TRY((launch_arith<T, CLS_WRAP>(ctx, p)));
@@ -1694,6 +1825,38 @@ extern "C" acu_status acu_neg(acu_ctx *ctx, acu_dtype dtype, int32_t checked, co
   return acu_with_native(
       dtype, [&](auto t) { return neg_typed<decltype(t)>(ctx, checked, a, out); },
       [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid arithmetic operation: dtype %d", (int)dtype); });
+}
+
+// bitwise.rs: array-array ops through `binary`, the _scalar forms and not through `unary` (arith_typed's scalar arm with
+// the array's nulls cloned; not reads its operand as both sides, the scalar side ignored by the row).
+extern "C" acu_status acu_bitwise(acu_ctx *ctx, acu_dtype dtype, acu_bitwise_op op, const acu_array *a, const acu_array *b,
+                                  acu_array_out *out) {
+  ACU_ENTER(ctx);
+  if (dtype < ACU_I8 || dtype > ACU_U64)  // PrimitiveArray<T> with T::Native: BitAnd + ... : the integer types only
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid bitwise operation: dtype %d", (int)dtype);
+  if (op < ACU_BITWISE_AND || op > ACU_BITWISE_NOT)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid bitwise operation: op %d", (int)op);
+  if (a->is_scalar) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "bitwise: the left operand must be an array");
+  acu_array self_b;
+  if (op == ACU_BITWISE_NOT) {
+    self_b = *a;
+    self_b.validity = nullptr;
+    self_b.null_count = 0;
+    self_b.len = 1;
+    self_b.is_scalar = 1;
+    b = &self_b;
+  } else if (!b) {
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "bitwise: op %d needs a right operand", (int)op);
+  } else if (b->is_scalar) {
+    if (op == ACU_BITWISE_AND_NOT) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "bitwise: and_not has no scalar form");
+    acu_status st;
+    const int64_t snc = acu_resolve_null_count(ctx, b, &st);
+    ACU_TRY(st);
+    if (snc != 0) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "bitwise: the scalar operand is a T::Native and cannot be null");
+  }
+  return acu_with_native(
+      dtype, [&](auto t) { return arith_typed<decltype(t)>(ctx, ACU_ADD_WRAPPING, a, b, out, nullptr, (int)op); },
+      [&] { return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "Invalid bitwise operation: dtype %d", (int)dtype); });
 }
 
 extern "C" acu_status acu_cmp(acu_ctx *ctx, acu_dtype dtype, acu_cmp_op op, const acu_array *a,

@@ -42,7 +42,9 @@ acu_status acu_take_col_finalize(acu_ctx *ctx, const acu_array *values, const ac
                                  const unsigned long long *hres, acu_array_out *out);
 acu_status acu_take_check_bounds(acu_ctx *ctx, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls, int64_t values_len);
 int acu_take_index_kind(acu_dtype t);  // -1 for non-integer index types
-// sum / min / max: nc[c] = resolved null count; result bits in res[c][RES_AUX0].
+// sum / min / max / product / bit_and / bit_or / bit_xor: nc[c] = resolved null count; result bits in res[c][RES_AUX0].
+// acu_agg_op_check refuses an op outside acu_agg_op, and a bit op of a float dtype, before anything is queued.
+acu_status acu_agg_op_check(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op);
 size_t acu_reduce_col_scratch(const acu_ctx *ctx);
 acu_status acu_reduce_cols_launch(acu_ctx *ctx, int n, const acu_dtype *dtypes, const acu_agg_op *ops, const acu_array *arrays,
                                   const int64_t *nc, uint8_t *scratch, size_t scratch_per_col, unsigned long long *const *res, int *launched);

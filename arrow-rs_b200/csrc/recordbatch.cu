@@ -229,6 +229,7 @@ extern "C" acu_status acu_aggregate_columns(acu_ctx *ctx, int32_t n_columns, con
   if (n_columns == 0) return ACU_OK;
   acu_status st;
   std::vector<int64_t> nc(n_columns, 0);
+  for (int32_t c = 0; c < n_columns; ++c) ACU_TRY(acu_agg_op_check(ctx, dtypes[c], ops[c]));
   for (int32_t c = 0; c < n_columns; ++c) {
     out_bits[c] = 0;
     nc[c] = acu_resolve_null_count(ctx, &arrays[c], &st);

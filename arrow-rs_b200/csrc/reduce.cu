@@ -1,10 +1,11 @@
-// reduce.cu — arrow-arith/src/aggregate.rs sum / min / max on the device.
+// reduce.cu — arrow-arith/src/aggregate.rs sum / min / max / product / bit_and / bit_or / bit_xor on the device.
 //
-// Reference: aggregate() :317-366, accumulators :52-176, sum :943, min :1012, max :1027.
-// sum wraps for integers (add_wrapping) and is IEEE for floats; min/max use the totalOrder
-// (arrow-array/src/arithmetic.rs:400-437). Float `sum` is order-dependent in the reference
-// itself (lane count depends on compile-time target features, aggregate.rs:303-313), so
-// parity for it is tolerance-based; everything else is bit-exact.
+// Reference: aggregate() :317-366, accumulators :52-176, sum :943, product :953, min :1012, max :1027,
+// bit_and / bit_or / bit_xor :788-875. sum and product wrap for integers (add_wrapping / mul_wrapping)
+// and are IEEE for floats; min/max use the totalOrder (arrow-array/src/arithmetic.rs:400-437). Float
+// `sum` and `product` are order-dependent in the reference itself (lane count depends on compile-time
+// target features, aggregate.rs:303-313), so parity for them is tolerance-based; everything else is
+// bit-exact (wrapping multiplication and the bit ops are associative and commutative).
 //
 // Design: one streaming pass (HBM-bound, 8N + N/8 bytes). Lane l of a warp owns rows l and
 // l+32 of each 64-row strip (one validity word per strip), 4 strips in flight. Per-thread
@@ -33,13 +34,18 @@ template <class T> __device__ __forceinline__ T from_key(typename KeyOf<T>::type
   else return k;
 }
 
-// accumulator domain: sum -> T itself; min/max -> totalOrder key
-template <class T, int OP> struct AccOf { using type = typename std::conditional<OP == ACU_SUM, T, typename KeyOf<T>::type>::type; };
+// accumulator domain: min/max -> totalOrder key; every other op -> T itself
+template <class T, int OP> struct AccOf {
+  using type = typename std::conditional<OP == ACU_MIN || OP == ACU_MAX, typename KeyOf<T>::type, T>::type;
+};
 
 template <class A, int OP> __device__ __forceinline__ A acc_identity() {
   if constexpr (OP == ACU_SUM) return A(0);
   else if constexpr (OP == ACU_MIN) return std::numeric_limits<A>::max();   // MAX_TOTAL_ORDER
-  else return std::numeric_limits<A>::lowest();                            // MIN_TOTAL_ORDER
+  else if constexpr (OP == ACU_MAX) return std::numeric_limits<A>::lowest();  // MIN_TOTAL_ORDER
+  else if constexpr (OP == ACU_PRODUCT) return A(1);
+  else if constexpr (OP == ACU_BIT_AND) return (A)~(A)0;                   // -1: all ones
+  else return A(0);                                                        // bit_or / bit_xor
 }
 template <class A, int OP> __device__ __forceinline__ A acc_merge(A a, A b) {
   if constexpr (OP == ACU_SUM) {
@@ -49,13 +55,26 @@ template <class A, int OP> __device__ __forceinline__ A acc_merge(A a, A b) {
     else return (A)((typename std::make_unsigned<A>::type)a + (typename std::make_unsigned<A>::type)b);  // add_wrapping
   } else if constexpr (OP == ACU_MIN) {
     return b < a ? b : a;
-  } else {
+  } else if constexpr (OP == ACU_MAX) {
     return b > a ? b : a;
+  } else if constexpr (OP == ACU_PRODUCT) {
+    if constexpr (std::is_same<A, double>::value) return __dmul_rn(a, b);
+    else if constexpr (std::is_same<A, float>::value) return __fmul_rn(a, b);
+    else {  // mul_wrapping in the unsigned type, at least 32 bits wide (a u16 x u16 would be promoted to int and overflow it)
+      using U = typename std::conditional<(sizeof(A) < 4), uint32_t, typename std::make_unsigned<A>::type>::type;
+      return (A)((U)a * (U)b);
+    }
+  } else if constexpr (OP == ACU_BIT_AND) {
+    return a & b;
+  } else if constexpr (OP == ACU_BIT_OR) {
+    return a | b;
+  } else {
+    return a ^ b;
   }
 }
 template <class T, int OP> __device__ __forceinline__ typename AccOf<T, OP>::type acc_lift(T v) {
-  if constexpr (OP == ACU_SUM) return v;
-  else return to_key<T>(v);
+  if constexpr (OP == ACU_MIN || OP == ACU_MAX) return to_key<T>(v);
+  else return v;
 }
 
 template <class A> __device__ __forceinline__ A shfl_down_any(A v, int o) {
@@ -165,8 +184,8 @@ __global__ void __launch_bounds__(256) k_reduce(const ReduceBatch batch) {
     for (int o = 16; o > 0; o >>= 1) f = acc_merge<A, OP>(f, shfl_down_any(f, o));
     if (lane == 0) {
       T r;
-      if constexpr (OP == ACU_SUM) r = f;
-      else r = from_key<T>(f);
+      if constexpr (OP == ACU_MIN || OP == ACU_MAX) r = from_key<T>(f);
+      else r = f;
       unsigned long long bits[2] = {0, 0};  // an i128 result fills RES_AUX0 (low) and RES_AUX1 (high)
       memcpy(bits, &r, sizeof(T));
       res[RES_AUX0] = bits[0];
@@ -186,13 +205,25 @@ acu_status reduce_launch(acu_ctx *ctx, const ReduceBatch &rb, int n_cols, int64_
   return ACU_OK;
 }
 
+// The (dtype, op) pair has passed acu_agg_op_check; the bit ops are instantiated for integer types only.
 template <class T>
 acu_status reduce_typed(acu_ctx *ctx, acu_agg_op op, const ReduceBatch &rb, int n_cols, int64_t max_len) {
+  constexpr bool INTEGRAL = std::is_integral<T>::value && sizeof(T) <= 8;
   switch (op) {
     case ACU_SUM: return reduce_launch<T, ACU_SUM>(ctx, rb, n_cols, max_len);
     case ACU_MIN: return reduce_launch<T, ACU_MIN>(ctx, rb, n_cols, max_len);
-    default: return reduce_launch<T, ACU_MAX>(ctx, rb, n_cols, max_len);
+    case ACU_MAX: return reduce_launch<T, ACU_MAX>(ctx, rb, n_cols, max_len);
+    default: break;
   }
+  if constexpr (sizeof(T) <= 8) {
+    if (op == ACU_PRODUCT) return reduce_launch<T, ACU_PRODUCT>(ctx, rb, n_cols, max_len);
+  }
+  if constexpr (INTEGRAL) {
+    if (op == ACU_BIT_AND) return reduce_launch<T, ACU_BIT_AND>(ctx, rb, n_cols, max_len);
+    if (op == ACU_BIT_OR) return reduce_launch<T, ACU_BIT_OR>(ctx, rb, n_cols, max_len);
+    if (op == ACU_BIT_XOR) return reduce_launch<T, ACU_BIT_XOR>(ctx, rb, n_cols, max_len);
+  }
+  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "aggregate: op %d", (int)op);
 }
 
 acu_status reduce_dispatch(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const ReduceBatch &rb, int n_cols, int64_t max_len) {
@@ -213,6 +244,16 @@ ReduceArgs reduce_args(const acu_array *a, int64_t nc, void *scratch, unsigned l
 }
 
 }  // namespace
+
+// sum / min / max / product take every native dtype, bit_and / bit_or / bit_xor the integer ones (aggregate.rs:788-875)
+acu_status acu_agg_op_check(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op) {
+  if (op == ACU_SUM || op == ACU_MIN || op == ACU_MAX || op == ACU_PRODUCT) return ACU_OK;
+  if (op != ACU_BIT_AND && op != ACU_BIT_OR && op != ACU_BIT_XOR)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "aggregate: op %d", (int)op);
+  if (acu_dtype_is_float(dtype))
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "aggregate: bit_and / bit_or / bit_xor of %s", acu_dtype_name(dtype));
+  return ACU_OK;
+}
 
 // per-column scratch of one queued reduction: one partial per CTA of the widest grid
 size_t acu_reduce_col_scratch(const acu_ctx *ctx) { return (size_t)ctx->sm_count * 8 * 8 * 16 + 4096; }
@@ -289,6 +330,8 @@ extern "C" acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op
                                     uint64_t *out_bits, int64_t *out_valid_count) {
   ACU_ENTER(ctx);
   *out_bits = 0;
+  *out_valid_count = 0;
+  ACU_TRY(acu_agg_op_check(ctx, dtype, op));
   return aggregate_one(ctx, dtype, op, a, false, out_bits, out_valid_count);
 }
 

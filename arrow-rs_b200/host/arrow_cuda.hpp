@@ -1340,6 +1340,51 @@ inline Result<BooleanArray> not_(const BooleanArray &a) { return detail4::boolea
 inline Result<BooleanArray> is_null(const Array &a) { return detail4::boolean_op(ACU_BOOL_IS_NULL, a, nullptr); }
 inline Result<BooleanArray> is_not_null(const Array &a) { return detail4::boolean_op(ACU_BOOL_IS_NOT_NULL, a, nullptr); }
 }  // namespace boolean
+
+// ---- kernels::bitwise (arrow-arith/src/bitwise.rs) -------------------------------------------
+// Integer PrimitiveArrays only (the reference's trait bounds exclude floats): the op at every slot, NullBuffer::union of
+// the operands (array forms) or the left operand's nulls (scalar forms, not). Shifts wrap the amount modulo the width.
+namespace bitwise {
+namespace detail5 {
+template <class T>
+Result<PrimitiveArray<T>> bitwise_op(acu_bitwise_op op, const PrimitiveArray<T> &l, const PrimitiveArray<T> *r, const T *scalar) {
+  static_assert(std::is_integral<T>::value, "bitwise operations take integer arrays");
+  Context &c = Context::get();
+  const int64_t n = l.len();
+  Buffer vb, nb;
+  acu_array a = l.view(), b{};
+  std::optional<PrimitiveArray<T>> s;
+  if (r) b = r->view();
+  if (scalar) {
+    s = PrimitiveArray<T>::from(std::vector<T>{*scalar});
+    b = s->view(true);
+  }
+  acu_array_out o = compute::detail::make_out(vb, nb, (size_t)std::max<int64_t>(n, 1) * sizeof(T), n);
+  acu_status st = acu_bitwise(c.raw(), NativeOf<T>::code, op, &a, (r || scalar) ? &b : nullptr, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return PrimitiveArray<T>(vb, o.len, compute::detail::out_nulls(o, nb));
+}
+}  // namespace detail5
+#define ACU_BITWISE(NAME, OP)                                                                                          \
+  template <class T> Result<PrimitiveArray<T>> NAME(const PrimitiveArray<T> &l, const PrimitiveArray<T> &r) {        \
+    return detail5::bitwise_op<T>(OP, l, &r, nullptr);                                                               \
+  }
+#define ACU_BITWISE_SCALAR(NAME, OP)                                                                                   \
+  template <class T> Result<PrimitiveArray<T>> NAME(const PrimitiveArray<T> &l, T scalar) {                          \
+    return detail5::bitwise_op<T>(OP, l, nullptr, &scalar);                                                          \
+  }
+ACU_BITWISE(bitwise_and, ACU_BITWISE_AND) ACU_BITWISE(bitwise_or, ACU_BITWISE_OR) ACU_BITWISE(bitwise_xor, ACU_BITWISE_XOR)
+ACU_BITWISE(bitwise_and_not, ACU_BITWISE_AND_NOT) ACU_BITWISE(bitwise_shift_left, ACU_BITWISE_SHIFT_LEFT)
+ACU_BITWISE(bitwise_shift_right, ACU_BITWISE_SHIFT_RIGHT)
+ACU_BITWISE_SCALAR(bitwise_and_scalar, ACU_BITWISE_AND) ACU_BITWISE_SCALAR(bitwise_or_scalar, ACU_BITWISE_OR)
+ACU_BITWISE_SCALAR(bitwise_xor_scalar, ACU_BITWISE_XOR) ACU_BITWISE_SCALAR(bitwise_shift_left_scalar, ACU_BITWISE_SHIFT_LEFT)
+ACU_BITWISE_SCALAR(bitwise_shift_right_scalar, ACU_BITWISE_SHIFT_RIGHT)
+#undef ACU_BITWISE
+#undef ACU_BITWISE_SCALAR
+template <class T> Result<PrimitiveArray<T>> bitwise_not(const PrimitiveArray<T> &a) {
+  return detail5::bitwise_op<T>(ACU_BITWISE_NOT, a, nullptr, nullptr);
+}
+}  // namespace bitwise
 }  // namespace kernels
 
 // ---- cast (arrow-cast/src/cast/mod.rs) -------------------------------------------------------
@@ -1441,18 +1486,30 @@ template <class T> std::optional<T> max(const DecimalArray<T> &a) { return detai
 template <class T> std::optional<T> sum(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_SUM, a); }
 template <class T> std::optional<T> min(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_MIN, a); }
 template <class T> std::optional<T> max(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_MAX, a); }
-// sum_checked (aggregate.rs:897-937): Ok(None) when every row is null, Err(ArithmeticOverflow) at the first overflowing add
-template <class T> Result<std::optional<T>> sum_checked(const PrimitiveArray<T> &a) {
+// product (aggregate.rs:953): mul_wrapping for integers; bit_and / bit_or / bit_xor (aggregate.rs:788-875): integers only
+template <class T> std::optional<T> product(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_PRODUCT, a); }
+template <class T> std::optional<T> bit_and(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_BIT_AND, a); }
+template <class T> std::optional<T> bit_or(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_BIT_OR, a); }
+template <class T> std::optional<T> bit_xor(const PrimitiveArray<T> &a) { return detail::aggregate(ACU_BIT_XOR, a); }
+namespace detail {
+template <class T>
+Result<std::optional<T>> checked_fold(acu_status (*fn)(acu_ctx *, acu_dtype, const acu_array *, uint64_t *, int64_t *),
+                                      const PrimitiveArray<T> &a) {
   uint64_t bits = 0;
   int64_t valid = 0;
   acu_array v = a.view();
-  acu_status st = acu_sum_checked(Context::get().raw(), NativeOf<T>::code, &v, &bits, &valid);
+  acu_status st = fn(Context::get().raw(), NativeOf<T>::code, &v, &bits, &valid);
   if (st != ACU_OK) return Context::get().last_error(st);
   if (valid == 0) return std::optional<T>(std::nullopt);
   T out;
   std::memcpy(&out, &bits, sizeof(T));
   return std::optional<T>(out);
 }
+}  // namespace detail
+// sum_checked (aggregate.rs:897-937): Ok(None) when every row is null, Err(ArithmeticOverflow) at the first overflowing add
+template <class T> Result<std::optional<T>> sum_checked(const PrimitiveArray<T> &a) { return detail::checked_fold(acu_sum_checked, a); }
+// product_checked (aggregate.rs:963-1001): Err(ArithmeticOverflow) at the first valid row whose running product overflows
+template <class T> Result<std::optional<T>> product_checked(const PrimitiveArray<T> &a) { return detail::checked_fold(acu_product_checked, a); }
 
 // min_string / max_string, min_string_view / max_string_view (aggregate.rs:520-568): the device returns the lowest row
 // holding the extremal value; its bytes are copied out (an owned value where the reference borrows from the array).

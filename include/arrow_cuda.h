@@ -110,8 +110,17 @@ typedef enum acu_cmp_op {
   ACU_DISTINCT = 6, ACU_NOT_DISTINCT = 7
 } acu_cmp_op;
 
-/* arrow-arith/src/aggregate.rs:943,1012,1027. */
-typedef enum acu_agg_op { ACU_SUM = 0, ACU_MIN = 1, ACU_MAX = 2 } acu_agg_op;
+/* arrow-arith/src/aggregate.rs:943,1012,1027 (sum / min / max), :953 (product), :850-875 (bit_and / bit_or / bit_xor). */
+typedef enum acu_agg_op {
+  ACU_SUM = 0, ACU_MIN = 1, ACU_MAX = 2,
+  ACU_PRODUCT = 3, ACU_BIT_AND = 4, ACU_BIT_OR = 5, ACU_BIT_XOR = 6
+} acu_agg_op;
+
+/* arrow-arith/src/bitwise.rs: bitwise_and / or / xor / and_not / shift_left / shift_right / not. */
+typedef enum acu_bitwise_op {
+  ACU_BITWISE_AND = 0, ACU_BITWISE_OR = 1, ACU_BITWISE_XOR = 2, ACU_BITWISE_AND_NOT = 3,
+  ACU_BITWISE_SHIFT_LEFT = 4, ACU_BITWISE_SHIFT_RIGHT = 5, ACU_BITWISE_NOT = 6
+} acu_bitwise_op;
 
 /* A borrowed, immutable view of a primitive / boolean array in HBM
  * (PrimitiveArray{values,nulls} arrow-array/src/array/primitive_array.rs:596-601;
@@ -185,8 +194,8 @@ int64_t acu_bytes_allocated(const acu_ctx *ctx);
  * aggregate bits), fills acu_filter_plan count / strategy, and returns the FIRST error in call order with its exact
  * reference text (the outputs of the calls after a failed one are unspecified, as after any failed call).
  *   - stream-ordered inside a section: acu_filter_plan_create, acu_filter_plan_create_cmp, acu_filter_primitive,
- *     acu_filter_boolean, acu_take_primitive / acu_take_boolean (check_bounds = 0), acu_arith, acu_decimal_arith, acu_cmp
- *     (ACU_I128 included), acu_neg (ACU_I128 only), acu_aggregate, acu_aggregate_i128, acu_aggregate_allreduce. Any other
+ *     acu_filter_boolean, acu_take_primitive / acu_take_boolean (check_bounds = 0), acu_arith, acu_bitwise,
+ *     acu_decimal_arith, acu_cmp (ACU_I128 included), acu_neg (ACU_I128 only), acu_aggregate, acu_aggregate_i128, acu_aggregate_allreduce. Any other
  *     entry point fails with ACU_ERR_INVALID_ARGUMENT (it would synchronise).
  *   - every output descriptor, scalar output pointer and plan passed to a queued call must stay alive until the fetch;
  *     input arrays must carry their cached null_count (-1 would need a device count = a synchronisation), except for
@@ -346,6 +355,23 @@ acu_status acu_arith(acu_ctx *ctx, acu_dtype dtype, acu_arith_op op, const acu_a
  * same reason a Decimal32 / Decimal64 negation is acu_neg(ACU_I32 / ACU_I64, checked = 1). */
 acu_status acu_neg(acu_ctx *ctx, acu_dtype dtype, int32_t checked, const acu_array *a,
                    acu_array_out *out);
+
+/* ------------------------------------------------------------------------- */
+/* bitwise — arrow-arith/src/bitwise.rs                                      */
+/* ------------------------------------------------------------------------- */
+/* bitwise_and / or / xor / and_not / shift_left / shift_right (array-array, through `binary`, arity.rs:104-135), their
+ * _scalar forms (b->is_scalar; and_not has none) and bitwise_not (b == NULL), through `unary`, for the integer dtypes
+ * ACU_I8 .. ACU_U64:
+ *   - the op is evaluated at every slot, so the values under nulls are op(a[i], b[i]); the result's NullBuffer is the
+ *     union of the inputs' (array-array) or a's (scalar forms, not); an empty array-array result has no NullBuffer;
+ *   - shifts are wrapping_shl / wrapping_shr by b's two's-complement bit pattern modulo the bit width (a u64 shifted by
+ *     u64::MAX shifts by 63); shift_right is arithmetic for signed and logical for unsigned types;
+ *   - length mismatch => ACU_ERR_COMPUTE "Cannot perform binary operation on arrays of different length";
+ *   - a scalar `a`, a null scalar `b`, a scalar and_not, b == NULL for any op but NOT, a float or ACU_I128 dtype, or an op
+ *     outside acu_bitwise_op => ACU_ERR_INVALID_ARGUMENT.
+ * In place as acu_arith; stream-ordered inside a section like acu_arith; kernel time counts in ACU_K_ARITH. */
+acu_status acu_bitwise(acu_ctx *ctx, acu_dtype dtype, acu_bitwise_op op, const acu_array *a, const acu_array *b,
+                       acu_array_out *out);
 
 /* ------------------------------------------------------------------------- */
 /* decimal arithmetic — decimal_op (arrow-arith/src/numeric.rs:970-1107)     */
@@ -649,7 +675,10 @@ acu_status acu_boolean(acu_ctx *ctx, acu_bool_op op, const acu_array *a, const a
 /* ------------------------------------------------------------------------- */
 /* sum/min/max (aggregate.rs:943,1012,1027): *out_bits = the native result's bit
  * pattern (zero-extended), *out_valid_count = number of non-null rows; the reference
- * returns None iff out_valid_count == 0 (aggregate.rs:320-323). */
+ * returns None iff out_valid_count == 0 (aggregate.rs:320-323).
+ * product (aggregate.rs:953) wraps for integers (mul_wrapping) and is IEEE for floats (association order unspecified, as
+ * for sum); bit_and / bit_or / bit_xor (aggregate.rs:788-875) take the integer dtypes only (a float =>
+ * ACU_ERR_INVALID_ARGUMENT). An op outside acu_agg_op => ACU_ERR_INVALID_ARGUMENT. */
 acu_status acu_aggregate(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a,
                          uint64_t *out_bits, int64_t *out_valid_count);
 /* sum / min / max of a Decimal128 (ACU_I128) column: out_bits[0] = low, out_bits[1] = high 64 bits of the i128 result;
@@ -664,6 +693,14 @@ acu_status acu_aggregate_i128(acu_ctx *ctx, acu_agg_op op, const acu_array *a, u
  * total would fit. Floats never fail (add_checked is the plain add): same as ACU_SUM. */
 acu_status acu_sum_checked(acu_ctx *ctx, acu_dtype dtype, const acu_array *a, uint64_t *out_bits,
                            int64_t *out_valid_count);
+/* product_checked (aggregate.rs:963-1001): the in-order fold acc.mul_checked(v) from 1. Integers:
+ * ACU_ERR_ARITHMETIC_OVERFLOW "Overflow happened on: {acc} * {value}" at the first valid row whose running product
+ * leaves the native range (index = that row, lhs_bits / rhs_bits = acc / value) — also when a later zero would bring the
+ * product back to 0. Floats never fail (mul_checked is the plain multiply): same as ACU_PRODUCT. Contract otherwise as
+ * acu_sum_checked. Synchronous: inside a stream-ordered section every call, float and empty inputs included, fails with
+ * ACU_ERR_INVALID_ARGUMENT before any device work. Kernel time in ACU_K_REDUCE. */
+acu_status acu_product_checked(acu_ctx *ctx, acu_dtype dtype, const acu_array *a, uint64_t *out_bits,
+                               int64_t *out_valid_count);
 
 /* min / max of Utf8 / Binary (offset_bytes 4), LargeUtf8 / LargeBinary (8), Utf8View / BinaryView and FixedSizeBinary
  * columns: min_max_helper / min_max_view_helper (aggregate.rs:460-518) behind min_string, max_binary_view,
@@ -876,7 +913,9 @@ acu_status acu_comm_allreduce_aggregates(acu_ctx *ctx, acu_dtype dtype, acu_agg_
 /* acu_aggregate over this rank's shard combined over all ranks in ONE call with ONE synchronisation: the partial stays in
  * HBM, a one-thread kernel re-encodes it (identity for a shard without valid rows, totalOrder key for float / signed
  * min / max), NCCL reduces {value, valid_count} in place on the ctx stream, and only the final pair crosses to the host
- * (no host bounce between the reduction kernel and the collective). Without a communicator it is acu_aggregate. */
+ * (no host bounce between the reduction kernel and the collective). Without a communicator it is acu_aggregate.
+ * Both all-reduce entry points take ACU_SUM / ACU_MIN / ACU_MAX only: any other op => ACU_ERR_NOT_YET_IMPLEMENTED before
+ * any collective runs, with or without a communicator (NCCL has no product or bitwise reduction). */
 acu_status acu_aggregate_allreduce(acu_ctx *ctx, acu_dtype dtype, acu_agg_op op, const acu_array *a,
                                    uint64_t *out_bits, int64_t *out_valid_count);
 /* Sum int64 scalars across ranks (row counts, null counts). */

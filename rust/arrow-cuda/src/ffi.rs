@@ -65,6 +65,18 @@ pub const ACU_BIT_LENGTH: i32 = 1;
 pub const ACU_SUM: i32 = 0;
 pub const ACU_MIN: i32 = 1;
 pub const ACU_MAX: i32 = 2;
+pub const ACU_PRODUCT: i32 = 3;
+pub const ACU_BIT_AND: i32 = 4;
+pub const ACU_BIT_OR: i32 = 5;
+pub const ACU_BIT_XOR: i32 = 6;
+// acu_bitwise_op (arrow-arith/src/bitwise.rs)
+pub const ACU_BITWISE_AND: i32 = 0;
+pub const ACU_BITWISE_OR: i32 = 1;
+pub const ACU_BITWISE_XOR: i32 = 2;
+pub const ACU_BITWISE_AND_NOT: i32 = 3;
+pub const ACU_BITWISE_SHIFT_LEFT: i32 = 4;
+pub const ACU_BITWISE_SHIFT_RIGHT: i32 = 5;
+pub const ACU_BITWISE_NOT: i32 = 6;
 pub const ACU_BOOL_AND: i32 = 0;
 pub const ACU_BOOL_OR: i32 = 1;
 pub const ACU_BOOL_AND_NOT: i32 = 2;
@@ -225,6 +237,8 @@ extern "C" {
     pub fn acu_aggregate_columns(ctx: *mut acu_ctx, n_columns: i32, dtypes: *const i32, ops: *const i32, arrays: *const acu_array,
                                  out_bits: *mut u64, out_valid_counts: *mut i64) -> acu_status;
     pub fn acu_sum_checked(ctx: *mut acu_ctx, dtype: i32, a: *const acu_array, out_bits: *mut u64, out_valid: *mut i64) -> acu_status;
+    pub fn acu_product_checked(ctx: *mut acu_ctx, dtype: i32, a: *const acu_array, out_bits: *mut u64, out_valid: *mut i64) -> acu_status;
+    pub fn acu_bitwise(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_aggregate_bytes(ctx: *mut acu_ctx, offset_bytes: i32, op: i32, a: *const acu_bytes_array, out_row: *mut i64,
                                out_valid: *mut i64) -> acu_status;
     pub fn acu_aggregate_byte_view(ctx: *mut acu_ctx, op: i32, a: *const acu_view_array, out_row: *mut i64, out_valid: *mut i64) -> acu_status;

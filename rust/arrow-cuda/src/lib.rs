@@ -13,7 +13,9 @@
 //!   compute::kernels::cmp::{eq .. not_distinct}                              arrow-ord/src/cmp.rs:79-202
 //!   compute::kernels::boolean::{and .. is_not_null}                          arrow-arith/src/boolean.rs:60-354
 //!   compute::{cast, cast_with_options, CastOptions}                          arrow-cast/src/cast/mod.rs:347,790
+//!   compute::kernels::bitwise::{bitwise_and .. bitwise_not}                  arrow-arith/src/bitwise.rs:25-207
 //!   compute::{sum, min, max, sum_checked}                                    arrow-arith/src/aggregate.rs:897-1027
+//!   compute::{product, product_checked, bit_and, bit_or, bit_xor}            arrow-arith/src/aggregate.rs:788-1001
 //!   compute::aggregate::{min_string .. max_fixed_size_binary, min_boolean,   arrow-arith/src/aggregate.rs:372-568, 880-889
 //!                        max_boolean, bool_and, bool_or}
 //!   compute::{nullif, zip, concat, concat_batches}                           arrow-select/src/{nullif,zip,concat}.rs
@@ -460,14 +462,27 @@ pub mod compute {
     pub fn sum<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_SUM, array) }
     pub fn min<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_MIN, array) }
     pub fn max<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_MAX, array) }
-    /// aggregate.rs:897-937
-    pub fn sum_checked<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Result<Option<T::Native>, ArrowError> {
+    /// aggregate.rs:953 (mul_wrapping for integers) and :850-875 (integer arrays only) — `None` iff no valid row.
+    pub fn product<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_PRODUCT, array) }
+    pub fn bit_and<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_BIT_AND, array) }
+    pub fn bit_or<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_BIT_OR, array) }
+    pub fn bit_xor<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Option<T::Native> { aggregate(ffi::ACU_BIT_XOR, array) }
+    type CheckedFold = unsafe extern "C" fn(*mut ffi::acu_ctx, i32, *const ffi::acu_array, *mut u64, *mut i64) -> ffi::acu_status;
+    fn checked_fold<T: ArrowPrimitiveType>(f: CheckedFold, array: &PrimitiveArray<T>) -> Result<Option<T::Native>, ArrowError> {
         let dtype = numeric_dtype("arithmetic", &T::DATA_TYPE)?;
         let ctx = Context::current()?;
         let a = DeviceArray::upload(&ctx, array, false)?;
         let (mut bits, mut valid) = (0u64, 0i64);
-        ctx.check(unsafe { ffi::acu_sum_checked(ctx.raw(), dtype, a.view(), &mut bits, &mut valid) })?;
+        ctx.check(unsafe { f(ctx.raw(), dtype, a.view(), &mut bits, &mut valid) })?;
         Ok((valid != 0).then(|| unsafe { std::ptr::read_unaligned(&bits as *const u64 as *const T::Native) }))
+    }
+    /// aggregate.rs:897-937
+    pub fn sum_checked<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Result<Option<T::Native>, ArrowError> {
+        checked_fold(ffi::acu_sum_checked, array)
+    }
+    /// aggregate.rs:963-1001: Err(ArithmeticOverflow) at the first valid row whose running product overflows
+    pub fn product_checked<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Result<Option<T::Native>, ArrowError> {
+        checked_fold(ffi::acu_product_checked, array)
     }
 
     /// min / max of byte, view, fixed-size-binary and boolean arrays (aggregate.rs:372-568, :880-889). The device returns the
@@ -1020,6 +1035,40 @@ pub mod compute {
             pub fn not(left: &BooleanArray) -> Result<BooleanArray, ArrowError> { boolean_op(ffi::ACU_BOOL_NOT, left, None) }
             pub fn is_null(input: &dyn Array) -> Result<BooleanArray, ArrowError> { boolean_op(ffi::ACU_BOOL_IS_NULL, input, None) }
             pub fn is_not_null(input: &dyn Array) -> Result<BooleanArray, ArrowError> { boolean_op(ffi::ACU_BOOL_IS_NOT_NULL, input, None) }
+        }
+
+        /// `arrow::compute::kernels::bitwise` (arrow-arith/src/bitwise.rs): integer arrays only; the op at every slot,
+        /// NullBuffer::union of the operands (array forms) or the left operand's nulls (scalar forms, not)
+        pub mod bitwise {
+            use super::*;
+            fn bitwise_op<T: ArrowPrimitiveType>(op: i32, left: &PrimitiveArray<T>, right: Option<&PrimitiveArray<T>>,
+                                                 scalar: Option<T::Native>) -> Result<PrimitiveArray<T>, ArrowError> {
+                let dtype = native_code(&T::DATA_TYPE)
+                    .ok_or_else(|| ArrowError::InvalidArgumentError(format!("Invalid bitwise operation: {}", T::DATA_TYPE)))?;
+                let ctx = Context::current()?;
+                let a = DeviceArray::upload(&ctx, left, false)?;
+                let s = scalar.map(|v| PrimitiveArray::<T>::from_value(v, 1));
+                let b = match (right, s.as_ref()) {
+                    (Some(r), _) => Some(DeviceArray::upload(&ctx, r, false)?),
+                    (None, Some(s)) => Some(DeviceArray::upload(&ctx, s, true)?),
+                    (None, None) => None,
+                };
+                let mut out = ColumnOut::new(&ctx, &T::DATA_TYPE, left.len(), 0)?;
+                ctx.check(unsafe { ffi::acu_bitwise(ctx.raw(), dtype, op, a.view(), b.as_ref().map_or(std::ptr::null(), |d| d.view() as *const _), out.array_out()) })?;
+                Ok(out.finish(&T::DATA_TYPE)?.as_any().downcast_ref::<PrimitiveArray<T>>().unwrap().clone())
+            }
+            pub fn bitwise_and<T: ArrowPrimitiveType>(left: &PrimitiveArray<T>, right: &PrimitiveArray<T>) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_AND, left, Some(right), None) }
+            pub fn bitwise_or<T: ArrowPrimitiveType>(left: &PrimitiveArray<T>, right: &PrimitiveArray<T>) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_OR, left, Some(right), None) }
+            pub fn bitwise_xor<T: ArrowPrimitiveType>(left: &PrimitiveArray<T>, right: &PrimitiveArray<T>) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_XOR, left, Some(right), None) }
+            pub fn bitwise_and_not<T: ArrowPrimitiveType>(left: &PrimitiveArray<T>, right: &PrimitiveArray<T>) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_AND_NOT, left, Some(right), None) }
+            pub fn bitwise_shift_left<T: ArrowPrimitiveType>(left: &PrimitiveArray<T>, right: &PrimitiveArray<T>) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_SHIFT_LEFT, left, Some(right), None) }
+            pub fn bitwise_shift_right<T: ArrowPrimitiveType>(left: &PrimitiveArray<T>, right: &PrimitiveArray<T>) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_SHIFT_RIGHT, left, Some(right), None) }
+            pub fn bitwise_and_scalar<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>, scalar: T::Native) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_AND, array, None, Some(scalar)) }
+            pub fn bitwise_or_scalar<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>, scalar: T::Native) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_OR, array, None, Some(scalar)) }
+            pub fn bitwise_xor_scalar<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>, scalar: T::Native) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_XOR, array, None, Some(scalar)) }
+            pub fn bitwise_shift_left_scalar<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>, scalar: T::Native) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_SHIFT_LEFT, array, None, Some(scalar)) }
+            pub fn bitwise_shift_right_scalar<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>, scalar: T::Native) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_SHIFT_RIGHT, array, None, Some(scalar)) }
+            pub fn bitwise_not<T: ArrowPrimitiveType>(array: &PrimitiveArray<T>) -> Result<PrimitiveArray<T>, ArrowError> { bitwise_op(ffi::ACU_BITWISE_NOT, array, None, None) }
         }
     }
 }

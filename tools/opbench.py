@@ -127,6 +127,11 @@ def main():
         I, J = b.arr(di, va, n, n - nva), b.arr(dj, vb, n, n - nvb)
         b.timed("add i64 checked", [abi.K_ARITH], 24 * n + 3 * n / 8, n, lambda: ctx.check(lib.acu_arith(h, abi.I64, abi.ADD, C.byref(I), C.byref(J), C.byref(o))))
         b.timed("add_wrapping i64", [abi.K_ARITH], 24 * n + 3 * n / 8, n, lambda: ctx.check(lib.acu_arith(h, abi.I64, abi.ADD_WRAPPING, C.byref(I), C.byref(J), C.byref(o))))
+        # bitwise (arrow-arith/src/bitwise.rs) on the same inputs: the k_arith skeleton and bytes of add_wrapping above
+        b.timed("bitwise_and i64", [abi.K_ARITH], 24 * n + 3 * n / 8, n, lambda: ctx.check(lib.acu_bitwise(h, abi.I64, abi.BITWISE_AND, C.byref(I), C.byref(J), C.byref(o))))
+        I32, s32 = b.arr(di, va, n, n - nva), b.arr(dj, None, 1, 0, scalar=1)
+        b.timed("shift_left i32 array<<scalar", [abi.K_ARITH], 8 * n + 2 * n / 8, n,
+                lambda: ctx.check(lib.acu_bitwise(h, abi.I32, abi.BITWISE_SHIFT_LEFT, C.byref(I32), C.byref(s32), C.byref(o))))
         # predicate construction (arrow-arith/src/boolean.rs): bitmaps only, 1e9 rows
         bl, nbl = b.bits(50, 0.5, n)
         br, nbr = b.bits(51, 0.5, n)
@@ -138,8 +143,28 @@ def main():
         ctx.free(br)
         # aggregates over a full column
         bits_, cnt_ = C.c_uint64(0), C.c_int64(0)
-        for name, dt, arr_, op in [("sum i64", abi.I64, I, abi.SUM), ("min f64", abi.F64, A, abi.MIN), ("sum f64", abi.F64, A, abi.SUM)]:
+        for name, dt, arr_, op in [("sum i64", abi.I64, I, abi.SUM), ("min f64", abi.F64, A, abi.MIN), ("sum f64", abi.F64, A, abi.SUM),
+                                   ("bit_xor i64", abi.I64, I, abi.BIT_XOR), ("product i64", abi.I64, I, abi.PRODUCT),
+                                   ("product f64", abi.F64, A, abi.PRODUCT)]:
             b.timed(name, [abi.K_REDUCE], 8 * n + n / 8, n, lambda dt=dt, arr_=arr_, op=op: ctx.check(lib.acu_aggregate(h, dt, op, C.byref(arr_), C.byref(bits_), C.byref(cnt_))))
+        # the checked folds on the same validity with values whose running sum / product fit (all -1; a zero would end
+        # product_checked's reads of its chunk): no error, so the timed work is the chunk-summary pass and the one-CTA scan
+        dones = ctx.malloc(n * 8 + 64)
+        ctx.check(lib.acu_memset(h, dones, 0xFF, n * 8))
+        ones = b.arr(dones, va, n, n - nva)
+        for name, fn in [("sum_checked i64", lib.acu_sum_checked), ("product_checked i64", lib.acu_product_checked)]:
+            b.timed(name, [abi.K_REDUCE], 8 * n + n / 8, n, lambda fn=fn: ctx.check(fn(h, abi.I64, C.byref(ones), C.byref(bits_), C.byref(cnt_))),
+                    note="all values -1")
+        ctx.free(dones)
+        # the same folds on the random Int64 column: both fail within the first rows, so the time is all three passes (the
+        # chunk summaries still read every row, the error walk reads one chunk)
+        def overflowing(fn):
+            st = fn(h, abi.I64, C.byref(I), C.byref(bits_), C.byref(cnt_))
+            if st != abi.ERR_ARITHMETIC_OVERFLOW:
+                raise RuntimeError(f"expected an overflow, got status {st}")
+
+        for name, fn in [("sum_checked i64 overflowing", lib.acu_sum_checked), ("product_checked i64 overflowing", lib.acu_product_checked)]:
+            b.timed(name, [abi.K_REDUCE], 8 * n + n / 8, n, lambda fn=fn: overflowing(fn), note="random values: ArithmeticOverflow near the first row")
         ctx.free(dj)
         # ---------------- config 2: filter + take Int64 1e9 ----------------
         # the same Int64 column one element in (values 8 bytes past a 16-byte boundary, validity offset 1), and its first n
