@@ -37,7 +37,7 @@ struct BytesSrc {
   static constexpr int KEY_BYTES = 8;
   BytesOperand s;
   __device__ __forceinline__ Cand load(int64_t i) const {
-    const BytesItem it = bytes_item(s, i);
+    const BytesItem it = s.item(i);
     return Cand{bswap64(ld_upto8(it.p, (uint32_t)(it.len < 8 ? it.len : 8))), i, it.p, it.len};
   }
 };
@@ -54,10 +54,10 @@ struct ViewSrc {
   static constexpr int KEY_BYTES = 4;
   ViewOperand s;
   __device__ __forceinline__ Cand load(int64_t i) const {
-    const uint4 v = ld_stream16(s.views + i);
+    const uint4 v = s.view(i);
     const uint32_t nb = v.x < 4u ? v.x : 4u;
     const uint32_t prefix = nb == 4u ? v.y : (v.y & ((1u << (nb * 8u)) - 1u));
-    const BytesItem it = view_item(s, v, s.views + i);  // a long value's bytes are only read on a key tie
+    const BytesItem it = s.item(v, s.views + i);  // a long value's bytes are only read on a key tie
     return Cand{(uint64_t)__byte_perm(prefix, 0, 0x0123) << 32, i, it.p, it.len};
   }
 };
@@ -176,12 +176,11 @@ __global__ void __launch_bounds__(256) k_arg_extreme(const ArgArgs p, const Src 
   }
 }
 
-// Shared front end: argument checks, None cases, the null count, one launch, one synchronisation.
-template <class Src>
-acu_status arg_extreme(acu_ctx *ctx, const char *what, acu_agg_op op, const acu_array *nulls, const Src &src, int64_t *out_row,
-                       int64_t *out_valid_count) {
-  *out_row = -1;
-  *out_valid_count = 0;
+// Shared front end: argument checks, None cases, the null count, one launch, one synchronisation. One scratch request
+// holds [table_bytes for make_src][per-CTA partials]; make_src(table_space, &src) builds the source.
+template <class Src, class MakeSrc>
+acu_status arg_extreme(acu_ctx *ctx, const char *what, acu_agg_op op, const acu_array *nulls, size_t table_bytes, MakeSrc make_src,
+                       int64_t *out_row, int64_t *out_valid_count) {
   if (op != ACU_MIN && op != ACU_MAX) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "%s: op must be min or max", what);
   if (nulls->is_scalar) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "%s: the input must be an array, not a scalar", what);
   const int64_t n = nulls->len;
@@ -199,21 +198,16 @@ acu_status arg_extreme(acu_ctx *ctx, const char *what, acu_agg_op op, const acu_
   const int64_t sgroups = (n + 2047) >> 11;
   const int grid = acu_grid(ctx, (sgroups + 7) / 8, 8);
   void *scratch;
-  ACU_TRY(acu_scratch(ctx, (size_t)grid * sizeof(Cand), &scratch));
-  a.partial = static_cast<Cand *>(scratch);
+  ACU_TRY(acu_scratch(ctx, table_bytes + (size_t)grid * sizeof(Cand), &scratch));
+  a.partial = reinterpret_cast<Cand *>(static_cast<uint8_t *>(scratch) + table_bytes);
+  Src src;
+  ACU_TRY(make_src(scratch, &src));
   ACU_TRY(acu_res_reset(ctx));
   if (op == ACU_MIN) ACU_LAUNCH_TIMED(ctx, ACU_K_REDUCE, (k_arg_extreme<ACU_MIN, Src>), grid, 256, 0, a, src);
   else ACU_LAUNCH_TIMED(ctx, ACU_K_REDUCE, (k_arg_extreme<ACU_MAX, Src>), grid, 256, 0, a, src);
   ACU_TRY(acu_res_fetch(ctx));
   *out_valid_count = (int64_t)ctx->h_res[RES_COUNT];
   *out_row = *out_valid_count ? (int64_t)ctx->h_res[RES_AUX0] : -1;
-  return ACU_OK;
-}
-
-acu_status not_in_section(acu_ctx *ctx) {
-  if (ctx->async_on)
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0,
-                    "this entry point synchronises and is not available between acu_async_begin and acu_results_fetch");
   return ACU_OK;
 }
 
@@ -224,10 +218,11 @@ extern "C" acu_status acu_aggregate_bytes(acu_ctx *ctx, int32_t offset_bytes, ac
   ACU_ENTER(ctx);
   *out_row = -1;
   *out_valid_count = 0;
-  ACU_TRY(not_in_section(ctx));
-  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
-  const BytesSrc src{BytesOperand{a->offsets, a->data, offset_bytes}};
-  return arg_extreme(ctx, "acu_aggregate_bytes", op, &a->nulls, src, out_row, out_valid_count);
+  ACU_TRY(acu_sync_only(ctx));
+  ACU_TRY(acu_offset_width_check(ctx, offset_bytes));
+  return arg_extreme<BytesSrc>(
+      ctx, "acu_aggregate_bytes", op, &a->nulls, 0,
+      [&](void *, BytesSrc *src) { return *src = BytesSrc{BytesOperand{a->offsets, a->data, offset_bytes}}, ACU_OK; }, out_row, out_valid_count);
 }
 
 extern "C" acu_status acu_aggregate_byte_view(acu_ctx *ctx, acu_agg_op op, const acu_view_array *a, int64_t *out_row,
@@ -235,25 +230,10 @@ extern "C" acu_status acu_aggregate_byte_view(acu_ctx *ctx, acu_agg_op op, const
   ACU_ENTER(ctx);
   *out_row = -1;
   *out_valid_count = 0;
-  ACU_TRY(not_in_section(ctx));
-  // the data-buffer pointer table goes to the device (its own allocation: the scratch holds the partials)
-  const int nb = a->n_buffers;
-  void *table = nullptr;
-  if (nb > 0 && a->nulls.len > 0) {
-    ACU_TRY(acu_malloc(ctx, (size_t)nb * sizeof(void *), &table));
-    const acu_status st = acu_memcpy_h2d(ctx, table, a->buffers, (size_t)nb * sizeof(void *));
-    if (st != ACU_OK) {
-      acu_free(ctx, table);
-      return st;
-    }
-  }
-  const ViewSrc src{ViewOperand{static_cast<const uint4 *>(a->views), static_cast<const uint8_t *const *>(table), nb}};
-  const acu_status st = arg_extreme(ctx, "acu_aggregate_byte_view", op, &a->nulls, src, out_row, out_valid_count);
-  if (table) {
-    const acu_status fs = acu_free(ctx, table);
-    if (st == ACU_OK && fs != ACU_OK) return fs;
-  }
-  return st;
+  ACU_TRY(acu_sync_only(ctx));
+  return arg_extreme<ViewSrc>(
+      ctx, "acu_aggregate_byte_view", op, &a->nulls, acu_view_table_bytes(a),
+      [&](void *table_space, ViewSrc *src) { return acu_view_operand(ctx, a, table_space, &src->s); }, out_row, out_valid_count);
 }
 
 extern "C" acu_status acu_aggregate_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, acu_agg_op op, const acu_array *a, int64_t *out_row,
@@ -261,10 +241,12 @@ extern "C" acu_status acu_aggregate_fixed_size_binary(acu_ctx *ctx, int32_t byte
   ACU_ENTER(ctx);
   *out_row = -1;
   *out_valid_count = 0;
-  ACU_TRY(not_in_section(ctx));
+  ACU_TRY(acu_sync_only(ctx));
   if (byte_width < 0) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "FixedSizeBinary width must be >= 0, got %d", (int)byte_width);
-  const FixedSrc src{static_cast<const uint8_t *>(a->values), (int64_t)byte_width};
-  return arg_extreme(ctx, "acu_aggregate_fixed_size_binary", op, a, src, out_row, out_valid_count);
+  return arg_extreme<FixedSrc>(
+      ctx, "acu_aggregate_fixed_size_binary", op, a, 0,
+      [&](void *, FixedSrc *src) { return *src = FixedSrc{static_cast<const uint8_t *>(a->values), (int64_t)byte_width}, ACU_OK; }, out_row,
+      out_valid_count);
 }
 
 // min_boolean is Some(false) iff a valid slot is false, max_boolean Some(true) iff a valid slot is true: one popcount of
@@ -273,7 +255,7 @@ extern "C" acu_status acu_aggregate_boolean(acu_ctx *ctx, acu_agg_op op, const a
   ACU_ENTER(ctx);
   *out_value = -1;
   *out_valid_count = 0;
-  ACU_TRY(not_in_section(ctx));
+  ACU_TRY(acu_sync_only(ctx));
   if (op != ACU_MIN && op != ACU_MAX) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "acu_aggregate_boolean: op must be min or max");
   if (a->is_scalar) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "acu_aggregate_boolean: the input must be an array, not a scalar");
   const int64_t n = a->len;

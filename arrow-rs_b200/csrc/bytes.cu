@@ -16,6 +16,7 @@
 #include <stdlib.h>
 
 #include "bitmap.cuh"
+#include "bytes_cmp.cuh"
 #include "bytes_engine.cuh"
 #include "internal.cuh"
 
@@ -24,10 +25,6 @@
 #define PLAN_SCAN_CHUNK 4096
 
 namespace {
-
-__device__ __forceinline__ int64_t ld_off(const void *offs, int ob, int64_t i) {
-  return ob == 4 ? (int64_t)__ldg(static_cast<const int32_t *>(offs) + i) : __ldg(static_cast<const int64_t *>(offs) + i);
-}
 
 template <int IT> struct IdxRaw;
 template <> struct IdxRaw<0> { using t = uint8_t; };
@@ -216,8 +213,8 @@ __device__ __forceinline__ void rows4(const BytesArgs &a, int64_t j0, int64_t be
     s[k] = 0;
     e[k] = 0;
     if (use[k]) {
-      s[k] = ld_off(a.offs, a.ob, (int64_t)ix[k]);
-      e[k] = ld_off(a.offs, a.ob, (int64_t)ix[k] + 1);
+      s[k] = ld_offset(a.offs, a.ob, (int64_t)ix[k]);
+      e[k] = ld_offset(a.offs, a.ob, (int64_t)ix[k] + 1);
     }
   }
 #pragma unroll
@@ -998,7 +995,7 @@ acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offse
                                      void *out_offsets, uint8_t *out_data, int64_t out_cap, acu_array_out *out_nulls, void *scratch,
                                      unsigned long long *res, acu_bytes_col_state *st) {
   *st = acu_bytes_col_state();
-  if (ob != 4 && ob != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_offset_width_check(ctx, ob));
   const int64_t m = indices->len;
   out_nulls->len = m;
   out_nulls->has_validity = 0;
@@ -1031,8 +1028,7 @@ acu_status acu_take_bytes_col_finalize(acu_ctx *ctx, const acu_array *nulls_of, 
   if (oob_row >= 0) {  // the reference panics on a bounds-checked slice index (take.rs:517)
     uint64_t raw = 0;
     const int sz = acu_dtype_size(index_dtype);
-    ACU_CUDA(ctx, cudaMemcpyAsync(&raw, static_cast<const uint8_t *>(indices->values) + (size_t)oob_row * sz, sz, cudaMemcpyDeviceToHost, ctx->stream));
-    ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    ACU_TRY(acu_memcpy_d2h(ctx, &raw, static_cast<const uint8_t *>(indices->values) + (size_t)oob_row * sz, sz));
     uint64_t widened = raw;
     if (index_dtype == ACU_I8) widened = (uint32_t)(int32_t)(int8_t)raw;
     else if (index_dtype == ACU_I16) widened = (uint32_t)(int32_t)(int16_t)raw;
@@ -1052,7 +1048,7 @@ acu_status acu_filter_bytes_col_launch(acu_ctx *ctx, const acu_filter_plan *plan
                                        const acu_array *nulls_of, void *out_offsets, uint8_t *out_data, int64_t out_cap, void *scratch,
                                        unsigned long long *res, acu_bytes_col_state *st) {
   *st = acu_bytes_col_state();
-  if (ob != 4 && ob != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_offset_width_check(ctx, ob));
   const int64_t count = acu_filter_plan_count(plan);
   if (count == 0) return zero_first_offset(ctx, out_offsets, ob);
   const void *idx;

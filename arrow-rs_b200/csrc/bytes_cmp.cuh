@@ -1,25 +1,46 @@
-// bytes_cmp.cuh — device helpers that read and order variable-width values (Utf8 / Binary, Utf8View / BinaryView),
-// shared by the comparison kernels (strcmp.cu), the min / max reductions (aggregate_bytes.cu) and the LIKE family (like.cu).
+// bytes_cmp.cuh — the one operand path of variable-width columns on the device: BytesOperand (Utf8 / Binary, i32 or i64
+// offsets) and ViewOperand (Utf8View / BinaryView) and their row reads, and the helpers that order and match the values.
+// Shared by the comparison kernels (strcmp.cu), the min / max reductions (aggregate_bytes.cu), the LIKE family (like.cu),
+// length / substring (substring.cu) and the gathers (bytes.cu, ld_offset only). The host builds the operands through
+// internal.cuh's front end (acu_offset_width_check, acu_view_operand), after acu_sync_only.
 //
 // Order: Rust's `Ord` for `&[u8]` (lexicographic on unsigned bytes, a proper prefix sorts first); `&str` orders the same.
 #pragma once
 #include "common.cuh"
 
+__device__ __forceinline__ int64_t ld_offset(const void *offs, int ob, int64_t i) {
+  return ob == 4 ? (int64_t)__ldg(static_cast<const int32_t *>(offs) + i) : __ldg(static_cast<const int64_t *>(offs) + i);
+}
+
+// One value: its bytes and length; pre = a view's 4-byte prefix word (0 for byte arrays)
+struct BytesItem {
+  const uint8_t *p;
+  int64_t len;
+  uint32_t pre;
+};
+
 struct BytesOperand {
   const void *offs;
   const uint8_t *data;
   int ob;
+  __device__ __forceinline__ BytesItem item(int64_t i) const {
+    const int64_t b = ld_offset(offs, ob, i), e = ld_offset(offs, ob, i + 1);
+    return BytesItem{data + b, e - b, 0u};
+  }
 };
 
+// views (arrow-data/src/byte_view.rs): x = length, y = prefix / inline[0..4), z, w = inline[4..12) or (buffer index, offset)
 struct ViewOperand {
   const uint4 *views;
   const uint8_t *const *buffers;  // device array of device pointers
   int n_buffers;
+  __device__ __forceinline__ uint4 view(int64_t i) const { return ld_stream16(views + i); }
+  // the value of view v held at `slot`: inline values are read from the slot itself, not from a data buffer
+  __device__ __forceinline__ BytesItem item(const uint4 &v, const uint4 *slot) const {
+    return BytesItem{v.x <= 12u ? reinterpret_cast<const uint8_t *>(slot) + 4 : buffers[v.z] + v.w, (int64_t)v.x, v.y};
+  }
+  __device__ __forceinline__ BytesItem item(int64_t i) const { return item(view(i), views + i); }
 };
-
-__device__ __forceinline__ int64_t ld_offset(const void *offs, int ob, int64_t i) {
-  return ob == 4 ? (int64_t)__ldg(static_cast<const int32_t *>(offs) + i) : __ldg(static_cast<const int64_t *>(offs) + i);
-}
 
 // Up to 8 bytes of p[0 .. nb) as a little-endian u64, zero above nb: aligned 8-byte loads that contain a requested byte.
 __device__ __forceinline__ uint64_t ld_upto8(const uint8_t *__restrict__ p, uint32_t nb) {
@@ -72,17 +93,6 @@ __device__ __forceinline__ bool bytes_lt(const uint8_t *a, int64_t la, const uin
   return la < lb;
 }
 
-struct BytesItem { const uint8_t *p; int64_t len; };
-__device__ __forceinline__ BytesItem bytes_item(const BytesOperand &s, int64_t i) {
-  const int64_t b = ld_offset(s.offs, s.ob, i), e = ld_offset(s.offs, s.ob, i + 1);
-  return BytesItem{s.data + b, e - b};
-}
-
-// ---- views (arrow-data/src/byte_view.rs): x = length, y = prefix / inline[0..4), z, w = inline[4..12) or (buffer index, offset)
-__device__ __forceinline__ BytesItem view_item(const ViewOperand &s, const uint4 &v, const uint4 *slot) {
-  if (v.x <= 12u) return BytesItem{reinterpret_cast<const uint8_t *>(slot) + 4, (int64_t)v.x};
-  return BytesItem{s.buffers[v.z] + v.w, (int64_t)v.x};
-}
 // GenericByteViewArray::inline_key_fast (byte_view_array.rs:872-874): (raw.swap_bytes() << 32) | len, compared as u128
 __device__ __forceinline__ bool inline_key_lt(const uint4 &a, const uint4 &b) {
   // the key's 128 bits, most significant first: inline bytes 0..11 in order (big endian), then the length

@@ -14,6 +14,7 @@
 #include <vector>
 
 #include "bitmap.cuh"
+#include "internal.cuh"
 
 namespace {
 
@@ -111,7 +112,7 @@ extern "C" acu_status acu_bitmap_fill(acu_ctx *ctx, uint8_t *dst, int64_t dst_of
 extern "C" acu_status acu_offsets_append(acu_ctx *ctx, int32_t offset_bytes, const void *src_offsets, int64_t first, int64_t count,
                                          int64_t base, void *dst_offsets, int64_t dst_first, int64_t *out_src_begin, int64_t *out_src_end) {
   ACU_ENTER(ctx);
-  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_offset_width_check(ctx, offset_bytes));
   if (count < 0) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offsets_append: negative count");
   ACU_TRY(acu_res_reset(ctx));
   const int grid = acu_grid(ctx, (count + 1 + 255) / 256, 8);
@@ -152,8 +153,7 @@ static acu_status concat_one_field(acu_ctx *ctx, int32_t n, const acu_column *co
                       "It is not possible to concatenate arrays of different data types (kind %d width %d, kind %d width %d).",
                       c0.kind, c0.width, c.kind, c.width);
   }
-  if (c0.kind == ACU_COL_BYTES && c0.width != 4 && c0.width != 8)
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  if (c0.kind == ACU_COL_BYTES) ACU_TRY(acu_offset_width_check(ctx, c0.width));
   int64_t total = 0;
   bool any_nulls = false;
   int64_t null_total = 0;

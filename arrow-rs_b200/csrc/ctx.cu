@@ -1,12 +1,14 @@
 // ctx.cu — acu_ctx (device + stream + scratch), DeviceBuffer allocation, copies, timing,
-// error detail, synthetic input generators. Boundary: include/arrow_cuda.h.
+// error detail, synthetic input generators, and the operand front end of the Utf8 / Binary / view entry points
+// (internal.cuh). Boundary: include/arrow_cuda.h.
 #include <stdarg.h>
 #include <stdio.h>
 #include <stdlib.h>
 
 #include <new>
 
-#include "common.cuh"
+#include "bytes_cmp.cuh"
+#include "internal.cuh"
 
 acu_status acu_fail(acu_ctx *ctx, acu_status st, int64_t index, uint64_t lhs, uint64_t rhs,
                     uint64_t len, const char *fmt, ...) {
@@ -63,6 +65,32 @@ acu_status acu_scratch(acu_ctx *ctx, size_t bytes, void **out) {
   return ACU_OK;
 }
 
+acu_status acu_sync_only(acu_ctx *ctx) {
+  if (ctx->async_on)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0,
+                    "this entry point synchronises and is not available between acu_async_begin and acu_results_fetch");
+  return ACU_OK;
+}
+
+acu_status acu_offset_width_check(acu_ctx *ctx, int32_t offset_bytes) {
+  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  return ACU_OK;
+}
+
+size_t acu_view_table_bytes(const acu_view_array *a) {
+  return ((size_t)(a->n_buffers > 0 ? a->n_buffers : 0) * sizeof(void *) + 255) & ~(size_t)255;
+}
+
+acu_status acu_view_operand(acu_ctx *ctx, const acu_view_array *a, void *table_space, ViewOperand *out) {
+  const uint8_t *const *table = nullptr;
+  if (a->n_buffers > 0) {
+    ACU_CUDA(ctx, cudaMemcpyAsync(table_space, a->buffers, (size_t)a->n_buffers * sizeof(void *), cudaMemcpyHostToDevice, ctx->stream));
+    table = static_cast<const uint8_t *const *>(table_space);
+  }
+  *out = ViewOperand{static_cast<const uint4 *>(a->views), table, a->n_buffers};
+  return ACU_OK;
+}
+
 __global__ void k_res_reset(unsigned long long *res, int slots) {
   int i = threadIdx.x;
   if (i < slots) res[i] = ((i % RES_SLOTS) == RES_ERR_INDEX || (i % RES_SLOTS) == RES_ERR2) ? ~0ull : 0ull;
@@ -73,9 +101,7 @@ __global__ void k_res_reset(unsigned long long *res, int slots) {
 // res_clean is dropped by the first reset after a fetch; a call that failed between its reset and its fetch leaves
 // res_clean false and the next reset launches k_res_reset itself. res_dirty_blocks = blocks possibly written since.
 acu_status acu_res_reset_n(acu_ctx *ctx, int blocks) {
-  if (ctx->async_on)  // entry points that have not been split into enqueue + finalise would synchronise here
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0,
-                    "this entry point synchronises and is not available between acu_async_begin and acu_results_fetch");
+  ACU_TRY(acu_sync_only(ctx));  // entry points that have not been split into enqueue + finalise would synchronise here
   if (blocks < 1) blocks = 1;
   if (blocks > RES_BLOCKS) blocks = RES_BLOCKS;
   if (!ctx->res_clean) {

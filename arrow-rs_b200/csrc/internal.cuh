@@ -21,6 +21,17 @@ auto acu_with_native(acu_dtype dt, F &&f, G &&otherwise) -> decltype(otherwise()
   }
 }
 
+// The operand front end of every entry point over Utf8 / Binary (acu_bytes_array) and view (acu_view_array) columns.
+// An entry point that synchronises (one not split into enqueue and finalise) refuses inside a stream-ordered section:
+// acu_sync_only is its first check, before any argument check or device work.
+acu_status acu_sync_only(acu_ctx *ctx);
+acu_status acu_offset_width_check(acu_ctx *ctx, int32_t offset_bytes);  // Utf8 / Binary offsets are 4 or 8 bytes wide
+// A view array's data-buffer pointer table goes to acu_view_table_bytes(a) bytes (a multiple of 256) of the caller's one
+// acu_scratch request; acu_view_operand queues the copy of a->buffers there on the ctx stream.
+struct ViewOperand;
+size_t acu_view_table_bytes(const acu_view_array *a);
+acu_status acu_view_operand(acu_ctx *ctx, const acu_view_array *a, void *table_space, ViewOperand *out);
+
 struct acu_filter_plan;
 const uint64_t *acu_plan_mask(const acu_filter_plan *p);      // normalised mask words (padded to x32)
 const uint64_t *acu_plan_tile_off(const acu_filter_plan *p);  // exclusive output offset per 1024-row tile

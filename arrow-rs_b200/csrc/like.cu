@@ -7,7 +7,7 @@
 // and U+017F (s), the simple case folds that reach ASCII. Every element matches one scalar, so a segment's leftmost start
 // is also its leftmost end and the matcher needs no backtracking. The host classifies a scalar pattern once
 // (Predicate::like's Eq / StartsWith / EndsWith / Contains); per-row patterns use the glob on the row's bytes. Row layout
-// as k_cmp_bytes; rows whose match scans more than LONG_ROW bytes are matched by one warp each (k_like_long).
+// as k_cmp_rows; rows whose match scans more than LONG_ROW bytes are matched by one warp each (k_like_long).
 #include <algorithm>
 #include <string>
 #include <type_traits>
@@ -27,30 +27,6 @@ enum { P_PCT = -1, P_ANY = -2 };
 constexpr int ROWS_PER_LANE = 4;
 constexpr int64_t LONG_ROW = 512;   // bytes a row's match may scan before it goes to the warp-per-row kernel
 constexpr int64_t LONG_CAP = 16384; // queued long rows per call; rows beyond it are matched in place
-
-struct RowItem {
-  const uint8_t *p;
-  int64_t len;
-  uint32_t pre;  // views: the 4-byte prefix word of the view
-};
-
-struct BytesAcc {
-  static constexpr bool kViews = false;
-  BytesOperand op;
-  __device__ __forceinline__ RowItem item(int64_t i) const {
-    const BytesItem b = bytes_item(op, i);
-    return RowItem{b.p, b.len, 0u};
-  }
-};
-struct ViewAcc {
-  static constexpr bool kViews = true;
-  ViewOperand op;
-  __device__ __forceinline__ RowItem item(int64_t i) const {
-    const uint4 v = ld_stream16(op.views + i);
-    const BytesItem b = view_item(op, v, op.views + i);  // inline values point into the view slot, not a data buffer
-    return RowItem{b.p, b.len, v.y};
-  }
-};
 
 struct LikeParams {
   int64_t n;
@@ -219,7 +195,7 @@ __device__ __forceinline__ bool glob_match(const uint8_t *P, int64_t pl, const u
 }
 
 template <bool WARP>
-__device__ __forceinline__ bool like_row(int mode, bool icase, const RowItem &h, const RowItem &nd, int lane) {
+__device__ __forceinline__ bool like_row(int mode, bool icase, const BytesItem &h, const BytesItem &nd, int lane) {
   switch (mode) {
     case LM_EQ: case LM_IEQ: return h.len == nd.len && range_eq<WARP>(h.p, nd.p, nd.len, mode == LM_IEQ, lane);
     case LM_PREFIX: case LM_IPREFIX: return h.len >= nd.len && range_eq<WARP>(h.p, nd.p, nd.len, mode == LM_IPREFIX, lane);
@@ -245,14 +221,14 @@ __device__ __forceinline__ bool has_non_ascii(const uint8_t *p, int64_t n) {
   return false;
 }
 
-template <class Acc, int MODE>
-__device__ __forceinline__ bool row_eval(const LikeParams &p, const RowItem &h, const RowItem &nd, int64_t i) {
+template <class Op, int MODE>
+__device__ __forceinline__ bool row_eval(const LikeParams &p, const BytesItem &h, const BytesItem &nd, int64_t i) {
   if (MODE == LM_GLOB && p.check_ascii && has_non_ascii(nd.p, nd.len)) {
     atomicMin(p.res + RES_ERR_INDEX, (unsigned long long)i);
     return false;
   }
   constexpr int mode = MODE;
-  if (Acc::kViews && h.len > 12 && mode != LM_CONTAINS && mode != LM_GLOB && mode != LM_SUFFIX && mode != LM_ISUFFIX) {
+  if (std::is_same<Op, ViewOperand>::value && h.len > 12 && mode != LM_CONTAINS && mode != LM_GLOB && mode != LM_SUFFIX && mode != LM_ISUFFIX) {
     // equal / prefix of an out-of-line view: the length and the view's 4-byte prefix decide before any data buffer is read
     const bool eq = mode == LM_EQ || mode == LM_IEQ, fold = mode == LM_IEQ || mode == LM_IPREFIX;
     if (eq ? h.len != nd.len : h.len < nd.len) return false;
@@ -273,30 +249,30 @@ __device__ __forceinline__ bool row_eval(const LikeParams &p, const RowItem &h, 
 }
 
 // One instantiation per mode: the mode's matcher inlined with no dispatch; the glob keeps one copy of its matcher.
-template <class Acc, int MODE>
-__global__ void __launch_bounds__(256, MODE == LM_GLOB ? 1 : 3) k_like(const LikeParams p, const Acc L, const Acc R) {
+template <class Op, int MODE>
+__global__ void __launch_bounds__(256, MODE == LM_GLOB ? 1 : 3) k_like(const LikeParams p, const Op L, const Op R) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t groups = (p.n + 31) >> 5;
   unsigned valid_cnt = 0;
-  RowItem sl{nullptr, 0, 0u};
-  const RowItem sr{p.needle, p.needle_len, 0u};
+  BytesItem sl{nullptr, 0, 0u};
+  const BytesItem sr{p.needle, p.needle_len, 0u};
   if (p.l_bcast) sl = L.item(0);
   for (int64_t g0 = warp * ROWS_PER_LANE; g0 < groups; g0 += nwarps * ROWS_PER_LANE) {
-    RowItem ih[ROWS_PER_LANE], in[ROWS_PER_LANE];
+    BytesItem ih[ROWS_PER_LANE], in[ROWS_PER_LANE];
 #pragma unroll
     for (int k = 0; k < ROWS_PER_LANE; ++k) {  // the offset / view loads of 4 rows in flight
       const int64_t i = (g0 + k) * 32 + lane;
       const bool live = i < p.n;
-      ih[k] = p.l_bcast ? sl : (live ? L.item(i) : RowItem{nullptr, 0, 0u});
-      in[k] = p.r_bcast ? sr : (live ? R.item(i) : RowItem{nullptr, 0, 0u});
+      ih[k] = p.l_bcast ? sl : (live ? L.item(i) : BytesItem{nullptr, 0, 0u});
+      in[k] = p.r_bcast ? sr : (live ? R.item(i) : BytesItem{nullptr, 0, 0u});
     }
 #pragma unroll (MODE == LM_GLOB ? 1 : ROWS_PER_LANE)
     for (int k = 0; k < ROWS_PER_LANE; ++k) {  // row k's items picked out of the registers
       const int64_t row0 = (g0 + k) * 32;
       if (row0 >= p.n) break;  // warp-uniform
-      RowItem h = ih[0], nd = in[0];
+      BytesItem h = ih[0], nd = in[0];
 #pragma unroll
       for (int j = 1; j < ROWS_PER_LANE; ++j)
         if (k == j) h = ih[j], nd = in[j];
@@ -307,7 +283,7 @@ __global__ void __launch_bounds__(256, MODE == LM_GLOB ? 1 : 3) k_like(const Lik
       if (p.rv) rw &= ld_bits32(p.rv, p.roff + row0, p.roff + p.n);
       const uint32_t valid = p.binary ? (lw & rw) : lw;
       const bool eval = ((p.binary ? valid : m) >> lane) & 1u;
-      const bool r = eval && row_eval<Acc, MODE>(p, h, nd, row0 + lane);
+      const bool r = eval && row_eval<Op, MODE>(p, h, nd, row0 + lane);
       uint32_t v = __ballot_sync(ACU_FULL_MASK, r);
       if (lane == 0) {
         if (p.neg) v = ~v;
@@ -323,26 +299,26 @@ __global__ void __launch_bounds__(256, MODE == LM_GLOB ? 1 : 3) k_like(const Lik
 }
 
 // The queued long rows, one warp each; the provisional bit (no match) is flipped where the row matches.
-template <class Acc, int MODE>
-__global__ void __launch_bounds__(256, 1) k_like_long(const LikeParams p, const Acc L, const Acc R, int64_t count) {
+template <class Op, int MODE>
+__global__ void __launch_bounds__(256, 1) k_like_long(const LikeParams p, const Op L, const Op R, int64_t count) {
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t k = warp; k < count; k += nwarps) {
     const int64_t i = p.long_rows[k];
-    const RowItem h = L.item(p.l_bcast ? 0 : i);
-    const RowItem nd = p.r_bcast ? RowItem{p.needle, p.needle_len, 0u} : R.item(i);
+    const BytesItem h = L.item(p.l_bcast ? 0 : i);
+    const BytesItem nd = p.r_bcast ? BytesItem{p.needle, p.needle_len, 0u} : R.item(i);
     if (like_row<true>(MODE, p.icase != 0, h, nd, lane) && lane == 0) atomicXor(p.out_bits + (i >> 5), 1u << (i & 31));
   }
 }
 
 // GenericByteViewArray::is_ascii (byte_view_array.rs:1177-1188): a valid slot holding a byte >= 0x80 sets RES_AUX1.
-template <class Acc>
-__global__ void __launch_bounds__(256) k_view_non_ascii(const Acc V, int64_t n, const uint8_t *valid, int64_t voff,
+template <class Op>
+__global__ void __launch_bounds__(256) k_view_non_ascii(const Op V, int64_t n, const uint8_t *valid, int64_t voff,
                                                         unsigned long long *res) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     if (valid && !ld_bit(valid, voff + i)) continue;
-    const RowItem it = V.item(i);
+    const BytesItem it = V.item(i);
     if (has_non_ascii(it.p, it.len)) atomicOr(res + RES_AUX1, 1ull);
   }
 }
@@ -384,58 +360,48 @@ int ilike_ascii_shape(const std::string &pat, std::string *needle) {
   return -1;
 }
 
-acu_status d2h(acu_ctx *ctx, void *dst, const void *src, size_t n) {
-  if (n) ACU_CUDA(ctx, cudaMemcpy(dst, src, n, cudaMemcpyDeviceToHost));
-  return ACU_OK;
-}
-
-// The bytes of row 0 of a scalar operand.
+// The bytes of row 0 of a scalar operand, read in stream order.
 acu_status scalar_bytes(acu_ctx *ctx, int ob, const acu_bytes_array *s, std::string *out) {
   int64_t o[2] = {0, 0};
   if (ob == 4) {
     int32_t o32[2];
-    ACU_TRY(d2h(ctx, o32, s->offsets, sizeof o32));
+    ACU_TRY(acu_memcpy_d2h(ctx, o32, s->offsets, sizeof o32));
     o[0] = o32[0], o[1] = o32[1];
   } else {
-    ACU_TRY(d2h(ctx, o, s->offsets, sizeof o));
+    ACU_TRY(acu_memcpy_d2h(ctx, o, s->offsets, sizeof o));
   }
   out->assign((size_t)(o[1] - o[0]), '\0');
-  return d2h(ctx, &(*out)[0], s->data + o[0], out->size());
+  return acu_memcpy_d2h(ctx, &(*out)[0], s->data + o[0], out->size());
 }
 acu_status scalar_bytes(acu_ctx *ctx, int, const acu_view_array *s, std::string *out) {
   uint32_t v[4];
-  ACU_TRY(d2h(ctx, v, s->views, sizeof v));
+  ACU_TRY(acu_memcpy_d2h(ctx, v, s->views, sizeof v));
   out->assign(v[0], '\0');
   if (v[0] <= 12) return memcpy(&(*out)[0], reinterpret_cast<const char *>(v) + 4, v[0]), ACU_OK;
   if (v[2] >= (uint32_t)s->n_buffers) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "view buffer index out of range");
-  return d2h(ctx, &(*out)[0], s->buffers[v[2]] + v[3], out->size());
+  return acu_memcpy_d2h(ctx, &(*out)[0], s->buffers[v[2]] + v[3], out->size());
 }
 
-// Device accessors; the view pointer tables go to `*cursor` (scratch).
-acu_status make_acc(acu_ctx *, int ob, const acu_bytes_array *a, uint8_t **, BytesAcc *acc) {
-  *acc = BytesAcc{BytesOperand{a->offsets, a->data, ob}};
-  return ACU_OK;
-}
-acu_status make_acc(acu_ctx *ctx, int, const acu_view_array *a, uint8_t **cursor, ViewAcc *acc) {
-  const uint8_t *const *table = nullptr;
-  if (a->n_buffers > 0) {
-    table = reinterpret_cast<const uint8_t *const *>(*cursor);
-    ACU_CUDA(ctx, cudaMemcpyAsync(*cursor, a->buffers, (size_t)a->n_buffers * sizeof(void *), cudaMemcpyHostToDevice, ctx->stream));
-    *cursor += ((size_t)a->n_buffers * sizeof(void *) + 255) & ~(size_t)255;
-  }
-  *acc = ViewAcc{ViewOperand{static_cast<const uint4 *>(a->views), table, a->n_buffers}};
-  return ACU_OK;
-}
+// The device operands; the view pointer tables go to `*cursor` (scratch).
 size_t table_bytes(const acu_bytes_array *) { return 0; }
-size_t table_bytes(const acu_view_array *a) { return ((size_t)(a->n_buffers > 0 ? a->n_buffers : 0) * sizeof(void *) + 255) & ~(size_t)255; }
+size_t table_bytes(const acu_view_array *a) { return acu_view_table_bytes(a); }
+acu_status make_operand(acu_ctx *, int ob, const acu_bytes_array *a, uint8_t **, BytesOperand *op) {
+  *op = BytesOperand{a->offsets, a->data, ob};
+  return ACU_OK;
+}
+acu_status make_operand(acu_ctx *ctx, int, const acu_view_array *a, uint8_t **cursor, ViewOperand *op) {
+  ACU_TRY(acu_view_operand(ctx, a, *cursor, op));
+  *cursor += acu_view_table_bytes(a);
+  return ACU_OK;
+}
 
 // k_like (count < 0) or k_like_long over `count` queued rows, instantiated for p.mode
-template <class Acc>
-acu_status launch_like(acu_ctx *ctx, const LikeParams &p, const Acc &L, const Acc &R, int grid, int64_t count) {
+template <class Op>
+acu_status launch_like(acu_ctx *ctx, const LikeParams &p, const Op &L, const Op &R, int grid, int64_t count) {
 #define LIKE_CASE(M)                                                                             \
   case M:                                                                                        \
-    if (count < 0) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_like<Acc, M>), grid, 256, 0, p, L, R);         \
-    else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_like_long<Acc, M>), grid, 256, 0, p, L, R, count);        \
+    if (count < 0) ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_like<Op, M>), grid, 256, 0, p, L, R);         \
+    else ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, (k_like_long<Op, M>), grid, 256, 0, p, L, R, count);        \
     return ACU_OK;
   switch (p.mode) {
     LIKE_CASE(LM_EQ) LIKE_CASE(LM_PREFIX) LIKE_CASE(LM_SUFFIX) LIKE_CASE(LM_CONTAINS)
@@ -525,15 +491,15 @@ acu_status like_run(acu_ctx *ctx, int ob, int32_t is_utf8, acu_like_op op, const
   void *scratch;
   ACU_TRY(acu_scratch(ctx, tb + nb + (size_t)LONG_CAP * sizeof(int64_t), &scratch));
   uint8_t *cursor = static_cast<uint8_t *>(scratch);
-  using Acc = typename std::conditional<std::is_same<Arr, acu_view_array>::value, ViewAcc, BytesAcc>::type;
-  Acc L, R;
-  ACU_TRY(make_acc(ctx, ob, l, &cursor, &L));
-  ACU_TRY(make_acc(ctx, ob, r, &cursor, &R));
+  using Op = typename std::conditional<std::is_same<Arr, acu_view_array>::value, ViewOperand, BytesOperand>::type;
+  Op L, R;
+  ACU_TRY(make_operand(ctx, ob, l, &cursor, &L));
+  ACU_TRY(make_operand(ctx, ob, r, &cursor, &R));
   uint8_t *d_needle = cursor;
   p.long_rows = reinterpret_cast<int64_t *>(cursor + nb);
   if (quirk) {
     ACU_TRY(acu_res_reset(ctx));
-    ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_view_non_ascii<Acc>, acu_grid(ctx, (len + 255) / 256, 8), 256, 0, L, len, l->nulls.validity,
+    ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_view_non_ascii<Op>, acu_grid(ctx, (len + 255) / 256, 8), 256, 0, L, len, l->nulls.validity,
                      l->nulls.validity_offset, ctx->d_res);
     ACU_TRY(acu_res_fetch(ctx));
     if (ctx->h_res[RES_AUX1] == 0) p.mode = quirk_mode, needle = quirk_needle;
@@ -566,12 +532,14 @@ acu_status like_run(acu_ctx *ctx, int ob, int32_t is_utf8, acu_like_op op, const
 extern "C" acu_status acu_like_bytes(acu_ctx *ctx, int32_t offset_bytes, int32_t is_utf8, acu_like_op op, const acu_bytes_array *l,
                                      const acu_bytes_array *r, acu_array_out *out) {
   ACU_ENTER(ctx);
-  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_sync_only(ctx));
+  ACU_TRY(acu_offset_width_check(ctx, offset_bytes));
   return like_run(ctx, offset_bytes, is_utf8, op, l, r, out);
 }
 
 extern "C" acu_status acu_like_byte_view(acu_ctx *ctx, int32_t is_utf8, acu_like_op op, const acu_view_array *l, const acu_view_array *r,
                                          acu_array_out *out) {
   ACU_ENTER(ctx);
+  ACU_TRY(acu_sync_only(ctx));
   return like_run(ctx, 0, is_utf8, op, l, r, out);
 }

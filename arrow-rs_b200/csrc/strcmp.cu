@@ -37,7 +37,7 @@ __device__ __forceinline__ bool view_is_eq(const ViewOperand &L, const uint4 &l,
   if (l.x == 0u) return true;
   if (l.y != r.y) return false;
   if (l.x <= 12u) return false;
-  const BytesItem a = view_item(L, l, lslot), b = view_item(R, r, rslot);
+  const BytesItem a = L.item(l, lslot), b = R.item(r, rslot);
   return bytes_eq(a.p, a.len, b.p, b.len);
 }
 __device__ __forceinline__ bool view_is_lt(const ViewOperand &L, const uint4 &l, const uint4 *lslot, const ViewOperand &R, const uint4 &r,
@@ -45,7 +45,7 @@ __device__ __forceinline__ bool view_is_lt(const ViewOperand &L, const uint4 &l,
   if (L.n_buffers == 0 && R.n_buffers == 0) return inline_key_lt(l, r);
   if (l.x <= 12u && r.x <= 12u) return inline_key_lt(l, r);
   if (l.y != r.y) return __byte_perm(l.y, 0, 0x0123) < __byte_perm(r.y, 0, 0x0123);
-  const BytesItem a = view_item(L, l, lslot), b = view_item(R, r, rslot);
+  const BytesItem a = L.item(l, lslot), b = R.item(r, rslot);
   return bytes_lt(a.p, a.len, b.p, b.len);
 }
 
@@ -70,65 +70,49 @@ __device__ __forceinline__ void finish_group(const RowCmpCommon &p, int64_t row0
 
 constexpr int ROWS_PER_LANE = 4;
 
-__global__ void __launch_bounds__(256) k_cmp_bytes(const RowCmpCommon p, const BytesOperand A, const BytesOperand B) {
+// byte arrays compare the items; views compare the view words first and read a value's bytes only when they must
+__device__ __forceinline__ BytesItem cmp_scalar(const BytesOperand &s) { return s.item(0); }
+__device__ __forceinline__ uint4 cmp_scalar(const ViewOperand &s) { return __ldg(s.views); }
+__device__ __forceinline__ BytesItem cmp_load(const BytesOperand &s, int64_t i) { return s.item(i); }
+__device__ __forceinline__ uint4 cmp_load(const ViewOperand &s, int64_t i) { return s.view(i); }
+__device__ __forceinline__ bool cmp_row(const RowCmpCommon &p, const BytesOperand &, const BytesItem &a, const BytesOperand &, const BytesItem &b,
+                                        int64_t) {
+  return p.lt ? bytes_lt(a.p, a.len, b.p, b.len) : bytes_eq(a.p, a.len, b.p, b.len);
+}
+__device__ __forceinline__ bool cmp_row(const RowCmpCommon &p, const ViewOperand &A, const uint4 &a, const ViewOperand &B, const uint4 &b,
+                                        int64_t i) {
+  const uint4 *as = A.views + (p.a_scalar ? 0 : i), *bs = B.views + (p.b_scalar ? 0 : i);
+  return p.lt ? view_is_lt(A, a, as, B, b, bs) : view_is_eq(A, a, as, B, b, bs);
+}
+
+// One kernel for both layouts (Op = BytesOperand or ViewOperand): only the row read and the compare differ.
+template <class Op>
+__global__ void __launch_bounds__(256) k_cmp_rows(const RowCmpCommon p, const Op A, const Op B) {
+  using Row = decltype(cmp_load(A, 0));
   const int lane = threadIdx.x & 31;
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
   const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   const int64_t groups = (p.n + 31) >> 5;
   unsigned valid_cnt = 0;
-  BytesItem sa{nullptr, 0}, sb{nullptr, 0};
-  if (p.a_scalar) sa = bytes_item(A, 0);
-  if (p.b_scalar) sb = bytes_item(B, 0);
+  Row sa{}, sb{};
+  if (p.a_scalar) sa = cmp_scalar(A);
+  if (p.b_scalar) sb = cmp_scalar(B);
   for (int64_t g0 = warp * ROWS_PER_LANE; g0 < groups; g0 += nwarps * ROWS_PER_LANE) {
-    BytesItem ia[ROWS_PER_LANE], ib[ROWS_PER_LANE];
+    Row ia[ROWS_PER_LANE], ib[ROWS_PER_LANE];
 #pragma unroll
-    for (int k = 0; k < ROWS_PER_LANE; ++k) {  // the offset loads of 4 rows in flight
+    for (int k = 0; k < ROWS_PER_LANE; ++k) {  // the offset / view loads of 4 rows in flight
       const int64_t i = (g0 + k) * 32 + lane;
       const bool live = i < p.n;
-      ia[k] = p.a_scalar ? sa : (live ? bytes_item(A, i) : BytesItem{nullptr, 0});
-      ib[k] = p.b_scalar ? sb : (live ? bytes_item(B, i) : BytesItem{nullptr, 0});
+      ia[k] = p.a_scalar ? sa : (live ? cmp_load(A, i) : Row{});
+      ib[k] = p.b_scalar ? sb : (live ? cmp_load(B, i) : Row{});
     }
 #pragma unroll
     for (int k = 0; k < ROWS_PER_LANE; ++k) {
       const int64_t row0 = (g0 + k) * 32;
       if (row0 >= p.n) break;  // warp-uniform
-      const bool live = row0 + lane < p.n;
-      bool r = false;
-      if (live) r = p.lt ? bytes_lt(ia[k].p, ia[k].len, ib[k].p, ib[k].len) : bytes_eq(ia[k].p, ia[k].len, ib[k].p, ib[k].len);
-      finish_group(p, row0, __ballot_sync(ACU_FULL_MASK, r), lane, valid_cnt);
-    }
-  }
-  if (p.out_valid && lane == 0 && valid_cnt) atomicAdd(p.res + RES_COUNT, (unsigned long long)valid_cnt);
-}
-
-__global__ void __launch_bounds__(256) k_cmp_views(const RowCmpCommon p, const ViewOperand A, const ViewOperand B) {
-  const int lane = threadIdx.x & 31;
-  const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
-  const int64_t nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
-  const int64_t groups = (p.n + 31) >> 5;
-  unsigned valid_cnt = 0;
-  uint4 sa = make_uint4(0, 0, 0, 0), sb = make_uint4(0, 0, 0, 0);
-  if (p.a_scalar) sa = __ldg(A.views);
-  if (p.b_scalar) sb = __ldg(B.views);
-  for (int64_t g0 = warp * ROWS_PER_LANE; g0 < groups; g0 += nwarps * ROWS_PER_LANE) {
-    uint4 va[ROWS_PER_LANE], vb[ROWS_PER_LANE];
-#pragma unroll
-    for (int k = 0; k < ROWS_PER_LANE; ++k) {
-      const int64_t i = (g0 + k) * 32 + lane;
-      const bool live = i < p.n;
-      va[k] = p.a_scalar ? sa : (live ? ld_stream16(A.views + i) : make_uint4(0, 0, 0, 0));
-      vb[k] = p.b_scalar ? sb : (live ? ld_stream16(B.views + i) : make_uint4(0, 0, 0, 0));
-    }
-#pragma unroll
-    for (int k = 0; k < ROWS_PER_LANE; ++k) {
-      const int64_t row0 = (g0 + k) * 32;
-      if (row0 >= p.n) break;
       const int64_t i = row0 + lane;
       bool r = false;
-      if (i < p.n) {
-        const uint4 *as = A.views + (p.a_scalar ? 0 : i), *bs = B.views + (p.b_scalar ? 0 : i);
-        r = p.lt ? view_is_lt(A, va[k], as, B, vb[k], bs) : view_is_eq(A, va[k], as, B, vb[k], bs);
-      }
+      if (i < p.n) r = cmp_row(p, A, ia[k], B, ib[k], i);
       finish_group(p, row0, __ballot_sync(ACU_FULL_MASK, r), lane, valid_cnt);
     }
   }
@@ -182,7 +166,8 @@ int cmp_grid(acu_ctx *ctx, int64_t n, int rows_per_lane) {
 extern "C" acu_status acu_cmp_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_cmp_op op, const acu_bytes_array *l, const acu_bytes_array *r,
                                     acu_array_out *out) {
   ACU_ENTER(ctx);
-  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_sync_only(ctx));
+  ACU_TRY(acu_offset_width_check(ctx, offset_bytes));
   acu_cmp_decision d;
   ACU_TRY(acu_cmp_decide(ctx, op, &l->nulls, &r->nulls, out, &d));
   if (d.len == 0) return ACU_OK;
@@ -190,7 +175,7 @@ extern "C" acu_status acu_cmp_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_cmp_
   const acu_bytes_array *x = d.swap ? r : l, *y = d.swap ? l : r;
   const BytesOperand A{x->offsets, x->data, offset_bytes}, B{y->offsets, y->data, offset_bytes};
   ACU_TRY(acu_res_reset(ctx));
-  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_bytes, cmp_grid(ctx, d.len, ROWS_PER_LANE), 256, 0, row_cmp_params(ctx, d, out), A, B);
+  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_rows<BytesOperand>, cmp_grid(ctx, d.len, ROWS_PER_LANE), 256, 0, row_cmp_params(ctx, d, out), A, B);
   ACU_TRY(acu_res_fetch(ctx));
   acu_cmp_finalize(d, ctx->h_res, out);
   return ACU_OK;
@@ -198,6 +183,7 @@ extern "C" acu_status acu_cmp_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_cmp_
 
 extern "C" acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_view_array *l, const acu_view_array *r, acu_array_out *out) {
   ACU_ENTER(ctx);
+  ACU_TRY(acu_sync_only(ctx));
   const bool ls = l->nulls.is_scalar != 0, rs = r->nulls.is_scalar != 0;
   // eq_inline_scalar (cmp.rs:282-300): == / != of an array against a non-null constant of <= 4 bytes
   if ((op == ACU_EQ || op == ACU_NEQ) && ls != rs) {
@@ -207,8 +193,7 @@ extern "C" acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_v
     if (sc->nulls.len >= 1) ACU_TRY(st);
     if (sc->nulls.len >= 1 && snc == 0) {
       uint64_t low = 0;
-      ACU_CUDA(ctx, cudaMemcpyAsync(&low, sc->views, 8, cudaMemcpyDeviceToHost, ctx->stream));
-      ACU_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      ACU_TRY(acu_memcpy_d2h(ctx, &low, sc->views, 8));
       const uint32_t needle_len = (uint32_t)low;
       if (needle_len <= 4) {
         const uint64_t significant = ~0ull >> (32 - needle_len * 8);
@@ -239,18 +224,13 @@ extern "C" acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_v
   if (d.all_null) return acu_new_null(ctx, d.len, acu_bitmap_bytes(d.len), out);
   const acu_view_array *x = d.swap ? r : l, *y = d.swap ? l : r;
   // the data-buffer pointer tables go to the device (scratch): [x buffers][y buffers]
-  const int nx = x->n_buffers, ny = y->n_buffers;
-  const uint8_t **table = nullptr;
-  if (nx + ny > 0) {
-    void *scratch;
-    ACU_TRY(acu_scratch(ctx, (size_t)(nx + ny) * sizeof(void *), &scratch));
-    table = static_cast<const uint8_t **>(scratch);
-    if (nx) ACU_CUDA(ctx, cudaMemcpyAsync(table, x->buffers, (size_t)nx * sizeof(void *), cudaMemcpyHostToDevice, ctx->stream));
-    if (ny) ACU_CUDA(ctx, cudaMemcpyAsync(table + nx, y->buffers, (size_t)ny * sizeof(void *), cudaMemcpyHostToDevice, ctx->stream));
-  }
-  const ViewOperand A{static_cast<const uint4 *>(x->views), table, nx}, B{static_cast<const uint4 *>(y->views), table ? table + nx : nullptr, ny};
+  void *scratch;
+  ACU_TRY(acu_scratch(ctx, acu_view_table_bytes(x) + acu_view_table_bytes(y), &scratch));
+  ViewOperand A, B;
+  ACU_TRY(acu_view_operand(ctx, x, scratch, &A));
+  ACU_TRY(acu_view_operand(ctx, y, static_cast<uint8_t *>(scratch) + acu_view_table_bytes(x), &B));
   ACU_TRY(acu_res_reset(ctx));
-  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_views, cmp_grid(ctx, d.len, ROWS_PER_LANE), 256, 0, row_cmp_params(ctx, d, out), A, B);
+  ACU_LAUNCH_TIMED(ctx, ACU_K_CMP, k_cmp_rows<ViewOperand>, cmp_grid(ctx, d.len, ROWS_PER_LANE), 256, 0, row_cmp_params(ctx, d, out), A, B);
   ACU_TRY(acu_res_fetch(ctx));
   acu_cmp_finalize(d, ctx->h_res, out);
   return ACU_OK;

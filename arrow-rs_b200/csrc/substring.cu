@@ -225,9 +225,7 @@ __device__ __forceinline__ void char_bounds(const uint8_t *p, int64_t L, int64_t
 }
 
 struct CharParams {
-  int ob;
-  const void *offs;
-  const uint8_t *data;
+  BytesOperand src;
   const uint8_t *valid;  // NULL = no nulls
   int64_t voff, n;
   int64_t start;
@@ -243,13 +241,13 @@ __global__ void __launch_bounds__(256) k_char_bounds(const CharParams p) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += stride) {
     int64_t b = 0, l = 0;
     if (!p.valid || ld_bit(p.valid, p.voff + i)) {  // null slots become empty
-      const int64_t p0 = ld_offset(p.offs, p.ob, i), p1 = ld_offset(p.offs, p.ob, i + 1);
+      const int64_t p0 = ld_offset(p.src.offs, p.src.ob, i), p1 = ld_offset(p.src.offs, p.src.ob, i + 1);
       const int64_t L = p1 - p0;
       if (L > LONG_ROW) {
         p.long_rows[atomicAdd(p.res + RES_AUX0, 1ull)] = i;
       } else {
         int64_t s, e;
-        char_bounds<false>(p.data + p0, L, p.start, p.has_len != 0, p.length, 0, &s, &e);
+        char_bounds<false>(p.src.data + p0, L, p.start, p.has_len != 0, p.length, 0, &s, &e);
         b = p0 + s, l = e - s;
       }
     }
@@ -265,9 +263,9 @@ __global__ void __launch_bounds__(256) k_char_long(const CharParams p) {
   const int64_t warp = ((int64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = ((int64_t)gridDim.x * blockDim.x) >> 5;
   for (int64_t k = warp; k < count; k += nwarps) {
     const int64_t i = p.long_rows[k];
-    const int64_t p0 = ld_offset(p.offs, p.ob, i), p1 = ld_offset(p.offs, p.ob, i + 1);
+    const int64_t p0 = ld_offset(p.src.offs, p.src.ob, i), p1 = ld_offset(p.src.offs, p.src.ob, i + 1);
     int64_t s, e;
-    char_bounds<true>(p.data + p0, p1 - p0, p.start, p.has_len != 0, p.length, lane, &s, &e);
+    char_bounds<true>(p.src.data + p0, p1 - p0, p.start, p.has_len != 0, p.length, lane, &s, &e);
     if (lane == 0) p.rb[i] = p0 + s, p.rl[i] = e - s;
   }
 }
@@ -275,8 +273,7 @@ __global__ void __launch_bounds__(256) k_char_long(const CharParams p) {
 // ---- substring of a view array (substring.rs:254-317) -----------------------------------------------------------------
 // Failure key of row j: 4j (start offset not a char boundary), 4j + 1 (end offset), 4j + 2 (the slice panics).
 struct ViewSubstr {
-  const uint4 *views;
-  const uint8_t *const *buffers;  // device array of the data buffers
+  ViewOperand src;
   const uint8_t *valid;
   int64_t voff, n;
   int64_t start;
@@ -293,9 +290,10 @@ __global__ void __launch_bounds__(256) k_substr_view(const ViewSubstr p) {
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < p.n; i += stride) {
     uint4 r = make_uint4(0, 0, 0, 0);  // a null slot: append_null's all-zero view
     if (!p.valid || ld_bit(p.valid, p.voff + i)) {
-      const uint4 v = ld_stream16(p.views + i);
-      const int64_t L = v.x;
-      const uint8_t *val = L <= 12 ? reinterpret_cast<const uint8_t *>(p.views + i) + 4 : p.buffers[v.z] + v.w;
+      const uint4 v = p.src.view(i);
+      const BytesItem it = p.src.item(v, p.src.views + i);
+      const int64_t L = it.len;
+      const uint8_t *val = it.p;
       int64_t s, e;
       view_range(L, p.start, p.has_len != 0, p.length, &s, &e);
       unsigned long long key = ~0ull;
@@ -337,11 +335,6 @@ __global__ void __launch_bounds__(256) k_fsb_substr(const uint8_t *__restrict__ 
 }
 
 // ---- host side -------------------------------------------------------------------------------------------------------
-acu_status d2h(acu_ctx *ctx, void *dst, const void *src, size_t n) {
-  if (n) ACU_CUDA(ctx, cudaMemcpy(dst, src, n, cudaMemcpyDeviceToHost));
-  return ACU_OK;
-}
-
 acu_status check_input(acu_ctx *ctx, const acu_array *nulls, const char *what) {
   if (nulls->is_scalar) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "%s takes an array, not a scalar", what);
   if (nulls->len < 0) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "%s: negative length", what);
@@ -433,7 +426,7 @@ acu_status substring_bytes_run(acu_ctx *ctx, int32_t is_utf8, int64_t start, boo
   if (key != ~0ull) {  // the failing row's offsets, recomputed as the kernel did
     const int64_t row = (int64_t)(key >= PANIC_KEY ? key - PANIC_KEY : key / 2);
     O o[2];
-    ACU_TRY(d2h(ctx, o, static_cast<const O *>(a->offsets) + row, sizeof o));
+    ACU_TRY(acu_memcpy_d2h(ctx, o, static_cast<const O *>(a->offsets) + row, sizeof o));
     O s, e;
     byte_range<O>(o[0], o[1], st, has_len, ln, &s, &e);
     const uint64_t us = (uint64_t)(int64_t)s, ue = (uint64_t)(int64_t)e;  // as_usize
@@ -451,7 +444,7 @@ acu_status substring_by_char_run(acu_ctx *ctx, int32_t ob, int64_t start, bool h
     const size_t eng = engine_scratch(n), ranges = align256((size_t)n * 8);
     ACU_TRY(acu_scratch(ctx, eng + 2 * ranges + ranges, &scratch));
     uint8_t *base = static_cast<uint8_t *>(scratch);
-    CharParams p{ob, a->offsets, a->data, a->nulls.validity, a->nulls.validity_offset, n, start, has_len, length,
+    CharParams p{BytesOperand{a->offsets, a->data, ob}, a->nulls.validity, a->nulls.validity_offset, n, start, has_len, length,
                  reinterpret_cast<int64_t *>(base + eng), reinterpret_cast<int64_t *>(base + eng + ranges),
                  reinterpret_cast<int64_t *>(base + eng + 2 * ranges), ctx->d_res};
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_char_bounds, acu_grid(ctx, (n + 255) / 256, 8), 256, 0, p);
@@ -471,10 +464,12 @@ acu_status substring_by_char_run(acu_ctx *ctx, int32_t ob, int64_t start, bool h
 
 }  // namespace
 
+// Every entry point starts with acu_res_reset, whose acu_sync_only refuses inside a stream-ordered section before any
+// argument check.
 extern "C" acu_status acu_length_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_length_op op, const acu_bytes_array *a, acu_array_out *out) {
   ACU_ENTER(ctx);
   ACU_TRY(acu_res_reset(ctx));
-  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_offset_width_check(ctx, offset_bytes));
   if (op != ACU_LENGTH && op != ACU_BIT_LENGTH) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "invalid length op %d", (int)op);
   ACU_TRY(check_input(ctx, &a->nulls, "length"));
   const int64_t n = a->nulls.len;
@@ -536,7 +531,7 @@ extern "C" acu_status acu_substring_bytes(acu_ctx *ctx, int32_t offset_bytes, in
                                           int64_t out_data_capacity, int64_t *out_data_len, acu_array_out *out_nulls) {
   ACU_ENTER(ctx);
   ACU_TRY(acu_res_reset(ctx));
-  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_offset_width_check(ctx, offset_bytes));
   ACU_TRY(check_input(ctx, &a->nulls, "substring"));
   if (data_len < 0) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "substring: negative data length");
   if (offset_bytes == 4)
@@ -551,7 +546,7 @@ extern "C" acu_status acu_substring_by_char(acu_ctx *ctx, int32_t offset_bytes, 
                                             int64_t *out_data_len, acu_array_out *out_nulls) {
   ACU_ENTER(ctx);
   ACU_TRY(acu_res_reset(ctx));
-  if (offset_bytes != 4 && offset_bytes != 8) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offset width must be 4 or 8");
+  ACU_TRY(acu_offset_width_check(ctx, offset_bytes));
   ACU_TRY(check_input(ctx, &a->nulls, "substring_by_char"));
   return substring_by_char_run(ctx, offset_bytes, start, has_length != 0, length, a, out_offsets, out_data, out_data_capacity, out_data_len,
                                out_nulls);
@@ -563,16 +558,11 @@ extern "C" acu_status acu_substring_byte_view(acu_ctx *ctx, int32_t is_utf8, int
   ACU_TRY(acu_res_reset(ctx));
   ACU_TRY(check_input(ctx, &a->nulls, "substring"));
   const int64_t n = a->nulls.len;
-  const uint8_t *const *table = nullptr;
   if (n > 0) {
-    if (a->n_buffers > 0) {
-      void *scratch;
-      ACU_TRY(acu_scratch(ctx, (size_t)a->n_buffers * sizeof(void *), &scratch));
-      ACU_CUDA(ctx, cudaMemcpyAsync(scratch, a->buffers, (size_t)a->n_buffers * sizeof(void *), cudaMemcpyHostToDevice, ctx->stream));
-      table = static_cast<const uint8_t *const *>(scratch);
-    }
-    ViewSubstr p{static_cast<const uint4 *>(a->views), table, a->nulls.validity, a->nulls.validity_offset, n, start, has_length, length,
-                 static_cast<uint4 *>(out_views), ctx->d_res};
+    void *scratch;
+    ACU_TRY(acu_scratch(ctx, acu_view_table_bytes(a), &scratch));
+    ViewSubstr p{{}, a->nulls.validity, a->nulls.validity_offset, n, start, has_length, length, static_cast<uint4 *>(out_views), ctx->d_res};
+    ACU_TRY(acu_view_operand(ctx, a, scratch, &p.src));
     const int grid = acu_grid(ctx, (n + 255) / 256, 8);
     if (is_utf8) ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_substr_view<true>, grid, 256, 0, p);
     else ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_substr_view<false>, grid, 256, 0, p);
@@ -584,7 +574,7 @@ extern "C" acu_status acu_substring_byte_view(acu_ctx *ctx, int32_t is_utf8, int
   if (n == 0 || key == ~0ull) return ACU_OK;
   const int64_t row = (int64_t)(key / 4);
   uint32_t v[4];
-  ACU_TRY(d2h(ctx, v, static_cast<const uint4 *>(a->views) + row, sizeof v));
+  ACU_TRY(acu_memcpy_d2h(ctx, v, static_cast<const uint4 *>(a->views) + row, sizeof v));
   int64_t s, e;
   view_range(v[0], start, has_length != 0, length, &s, &e);
   if (key % 4 == 2) return slice_panic(ctx, row, (uint64_t)s, (uint64_t)e, v[0]);

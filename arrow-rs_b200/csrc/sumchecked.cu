@@ -443,8 +443,6 @@ extern "C" acu_status acu_product_checked(acu_ctx *ctx, acu_dtype dtype, const a
   ACU_ENTER(ctx);
   *out_bits = 0;
   *out_valid_count = 0;
-  if (ctx->async_on)  // refused whatever the input, before any device work (also for floats and empty inputs)
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0,
-                    "this entry point synchronises and is not available between acu_async_begin and acu_results_fetch");
+  ACU_TRY(acu_sync_only(ctx));  // refused whatever the input, before any device work (also for floats and empty inputs)
   return checked_fold<true>(ctx, dtype, a, out_bits, out_valid_count);
 }

@@ -10,7 +10,7 @@ import pytest
 
 import acu
 from acu import _abi as abi
-from acu import BOOL, ArrowError, HostArray, ViewColumn, bitmap_bytes
+from acu import BOOL, ArrowError, FixedSizeBinaryColumn, HostArray, ViewColumn, bitmap_bytes
 
 from test_gpu_parity import assert_same, rand_array, rand_bool
 from test_oracle_cmp_bytes import rand_strings, utf8_column
@@ -188,3 +188,82 @@ def test_comparison_brackets_in_section(gpu):
     assert_same(gpu.download_out(out, BOOL), expected, "acu_cmp queued in a section")
     dx.free()
     dy.free()
+
+
+def test_byte_entry_points_refuse_in_section(gpu):
+    """Every Utf8 / Binary / view entry point synchronises, so inside a section it refuses before any argument check or
+    device work, with the one message, and leaves its output descriptor untouched; after the fetch the same calls run
+    as usual. cmp_view == against a non-null scalar of <= 4 bytes (eq_inline_scalar) and like with a scalar pattern
+    read a device value on the host before they launch."""
+    lib, h = gpu.lib, gpu.h
+    rng = np.random.default_rng(9)
+    n = 300
+    sa, sb = utf8_column(rand_strings(rng, n, 0.1)), utf8_column(rand_strings(rng, n, 0.2))
+    va, vb = ViewColumn.from_values(rand_strings(rng, n, 0.1)), ViewColumn.from_values(rand_strings(rng, n, 0.2))
+    s_pat, v_pat = utf8_column([b"pre%"], scalar=True), ViewColumn.from_values([b"pre%"], scalar=True)
+    v_abc = ViewColumn.from_values([b"abc"], scalar=True)
+    fsb = FixedSizeBinaryColumn.from_values([bytes(rng.integers(0, 256, 5, dtype=np.uint8)) for _ in range(n)], 5)
+    boo = rand_bool(rng, n, 0.5, 0.1, 0)
+    expected = {"cmp_bytes": gpu.cmp_bytes(acu.LT_EQ, sa, sb), "cmp_view": gpu.cmp_view(acu.LT_EQ, va, vb),
+                "cmp_view_eq_inline": gpu.cmp_view(acu.EQ, va, v_abc), "like_bytes": gpu.like_bytes(abi.LIKE, sa, s_pat),
+                "like_view": gpu.like_view(abi.LIKE, va, v_pat)}
+    expected_agg = {"aggregate_bytes": gpu.min_max_row(acu.MIN, sa), "aggregate_byte_view": gpu.min_max_row(acu.MAX, va),
+                    "aggregate_fixed_size_binary": gpu.min_max_row(acu.MIN, fsb), "aggregate_boolean": gpu.aggregate_boolean(acu.MAX, boo)}
+    owned, keep = [], []
+    d_sa, d_sb, d_spat = (gpu._upload_bytes_col(c, owned) for c in (sa, sb, s_pat))
+    d_va, d_vb, d_vpat, d_vabc = (gpu._upload_view_col(c, owned, keep) for c in (va, vb, v_pat, v_abc))
+    d_fsb = gpu._upload_fsb(fsb, owned)
+    d_boo = gpu.upload(boo)
+    dbd = d_boo.descriptor()
+    buf = gpu.malloc(n * 16 + 64)  # offsets / views / data of the substring outputs
+    owned.append(buf)
+    total, width, row, cnt, val = C.c_int64(-7), C.c_int32(-7), C.c_int64(0), C.c_int64(0), C.c_int32(0)
+    R = C.byref
+    calls = {
+        "cmp_bytes": lambda o: lib.acu_cmp_bytes(h, 4, acu.LT_EQ, R(d_sa), R(d_sb), R(o)),
+        "cmp_view": lambda o: lib.acu_cmp_byte_view(h, acu.LT_EQ, R(d_va), R(d_vb), R(o)),
+        "cmp_view_eq_inline": lambda o: lib.acu_cmp_byte_view(h, acu.EQ, R(d_va), R(d_vabc), R(o)),
+        "like_bytes": lambda o: lib.acu_like_bytes(h, 4, 1, abi.LIKE, R(d_sa), R(d_spat), R(o)),
+        "like_view": lambda o: lib.acu_like_byte_view(h, 1, abi.LIKE, R(d_va), R(d_vpat), R(o)),
+        "length_bytes": lambda o: lib.acu_length_bytes(h, 4, abi.LENGTH, R(d_sa), R(o)),
+        "length_byte_view": lambda o: lib.acu_length_byte_view(h, abi.LENGTH, R(d_va), R(o)),
+        "length_fixed_size_binary": lambda o: lib.acu_length_fixed_size_binary(h, 5, abi.LENGTH, R(d_fsb), R(o)),
+        "substring_bytes": lambda o: lib.acu_substring_bytes(h, 4, 0, 1, 0, 0, R(d_sa), sa.data.nbytes, buf, None, 0, R(total), R(o)),
+        "substring_by_char": lambda o: lib.acu_substring_by_char(h, 4, 1, 0, 0, R(d_sa), buf, None, 0, R(total), R(o)),
+        "substring_byte_view": lambda o: lib.acu_substring_byte_view(h, 0, 1, 0, 0, R(d_va), buf, R(o)),
+        "substring_fixed_size_binary": lambda o: lib.acu_substring_fixed_size_binary(h, 5, 1, 0, 0, R(d_fsb), R(width), R(o)),
+        "aggregate_bytes": lambda o: lib.acu_aggregate_bytes(h, 4, acu.MIN, R(d_sa), R(row), R(cnt)),
+        "aggregate_byte_view": lambda o: lib.acu_aggregate_byte_view(h, acu.MAX, R(d_va), R(row), R(cnt)),
+        "aggregate_fixed_size_binary": lambda o: lib.acu_aggregate_fixed_size_binary(h, 5, acu.MIN, R(d_fsb), R(row), R(cnt)),
+        "aggregate_boolean": lambda o: lib.acu_aggregate_boolean(h, acu.MAX, R(dbd), R(val), R(cnt)),
+    }
+    outs = {name: gpu.alloc_out(n * 8 + 16, n) for name in calls}
+    try:
+        gpu.async_begin()
+        for name, call in calls.items():
+            o = outs[name]
+            o.len, o.null_count, o.has_validity = -7, -7, 7
+            assert call(o) == abi.ERR_INVALID_ARGUMENT, name
+            msg = lib.acu_last_error(h).contents.message
+            assert msg == b"Invalid argument error: this entry point synchronises and is not available between acu_async_begin and acu_results_fetch", name
+            assert (o.len, o.null_count, o.has_validity) == (-7, -7, 7), name
+        assert (total.value, width.value) == (-7, -7)
+        gpu.results_fetch()
+        for name, call in calls.items():
+            gpu.check(call(outs[name]))
+            if name in expected:
+                got, outs[name] = gpu.download_out(outs[name], BOOL), None  # download_out frees the buffers
+                assert_same(got, expected[name], name + " after the section")
+            elif name == "aggregate_boolean":
+                assert (val.value, cnt.value) == expected_agg[name], name
+            elif name in expected_agg:
+                assert (row.value, cnt.value) == expected_agg[name], name
+            else:
+                assert outs[name].len == n, name
+    finally:
+        for o in outs.values():
+            if o is not None:
+                gpu._free_out(o)
+        d_boo.free()
+        for p in owned:
+            gpu.free(p)
