@@ -5,13 +5,21 @@
 //                (arrow-cast/src/cast/dictionary.rs:310-317)
 //   filter_bytes (arrow-select/src/filter.rs:893-928)
 //
-// Design: lengths -> device-wide inclusive scan -> byte copy.
+// Both are a gather of source rows (filter gathers the plan's selected rows):
 //   1. nulls first (take_nulls / filter_nulls), exactly like the reference;
 //   2. len[j] = offsets[idx+1]-offsets[idx] for valid output slots, 0 for null slots
 //      (take.rs:556-583; filter copies null slots too, filter.rs:891-892);
-//   3. three-level decoupled scan over int64 lengths (4096 elements per CTA) gives the new
-//      offsets; i32 overflow reports the first running total above i32::MAX (take.rs:520-523);
-//   4. copy: one warp per 32 rows, each lane streams its row's bytes.
+//   3. pass 1 sums the bytes of every 2048-row block, and a device-wide inclusive scan of the
+//      block totals gives each block its first output byte;
+//   4. pass 2 writes the new offsets (an i32 overflow reports the first row whose end passes
+//      i32::MAX, take.rs:520-523) and copies the bytes. It runs one of three kernels:
+//      k_dict_copy           i32 offsets, 32-bit indices with a 16-byte aligned base, a source of
+//                            1 .. 8192 rows none longer than 16 bytes, and at least 65536 output
+//                            rows: the source is kept in shared memory;
+//      k_gather_copy         any other source with i32 offsets and 32-bit indices with a 16-byte
+//                            aligned base;
+//      k_bytes_offsets_copy  everything else: i64 offsets, 8-, 16- or 64-bit indices, or an
+//                            index base that is not 16-byte aligned (bytes_engine.cuh).
 #include <stdio.h>
 #include <stdlib.h>
 
@@ -26,13 +34,7 @@
 
 namespace {
 
-template <int IT> struct IdxRaw;
-template <> struct IdxRaw<0> { using t = uint8_t; };
-template <> struct IdxRaw<1> { using t = int8_t; };
-template <> struct IdxRaw<2> { using t = uint16_t; };
-template <> struct IdxRaw<3> { using t = int16_t; };
-template <> struct IdxRaw<4> { using t = uint32_t; };
-template <> struct IdxRaw<5> { using t = uint64_t; };
+// kind: acu_take_index_kind of the index type
 __device__ __forceinline__ uint64_t ld_index(const void *idx, int kind, int64_t j) {
   switch (kind) {
     case 0: return __ldg(static_cast<const uint8_t *>(idx) + j);
@@ -46,33 +48,15 @@ __device__ __forceinline__ uint64_t ld_index(const void *idx, int kind, int64_t 
 
 // ---- device-wide inclusive scan of int64 (in place) ------------------------------------
 __global__ void __launch_bounds__(1024) k_scan_block(int64_t *__restrict__ data, int64_t n, int64_t *__restrict__ block_tot) {
-  __shared__ int64_t warp_tot[32];
+  __shared__ uint64_t warp_tot[33];
   const int64_t base = (int64_t)blockIdx.x * SCAN_ELEMS + (int64_t)threadIdx.x * 4;
   int64_t c[4];
 #pragma unroll
   for (int k = 0; k < 4; ++k) c[k] = (base + k < n) ? data[base + k] : 0;
   c[1] += c[0]; c[2] += c[1]; c[3] += c[2];
-  int64_t incl = c[3];
-  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) {
-    int64_t y = __shfl_up_sync(ACU_FULL_MASK, incl, o);
-    if (lane >= o) incl += y;
-  }
-  if (lane == 31) warp_tot[wid] = incl;
-  __syncthreads();
-  if (wid == 0) {
-    int64_t w = warp_tot[lane], wi = w;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      int64_t y = __shfl_up_sync(ACU_FULL_MASK, wi, o);
-      if (lane >= o) wi += y;
-    }
-    warp_tot[lane] = wi - w;
-    if (lane == 31 && block_tot) block_tot[blockIdx.x] = wi;
-  }
-  __syncthreads();
-  const int64_t excl = warp_tot[wid] + incl - c[3];
+  uint64_t total;
+  const int64_t excl = (int64_t)cta_scan_excl((uint64_t)c[3], warp_tot, &total);
+  if (threadIdx.x == 0 && block_tot) block_tot[blockIdx.x] = (int64_t)total;
 #pragma unroll
   for (int k = 0; k < 4; ++k)
     if (base + k < n) data[base + k] = excl + c[k];
@@ -126,20 +110,12 @@ __global__ void __launch_bounds__(256) k_plan_indices(const uint64_t *__restrict
   }
 }
 
-int index_kind(acu_dtype t) {
-  switch (t) {
-    case ACU_U8: return 0; case ACU_I8: return 1; case ACU_U16: return 2; case ACU_I16: return 3;
-    case ACU_U32: case ACU_I32: return 4; case ACU_U64: case ACU_I64: return 5;
-    default: return -1;
-  }
-}
-
 // ---- fused lengths / scan / offsets / copy -------------------------------------------------
 // CTA = BY_THREADS threads x 4 CONSECUTIVE rows (BY_ROWS rows): a thread's four indices are
-// one 128-bit load, its four new offsets one 128-bit store, its four validity bits a nibble of
-// one u32, and the CTA-wide scan runs once over per-thread sums (two barriers) instead of once
-// per row round. All eight source-offset loads of a thread are issued before any is used.
-// FAST = i32 offsets + 32-bit indices with 16-B aligned index / offset buffers.
+// one 128-bit load (FAST), its four validity bits a nibble of one u32, and the CTA-wide scan
+// runs once over per-thread sums (two barriers) instead of once per row round. All eight
+// source-offset loads of a thread are issued before any is used.
+// FAST = i32 offsets + 32-bit indices with a 16-B aligned index buffer.
 struct BytesArgs {
   const void *offs;        // source offsets (i32 or i64)
   const uint8_t *data;     // source value bytes
@@ -227,7 +203,6 @@ __device__ __forceinline__ void rows4(const BytesArgs &a, int64_t j0, int64_t be
 // The take / filter producer of bytes_engine.cuh.
 template <bool FAST>
 struct GatherRows : BytesArgs {
-  static constexpr bool kVec4 = FAST;
   __device__ __forceinline__ void ranges4(int64_t j0, int64_t begin[4], uint64_t len[4], unsigned long long *err) const {
     rows4<FAST>(*this, j0, begin, len, err);
   }
@@ -242,20 +217,130 @@ struct GatherRows : BytesArgs {
 // LDS.128 / LDS.U8.
 //   pass 1 (k_dict_block_totals): a WARP owns a 2048-row block — 16 x (one 128-bit load of 4 keys per lane, 4 LDS.U8),
 //     one redux.sync, no CTA barrier.
-//   pass 2 (k_dict_copy): a CTA owns a 2048-row block (16 warps x 4 x 32 rows, lane == row % 32 so that the 32 rows of
-//     an instruction land ~8 bytes apart: ~2-way bank conflicts). The four 32-row scans of a warp are two packed 16-bit
-//     scans; a row's bytes reach their position in a zeroed 32-KB shared-memory IMAGE of the CTA's output (which mirrors
-//     the output's 16-byte alignment) by funnel shifts + predicated ATOMS.OR; the image leaves as coalesced 128-bit stores
-//     (only the first / last chunk of a CTA, shared with its neighbours, is written bytewise) and is re-zeroed on the way.
-//     All positions inside a round are 32-bit. The first version of this path (warp-private rings, 64-bit positions,
-//     bytewise head / tail per warp) was issue-bound.
+//   pass 2 (k_dict_copy): a CTA owns a 2048-row block per round (see the round skeleton below), lane == row % 32 so that
+//     the 32 rows of an instruction land ~8 bytes apart: ~2-way bank conflicts. A row's bytes reach their position in the
+//     round's image by funnel shifts + predicated ATOMS.OR. All positions inside a round are 32-bit. The first version of
+//     this path (warp-private rings, 64-bit positions, bytewise head / tail per warp) was issue-bound.
 #define DG_THREADS 512
 #define DG_WARPS (DG_THREADS / 32)
 #define DG_WROWS (BY_ROWS / DG_WARPS)   // 128 rows per warp and round
 #define DG_ITERS (DG_WROWS / 32)        // 4 x 32 rows
 #define DG_IMG_BYTES (BY_ROWS * 16 + 32)  // image of one CTA round: <= 2048 x 16 bytes + alignment slack
 #define DG_MAX_ENTRIES 8192
-static_assert(DG_ITERS == 4, "k_dict_copy packs the four 32-row scans of a warp into two registers");
+static_assert(DG_ITERS == 4, "round_place packs the four 32-row scans of a warp into two registers");
+
+// ---- the round skeleton of k_dict_copy and k_gather_copy ---------------------------------------------------------------------
+// A CTA of DG_WARPS warps owns one 2048-row block per round; a lane's rows are r0 + 32 i (r0 = warp * 128 + lane, i < 4).
+// With the rows' lengths known, the four 32-row scans of a warp run as two packed 16-bit scans (round_place), the new
+// offsets follow (round_offsets), the rows' bytes are ORed into a zeroed 32-KB shared-memory IMAGE of the round's output
+// that mirrors the output's 16-byte alignment (each kernel's own code), and the image leaves as coalesced 128-bit stores,
+// re-zeroed on the way (image_flush).
+__device__ __forceinline__ uint32_t round_rows(int64_t m, int64_t blk) {
+  const int64_t left = m - blk * BY_ROWS;
+  return left < BY_ROWS ? (uint32_t)left : (uint32_t)BY_ROWS;
+}
+
+// A lane's four 32-bit indices of round `blk` (~0 for rows past the end) and, in lanes i < 4, the validity word of the
+// warp's i-th 32-row group (all ones without a bitmap, 0 past the end).
+__device__ __forceinline__ void round_load(const uint32_t *idx, const uint32_t *out_valid, int64_t m, int64_t blk, uint32_t ix[DG_ITERS], uint32_t &vw) {
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int64_t base = blk * BY_ROWS;
+  const uint32_t rows_here = round_rows(m, blk);
+  const uint32_t r0 = wid * DG_WROWS + lane;
+  const uint32_t *ip = idx + base + r0;
+#pragma unroll
+  for (int i = 0; i < DG_ITERS; ++i) ix[i] = (r0 + i * 32 < rows_here) ? __ldg(ip + i * 32) : 0xffffffffu;
+  vw = 0xffffffffu;
+  if (out_valid) vw = (lane < DG_ITERS && wid * DG_WROWS + lane * 32 < rows_here) ? __ldg(out_valid + (base >> 5) + wid * DG_ITERS + lane) : 0u;
+}
+
+// pre[i] = the first byte of row r0 + 32 i within its warp's bytes, wbase = the bytes of the warps before this one; returns
+// the round's byte total. Every 32-row total must fit 16 bits (rows of at most 16 bytes, or a round of at most 32 KB).
+// One barrier; s_wtot holds DG_WARPS words.
+__device__ __forceinline__ uint32_t round_place(const uint32_t len[DG_ITERS], uint32_t *s_wtot, uint32_t pre[DG_ITERS], uint32_t &wbase) {
+  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const uint32_t p01 = len[0] | (len[1] << 16), p23 = len[2] | (len[3] << 16);
+  uint32_t i01 = p01, i23 = p23;
+#pragma unroll
+  for (int o = 1; o < 32; o <<= 1) {
+    const uint32_t y01 = __shfl_up_sync(ACU_FULL_MASK, i01, o), y23 = __shfl_up_sync(ACU_FULL_MASK, i23, o);
+    if (lane >= (uint32_t)o) { i01 += y01; i23 += y23; }
+  }
+  const uint32_t t01 = __shfl_sync(ACU_FULL_MASK, i01, 31), t23 = __shfl_sync(ACU_FULL_MASK, i23, 31);
+  const uint32_t e01 = i01 - p01, e23 = i23 - p23;  // exclusive (no borrow between the fields: each inclusive field >= its own term)
+  const uint32_t tot0 = t01 & 0xffffu, tot1 = t01 >> 16, tot2 = t23 & 0xffffu;
+  pre[0] = e01 & 0xffffu;
+  pre[1] = tot0 + (e01 >> 16);
+  pre[2] = tot0 + tot1 + (e23 & 0xffffu);
+  pre[3] = tot0 + tot1 + tot2 + (e23 >> 16);
+  if (lane == 0) s_wtot[wid] = tot0 + tot1 + tot2 + (t23 >> 16);
+  __syncthreads();
+  const uint32_t wv = lane < DG_WARPS ? s_wtot[lane] : 0u;
+  wbase = __reduce_add_sync(ACU_FULL_MASK, lane < wid ? wv : 0u);
+  return __reduce_add_sync(ACU_FULL_MASK, wv);
+}
+
+// The new offsets of a round's rows (32-bit wrapping arithmetic on the truncated base: an overflow is reported, not stored),
+// the lowest row whose end passes `limit` into err (take.rs:521 "offset overflow"), and offsets[m] from the lane holding
+// the last row.
+__device__ __forceinline__ void round_offsets(int32_t *out_offs, int64_t m, int64_t base, uint32_t r0, uint32_t rows_here, int64_t cta_begin,
+                                              uint32_t T, uint32_t wbase, const uint32_t pre[DG_ITERS], const uint32_t len[DG_ITERS], int64_t limit,
+                                              unsigned long long &err) {
+  const uint32_t o32 = (uint32_t)cta_begin + wbase;
+  uint32_t *op = reinterpret_cast<uint32_t *>(out_offs) + base + r0;
+#pragma unroll
+  for (int i = 0; i < DG_ITERS; ++i)
+    if (r0 + i * 32 < rows_here) op[i * 32] = o32 + pre[i];
+  if (cta_begin + T > limit) {
+    const int64_t o0 = cta_begin + wbase;
+#pragma unroll
+    for (int i = 0; i < DG_ITERS; ++i)
+      if (r0 + i * 32 < rows_here && o0 + pre[i] + len[i] > limit && (unsigned long long)(base + r0 + i * 32) < err)
+        err = (unsigned long long)(base + r0 + i * 32);
+  }
+  if (base + rows_here == m) {
+#pragma unroll
+    for (int i = 0; i < DG_ITERS; ++i)
+      if (r0 + i * 32 + 1 == rows_here) reinterpret_cast<uint32_t *>(out_offs)[m] = o32 + pre[i] + len[i];
+  }
+}
+
+// OR `x` into the shared-memory word at byte address `saddr + OFF` (RED: no return value)
+template <int OFF>
+__device__ __forceinline__ void red_or(uint32_t saddr, uint32_t x) {
+  asm volatile("red.shared.or.b32 [%0+%2], %1;" ::"r"(saddr), "r"(x), "n"(OFF) : "memory");
+}
+
+// After a barrier (every row is in the image): the round's T bytes, image bytes A .. A + T (A = the output's misalignment
+// at cta_begin), to out_data + cta_begin. The first / last chunk is shared with the neighbouring rounds' bytes: it is
+// written by whole words, then single bytes. Every chunk read is zeroed again.
+__device__ __forceinline__ void image_flush(uint4 *img4, uint8_t *out_data, int64_t cta_begin, uint32_t A, uint32_t T) {
+  __syncthreads();
+  const uint32_t end = A + T;
+  const uint32_t chunks = (end + 15u) >> 4;
+  const uint32_t first_full = (A + 15u) >> 4, n_full = (end >> 4) > first_full ? (end >> 4) - first_full : 0u;
+  uint8_t *gb = out_data + cta_begin - A;  // 16-byte aligned
+  for (uint32_t c = threadIdx.x; c < chunks; c += DG_THREADS) {
+    const uint4 q = img4[c];
+    img4[c] = make_uint4(0, 0, 0, 0);
+    if (c - first_full < n_full) {
+      reinterpret_cast<uint4 *>(gb)[c] = q;
+    } else {
+      const uint32_t qw[4] = {q.x, q.y, q.z, q.w};
+#pragma unroll
+      for (uint32_t w4 = 0; w4 < 4; ++w4) {
+        const uint32_t lo = (c << 4) + 4u * w4;
+        if (lo >= A && lo + 4u <= end) {
+          *reinterpret_cast<uint32_t *>(gb + lo) = qw[w4];
+        } else {
+#pragma unroll
+          for (uint32_t b = 0; b < 4; ++b)
+            if (lo + b >= A && lo + b < end) gb[lo + b] = (uint8_t)(qw[w4] >> (8u * b));
+        }
+      }
+    }
+  }
+}
 
 __global__ void __launch_bounds__(256) k_dict_table(const int32_t *__restrict__ offs, const uint8_t *__restrict__ data, int64_t n_src,
                                                     uint4 *__restrict__ table, uint8_t *__restrict__ lens, int *__restrict__ too_long) {
@@ -348,12 +433,6 @@ __global__ void __launch_bounds__(DG_THREADS) k_dict_block_totals(const DictArgs
   if (a.detect_oob && err != ~0ull) atomicMin(res + RES_ERR_INDEX, err);
 }
 
-// OR `x` into the shared-memory word at byte address `saddr + OFF` (RED: no return value)
-template <int OFF>
-__device__ __forceinline__ void red_or(uint32_t saddr, uint32_t x) {
-  asm volatile("red.shared.or.b32 [%0+%2], %1;" ::"r"(saddr), "r"(x), "n"(OFF) : "memory");
-}
-
 // pass 2: new offsets + bytes. A CTA round is a dependent chain (keys -> lengths -> scan -> barrier -> image -> barrier ->
 // flush -> barrier) with only two CTAs per SM, so the NEXT round's keys, validity words and base offset are loaded at the
 // top of the current round (software prefetch): without it every round exposes a full DRAM latency.
@@ -365,17 +444,9 @@ struct DictRound {
 };
 
 __device__ __forceinline__ void dict_round_load(const DictArgs &a, const int64_t *__restrict__ block_incl, int64_t blk, DictRound &r) {
-  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t base = blk * BY_ROWS;
-  const int64_t left = a.m - base;
-  r.rows_here = left < BY_ROWS ? (uint32_t)left : (uint32_t)BY_ROWS;
+  r.rows_here = round_rows(a.m, blk);
   r.cta_begin = blk ? __ldg(block_incl + blk - 1) : 0;
-  const uint32_t r0 = wid * DG_WROWS + lane;
-  const uint32_t *kp = a.keys + base + r0;
-#pragma unroll
-  for (int i = 0; i < DG_ITERS; ++i) r.key[i] = (r0 + i * 32 < r.rows_here) ? __ldg(kp + i * 32) : 0xffffffffu;
-  r.vw = 0xffffffffu;
-  if (a.out_valid) r.vw = (lane < DG_ITERS && wid * DG_WROWS + lane * 32 < r.rows_here) ? __ldg(a.out_valid + (base >> 5) + wid * DG_ITERS + lane) : 0u;
+  round_load(a.keys, a.out_valid, a.m, blk, r.key, r.vw);
 }
 
 __global__ void __launch_bounds__(DG_THREADS, 2) k_dict_copy(const DictArgs a, const int64_t *__restrict__ block_incl, int64_t blocks,
@@ -384,10 +455,7 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_dict_copy(const DictArgs a, c
   extern __shared__ __align__(16) uint8_t s_dyn[];
   __shared__ uint32_t s_wtot[DG_WARPS];
   if (*a.too_long) return;
-  if (out_data != nullptr && total_ptr != nullptr) {  // decided on the device: no host round trip between the passes
-    const int64_t total = __ldg(total_ptr);
-    if (total > out_cap || total > limit) out_data = nullptr;
-  }
+  skip_copy_if_too_large(out_data, total_ptr, out_cap, limit);
   const uint32_t n_src = a.n_src;  // the shared-memory table has n_src + 1 entries: the last one is the empty string
   uint4 *s_tab = reinterpret_cast<uint4 *>(s_dyn);
   uint8_t *s_len = s_dyn + ((size_t)n_src + 1) * 16;
@@ -401,7 +469,6 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_dict_copy(const DictArgs a, c
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint32_t r0 = wid * DG_WROWS + lane;  // this lane's rows of a round: r0 + 32 i
   const uint32_t img = (uint32_t)__cvta_generic_to_shared(s_img);
-  uint4 *img4 = reinterpret_cast<uint4 *>(s_img);
   unsigned long long err = ~0ull;
   for (int64_t blk = blockIdx.x; blk < blocks; blk += gridDim.x) {
     const int64_t base = blk * BY_ROWS;
@@ -416,49 +483,12 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_dict_copy(const DictArgs a, c
       len[i] = s_len[key[i]];
     }
     if (blk + gridDim.x < blocks) dict_round_load(a, block_incl, blk + gridDim.x, cur);  // in flight during this round
-    // four inclusive 32-row scans as two packed 16-bit scans (a 32-row total is <= 512)
-    const uint32_t p01 = len[0] | (len[1] << 16), p23 = len[2] | (len[3] << 16);
-    uint32_t i01 = p01, i23 = p23;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) {
-      const uint32_t y01 = __shfl_up_sync(ACU_FULL_MASK, i01, o), y23 = __shfl_up_sync(ACU_FULL_MASK, i23, o);
-      if (lane >= (uint32_t)o) { i01 += y01; i23 += y23; }
-    }
-    const uint32_t t01 = __shfl_sync(ACU_FULL_MASK, i01, 31), t23 = __shfl_sync(ACU_FULL_MASK, i23, 31);
-    const uint32_t e01 = i01 - p01, e23 = i23 - p23;  // exclusive (no borrow between the fields: each inclusive field >= its own term)
-    const uint32_t tot0 = t01 & 0xffffu, tot1 = t01 >> 16, tot2 = t23 & 0xffffu;
-    uint32_t pre[DG_ITERS];
-    pre[0] = e01 & 0xffffu;
-    pre[1] = tot0 + (e01 >> 16);
-    pre[2] = tot0 + tot1 + (e23 & 0xffffu);
-    pre[3] = tot0 + tot1 + tot2 + (e23 >> 16);
-    const uint32_t run = tot0 + tot1 + tot2 + (t23 >> 16);
-    if (lane == 0) s_wtot[wid] = run;
-    __syncthreads();
-    const uint32_t wv = lane < DG_WARPS ? s_wtot[lane] : 0u;
-    const uint32_t T = __reduce_add_sync(ACU_FULL_MASK, wv);                      // bytes of this CTA round
-    const uint32_t wbase = __reduce_add_sync(ACU_FULL_MASK, lane < wid ? wv : 0u);  // bytes of the warps before this one
-    // ---- new offsets (32-bit wrapping arithmetic on the truncated base: an overflow is reported, not stored) ----
-    const uint32_t o32 = (uint32_t)cta_begin + wbase;
-    uint32_t *op = reinterpret_cast<uint32_t *>(out_offs) + base + r0;
-#pragma unroll
-    for (int i = 0; i < DG_ITERS; ++i)
-      if (r0 + i * 32 < rows_here) op[i * 32] = o32 + pre[i];
-    if (cta_begin + T > limit) {  // the first row whose end passes the offset type (take.rs:521 "offset overflow")
-      const int64_t o0 = cta_begin + wbase;
-#pragma unroll
-      for (int i = 0; i < DG_ITERS; ++i)
-        if (r0 + i * 32 < rows_here && o0 + pre[i] + len[i] > limit && (unsigned long long)(base + r0 + i * 32) < err)
-          err = (unsigned long long)(base + r0 + i * 32);
-    }
-    if (base + rows_here == a.m) {  // the last block: the lane holding the last row also writes offsets[m]
-#pragma unroll
-      for (int i = 0; i < DG_ITERS; ++i)
-        if (r0 + i * 32 + 1 == rows_here) reinterpret_cast<uint32_t *>(out_offs)[a.m] = o32 + pre[i] + len[i];
-    }
+    uint32_t pre[DG_ITERS], wbase;
+    const uint32_t T = round_place(len, s_wtot, pre, wbase);
+    round_offsets(out_offs, a.m, base, r0, rows_here, cta_begin, T, wbase, pre, len, limit, err);
     // ---- bytes: rows -> image (predicated RED.OR), image -> global (128-bit stores) ----
     if (out_data != nullptr) {
-      const uint32_t A = (uint32_t)((uintptr_t)(out_data + cta_begin) & 15);  // the image mirrors the output's 16-byte alignment
+      const uint32_t A = (uint32_t)((uintptr_t)(out_data + cta_begin) & 15);
 #pragma unroll
       for (int i = 0; i < DG_ITERS; ++i) {
         const uint4 e = s_tab[key[i]];  // zero beyond the entry's length
@@ -475,65 +505,21 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_dict_copy(const DictArgs a, c
         const uint32_t x4 = __funnelshift_l(e.w, 0u, dsh);
         if (__any_sync(ACU_FULL_MASK, x4 != 0u)) red_or<16>(w, x4);
       }
-      __syncthreads();
-      const uint32_t end = A + T;
-      const uint32_t chunks = (end + 15u) >> 4;
-      const uint32_t first_full = (A + 15u) >> 4, n_full = (end >> 4) > first_full ? (end >> 4) - first_full : 0u;
-      uint8_t *gb = out_data + cta_begin - A;  // 16-byte aligned
-      for (uint32_t c = threadIdx.x; c < chunks; c += DG_THREADS) {
-        const uint4 q = img4[c];
-        img4[c] = make_uint4(0, 0, 0, 0);
-        if (c - first_full < n_full) {
-          reinterpret_cast<uint4 *>(gb)[c] = q;
-        } else {  // first / last chunk of the round (shared with the neighbouring CTAs' bytes): whole words, then single bytes
-          const uint32_t qw[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-          for (uint32_t w4 = 0; w4 < 4; ++w4) {
-            const uint32_t lo = (c << 4) + 4u * w4;
-            if (lo >= A && lo + 4u <= end) {
-              *reinterpret_cast<uint32_t *>(gb + lo) = qw[w4];
-            } else {
-#pragma unroll
-              for (uint32_t b = 0; b < 4; ++b)
-                if (lo + b >= A && lo + b < end) gb[lo + b] = (uint8_t)(qw[w4] >> (8u * b));
-            }
-          }
-        }
-      }
+      image_flush(reinterpret_cast<uint4 *>(s_img), out_data, cta_begin, A, T);
     }
     __syncthreads();  // the image is zero again, s_wtot can be rewritten
   }
   if (err != ~0ull) atomicMin(res + RES_ERR2, err);
 }
 
-// ---- generic gather, FAST case (i32 offsets, 32-bit indices), round 2 ------------------------------------------------------
-// The dictionary kernel's recipe applied to an arbitrary source: lane = row mod 32 (16 warps x 4 x 32 rows per 2048-row CTA
-// round), packed 16-bit scans, 32-bit positions, a zeroed 32-KB shared-memory image of the round's output filled by funnel
-// shifts + RED.OR and written back as 128-bit stores. What differs is where a row's bytes come from — two scattered offset
-// loads, then up to 16 bytes by three predicated aligned 8-byte loads (rows longer than 16 bytes loop in 16-byte pieces) —
-// and that those loads are software-pipelined over THREE rounds (indices of round r + 2, offsets of round r + 1, bytes of
-// round r in flight together), because a round is one dependent chain of three DRAM round trips. A block whose bytes do
-// not fit the image (T > 32 KB, i.e. rows averaging more than 16 bytes) takes a slow direct-copy path in the same kernel.
+// ---- generic gather, FAST case (i32 offsets, 32-bit indices) -------------------------------------------------------------
+// The round skeleton applied to an arbitrary source. Where a row's bytes come from differs from the dictionary kernel —
+// two scattered offset loads, then up to 16 bytes by three predicated aligned 8-byte loads (rows longer than 16 bytes loop
+// in 8-byte pieces) — and those loads are software-pipelined over THREE rounds (indices of round r + 2, offsets of round
+// r + 1, bytes of round r in flight together), because a round is one dependent chain of three DRAM round trips. A block
+// whose bytes do not fit the image (T > 32 KB, i.e. rows averaging more than 16 bytes) takes a slow direct-copy path in the
+// same kernel.
 #define GC_IMG_BYTES (BY_ROWS * 16)
-
-__device__ __forceinline__ uint32_t gather_rows_here(const BytesArgs &a, int64_t blk) {
-  const int64_t left = a.m - blk * BY_ROWS;
-  return left < BY_ROWS ? (uint32_t)left : (uint32_t)BY_ROWS;
-}
-
-// stage 1 (two rounds ahead): this lane's four indices + the validity words of the warp's four 32-row groups (lane i < 4;
-// all ones without a bitmap, 0 past the end)
-__device__ __forceinline__ void gather_load_idx(const BytesArgs &a, int64_t blk, uint32_t idx[DG_ITERS], uint32_t &vw) {
-  const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int64_t base = blk * BY_ROWS;
-  const uint32_t rows_here = gather_rows_here(a, blk);
-  const uint32_t r0 = wid * DG_WROWS + lane;
-  const uint32_t *ip = static_cast<const uint32_t *>(a.idx) + base + r0;
-#pragma unroll
-  for (int i = 0; i < DG_ITERS; ++i) idx[i] = (r0 + i * 32 < rows_here) ? __ldg(ip + i * 32) : 0u;
-  vw = 0xffffffffu;
-  if (a.out_valid) vw = (lane < DG_ITERS && wid * DG_WROWS + lane * 32 < rows_here) ? __ldg(a.out_valid + (base >> 5) + wid * DG_ITERS + lane) : 0u;
-}
 
 // stage 2 (one round ahead): source byte range of this lane's four rows (0 / 0 for rows past the end, null slots and
 // out-of-bounds indices) + the block's first output byte and its byte count (saturated to 32 bits)
@@ -541,7 +527,7 @@ __device__ __forceinline__ void gather_load_offsets(const BytesArgs &a, const in
                                                     uint32_t vw_lanes, int32_t s[DG_ITERS], int32_t e[DG_ITERS], int64_t &cta_begin, uint32_t &T32) {
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint32_t r0 = wid * DG_WROWS + lane;
-  const uint32_t rows_here = gather_rows_here(a, blk);
+  const uint32_t rows_here = round_rows(a.m, blk);
   const bool all_in = a.n_src > (int64_t)0xffffffffll;
   const uint32_t n32 = all_in ? 0xffffffffu : (uint32_t)a.n_src;
   const int32_t *offs = static_cast<const int32_t *>(a.offs);
@@ -567,16 +553,14 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_gather_copy(const BytesArgs a
   extern __shared__ __align__(16) uint8_t s_dyn[];
   __shared__ uint32_t s_wtot[DG_WARPS];
   __shared__ unsigned long long s_wtot64[DG_WARPS];
-  if (out_data != nullptr && total_ptr != nullptr) {  // decided on the device: no host round trip between the passes
-    const int64_t total = __ldg(total_ptr);
-    if (total > out_cap || total > limit) out_data = nullptr;
-  }
+  skip_copy_if_too_large(out_data, total_ptr, out_cap, limit);
   uint32_t *s_img = reinterpret_cast<uint32_t *>(s_dyn);
   uint4 *img4 = reinterpret_cast<uint4 *>(s_dyn);
   for (uint32_t i = threadIdx.x; i < (GC_IMG_BYTES + 32) / 16; i += DG_THREADS) img4[i] = make_uint4(0, 0, 0, 0);
   const uint32_t lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const uint32_t r0 = wid * DG_WROWS + lane;
   const uint32_t img = (uint32_t)__cvta_generic_to_shared(s_img);
+  const uint32_t *idx = static_cast<const uint32_t *>(a.idx);
   const uint8_t *__restrict__ data = a.data;
   unsigned long long err = ~0ull;
   // pipeline state: (s, e, first output byte, byte count) of the current round, (indices, validity words) of the next one
@@ -587,14 +571,14 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_gather_copy(const BytesArgs a
   int64_t blk = blockIdx.x;
   if (blk < blocks) {
     uint32_t idx0[DG_ITERS], vw0;
-    gather_load_idx(a, blk, idx0, vw0);
+    round_load(idx, a.out_valid, a.m, blk, idx0, vw0);
     gather_load_offsets(a, block_incl, blk, idx0, vw0, s, e, begin_c, T_c);
-    if (blk + stride < blocks) gather_load_idx(a, blk + stride, idx_n, vw_n);
+    if (blk + stride < blocks) round_load(idx, a.out_valid, a.m, blk + stride, idx_n, vw_n);
   }
   __syncthreads();
   for (; blk < blocks; blk += stride) {
     const int64_t base = blk * BY_ROWS;
-    const uint32_t rows_here = gather_rows_here(a, blk);
+    const uint32_t rows_here = round_rows(a.m, blk);
     const int64_t cta_begin = begin_c;
     const uint32_t Tblk = T_c;
     uint32_t len[DG_ITERS];
@@ -607,7 +591,7 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_gather_copy(const BytesArgs a
     // next round's offsets (its indices arrived during the previous round) and the round after's indices
     if (blk + stride < blocks) {
       gather_load_offsets(a, block_incl, blk + stride, idx_n, vw_n, s, e, begin_c, T_c);
-      if (blk + 2 * stride < blocks) gather_load_idx(a, blk + 2 * stride, idx_n, vw_n);
+      if (blk + 2 * stride < blocks) round_load(idx, a.out_valid, a.m, blk + 2 * stride, idx_n, vw_n);
     }
     if (Tblk <= (uint32_t)GC_IMG_BYTES) {
       // ---- the first 16 bytes of every row: three predicated aligned 8-byte loads each, all issued before the scan ----
@@ -626,45 +610,9 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_gather_copy(const BytesArgs a
           w[i][2] = bits > 128u ? __ldg(p + 2) : 0ull;
         }
       }
-      // four inclusive 32-row scans as two packed 16-bit scans (T <= 32 KB: every partial sum fits 16 bits)
-      const uint32_t p01 = len[0] | (len[1] << 16), p23 = len[2] | (len[3] << 16);
-      uint32_t i01 = p01, i23 = p23;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) {
-        const uint32_t y01 = __shfl_up_sync(ACU_FULL_MASK, i01, o), y23 = __shfl_up_sync(ACU_FULL_MASK, i23, o);
-        if (lane >= (uint32_t)o) { i01 += y01; i23 += y23; }
-      }
-      const uint32_t t01 = __shfl_sync(ACU_FULL_MASK, i01, 31), t23 = __shfl_sync(ACU_FULL_MASK, i23, 31);
-      const uint32_t e01 = i01 - p01, e23 = i23 - p23;
-      const uint32_t tot0 = t01 & 0xffffu, tot1 = t01 >> 16, tot2 = t23 & 0xffffu;
-      uint32_t pre[DG_ITERS];
-      pre[0] = e01 & 0xffffu;
-      pre[1] = tot0 + (e01 >> 16);
-      pre[2] = tot0 + tot1 + (e23 & 0xffffu);
-      pre[3] = tot0 + tot1 + tot2 + (e23 >> 16);
-      if (lane == 0) s_wtot[wid] = tot0 + tot1 + tot2 + (t23 >> 16);
-      __syncthreads();
-      const uint32_t wv = lane < DG_WARPS ? s_wtot[lane] : 0u;
-      const uint32_t T = Tblk;
-      const uint32_t wbase = __reduce_add_sync(ACU_FULL_MASK, lane < wid ? wv : 0u);
-      // ---- new offsets ----
-      const uint32_t o32 = (uint32_t)cta_begin + wbase;
-      uint32_t *op = reinterpret_cast<uint32_t *>(out_offs) + base + r0;
-#pragma unroll
-      for (int i = 0; i < DG_ITERS; ++i)
-        if (r0 + i * 32 < rows_here) op[i * 32] = o32 + pre[i];
-      if (cta_begin + T > limit) {
-        const int64_t o0 = cta_begin + wbase;
-#pragma unroll
-        for (int i = 0; i < DG_ITERS; ++i)
-          if (r0 + i * 32 < rows_here && o0 + pre[i] + len[i] > limit && (unsigned long long)(base + r0 + i * 32) < err)
-            err = (unsigned long long)(base + r0 + i * 32);
-      }
-      if (base + rows_here == a.m) {
-#pragma unroll
-        for (int i = 0; i < DG_ITERS; ++i)
-          if (r0 + i * 32 + 1 == rows_here) reinterpret_cast<uint32_t *>(out_offs)[a.m] = o32 + pre[i] + len[i];
-      }
+      uint32_t pre[DG_ITERS], wbase;
+      round_place(len, s_wtot, pre, wbase);  // (the round's total is Tblk: T <= 32 KB, so every partial sum fits 16 bits)
+      round_offsets(out_offs, a.m, base, r0, rows_here, cta_begin, Tblk, wbase, pre, len, limit, err);
       if (out_data != nullptr) {
         const uint32_t A = (uint32_t)((uintptr_t)(out_data + cta_begin) & 15);
 #pragma unroll
@@ -701,31 +649,7 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_gather_copy(const BytesArgs a
             red_or<8>(w2, __funnelshift_l(vy, 0u, ds2));
           }
         }
-        __syncthreads();
-        const uint32_t end = A + T;
-        const uint32_t chunks = (end + 15u) >> 4;
-        const uint32_t first_full = (A + 15u) >> 4, n_full = (end >> 4) > first_full ? (end >> 4) - first_full : 0u;
-        uint8_t *gb = out_data + cta_begin - A;
-        for (uint32_t c = threadIdx.x; c < chunks; c += DG_THREADS) {
-          const uint4 q = img4[c];
-          img4[c] = make_uint4(0, 0, 0, 0);
-          if (c - first_full < n_full) {
-            reinterpret_cast<uint4 *>(gb)[c] = q;
-          } else {
-            const uint32_t qw[4] = {q.x, q.y, q.z, q.w};
-#pragma unroll
-            for (uint32_t w4 = 0; w4 < 4; ++w4) {
-              const uint32_t lo4 = (c << 4) + 4u * w4;
-              if (lo4 >= A && lo4 + 4u <= end) {
-                *reinterpret_cast<uint32_t *>(gb + lo4) = qw[w4];
-              } else {
-#pragma unroll
-                for (uint32_t b = 0; b < 4; ++b)
-                  if (lo4 + b >= A && lo4 + b < end) gb[lo4 + b] = (uint8_t)(qw[w4] >> (8u * b));
-              }
-            }
-          }
-        }
+        image_flush(img4, out_data, cta_begin, A, Tblk);
       }
       __syncthreads();
     } else {
@@ -754,7 +678,7 @@ __global__ void __launch_bounds__(DG_THREADS, 2) k_gather_copy(const BytesArgs a
           out_offs[base + r0 + i * 32] = (int32_t)start;
           if (start + (int64_t)len[i] > limit && (unsigned long long)(base + r0 + i * 32) < err) err = (unsigned long long)(base + r0 + i * 32);
           if (r0 + i * 32 + 1 == rows_here && base + rows_here == a.m) out_offs[a.m] = (int32_t)(start + (int64_t)len[i]);
-          if (out_data != nullptr && len[i]) copy_row_direct<false>(out_data + start, data, (int64_t)sc[i], (uint64_t)len[i]);
+          if (out_data != nullptr && len[i]) copy_row_direct(out_data + start, data, (int64_t)sc[i], (uint64_t)len[i]);
         }
       }
       __syncthreads();
@@ -774,13 +698,25 @@ size_t gather_block_bytes(int64_t m) {
 // block totals / scan scratch + the dictionary table of the small-source path (16-byte entries, length bytes, flag)
 size_t gather_scratch_bytes(int64_t m) { return gather_block_bytes(m) + (size_t)DG_MAX_ENTRIES * 17 + 256; }
 
+// Grid of a round kernel with `smem` bytes of dynamic shared memory: one CTA per 2048-row block, at most as many as are
+// resident at once (a CTA loops over blocks). The dictionary kernel's shared memory depends on the source's size.
+template <class K>
+acu_status round_grid(acu_ctx *ctx, K kernel, size_t smem, int64_t blocks, int *grid) {
+  ACU_CUDA(ctx, cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+  int per_sm = 1;
+  if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, DG_THREADS, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
+  *grid = acu_grid(ctx, blocks, per_sm);
+  return ACU_OK;
+}
+
 acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const uint8_t *data, const void *idx, int kind,
                          int64_t m, int64_t n_src, const uint8_t *out_valid, bool detect_oob, void *out_offsets,
                          uint8_t *out_data, int64_t out_cap, void *scratch, unsigned long long *res, acu_bytes_col_state *gs) {
   const int64_t blocks = (m + BY_ROWS - 1) / BY_ROWS;
   int64_t *block_tot = static_cast<int64_t *>(scratch);
   BytesArgs a{offsets, data, idx, kind, (int)ob, m, n_src, reinterpret_cast<const uint32_t *>(out_valid), detect_oob ? 1 : 0};
-  const bool fast = ob == 4 && kind == 4 && ((uintptr_t)idx % 16 == 0) && ((uintptr_t)offsets % 4 == 0);
+  // pass 1 of the fast kernels reads four indices as one 128-bit load
+  const bool fast = ob == 4 && kind == 4 && ((uintptr_t)idx % 16 == 0);
   const int64_t limit = ob == 4 ? (int64_t)INT32_MAX : INT64_MAX;
   gs->gathered = true;
   gs->ob = ob;
@@ -797,7 +733,7 @@ acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const ui
   gs->out_data = out_data;
   gs->out_cap = out_cap;
   // small source (a dictionary): table in shared memory, see k_dict_copy
-  if (fast && n_src <= DG_MAX_ENTRIES && n_src > 0 && m >= 65536 && ((uintptr_t)out_offsets % 4 == 0)) {
+  if (fast && n_src <= DG_MAX_ENTRIES && n_src > 0 && m >= 65536) {
     uint8_t *extra = static_cast<uint8_t *>(scratch) + gather_block_bytes(m);
     uint4 *table = reinterpret_cast<uint4 *>(extra);
     uint8_t *lens = extra + (size_t)DG_MAX_ENTRIES * 16;
@@ -810,10 +746,9 @@ acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const ui
     if (!too_long) {
       DictArgs da{static_cast<const uint32_t *>(idx), m, (uint32_t)n_src, reinterpret_cast<const uint32_t *>(out_valid), detect_oob ? 1 : 0, table, lens, flag};
       const size_t smem1 = (size_t)n_src, smem2 = ((size_t)n_src + 1) * 16 + (((size_t)n_src + 16) & ~(size_t)15) + DG_IMG_BYTES;
-      ACU_CUDA(ctx, cudaFuncSetAttribute(k_dict_copy, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem2));
-      int per_sm = 1;
-      if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_dict_copy, DG_THREADS, smem2) != cudaSuccess || per_sm < 1) per_sm = 1;
-      const int g1 = acu_grid(ctx, (blocks + DG_WARPS - 1) / DG_WARPS, 4), g2 = acu_grid(ctx, blocks, per_sm);
+      int g2 = 0;
+      ACU_TRY(round_grid(ctx, k_dict_copy, smem2, blocks, &g2));
+      const int g1 = acu_grid(ctx, (blocks + DG_WARPS - 1) / DG_WARPS, 4);
       ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_dict_block_totals, g1, DG_THREADS, smem1, da, blocks, block_tot, res);
       ACU_TRY(scan_inclusive(ctx, block_tot, blocks, block_tot + blocks));
       ACU_CUDA(ctx, cudaMemcpyAsync(res + RES_AUX0, block_tot + (blocks - 1), 8, cudaMemcpyDeviceToDevice, ctx->stream));
@@ -827,20 +762,15 @@ acu_status gather_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const ui
   else ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_block_totals<GatherRows<false>>, (unsigned)blocks, BY_THREADS, 0, GatherRows<false>{a}, block_tot, res);
   ACU_TRY(scan_inclusive(ctx, block_tot, blocks, block_tot + blocks));
   ACU_CUDA(ctx, cudaMemcpyAsync(res + RES_AUX0, block_tot + (blocks - 1), 8, cudaMemcpyDeviceToDevice, ctx->stream));
-  const int stage_cap = BY_STAGE_CAP;
   a.detect_oob = 0;
-  if (fast && ((uintptr_t)out_offsets % 4 == 0)) {
+  if (fast) {
     const size_t smem = GC_IMG_BYTES + 32;
-    ACU_CUDA(ctx, cudaFuncSetAttribute(k_gather_copy, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    int per_sm = 1;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_gather_copy, DG_THREADS, smem) != cudaSuccess || per_sm < 1) per_sm = 1;
-    ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_gather_copy, acu_grid(ctx, blocks, per_sm), DG_THREADS, smem, a, block_tot, blocks, static_cast<int32_t *>(out_offsets),
-                     out_data, limit, res, block_tot + (blocks - 1), out_cap);
-  } else if (fast) {
-    ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<GatherRows<true>>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
-    ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<GatherRows<true>>, (unsigned)blocks, BY_THREADS, stage_cap, GatherRows<true>{a}, block_tot, (int64_t)0, out_offsets,
-                     out_data, limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
+    int grid = 0;
+    ACU_TRY(round_grid(ctx, k_gather_copy, smem, blocks, &grid));
+    ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_gather_copy, grid, DG_THREADS, smem, a, block_tot, blocks, static_cast<int32_t *>(out_offsets), out_data, limit, res,
+                     block_tot + (blocks - 1), out_cap);
   } else {
+    const int stage_cap = BY_STAGE_CAP;
     ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<GatherRows<false>>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<GatherRows<false>>, (unsigned)blocks, BY_THREADS, stage_cap, GatherRows<false>{a}, block_tot, (int64_t)0, out_offsets,
                      out_data, limit, (int64_t)-1, res, stage_cap, block_tot + (blocks - 1), out_cap);
@@ -869,6 +799,13 @@ acu_status gather_finalize(acu_ctx *ctx, const acu_bytes_col_state &gs, const un
   if (gs.out_data && *out_len > gs.out_cap)
     return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, (uint64_t)*out_len,
                     "output data capacity %lld < required %lld", (long long)gs.out_cap, (long long)*out_len);
+  return ACU_OK;
+}
+
+// Every kernel reads and writes offsets as whole ob-byte words (ob already checked to be 4 or 8).
+acu_status offsets_aligned(acu_ctx *ctx, int32_t ob, const void *offsets, const void *out_offsets) {
+  if (((uintptr_t)offsets | (uintptr_t)out_offsets) % (uintptr_t)ob != 0)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "offsets must be %d-byte aligned", (int)ob);
   return ACU_OK;
 }
 
@@ -996,6 +933,7 @@ acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offse
                                      unsigned long long *res, acu_bytes_col_state *st) {
   *st = acu_bytes_col_state();
   ACU_TRY(acu_offset_width_check(ctx, ob));
+  ACU_TRY(offsets_aligned(ctx, ob, offsets, out_offsets));
   const int64_t m = indices->len;
   out_nulls->len = m;
   out_nulls->has_validity = 0;
@@ -1013,7 +951,7 @@ acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offse
     if (idx_nulls) ov = out_nulls->validity;
   }
   // with value nulls the take kernel of the validity gather reports an out-of-bounds index
-  return gather_launch(ctx, ob, offsets, data, indices->values, index_kind(index_dtype), m, nulls_of->len, ov, !val_nulls, out_offsets,
+  return gather_launch(ctx, ob, offsets, data, indices->values, acu_take_index_kind(index_dtype), m, nulls_of->len, ov, !val_nulls, out_offsets,
                        out_data, out_cap, scratch, res, st);
 }
 
@@ -1049,6 +987,7 @@ acu_status acu_filter_bytes_col_launch(acu_ctx *ctx, const acu_filter_plan *plan
                                        unsigned long long *res, acu_bytes_col_state *st) {
   *st = acu_bytes_col_state();
   ACU_TRY(acu_offset_width_check(ctx, ob));
+  ACU_TRY(offsets_aligned(ctx, ob, offsets, out_offsets));
   const int64_t count = acu_filter_plan_count(plan);
   if (count == 0) return zero_first_offset(ctx, out_offsets, ob);
   const void *idx;

@@ -4,7 +4,6 @@
 // the producer.
 //
 // A producer `R` is a trivially copyable struct with
-//   static constexpr bool kVec4;  // i32 offsets whose new offsets may leave as one 128-bit store per thread
 //   int ob; int64_t m;            // offset width, output rows
 //   const uint8_t *data;          // the source value bytes the ranges point into
 //   int detect_oob;               // k_bytes_block_totals: *err of the first pass goes to res[RES_ERR_INDEX] (atomicMin)
@@ -107,25 +106,6 @@ struct WordEmitter {
     acc = t >= 8u ? x2 : (t >= 4u ? x1 : x0);
     nacc = t & 3u;
   }
-  // EXPERIMENT (off by default, -DACU_BYTES_PUSH16; DESIGN.md §9): a whole <= 16-byte row in one step — one 5-word
-  // shift instead of two 3-word ones. v = (w1:w0), bytes at positions >= nb are zero, nb in 0..16.
-  __device__ __forceinline__ void push16(uint64_t w0, uint64_t w1, uint32_t nb) {
-    const uint32_t sh = nacc * 8u;
-    const uint32_t v0 = (uint32_t)w0, v1 = (uint32_t)(w0 >> 32), v2 = (uint32_t)w1, v3 = (uint32_t)(w1 >> 32);
-    const uint32_t x0 = acc | (v0 << sh);
-    const uint32_t x1 = __funnelshift_l(v0, v1, sh);
-    const uint32_t x2 = __funnelshift_l(v1, v2, sh);
-    const uint32_t x3 = __funnelshift_l(v2, v3, sh);
-    const uint32_t x4 = __funnelshift_l(v3, 0u, sh);
-    const uint32_t t = nacc + nb;  // 0..19 bytes available
-    if (t >= 4u) store(x0);
-    if (t >= 8u) store(x1);
-    if (t >= 12u) store(x2);
-    if (t >= 16u) store(x3);
-    const uint32_t k = t >> 2;     // words that left
-    acc = k == 0u ? x0 : k == 1u ? x1 : k == 2u ? x2 : k == 3u ? x3 : x4;
-    nacc = t & 3u;
-  }
   __device__ __forceinline__ void finish() {
     if (acc != 0u) atomicOr(w, acc);
   }
@@ -162,7 +142,6 @@ __device__ __forceinline__ void load_upto16(const uint8_t *__restrict__ data, in
   *w1 = hi & (n1 >= 8u ? ~0ull : ((1ull << (n1 * 8u)) - 1ull));
 }
 
-template <bool STAGED>
 __device__ __forceinline__ void copy_row_direct(uint8_t *__restrict__ dst, const uint8_t *__restrict__ data, int64_t src, uint64_t len) {
   for (uint64_t c = 0; c < len; c += 8) {
     const uint64_t w = ld_bits64(data, (src + (int64_t)c) << 3, (src + (int64_t)len) << 3);
@@ -170,6 +149,15 @@ __device__ __forceinline__ void copy_row_direct(uint8_t *__restrict__ dst, const
 #pragma unroll
     for (int bidx = 0; bidx < 8; ++bidx)
       if (bidx < nb) dst[c + bidx] = (uint8_t)(w >> (8 * bidx));
+  }
+}
+
+// Skips the byte copy (grid-uniformly: out_data becomes NULL) when the total does not fit the caller's buffer or the offset
+// type: decided on the device so that no host round trip sits between the sizing pass and the copy.
+__device__ __forceinline__ void skip_copy_if_too_large(uint8_t *__restrict__ &out_data, const int64_t *total_ptr, int64_t out_cap, int64_t limit) {
+  if (out_data != nullptr && total_ptr != nullptr) {
+    const int64_t total = __ldg(total_ptr);
+    if (total > out_cap || total > limit) out_data = nullptr;
   }
 }
 
@@ -185,13 +173,7 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a,
                                                              int stage_cap, const int64_t *__restrict__ total_ptr, int64_t out_cap) {
   extern __shared__ __align__(16) uint8_t s_out[];
   __shared__ uint64_t warp_tot[33];
-  // the byte copy is skipped (grid-uniformly) when the total does not fit the caller's buffer or
-  // the offset type: decided on the device so that no host round trip sits between the sizing
-  // pass and this one
-  if (out_data != nullptr && total_ptr != nullptr) {
-    const int64_t total = __ldg(total_ptr);
-    if (total > out_cap || total > limit) out_data = nullptr;
-  }
+  skip_copy_if_too_large(out_data, total_ptr, out_cap, limit);
   const int64_t blk = first_block + blockIdx.x;
   const int64_t cta_begin = blk ? block_incl[blk - 1] : 0, cta_end = block_incl[blk];
   const int64_t stage_origin = cta_begin - (int64_t)((uintptr_t)(out_data + cta_begin) & 15);  // global byte that maps to s_out[0]
@@ -225,21 +207,17 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a,
     return;
   }
   if (err != ~0ull) atomicMin(res + RES_ERR2, err);
-  // new offsets: out[j0] = end of the previous row, out[j0+1..j0+3] = the first three ends (one aligned 128-bit store);
+  // new offsets: out[j0] = end of the previous row, out[j0+1..j0+3] = the first three ends;
   // the thread holding the last row also writes out[m]
   if (j0 <= a.m) {
     const int64_t first = cta_begin + (int64_t)rel;
-    if (R::kVec4 && j0 + 3 <= a.m && ((uintptr_t)out_offs & 15) == 0) {
-      *reinterpret_cast<int4 *>(static_cast<int32_t *>(out_offs) + j0) = make_int4((int32_t)first, (int32_t)end[0], (int32_t)end[1], (int32_t)end[2]);
-    } else {
 #pragma unroll
-      for (int k = 0; k < 4; ++k)
-        if (j0 + k <= a.m) {
-          const int64_t v = k == 0 ? first : end[k - 1];
-          if (a.ob == 4) static_cast<int32_t *>(out_offs)[j0 + k] = (int32_t)v;
-          else static_cast<int64_t *>(out_offs)[j0 + k] = v;
-        }
-    }
+    for (int k = 0; k < 4; ++k)
+      if (j0 + k <= a.m) {
+        const int64_t v = k == 0 ? first : end[k - 1];
+        if (a.ob == 4) static_cast<int32_t *>(out_offs)[j0 + k] = (int32_t)v;
+        else static_cast<int64_t *>(out_offs)[j0 + k] = v;
+      }
     if (j0 + 4 == a.m) {
       if (a.ob == 4) static_cast<int32_t *>(out_offs)[a.m] = (int32_t)end[3];
       else static_cast<int64_t *>(out_offs)[a.m] = end[3];
@@ -256,12 +234,8 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a,
       const uint32_t n0 = l32 < 8u ? l32 : 8u, n1 = l32 - n0;
       uint64_t w0, w1;
       load_upto16(a.data, begin[k], l32, &w0, &w1);
-#ifdef ACU_BYTES_PUSH16
-      em.push16(w0, w1, l32);
-#else
       em.push8(w0, n0);
       em.push8(w1, n1);
-#endif
       // ... the rest of a long row 8 bytes at a time
       for (uint64_t c = 16; c < len[k]; c += 8) {
         const uint32_t nb = (uint32_t)((len[k] - c) < 8 ? (len[k] - c) : 8);
@@ -284,7 +258,7 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a,
     int64_t pos = cta_begin + (int64_t)rel;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      if (len[k]) copy_row_direct<false>(out_data + pos, a.data, begin[k], len[k]);
+      if (len[k]) copy_row_direct(out_data + pos, a.data, begin[k], len[k]);
       pos += (int64_t)len[k];
     }
   }

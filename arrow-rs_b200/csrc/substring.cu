@@ -120,7 +120,6 @@ __global__ void __launch_bounds__(256) k_fill_i32(int32_t *__restrict__ out, int
 // Failure key of row j: 2j (start offset not a char boundary), 2j + 1 (end offset), PANIC_KEY | j (the slice panics).
 template <class O, bool UTF8>
 struct SubstrRows {
-  static constexpr bool kVec4 = false;
   int ob;
   int64_t m;
   const uint8_t *data;
@@ -158,7 +157,6 @@ struct SubstrRows {
 
 // Precomputed ranges (substring_by_char).
 struct RangeRows {
-  static constexpr bool kVec4 = false;
   int ob;
   int64_t m;
   const uint8_t *data;

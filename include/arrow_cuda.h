@@ -276,7 +276,9 @@ acu_status acu_filter_boolean(acu_ctx *ctx, const acu_filter_plan *plan, const a
                               acu_array_out *out);
 /* filter_bytes for Utf8/Binary (offset_bytes = 4) and Large* (8) (filter.rs:893-928).
  * Two-phase: out_offsets (count+1 entries) is always written and *out_data_len returned;
- * value bytes are copied only if out_data != NULL (capacity out_data_capacity). */
+ * value bytes are copied only if out_data != NULL (capacity out_data_capacity). `offsets` and
+ * `out_offsets` must be aligned to offset_bytes (a misaligned pointer => ACU_ERR_INVALID_ARGUMENT,
+ * and out_offsets is not written). */
 acu_status acu_filter_bytes(acu_ctx *ctx, const acu_filter_plan *plan, int32_t offset_bytes,
                             const void *offsets, const uint8_t *data, const acu_array *nulls_of,
                             void *out_offsets, uint8_t *out_data, int64_t out_data_capacity,
@@ -327,7 +329,8 @@ acu_status acu_take_boolean(acu_ctx *ctx, const acu_array *values, const acu_arr
 /* take_bytes (take.rs:499-627); also Dictionary<K,Utf8> -> Utf8 cast =
  * unpack_dictionary (arrow-cast/src/cast/dictionary.rs:310-317) with values = the
  * dictionary and indices = the keys. i32 offset overflow => ACU_ERR_OFFSET_OVERFLOW
- * (take.rs:520-523). Two-phase like acu_filter_bytes. `nulls_of` carries the
+ * (take.rs:520-523). Two-phase like acu_filter_bytes, with the same alignment rule for
+ * `offsets` and `out_offsets`. `nulls_of` carries the
  * validity/len/null_count of the byte array (its `values` member is ignored). */
 acu_status acu_take_bytes(acu_ctx *ctx, int32_t offset_bytes, const void *offsets,
                           const uint8_t *data, const acu_array *nulls_of,
@@ -743,7 +746,8 @@ typedef struct acu_column {
 
 /* Caller-owned output of one column. `array.values` receives the values (PRIMITIVE /
  * BOOLEAN) or the new offsets (BYTES, rows + 1 entries); `data` (capacity
- * `data_capacity`) the value bytes; `data_len` is set to the bytes required/written. */
+ * `data_capacity`) the value bytes; `data_len` is set to the bytes required/written.
+ * BYTES offsets, in and out, must be aligned to `width`, as for acu_take_bytes. */
 typedef struct acu_column_out {
   acu_array_out array;
   uint8_t *data;

@@ -869,3 +869,60 @@ def test_imported_device_slice(gpu, oracle, dtype, fmt, k):
         same_scalar(gpu_aggregate(gpu, dtype, abi.SUM, d), oracle.sum(h), "sum of an imported slice")
     finally:
         dev.free()
+
+
+# ---- 6. offset alignment -----------------------------------------------------------------------------------------------------
+@pytest.mark.parametrize("odt", [np.int32, np.int64])
+def test_byte_gathers_refuse_misaligned_offsets(gpu, odt):
+    """Every byte kernel reads and writes offsets as whole 4- or 8-byte words: take_bytes, filter_bytes and a Utf8 column of
+    take_record_batch / filter_record_batch refuse a source or output offset buffer half a word off, before anything writes
+    the output offsets. 70,000 aligned 32-bit keys into 100 rows would take the dictionary kernels with i32 offsets."""
+    ob = np.dtype(odt).itemsize
+    half = ob // 2
+    rng = np.random.default_rng(24_200 + ob)
+    n, m = 100, 70_000
+    src = SlicedUtf8(gpu, rng, n, 0, odt, 0.1)
+    icol, _, idd = index_column(gpu, rng, abi.U32, m, n, 0, 0.1)
+    plan = Plan(gpu, rand_bool(rng, n, 0.5, None))
+    d_src, d_out, d_data = gpu.malloc((n + 1) * ob + 16), gpu.malloc((m + 1) * ob + 16), gpu.malloc(16 * m + 16)
+    gpu.h2d(d_src + half, src.host.offsets)
+    out = gpu.alloc_out(0, m)
+    total = C.c_int64(0)
+
+    def record_batch(take, off, out_off):
+        col = src.column()
+        col.array.values = off
+        cols = (abi.Column * 1)(col)
+        outs = (abi.ColumnOut * 1)()
+        outs[0].array.values, outs[0].array.validity = out_off, out.validity
+        outs[0].data, outs[0].data_capacity = d_data, 16 * m
+        if take:
+            return gpu.lib.acu_take_record_batch(gpu.h, 1, cols, C.byref(idd), abi.U32, 0, outs)
+        return gpu.lib.acu_filter_record_batch(gpu.h, plan.h, 1, cols, outs)
+
+    calls = {
+        "take_bytes": lambda off, oo: gpu.lib.acu_take_bytes(gpu.h, ob, off, src.d_data, C.byref(src.nulls), C.byref(idd), abi.U32, 0, oo,
+                                                             d_data, 16 * m, C.byref(total), C.byref(out)),
+        "filter_bytes": lambda off, oo: gpu.lib.acu_filter_bytes(gpu.h, plan.h, ob, off, src.d_data, C.byref(src.nulls), oo, d_data, 16 * m,
+                                                                 C.byref(total), C.byref(out)),
+        "take_record_batch": lambda off, oo: record_batch(True, off, oo),
+        "filter_record_batch": lambda off, oo: record_batch(False, off, oo),
+    }
+    sentinel = np.full((m + 1) * ob + 16, 0xA5, dtype=np.uint8)
+    try:
+        for name, call in calls.items():
+            for off, out_off, which in [(src.d_off, d_out + half, "out_offsets"), (d_src + half, d_out, "offsets")]:
+                gpu.h2d(d_out, sentinel)
+                with pytest.raises(acu.ArrowError) as e:
+                    gpu.check(call(off, out_off))
+                assert e.value.status == abi.ERR_INVALID_ARGUMENT and str(e.value) == f"Invalid argument error: offsets must be {ob}-byte aligned", \
+                    f"{name}, {which} at +{half}: {e.value.status} {e.value}"
+                assert np.array_equal(gpu.d2h(d_out, sentinel.nbytes), sentinel), f"{name}, {which} at +{half}: out_offsets written"
+            gpu.check(call(src.d_off, d_out))  # the same call on aligned buffers runs
+    finally:
+        gpu._free_out(out)
+        for p in (d_src, d_out, d_data):
+            gpu.free(p)
+        plan.free()
+        icol.free()
+        src.free()

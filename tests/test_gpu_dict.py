@@ -79,3 +79,17 @@ def test_dictionary_gather_offset_overflow(gpu, oracle):
         errs.append(e.value)
     assert errs[0].status == errs[1].status == abi.ERR_OFFSET_OVERFLOW
     assert str(errs[0]) == str(errs[1])
+
+
+@pytest.mark.parametrize("d,per_sm", [(4096, 2), (8192, 1)])
+def test_dictionary_gather_multi_round(gpu, oracle, d, per_sm):
+    """k_dict_copy keeps per_sm CTAs resident per SM (its shared-memory table grows with D) and each CTA loops over 2048-row
+    rounds, prefetching the next round's keys: sizes that give every CTA at least two rounds, with key and dictionary nulls."""
+    import torch
+    sms = torch.cuda.get_device_properties(0).multi_processor_count
+    m = 2 * sms * per_sm * 2048 + 1001
+    rng = np.random.default_rng(d + 7)
+    offs, data, nulls = make_dict(rng, d, 16, 0.2)
+    keys_v = rng.integers(0, d, m).astype(np.int32)
+    keys = HostArray.from_numpy(abi.I32, keys_v, rng.random(m) >= 0.05)
+    check(gpu, oracle, offs, data, nulls, keys, f"D={d} m={m} over {sms} SMs")
