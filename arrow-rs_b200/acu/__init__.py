@@ -1317,6 +1317,112 @@ class Context:
             for p in owned:
                 self.free(p)
 
+    # -- concat_elements (arrow-string/src/concat_elements.rs) ------------------------------------------------------
+    @staticmethod
+    def _concat_type(col, is_utf8):
+        """Display of the DataType concat_elements_dyn matches on."""
+        if isinstance(col, Utf8Column):
+            large = "Large" if col.offsets.dtype == np.int64 else ""
+            return large + ("Utf8" if is_utf8 else "Binary")
+        if isinstance(col, ViewColumn):
+            return "Utf8View" if is_utf8 else "BinaryView"
+        if isinstance(col, FixedSizeBinaryColumn):
+            return f"FixedSizeBinary({col.width})"
+        if isinstance(col, DecimalArray):
+            return col.data_type()
+        if col.dtype == BOOL:
+            return "Boolean"
+        return abi.DTYPE_NAMES[col.dtype].capitalize().replace("Uint", "UInt")
+
+    def _concat_offsets(self, fn, n, ob, data_capacity):
+        """Two-phase byte-array concat, as _substring_offsets: fn(d_out_off, d_out_data, capacity, total_ref, out)."""
+        d_out_off = self.malloc((n + 1) * ob + 16)
+        out = self.alloc_out(0, n)
+        d_out_data = None
+        try:
+            total = C.c_int64(0)
+            self.check(fn(d_out_off, None, 0, C.byref(total), C.byref(out)))
+            cap = total.value if data_capacity is None else data_capacity
+            d_out_data = self.malloc(cap + 16)
+            self.check(fn(d_out_off, d_out_data, cap, C.byref(total), C.byref(out)))
+            o = self.d2h(d_out_off, (n + 1) * ob, np.int32 if ob == 4 else np.int64)
+            b = self.d2h(d_out_data, total.value)
+            validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+            return Utf8Column(o, b, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
+        finally:
+            self._free_out(out)
+            for p in (d_out_off, d_out_data):
+                self.free(p)
+
+    def concat_elements(self, l, r, is_utf8=True, data_capacity=None):
+        """arrow_string::concat_elements::concat_elements_dyn(l, r) of two Utf8Column (is_utf8=False: Binary / LargeBinary),
+        ViewColumn (is_utf8=False: BinaryView) or FixedSizeBinaryColumn operands of one type. A view result has one new data
+        buffer (none when no result is longer than 12 bytes). `data_capacity` as for substring."""
+        lt, rt = self._concat_type(l, is_utf8), self._concat_type(r, is_utf8)
+        both_fsb = isinstance(l, FixedSizeBinaryColumn) and isinstance(r, FixedSizeBinaryColumn)
+        if lt != rt and not both_fsb:
+            raise ArrowError(abi.ERR_COMPUTE, f"Compute error: Cannot concat arrays of different types: {lt} != {rt}")
+        if not isinstance(l, (Utf8Column, ViewColumn, FixedSizeBinaryColumn)):
+            raise ArrowError(abi.ERR_NOT_YET_IMPLEMENTED, f"Not yet implemented: concat not supported for {lt}")
+        owned, keep = [], []
+        n = l.length
+        try:
+            if isinstance(l, Utf8Column):
+                dl, dr = self._upload_bytes_col(l, owned), self._upload_bytes_col(r, owned)
+                ob = l.offsets.dtype.itemsize
+                return self._concat_offsets(
+                    lambda oo, od, cap, tot, out: self.lib.acu_concat_elements_bytes(self.h, ob, C.byref(dl), C.byref(dr), oo, od, cap, tot, out),
+                    n, ob, data_capacity)
+            if isinstance(l, ViewColumn):
+                dl, dr = self._upload_view_col(l, owned, keep), self._upload_view_col(r, owned, keep)
+                d_views = self.malloc(n * 16 + 16)
+                owned.append(d_views)
+                out = self.alloc_out(0, n)
+                try:
+                    total = C.c_int64(0)
+                    self.check(self.lib.acu_concat_elements_byte_view(self.h, C.byref(dl), C.byref(dr), None, None, 0, C.byref(total), C.byref(out)))
+                    cap = total.value if data_capacity is None else data_capacity
+                    d_data = self.malloc(cap + 16)
+                    owned.append(d_data)
+                    self.check(self.lib.acu_concat_elements_byte_view(self.h, C.byref(dl), C.byref(dr), d_views, d_data, cap, C.byref(total),
+                                                                      C.byref(out)))
+                    views = self.d2h(d_views, n * 16).reshape(n, 16)
+                    buffers = [self.d2h(d_data, total.value)] if total.value else []
+                    validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+                finally:
+                    self._free_out(out)
+                nulls = HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0)
+                return ViewColumn(views, buffers, nulls)
+            dl, dr = self._upload_fsb(l, owned), self._upload_fsb(r, owned)
+            out = self.alloc_out(n * (l.width + r.width), n)
+            try:
+                w = C.c_int32(0)
+                self.check(self.lib.acu_concat_elements_fixed_size_binary(self.h, l.width, C.byref(dl), r.width, C.byref(dr), C.byref(w),
+                                                                          C.byref(out)))
+                vals = self.d2h(out.values, n * w.value).reshape(n, w.value)
+                validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+            finally:
+                self._free_out(out)
+            return FixedSizeBinaryColumn(vals, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
+        finally:
+            for p in owned:
+                self.free(p)
+
+    def concat_elements_utf8_many(self, cols, data_capacity=None):
+        """arrow_string::concat_elements::concat_elements_utf8_many of Utf8Column operands with one offset width (the device
+        path is the same for Binary / LargeBinary operands)."""
+        owned = []
+        try:
+            descs = (abi.BytesArray * max(len(cols), 1))(*[self._upload_bytes_col(c, owned) for c in cols])
+            ob = cols[0].offsets.dtype.itemsize if cols else 4
+            n = cols[0].length if cols else 0
+            return self._concat_offsets(
+                lambda oo, od, cap, tot, out: self.lib.acu_concat_elements_bytes_many(self.h, ob, len(cols), descs, oo, od, cap, tot, out),
+                n, ob, data_capacity)
+        finally:
+            for p in owned:
+                self.free(p)
+
     # -- fused compare -> filter (cmp.rs:220-382 feeding filter.rs:254-273) -------------------
     def filter_cmp(self, values, op, a, b):
         """filter(values, &cmp::op(a, b)?) with the predicate never materialised: the comparison writes the filter plan."""

@@ -227,6 +227,10 @@ PROTOTYPES = {
     "acu_substring_by_char": (i32, [vp, i32, i64, i32, u64, P(BytesArray), vp, vp, i64, P(i64), P(ArrayOut)]),
     "acu_substring_byte_view": (i32, [vp, i32, i64, i32, u64, P(ViewArray), vp, P(ArrayOut)]),
     "acu_substring_fixed_size_binary": (i32, [vp, i32, i64, i32, u64, P(Array), P(i32), P(ArrayOut)]),
+    "acu_concat_elements_bytes": (i32, [vp, i32, P(BytesArray), P(BytesArray), vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_concat_elements_bytes_many": (i32, [vp, i32, i32, P(BytesArray), vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_concat_elements_byte_view": (i32, [vp, P(ViewArray), P(ViewArray), vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_concat_elements_fixed_size_binary": (i32, [vp, i32, P(Array), i32, P(Array), P(i32), P(ArrayOut)]),
     "acu_cast_numeric": (i32, [vp, i32, i32, i32, P(Array), P(ArrayOut)]),
     "acu_cast_decimal": (i32, [vp, P(DecimalType), P(DecimalType), i32, P(Array), P(ArrayOut)]),
     "acu_cast_to_decimal": (i32, [vp, i32, P(DecimalType), i32, P(Array), P(ArrayOut)]),

@@ -1,7 +1,7 @@
 // bytes_engine.cuh — the offsets-and-copy stage of the variable-width kernels: a producer gives each row's source byte
 // range, the engine sums them per CTA (k_bytes_block_totals), and after a device-wide scan of the CTA totals writes the new
-// offsets and copies the bytes (k_bytes_offsets_copy). take / filter (bytes.cu) and substring (substring.cu) differ only in
-// the producer.
+// offsets and copies the bytes (k_bytes_offsets_copy). take / filter (bytes.cu), substring (substring.cu) and concat_elements
+// (concat_elements.cu) differ only in the producer.
 //
 // A producer `R` is a trivially copyable struct with
 //   int ob; int64_t m;            // offset width, output rows
@@ -9,14 +9,28 @@
 //   int detect_oob;               // k_bytes_block_totals: *err of the first pass goes to res[RES_ERR_INDEX] (atomicMin)
 //   void ranges4(int64_t j0, int64_t begin[4], uint64_t len[4], unsigned long long *err) const;
 // where ranges4 gives the byte ranges of rows j0 .. j0+3 (zero length past m) and lowers *err to a failing row's key.
+//
+// A multi-segment producer (concat_elements.cu) builds each row from K >= 1 source segments, each with its own pointer (a
+// different operand's buffer, or a view slot's inline bytes). Instead of `data` it has
+//   int nsegs() const;                                                   // K
+//   void segment(int64_t row, int s, const uint8_t **p, uint64_t *len) const;
+// its ranges4 gives each row's total length (begin unused), and the copy pushes the segments of every non-empty row one
+// after another through the same staging / direct paths.
 #pragma once
-#include "common.cuh"
+#include <type_traits>
+
+#include "internal.cuh"
 
 #define BY_THREADS 512                 // CTA of the bytes kernels: 512 threads x 4 consecutive rows,
 #define BY_ROWS (BY_THREADS * 4)       // two CTAs resident per SM so that one loads while the other assembles
 #define BY_STAGE_CAP (48 * 1024)
 
 namespace {
+
+template <class R, class = void>
+struct has_segments : std::false_type {};
+template <class R>
+struct has_segments<R, std::void_t<decltype(std::declval<const R &>().nsegs())>> : std::true_type {};
 
 // CTA-wide exclusive scan of one u64 per thread (up to 1024 threads); returns the thread's exclusive
 // prefix, *total = the CTA total. Two barriers.
@@ -142,6 +156,22 @@ __device__ __forceinline__ void load_upto16(const uint8_t *__restrict__ data, in
   *w1 = hi & (n1 >= 8u ? ~0ull : ((1ull << (n1 * 8u)) - 1ull));
 }
 
+// The bytes data[pos .. pos+len) into the emitter: the first 16 without branches (short strings are the common case), then
+// the rest of a long range 8 at a time. The single-range producers keep these lines inline in k_bytes_offsets_copy: called
+// through this helper, their kernels compile to different SASS.
+__device__ __forceinline__ void emit_range(WordEmitter &em, const uint8_t *data, int64_t pos, uint64_t len) {
+  const uint32_t l32 = len > 16 ? 16u : (uint32_t)len;
+  const uint32_t n0 = l32 < 8u ? l32 : 8u, n1 = l32 - n0;
+  uint64_t w0, w1;
+  load_upto16(data, pos, l32, &w0, &w1);
+  em.push8(w0, n0);
+  em.push8(w1, n1);
+  for (uint64_t c = 16; c < len; c += 8) {
+    const uint32_t nb = (uint32_t)((len - c) < 8 ? (len - c) : 8);
+    em.push8(load_upto8(data, pos + (int64_t)c, nb), nb);
+  }
+}
+
 __device__ __forceinline__ void copy_row_direct(uint8_t *__restrict__ dst, const uint8_t *__restrict__ data, int64_t src, uint64_t len) {
   for (uint64_t c = 0; c < len; c += 8) {
     const uint64_t w = ld_bits64(data, (src + (int64_t)c) << 3, (src + (int64_t)len) << 3);
@@ -229,17 +259,27 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a,
     em.init(s_out, lead + (uint32_t)rel);
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      // the first 16 bytes of every row without branches (short strings are the common case) ...
-      const uint32_t l32 = len[k] > 16 ? 16u : (uint32_t)len[k];
-      const uint32_t n0 = l32 < 8u ? l32 : 8u, n1 = l32 - n0;
-      uint64_t w0, w1;
-      load_upto16(a.data, begin[k], l32, &w0, &w1);
-      em.push8(w0, n0);
-      em.push8(w1, n1);
-      // ... the rest of a long row 8 bytes at a time
-      for (uint64_t c = 16; c < len[k]; c += 8) {
-        const uint32_t nb = (uint32_t)((len[k] - c) < 8 ? (len[k] - c) : 8);
-        em.push8(load_upto8(a.data, begin[k] + (int64_t)c, nb), nb);
+      if constexpr (has_segments<R>::value) {
+        if (len[k])
+          for (int s = 0; s < a.nsegs(); ++s) {
+            const uint8_t *p;
+            uint64_t l;
+            a.segment(j0 + k, s, &p, &l);
+            emit_range(em, p, 0, l);
+          }
+      } else {
+        // the first 16 bytes of every row without branches (short strings are the common case) ...
+        const uint32_t l32 = len[k] > 16 ? 16u : (uint32_t)len[k];
+        const uint32_t n0 = l32 < 8u ? l32 : 8u, n1 = l32 - n0;
+        uint64_t w0, w1;
+        load_upto16(a.data, begin[k], l32, &w0, &w1);
+        em.push8(w0, n0);
+        em.push8(w1, n1);
+        // ... the rest of a long row 8 bytes at a time
+        for (uint64_t c = 16; c < len[k]; c += 8) {
+          const uint32_t nb = (uint32_t)((len[k] - c) < 8 ? (len[k] - c) : 8);
+          em.push8(load_upto8(a.data, begin[k] + (int64_t)c, nb), nb);
+        }
       }
     }
     em.finish();
@@ -258,10 +298,54 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a,
     int64_t pos = cta_begin + (int64_t)rel;
 #pragma unroll
     for (int k = 0; k < 4; ++k) {
-      if (len[k]) copy_row_direct(out_data + pos, a.data, begin[k], len[k]);
+      if constexpr (has_segments<R>::value) {
+        int64_t at = pos;
+        if (len[k])
+          for (int s = 0; s < a.nsegs(); ++s) {
+            const uint8_t *p;
+            uint64_t l;
+            a.segment(j0 + k, s, &p, &l);
+            if (l) copy_row_direct(out_data + at, p, 0, l);
+            at += (int64_t)l;
+          }
+      } else {
+        if (len[k]) copy_row_direct(out_data + pos, a.data, begin[k], len[k]);
+      }
       pos += (int64_t)len[k];
     }
   }
+}
+
+// ---- host side: the launch sequence shared by substring.cu and concat_elements.cu ------------------------------------
+inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
+
+// block totals -> scan -> offsets (+ bytes when out_data != NULL and the total fits out_cap and `limit`); RES_AUX0 = the
+// total, RES_ERR2 = the lowest row whose end passes `limit` (the largest value the output offset type holds).
+template <class R>
+acu_status engine_launch(acu_ctx *ctx, R rows, int64_t *block_tot, void *out_offsets, uint8_t *out_data, int64_t out_cap, int64_t limit) {
+  const int64_t blocks = (rows.m + BY_ROWS - 1) / BY_ROWS;
+  rows.detect_oob = 1;
+  ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_block_totals<R>, (unsigned)blocks, BY_THREADS, 0, rows, block_tot, ctx->d_res);
+  ACU_TRY(acu_scan_inclusive_i64(ctx, block_tot, blocks, block_tot + blocks));
+  ACU_CUDA(ctx, cudaMemcpyAsync(ctx->d_res + RES_AUX0, block_tot + (blocks - 1), 8, cudaMemcpyDeviceToDevice, ctx->stream));
+  rows.detect_oob = 0;
+  const int stage_cap = BY_STAGE_CAP;
+  ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
+  ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<R>, (unsigned)blocks, BY_THREADS, stage_cap, rows, block_tot, (int64_t)0, out_offsets,
+                   out_data, limit, (int64_t)-1, ctx->d_res, stage_cap, block_tot + (blocks - 1), out_cap);
+  return ACU_OK;
+}
+inline size_t engine_scratch(int64_t m) {
+  const int64_t blocks = (m + BY_ROWS - 1) / BY_ROWS;
+  return align256((size_t)(blocks + blocks / 4096 + 64) * 8);
+}
+
+inline acu_status finish_bytes(acu_ctx *ctx, uint8_t *out_data, int64_t out_cap, int64_t *out_data_len) {
+  *out_data_len = (int64_t)ctx->h_res[RES_AUX0];
+  if (out_data && *out_data_len > out_cap)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, (uint64_t)*out_data_len, "output data capacity %lld < required %lld",
+                    (long long)out_cap, (long long)*out_data_len);
+  return ACU_OK;
 }
 
 }  // namespace

@@ -364,36 +364,6 @@ acu_status boundary_error(acu_ctx *ctx, int64_t row, uint64_t off) {
   return acu_fail(ctx, ACU_ERR_COMPUTE, row, off, 0, 0, "The offset %llu is at an invalid utf-8 boundary.", (unsigned long long)off);
 }
 
-size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
-
-// bytes engine: block totals -> scan -> offsets (+ bytes when out_data != NULL and the total fits out_cap); RES_AUX0 = total
-template <class R>
-acu_status engine_launch(acu_ctx *ctx, R rows, int64_t *block_tot, void *out_offsets, uint8_t *out_data, int64_t out_cap) {
-  const int64_t blocks = (rows.m + BY_ROWS - 1) / BY_ROWS;
-  rows.detect_oob = 1;
-  ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_block_totals<R>, (unsigned)blocks, BY_THREADS, 0, rows, block_tot, ctx->d_res);
-  ACU_TRY(acu_scan_inclusive_i64(ctx, block_tot, blocks, block_tot + blocks));
-  ACU_CUDA(ctx, cudaMemcpyAsync(ctx->d_res + RES_AUX0, block_tot + (blocks - 1), 8, cudaMemcpyDeviceToDevice, ctx->stream));
-  rows.detect_oob = 0;
-  const int stage_cap = BY_STAGE_CAP;
-  ACU_CUDA(ctx, cudaFuncSetAttribute(k_bytes_offsets_copy<R>, cudaFuncAttributeMaxDynamicSharedMemorySize, stage_cap));
-  ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_bytes_offsets_copy<R>, (unsigned)blocks, BY_THREADS, stage_cap, rows, block_tot, (int64_t)0, out_offsets,
-                   out_data, INT64_MAX, (int64_t)-1, ctx->d_res, stage_cap, block_tot + (blocks - 1), out_cap);
-  return ACU_OK;
-}
-size_t engine_scratch(int64_t m) {
-  const int64_t blocks = (m + BY_ROWS - 1) / BY_ROWS;
-  return align256((size_t)(blocks + blocks / 4096 + 64) * 8);
-}
-
-acu_status finish_bytes(acu_ctx *ctx, uint8_t *out_data, int64_t out_cap, int64_t *out_data_len) {
-  *out_data_len = (int64_t)ctx->h_res[RES_AUX0];
-  if (out_data && *out_data_len > out_cap)
-    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, (uint64_t)*out_data_len, "output data capacity %lld < required %lld",
-                    (long long)out_cap, (long long)*out_data_len);
-  return ACU_OK;
-}
-
 template <class O>
 acu_status substring_bytes_run(acu_ctx *ctx, int32_t is_utf8, int64_t start, bool has_len, uint64_t length, const acu_bytes_array *a,
                                int64_t data_len, void *out_offsets, uint8_t *out_data, int64_t out_cap, int64_t *out_data_len,
@@ -407,10 +377,10 @@ acu_status substring_bytes_run(acu_ctx *ctx, int32_t is_utf8, int64_t start, boo
     const O *offs = static_cast<const O *>(a->offsets);
     if (is_utf8) {
       SubstrRows<O, true> r{(int)sizeof(O), n, a->data, 0, offs, data_len, st, ln, has_len};
-      ACU_TRY(engine_launch(ctx, r, static_cast<int64_t *>(scratch), out_offsets, out_data, out_cap));
+      ACU_TRY(engine_launch(ctx, r, static_cast<int64_t *>(scratch), out_offsets, out_data, out_cap, INT64_MAX));
     } else {
       SubstrRows<O, false> r{(int)sizeof(O), n, a->data, 0, offs, data_len, st, ln, has_len};
-      ACU_TRY(engine_launch(ctx, r, static_cast<int64_t *>(scratch), out_offsets, out_data, out_cap));
+      ACU_TRY(engine_launch(ctx, r, static_cast<int64_t *>(scratch), out_offsets, out_data, out_cap, INT64_MAX));
     }
   } else {
     ACU_CUDA(ctx, cudaMemsetAsync(out_offsets, 0, sizeof(O), ctx->stream));
@@ -448,7 +418,7 @@ acu_status substring_by_char_run(acu_ctx *ctx, int32_t ob, int64_t start, bool h
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_char_bounds, acu_grid(ctx, (n + 255) / 256, 8), 256, 0, p);
     ACU_LAUNCH_TIMED(ctx, ACU_K_BYTES, k_char_long, acu_grid(ctx, (n + 7) / 8, 16), 256, 0, p);  // one warp per queued row
     RangeRows r{ob, n, a->data, 0, p.rb, p.rl};
-    ACU_TRY(engine_launch(ctx, r, reinterpret_cast<int64_t *>(base), out_offsets, out_data, out_cap));
+    ACU_TRY(engine_launch(ctx, r, reinterpret_cast<int64_t *>(base), out_offsets, out_data, out_cap, INT64_MAX));
   } else {
     ACU_CUDA(ctx, cudaMemsetAsync(out_offsets, 0, (size_t)ob, ctx->stream));
   }

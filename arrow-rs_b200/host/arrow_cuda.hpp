@@ -1699,6 +1699,82 @@ inline Result<StringArray> substring_by_char(const StringArray &a, int64_t start
   });
 }
 
+// ---- concat_elements (arrow-string/src/concat_elements.rs) -------------------------------------------------------
+// concat_elements_utf8 / concat_elements_utf8_many on Utf8 (StringArray), concat_elements_string_view_array on Utf8View
+// (StringViewArray) and concat_elements_dyn, through acu_concat_elements_bytes / _bytes_many / _byte_view. A view result
+// has the reference's layout: one new data buffer, none when no result is longer than 12 bytes.
+namespace detail {
+// The two-phase byte-array call over n rows: the offsets and the byte count, then the bytes.
+template <class F>
+inline Result<StringArray> concat_two_phase(int64_t n, F call) {
+  Context &c = Context::get();
+  Buffer offs = Buffer::allocate((size_t)(n + 1) * 4), nb = Buffer::allocate(acu_bitmap_bytes(std::max<int64_t>(n, 1)));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  int64_t total = 0;
+  acu_status st = call(offs.data(), nullptr, 0, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  Buffer data = Buffer::allocate((size_t)std::max<int64_t>(total, 1));
+  st = call(offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return StringArray(offs, data, o.len, out_nulls(o, nb));
+}
+}  // namespace detail
+
+inline Result<StringArray> concat_elements_utf8(const StringArray &left, const StringArray &right) {
+  const acu_bytes_array l = kernels::cmp::bytes_view(left, false), r = kernels::cmp::bytes_view(right, false);
+  return detail::concat_two_phase(left.len(), [&](void *offs, uint8_t *data, int64_t cap, int64_t *total, acu_array_out *o) {
+    return acu_concat_elements_bytes(Context::get().raw(), 4, &l, &r, offs, data, cap, total, o);
+  });
+}
+
+inline Result<StringArray> concat_elements_utf8_many(const std::vector<const StringArray *> &arrays) {
+  std::vector<acu_bytes_array> xs;
+  for (const StringArray *a : arrays) xs.push_back(kernels::cmp::bytes_view(*a, false));
+  return detail::concat_two_phase(arrays.empty() ? 0 : arrays[0]->len(), [&](void *offs, uint8_t *data, int64_t cap, int64_t *total, acu_array_out *o) {
+    return acu_concat_elements_bytes_many(Context::get().raw(), 4, (int32_t)xs.size(), xs.data(), offs, data, cap, total, o);
+  });
+}
+
+inline Result<StringViewArray> concat_elements_string_view_array(const StringViewArray &left, const StringViewArray &right) {
+  Context &c = Context::get();
+  const like::detail::ViewDesc l(left, false), r(right, false);
+  const int64_t n = left.len();
+  Buffer views = Buffer::allocate((size_t)std::max<int64_t>(n, 1) * 16), nb = Buffer::allocate(acu_bitmap_bytes(std::max<int64_t>(n, 1)));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  int64_t total = 0;
+  acu_status st = acu_concat_elements_byte_view(c.raw(), &l.v, &r.v, nullptr, nullptr, 0, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  Buffer data = Buffer::allocate((size_t)std::max<int64_t>(total, 1));
+  st = acu_concat_elements_byte_view(c.raw(), &l.v, &r.v, views.data(), static_cast<uint8_t *>(data.data()), total, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  std::vector<bool> valid((size_t)o.len, true);
+  if (o.has_validity) {
+    std::vector<uint8_t> bits(acu_bitmap_bytes(o.len));
+    nb.to_host(bits.data(), bits.size());
+    for (size_t i = 0; i < valid.size(); ++i) valid[i] = (bits[i >> 3] >> (i & 7)) & 1;
+  }
+  std::vector<ViewDataBuffer> bufs;
+  if (total > 0) bufs.push_back(ViewDataBuffer{data, (size_t)total, (size_t)total});
+  return StringViewArray(views, 0, o.len, std::move(bufs), std::move(valid));
+}
+
+// concat_elements_dyn (concat_elements.rs:419-476): Utf8 operands; any other pair fails as the reference does.
+inline Result<ArrayRef> concat_elements_dyn(const Array &left, const Array &right) {
+  if (left.data_type() != right.data_type())
+    return ArrowError{ACU_ERR_COMPUTE, std::string("Compute error: Cannot concat arrays of different types: ") + detail::dtype_display(left.data_type()) +
+                                           " != " + detail::dtype_display(right.data_type())};
+  if (left.data_type() != DataType::Utf8)
+    return ArrowError{ACU_ERR_NOT_YET_IMPLEMENTED, std::string("Not yet implemented: concat not supported for ") + detail::dtype_display(left.data_type())};
+  auto r = concat_elements_utf8(static_cast<const StringArray &>(left), static_cast<const StringArray &>(right));
+  if (r.is_err()) return r.unwrap_err();
+  return ArrayRef(std::make_shared<StringArray>(r.unwrap()));
+}
+inline Result<StringViewArray> concat_elements_dyn(const StringViewArray &left, const StringViewArray &right) {
+  return concat_elements_string_view_array(left, right);
+}
+
 
 // ---- nullif / zip (arrow-select/src/nullif.rs:44-113, zip.rs:99-226) -------------------------------------------
 namespace detail {

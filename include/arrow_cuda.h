@@ -557,6 +557,52 @@ acu_status acu_substring_byte_view(acu_ctx *ctx, int32_t is_utf8, int64_t start,
 acu_status acu_substring_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, int64_t start, int32_t has_length, uint64_t length,
                                            const acu_array *a, int32_t *out_byte_width, acu_array_out *out);
 
+/* ------------------------------------------------------------------------- */
+/* concat_elements — arrow-string/src/concat_elements.rs                     */
+/* ------------------------------------------------------------------------- */
+/* The element-wise concatenation of equally long arrays (concat_elements.rs:31-407). Row i of the result is the operands'
+ * values at row i, one after another. Nulls are NullBuffer::union of the operands': out_nulls / out carries a validity
+ * (normalised to bit offset 0, capacity acu_bitmap_bytes(len)) only when some row is null, also when an operand has a
+ * NullBuffer without nulls. Lengths that differ => ACU_ERR_COMPUTE "Arrays must have the same length: {l} != {r}".
+ *
+ * acu_concat_elements_bytes — concat_elements_bytes / _utf8 / concat_element_binary (:31-104) for Utf8 / Binary
+ *   (offset_bytes 4) and LargeUtf8 / LargeBinary (8); no byte is validated, so one entry point serves both. Every row is
+ *   concatenated, null rows included (the bytes under a null slot are copied). out_offsets: len + 1 entries starting at 0
+ *   (also for sliced operands, which may be sliced differently). With i32 offsets, the first row whose end passes i32::MAX
+ *   is the reference's `from_usize(..).unwrap()` panic: ACU_ERR_PANIC_OUT_OF_BOUNDS "called `Option::unwrap()` on a `None`
+ *   value", detail.index = that row. Two-phase like acu_substring_bytes: out_data == NULL writes the offsets and
+ *   *out_data_len only; both calls run the offsets pass and the overflow check. A copy call whose out_data_capacity is
+ *   below the total => ACU_ERR_INVALID_ARGUMENT, no byte written.
+ * acu_concat_elements_bytes_many — concat_elements_utf8_many (:113-173) over n_arrays >= 1 operands, `arrays` a HOST array
+ *   of descriptors; output as above. n_arrays < 1 => ACU_ERR_COMPUTE "concat requires input of at least one array"; an
+ *   operand whose length differs from arrays[0]'s => ACU_ERR_COMPUTE "Arrays must have the same length of {len}".
+ * acu_concat_elements_byte_view — concat_elements_string_view_array / binary_view_array (:230-407), with the reference's
+ *   layout bit for bit: a null row is an all-zero view and its operands' views are never read; a result of at most 12 bytes
+ *   is an inline view, zero padded; a longer one is appended, in row order, to ONE new data buffer (out_data) and its view
+ *   is (length, first 4 bytes, buffer 0, offset). The result has that one data buffer when *out_data_len > 0 and none
+ *   otherwise. Two-phase: out_views == NULL is the sizing call (*out_data_len = the bytes of the non-null results longer
+ *   than 12 bytes); the copy call writes out_views (16 bytes per row, 16-byte aligned) and out_data. A data buffer longer
+ *   than i32::MAX => ACU_ERR_ARITHMETIC_OVERFLOW "byte array offset overflow" before any row is written; a copy call whose
+ *   out_data_capacity is below *out_data_len => ACU_ERR_INVALID_ARGUMENT, nothing written.
+ * acu_concat_elements_fixed_size_binary — concat_elements_fixed_size_binary (:181-228): *out_byte_width = l_width + r_width,
+ *   row i = left row i then right row i; a null row is zero bytes (append_null). After the length check, a negative width
+ *   => ACU_ERR_INVALID_ARGUMENT "Invalid size of FixedSizeBinaryArray({w})", left before right; a sum past i32::MAX is the
+ *   reference's builder panic, also with zero rows: ACU_ERR_PANIC_OUT_OF_BOUNDS "value length ({sum as i32}) of the array
+ *   must >= 0". out->values: len x (l_width + r_width) bytes.
+ * Type dispatch (concat_elements_dyn, :419-476) belongs to the typed host layers. A scalar operand or an offset width other
+ * than 4 / 8 => ACU_ERR_INVALID_ARGUMENT. Synchronous (not available inside a stream-ordered section); kernel time is
+ * counted in ACU_K_BYTES. */
+acu_status acu_concat_elements_bytes(acu_ctx *ctx, int32_t offset_bytes, const acu_bytes_array *l, const acu_bytes_array *r,
+                                     void *out_offsets, uint8_t *out_data, int64_t out_data_capacity, int64_t *out_data_len,
+                                     acu_array_out *out_nulls);
+acu_status acu_concat_elements_bytes_many(acu_ctx *ctx, int32_t offset_bytes, int32_t n_arrays, const acu_bytes_array *arrays,
+                                          void *out_offsets, uint8_t *out_data, int64_t out_data_capacity, int64_t *out_data_len,
+                                          acu_array_out *out_nulls);
+acu_status acu_concat_elements_byte_view(acu_ctx *ctx, const acu_view_array *l, const acu_view_array *r, void *out_views,
+                                         uint8_t *out_data, int64_t out_data_capacity, int64_t *out_data_len, acu_array_out *out_nulls);
+acu_status acu_concat_elements_fixed_size_binary(acu_ctx *ctx, int32_t l_width, const acu_array *l, int32_t r_width,
+                                                 const acu_array *r, int32_t *out_byte_width, acu_array_out *out);
+
 /* Utf8View / BinaryView buffer management for BatchCoalescer (InProgressByteViewArray, arrow-select/src/coalesce/
  * byte_view.rs). The reference decides per source array whether its data buffers are compacted ("gc": when they hold more
  * than twice the bytes its views use, :366-381) and how output buffers are sized (BufferSource, :526-559); that policy stays

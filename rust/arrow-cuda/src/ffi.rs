@@ -270,6 +270,17 @@ extern "C" {
                                    out_views: *mut c_void, out_nulls: *mut acu_array_out) -> acu_status;
     pub fn acu_substring_fixed_size_binary(ctx: *mut acu_ctx, byte_width: i32, start: i64, has_length: i32, length: u64, a: *const acu_array,
                                            out_byte_width: *mut i32, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_concat_elements_bytes(ctx: *mut acu_ctx, offset_bytes: i32, l: *const acu_bytes_array, r: *const acu_bytes_array,
+                                     out_offsets: *mut c_void, out_data: *mut u8, out_data_capacity: i64, out_data_len: *mut i64,
+                                     out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_concat_elements_bytes_many(ctx: *mut acu_ctx, offset_bytes: i32, n_arrays: i32, arrays: *const acu_bytes_array,
+                                          out_offsets: *mut c_void, out_data: *mut u8, out_data_capacity: i64, out_data_len: *mut i64,
+                                          out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_concat_elements_byte_view(ctx: *mut acu_ctx, l: *const acu_view_array, r: *const acu_view_array, out_views: *mut c_void,
+                                         out_data: *mut u8, out_data_capacity: i64, out_data_len: *mut i64,
+                                         out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_concat_elements_fixed_size_binary(ctx: *mut acu_ctx, l_width: i32, l: *const acu_array, r_width: i32, r: *const acu_array,
+                                                 out_byte_width: *mut i32, out: *mut acu_array_out) -> acu_status;
     pub fn acu_concat(ctx: *mut acu_ctx, n_arrays: i32, arrays: *const acu_column, out: *mut acu_column_out) -> acu_status;
     pub fn acu_concat_batches(ctx: *mut acu_ctx, n_batches: i32, n_columns: i32, columns: *const acu_column, outs: *mut acu_column_out,
                               out_rows: *mut i64) -> acu_status;

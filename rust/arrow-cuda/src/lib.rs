@@ -587,7 +587,7 @@ pub mod compute {
             ffi::acu_bytes_array { offsets: a.view().values, data: a.column.data, nulls: *a.view() }
         }
 
-        fn view_operand<T: ByteViewType + ?Sized>(ctx: &Context, a: &GenericByteViewArray<T>, bufs: &mut Vec<DeviceBuffer>,
+        pub(super) fn view_operand<T: ByteViewType + ?Sized>(ctx: &Context, a: &GenericByteViewArray<T>, bufs: &mut Vec<DeviceBuffer>,
                                                   ptrs: &mut Vec<*const u8>) -> Result<ffi::acu_view_array, ArrowError> {
             let (validity, validity_offset, null_count) = match a.nulls() {
                 Some(n) => {
@@ -611,7 +611,7 @@ pub mod compute {
             Ok(ffi::acu_view_array { views, buffers: ptrs.as_ptr(), n_buffers: ptrs.len() as i32, reserved: 0, nulls })
         }
 
-        fn fsb_operand(ctx: &Context, a: &dyn Array, width: usize, bufs: &mut Vec<DeviceBuffer>) -> Result<ffi::acu_array, ArrowError> {
+        pub(super) fn fsb_operand(ctx: &Context, a: &dyn Array, width: usize, bufs: &mut Vec<DeviceBuffer>) -> Result<ffi::acu_array, ArrowError> {
             let d = a.to_data();
             let (validity, validity_offset, null_count) = match d.nulls() {
                 Some(n) => {
@@ -745,6 +745,141 @@ pub mod compute {
             two_phase(&ctx, array, &|x, offs, data, cap, total, nulls| unsafe {
                 ffi::acu_substring_by_char(ctx.raw(), ob, start, has_len, len, x, offs, data, cap, total, nulls)
             })
+        }
+    }
+
+    /// `arrow_string::concat_elements` (concat_elements.rs:31-476) on the device.
+    pub mod concat_elements {
+        use super::super::{ffi, ColumnOut, Context, DeviceArray, DeviceBuffer};
+        use super::substring::{fsb_operand, view_operand};
+        use arrow_array::cast::AsArray;
+        use arrow_array::types::ByteViewType;
+        use arrow_array::*;
+        use arrow_buffer::{BooleanBuffer, Buffer, NullBuffer, ScalarBuffer};
+        use arrow_data::ArrayData;
+        use arrow_schema::{ArrowError, DataType};
+        use std::sync::Arc;
+
+        fn nulls_of(validity: &DeviceBuffer, o: &ffi::acu_array_out, n: usize) -> Result<Option<NullBuffer>, ArrowError> {
+            if o.has_validity == 0 { return Ok(None); }
+            let bits = BooleanBuffer::new(validity.to_host(super::super::bitmap_bytes(n))?, 0, n);
+            Ok(Some(unsafe { NullBuffer::new_unchecked(bits, o.null_count as usize) }))
+        }
+
+        /// The two-phase byte-array call over `arrays` (one offset width): offsets and the byte count, then the bytes.
+        fn bytes_many(arrays: &[&dyn Array]) -> Result<ArrayRef, ArrowError> {
+            let ctx = Context::current()?;
+            let dt = arrays.first().map(|a| a.data_type().clone()).unwrap_or(DataType::Utf8);
+            let ob = if matches!(dt, DataType::LargeUtf8 | DataType::LargeBinary) { 8 } else { 4 };
+            let uploaded = arrays.iter().map(|a| DeviceArray::upload(&ctx, *a, false)).collect::<Result<Vec<_>, _>>()?;
+            let xs: Vec<ffi::acu_bytes_array> = uploaded.iter()
+                .map(|a| ffi::acu_bytes_array { offsets: a.view().values, data: a.column.data, nulls: *a.view() }).collect();
+            let n = arrays.first().map(|a| a.len()).unwrap_or(0);
+            let mut sizing = ColumnOut::new(&ctx, &dt, n, 0)?;
+            let mut total = 0i64;
+            ctx.check(unsafe { ffi::acu_concat_elements_bytes_many(ctx.raw(), ob, xs.len() as i32, xs.as_ptr(), sizing.out.array.values,
+                                                                   std::ptr::null_mut(), 0, &mut total, &mut sizing.out.array) })?;
+            let mut out = ColumnOut::new(&ctx, &dt, n, total as usize)?;
+            let (offs, data, cap) = (out.out.array.values, out.out.data, out.out.data_capacity);
+            ctx.check(unsafe { ffi::acu_concat_elements_bytes_many(ctx.raw(), ob, xs.len() as i32, xs.as_ptr(), offs, data, cap,
+                                                                   &mut out.out.data_len, &mut out.out.array) })?;
+            out.finish(&dt)
+        }
+
+        fn check_len(l: usize, r: usize) -> Result<(), ArrowError> {
+            if l != r { return Err(ArrowError::ComputeError(format!("Arrays must have the same length: {l} != {r}"))); }
+            Ok(())
+        }
+
+        /// `concat_elements_bytes` (:31-75).
+        pub fn concat_elements_bytes<T: types::ByteArrayType>(left: &GenericByteArray<T>, right: &GenericByteArray<T>)
+                                                               -> Result<GenericByteArray<T>, ArrowError> {
+            check_len(left.len(), right.len())?;
+            Ok(bytes_many(&[left as &dyn Array, right as &dyn Array])?.as_bytes::<T>().clone())
+        }
+        /// `concat_elements_utf8` (:91-96).
+        pub fn concat_elements_utf8<O: OffsetSizeTrait>(left: &GenericStringArray<O>, right: &GenericStringArray<O>)
+                                                         -> Result<GenericStringArray<O>, ArrowError> {
+            concat_elements_bytes(left, right)
+        }
+        /// `concat_element_binary` (:99-104).
+        pub fn concat_element_binary<O: OffsetSizeTrait>(left: &GenericBinaryArray<O>, right: &GenericBinaryArray<O>)
+                                                          -> Result<GenericBinaryArray<O>, ArrowError> {
+            concat_elements_bytes(left, right)
+        }
+        /// `concat_elements_utf8_many` (:113-173).
+        pub fn concat_elements_utf8_many<O: OffsetSizeTrait>(arrays: &[&GenericStringArray<O>]) -> Result<GenericStringArray<O>, ArrowError> {
+            let dyns: Vec<&dyn Array> = arrays.iter().map(|a| *a as &dyn Array).collect();
+            Ok(bytes_many(&dyns)?.as_string::<O>().clone())
+        }
+
+        /// `concat_elements_fixed_size_binary` (:181-228).
+        pub fn concat_elements_fixed_size_binary(left: &FixedSizeBinaryArray, right: &FixedSizeBinaryArray)
+                                                 -> Result<FixedSizeBinaryArray, ArrowError> {
+            let ctx = Context::current()?;
+            let (lw, rw) = (left.value_length(), right.value_length());
+            let mut bufs = Vec::new();
+            let l = fsb_operand(&ctx, left, lw.max(0) as usize, &mut bufs)?;
+            let r = fsb_operand(&ctx, right, rw.max(0) as usize, &mut bufs)?;
+            let n = left.len();
+            let w = (lw.max(0) as usize) + (rw.max(0) as usize);
+            let values = DeviceBuffer::allocate(&ctx, (n * w).max(1))?;
+            let validity = DeviceBuffer::allocate(&ctx, super::super::bitmap_bytes(n.max(1)))?;
+            let mut o = ffi::acu_array_out { values: values.as_ptr(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0,
+                                             has_validity: 0, reserved: 0 };
+            let mut width = 0i32;
+            ctx.check(unsafe { ffi::acu_concat_elements_fixed_size_binary(ctx.raw(), lw, &l, rw, &r, &mut width, &mut o) })?;
+            let d = ArrayData::builder(DataType::FixedSizeBinary(width)).len(n).nulls(nulls_of(&validity, &o, n)?)
+                .add_buffer(values.to_host(n * width as usize)?);
+            Ok(FixedSizeBinaryArray::from(unsafe { d.build_unchecked() }))
+        }
+
+        fn view_concat<T: ByteViewType + ?Sized>(left: &GenericByteViewArray<T>, right: &GenericByteViewArray<T>)
+                                                 -> Result<GenericByteViewArray<T>, ArrowError> {
+            let ctx = Context::current()?;
+            let (mut bufs, mut lp, mut rp) = (Vec::new(), Vec::new(), Vec::new());
+            let l = view_operand(&ctx, left, &mut bufs, &mut lp)?;
+            let r = view_operand(&ctx, right, &mut bufs, &mut rp)?;
+            let n = left.len();
+            let validity = DeviceBuffer::allocate(&ctx, super::super::bitmap_bytes(n.max(1)))?;
+            let mut o = ffi::acu_array_out { values: std::ptr::null_mut(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0,
+                                             has_validity: 0, reserved: 0 };
+            let mut total = 0i64;
+            ctx.check(unsafe { ffi::acu_concat_elements_byte_view(ctx.raw(), &l, &r, std::ptr::null_mut(), std::ptr::null_mut(), 0, &mut total,
+                                                                  &mut o) })?;
+            let views = DeviceBuffer::allocate(&ctx, n.max(1) * 16)?;
+            let data = DeviceBuffer::allocate(&ctx, (total as usize).max(1))?;
+            ctx.check(unsafe { ffi::acu_concat_elements_byte_view(ctx.raw(), &l, &r, views.as_ptr(), data.as_ptr() as *mut u8, total, &mut total,
+                                                                  &mut o) })?;
+            let v = ScalarBuffer::<u128>::new(views.to_host(n * 16)?, 0, n);
+            let buffers: Vec<Buffer> = if total > 0 { vec![data.to_host(total as usize)?] } else { vec![] };
+            Ok(unsafe { GenericByteViewArray::<T>::new_unchecked(v, buffers, nulls_of(&validity, &o, n)?) })
+        }
+        /// `concat_elements_binary_view_array` (:388-393).
+        pub fn concat_elements_binary_view_array(left: &BinaryViewArray, right: &BinaryViewArray) -> Result<BinaryViewArray, ArrowError> {
+            view_concat(left, right)
+        }
+        /// `concat_elements_string_view_array` (:402-407).
+        pub fn concat_elements_string_view_array(left: &StringViewArray, right: &StringViewArray) -> Result<StringViewArray, ArrowError> {
+            view_concat(left, right)
+        }
+
+        /// `concat_elements_dyn` (:419-476).
+        pub fn concat_elements_dyn(left: &dyn Array, right: &dyn Array) -> Result<ArrayRef, ArrowError> {
+            use DataType::*;
+            match (left.data_type(), right.data_type()) {
+                (Utf8, Utf8) => Ok(Arc::new(concat_elements_utf8(left.as_string::<i32>(), right.as_string::<i32>())?)),
+                (LargeUtf8, LargeUtf8) => Ok(Arc::new(concat_elements_utf8(left.as_string::<i64>(), right.as_string::<i64>())?)),
+                (Binary, Binary) => Ok(Arc::new(concat_element_binary(left.as_binary::<i32>(), right.as_binary::<i32>())?)),
+                (LargeBinary, LargeBinary) => Ok(Arc::new(concat_element_binary(left.as_binary::<i64>(), right.as_binary::<i64>())?)),
+                (Utf8View, Utf8View) => Ok(Arc::new(concat_elements_string_view_array(left.as_string_view(), right.as_string_view())?)),
+                (BinaryView, BinaryView) => Ok(Arc::new(concat_elements_binary_view_array(left.as_binary_view(), right.as_binary_view())?)),
+                (FixedSizeBinary(_), FixedSizeBinary(_)) => {
+                    Ok(Arc::new(concat_elements_fixed_size_binary(left.as_fixed_size_binary(), right.as_fixed_size_binary())?))
+                }
+                (l, r) if l != r => Err(ArrowError::ComputeError(format!("Cannot concat arrays of different types: {l} != {r}"))),
+                (l, _) => Err(ArrowError::NotYetImplemented(format!("concat not supported for {l}"))),
+            }
         }
     }
 

@@ -253,6 +253,9 @@ def main():
         # ---------------- length / substring (arrow-string/src/length.rs, substring.rs) ----------------
         if not b.only or any(t in "substring length" for t in b.only.split("|")):
             substring_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D)
+        # ---------------- concat_elements (arrow-string/src/concat_elements.rs) ----------------
+        if not b.only or any(t in "concat_elements" for t in b.only.split("|")):
+            concat_elements_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D)
     print("\n| op | rows | kernel ms | GB/s (algorithmic) | % of measured HBM peak | Mrows/s |")
     print("|---|---|---|---|---|---|")
     for r in b.rows:
@@ -493,6 +496,76 @@ def substring_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out
     ctx._free_out(ol)
     ctx._free_out(ovs)
     ctx._free_out(ovw)
+
+
+def concat_elements_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D):
+    """concat_elements(s, s), concat_elements_utf8_many(s, s, s), the view form on the same values and FixedSizeBinary 8 + 8, on
+    the dictionary-decoded Utf8 column of config 4 (D = 4096 values of 4..12 bytes, 5 % nulls). The yardstick is the same
+    bytes engine's copy, substring(s, 0, None), timed in the same run. A byte concat is timed as the sizing call plus the copy.
+    The three-operand row runs on the first half of the rows, since 3S passes i32::MAX.
+    Algorithmic bytes (DESIGN.md §3), S = the column's value bytes, K operands: K(4(N+1) + S) read + 4(N+1) + KS written +
+    (K + 1)N/8 validity; views: 2 x 16N read + 16N + L written (L = the bytes of the results longer than 12) + 3N/8;
+    FixedSizeBinary 8 + 8: 16N read + 16N written + 3N/8."""
+    lib, h = ctx.lib, ctx.h
+    total = C.c_int64(0)
+    ctx.check(lib.acu_take_bytes(h, 4, d_off, d_data, C.byref(dict_nulls), C.byref(keys), abi.I32, 0, d_out_off, d_out_data, ns * 13,
+                                 C.byref(total), C.byref(on)))
+    U = abi.BytesArray()
+    U.offsets, U.data = d_out_off, d_out_data
+    U.nulls = b.arr(None, on.validity, ns, on.null_count)
+    S = total.value
+    note = f"D={D}, lengths 4..12, 5% nulls, S = {S} bytes"
+    o_off, o_data = ctx.malloc((ns + 1) * 4 + 64), ctx.malloc(3 * S + 64)
+    onn = abi.ArrayOut()
+    onn.validity = ctx.malloc(abi.bitmap_bytes(ns) + 64)
+    out_len = C.c_int64(0)
+
+    def substring(cap, out):
+        ctx.check(lib.acu_substring_bytes(h, 4, 1, 0, 0, 0, C.byref(U), S, o_off, out, cap, C.byref(out_len), C.byref(onn)))
+    b.timed("concat_elements: yardstick substring(s, 0, None) utf8 dict-decoded", [abi.K_BYTES], 8 * (ns + 1) + 2 * S + 2 * ns / 8, ns,
+            lambda: (substring(0, None), substring(S, o_data)), note="the bytes engine's copy rate: sizing + copy call; " + note)
+
+    def pair(cap, out):
+        ctx.check(lib.acu_concat_elements_bytes(h, 4, C.byref(U), C.byref(U), o_off, out, cap, C.byref(out_len), C.byref(onn)))
+    b.timed("concat_elements: concat_elements(s, s) utf8 dict-decoded", [abi.K_BYTES], 3 * 4 * (ns + 1) + 4 * S + 3 * ns / 8, ns,
+            lambda: (pair(0, None), pair(2 * S, o_data)), note="sizing + copy call; " + note)
+    # three operands over the whole column would pass i32::MAX (3S > 2^31): the first half of the rows
+    nh = ns // 2
+    Uh = abi.BytesArray()
+    Uh.offsets, Uh.data = d_out_off, d_out_data
+    Uh.nulls = b.arr(None, on.validity, nh, -1)
+    three = (abi.BytesArray * 3)(Uh, Uh, Uh)
+
+    def many(cap, out):
+        ctx.check(lib.acu_concat_elements_bytes_many(h, 4, 3, three, o_off, out, cap, C.byref(out_len), C.byref(onn)))
+    many(0, None)
+    Sh = out_len.value // 3
+    b.timed("concat_elements: concat_elements_utf8_many(s, s, s) utf8 dict-decoded", [abi.K_BYTES], 4 * 4 * (nh + 1) + 6 * Sh + 4 * nh / 8, nh,
+            lambda: (many(0, None), many(3 * Sh, o_data)), note=f"sizing + copy call; the first {nh} rows, S = {Sh} bytes")
+    ctx.free(o_off)
+    V, ovw = dict_view_column(b, ctx, keys, offs, data, D, ns)
+    ovs = b.out(ns * 16, ns)
+    ctx.check(lib.acu_concat_elements_byte_view(h, C.byref(V), C.byref(V), None, None, 0, C.byref(out_len), C.byref(ovs)))
+    L = out_len.value
+
+    def views(cap, vo, out):
+        ctx.check(lib.acu_concat_elements_byte_view(h, C.byref(V), C.byref(V), vo, out, cap, C.byref(out_len), C.byref(ovs)))
+    b.timed("concat_elements: concat_elements(v, v) view dict-decoded", [abi.K_BYTES], 48 * ns + L + 3 * ns / 8, ns,
+            lambda: (views(0, None, None), views(L, ovs.values, o_data)), note=f"sizing + copy call; L = {L} bytes of long results")
+    ctx._free_out(ovs)
+    ctx._free_out(ovw)
+    ctx.free(o_data)
+    fl, fr = b.gen(1, 50, ns, 8), b.gen(1, 51, ns, 8)
+    vr, nvr = b.bits(52, 0.95, ns)
+    FL, FR = b.arr(fl, on.validity, ns, on.null_count), b.arr(fr, vr, ns, ns - nvr)
+    of = b.out(ns * 16, ns)
+    w = C.c_int32(0)
+    b.timed("concat_elements: fixed_size_binary 8 + 8", [abi.K_BYTES], 32 * ns + 3 * ns / 8, ns,
+            lambda: ctx.check(lib.acu_concat_elements_fixed_size_binary(h, 8, C.byref(FL), 8, C.byref(FR), C.byref(w), C.byref(of))),
+            note="5% nulls on each side")
+    for p in (fl, fr, vr, onn.validity):
+        ctx.free(p)
+    ctx._free_out(of)
 
 
 def like_rows(b, ctx, ns, d_off, d_data, keys, dict_nulls, d_out_off, d_out_data, on, offs, data, D):
