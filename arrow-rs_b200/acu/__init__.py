@@ -362,6 +362,32 @@ class FixedSizeBinaryColumn:
         return FixedSizeBinaryColumn(vals, nulls)
 
 
+class ListColumn:
+    """A List (np.int32 offsets) / LargeList (np.int64) column on the host (GenericListArray,
+    arrow-array/src/array/list_array.rs): `offsets` has rows + 1 entries from logical row 0 and holds ABSOLUTE child rows
+    (a sliced list has offsets[0] != 0), `child` is a HostArray, Utf8Column, ViewColumn or list column, `nulls` a HostArray
+    carrying validity / length."""
+
+    def __init__(self, offsets, child, nulls):
+        self.offsets, self.child, self.nulls = offsets, child, nulls
+
+    @property
+    def length(self):
+        return len(self.offsets) - 1
+
+
+class FixedSizeListColumn:
+    """A FixedSizeList(size) column on the host (FixedSizeListArray): row i is child rows [i * size, (i + 1) * size); the
+    child starts at the list's logical row 0."""
+
+    def __init__(self, size, child, nulls):
+        self.size, self.child, self.nulls = size, child, nulls
+
+    @property
+    def length(self):
+        return self.nulls.length
+
+
 def column_value(col, row):
     """The bytes of logical row `row` of a Utf8Column / ViewColumn / FixedSizeBinaryColumn (`array.value(row)`)."""
     if isinstance(col, Utf8Column):
@@ -1698,3 +1724,245 @@ class Context:
     def max_boolean(self, a): return self._boolean_value(MAX, a)
     def bool_and(self, a): return self._boolean_value(MIN, a)
     def bool_or(self, a): return self._boolean_value(MAX, a)
+
+
+    # -- List / LargeList / FixedSizeList (filter.rs:535-625, take.rs:646-795) -----------------
+    # One C call per level: the list call returns the child's plan / row map, and the child is filtered / taken with it
+    # through the entry point of its own type (the list calls again for a nested list).
+    def _list_descriptor(self, col, owned):
+        d = abi.ListArray()
+        if isinstance(col, FixedSizeListColumn):
+            d.kind, d.list_size = abi.FIXED_SIZE_LIST, col.size
+        else:
+            d.kind = abi.LARGE_LIST if col.offsets.dtype == np.int64 else abi.LIST
+            off = np.ascontiguousarray(col.offsets)
+            d.offsets = self.malloc(off.nbytes + 16)
+            owned.append(d.offsets)
+            self.h2d(d.offsets, off)
+        d.nulls = self._upload_nulls(col.nulls, owned)
+        d.child_len = col.child.length
+        return d
+
+    def _nulls_out(self, out, n):
+        validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+        return HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0)
+
+    def filter_list(self, col, predicate):
+        """arrow::compute::filter of a ListColumn / FixedSizeListColumn (any nesting of the supported children)."""
+        dp = self.upload(predicate)
+        plan = C.c_void_p()
+        try:
+            pd = dp.descriptor()
+            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
+            return self._filter_with_plan(col, plan)
+        finally:
+            if plan:
+                self.lib.acu_filter_plan_destroy(self.h, plan)
+            dp.free()
+
+    def _filter_with_plan(self, col, plan):
+        count = self.lib.acu_filter_plan_count(plan)
+        owned, out = [], None
+        try:
+            if isinstance(col, (ListColumn, FixedSizeListColumn)):
+                d = self._list_descriptor(col, owned)
+                fixed = isinstance(col, FixedSizeListColumn)
+                d_off = None if fixed else self.malloc((count + 1) * col.offsets.itemsize + 16)
+                if d_off:
+                    owned.append(d_off)
+                out = self.alloc_out(0, count)
+                child_plan = C.c_void_p()
+                self.check(self.lib.acu_filter_list(self.h, plan, C.byref(d), d_off, C.byref(out), C.byref(child_plan)))
+                try:
+                    child = self._filter_with_plan(col.child, child_plan)
+                finally:
+                    self.lib.acu_filter_plan_destroy(self.h, child_plan)
+                nulls = self._nulls_out(out, count)
+                if fixed:
+                    return FixedSizeListColumn(col.size, child, nulls)
+                return ListColumn(self.d2h(d_off, (count + 1) * col.offsets.itemsize, col.offsets.dtype), child, nulls)
+            if isinstance(col, Utf8Column):
+                bd = self._upload_bytes_col(col, owned)
+                ob = col.offsets.dtype.itemsize
+                d_off = self.malloc((count + 1) * ob + 16)
+                owned.append(d_off)
+                out = self.alloc_out(0, count)
+                total = C.c_int64(0)
+                self.check(self.lib.acu_filter_bytes(self.h, plan, ob, bd.offsets, bd.data, C.byref(bd.nulls), d_off, None, 0,
+                                                     C.byref(total), C.byref(out)))
+                d_data = self.malloc(total.value + 16)
+                owned.append(d_data)
+                self.check(self.lib.acu_filter_bytes(self.h, plan, ob, bd.offsets, bd.data, C.byref(bd.nulls), d_off, d_data,
+                                                     total.value, C.byref(total), C.byref(out)))
+                return Utf8Column(self.d2h(d_off, (count + 1) * ob, col.offsets.dtype), self.d2h(d_data, total.value),
+                                  self._nulls_out(out, count))
+            if isinstance(col, ViewColumn):  # the views filter as 16-byte values; the data buffers are shared
+                keep = []
+                vd = self._upload_view_col(col, owned, keep)
+                arr = vd.nulls
+                arr.values = vd.views
+                out = self.alloc_out(count * 16, count)
+                self.check(self.lib.acu_filter_primitive(self.h, plan, 16, C.byref(arr), C.byref(out)))
+                views = self.d2h(out.values, count * 16).reshape(-1, 16)
+                return ViewColumn(views, col.buffers, self._nulls_out(out, count))
+            dv = self.upload(col)
+            owned_arr = dv
+            try:
+                out = self.alloc_out(count * col.width(), count)
+                vd = dv.descriptor()
+                if col.dtype == BOOL:
+                    self.check(self.lib.acu_filter_boolean(self.h, plan, C.byref(vd), C.byref(out)))
+                else:
+                    self.check(self.lib.acu_filter_primitive(self.h, plan, col.width(), C.byref(vd), C.byref(out)))
+                res, out = self.download_out(out, col.dtype), None
+                return col.like(res) if isinstance(col, DecimalArray) else res
+            finally:
+                owned_arr.free()
+        finally:
+            if out is not None:
+                self._free_out(out)
+            for p in owned:
+                self.free(p)
+
+    def take_list(self, col, indices, check_bounds=False):
+        """arrow::compute::take of a ListColumn / FixedSizeListColumn by a HostArray of integer indices."""
+        di = self.upload(indices)
+        try:
+            idd = di.descriptor()
+            return self._take_level(col, idd, indices.dtype, check_bounds, False)
+        finally:
+            di.free()
+
+    def _child_error_first(self, col, d, idd, index_dtype, row, owned):
+        """The List `col` (descriptor d) passes i32::MAX at output row `row`. The reference extends the child of rows
+        0 ..= row before it unwraps that row's offset, so the child's own offset overflow comes first: raise it if there is
+        one (the caller then raises the panic)."""
+        if isinstance(col.child, (HostArray, ViewColumn)):
+            return
+        head = abi.Array.from_buffer_copy(idd)
+        head.len = row
+        rmap, _, _, _, cdt, _, _ = self._row_map(d, head, index_dtype, False, False, row, owned)
+        n0 = self._last_rows
+        raw = self.d2h(idd.values + row * abi.DTYPE_SIZE[index_dtype], abi.DTYPE_SIZE[index_dtype], NP_DTYPES[index_dtype])
+        ix = int(raw[0]) & (0xFFFFFFFF if index_dtype in (abi.I8, abi.I16, abi.I32) else 0xFFFFFFFFFFFFFFFF)
+        w = abi.DTYPE_SIZE[cdt]
+        extra = np.arange(int(col.offsets[ix]), int(col.offsets[ix + 1]), dtype=NP_DTYPES[cdt])
+        full = self.malloc((n0 + len(extra)) * w + 16)
+        owned.append(full)
+        if n0:
+            self.check(self.lib.acu_memcpy_d2d(self.h, full, rmap, n0 * w))
+        if len(extra):
+            self.h2d(full + n0 * w, extra)
+        cd = abi.Array()
+        cd.values, cd.len = full, n0 + len(extra)
+        self._take_level(col.child, cd, cdt, False, True)
+
+    def _row_map(self, d, idd, index_dtype, check_bounds, keep, m, owned):
+        """acu_take_list both phases: (device row map, out ArrayOut of the list nulls, device offsets or None, child-index
+        ArrayOut, row map dtype, offset width, a FixedSizeList's take_bits panic deferred behind its child)."""
+        fixed = d.kind == abi.FIXED_SIZE_LIST
+        ob = 0 if fixed else (8 if d.kind == abi.LARGE_LIST else 4)
+        d_off = self.malloc((m + 1) * max(ob, 1) + 16)
+        owned.append(d_off)
+        out = self.alloc_out(0, m)
+        owned += [out.values, out.validity]
+        cdt = abi.U32 if fixed or d.child_len <= 0xFFFFFFFF else abi.U64
+        rows = C.c_int64(0)
+        cn = abi.ArrayOut()
+        self.check(self.lib.acu_take_list(self.h, C.byref(d), C.byref(idd), index_dtype, int(check_bounds), int(keep), d_off, C.byref(out),
+                                          cdt, None, 0, C.byref(rows), C.byref(cn)))
+        n = rows.value
+        rmap = self.malloc(n * abi.DTYPE_SIZE[cdt] + 16)
+        owned.append(rmap)
+        cn.validity = self.malloc(bitmap_bytes(n) + 8)
+        owned.append(cn.validity)
+        deferred = None
+        try:
+            self.check(self.lib.acu_take_list(self.h, C.byref(d), C.byref(idd), index_dtype, int(check_bounds), int(keep), d_off,
+                                              C.byref(out), cdt, rmap, n, C.byref(rows), C.byref(cn)))
+        except ArrowError as e:
+            if not fixed or e.status != abi.ERR_PANIC_OUT_OF_BOUNDS:
+                raise
+            deferred = e
+        self._last_rows = n
+        return rmap, out, (d_off if ob else None), cn, cdt, ob, deferred
+
+    def _take_level(self, col, idd, index_dtype, check_bounds, keep, host_map=None):
+        """Take `col` by the device indices `idd` (or the host row map `host_map`). keep: this level is a child step of a
+        List / LargeList take (MutableArrayData::extend: every row keeps its range or bytes)."""
+        owned, dh = [], None
+        try:
+            if host_map is not None:
+                dh = self.upload(HostArray.from_numpy(index_dtype, host_map))
+                idd = dh.descriptor()
+            m = idd.len
+            if isinstance(col, (ListColumn, FixedSizeListColumn)):
+                d = self._list_descriptor(col, owned)
+                try:
+                    rmap, out, d_off, cn, cdt, ob, deferred = self._row_map(d, idd, index_dtype, check_bounds, keep, m, owned)
+                except ArrowError as e:
+                    if e.status == abi.ERR_PANIC_OUT_OF_BOUNDS and e.message.startswith("called `Option::unwrap()`"):
+                        self._child_error_first(col, d, idd, index_dtype, e.index, owned)
+                    raise
+                n = self._last_rows
+                cd = abi.Array()
+                cd.values, cd.len = rmap, n
+                if cn.has_validity:
+                    cd.validity, cd.null_count = cn.validity, cn.null_count
+                # a List's child is extended (MutableArrayData); a FixedSizeList's child is taken (take_impl)
+                child = self._take_level(col.child, cd, cdt, False, keep or ob != 0)
+                if deferred is not None:  # take_fixed_size_list: the child's take ran first and did not fail
+                    raise deferred
+                nulls = self._nulls_out(out, m)
+                if not ob:
+                    return FixedSizeListColumn(col.size, child, nulls)
+                return ListColumn(self.d2h(d_off, (m + 1) * ob, np.int32 if ob == 4 else np.int64), child, nulls)
+            if isinstance(col, Utf8Column):
+                bd = self._upload_bytes_col(col, owned)
+                ob = col.offsets.dtype.itemsize
+                d_off = self.malloc((m + 1) * ob + 16)
+                owned.append(d_off)
+                out = self.alloc_out(0, m)
+                owned += [out.values, out.validity]
+                total = C.c_int64(0)
+
+                def call(d_data, cap):
+                    if keep:
+                        return self.lib.acu_take_bytes_extend(self.h, ob, bd.offsets, bd.data, C.byref(bd.nulls), C.byref(idd), index_dtype,
+                                                              d_off, d_data, cap, C.byref(total), C.byref(out))
+                    return self.lib.acu_take_bytes(self.h, ob, bd.offsets, bd.data, C.byref(bd.nulls), C.byref(idd), index_dtype,
+                                                   int(check_bounds), d_off, d_data, cap, C.byref(total), C.byref(out))
+                self.check(call(None, 0))
+                d_data = self.malloc(total.value + 16)
+                owned.append(d_data)
+                self.check(call(d_data, total.value))
+                return Utf8Column(self.d2h(d_off, (m + 1) * ob, col.offsets.dtype), self.d2h(d_data, total.value), self._nulls_out(out, m))
+            if isinstance(col, ViewColumn):  # the views take as 16-byte values; the data buffers are shared
+                keep_tables = []
+                vd = self._upload_view_col(col, owned, keep_tables)
+                arr = vd.nulls
+                arr.values = vd.views
+                out = self.alloc_out(m * 16, m)
+                owned += [out.values, out.validity]
+                self.check(self.lib.acu_take_primitive(self.h, 16, C.byref(arr), C.byref(idd), index_dtype, int(check_bounds), C.byref(out)))
+                return ViewColumn(self.d2h(out.values, m * 16).reshape(-1, 16), col.buffers, self._nulls_out(out, m))
+            dv = self.upload(col)
+            try:
+                out = self.alloc_out(m * col.width(), m)
+                vd = dv.descriptor()
+                if col.dtype == BOOL:
+                    st = self.lib.acu_take_boolean(self.h, C.byref(vd), C.byref(idd), index_dtype, int(check_bounds), C.byref(out))
+                else:
+                    st = self.lib.acu_take_primitive(self.h, col.width(), C.byref(vd), C.byref(idd), index_dtype, int(check_bounds), C.byref(out))
+                if st != abi.OK:
+                    self._free_out(out)
+                    self.check(st)
+                res = self.download_out(out, col.dtype)
+                return col.like(res) if isinstance(col, DecimalArray) else res
+            finally:
+                dv.free()
+        finally:
+            for p in owned:
+                self.free(p)
+            if dh is not None:
+                dh.free()

@@ -103,6 +103,14 @@ class ViewArray(C.Structure):
     _fields_ = [("views", C.c_void_p), ("buffers", C.POINTER(C.c_void_p)), ("n_buffers", C.c_int32), ("reserved", C.c_int32), ("nulls", Array)]
 
 
+LIST, LARGE_LIST, FIXED_SIZE_LIST = range(3)
+
+
+class ListArray(C.Structure):
+    """acu_list_array: one level of a List / LargeList / FixedSizeList column (the child is described separately)."""
+    _fields_ = [("kind", C.c_int32), ("list_size", C.c_int32), ("offsets", C.c_void_p), ("nulls", Array), ("child_len", C.c_int64)]
+
+
 COL_PRIMITIVE, COL_BOOLEAN, COL_BYTES = range(3)
 BOOL_AND, BOOL_OR, BOOL_AND_NOT, BOOL_AND_KLEENE, BOOL_OR_KLEENE, BOOL_NOT, BOOL_IS_NULL, BOOL_IS_NOT_NULL = range(8)
 MAX_BATCH_COLUMNS = 64
@@ -211,6 +219,9 @@ PROTOTYPES = {
     "acu_take_primitive": (i32, [vp, i32, P(Array), P(Array), i32, i32, P(ArrayOut)]),
     "acu_take_boolean": (i32, [vp, P(Array), P(Array), i32, i32, P(ArrayOut)]),
     "acu_take_bytes": (i32, [vp, i32, vp, vp, P(Array), P(Array), i32, i32, vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_take_bytes_extend": (i32, [vp, i32, vp, vp, P(Array), P(Array), i32, vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_filter_list": (i32, [vp, vp, P(ListArray), vp, P(ArrayOut), P(vp)]),
+    "acu_take_list": (i32, [vp, P(ListArray), P(Array), i32, i32, i32, vp, P(ArrayOut), i32, vp, i64, P(i64), P(ArrayOut)]),
     "acu_arith": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_bitwise": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_neg": (i32, [vp, i32, i32, P(Array), P(ArrayOut)]),

@@ -34,18 +34,6 @@
 
 namespace {
 
-// kind: acu_take_index_kind of the index type
-__device__ __forceinline__ uint64_t ld_index(const void *idx, int kind, int64_t j) {
-  switch (kind) {
-    case 0: return __ldg(static_cast<const uint8_t *>(idx) + j);
-    case 1: return (uint64_t)(uint32_t)(int32_t)__ldg(static_cast<const int8_t *>(idx) + j);
-    case 2: return __ldg(static_cast<const uint16_t *>(idx) + j);
-    case 3: return (uint64_t)(uint32_t)(int32_t)__ldg(static_cast<const int16_t *>(idx) + j);
-    case 4: return __ldg(static_cast<const uint32_t *>(idx) + j);
-    default: return __ldg(static_cast<const uint64_t *>(idx) + j);
-  }
-}
-
 // ---- device-wide inclusive scan of int64 (in place) ------------------------------------
 __global__ void __launch_bounds__(1024) k_scan_block(int64_t *__restrict__ data, int64_t n, int64_t *__restrict__ block_tot) {
   __shared__ uint64_t warp_tot[33];
@@ -794,6 +782,8 @@ acu_status gather_finalize(acu_ctx *ctx, const acu_bytes_col_state &gs, const un
                INT64_MAX, j, ctx->d_res, 0, static_cast<const int64_t *>(nullptr), (int64_t)0);
     ACU_TRY(acu_res_fetch(ctx));
     const long long cap = (long long)ctx->h_res[RES_AUX1];
+    if (gs.extend)  // try_extend_offsets (arrow-data/src/transform/utils.rs)
+      return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, j, 0, 0, (uint64_t)cap, "%s", acu_extend_overflow_text);
     return acu_fail(ctx, ACU_ERR_OFFSET_OVERFLOW, j, 0, 0, (uint64_t)cap, "%lld", cap);
   }
   if (gs.out_data && *out_len > gs.out_cap)
@@ -930,8 +920,9 @@ size_t acu_bytes_col_scratch(int64_t out_rows) { return gather_scratch_bytes(out
 acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const uint8_t *data, const acu_array *nulls_of,
                                      bool val_nulls, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls,
                                      void *out_offsets, uint8_t *out_data, int64_t out_cap, acu_array_out *out_nulls, void *scratch,
-                                     unsigned long long *res, acu_bytes_col_state *st) {
+                                     unsigned long long *res, acu_bytes_col_state *st, bool extend) {
   *st = acu_bytes_col_state();
+  st->extend = extend;
   ACU_TRY(acu_offset_width_check(ctx, ob));
   ACU_TRY(offsets_aligned(ctx, ob, offsets, out_offsets));
   const int64_t m = indices->len;
@@ -941,7 +932,7 @@ acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offse
   if (m == 0) return zero_first_offset(ctx, out_offsets, ob);
   const uint8_t *ov = nullptr;
   if (val_nulls) {
-    ov = out_nulls->validity;  // take_bits(values.nulls), gathered by acu_take_cols_launch
+    if (!extend) ov = out_nulls->validity;  // take_bits(values.nulls), gathered by acu_take_cols_launch
   } else if (indices->validity) {
     // values without nulls: take_nulls = indices.nulls().cloned() (take.rs:429) is a bitmap copy, and the
     // out-of-bounds check rides in the first bytes pass — no separate gather pass.

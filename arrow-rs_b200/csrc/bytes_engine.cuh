@@ -32,6 +32,18 @@ struct has_segments : std::false_type {};
 template <class R>
 struct has_segments<R, std::void_t<decltype(std::declval<const R &>().nsegs())>> : std::true_type {};
 
+// kind: acu_take_index_kind of the index type
+__device__ __forceinline__ uint64_t ld_index(const void *idx, int kind, int64_t j) {
+  switch (kind) {
+    case 0: return __ldg(static_cast<const uint8_t *>(idx) + j);
+    case 1: return (uint64_t)(uint32_t)(int32_t)__ldg(static_cast<const int8_t *>(idx) + j);
+    case 2: return __ldg(static_cast<const uint16_t *>(idx) + j);
+    case 3: return (uint64_t)(uint32_t)(int32_t)__ldg(static_cast<const int16_t *>(idx) + j);
+    case 4: return __ldg(static_cast<const uint32_t *>(idx) + j);
+    default: return __ldg(static_cast<const uint64_t *>(idx) + j);
+  }
+}
+
 // CTA-wide exclusive scan of one u64 per thread (up to 1024 threads); returns the thread's exclusive
 // prefix, *total = the CTA total. Two barriers.
 __device__ __forceinline__ uint64_t cta_scan_excl(uint64_t v, uint64_t *warp_tot /* [33] shared */, uint64_t *total) {

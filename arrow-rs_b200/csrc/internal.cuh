@@ -67,6 +67,7 @@ acu_status acu_reduce_cols_launch(acu_ctx *ctx, int n, const acu_dtype *dtypes, 
 struct acu_bytes_col_state {
   bool gathered = false;          // the offsets / bytes gather was queued (output rows > 0)
   bool idx_nulls_copied = false;  // take: the output validity is a copy of the indices' (valid count in RES_COUNT)
+  bool extend = false;            // MutableArrayData::extend: null rows keep their bytes, overflow is try_extend_offsets'
   // the gather's arguments, for the finaliser's offset-overflow diagnosis and capacity check
   int32_t ob = 0;
   int kind = 0;
@@ -80,11 +81,12 @@ struct acu_bytes_col_state {
   int64_t out_cap = 0;
 };
 size_t acu_bytes_col_scratch(int64_t out_rows);
+extern const char *const acu_extend_overflow_text;  // try_extend_offsets' InvalidArgumentError (list.cu)
 acu_status acu_plan_cached_indices(acu_ctx *ctx, const acu_filter_plan *plan, const void **out_idx, int *out_kind);
 acu_status acu_take_bytes_col_launch(acu_ctx *ctx, int32_t ob, const void *offsets, const uint8_t *data, const acu_array *nulls_of,
                                      bool val_nulls, const acu_array *indices, acu_dtype index_dtype, bool idx_nulls,
                                      void *out_offsets, uint8_t *out_data, int64_t out_cap, acu_array_out *out_nulls, void *scratch,
-                                     unsigned long long *res, acu_bytes_col_state *st);
+                                     unsigned long long *res, acu_bytes_col_state *st, bool extend = false);
 acu_status acu_take_bytes_col_finalize(acu_ctx *ctx, const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype,
                                        const acu_bytes_col_state *st, const unsigned long long *hres, int64_t *out_data_len,
                                        acu_array_out *out_nulls);

@@ -81,7 +81,7 @@ acu_status filter_columns(acu_ctx *ctx, const acu_filter_plan *plan, int32_t n_c
 }
 
 acu_status take_columns(acu_ctx *ctx, int32_t n_columns, const acu_column *columns, const acu_array *indices, acu_dtype index_dtype,
-                        int32_t check_bounds, acu_column_out *outs) {
+                        int32_t check_bounds, acu_column_out *outs, bool extend = false) {
   if (n_columns < 0 || n_columns > ACU_MAX_BATCH_COLUMNS) return bad_columns(ctx, n_columns);
   if (n_columns == 0) return ACU_OK;
   if (acu_take_index_kind(index_dtype) < 0)  // take.rs:103
@@ -143,7 +143,7 @@ acu_status take_columns(acu_ctx *ctx, int32_t n_columns, const acu_column *colum
     if (col.kind != ACU_COL_BYTES) continue;
     st = acu_take_bytes_col_launch(ctx, col.width, col.array.values, col.data, &col.array, val_nulls[c], indices, index_dtype, idx_nulls,
                                    outs[c].array.values, outs[c].data, outs[c].data_capacity, &outs[c].array, scratch + per_col * k++,
-                                   acu_dres(ctx, c), &bstate[c]);
+                                   acu_dres(ctx, c), &bstate[c], extend);
     if (st != ACU_OK) return drain(ctx, st);
   }
   ACU_TRY(acu_res_fetch_n(ctx, n_columns));
@@ -219,6 +219,23 @@ extern "C" acu_status acu_take_bytes(acu_ctx *ctx, int32_t offset_bytes, const v
   const acu_column col = bytes_column(offset_bytes, offsets, data, nulls_of);
   acu_column_out out = bytes_column_out(out_offsets, out_data, out_data_capacity, out_nulls);
   const acu_status st = take_columns(ctx, 1, &col, indices, index_dtype, check_bounds, &out);
+  return bytes_result(out, st, out_data_len, out_nulls);
+}
+
+extern "C" acu_status acu_take_bytes_extend(acu_ctx *ctx, int32_t offset_bytes, const void *offsets, const uint8_t *data,
+                                            const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype, void *out_offsets,
+                                            uint8_t *out_data, int64_t out_data_capacity, int64_t *out_data_len, acu_array_out *out_nulls) {
+  ACU_ENTER(ctx);
+  ACU_TRY(acu_sync_only(ctx));
+  if (indices->validity && indices->len > 0) {
+    acu_status st;
+    const int64_t nc = acu_resolve_null_count(ctx, indices, &st);
+    ACU_TRY(st);
+    if (nc > 0) return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "take_bytes_extend: the row map has a null");
+  }
+  const acu_column col = bytes_column(offset_bytes, offsets, data, nulls_of);
+  acu_column_out out = bytes_column_out(out_offsets, out_data, out_data_capacity, out_nulls);
+  const acu_status st = take_columns(ctx, 1, &col, indices, index_dtype, 0, &out, true);
   return bytes_result(out, st, out_data_len, out_nulls);
 }
 

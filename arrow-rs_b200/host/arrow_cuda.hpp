@@ -141,7 +141,8 @@ inline std::vector<uint8_t> pack_bits(const std::vector<bool> &bits) {
 // ---------------------------------------------------------------------------------------
 // DataType / native type traits (arrow-array/src/types.rs:67-80)
 // ---------------------------------------------------------------------------------------
-enum class DataType { Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Boolean, Utf8, Decimal32, Decimal64, Decimal128 };
+enum class DataType { Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Boolean, Utf8, Decimal32, Decimal64, Decimal128,
+                      List, LargeList, FixedSizeList };
 
 template <class T> struct NativeOf;
 #define ACU_NATIVE(T, DT, CODE) \
@@ -465,6 +466,62 @@ class StringArray : public Array {
   Buffer offsets_, data_;
 };
 
+// GenericListArray<O> (arrow-array/src/array/list_array.rs): len + 1 offsets from logical row 0, ABSOLUTE rows of the child
+// `values` (a slice keeps the whole child), and the nulls. ListArray = i32 offsets, LargeListArray = i64.
+template <class O>
+class GenericListArray : public Array {
+ public:
+  GenericListArray(Buffer offsets, ArrayRef values, int64_t len, std::optional<NullBuffer> nulls)
+      : offsets_(std::move(offsets)), values_(std::move(values)) { len_ = len; nulls_ = std::move(nulls); }
+  // GenericListArray::new(field, OffsetBuffer, values, nulls)
+  static GenericListArray from(const std::vector<O> &offsets, ArrayRef values, const std::vector<bool> &valid = {}) {
+    return GenericListArray(Buffer::from_host(offsets.data(), offsets.size() * sizeof(O)), std::move(values), (int64_t)offsets.size() - 1,
+                            valid.empty() ? std::nullopt : nulls_from_mask(valid));
+  }
+  DataType data_type() const override { return sizeof(O) == 4 ? DataType::List : DataType::LargeList; }
+  const Buffer &offsets() const { return offsets_; }
+  const ArrayRef &values() const { return values_; }
+  std::vector<O> value_offsets() const {
+    std::vector<O> v((size_t)len_ + 1);
+    offsets_.to_host(v.data(), v.size() * sizeof(O));
+    return v;
+  }
+  GenericListArray slice(int64_t offset, int64_t length) const {  // Array::slice
+    GenericListArray out(Buffer(), values_, length, nulls_);
+    std::vector<O> o = value_offsets();
+    out.offsets_ = Buffer::from_host(o.data() + offset, (size_t)(length + 1) * sizeof(O));
+    if (out.nulls_) { out.nulls_->offset += offset; out.nulls_->len = length; out.nulls_->null_count = -1; }
+    return out;
+  }
+ protected:
+  const void *values_ptr() const override { return nullptr; }
+ private:
+  Buffer offsets_;
+  ArrayRef values_;
+};
+using ListArray = GenericListArray<int32_t>;
+using LargeListArray = GenericListArray<int64_t>;
+
+// FixedSizeListArray (arrow-array/src/array/fixed_size_list_array.rs): row i is values rows [i * size, (i + 1) * size).
+class FixedSizeListArray : public Array {
+ public:
+  FixedSizeListArray(int32_t size, ArrayRef values, int64_t len, std::optional<NullBuffer> nulls)
+      : size_(size), values_(std::move(values)) { len_ = len; nulls_ = std::move(nulls); }
+  // FixedSizeListArray::new(field, size, values, nulls)
+  static FixedSizeListArray from(int32_t size, ArrayRef values, const std::vector<bool> &valid = {}) {
+    const int64_t len = size ? values->len() / size : (int64_t)valid.size();
+    return FixedSizeListArray(size, std::move(values), len, valid.empty() ? std::nullopt : nulls_from_mask(valid));
+  }
+  DataType data_type() const override { return DataType::FixedSizeList; }
+  int32_t value_length() const { return size_; }
+  const ArrayRef &values() const { return values_; }
+ protected:
+  const void *values_ptr() const override { return nullptr; }
+ private:
+  int32_t size_;
+  ArrayRef values_;
+};
+
 // Datum (arrow-array/src/scalar.rs:78-152): an array, or a Scalar wrapping a 1-element array
 template <class A>
 struct Scalar {
@@ -552,7 +609,7 @@ inline ArrayRef make_primitive(DataType dt, Buffer values, int64_t len, std::opt
 }
 inline const char *dtype_display(DataType t) {
   static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64", "Boolean", "Utf8",
-                            "Decimal32", "Decimal64", "Decimal128"};
+                            "Decimal32", "Decimal64", "Decimal128", "List", "LargeList", "FixedSizeList"};
   return n[(int)t];
 }
 template <class A> std::string type_text(const A &a) {
@@ -771,6 +828,154 @@ inline Result<ArrayRef> take(const Array &values, const Array &indices, std::opt
   acu_array_out o = detail::make_out(vb, nb, (size_t)m * w, m);
   if ((st = acu_take_primitive(c.raw(), w, &v, &ix, (acu_dtype)dtype_code(it), cb, &o)) != ACU_OK) return c.last_error(st);
   return detail::make_primitive(values.data_type(), vb, o.len, detail::out_nulls(o, nb));
+}
+
+// ---- filter / take of List, LargeList, FixedSizeList (filter.rs:535-625, take.rs:646-795) ---------------------------------
+// One C call per level: acu_filter_list / acu_take_list return the child's plan / row map, and the child goes through the
+// entry point of its own type (the list calls again for a nested list). A List's child is extended (MutableArrayData: a
+// Utf8 child keeps the bytes under its null rows, acu_take_bytes_extend); a FixedSizeList's child is taken.
+// Not reproduced here: when a List's i32 offsets and its child's both overflow, this mirror reports the List's unwrap panic
+// (the Python layer reports the child's error first, as the reference does).
+namespace detail {
+inline acu_list_array list_view(const Array &a) {
+  acu_list_array l{};
+  l.nulls = a.view();
+  l.nulls.values = nullptr;
+  if (a.data_type() == DataType::FixedSizeList) {
+    const auto &f = static_cast<const FixedSizeListArray &>(a);
+    l.kind = ACU_FIXED_SIZE_LIST;
+    l.list_size = f.value_length();
+    l.child_len = f.values()->len();
+  } else if (a.data_type() == DataType::List) {
+    const auto &g = static_cast<const ListArray &>(a);
+    l.kind = ACU_LIST;
+    l.offsets = g.offsets().data();
+    l.child_len = g.values()->len();
+  } else {
+    const auto &g = static_cast<const LargeListArray &>(a);
+    l.kind = ACU_LARGE_LIST;
+    l.offsets = g.offsets().data();
+    l.child_len = g.values()->len();
+  }
+  return l;
+}
+inline bool is_list(DataType t) { return t == DataType::List || t == DataType::LargeList || t == DataType::FixedSizeList; }
+inline const ArrayRef &list_values(const Array &a) {
+  if (a.data_type() == DataType::FixedSizeList) return static_cast<const FixedSizeListArray &>(a).values();
+  if (a.data_type() == DataType::List) return static_cast<const ListArray &>(a).values();
+  return static_cast<const LargeListArray &>(a).values();
+}
+inline ArrayRef list_like(const Array &a, Buffer offsets, ArrayRef child, int64_t len, std::optional<NullBuffer> nulls) {
+  if (a.data_type() == DataType::FixedSizeList)
+    return std::make_shared<FixedSizeListArray>(static_cast<const FixedSizeListArray &>(a).value_length(), std::move(child), len, std::move(nulls));
+  if (a.data_type() == DataType::List) return std::make_shared<ListArray>(std::move(offsets), std::move(child), len, std::move(nulls));
+  return std::make_shared<LargeListArray>(std::move(offsets), std::move(child), len, std::move(nulls));
+}
+
+inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan) {
+  if (!is_list(values.data_type())) return pred.filter(values);
+  Context &c = Context::get();
+  const int64_t n = pred.count();
+  const acu_list_array l = list_view(values);
+  const size_t ob = l.kind == ACU_LIST ? 4 : 8;
+  Buffer offs = Buffer::allocate((size_t)(n + 1) * ob), nb = Buffer::allocate(acu_bitmap_bytes(n));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  acu_filter_plan *child_plan = nullptr;
+  acu_status st = acu_filter_list(c.raw(), plan, &l, offs.data(), &o, &child_plan);
+  if (st != ACU_OK) return c.last_error(st);
+  FilterPredicate cp(child_plan);
+  auto child = filter_any(*list_values(values), cp, child_plan);
+  if (child.is_err()) return child.unwrap_err();
+  return list_like(values, offs, child.unwrap(), o.len, out_nulls(o, nb));
+}
+
+inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool extend);
+
+inline Result<ArrayRef> take_list_level(const Array &values, const Array &indices, int cb, bool keep) {
+  Context &c = Context::get();
+  const int64_t m = indices.len();
+  const acu_list_array l = list_view(values);
+  const bool fixed = l.kind == ACU_FIXED_SIZE_LIST;
+  const size_t ob = l.kind == ACU_LIST ? 4 : 8;
+  const acu_dtype cdt = fixed || l.child_len <= (int64_t)UINT32_MAX ? ACU_U32 : ACU_U64;
+  const acu_array ix = indices.view();
+  const acu_dtype it = (acu_dtype)dtype_code(indices.data_type());
+  Buffer offs = Buffer::allocate((size_t)(m + 1) * ob), nb = Buffer::allocate(acu_bitmap_bytes(m));
+  acu_array_out o{}, cn{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  int64_t rows = 0;
+  acu_status st = acu_take_list(c.raw(), &l, &ix, it, cb, keep ? 1 : 0, offs.data(), &o, cdt, nullptr, 0, &rows, &cn);
+  if (st != ACU_OK) return c.last_error(st);
+  Buffer map = Buffer::allocate((size_t)rows * (cdt == ACU_U32 ? 4 : 8)), cnb = Buffer::allocate(acu_bitmap_bytes(rows));
+  cn.validity = static_cast<uint8_t *>(cnb.data());
+  st = acu_take_list(c.raw(), &l, &ix, it, cb, keep ? 1 : 0, offs.data(), &o, cdt, map.data(), rows, &rows, &cn);
+  std::optional<ArrowError> deferred;  // take_fixed_size_list: the child is taken before the list's validity is read
+  if (st != ACU_OK) {
+    if (!fixed || st != ACU_ERR_PANIC_OUT_OF_BOUNDS) return c.last_error(st);
+    deferred = c.last_error(st);
+  }
+  std::optional<NullBuffer> map_nulls;
+  if (cn.has_validity) map_nulls = NullBuffer{cnb, 0, rows, cn.null_count};
+  ArrayRef rm = cdt == ACU_U32 ? ArrayRef(std::make_shared<PrimitiveArray<uint32_t>>(map, rows, map_nulls))
+                               : ArrayRef(std::make_shared<PrimitiveArray<uint64_t>>(map, rows, map_nulls));
+  auto child = take_any(*list_values(values), *rm, 0, keep || !fixed);
+  if (child.is_err()) return child.unwrap_err();
+  if (deferred) return *deferred;
+  return list_like(values, offs, child.unwrap(), o.len, out_nulls(o, nb));
+}
+
+inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool extend) {
+  if (is_list(values.data_type())) return take_list_level(values, indices, cb, extend);
+  if (!extend || values.data_type() != DataType::Utf8) return take(values, indices, TakeOptions{cb != 0});
+  Context &c = Context::get();
+  const auto &s = static_cast<const StringArray &>(values);
+  const int64_t m = indices.len();
+  const acu_array v = values.view(), ix = indices.view();
+  const acu_dtype it = (acu_dtype)dtype_code(indices.data_type());
+  Buffer offs = Buffer::allocate((size_t)(m + 1) * 4), nb = Buffer::allocate(acu_bitmap_bytes(m));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  int64_t total = 0;
+  const uint8_t *src = static_cast<const uint8_t *>(s.value_data().data());
+  acu_status st = acu_take_bytes_extend(c.raw(), 4, s.offsets().data(), src, &v, &ix, it, offs.data(), nullptr, 0, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  Buffer data = Buffer::allocate((size_t)total);
+  st = acu_take_bytes_extend(c.raw(), 4, s.offsets().data(), src, &v, &ix, it, offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, out_nulls(o, nb)));
+}
+
+template <class L>
+Result<ArrayRef> filter_list(const L &values, const BooleanArray &predicate) {
+  acu_array p = predicate.view();
+  acu_filter_plan *plan = nullptr;
+  Context &c = Context::get();
+  acu_status st = acu_filter_plan_create(c.raw(), &p, &plan);
+  if (st != ACU_OK) return c.last_error(st);
+  FilterPredicate pred(plan);
+  return filter_any(values, pred, plan);
+}
+template <class L>
+Result<ArrayRef> take_list(const L &values, const Array &indices, std::optional<TakeOptions> options) {
+  const DataType it = indices.data_type();
+  if ((int)it > (int)DataType::UInt64)  // take.rs:103
+    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + dtype_display(it)};
+  return take_list_level(values, indices, options && options->check_bounds ? 1 : 0, false);
+}
+}  // namespace detail
+
+inline Result<ArrayRef> filter(const ListArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
+inline Result<ArrayRef> filter(const LargeListArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
+inline Result<ArrayRef> filter(const FixedSizeListArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
+inline Result<ArrayRef> take(const ListArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+  return detail::take_list(values, indices, options);
+}
+inline Result<ArrayRef> take(const LargeListArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+  return detail::take_list(values, indices, options);
+}
+inline Result<ArrayRef> take(const FixedSizeListArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+  return detail::take_list(values, indices, options);
 }
 
 // take.rs:1123-1133: every column gathered with the same indices, one synchronisation per (up to 64-column) call.

@@ -339,6 +339,76 @@ acu_status acu_take_bytes(acu_ctx *ctx, int32_t offset_bytes, const void *offset
                           int64_t *out_data_len, acu_array_out *out_nulls);
 
 /* ------------------------------------------------------------------------- */
+/* filter / take of List, LargeList and FixedSizeList columns                */
+/* ------------------------------------------------------------------------- */
+/* One level of a list column (GenericListArray / FixedSizeListArray). The child is NOT described here: the calls work on one
+ * level at a time and the caller filters / takes the child with the plan / row map they return, through any filter / take
+ * entry point (or these calls again for a nested list).
+ *   kind      ACU_LIST (i32 offsets), ACU_LARGE_LIST (i64) or ACU_FIXED_SIZE_LIST (list_size >= 0 children per row);
+ *   offsets   LIST / LARGE_LIST: nulls.len + 1 entries from logical row 0, ABSOLUTE child rows (a sliced list has
+ *             offsets[0] != 0), aligned to their width; ignored for FIXED_SIZE_LIST, whose row i is the child rows
+ *             [i * list_size, (i + 1) * list_size) (the child is already advanced to the list's logical row 0);
+ *   nulls     len / validity / validity_offset / null_count of the list (`values` ignored);
+ *   child_len rows of the child. */
+typedef enum acu_list_kind { ACU_LIST = 0, ACU_LARGE_LIST = 1, ACU_FIXED_SIZE_LIST = 2 } acu_list_kind;
+typedef struct acu_list_array {
+  int32_t kind;
+  int32_t list_size;
+  const void *offsets;
+  acu_array nulls;
+  int64_t child_len;
+} acu_list_array;
+
+/* filter of a list (filter.rs:535-625: the MutableArrayData fallback). Every selected row keeps its whole child range, null
+ * rows included. out_offsets (LIST / LARGE_LIST only, count + 1 entries of the list's width, starting at 0) and out_nulls
+ * (filter_nulls: a NullBuffer only when the result has a null; capacity acu_bitmap_bytes(count)). *out_child_plan is a new
+ * plan over the child rows [0, offsets[plan len]) selecting the selected rows' ranges; the caller filters the child with it
+ * and destroys it. Predicate longer than the list => ACU_ERR_INVALID_ARGUMENT "Filter predicate of length {p} is larger
+ * than target array of length {n}". Strategy NONE / ALL: the reference returns an empty array / values.slice(0, count);
+ * here the offsets are rebased to 0 and the child is cut to the selected range, which arrow-data's equality treats as the
+ * same array, and the NullBuffer presence is that of acu_filter_primitive (ALL keeps the list's NullBuffer as it is).
+ * Synchronous (not available inside a stream-ordered section); the child plan's expansion counts in ACU_K_FILTER_PLAN. */
+acu_status acu_filter_list(acu_ctx *ctx, const acu_filter_plan *plan, const acu_list_array *list, void *out_offsets,
+                           acu_array_out *out_nulls, acu_filter_plan **out_child_plan);
+
+/* take of a list. Two-phase: out_child_indices == NULL sizes only (writes out_offsets, out_nulls and *out_child_rows); the
+ * second call also writes the child row map, out_child_indices[k] = the child row that becomes output child row k, as
+ * child_index_dtype ACU_U32 or ACU_U64 (ACU_U32 needs child_len <= UINT32_MAX; FIXED_SIZE_LIST takes ACU_U32 only, as the
+ * reference does); capacity < *out_child_rows => ACU_ERR_INVALID_ARGUMENT. The caller then takes the child with that map.
+ * keep_null_ranges = 0 is take_list (take.rs:646-727) / take_fixed_size_list (:765-795):
+ *   - out_nulls = take_nulls(list.nulls, indices) (a NullBuffer only when some row is null for FIXED_SIZE_LIST);
+ *   - LIST / LARGE_LIST: a null output row gets an empty range, out_offsets start at 0, the map has no nulls;
+ *   - FIXED_SIZE_LIST: row i maps to the u32 child rows (u32)(index * list_size) + k, wrapping, and a null index to
+ *     list_size null child rows (out_child_index_nulls, capacity acu_bitmap_bytes(rows); has_validity iff an index is null);
+ *   - check_bounds != 0: ACU_ERR_COMPUTE "Array index out of bounds, cannot get item at index {i} from {len} entries";
+ *   - otherwise a valid out-of-bounds index is the reference's panic, ACU_ERR_PANIC_OUT_OF_BOUNDS at the lowest such row:
+ *     "assertion failed: idx < self.bit_len" (take_bits) when the list has a null, else "index out of bounds: the len is
+ *     {len + 1} but the index is {i}" (the offsets slice). A FIXED_SIZE_LIST takes its child before it reads the list's
+ *     validity: its sizing call succeeds and the call that writes the row map writes it, then returns the take_bits panic,
+ *     so that the caller can take the child first and report the child's own error ahead of it;
+ *   - LIST: the first output row whose end passes i32::MAX is from_usize(..).unwrap()'s panic: ACU_ERR_PANIC_OUT_OF_BOUNDS
+ *     "called `Option::unwrap()` on a `None` value" (without list nulls the lower of this row and an out-of-bounds row).
+ * keep_null_ranges = 1 is the child step of a parent list's take (MutableArrayData::extend, arrow-data/src/transform/
+ * list.rs): every row keeps its range, null rows included; the indices carry no nulls; the nulls are those of take_nulls;
+ * an i32 offset overflow is ACU_ERR_INVALID_ARGUMENT "offset overflow: data exceeds the capacity of the offset type. ..."
+ * (try_extend_offsets) at the first such row. Synchronous; the row map's kernels count in ACU_K_TAKE and the offsets pass
+ * in ACU_K_BYTES, like every user of the offsets engine. */
+acu_status acu_take_list(acu_ctx *ctx, const acu_list_array *list, const acu_array *indices, acu_dtype index_dtype,
+                         int32_t check_bounds, int32_t keep_null_ranges, void *out_offsets, acu_array_out *out_nulls,
+                         acu_dtype child_index_dtype, void *out_child_indices, int64_t capacity, int64_t *out_child_rows,
+                         acu_array_out *out_child_index_nulls);
+
+/* The Utf8 / Binary child of a list take: MutableArrayData::extend of every row of `indices` (a child row map without
+ * nulls), so null rows keep their bytes, unlike acu_take_bytes. Nulls as take_nulls (a NullBuffer only when some row is
+ * null). An i32 offset overflow => ACU_ERR_INVALID_ARGUMENT "offset overflow: data exceeds the capacity of the offset type.
+ * Try splitting into smaller batches or using a larger type (e.g. LargeStringArray / LargeBinaryArray instead of
+ * StringArray / BinaryArray)", detail.index = the first row whose end passes i32::MAX. Indices with a null =>
+ * ACU_ERR_INVALID_ARGUMENT. Two-phase like acu_take_bytes; synchronous; kernel time in ACU_K_BYTES. */
+acu_status acu_take_bytes_extend(acu_ctx *ctx, int32_t offset_bytes, const void *offsets, const uint8_t *data,
+                                 const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype, void *out_offsets,
+                                 uint8_t *out_data, int64_t out_data_capacity, int64_t *out_data_len, acu_array_out *out_nulls);
+
+/* ------------------------------------------------------------------------- */
 /* numeric — arrow-arith/src/numeric.rs, arity.rs                            */
 /* ------------------------------------------------------------------------- */
 /* add/add_wrapping/sub/sub_wrapping/mul/mul_wrapping/div/rem (numeric.rs:36-81).

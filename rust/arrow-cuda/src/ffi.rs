@@ -160,6 +160,20 @@ pub struct acu_column_out {
     pub data_len: i64,
 }
 
+/// acu_list_array: one level of a List / LargeList / FixedSizeList column (the child is described separately).
+pub const ACU_LIST: i32 = 0;
+pub const ACU_LARGE_LIST: i32 = 1;
+pub const ACU_FIXED_SIZE_LIST: i32 = 2;
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct acu_list_array {
+    pub kind: i32,
+    pub list_size: i32,
+    pub offsets: *const c_void,
+    pub nulls: acu_array,
+    pub child_len: i64,
+}
+
 /// acu_bytes_array / acu_view_array: operands of acu_cmp_bytes / acu_cmp_byte_view.
 #[repr(C)]
 #[derive(Clone, Copy)]
@@ -214,6 +228,15 @@ extern "C" {
     pub fn acu_take_bytes(ctx: *mut acu_ctx, offset_bytes: i32, offsets: *const c_void, data: *const u8, nulls_of: *const acu_array,
                           indices: *const acu_array, index_dtype: i32, check_bounds: i32, out_offsets: *mut c_void,
                           out_data: *mut u8, out_data_capacity: i64, out_data_len: *mut i64, out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_take_bytes_extend(ctx: *mut acu_ctx, offset_bytes: i32, offsets: *const c_void, data: *const u8, nulls_of: *const acu_array,
+                                 indices: *const acu_array, index_dtype: i32, out_offsets: *mut c_void, out_data: *mut u8,
+                                 out_data_capacity: i64, out_data_len: *mut i64, out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_filter_list(ctx: *mut acu_ctx, plan: *const acu_filter_plan, list: *const acu_list_array, out_offsets: *mut c_void,
+                           out_nulls: *mut acu_array_out, out_child_plan: *mut *mut acu_filter_plan) -> acu_status;
+    pub fn acu_take_list(ctx: *mut acu_ctx, list: *const acu_list_array, indices: *const acu_array, index_dtype: i32, check_bounds: i32,
+                         keep_null_ranges: i32, out_offsets: *mut c_void, out_nulls: *mut acu_array_out, child_index_dtype: i32,
+                         out_child_indices: *mut c_void, capacity: i64, out_child_rows: *mut i64,
+                         out_child_index_nulls: *mut acu_array_out) -> acu_status;
     pub fn acu_arith(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_neg(ctx: *mut acu_ctx, dtype: i32, checked: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_decimal_arith(ctx: *mut acu_ctx, op: i32, lt: *const acu_decimal_type, a: *const acu_array, rt: *const acu_decimal_type,

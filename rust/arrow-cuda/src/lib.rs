@@ -292,6 +292,9 @@ pub mod compute {
         pub fn count(&self) -> usize { unsafe { ffi::acu_filter_plan_count(self.plan.raw) as usize } }
         pub fn filter(&self, values: &dyn Array) -> Result<ArrayRef, ArrowError> {
             let ctx = &self.plan.ctx;
+            if let DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) = values.data_type() {
+                return list::filter(ctx, self.plan.raw, values);
+            }
             let v = DeviceArray::upload(ctx, values, false)?;
             let mut out = ColumnOut::new(ctx, values.data_type(), self.count(), v.data_bytes)?;
             let st = match kind_of(values.data_type())? {
@@ -350,6 +353,9 @@ pub mod compute {
         let ctx = Context::current()?;
         let idt = index_dtype(indices)?;
         let check = options.unwrap_or_default().check_bounds as i32;
+        if let DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) = values.data_type() {
+            return list::take(&ctx, values, indices, idt, check, false);
+        }
         let (v, ix) = (DeviceArray::upload(&ctx, values, false)?, DeviceArray::upload(&ctx, indices, false)?);
         let m = indices.len();
         let st;
@@ -381,6 +387,129 @@ pub mod compute {
         ctx.check(st)?; // ACU_ERR_PANIC_OUT_OF_BOUNDS panics inside, like take.rs:447
         out.finish(values.data_type())
     }
+    // ---- List / LargeList / FixedSizeList (filter.rs:535-625, take.rs:646-795) ----------------------------------------
+    /// One C call per level: acu_filter_list / acu_take_list return the child's plan / row map, and the child goes through
+    /// filter / take of its own type (these functions again for a nested list). A List's child is extended
+    /// (MutableArrayData: a Utf8 / Binary child keeps the bytes under its null rows, acu_take_bytes_extend); a
+    /// FixedSizeList's child is taken, and its take_bits panic comes after the child's own errors.
+    mod list {
+        use super::*;
+        use arrow_array::types::{UInt32Type, UInt64Type};
+        use arrow_array::{Array, FixedSizeListArray, GenericListArray, OffsetSizeTrait};
+
+        struct Level { list: ffi::acu_list_array, child: ArrayRef, ob: usize, _bufs: Vec<DeviceBuffer>, _nulls: DeviceArray }
+
+        fn level(ctx: &Context, values: &dyn Array) -> Result<Level, ArrowError> {
+            fn generic<O: OffsetSizeTrait>(ctx: &Context, a: &GenericListArray<O>, kind: i32, bufs: &mut Vec<DeviceBuffer>)
+                                           -> Result<(ffi::acu_list_array, ArrayRef, DeviceArray), ArrowError> {
+                let offs = DeviceBuffer::from_host(ctx, a.offsets().inner().inner().as_slice())?;
+                let nulls = DeviceArray::upload(ctx, &BooleanArray::new(BooleanBuffer::new_set(a.len()), a.nulls().cloned()), false)?;
+                let mut l = ffi::acu_list_array { kind, list_size: 0, offsets: offs.as_ptr(), nulls: *nulls.view(), child_len: a.values().len() as i64 };
+                l.nulls.values = std::ptr::null();
+                bufs.push(offs);
+                Ok((l, a.values().clone(), nulls))
+            }
+            let mut bufs = Vec::new();
+            let (list, child, ob, nulls) = match values.data_type() {
+                DataType::List(_) => { let (l, c, n) = generic(ctx, values.as_any().downcast_ref::<GenericListArray<i32>>().unwrap(), ffi::ACU_LIST, &mut bufs)?; (l, c, 4, n) }
+                DataType::LargeList(_) => { let (l, c, n) = generic(ctx, values.as_any().downcast_ref::<GenericListArray<i64>>().unwrap(), ffi::ACU_LARGE_LIST, &mut bufs)?; (l, c, 8, n) }
+                _ => {
+                    let a = values.as_any().downcast_ref::<FixedSizeListArray>().unwrap();
+                    let nulls = DeviceArray::upload(ctx, &BooleanArray::new(BooleanBuffer::new_set(a.len()), a.nulls().cloned()), false)?;
+                    let mut l = ffi::acu_list_array { kind: ffi::ACU_FIXED_SIZE_LIST, list_size: a.value_length(), offsets: std::ptr::null(),
+                                                      nulls: *nulls.view(), child_len: a.values().len() as i64 };
+                    l.nulls.values = std::ptr::null();
+                    (l, a.values().clone(), 0, nulls)
+                }
+            };
+            Ok(Level { list, child, ob, _bufs: bufs, _nulls: nulls })
+        }
+
+        fn rebuild(values: &dyn Array, offsets: Option<Buffer>, child: ArrayRef, len: usize, nulls: Option<NullBuffer>) -> ArrayRef {
+            let mut b = ArrayData::builder(values.data_type().clone()).len(len).nulls(nulls).add_child_data(child.to_data());
+            if let Some(o) = offsets { b = b.add_buffer(o); }
+            make_array(unsafe { b.build_unchecked() })
+        }
+
+        fn nulls_of(validity: &DeviceBuffer, o: &ffi::acu_array_out) -> Result<Option<NullBuffer>, ArrowError> {
+            if o.has_validity == 0 { return Ok(None); }
+            let bits = BooleanBuffer::new(validity.to_host(bitmap_bytes(o.len as usize))?, 0, o.len as usize);
+            Ok(Some(unsafe { NullBuffer::new_unchecked(bits, o.null_count as usize) }))
+        }
+
+        pub(super) fn filter(ctx: &Context, plan: *mut ffi::acu_filter_plan, values: &dyn Array) -> Result<ArrayRef, ArrowError> {
+            let lv = level(ctx, values)?;
+            let n = unsafe { ffi::acu_filter_plan_count(plan) } as usize;
+            let offs = DeviceBuffer::allocate(ctx, (n + 1) * lv.ob.max(1))?;
+            let validity = DeviceBuffer::allocate(ctx, bitmap_bytes(n.max(1)))?;
+            let mut o = ffi::acu_array_out { values: std::ptr::null_mut(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0, has_validity: 0, reserved: 0 };
+            let mut child_plan = std::ptr::null_mut();
+            ctx.check(unsafe { ffi::acu_filter_list(ctx.raw(), plan, &lv.list, offs.as_ptr(), &mut o, &mut child_plan) })?;
+            let child_plan = Plan { ctx: ctx.clone(), raw: child_plan };
+            let child = FilterPredicate { plan: child_plan }.filter(lv.child.as_ref())?;
+            let offsets = if lv.ob > 0 { Some(offs.to_host((n + 1) * lv.ob)?) } else { None };
+            Ok(rebuild(values, offsets, child, n, nulls_of(&validity, &o)?))
+        }
+
+        pub(super) fn take(ctx: &Context, values: &dyn Array, indices: &dyn Array, idt: i32, check: i32, keep: bool) -> Result<ArrayRef, ArrowError> {
+            let lv = level(ctx, values)?;
+            let ix = DeviceArray::upload(ctx, indices, false)?;
+            let m = indices.len();
+            let wide = lv.ob > 0 && lv.list.child_len > u32::MAX as i64;
+            let cdt = if wide { 7 } else { 6 }; // ACU_U64 / ACU_U32
+            let offs = DeviceBuffer::allocate(ctx, (m + 1) * lv.ob.max(1))?;
+            let validity = DeviceBuffer::allocate(ctx, bitmap_bytes(m.max(1)))?;
+            let mut o = ffi::acu_array_out { values: std::ptr::null_mut(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0, has_validity: 0, reserved: 0 };
+            let mut rows = 0i64;
+            let mut cn = ffi::acu_array_out { values: std::ptr::null_mut(), validity: std::ptr::null_mut(), len: 0, null_count: 0, has_validity: 0, reserved: 0 };
+            ctx.check(unsafe { ffi::acu_take_list(ctx.raw(), &lv.list, ix.view(), idt, check, keep as i32, offs.as_ptr(), &mut o, cdt,
+                                                  std::ptr::null_mut(), 0, &mut rows, &mut cn) })?;
+            let n = rows as usize;
+            let map = DeviceBuffer::allocate(ctx, n.max(1) * if wide { 8 } else { 4 })?;
+            let map_valid = DeviceBuffer::allocate(ctx, bitmap_bytes(n.max(1)))?;
+            cn.validity = map_valid.as_ptr() as *mut u8;
+            let st = unsafe { ffi::acu_take_list(ctx.raw(), &lv.list, ix.view(), idt, check, keep as i32, offs.as_ptr(), &mut o, cdt,
+                                                 map.as_ptr(), rows, &mut rows, &mut cn) };
+            let deferred = if st != ffi::ACU_OK && lv.ob == 0 { Some(ctx.check(st).unwrap_err()) } else { ctx.check(st).map(|_| None)? };
+            let map_nulls = nulls_of(&map_valid, &cn)?;
+            let rm: ArrayRef = if wide {
+                Arc::new(PrimitiveArray::<UInt64Type>::new(map.to_host(n * 8)?.into(), map_nulls))
+            } else {
+                Arc::new(PrimitiveArray::<UInt32Type>::new(map.to_host(n * 4)?.into(), map_nulls))
+            };
+            // a List's child is extended, a FixedSizeList's child is taken
+            let child = child_take(ctx, lv.child.as_ref(), rm.as_ref(), cdt, keep || lv.ob > 0)?;
+            if let Some(e) = deferred { return Err(e); }
+            let offsets = if lv.ob > 0 { Some(offs.to_host((m + 1) * lv.ob)?) } else { None };
+            Ok(rebuild(values, offsets, child, m, nulls_of(&validity, &o)?))
+        }
+
+        fn child_take(ctx: &Context, child: &dyn Array, map: &dyn Array, cdt: i32, extend: bool) -> Result<ArrayRef, ArrowError> {
+            match child.data_type() {
+                DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) => take(ctx, child, map, cdt, 0, extend),
+                DataType::Utf8 | DataType::Binary | DataType::LargeUtf8 | DataType::LargeBinary if extend => {
+                    let ob = match kind_of(child.data_type())? { Kind::Bytes(ob) => ob, _ => unreachable!() };
+                    let (v, ix) = (DeviceArray::upload(ctx, child, false)?, DeviceArray::upload(ctx, map, false)?);
+                    let m = map.len();
+                    let mut probe = ColumnOut::new(ctx, child.data_type(), m, 0)?;
+                    let mut need = 0i64;
+                    ctx.check(unsafe {
+                        ffi::acu_take_bytes_extend(ctx.raw(), ob as i32, v.view().values, v.column.data, v.view(), ix.view(), cdt,
+                                                   probe.out.array.values, std::ptr::null_mut(), 0, &mut need, &mut probe.out.array)
+                    })?;
+                    let mut out = ColumnOut::new(ctx, child.data_type(), m, need as usize)?;
+                    ctx.check(unsafe {
+                        ffi::acu_take_bytes_extend(ctx.raw(), ob as i32, v.view().values, v.column.data, v.view(), ix.view(), cdt,
+                                                   out.out.array.values, out.out.data, out.out.data_capacity, &mut out.out.data_len,
+                                                   &mut out.out.array)
+                    })?;
+                    out.finish(child.data_type())
+                }
+                _ => super::take(child, map, None),
+            }
+        }
+    }
+
     /// `arrow::compute::take_arrays` (take.rs:155-164).
     pub fn take_arrays(arrays: &[ArrayRef], indices: &dyn Array, options: Option<TakeOptions>) -> Result<Vec<ArrayRef>, ArrowError> {
         arrays.iter().map(|a| take(a.as_ref(), indices, options.clone())).collect()
