@@ -1760,7 +1760,10 @@ class Context:
                 self.lib.acu_filter_plan_destroy(self.h, plan)
             dp.free()
 
-    def _filter_with_plan(self, col, plan):
+    def _filter_with_plan(self, col, plan, child_step=None):
+        """child_step: this level is the child of a list filtered with a plan that is not IterationStrategy::All (None at
+        the top). The reference then builds every level below it with MutableArrayData, whose freeze drops a NullBuffer
+        without nulls (arrow-data/src/transform/mod.rs:936), also where the child's own plan selects every row."""
         count = self.lib.acu_filter_plan_count(plan)
         owned, out = [], None
         try:
@@ -1773,10 +1776,13 @@ class Context:
                 out = self.alloc_out(0, count)
                 child_plan = C.c_void_p()
                 self.check(self.lib.acu_filter_list(self.h, plan, C.byref(d), d_off, C.byref(out), C.byref(child_plan)))
+                # only the top level decides: under a top-level All the reference slices every level as it is
+                step = child_step if child_step is not None else count != self.lib.acu_filter_plan_len(plan)
                 try:
-                    child = self._filter_with_plan(col.child, child_plan)
+                    child = self._filter_with_plan(col.child, child_plan, step)
                 finally:
                     self.lib.acu_filter_plan_destroy(self.h, child_plan)
+                self._drop_empty_nulls(out, child_step)
                 nulls = self._nulls_out(out, count)
                 if fixed:
                     return FixedSizeListColumn(col.size, child, nulls)
@@ -1794,6 +1800,7 @@ class Context:
                 owned.append(d_data)
                 self.check(self.lib.acu_filter_bytes(self.h, plan, ob, bd.offsets, bd.data, C.byref(bd.nulls), d_off, d_data,
                                                      total.value, C.byref(total), C.byref(out)))
+                self._drop_empty_nulls(out, child_step)
                 return Utf8Column(self.d2h(d_off, (count + 1) * ob, col.offsets.dtype), self.d2h(d_data, total.value),
                                   self._nulls_out(out, count))
             if isinstance(col, ViewColumn):  # the views filter as 16-byte values; the data buffers are shared
@@ -1803,6 +1810,7 @@ class Context:
                 arr.values = vd.views
                 out = self.alloc_out(count * 16, count)
                 self.check(self.lib.acu_filter_primitive(self.h, plan, 16, C.byref(arr), C.byref(out)))
+                self._drop_empty_nulls(out, child_step)
                 views = self.d2h(out.values, count * 16).reshape(-1, 16)
                 return ViewColumn(views, col.buffers, self._nulls_out(out, count))
             dv = self.upload(col)
@@ -1814,6 +1822,7 @@ class Context:
                     self.check(self.lib.acu_filter_boolean(self.h, plan, C.byref(vd), C.byref(out)))
                 else:
                     self.check(self.lib.acu_filter_primitive(self.h, plan, col.width(), C.byref(vd), C.byref(out)))
+                self._drop_empty_nulls(out, child_step)
                 res, out = self.download_out(out, col.dtype), None
                 return col.like(res) if isinstance(col, DecimalArray) else res
             finally:
@@ -1823,6 +1832,11 @@ class Context:
                 self._free_out(out)
             for p in owned:
                 self.free(p)
+
+    @staticmethod
+    def _drop_empty_nulls(out, child_step):
+        if child_step and out.has_validity and out.null_count == 0:
+            out.has_validity = 0
 
     def take_list(self, col, indices, check_bounds=False):
         """arrow::compute::take of a ListColumn / FixedSizeListColumn by a HostArray of integer indices."""

@@ -321,7 +321,12 @@ extern "C" acu_status acu_take_list(acu_ctx *ctx, const acu_list_array *list, co
     return acu_fail(ctx, ACU_ERR_PANIC_OUT_OF_BOUNDS, (int64_t)ovf, 0, 0, 0, "called `Option::unwrap()` on a `None` value");
   }
   if (!bit_len_panic) {
-    ACU_TRY(acu_take_col_finalize(ctx, &list->nulls, indices, index_dtype, mode, h, out_nulls));
+    // without list nulls take_fixed_size_list reads no list row (is_null of a list without a NullBuffer): a valid index
+    // past the list is the child take's to report, or nothing when (u32)(index * size) + k lands back in the child
+    unsigned long long hf[RES_SLOTS];
+    std::copy(h, h + RES_SLOTS, hf);
+    if (!ob && !val_nulls) hf[RES_ERR_INDEX] = ~0ull;
+    ACU_TRY(acu_take_col_finalize(ctx, &list->nulls, indices, index_dtype, mode, hf, out_nulls));
     if (!ob && out_nulls->null_count == 0) out_nulls->has_validity = 0;  // NullBuffer::from_unsliced_buffer
   }
   *out_child_rows = total;

@@ -198,6 +198,10 @@ class Array {
   }
   bool is_null(int64_t i) const { return !valid_mask()[(size_t)i]; }
   bool is_valid(int64_t i) const { return !is_null(i); }
+  // MutableArrayData::freeze keeps a NullBuffer only if it has a null (arrow-data/src/transform/mod.rs:936)
+  void drop_empty_nulls() {
+    if (nulls_ && nulls_->null_count == 0) nulls_.reset();
+  }
  protected:
   virtual const void *values_ptr() const = 0;
   virtual int64_t values_bit_offset() const { return 0; }
@@ -872,8 +876,18 @@ inline ArrayRef list_like(const Array &a, Buffer offsets, ArrayRef child, int64_
   return std::make_shared<LargeListArray>(std::move(offsets), std::move(child), len, std::move(nulls));
 }
 
-inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan) {
-  if (!is_list(values.data_type())) return pred.filter(values);
+// child_step: `values` is a child of a list whose top level was filtered with a plan other than All (nullopt at the top).
+// The reference builds those levels with MutableArrayData (filter.rs:600), which drops a NullBuffer without nulls even
+// where the level's own plan selects every row; under a top-level All it slices every level as it is.
+inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan,
+                                   std::optional<bool> child_step = std::nullopt) {
+  if (!is_list(values.data_type())) {
+    auto r = pred.filter(values);
+    if (r.is_err() || !child_step.value_or(false)) return r;
+    ArrayRef a = r.unwrap();
+    a->drop_empty_nulls();
+    return a;
+  }
   Context &c = Context::get();
   const int64_t n = pred.count();
   const acu_list_array l = list_view(values);
@@ -885,8 +899,10 @@ inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &p
   acu_status st = acu_filter_list(c.raw(), plan, &l, offs.data(), &o, &child_plan);
   if (st != ACU_OK) return c.last_error(st);
   FilterPredicate cp(child_plan);
-  auto child = filter_any(*list_values(values), cp, child_plan);
+  const bool step = child_step ? *child_step : n != acu_filter_plan_len(plan);
+  auto child = filter_any(*list_values(values), cp, child_plan, step);
   if (child.is_err()) return child.unwrap_err();
+  if (child_step.value_or(false) && o.has_validity && o.null_count == 0) o.has_validity = 0;
   return list_like(values, offs, child.unwrap(), o.len, out_nulls(o, nb));
 }
 

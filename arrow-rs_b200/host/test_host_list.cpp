@@ -126,6 +126,19 @@ static void test_take_fixed_size_list() {
   CHECK((child == std::vector<O<int32_t>>{0, 1, std::nullopt, std::nullopt}));
 }
 
+// A List filtered with a plan other than All goes through MutableArrayData (filter.rs:600), whose freeze keeps the
+// child's NullBuffer only if the result has a null (arrow-data/src/transform/mod.rs:936): here the unselected row is
+// empty, so the child plan selects all of [0, 4), and the child's only null lies past it. Under a top-level All the
+// reference slices, and the child keeps its NullBuffer.
+static void test_filter_child_plan_all() {
+  auto a = ListArray::from({0, 2, 2, 4}, ints({0, 1, 2, 3, 4, 5, std::nullopt}));
+  auto r = filter(a, BooleanArray::from(std::vector<bool>{true, false, true})).unwrap();
+  CHECK((rows_of(*r) == Rows{iv({0, 1}), iv({2, 3})}));
+  CHECK(!compute::detail::list_values(*r)->nulls().has_value());
+  r = filter(a, BooleanArray::from(std::vector<bool>{true, true, true})).unwrap();
+  CHECK(compute::detail::list_values(*r)->nulls().has_value());
+}
+
 int main() {
   try {
     Context::get();
@@ -135,6 +148,7 @@ int main() {
   }
   test_filter_list_array();
   test_filter_fixed_size_list();
+  test_filter_child_plan_all();
   test_take_list_macros<ListArray, int32_t>();
   test_take_list_macros<LargeListArray, int64_t>();
   test_take_list_out_of_bounds();

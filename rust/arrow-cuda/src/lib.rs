@@ -293,7 +293,7 @@ pub mod compute {
         pub fn filter(&self, values: &dyn Array) -> Result<ArrayRef, ArrowError> {
             let ctx = &self.plan.ctx;
             if let DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) = values.data_type() {
-                return list::filter(ctx, self.plan.raw, values);
+                return list::filter(ctx, self.plan.raw, values, None);
             }
             let v = DeviceArray::upload(ctx, values, false)?;
             let mut out = ColumnOut::new(ctx, values.data_type(), self.count(), v.data_bytes)?;
@@ -437,7 +437,12 @@ pub mod compute {
             Ok(Some(unsafe { NullBuffer::new_unchecked(bits, o.null_count as usize) }))
         }
 
-        pub(super) fn filter(ctx: &Context, plan: *mut ffi::acu_filter_plan, values: &dyn Array) -> Result<ArrayRef, ArrowError> {
+        /// `child_step`: `values` is a child of a list whose top level was filtered with a plan other than All (None at the
+        /// top). The reference builds those levels with MutableArrayData (filter.rs:600), whose freeze drops a NullBuffer
+        /// without nulls (arrow-data/src/transform/mod.rs:936) even where the level's own plan selects every row; under a
+        /// top-level All it slices every level as it is.
+        pub(super) fn filter(ctx: &Context, plan: *mut ffi::acu_filter_plan, values: &dyn Array, child_step: Option<bool>)
+                             -> Result<ArrayRef, ArrowError> {
             let lv = level(ctx, values)?;
             let n = unsafe { ffi::acu_filter_plan_count(plan) } as usize;
             let offs = DeviceBuffer::allocate(ctx, (n + 1) * lv.ob.max(1))?;
@@ -446,9 +451,22 @@ pub mod compute {
             let mut child_plan = std::ptr::null_mut();
             ctx.check(unsafe { ffi::acu_filter_list(ctx.raw(), plan, &lv.list, offs.as_ptr(), &mut o, &mut child_plan) })?;
             let child_plan = Plan { ctx: ctx.clone(), raw: child_plan };
-            let child = FilterPredicate { plan: child_plan }.filter(lv.child.as_ref())?;
+            let step = child_step.unwrap_or(n != unsafe { ffi::acu_filter_plan_len(plan) } as usize);
+            let child = match lv.child.data_type() {
+                DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) => filter(ctx, child_plan.raw, lv.child.as_ref(), Some(step))?,
+                _ => {
+                    let c = FilterPredicate { plan: child_plan }.filter(lv.child.as_ref())?;
+                    if step { drop_empty_nulls(c) } else { c }
+                }
+            };
+            if child_step == Some(true) && o.null_count == 0 { o.has_validity = 0; }
             let offsets = if lv.ob > 0 { Some(offs.to_host((n + 1) * lv.ob)?) } else { None };
             Ok(rebuild(values, offsets, child, n, nulls_of(&validity, &o)?))
+        }
+
+        fn drop_empty_nulls(a: ArrayRef) -> ArrayRef {
+            if a.nulls().map_or(true, |n| n.null_count() > 0) { return a; }
+            make_array(unsafe { a.to_data().into_builder().nulls(None).build_unchecked() })
         }
 
         pub(super) fn take(ctx: &Context, values: &dyn Array, indices: &dyn Array, idt: i32, check: i32, keep: bool) -> Result<ArrayRef, ArrowError> {

@@ -104,8 +104,12 @@ def filter_mask(predicate):
     return predicate.value_array() & predicate.valid_mask()
 
 
-def filter(col, mask):
-    """filter(col, predicate) with mask = filter_mask(predicate) (len <= col length)."""
+def filter(col, mask, child_step=None):
+    """filter(col, predicate) with mask = filter_mask(predicate) (len <= col length). child_step: `col` is a child of a
+    list whose top level was filtered with a plan other than All (None at the top level). The reference builds that list
+    with MutableArrayData (filter.rs:600), whose freeze keeps a level's NullBuffer only if it has a null
+    (arrow-data/src/transform/mod.rs:936), also where this level's own plan selects every row; under a top-level All the
+    reference slices every level as it is."""
     n = len(mask)
     if n > length(col):
         raise OracleError(abi.ERR_INVALID_ARGUMENT, f"Filter predicate of length {n} is larger than target array of length {length(col)}")
@@ -116,10 +120,11 @@ def filter(col, mask):
     nulls_as_is = col.validity is not None if isinstance(col, HostArray) else col.nulls.validity is not None
     if count == 0:
         present = False
-    elif count == n:  # IterationStrategy::All: the slice keeps its NullBuffer
+    elif count == n and not child_step:  # IterationStrategy::All: the slice keeps its NullBuffer
         present = nulls_as_is
     else:
         present = _has_nulls(col) and not all(out_mask)
+    step = child_step if child_step is not None else count != n
     if isinstance(col, (HostArray, ViewColumn)):
         return _rebuild(col, rows, out_mask, present)
     if isinstance(col, Utf8Column):
@@ -128,14 +133,14 @@ def filter(col, mask):
         cmask = np.zeros(n * col.size, dtype=bool)
         for r in rows:
             cmask[r * col.size:(r + 1) * col.size] = True
-        return FixedSizeListColumn(col.size, filter(col.child, cmask), _nulls(out_mask, present))
+        return FixedSizeListColumn(col.size, filter(col.child, cmask, step), _nulls(out_mask, present))
     offs = [int(x) for x in col.offsets]
     cmask = np.zeros(offs[n] if n else offs[0], dtype=bool)
     new = [0]
     for r in rows:
         cmask[offs[r]:offs[r + 1]] = True
         new.append(new[-1] + offs[r + 1] - offs[r])
-    return ListColumn(np.array(new, dtype=col.offsets.dtype), filter(col.child, cmask), _nulls(out_mask, present))
+    return ListColumn(np.array(new, dtype=col.offsets.dtype), filter(col.child, cmask, step), _nulls(out_mask, present))
 
 
 # ---- take ---------------------------------------------------------------------------------------------------------------
