@@ -388,6 +388,50 @@ class FixedSizeListColumn:
         return self.nulls.length
 
 
+class RunEndColumn:
+    """A RunEndEncoded column on the host (RunArray, arrow-array/src/array/run_array.rs): `run_ends` (np.int16 | np.int32 |
+    np.int64) are the physical run ends from physical entry 0, `values` the values child (one row per physical run: a
+    HostArray, DecimalArray, Utf8Column, ViewColumn or list column), `offset` / `length` the logical slice."""
+
+    def __init__(self, run_ends, values, offset=0, length=None):
+        self.run_ends, self.values, self.offset = np.ascontiguousarray(run_ends), values, offset
+        self.length = (int(self.run_ends[-1]) - offset if len(self.run_ends) else 0) if length is None else length
+
+    def slice(self, offset, length):
+        """RunArray::slice: only the logical window moves (run_array.rs, RunEndBuffer::slice run.rs:269-285)."""
+        assert offset + length <= self.length, "the length + offset of the sliced RunEndBuffer cannot exceed the existing length"
+        return RunEndColumn(self.run_ends, self.values, self.offset + offset, length)
+
+
+def slice_column(col, offset, length):
+    """Array::slice of any host column: the same buffers, a new logical window."""
+    if isinstance(col, HostArray):  # DecimalArray included
+        return col.slice(offset, length)
+    nulls = col.nulls.slice(offset, length)
+    if isinstance(col, Utf8Column):
+        return Utf8Column(col.offsets[offset:offset + length + 1], col.data, nulls)
+    if isinstance(col, ViewColumn):
+        return ViewColumn(col.views[offset:offset + length], col.buffers, nulls)
+    if isinstance(col, ListColumn):
+        return ListColumn(col.offsets[offset:offset + length + 1], col.child, nulls)
+    if isinstance(col, FixedSizeListColumn):
+        return FixedSizeListColumn(col.size, slice_column(col.child, offset * col.size, length * col.size), nulls)
+    if isinstance(col, RunEndColumn):
+        return col.slice(offset, length)
+    raise TypeError(f"cannot slice {type(col).__name__}")
+
+
+def empty_column(col):
+    """new_empty_array of col's type: no rows and no NullBuffer."""
+    e = slice_column(col, 0, 0)
+    tgt = e if isinstance(e, HostArray) else (None if isinstance(e, RunEndColumn) else e.nulls)
+    if tgt is not None:
+        tgt.validity, tgt.validity_offset, tgt.null_count = None, 0, 0
+    if isinstance(e, (ListColumn, FixedSizeListColumn)):
+        e.child = empty_column(e.child)
+    return e
+
+
 def column_value(col, row):
     """The bytes of logical row `row` of a Utf8Column / ViewColumn / FixedSizeBinaryColumn (`array.value(row)`)."""
     if isinstance(col, Utf8Column):
@@ -1980,3 +2024,94 @@ class Context:
                 self.free(p)
             if dh is not None:
                 dh.free()
+
+    # -- RunEndEncoded (filter_run_end_array filter.rs:628-677, take_run take.rs:948-995) ---------------------------
+    # The run-end calls work on the run ends; the values child is filtered / taken with the plan / value indices they
+    # return through the path of its own type, as a list hands its child plan / row map on.
+    def _run_descriptor(self, col, owned):
+        d = abi.RunArray()
+        d.run_end_dtype = {2: abi.I16, 4: abi.I32, 8: abi.I64}[col.run_ends.dtype.itemsize]
+        d.run_ends = self.malloc(col.run_ends.nbytes + 16)
+        owned.append(d.run_ends)
+        if col.run_ends.nbytes:
+            self.h2d(d.run_ends, col.run_ends)
+        d.n_runs, d.offset, d.len = len(col.run_ends), col.offset, col.length
+        return d
+
+    def filter_run_end(self, col, predicate):
+        """arrow::compute::filter of a RunEndColumn: the run ends keep their type, the values child is any column this
+        package filters."""
+        dp = self.upload(predicate)
+        plan, vplan, owned = C.c_void_p(), C.c_void_p(), []
+        try:
+            pd = dp.descriptor()
+            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
+            d = self._run_descriptor(col, owned)
+            count = self.lib.acu_filter_plan_count(plan)
+            w = col.run_ends.itemsize
+            d_ends = self.malloc(max(min(count, len(col.run_ends)), 1) * w + 16)
+            owned.append(d_ends)
+            runs, vstart = C.c_int64(0), C.c_int64(0)
+            self.check(self.lib.acu_filter_run_end(self.h, plan, C.byref(d), d_ends, C.byref(runs), C.byref(vstart), C.byref(vplan)))
+            if not vplan:
+                if self.lib.acu_filter_plan_strategy(plan) == abi.FILTER_ALL:
+                    return col.slice(0, count)  # values.slice(0, count) (filter.rs:546)
+                return RunEndColumn(np.zeros(0, col.run_ends.dtype), empty_column(col.values), 0, 0)
+            values = self._filter_with_plan(slice_column(col.values, vstart.value, self.lib.acu_filter_plan_len(vplan)), vplan)
+            ends = self.d2h(d_ends, runs.value * w, col.run_ends.dtype)
+            return RunEndColumn(ends, values, 0, int(ends[-1]))
+        finally:
+            if vplan:
+                self.lib.acu_filter_plan_destroy(self.h, vplan)
+            if plan:
+                self.lib.acu_filter_plan_destroy(self.h, plan)
+            for p in owned:
+                self.free(p)
+            dp.free()
+
+    def _run_values(self, col, owned, keep):
+        """acu_run_values of a values child for take's run merge (uploads appended to owned / keep)."""
+        v = abi.RunValues()
+        if isinstance(col, (ListColumn, FixedSizeListColumn, RunEndColumn)):
+            v.kind = abi.RUN_VALUES_NESTED
+        elif isinstance(col, Utf8Column):
+            v.kind, v.width, v.bytes = abi.RUN_VALUES_BYTES, col.offsets.itemsize, self._upload_bytes_col(col, owned)
+        elif isinstance(col, ViewColumn):
+            v.kind, v.view = abi.RUN_VALUES_VIEW, self._upload_view_col(col, owned, keep)
+        else:
+            dv = self.upload(col)
+            keep.append(dv)
+            v.array = dv.descriptor()
+            v.kind, v.width = (abi.RUN_VALUES_BOOLEAN, 0) if col.dtype == BOOL else (abi.RUN_VALUES_FIXED, col.width())
+        return v
+
+    def take_run_end(self, col, indices, check_bounds=False):
+        """arrow::compute::take of a RunEndColumn by a HostArray of integer indices (values: primitive, decimal, Boolean,
+        Utf8 / Binary and view columns)."""
+        di = self.upload(indices)
+        owned, keep = [], []
+        try:
+            idd = di.descriptor()
+            d = self._run_descriptor(col, owned)
+            vd = self._run_values(col.values, owned, keep)
+            m = indices.length
+            wide = indices.dtype in (abi.I64, abi.U64)
+            d_ends = self.malloc(max(m, 1) * col.run_ends.itemsize + 16)
+            d_vi = self.malloc(max(m, 1) * (8 if wide else 4) + 16)
+            owned += [d_ends, d_vi]
+            runs = C.c_int64(0)
+            self.check(self.lib.acu_take_run_end(self.h, C.byref(d), C.byref(vd), C.byref(idd), indices.dtype, int(check_bounds), d_ends,
+                                                 d_vi, C.byref(runs)))
+            if m == 0:
+                return RunEndColumn(np.zeros(0, col.run_ends.dtype), empty_column(col.values), 0, 0)
+            cd = abi.Array()
+            cd.values, cd.len = d_vi, runs.value
+            values = self._take_level(col.values, cd, abi.U64 if wide else abi.U32, False, False)
+            return RunEndColumn(self.d2h(d_ends, runs.value * col.run_ends.itemsize, col.run_ends.dtype), values, 0, m)
+        finally:
+            for k in keep:
+                if isinstance(k, DeviceArray):
+                    k.free()
+            for p in owned:
+                self.free(p)
+            di.free()

@@ -111,6 +111,20 @@ class ListArray(C.Structure):
     _fields_ = [("kind", C.c_int32), ("list_size", C.c_int32), ("offsets", C.c_void_p), ("nulls", Array), ("child_len", C.c_int64)]
 
 
+class RunArray(C.Structure):
+    """acu_run_array: the run ends of a RunEndEncoded column and its logical slice (the values child is separate)."""
+    _fields_ = [("run_end_dtype", C.c_int32), ("reserved", C.c_int32), ("run_ends", C.c_void_p), ("n_runs", C.c_int64),
+                ("offset", C.c_int64), ("len", C.c_int64)]
+
+
+RUN_VALUES_FIXED, RUN_VALUES_BOOLEAN, RUN_VALUES_BYTES, RUN_VALUES_VIEW, RUN_VALUES_NESTED = range(5)
+
+
+class RunValues(C.Structure):
+    """acu_run_values: the values child of a RunEndEncoded column as take's run merge compares it."""
+    _fields_ = [("kind", C.c_int32), ("width", C.c_int32), ("array", Array), ("bytes", BytesArray), ("view", ViewArray)]
+
+
 COL_PRIMITIVE, COL_BOOLEAN, COL_BYTES = range(3)
 BOOL_AND, BOOL_OR, BOOL_AND_NOT, BOOL_AND_KLEENE, BOOL_OR_KLEENE, BOOL_NOT, BOOL_IS_NULL, BOOL_IS_NOT_NULL = range(8)
 MAX_BATCH_COLUMNS = 64
@@ -222,6 +236,8 @@ PROTOTYPES = {
     "acu_take_bytes_extend": (i32, [vp, i32, vp, vp, P(Array), P(Array), i32, vp, vp, i64, P(i64), P(ArrayOut)]),
     "acu_filter_list": (i32, [vp, vp, P(ListArray), vp, P(ArrayOut), P(vp)]),
     "acu_take_list": (i32, [vp, P(ListArray), P(Array), i32, i32, i32, vp, P(ArrayOut), i32, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_filter_run_end": (i32, [vp, vp, P(RunArray), vp, P(i64), P(i64), P(vp)]),
+    "acu_take_run_end": (i32, [vp, P(RunArray), P(RunValues), P(Array), i32, i32, vp, vp, P(i64)]),
     "acu_arith": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_bitwise": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_neg": (i32, [vp, i32, i32, P(Array), P(ArrayOut)]),

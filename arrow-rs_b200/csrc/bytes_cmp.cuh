@@ -1,7 +1,8 @@
 // bytes_cmp.cuh — the one operand path of variable-width columns on the device: BytesOperand (Utf8 / Binary, i32 or i64
 // offsets) and ViewOperand (Utf8View / BinaryView) and their row reads, and the helpers that order and match the values.
 // Shared by the comparison kernels (strcmp.cu), the min / max reductions (aggregate_bytes.cu), the LIKE family (like.cu),
-// length / substring (substring.cu) and the gathers (bytes.cu, ld_offset only). The host builds the operands through
+// length / substring (substring.cu), the run merge of a RunEndEncoded take (run_end.cu) and the gathers (bytes.cu,
+// ld_offset only). The host builds the operands through
 // internal.cuh's front end (acu_offset_width_check, acu_view_operand), after acu_sync_only.
 //
 // Order: Rust's `Ord` for `&[u8]` (lexicographic on unsigned bytes, a proper prefix sorts first); `&str` orders the same.
@@ -82,6 +83,19 @@ __device__ __forceinline__ bool bytes_range_eq(const uint8_t *a, const uint8_t *
 // `&[u8]` equality / ordering of Rust (lexicographic on unsigned bytes, then length)
 __device__ __forceinline__ bool bytes_eq(const uint8_t *a, int64_t la, const uint8_t *b, int64_t lb) {
   return la == lb && bytes_range_eq<false>(a, b, la);
+}
+// view equality (cmp.rs:810-862): the 16 view bytes when no value lives in a data buffer, else length and prefix first
+__device__ __forceinline__ bool view_bits_eq(const uint4 &a, const uint4 &b) { return a.x == b.x && a.y == b.y && a.z == b.z && a.w == b.w; }
+__device__ __forceinline__ bool view_is_eq(const ViewOperand &L, const uint4 &l, const uint4 *lslot, const ViewOperand &R, const uint4 &r,
+                                           const uint4 *rslot) {
+  if (L.n_buffers == 0 && R.n_buffers == 0) return view_bits_eq(l, r);
+  if (view_bits_eq(l, r) && l.x <= 12u) return true;
+  if (l.x != r.x) return false;
+  if (l.x == 0u) return true;
+  if (l.y != r.y) return false;
+  if (l.x <= 12u) return false;
+  const BytesItem a = L.item(l, lslot), b = R.item(r, rslot);
+  return bytes_eq(a.p, a.len, b.p, b.len);
 }
 __device__ __forceinline__ bool bytes_lt(const uint8_t *a, int64_t la, const uint8_t *b, int64_t lb) {
   const int64_t n = la < lb ? la : lb;

@@ -28,18 +28,6 @@ struct RowCmpCommon {
   unsigned long long *res;
 };
 
-__device__ __forceinline__ bool view_bits_eq(const uint4 &a, const uint4 &b) { return a.x == b.x && a.y == b.y && a.z == b.z && a.w == b.w; }
-__device__ __forceinline__ bool view_is_eq(const ViewOperand &L, const uint4 &l, const uint4 *lslot, const ViewOperand &R, const uint4 &r,
-                                           const uint4 *rslot) {  // cmp.rs:810-862
-  if (L.n_buffers == 0 && R.n_buffers == 0) return view_bits_eq(l, r);
-  if (view_bits_eq(l, r) && l.x <= 12u) return true;
-  if (l.x != r.x) return false;
-  if (l.x == 0u) return true;
-  if (l.y != r.y) return false;
-  if (l.x <= 12u) return false;
-  const BytesItem a = L.item(l, lslot), b = R.item(r, rslot);
-  return bytes_eq(a.p, a.len, b.p, b.len);
-}
 __device__ __forceinline__ bool view_is_lt(const ViewOperand &L, const uint4 &l, const uint4 *lslot, const ViewOperand &R, const uint4 &r,
                                            const uint4 *rslot) {  // cmp.rs:864-893
   if (L.n_buffers == 0 && R.n_buffers == 0) return inline_key_lt(l, r);

@@ -21,6 +21,7 @@
 // No CPU fallback: Context::get() throws if no CUDA device / library is available.
 #pragma once
 
+#include <algorithm>
 #include <cstdint>
 #include <cstring>
 #include <functional>
@@ -142,7 +143,7 @@ inline std::vector<uint8_t> pack_bits(const std::vector<bool> &bits) {
 // DataType / native type traits (arrow-array/src/types.rs:67-80)
 // ---------------------------------------------------------------------------------------
 enum class DataType { Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Boolean, Utf8, Decimal32, Decimal64, Decimal128,
-                      List, LargeList, FixedSizeList };
+                      List, LargeList, FixedSizeList, RunEndEncoded };
 
 template <class T> struct NativeOf;
 #define ACU_NATIVE(T, DT, CODE) \
@@ -526,6 +527,72 @@ class FixedSizeListArray : public Array {
   ArrayRef values_;
 };
 
+// RunArray<R> (arrow-array/src/array/run_array.rs): the run ends (RunEndBuffer, arrow-buffer/src/buffer/run.rs) from
+// physical entry 0, a logical window (offset, len) over them, and the values child, one row per physical run.
+// Int16RunArray / Int32RunArray / Int64RunArray.
+template <class R>
+class RunArray : public Array {
+ public:
+  RunArray(Buffer run_ends, int64_t n_runs, ArrayRef values, int64_t offset, int64_t len)
+      : run_ends_(std::move(run_ends)), n_runs_(n_runs), values_(std::move(values)), offset_(offset) { len_ = len; }
+  // RunArray::try_new(run_ends, values): the logical length is the last run end
+  static RunArray from(const std::vector<R> &run_ends, ArrayRef values) {
+    return RunArray(Buffer::from_host(run_ends.data(), run_ends.size() * sizeof(R)), (int64_t)run_ends.size(), std::move(values), 0,
+                    run_ends.empty() ? 0 : (int64_t)run_ends.back());
+  }
+  DataType data_type() const override { return DataType::RunEndEncoded; }
+  // RunEndBuffer::values: every physical run end (not advanced by the offset)
+  std::vector<R> run_ends() const {
+    std::vector<R> v((size_t)n_runs_);
+    run_ends_.to_host(v.data(), v.size() * sizeof(R));
+    return v;
+  }
+  const Buffer &run_ends_buffer() const { return run_ends_; }
+  int64_t num_runs() const { return n_runs_; }
+  int64_t offset() const { return offset_; }
+  const ArrayRef &values() const { return values_; }
+  // RunArray::slice: only the logical window moves (RunEndBuffer::slice, run.rs:269-285)
+  RunArray slice(int64_t offset, int64_t length) const {
+    if (offset + length > len_) throw std::runtime_error("the length + offset of the sliced RunEndBuffer cannot exceed the existing length");
+    return RunArray(run_ends_, n_runs_, values_, offset_ + offset, length);
+  }
+  // RunArray::get_physical_indices (run_array.rs:343-356, RunEndBuffer::get_physical_indices run.rs:321-378), on the host:
+  // the run of every logical index, or the largest index when it is out of bounds
+  template <class I>
+  Result<std::vector<size_t>> get_physical_indices(const std::vector<I> &logical) const {
+    std::vector<size_t> out(logical.size());
+    if (logical.empty()) return out;
+    const I mx = *std::max_element(logical.begin(), logical.end());
+    if ((uint64_t)mx >= (uint64_t)len_)
+      return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: Logical index " + std::to_string((uint64_t)mx) +
+                                                      " is out of bounds for RunArray of length " + std::to_string(len_)};
+    const std::vector<R> ends = run_ends();
+    for (size_t j = 0; j < logical.size(); ++j)
+      out[j] = (size_t)(std::upper_bound(ends.begin(), ends.end(), (int64_t)(offset_ + (int64_t)logical[j]),
+                                         [](int64_t x, R e) { return x < (int64_t)e; }) - ends.begin());
+    return out;
+  }
+  acu_run_array run_view() const {
+    acu_run_array r{};
+    r.run_end_dtype = sizeof(R) == 2 ? ACU_I16 : sizeof(R) == 4 ? ACU_I32 : ACU_I64;
+    r.run_ends = run_ends_.data();
+    r.n_runs = n_runs_;
+    r.offset = offset_;
+    r.len = len_;
+    return r;
+  }
+ protected:
+  const void *values_ptr() const override { return nullptr; }
+ private:
+  Buffer run_ends_;
+  int64_t n_runs_;
+  ArrayRef values_;
+  int64_t offset_;
+};
+using Int16RunArray = RunArray<int16_t>;
+using Int32RunArray = RunArray<int32_t>;
+using Int64RunArray = RunArray<int64_t>;
+
 // Datum (arrow-array/src/scalar.rs:78-152): an array, or a Scalar wrapping a 1-element array
 template <class A>
 struct Scalar {
@@ -613,7 +680,7 @@ inline ArrayRef make_primitive(DataType dt, Buffer values, int64_t len, std::opt
 }
 inline const char *dtype_display(DataType t) {
   static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64", "Boolean", "Utf8",
-                            "Decimal32", "Decimal64", "Decimal128", "List", "LargeList", "FixedSizeList"};
+                            "Decimal32", "Decimal64", "Decimal128", "List", "LargeList", "FixedSizeList", "RunEndEncoded"};
   return n[(int)t];
 }
 template <class A> std::string type_text(const A &a) {
@@ -992,6 +1059,141 @@ inline Result<ArrayRef> take(const LargeListArray &values, const Array &indices,
 }
 inline Result<ArrayRef> take(const FixedSizeListArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
   return detail::take_list(values, indices, options);
+}
+
+// ---- filter / take of RunEndEncoded (filter_run_end_array filter.rs:628-677, take_run take.rs:948-995) -------------------
+// acu_filter_run_end / acu_take_run_end write the new run ends and return the values child's plan / value indices; the
+// values child goes through the entry point of its own type. Values: primitive, Boolean and Utf8 (and lists, filter only).
+namespace detail {
+template <class T> ArrayRef slice_prim(const Array &a, int64_t off, int64_t len) {
+  return std::make_shared<PrimitiveArray<T>>(static_cast<const PrimitiveArray<T> &>(a).slice(off, len));
+}
+// Array::slice of the value types above
+inline ArrayRef slice_any(const Array &a, int64_t off, int64_t len) {
+  std::optional<NullBuffer> nulls = a.nulls();
+  if (nulls) { nulls->offset += off; nulls->len = len; nulls->null_count = -1; }
+  switch (a.data_type()) {
+    case DataType::Int8: return slice_prim<int8_t>(a, off, len);
+    case DataType::Int16: return slice_prim<int16_t>(a, off, len);
+    case DataType::Int32: return slice_prim<int32_t>(a, off, len);
+    case DataType::Int64: return slice_prim<int64_t>(a, off, len);
+    case DataType::UInt8: return slice_prim<uint8_t>(a, off, len);
+    case DataType::UInt16: return slice_prim<uint16_t>(a, off, len);
+    case DataType::UInt32: return slice_prim<uint32_t>(a, off, len);
+    case DataType::UInt64: return slice_prim<uint64_t>(a, off, len);
+    case DataType::Float32: return slice_prim<float>(a, off, len);
+    case DataType::Float64: return slice_prim<double>(a, off, len);
+    case DataType::Boolean: return std::make_shared<BooleanArray>(static_cast<const BooleanArray &>(a).slice(off, len));
+    case DataType::List: return std::make_shared<ListArray>(static_cast<const ListArray &>(a).slice(off, len));
+    case DataType::LargeList: return std::make_shared<LargeListArray>(static_cast<const LargeListArray &>(a).slice(off, len));
+    case DataType::FixedSizeList: {
+      const auto &f = static_cast<const FixedSizeListArray &>(a);
+      return std::make_shared<FixedSizeListArray>(f.value_length(), slice_any(*f.values(), off * f.value_length(), len * f.value_length()), len,
+                                                  nulls);
+    }
+    case DataType::Utf8: {  // the offsets from the new row 0; the value bytes are shared
+      const auto &s = static_cast<const StringArray &>(a);
+      std::vector<int32_t> o((size_t)a.len() + 1);
+      s.offsets().to_host(o.data(), o.size() * 4);
+      return std::make_shared<StringArray>(Buffer::from_host(o.data() + off, (size_t)(len + 1) * 4), s.value_data(), len, nulls);
+    }
+    default: throw std::runtime_error(std::string("RunArray values of type ") + dtype_display(a.data_type()) + " are not supported by this mirror");
+  }
+}
+template <class T> ArrayRef empty_prim() { return std::make_shared<PrimitiveArray<T>>(PrimitiveArray<T>::from(std::vector<T>{})); }
+// new_empty_array: no rows and no NullBuffer
+inline ArrayRef empty_like(const Array &a) {
+  switch (a.data_type()) {
+    case DataType::Int8: return empty_prim<int8_t>();
+    case DataType::Int16: return empty_prim<int16_t>();
+    case DataType::Int32: return empty_prim<int32_t>();
+    case DataType::Int64: return empty_prim<int64_t>();
+    case DataType::UInt8: return empty_prim<uint8_t>();
+    case DataType::UInt16: return empty_prim<uint16_t>();
+    case DataType::UInt32: return empty_prim<uint32_t>();
+    case DataType::UInt64: return empty_prim<uint64_t>();
+    case DataType::Float32: return empty_prim<float>();
+    case DataType::Float64: return empty_prim<double>();
+    case DataType::Boolean: return std::make_shared<BooleanArray>(BooleanArray::from(std::vector<bool>{}));
+    case DataType::Utf8: return std::make_shared<StringArray>(StringArray::from(std::vector<std::string>{}));
+    case DataType::List: return std::make_shared<ListArray>(ListArray::from({0}, empty_like(*list_values(a))));
+    case DataType::LargeList: return std::make_shared<LargeListArray>(LargeListArray::from({0}, empty_like(*list_values(a))));
+    case DataType::FixedSizeList:
+      return std::make_shared<FixedSizeListArray>(static_cast<const FixedSizeListArray &>(a).value_length(), empty_like(*list_values(a)), 0,
+                                                  std::nullopt);
+    default: throw std::runtime_error(std::string("RunArray values of type ") + dtype_display(a.data_type()) + " are not supported by this mirror");
+  }
+}
+}  // namespace detail
+
+template <class R>
+Result<ArrayRef> filter(const RunArray<R> &values, const BooleanArray &predicate) {
+  Context &c = Context::get();
+  acu_array p = predicate.view();
+  acu_filter_plan *plan = nullptr;
+  acu_status st = acu_filter_plan_create(c.raw(), &p, &plan);
+  if (st != ACU_OK) return c.last_error(st);
+  FilterPredicate pred(plan);
+  const acu_run_array r = values.run_view();
+  const int64_t count = pred.count();
+  Buffer ends = Buffer::allocate((size_t)std::max<int64_t>(std::min(count, values.num_runs()), 1) * sizeof(R));
+  int64_t runs = 0, start = 0;
+  acu_filter_plan *vplan = nullptr;
+  if ((st = acu_filter_run_end(c.raw(), plan, &r, ends.data(), &runs, &start, &vplan)) != ACU_OK) return c.last_error(st);
+  if (!vplan) {
+    if (acu_filter_plan_strategy(plan) == ACU_FILTER_ALL) return ArrayRef(std::make_shared<RunArray<R>>(values.slice(0, count)));
+    return ArrayRef(std::make_shared<RunArray<R>>(Buffer::allocate(0), 0, detail::empty_like(*values.values()), 0, 0));
+  }
+  FilterPredicate vpred(vplan);
+  auto v = detail::filter_any(*detail::slice_any(*values.values(), start, acu_filter_plan_len(vplan)), vpred, vplan);
+  if (v.is_err()) return v.unwrap_err();
+  std::vector<R> host((size_t)runs);
+  ends.to_host(host.data(), host.size() * sizeof(R));
+  return ArrayRef(std::make_shared<RunArray<R>>(ends, runs, v.unwrap(), 0, (int64_t)host.back()));  // the last new run end
+}
+
+template <class R>
+Result<ArrayRef> take(const RunArray<R> &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+  Context &c = Context::get();
+  const DataType it = indices.data_type();
+  if ((int)it > (int)DataType::UInt64)  // take.rs:103
+    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + detail::dtype_display(it)};
+  const Array &vals = *values.values();
+  acu_run_values rv{};
+  switch (vals.data_type()) {
+    case DataType::Boolean: rv.kind = ACU_RUN_VALUES_BOOLEAN; rv.array = vals.view(); break;
+    case DataType::Utf8: {
+      const auto &s = static_cast<const StringArray &>(vals);
+      rv.kind = ACU_RUN_VALUES_BYTES;
+      rv.width = 4;
+      rv.bytes.offsets = s.offsets().data();
+      rv.bytes.data = static_cast<const uint8_t *>(s.value_data().data());
+      rv.bytes.nulls = vals.view();
+      break;
+    }
+    case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: rv.kind = ACU_RUN_VALUES_NESTED; break;
+    default:
+      if (dtype_width(vals.data_type()) == 0)
+        throw std::runtime_error(std::string("RunArray values of type ") + detail::dtype_display(vals.data_type()) + " are not supported by this mirror");
+      rv.kind = ACU_RUN_VALUES_FIXED;
+      rv.width = dtype_width(vals.data_type());
+      rv.array = vals.view();
+  }
+  const int64_t m = indices.len();
+  const bool wide = it == DataType::Int64 || it == DataType::UInt64;  // ToIndices: UInt64 value indices
+  const acu_run_array r = values.run_view();
+  const acu_array ix = indices.view();
+  Buffer ends = Buffer::allocate((size_t)std::max<int64_t>(m, 1) * sizeof(R)), vi = Buffer::allocate((size_t)std::max<int64_t>(m, 1) * (wide ? 8 : 4));
+  int64_t runs = 0;
+  acu_status st = acu_take_run_end(c.raw(), &r, &rv, &ix, (acu_dtype)dtype_code(it), options && options->check_bounds ? 1 : 0, ends.data(),
+                                   vi.data(), &runs);
+  if (st != ACU_OK) return c.last_error(st);
+  if (m == 0) return ArrayRef(std::make_shared<RunArray<R>>(Buffer::allocate(0), 0, detail::empty_like(vals), 0, 0));
+  ArrayRef vix = wide ? ArrayRef(std::make_shared<PrimitiveArray<uint64_t>>(vi, runs, std::nullopt))
+                      : ArrayRef(std::make_shared<PrimitiveArray<uint32_t>>(vi, runs, std::nullopt));
+  auto v = take(vals, *vix);
+  if (v.is_err()) return v.unwrap_err();
+  return ArrayRef(std::make_shared<RunArray<R>>(ends, runs, v.unwrap(), 0, m));
 }
 
 // take.rs:1123-1133: every column gathered with the same indices, one synchronisation per (up to 64-column) call.

@@ -529,6 +529,84 @@ acu_status acu_cmp_byte_view(acu_ctx *ctx, acu_cmp_op op, const acu_view_array *
                              acu_array_out *out);
 
 /* ------------------------------------------------------------------------- */
+/* filter / take of RunEndEncoded columns                                    */
+/* ------------------------------------------------------------------------- */
+/* The run ends of a RunArray (arrow-array/src/array/run_array.rs, RunEndBuffer arrow-buffer/src/buffer/run.rs). The values
+ * child is NOT described here: the calls return a plan / value indices and the caller filters / takes the values child with
+ * them through the entry point of its type, as for a list's child.
+ *   run_end_dtype ACU_I16, ACU_I32 or ACU_I64;
+ *   run_ends      n_runs entries from physical entry 0 (not advanced by `offset`), aligned to their width;
+ *   offset, len   the logical slice: logical row i is the first physical run whose end is > offset + i.
+ * A malformed run-ends buffer (not strictly increasing, or not covering offset + len) gives an unspecified result, but
+ * every search is clamped to [0, n_runs). n_runs == 0 with len > 0, a negative offset / len or an unaligned pointer =>
+ * ACU_ERR_INVALID_ARGUMENT. */
+typedef struct acu_run_array {
+  int32_t run_end_dtype;
+  int32_t reserved;
+  const void *run_ends;
+  int64_t n_runs;
+  int64_t offset;
+  int64_t len;
+} acu_run_array;
+
+/* filter of a RunArray (filter_run_end_array, arrow-select/src/filter.rs:628-677). Predicate longer than the logical length =>
+ * ACU_ERR_INVALID_ARGUMENT "Filter predicate of length {p} is larger than target array of length {n}"; a shorter one drops the
+ * runs past it. Strategy NONE / ALL: nothing is written, *out_runs = 0 and *out_values_plan = NULL; the reference returns an
+ * empty RunArray / values.slice(0, count) (the run ends and values as they are, logical length count). Otherwise, over the
+ * physical runs [start, end] of the slice (get_start_physical_index / get_end_physical_index, run.rs:232-267), a run is kept
+ * iff a selected row lies in [previous clipped end, min(run_end - offset, p)), and its new end is the number of selected
+ * rows below that clipped end: out_run_ends (capacity min(count, n_runs) entries of the run-end type) gets the *out_runs
+ * kept runs' ends, *out_values_start = start, and *out_values_plan is a new plan over the values rows [start, end] (length
+ * end - start + 1) selecting the kept runs. The caller filters values.slice(start, end - start + 1) with it (a top-level
+ * filter of the values child, with that plan's own strategy) and destroys it. Synchronous; the physical bounds and the
+ * keep / rank pass count in ACU_K_FILTER_PLAN, the run-end compaction in ACU_K_FILTER. */
+acu_status acu_filter_run_end(acu_ctx *ctx, const acu_filter_plan *plan, const acu_run_array *ree, void *out_run_ends,
+                              int64_t *out_runs, int64_t *out_values_start, acu_filter_plan **out_values_plan);
+
+/* The values child of a RunArray as take_run's merge compares it (make_comparator with SortOptions::default(), arrow-ord/src/
+ * ord.rs): two nulls are equal, a null never equals a valid value, two valid values are equal iff
+ *   ACU_RUN_VALUES_FIXED   their `width` (1, 2, 4, 8 or 16) bytes are equal: integers, Decimal32/64/128, and floats under
+ *                          total_cmp (so -0.0 != 0.0 and NaNs with different payloads differ); `array` from physical row 0;
+ *   ACU_RUN_VALUES_BOOLEAN their bits are equal; `array` (values bitmap at values_offset) from physical row 0;
+ *   ACU_RUN_VALUES_BYTES   their bytes are equal; `bytes` with offsets of `width` 4 (Utf8 / Binary) or 8 (Large*);
+ *   ACU_RUN_VALUES_VIEW    their bytes are equal; `view` (Utf8View / BinaryView).
+ * ACU_RUN_VALUES_NESTED (a list or other nested child) is refused by acu_take_run_end (below); any other kind or width =>
+ * ACU_ERR_INVALID_ARGUMENT. */
+typedef enum acu_run_values_kind {
+  ACU_RUN_VALUES_FIXED = 0, ACU_RUN_VALUES_BOOLEAN = 1, ACU_RUN_VALUES_BYTES = 2, ACU_RUN_VALUES_VIEW = 3,
+  ACU_RUN_VALUES_NESTED = 4
+} acu_run_values_kind;
+typedef struct acu_run_values {
+  int32_t kind;
+  int32_t width;
+  acu_array array;
+  acu_bytes_array bytes;
+  acu_view_array view;
+} acu_run_values;
+
+/* take of a RunArray (take_run, arrow-select/src/take.rs:948-995). In order:
+ *   - a non-integer index type => ACU_ERR_INVALID_ARGUMENT "Take only supported for integers, got {type}";
+ *   - check_bounds != 0 (take.rs:167-209, null slots ignored): ACU_ERR_COMPUTE "Array index out of bounds, cannot get item
+ *     at index {i} from {len} entries";
+ *   - no indices: *out_runs = 0 (new_empty_array);
+ *   - the indices converted by ToIndices (take.rs:1030-1084: Int8 / Int16 sign-extend to UInt32, Int32 reinterprets as UInt32,
+ *     Int64 as UInt64), their largest VALUE, null slots included, at least len => ACU_ERR_INVALID_ARGUMENT "Logical index
+ *     {max} is out of bounds for RunArray of length {len}" (get_physical_indices, run.rs:321-378, run_array.rs:343-356);
+ *   - a nested values child, where take_run builds its comparator => ACU_ERR_NOT_YET_IMPLEMENTED "take of a RunEndEncoded
+ *     column with nested values is not yet implemented";
+ *   - more output rows than the run-end type holds (from_usize(..).unwrap()) => ACU_ERR_PANIC_OUT_OF_BOUNDS "called
+ *     `Option::unwrap()` on a `None` value".
+ * Output row ix >= 1 starts a new run iff its physical run differs from row ix - 1's and their values are not equal under
+ * `values` (above). out_run_ends gets the *out_runs run ends (the last is indices.len) in the run-end type; out_value_indices
+ * the physical row of each run's last row, UInt32 for indices that convert to UInt32 and UInt64 for Int64 / UInt64 (more than
+ * 2^32 runs with UInt32 indices => ACU_ERR_NOT_YET_IMPLEMENTED). Both need capacity indices.len entries. The caller then
+ * takes the values child with out_value_indices (no nulls) through the take entry point of its type. Synchronous; kernel
+ * time counts in ACU_K_TAKE, the boundary plan and its compaction in ACU_K_FILTER_PLAN / ACU_K_FILTER. */
+acu_status acu_take_run_end(acu_ctx *ctx, const acu_run_array *ree, const acu_run_values *values, const acu_array *indices,
+                            acu_dtype index_dtype, int32_t check_bounds, void *out_run_ends, void *out_value_indices,
+                            int64_t *out_runs);
+
+/* ------------------------------------------------------------------------- */
 /* like — arrow-string/src/like.rs                                           */
 /* ------------------------------------------------------------------------- */
 /* arrow-string/src/like.rs `enum Op` */

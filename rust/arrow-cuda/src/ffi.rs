@@ -191,6 +191,33 @@ pub struct acu_view_array {
     pub reserved: i32,
     pub nulls: acu_array,
 }
+
+/// acu_run_array: the run ends of a RunEndEncoded column from physical entry 0 and its logical slice; acu_run_values: its
+/// values child as take's run merge compares it (the values child itself is filtered / taken separately).
+pub const ACU_RUN_VALUES_FIXED: i32 = 0;
+pub const ACU_RUN_VALUES_BOOLEAN: i32 = 1;
+pub const ACU_RUN_VALUES_BYTES: i32 = 2;
+pub const ACU_RUN_VALUES_VIEW: i32 = 3;
+pub const ACU_RUN_VALUES_NESTED: i32 = 4;
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct acu_run_array {
+    pub run_end_dtype: i32,
+    pub reserved: i32,
+    pub run_ends: *const c_void,
+    pub n_runs: i64,
+    pub offset: i64,
+    pub len: i64,
+}
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct acu_run_values {
+    pub kind: i32,
+    pub width: i32,
+    pub array: acu_array,
+    pub bytes: acu_bytes_array,
+    pub view: acu_view_array,
+}
 #[repr(C)]
 pub struct acu_ipc_stream { _private: [u8; 0] }
 
@@ -237,6 +264,11 @@ extern "C" {
                          keep_null_ranges: i32, out_offsets: *mut c_void, out_nulls: *mut acu_array_out, child_index_dtype: i32,
                          out_child_indices: *mut c_void, capacity: i64, out_child_rows: *mut i64,
                          out_child_index_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_filter_run_end(ctx: *mut acu_ctx, plan: *const acu_filter_plan, ree: *const acu_run_array, out_run_ends: *mut c_void,
+                              out_runs: *mut i64, out_values_start: *mut i64, out_values_plan: *mut *mut acu_filter_plan) -> acu_status;
+    pub fn acu_take_run_end(ctx: *mut acu_ctx, ree: *const acu_run_array, values: *const acu_run_values, indices: *const acu_array,
+                            index_dtype: i32, check_bounds: i32, out_run_ends: *mut c_void, out_value_indices: *mut c_void,
+                            out_runs: *mut i64) -> acu_status;
     pub fn acu_arith(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_neg(ctx: *mut acu_ctx, dtype: i32, checked: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_decimal_arith(ctx: *mut acu_ctx, op: i32, lt: *const acu_decimal_type, a: *const acu_array, rt: *const acu_decimal_type,

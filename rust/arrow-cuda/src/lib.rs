@@ -295,6 +295,9 @@ pub mod compute {
             if let DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) = values.data_type() {
                 return list::filter(ctx, self.plan.raw, values, None);
             }
+            if let DataType::RunEndEncoded(_, _) = values.data_type() {
+                return run_end::filter(ctx, self.plan.raw, values);
+            }
             let v = DeviceArray::upload(ctx, values, false)?;
             let mut out = ColumnOut::new(ctx, values.data_type(), self.count(), v.data_bytes)?;
             let st = match kind_of(values.data_type())? {
@@ -356,6 +359,9 @@ pub mod compute {
         if let DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) = values.data_type() {
             return list::take(&ctx, values, indices, idt, check, false);
         }
+        if let DataType::RunEndEncoded(_, _) = values.data_type() {
+            return run_end::take(&ctx, values, indices, idt, check);
+        }
         let (v, ix) = (DeviceArray::upload(&ctx, values, false)?, DeviceArray::upload(&ctx, indices, false)?);
         let m = indices.len();
         let st;
@@ -387,6 +393,110 @@ pub mod compute {
         ctx.check(st)?; // ACU_ERR_PANIC_OUT_OF_BOUNDS panics inside, like take.rs:447
         out.finish(values.data_type())
     }
+    // ---- RunEndEncoded (filter_run_end_array filter.rs:628-677, take_run take.rs:948-995) -----------------------------
+    /// acu_filter_run_end / acu_take_run_end write the new run ends and return the plan / value indices of the values child,
+    /// which then goes through filter / take of its own type.
+    mod run_end {
+        use super::*;
+        use arrow_array::cast::AsArray;
+        use arrow_array::types::{Int16Type, Int32Type, Int64Type, RunEndIndexType, UInt32Type, UInt64Type};
+        use arrow_array::{new_empty_array, Array, RunArray};
+        use arrow_buffer::ScalarBuffer;
+
+        struct Ree { r: ffi::acu_run_array, width: usize, _ends: DeviceBuffer }
+
+        fn describe<R: RunEndIndexType>(ctx: &Context, a: &RunArray<R>) -> Result<Ree, ArrowError> {
+            let ends = a.run_ends();
+            let dev = DeviceBuffer::from_host(ctx, ends.inner().inner().as_slice())?;
+            let r = ffi::acu_run_array { run_end_dtype: dtype_code(&R::DATA_TYPE).unwrap(), reserved: 0, run_ends: dev.as_ptr(),
+                                         n_runs: ends.values().len() as i64, offset: ends.offset() as i64, len: ends.len() as i64 };
+            Ok(Ree { r, width: std::mem::size_of::<R::Native>(), _ends: dev })
+        }
+
+        fn run_array<R: RunEndIndexType>(ends: &DeviceBuffer, runs: usize, width: usize, values: &dyn Array) -> Result<ArrayRef, ArrowError> {
+            let re = PrimitiveArray::<R>::new(ScalarBuffer::new(ends.to_host(runs * width)?, 0, runs), None);
+            Ok(Arc::new(RunArray::<R>::try_new(&re, values)?))
+        }
+
+        pub(super) fn filter(ctx: &Context, plan: *mut ffi::acu_filter_plan, values: &dyn Array) -> Result<ArrayRef, ArrowError> {
+            match values.data_type() {
+                DataType::RunEndEncoded(f, _) => match f.data_type() {
+                    DataType::Int16 => filter_typed(ctx, plan, values.as_run::<Int16Type>()),
+                    DataType::Int32 => filter_typed(ctx, plan, values.as_run::<Int32Type>()),
+                    _ => filter_typed(ctx, plan, values.as_run::<Int64Type>()),
+                },
+                _ => unreachable!(),
+            }
+        }
+
+        fn filter_typed<R: RunEndIndexType>(ctx: &Context, plan: *mut ffi::acu_filter_plan, a: &RunArray<R>) -> Result<ArrayRef, ArrowError> {
+            let d = describe(ctx, a)?;
+            let count = unsafe { ffi::acu_filter_plan_count(plan) } as usize;
+            let ends = DeviceBuffer::allocate(ctx, count.min(a.run_ends().values().len()).max(1) * d.width)?;
+            let (mut runs, mut start, mut vplan) = (0i64, 0i64, std::ptr::null_mut());
+            ctx.check(unsafe { ffi::acu_filter_run_end(ctx.raw(), plan, &d.r, ends.as_ptr(), &mut runs, &mut start, &mut vplan) })?;
+            if vplan.is_null() {  // filter.rs:545-546: new_empty_array / values.slice(0, count)
+                return Ok(if unsafe { ffi::acu_filter_plan_strategy(plan) } == 1 { Array::slice(a, 0, count) } else { new_empty_array(a.data_type()) });
+            }
+            let vplan = Plan { ctx: ctx.clone(), raw: vplan };
+            let vlen = unsafe { ffi::acu_filter_plan_len(vplan.raw) } as usize;
+            let v = FilterPredicate { plan: vplan }.filter(a.values().slice(start as usize, vlen).as_ref())?;
+            run_array::<R>(&ends, runs as usize, d.width, v.as_ref())
+        }
+
+        pub(super) fn take(ctx: &Context, values: &dyn Array, indices: &dyn Array, idt: i32, check: i32) -> Result<ArrayRef, ArrowError> {
+            match values.data_type() {
+                DataType::RunEndEncoded(f, _) => match f.data_type() {
+                    DataType::Int16 => take_typed(ctx, values.as_run::<Int16Type>(), indices, idt, check),
+                    DataType::Int32 => take_typed(ctx, values.as_run::<Int32Type>(), indices, idt, check),
+                    _ => take_typed(ctx, values.as_run::<Int64Type>(), indices, idt, check),
+                },
+                _ => unreachable!(),
+            }
+        }
+
+        fn take_typed<R: RunEndIndexType>(ctx: &Context, a: &RunArray<R>, indices: &dyn Array, idt: i32, check: i32) -> Result<ArrayRef, ArrowError> {
+            let d = describe(ctx, a)?;
+            let vals = a.values();
+            let mut rv: ffi::acu_run_values = unsafe { std::mem::zeroed() };
+            let _up = match vals.data_type() {
+                DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) | DataType::RunEndEncoded(_, _) => {
+                    rv.kind = ffi::ACU_RUN_VALUES_NESTED;
+                    None
+                }
+                t => {
+                    let u = DeviceArray::upload(ctx, vals.as_ref(), false)?;
+                    match kind_of(t)? {
+                        Kind::Primitive(w) => { rv.kind = ffi::ACU_RUN_VALUES_FIXED; rv.width = w as i32; rv.array = *u.view(); }
+                        Kind::Boolean => { rv.kind = ffi::ACU_RUN_VALUES_BOOLEAN; rv.array = *u.view(); }
+                        Kind::Bytes(ob) => {
+                            rv.kind = ffi::ACU_RUN_VALUES_BYTES;
+                            rv.width = ob as i32;
+                            rv.bytes = ffi::acu_bytes_array { offsets: u.view().values, data: u.column.data, nulls: *u.view() };
+                        }
+                    }
+                    Some(u)
+                }
+            };
+            let ix = DeviceArray::upload(ctx, indices, false)?;
+            let m = indices.len();
+            let wide = matches!(indices.data_type(), DataType::Int64 | DataType::UInt64);  // ToIndices: UInt64 value indices
+            let ends = DeviceBuffer::allocate(ctx, m.max(1) * d.width)?;
+            let vi = DeviceBuffer::allocate(ctx, m.max(1) * if wide { 8 } else { 4 })?;
+            let mut runs = 0i64;
+            ctx.check(unsafe { ffi::acu_take_run_end(ctx.raw(), &d.r, &rv, ix.view(), idt, check, ends.as_ptr(), vi.as_ptr(), &mut runs) })?;
+            if m == 0 { return Ok(new_empty_array(a.data_type())); }  // take.rs:216-218
+            let n = runs as usize;
+            let vix: ArrayRef = if wide {
+                Arc::new(PrimitiveArray::<UInt64Type>::new(vi.to_host(n * 8)?.into(), None))
+            } else {
+                Arc::new(PrimitiveArray::<UInt32Type>::new(vi.to_host(n * 4)?.into(), None))
+            };
+            let v = super::take(vals.as_ref(), vix.as_ref(), None)?;
+            run_array::<R>(&ends, n, d.width, v.as_ref())
+        }
+    }
+
     // ---- List / LargeList / FixedSizeList (filter.rs:535-625, take.rs:646-795) ----------------------------------------
     /// One C call per level: acu_filter_list / acu_take_list return the child's plan / row map, and the child goes through
     /// filter / take of its own type (these functions again for a nested list). A List's child is extended
