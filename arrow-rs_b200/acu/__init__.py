@@ -474,6 +474,68 @@ class DeviceArray:
         self._owned = []
 
 
+class _Scope:
+    """The owner of everything one Context call allocates: device pointers, uploaded DeviceArrays, ArrayOuts, filter plans
+    (also those an entry point fills in as out-parameters) and host objects the device reads during the call, such as
+    view pointer tables. On exit it releases them in reverse order and always attempts every release. A release error
+    never replaces an exception already propagating; without one, the first release error is raised after the other
+    releases have run. It allocates through ctx.malloc and releases through ctx.free and ctx.lib.acu_filter_plan_destroy,
+    so a fake context can stand in for a Context.
+
+    The upload helpers take an `owned` list that device pointers are appended to and a `keep` list for host objects; a
+    scope stands in for the first (append) and its `keep` list for the second."""
+
+    def __init__(self, ctx):
+        self.ctx, self._held = ctx, []
+        self.keep = []  # host objects the device reads during the call, dropped on exit
+
+    def __enter__(self):
+        return self
+
+    def __exit__(self, exc_type, exc, tb):
+        first = None
+        while self._held:
+            release, x = self._held.pop()
+            try:
+                release(x)
+            except Exception as e:
+                first = e if first is None else first
+        self.keep.clear()
+        if first is not None and exc_type is None:
+            raise first
+        return False
+
+    def _hold(self, release, x):
+        self._held.append((release, x))
+        return x
+
+    def append(self, p):
+        """Own the device pointer p (a scope stands wherever a list of owned pointers is expected)."""
+        return self._hold(self.ctx.free, p)
+
+    def malloc(self, nbytes):
+        return self.append(self.ctx.malloc(nbytes))
+
+    def upload(self, h):
+        """Context.upload(h), freed on exit."""
+        return self._hold(DeviceArray.free, self.ctx.upload(h))
+
+    def out(self, nbytes_values, n_rows):
+        """An ArrayOut as Context.alloc_out allocates it."""
+        out = abi.ArrayOut()
+        out.values = self.malloc(nbytes_values + 16)
+        out.validity = self.malloc(bitmap_bytes(n_rows) + 8)
+        return out
+
+    def plan(self):
+        """A filter-plan handle for an entry point to fill in; destroyed on exit only if it was set."""
+        return self._hold(self._destroy_plan, C.c_void_p())
+
+    def _destroy_plan(self, plan):
+        if plan:
+            self.ctx.lib.acu_filter_plan_destroy(self.ctx.h, plan)
+
+
 class Context:
     """acu_ctx wrapper: one device, one stream."""
 
@@ -497,6 +559,10 @@ class Context:
 
     def __exit__(self, *a):
         self.close()
+
+    def _scope(self):
+        """`with self._scope() as s:` owns what one call allocates (see _Scope)."""
+        return _Scope(self)
 
     # -- errors / memory -----------------------------------------------------------------
     def check(self, st):
@@ -557,13 +623,28 @@ class Context:
         return DeviceArray(self, h.dtype, h.length, dv, h.values_offset, dn, h.validity_offset,
                            h.null_count if h.validity is not None else 0, h.is_scalar, owned)
 
+    def _copy_in(self, arr, owned, pad=16):
+        """A device copy of the numpy array `arr` in a buffer `pad` bytes longer; the pointer is appended to `owned`."""
+        arr = np.ascontiguousarray(arr)
+        p = self.malloc(arr.nbytes + pad)
+        owned.append(p)
+        if arr.nbytes:
+            self.h2d(p, arr)
+        return p
+
     def alloc_out(self, nbytes_values, n_rows):
         out = abi.ArrayOut()
         out.values = self.malloc(nbytes_values + 16)
         out.validity = self.malloc(bitmap_bytes(n_rows) + 8)
         return out
 
-    def download_out(self, out, dtype):
+    def _nulls_out(self, out, n):
+        """The NullBuffer of the n-row result `out` (an ArrayOut) as a HostArray without values."""
+        validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
+        return HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0)
+
+    def _read_out(self, out, dtype):
+        """The result ArrayOut `out` read back as a HostArray of `dtype`; its buffers stay allocated."""
         n = out.len
         if dtype == BOOL:
             vals = self.d2h(out.values, bitmap_bytes(n))
@@ -571,103 +652,94 @@ class Context:
             vals = self.d2h(out.values, n * 16, np.uint64).reshape(-1, 2)
         else:
             vals = self.d2h(out.values, n * abi.DTYPE_SIZE[dtype], NP_DTYPES[dtype])
-        validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-        res = HostArray(dtype, vals, n, validity, 0, 0, out.null_count if out.has_validity else 0)
-        self.free(out.values)
-        self.free(out.validity)
+        nulls = self._nulls_out(out, n)
+        return HostArray(dtype, vals, n, nulls.validity, 0, 0, nulls.null_count)
+
+    def download_out(self, out, dtype):
+        """_read_out, then the buffers of `out` are freed."""
+        res = self._read_out(out, dtype)
+        self._free_out(out)
         return res
 
     def _free_out(self, out):
         self.free(out.values)
         self.free(out.validity)
 
+    def _call_out(self, inputs, nbytes_values, n_rows, call, dtype):
+        """Upload the HostArrays `inputs` (None passes as a null descriptor), allocate an ArrayOut, run
+        call(*input descriptors, out) and read the result back as `dtype`."""
+        with self._scope() as s:
+            descs = [None if x is None else s.upload(x).descriptor() for x in inputs]
+            out = s.out(nbytes_values, n_rows)
+            self.check(call(*[None if d is None else C.byref(d) for d in descs], C.byref(out)))
+            return self._read_out(out, dtype)
+
+    def _bytes_out(self, s, fn, n, ob, data_capacity=None, child_step=None):
+        """A Utf8Column of n rows (ob-byte offsets) produced in two phases: the sizing call without a data buffer, then the
+        copy into `data_capacity` bytes (default: exactly the size). fn(d_out_off, d_out_data, capacity, total_ref, out)
+        calls the entry point; the buffers belong to the scope s. child_step as for _filter_with_plan."""
+        d_off = s.malloc((n + 1) * ob + 16)
+        out = s.out(0, n)
+        total = C.c_int64(0)
+        self.check(fn(d_off, None, 0, C.byref(total), C.byref(out)))
+        cap = total.value if data_capacity is None else data_capacity
+        d_data = s.malloc(cap + 16)
+        self.check(fn(d_off, d_data, cap, C.byref(total), C.byref(out)))
+        self._drop_empty_nulls(out, child_step)
+        return Utf8Column(self.d2h(d_off, (n + 1) * ob, np.int32 if ob == 4 else np.int64), self.d2h(d_data, total.value),
+                          self._nulls_out(out, n))
+
     # -- filter (arrow-select/src/filter.rs) ----------------------------------------------
+    def _plan(self, s, predicate):
+        """The filter plan of `predicate` (acu_filter_plan_create), owned by the scope s."""
+        pd = s.upload(predicate).descriptor()
+        plan = s.plan()
+        self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
+        return plan
+
     def filter(self, values, predicate):
         """arrow::compute::filter(values, predicate) for primitive and boolean arrays."""
-        dv, dp = self.upload(values), self.upload(predicate)
-        plan = C.c_void_p()
-        out = None
-        try:
-            pd = dp.descriptor()
-            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
-            count = self.lib.acu_filter_plan_count(plan)
-            out = self.alloc_out(count * values.width(), count)
-            vd = dv.descriptor()
-            if values.dtype == BOOL:
-                self.check(self.lib.acu_filter_boolean(self.h, plan, C.byref(vd), C.byref(out)))
-            else:
-                self.check(self.lib.acu_filter_primitive(self.h, plan, values.width(), C.byref(vd), C.byref(out)))
-            res, out = self.download_out(out, values.dtype), None
-            return values.like(res) if isinstance(values, DecimalArray) else res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            dv.free()
-            dp.free()
+        with self._scope() as s:
+            return self._filter_with_plan(values, self._plan(s, predicate))
 
     def filter_plan(self, predicate):
         """FilterBuilder::new(predicate).optimize().build() -> (count, strategy)."""
-        dp = self.upload(predicate)
-        plan = C.c_void_p()
-        try:
-            pd = dp.descriptor()
-            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
+        with self._scope() as s:
+            plan = self._plan(s, predicate)
             return self.lib.acu_filter_plan_count(plan), self.lib.acu_filter_plan_strategy(plan)
-        finally:
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            dp.free()
 
     def filter_slices(self, predicate):
         """SlicesIterator::new(&prep_null_mask_filter(predicate)).collect() -> [(start, end)] (filter.rs:44-77)."""
-        dp = self.upload(predicate)
-        plan = C.c_void_p()
-        out = None
-        try:
-            pd = dp.descriptor()
-            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
+        with self._scope() as s:
+            plan = self._plan(s, predicate)
             n = C.c_int64(0)
             self.check(self.lib.acu_filter_plan_slices(self.h, plan, None, 0, C.byref(n)))
             if n.value == 0:
                 return []
-            out = self.malloc(n.value * 16 + 16)
+            out = s.malloc(n.value * 16 + 16)
             self.check(self.lib.acu_filter_plan_slices(self.h, plan, out, n.value, C.byref(n)))
             pairs = self.d2h(out, n.value * 16, np.uint64).reshape(-1, 2)
             return [(int(a), int(b)) for a, b in pairs]
-        finally:
-            if out:
-                self.free(out)
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            dp.free()
 
     def chain(self, col, pred, idx, a, b, arith_op=ADD, agg_op=SUM, cmp_with=None):
         """filter(col, pred) -> take(col, idx) -> arith(a, b) -> aggregate(taken) queued in ONE stream-ordered section
         (acu_async_begin ... acu_results_fetch): one synchronisation for the five calls. With cmp_with = (op, x, y) the
         predicate is cmp(op, x, y) computed inside the section too (`pred` is ignored). Returns
         (filtered, taken, arith result, aggregate or None); raises the first error in call order at the fetch."""
-        ups = [self.upload(x) for x in (col, idx, a, b)]
-        dcol, didx, da, db = ups
-        plan = C.c_void_p()
-        outs = []
         n_pred = (cmp_with[2].length if cmp_with[1].is_scalar else cmp_with[1].length) if cmp_with else pred.length
-        try:
+        with self._scope() as s:
+            dcol, didx, da, db = (s.upload(x) for x in (col, idx, a, b))
+            plan = s.plan()
             if cmp_with:
-                cx, cy = self.upload(cmp_with[1]), self.upload(cmp_with[2])
-                ups += [cx, cy]
-                o_pred = self.alloc_out(bitmap_bytes(n_pred), n_pred)
-                outs.append(o_pred)
+                cx, cy = s.upload(cmp_with[1]), s.upload(cmp_with[2])
+                o_pred = s.out(bitmap_bytes(n_pred), n_pred)
             else:
-                dpred = self.upload(pred)
-                ups.append(dpred)
+                dpred = s.upload(pred)
             # outputs of a filter whose plan is pending are sized for the predicate length
-            o_f = self.alloc_out(max(n_pred, 1) * col.width(), n_pred)
-            o_t = self.alloc_out(idx.length * col.width(), idx.length)
+            o_f = s.out(max(n_pred, 1) * col.width(), n_pred)
+            o_t = s.out(idx.length * col.width(), idx.length)
             n_ar = b.length if a.is_scalar and not b.is_scalar else a.length
-            o_a = self.alloc_out(n_ar * a.width(), n_ar)
-            outs += [o_f, o_t, o_a]
+            o_a = s.out(n_ar * a.width(), n_ar)
             bits, cnt = C.c_uint64(0), C.c_int64(0)
             cd, idd, ad, bd = dcol.descriptor(), didx.descriptor(), da.descriptor(), db.descriptor()
             self.async_begin()
@@ -703,184 +775,96 @@ class Context:
                     pass
                 raise
             self.results_fetch()
-            pred_out = self.download_out(outs.pop(0), BOOL) if cmp_with else None
-            filtered = self.download_out(o_f, col.dtype)
-            taken_h = self.download_out(o_t, col.dtype)
-            added = self.download_out(o_a, a.dtype)
-            outs = []
+            pred_out = self._read_out(o_pred, BOOL) if cmp_with else None
+            filtered = self._read_out(o_f, col.dtype)
+            taken_h = self._read_out(o_t, col.dtype)
+            added = self._read_out(o_a, a.dtype)
             agg = None
             if do_agg and cnt.value != 0:
                 agg = np.array([bits.value], dtype=np.uint64).view(NP_DTYPES[col.dtype])[0].item()
             res = (filtered, taken_h, added, agg)
             return res + (pred_out,) if cmp_with else res
-        finally:
-            for o in outs:
-                self._free_out(o)
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            for u in ups:
-                u.free()
 
     # -- take (arrow-select/src/take.rs) ----------------------------------------------------
     def take(self, values, indices, check_bounds=False):
-        dv, di = self.upload(values), self.upload(indices)
-        out = self.alloc_out(indices.length * values.width(), indices.length)
-        try:
-            vd, idd = dv.descriptor(), di.descriptor()
-            if values.dtype == BOOL:
-                self.check(self.lib.acu_take_boolean(self.h, C.byref(vd), C.byref(idd), indices.dtype, int(check_bounds), C.byref(out)))
-            else:
-                self.check(self.lib.acu_take_primitive(self.h, values.width(), C.byref(vd), C.byref(idd), indices.dtype,
-                                                       int(check_bounds), C.byref(out)))
-            res, out = self.download_out(out, values.dtype), None
-            return values.like(res) if isinstance(values, DecimalArray) else res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            dv.free()
-            di.free()
+        with self._scope() as s:
+            return self._take_level(values, s.upload(indices).descriptor(), indices.dtype, check_bounds, False)
 
     # -- variable width (Utf8) ---------------------------------------------------------------
     def take_bytes(self, offsets, data, nulls_of, indices, check_bounds=False):
         """take on a Utf8/Binary array given as (offsets np.int32/int64, data np.uint8, nulls_of HostArray
         carrying validity/len). Returns (offsets, data, nulls HostArray)."""
-        ob = offsets.dtype.itemsize
-        d_off = self.malloc(offsets.nbytes + 16)
-        self.h2d(d_off, offsets)
-        d_data = self.malloc(data.nbytes + 16)
-        if data.nbytes:
-            self.h2d(d_data, data)
-        dn, di = self.upload(nulls_of), self.upload(indices)
-        m = indices.length
-        d_out_off = self.malloc((m + 1) * ob + 16)
-        out = self.alloc_out(0, m)
-        d_out_data = None
-        try:
-            total = C.c_int64(0)
-            nd, idd = dn.descriptor(), di.descriptor()
-            self.check(self.lib.acu_take_bytes(self.h, ob, d_off, d_data, C.byref(nd), C.byref(idd), indices.dtype,
-                                               int(check_bounds), d_out_off, None, 0, C.byref(total), C.byref(out)))
-            d_out_data = self.malloc(total.value + 16)
-            self.check(self.lib.acu_take_bytes(self.h, ob, d_off, d_data, C.byref(nd), C.byref(idd), indices.dtype,
-                                               int(check_bounds), d_out_off, d_out_data, total.value, C.byref(total), C.byref(out)))
-            o = self.d2h(d_out_off, (m + 1) * ob, offsets.dtype)
-            b = self.d2h(d_out_data, total.value)
-            validity = self.d2h(out.validity, bitmap_bytes(m)) if out.has_validity else None
-            return o, b, HostArray(U8, np.zeros(0, np.uint8), m, validity, 0, 0, out.null_count if out.has_validity else 0)
-        finally:
-            self._free_out(out)
-            for p in (d_off, d_data, d_out_off, d_out_data):
-                self.free(p)
-            dn.free()
-            di.free()
+        r = self.take(Utf8Column(offsets, data, nulls_of), indices, check_bounds)
+        return r.offsets, r.data, r.nulls
 
     def filter_bytes(self, offsets, data, nulls_of, predicate):
-        ob = offsets.dtype.itemsize
-        d_off = self.malloc(offsets.nbytes + 16)
-        self.h2d(d_off, offsets)
-        d_data = self.malloc(data.nbytes + 16)
-        if data.nbytes:
-            self.h2d(d_data, data)
-        dn, dp = self.upload(nulls_of), self.upload(predicate)
-        plan = C.c_void_p()
-        d_out_off = d_out_data = None
-        out = None
-        try:
-            pd = dp.descriptor()
-            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
-            count = self.lib.acu_filter_plan_count(plan)
-            d_out_off = self.malloc((count + 1) * ob + 16)
-            out = self.alloc_out(0, count)
-            total = C.c_int64(0)
-            nd = dn.descriptor()
-            self.check(self.lib.acu_filter_bytes(self.h, plan, ob, d_off, d_data, C.byref(nd), d_out_off, None, 0,
-                                                 C.byref(total), C.byref(out)))
-            d_out_data = self.malloc(total.value + 16)
-            self.check(self.lib.acu_filter_bytes(self.h, plan, ob, d_off, d_data, C.byref(nd), d_out_off, d_out_data,
-                                                 total.value, C.byref(total), C.byref(out)))
-            o = self.d2h(d_out_off, (count + 1) * ob, offsets.dtype)
-            b = self.d2h(d_out_data, total.value)
-            validity = self.d2h(out.validity, bitmap_bytes(count)) if out.has_validity else None
-            return o, b, HostArray(U8, np.zeros(0, np.uint8), count, validity, 0, 0, out.null_count if out.has_validity else 0)
-        finally:
-            if out is not None:
-                self._free_out(out)
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            for p in (d_off, d_data, d_out_off, d_out_data):
-                self.free(p)
-            dn.free()
-            dp.free()
+        r = self.filter(Utf8Column(offsets, data, nulls_of), predicate)
+        return r.offsets, r.data, r.nulls
 
     # -- RecordBatch level (filter.rs:225-244, take.rs:1123-1133) ----------------------------
     # A batch is a list of columns; a column is a HostArray (primitive / boolean) or a
     # Utf8Column(offsets, data, nulls). Results keep the column order and kinds.
-    def _upload_columns(self, columns):
-        cols = (abi.Column * len(columns))()
-        owned = []
-        for c, col in enumerate(columns):
-            if isinstance(col, Utf8Column):
-                d_off = self.malloc(col.offsets.nbytes + 16)
-                self.h2d(d_off, col.offsets)
-                d_data = self.malloc(col.data.nbytes + 16)
-                if col.data.nbytes:
-                    self.h2d(d_data, col.data)
-                dn = self.upload(col.nulls)
-                owned += [("ptr", d_off), ("ptr", d_data), ("arr", dn)]
-                cols[c].kind, cols[c].width = abi.COL_BYTES, col.offsets.dtype.itemsize
-                cols[c].array = dn.descriptor()
-                cols[c].array.values = d_off
-                cols[c].array.values_offset = 0
-                cols[c].data = d_data
-            else:
-                dv = self.upload(col)
-                owned.append(("arr", dv))
-                cols[c].kind = abi.COL_BOOLEAN if col.dtype == BOOL else abi.COL_PRIMITIVE
-                cols[c].width = 0 if col.dtype == BOOL else col.width()
-                cols[c].array = dv.descriptor()
-        return cols, owned
+    @staticmethod
+    def _column_kind(col):
+        """(acu_column kind, width) of a host column: a Utf8Column's width is its offset width."""
+        if isinstance(col, Utf8Column):
+            return abi.COL_BYTES, col.offsets.dtype.itemsize
+        return (abi.COL_BOOLEAN, 0) if col.dtype == BOOL else (abi.COL_PRIMITIVE, col.width())
 
-    def _alloc_column_outs(self, columns, rows, data_caps):
+    def _upload_columns(self, columns, s):
+        cols = (abi.Column * len(columns))()
+        for c, col in enumerate(columns):
+            cols[c].kind, cols[c].width = self._column_kind(col)
+            if isinstance(col, Utf8Column):
+                bd = self._upload_bytes_col(col, s)
+                cols[c].array = bd.nulls
+                cols[c].array.values = bd.offsets
+                cols[c].data = bd.data
+            else:
+                cols[c].array = s.upload(col).descriptor()
+        return cols
+
+    def _alloc_column_outs(self, columns, rows, data_caps, owned=None):
+        """ColumnOuts for `columns`; the device pointers are appended to `owned` (None: _free_columns releases them)."""
+        owned = [] if owned is None else owned
+
+        def malloc(nbytes):
+            p = self.malloc(nbytes)
+            owned.append(p)
+            return p
         outs = (abi.ColumnOut * len(columns))()
         for c, col in enumerate(columns):
             if isinstance(col, Utf8Column):
-                outs[c].array.values = self.malloc((rows + 1) * col.offsets.dtype.itemsize + 16)
-                outs[c].array.validity = self.malloc(bitmap_bytes(rows) + 8)
-                outs[c].data = self.malloc(data_caps[c] + 16)
+                outs[c].array.values = malloc((rows + 1) * col.offsets.dtype.itemsize + 16)
+                outs[c].array.validity = malloc(bitmap_bytes(rows) + 8)
+                outs[c].data = malloc(data_caps[c] + 16)
                 outs[c].data_capacity = data_caps[c]
             else:
-                outs[c].array.values = self.malloc((bitmap_bytes(rows) if col.dtype == BOOL else rows * col.width()) + 16)
-                outs[c].array.validity = self.malloc(bitmap_bytes(rows) + 8)
+                outs[c].array.values = malloc((bitmap_bytes(rows) if col.dtype == BOOL else rows * col.width()) + 16)
+                outs[c].array.validity = malloc(bitmap_bytes(rows) + 8)
         return outs
 
-    def _download_columns(self, columns, outs):
-        res = []
-        for c, col in enumerate(columns):
-            o = outs[c]
-            n = o.array.len
-            validity = self.d2h(o.array.validity, bitmap_bytes(n)) if o.array.has_validity else None
-            nc = o.array.null_count if o.array.has_validity else 0
-            if isinstance(col, Utf8Column):
-                offs = self.d2h(o.array.values, (n + 1) * col.offsets.dtype.itemsize, col.offsets.dtype)
-                data = self.d2h(o.data, o.data_len)
-                res.append(Utf8Column(offs, data, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, nc)))
-            elif col.dtype == BOOL:
-                res.append(HostArray(BOOL, self.d2h(o.array.values, bitmap_bytes(n)), n, validity, 0, 0, nc))
-            else:
-                res.append(HostArray(col.dtype, self.d2h(o.array.values, n * col.width(), NP_DTYPES[col.dtype]), n, validity, 0, 0, nc))
-        return res
-
     def _free_columns(self, owned, outs):
-        for kind, x in owned:
-            if kind == "ptr":
-                self.free(x)
-            else:
-                x.free()
-        if outs is not None:
-            for o in outs:
-                for p in (o.array.values, o.array.validity, o.data):
-                    if p:
-                        self.free(p)
+        """Release the device pointers `owned` and the buffers of the ColumnOuts `outs` (None: none), as _free_out releases
+        an ArrayOut, for callers that hold them without a scope."""
+        with self._scope() as s:
+            for p in list(owned) + [q for o in outs or () for q in (o.array.values, o.array.validity, o.data)]:
+                s.append(p)
+
+    def _read_column(self, kind, width, dtype, arr, data, data_len=None):
+        """A column read back from the device buffers of an acu_column / acu_column_out: `arr` is an ArrayOut of its values
+        (the offsets of a COL_BYTES column, `width` bytes each), validity and rows; `data` the bytes of a COL_BYTES column,
+        data_len of them (None: up to the last offset). Returns a Utf8Column, or a HostArray of `dtype`."""
+        if kind != abi.COL_BYTES:
+            return self._read_out(arr, BOOL if kind == abi.COL_BOOLEAN else dtype)
+        n = arr.len
+        nulls = self._nulls_out(arr, n)
+        offs = self.d2h(arr.values, (n + 1) * width, np.int32 if width == 4 else np.int64)
+        return Utf8Column(offs, self.d2h(data, (int(offs[-1]) if n else 0) if data_len is None else data_len), nulls)
+
+    def _download_columns(self, columns, outs):
+        return [self._read_column(*self._column_kind(col), col.dtype if isinstance(col, HostArray) else None, o.array, o.data,
+                                  o.data_len) for col, o in zip(columns, outs)]
 
     # -- Arrow IPC stream -> HBM (arrow-ipc/src/reader.rs StreamReader) ---------------------------
     def ipc_read_stream(self, stream_bytes, on_batch=None):
@@ -910,18 +894,9 @@ class Context:
                     continue
                 out = []
                 for i, (name, kind, width, dtype, _) in enumerate(schema):
-                    c, m = cols[i], rows.value
-                    validity = self.d2h(c.array.validity, bitmap_bytes(m)) if c.array.validity else None
-                    nc = c.array.null_count if c.array.validity else 0
-                    if kind == abi.COL_BYTES:
-                        odt = np.int32 if width == 4 else np.int64
-                        offs = self.d2h(c.array.values, (m + 1) * width, odt)
-                        data = self.d2h(c.data, int(offs[-1]) if m else 0)
-                        out.append(Utf8Column(offs, data, HostArray(U8, np.zeros(0, np.uint8), m, validity, 0, 0, nc)))
-                    elif kind == abi.COL_BOOLEAN:
-                        out.append(HostArray(BOOL, self.d2h(c.array.values, bitmap_bytes(m)), m, validity, 0, 0, nc))
-                    else:
-                        out.append(HostArray(dtype, self.d2h(c.array.values, m * width, NP_DTYPES[dtype]), m, validity, 0, 0, nc))
+                    a = cols[i].array
+                    arr = abi.ArrayOut(a.values, a.validity, rows.value, a.null_count, 1 if a.validity else 0)
+                    out.append(self._read_column(kind, width, dtype, arr, cols[i].data))
                 batches.append(out)
             return schema, batches
         finally:
@@ -930,61 +905,45 @@ class Context:
     # -- concat / concat_batches (arrow-select/src/concat.rs:495-640) ---------------------------
     def concat(self, columns):
         """arrow::compute::concat(&[..]): columns = HostArrays or Utf8Columns of one type."""
-        cols, owned = self._upload_columns(columns) if columns else ((abi.Column * 1)(), [])
-        outs = None
-        try:
+        with self._scope() as s:
+            cols = self._upload_columns(columns, s) if columns else (abi.Column * 1)()
             rows = sum(c.length for c in columns)
             proto = columns[:1] if columns else [HostArray(U8, np.zeros(0, np.uint8), 0)]
             caps = [sum(int(c.data.nbytes) for c in columns)] if columns and isinstance(columns[0], Utf8Column) else [0]
-            outs = self._alloc_column_outs(proto, max(rows, 1), caps)
+            outs = self._alloc_column_outs(proto, max(rows, 1), caps, s)
             self.check(self.lib.acu_concat(self.h, len(columns), cols, outs))
             return self._download_columns(proto, outs)[0]
-        finally:
-            self._free_columns(owned, outs)
 
     def concat_batches(self, batches):
         """arrow::compute::concat_batches(schema, batches): batches = lists of columns (same schema)."""
         ncols = len(batches[0]) if batches else 0
         flat = [c for b in batches for c in b]
-        cols, owned = self._upload_columns(flat) if flat else ((abi.Column * 1)(), [])
-        outs = None
-        try:
+        with self._scope() as s:
+            cols = self._upload_columns(flat, s) if flat else (abi.Column * 1)()
             rows = sum(b[0].length for b in batches) if ncols else 0
             proto = list(batches[0]) if batches else []
             caps = [sum(int(b[c].data.nbytes) for b in batches) if isinstance(proto[c], Utf8Column) else 0 for c in range(ncols)]
-            outs = self._alloc_column_outs(proto, max(rows, 1), caps) if ncols else (abi.ColumnOut * 1)()
+            outs = self._alloc_column_outs(proto, max(rows, 1), caps, s) if ncols else (abi.ColumnOut * 1)()
             n = C.c_int64(0)
             self.check(self.lib.acu_concat_batches(self.h, len(batches), ncols, cols, outs, C.byref(n)))
             return self._download_columns(proto, outs) if ncols else []
-        finally:
-            self._free_columns(owned, outs if ncols else None)
 
     def filter_record_batch(self, columns, predicate):
         """arrow::compute::filter_record_batch: one plan, every column, one synchronisation."""
-        cols, owned = self._upload_columns(columns)
-        dp = self.upload(predicate)
-        plan = C.c_void_p()
-        outs = None
-        try:
-            pd = dp.descriptor()
-            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
+        with self._scope() as s:
+            cols = self._upload_columns(columns, s)
+            plan = self._plan(s, predicate)
             count = self.lib.acu_filter_plan_count(plan)
             caps = [int(col.data.nbytes) if isinstance(col, Utf8Column) else 0 for col in columns]
-            outs = self._alloc_column_outs(columns, count, caps)
+            outs = self._alloc_column_outs(columns, count, caps, s)
             self.check(self.lib.acu_filter_record_batch(self.h, plan, len(columns), cols, outs))
             return self._download_columns(columns, outs)
-        finally:
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            self._free_columns(owned, outs)
-            dp.free()
 
     def take_record_batch(self, columns, indices, check_bounds=False, data_capacity=None):
         """arrow::compute::take_record_batch / take_arrays."""
-        cols, owned = self._upload_columns(columns)
-        di = self.upload(indices)
-        outs = None
-        try:
+        with self._scope() as s:
+            cols = self._upload_columns(columns, s)
+            idd = s.upload(indices).descriptor()
             m = indices.length
             caps = []
             for col in columns:
@@ -993,53 +952,34 @@ class Context:
                     caps.append(int(data_capacity) if data_capacity is not None else int((lens.max() if lens.size else 0) * m))
                 else:
                     caps.append(0)
-            outs = self._alloc_column_outs(columns, m, caps)
-            idd = di.descriptor()
+            outs = self._alloc_column_outs(columns, m, caps, s)
             self.check(self.lib.acu_take_record_batch(self.h, len(columns), cols, C.byref(idd), indices.dtype, int(check_bounds), outs))
             return self._download_columns(columns, outs)
-        finally:
-            self._free_columns(owned, outs)
-            di.free()
 
     def aggregate_columns(self, ops, columns):
         """[sum|min|max|product|bit_and|bit_or|bit_xor](column) for several primitive columns with one synchronisation ->
         [(value|None)]."""
         n = len(columns)
-        das = [self.upload(c) for c in columns]
-        try:
-            arrs = (abi.Array * n)(*[d.descriptor() for d in das])
+        with self._scope() as s:
+            arrs = (abi.Array * n)(*[s.upload(c).descriptor() for c in columns])
             dts = (C.c_int32 * n)(*[c.dtype for c in columns])
             opv = (C.c_int32 * n)(*ops)
             bits, cnts = (C.c_uint64 * n)(), (C.c_int64 * n)()
             self.check(self.lib.acu_aggregate_columns(self.h, n, dts, opv, arrs, bits, cnts))
-            out = []
-            for i, c in enumerate(columns):
-                if cnts[i] == 0:
-                    out.append(None)
-                else:
-                    raw = np.array([bits[i]], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[c.dtype]]
-                    out.append(raw.view(NP_DTYPES[c.dtype])[0].item())
-            return out
-        finally:
-            for d in das:
-                d.free()
+        out = []
+        for i, c in enumerate(columns):
+            if cnts[i] == 0:
+                out.append(None)
+            else:
+                raw = np.array([bits[i]], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[c.dtype]]
+                out.append(raw.view(NP_DTYPES[c.dtype])[0].item())
+        return out
 
     # -- numeric (arrow-arith/src/numeric.rs) -----------------------------------------------
     def arith(self, op, a, b):
         assert a.dtype == b.dtype
         n = b.length if a.is_scalar and not b.is_scalar else a.length
-        da, db = self.upload(a), self.upload(b)
-        out = self.alloc_out(n * a.width(), n)
-        try:
-            ad, bd = da.descriptor(), db.descriptor()
-            self.check(self.lib.acu_arith(self.h, a.dtype, op, C.byref(ad), C.byref(bd), C.byref(out)))
-            res, out = self.download_out(out, a.dtype), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
-            db.free()
+        return self._call_out((a, b), n * a.width(), n, lambda ad, bd, out: self.lib.acu_arith(self.h, a.dtype, op, ad, bd, out), a.dtype)
 
     def add(self, a, b): return self.arith(ADD, a, b)
     def add_wrapping(self, a, b): return self.arith(ADD_WRAPPING, a, b)
@@ -1051,17 +991,8 @@ class Context:
     def rem(self, a, b): return self.arith(REM, a, b)
 
     def neg(self, a, checked=True):
-        da = self.upload(a)
-        out = self.alloc_out(a.length * a.width(), a.length)
-        try:
-            ad = da.descriptor()
-            self.check(self.lib.acu_neg(self.h, a.dtype, int(checked), C.byref(ad), C.byref(out)))
-            res, out = self.download_out(out, a.dtype), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
+        return self._call_out((a,), a.length * a.width(), a.length,
+                              lambda ad, out: self.lib.acu_neg(self.h, a.dtype, int(checked), ad, out), a.dtype)
 
     def neg_wrapping(self, a): return self.neg(a, checked=False)
 
@@ -1070,21 +1001,8 @@ class Context:
         """bitwise_and / or / xor / and_not / shift_left / shift_right (acu_bitwise_op) of two integer HostArrays, their
         _scalar forms (b a scalar HostArray) and bitwise_not (op = BITWISE_NOT, b None)."""
         assert b is None or a.dtype == b.dtype
-        da = self.upload(a)
-        db = self.upload(b) if b is not None else None
-        out = self.alloc_out(a.length * a.width(), a.length)
-        try:
-            ad = da.descriptor()
-            bd = db.descriptor() if db is not None else None
-            self.check(self.lib.acu_bitwise(self.h, a.dtype, op, C.byref(ad), C.byref(bd) if bd is not None else None, C.byref(out)))
-            res, out = self.download_out(out, a.dtype), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
-            if db is not None:
-                db.free()
+        return self._call_out((a, b), a.length * a.width(), a.length,
+                              lambda ad, bd, out: self.lib.acu_bitwise(self.h, a.dtype, op, ad, bd, out), a.dtype)
 
     def bitwise_and(self, a, b): return self.bitwise(abi.BITWISE_AND, a, b)
     def bitwise_or(self, a, b): return self.bitwise(abi.BITWISE_OR, a, b)
@@ -1099,20 +1017,10 @@ class Context:
         """add / sub / mul / div / rem (acu_arith_op) of two DecimalArrays (either may be a scalar): a DecimalArray of the
         reference's result type; raises ArrowError with the reference's text."""
         n = b.length if a.is_scalar and not b.is_scalar else a.length
-        da, db = self.upload(a), self.upload(b)
-        out = self.alloc_out(n * a.byte_width, n)
-        try:
-            lt, rt, ot = (abi.DecimalType(x.byte_width, x.precision, x.scale) for x in (a, b, a))
-            ad, bd = da.descriptor(), db.descriptor()
-            self.check(self.lib.acu_decimal_arith(self.h, op, C.byref(lt), C.byref(ad), C.byref(rt), C.byref(bd), C.byref(ot),
-                                                  C.byref(out)))
-            res, out = self.download_out(out, a.dtype), None
-            return a.like(res, ot.precision, ot.scale)
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
-            db.free()
+        lt, rt, ot = (abi.DecimalType(x.byte_width, x.precision, x.scale) for x in (a, b, a))
+        res = self._call_out((a, b), n * a.byte_width, n, lambda ad, bd, out: self.lib.acu_decimal_arith(
+            self.h, op, C.byref(lt), ad, C.byref(rt), bd, C.byref(ot), out), a.dtype)
+        return a.like(res, ot.precision, ot.scale)
 
     def decimal_add(self, a, b): return self.decimal_arith(ADD, a, b)
     def decimal_sub(self, a, b): return self.decimal_arith(SUB, a, b)
@@ -1143,18 +1051,7 @@ class Context:
         self.check_decimal_cmp(op, a, b)
         assert a.dtype == b.dtype
         n = b.length if a.is_scalar else a.length
-        da, db = self.upload(a), self.upload(b)
-        out = self.alloc_out(bitmap_bytes(n), n)
-        try:
-            ad, bd = da.descriptor(), db.descriptor()
-            self.check(self.lib.acu_cmp(self.h, a.dtype, op, C.byref(ad), C.byref(bd), C.byref(out)))
-            res, out = self.download_out(out, BOOL), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
-            db.free()
+        return self._call_out((a, b), bitmap_bytes(n), n, lambda ad, bd, out: self.lib.acu_cmp(self.h, a.dtype, op, ad, bd, out), BOOL)
 
     # -- cmp on Utf8 / Binary and Utf8View / BinaryView operands (cmp.rs:783-898) -----------------
     def _upload_nulls(self, nulls, owned):
@@ -1163,145 +1060,81 @@ class Context:
         d.validity_offset = nulls.validity_offset
         d.null_count = nulls.null_count if nulls.validity is not None else 0
         if nulls.validity is not None:
-            dn = self.malloc(nulls.validity.nbytes + 8)
-            self.h2d(dn, nulls.validity)
-            owned.append(dn)
-            d.validity = dn
+            d.validity = self._copy_in(nulls.validity, owned, 8)
         return d
 
     def _upload_bytes_col(self, col, owned):
         """acu_bytes_array of a Utf8Column uploaded to HBM (device pointers appended to `owned`)."""
         d = abi.BytesArray()
-        d_off, d_data = self.malloc(col.offsets.nbytes + 16), self.malloc(col.data.nbytes + 16)
-        owned += [d_off, d_data]
-        self.h2d(d_off, col.offsets)
-        if col.data.nbytes:
-            self.h2d(d_data, col.data)
-        d.offsets, d.data, d.nulls = d_off, d_data, self._upload_nulls(col.nulls, owned)
+        d.offsets, d.data = self._copy_in(col.offsets, owned), self._copy_in(col.data, owned)
+        d.nulls = self._upload_nulls(col.nulls, owned)
         return d
 
     def _upload_view_col(self, col, owned, keep):
         """acu_view_array of a ViewColumn uploaded to HBM; the host pointer table is appended to `keep`."""
         d = abi.ViewArray()
-        views = np.ascontiguousarray(col.views)
-        d_views = self.malloc(views.nbytes + 16)
-        owned.append(d_views)
-        if views.nbytes:
-            self.h2d(d_views, views)
-        ptrs = []
-        for buf in col.buffers:
-            db = self.malloc(buf.nbytes + 16)
-            owned.append(db)
-            self.h2d(db, buf)
-            ptrs.append(db)
+        d.views = self._copy_in(col.views, owned)
+        ptrs = [self._copy_in(buf, owned) for buf in col.buffers]
         table = (C.c_void_p * max(len(ptrs), 1))(*ptrs)
         keep.append(table)
-        d.views, d.buffers, d.n_buffers = d_views, table, len(ptrs)
+        d.buffers, d.n_buffers = table, len(ptrs)
         d.nulls = self._upload_nulls(col.nulls, owned)
         return d
+
+    def _upload_fsb(self, col, owned):
+        d = self._upload_nulls(col.nulls, owned)
+        d.values = self._copy_in(col.values, owned)
+        return d
+
+    def _bytes_predicate(self, a, b, call):
+        """A boolean result of two Utf8Column or two ViewColumn operands (nulls.is_scalar marks a Datum scalar):
+        call(a descriptor, b descriptor, out) calls the entry point."""
+        n = max(a.nulls.length if not a.nulls.is_scalar else 0, b.nulls.length if not b.nulls.is_scalar else 0, 1)
+        with self._scope() as s:
+            out = s.out(bitmap_bytes(n), n)
+            if isinstance(a, Utf8Column):
+                da, db = self._upload_bytes_col(a, s), self._upload_bytes_col(b, s)
+            else:
+                da, db = self._upload_view_col(a, s, s.keep), self._upload_view_col(b, s, s.keep)
+            self.check(call(C.byref(da), C.byref(db), C.byref(out)))
+            return self._read_out(out, BOOL)
 
     def cmp_bytes(self, op, a, b):
         """a, b: Utf8Column (offsets, data, nulls); nulls.is_scalar marks a Datum scalar."""
         assert a.offsets.dtype == b.offsets.dtype
-        owned = []
-        n = max(a.nulls.length if not a.nulls.is_scalar else 0, b.nulls.length if not b.nulls.is_scalar else 0, 1)
-        out = self.alloc_out(bitmap_bytes(n), n)
-        try:
-            descs = [self._upload_bytes_col(col, owned) for col in (a, b)]
-            self.check(self.lib.acu_cmp_bytes(self.h, a.offsets.dtype.itemsize, op, C.byref(descs[0]), C.byref(descs[1]), C.byref(out)))
-            res, out = self.download_out(out, BOOL), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            for p in owned:
-                self.free(p)
+        return self._bytes_predicate(a, b, lambda da, db, out: self.lib.acu_cmp_bytes(self.h, a.offsets.dtype.itemsize, op, da, db, out))
 
     def cmp_view(self, op, a, b):
         """a, b: ViewColumn."""
-        owned = []
-        n = max(a.length if not a.nulls.is_scalar else 0, b.length if not b.nulls.is_scalar else 0, 1)
-        out = self.alloc_out(bitmap_bytes(n), n)
-        try:
-            keep = []
-            descs = [self._upload_view_col(col, owned, keep) for col in (a, b)]
-            self.check(self.lib.acu_cmp_byte_view(self.h, op, C.byref(descs[0]), C.byref(descs[1]), C.byref(out)))
-            res, out = self.download_out(out, BOOL), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            for p in owned:
-                self.free(p)
+        return self._bytes_predicate(a, b, lambda da, db, out: self.lib.acu_cmp_byte_view(self.h, op, da, db, out))
 
     # -- like / ilike / contains / starts_with / ends_with / eq_ignore_ascii_case (arrow-string/src/like.rs) -------
     def like_bytes(self, op, a, b, is_utf8=True):
         """a (haystack), b (pattern / needle): Utf8Column; is_utf8=False for Binary / LargeBinary."""
         assert a.offsets.dtype == b.offsets.dtype
-        owned = []
-        n = max(a.nulls.length if not a.nulls.is_scalar else 0, b.nulls.length if not b.nulls.is_scalar else 0, 1)
-        out = self.alloc_out(bitmap_bytes(n), n)
-        try:
-            descs = [self._upload_bytes_col(col, owned) for col in (a, b)]
-            self.check(self.lib.acu_like_bytes(self.h, a.offsets.dtype.itemsize, int(is_utf8), op, C.byref(descs[0]), C.byref(descs[1]),
-                                               C.byref(out)))
-            res, out = self.download_out(out, BOOL), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            for p in owned:
-                self.free(p)
+        return self._bytes_predicate(a, b, lambda da, db, out: self.lib.acu_like_bytes(self.h, a.offsets.dtype.itemsize, int(is_utf8),
+                                                                                          op, da, db, out))
 
     def like_view(self, op, a, b, is_utf8=True):
         """a (haystack), b (pattern / needle): ViewColumn; is_utf8=False for BinaryView."""
-        owned = []
-        n = max(a.length if not a.nulls.is_scalar else 0, b.length if not b.nulls.is_scalar else 0, 1)
-        out = self.alloc_out(bitmap_bytes(n), n)
-        try:
-            keep = []
-            descs = [self._upload_view_col(col, owned, keep) for col in (a, b)]
-            self.check(self.lib.acu_like_byte_view(self.h, int(is_utf8), op, C.byref(descs[0]), C.byref(descs[1]), C.byref(out)))
-            res, out = self.download_out(out, BOOL), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            for p in owned:
-                self.free(p)
+        return self._bytes_predicate(a, b, lambda da, db, out: self.lib.acu_like_byte_view(self.h, int(is_utf8), op, da, db, out))
 
     # -- length / bit_length / substring / substring_by_char (arrow-string/src/length.rs, substring.rs) ------
-    def _upload_fsb(self, col, owned):
-        d = self._upload_nulls(col.nulls, owned)
-        dv = self.malloc(col.values.nbytes + 16)
-        owned.append(dv)
-        if col.values.nbytes:
-            self.h2d(dv, col.values)
-        d.values = dv
-        return d
-
     def _length(self, op, col):
-        owned, keep = [], []
         n = col.length
         wide = isinstance(col, Utf8Column) and col.offsets.dtype == np.int64
-        out = self.alloc_out(n * (8 if wide else 4), n)
-        try:
+        with self._scope() as s:
+            out = s.out(n * (8 if wide else 4), n)
             if isinstance(col, Utf8Column):
-                d = self._upload_bytes_col(col, owned)
+                d = self._upload_bytes_col(col, s)
                 self.check(self.lib.acu_length_bytes(self.h, col.offsets.dtype.itemsize, op, C.byref(d), C.byref(out)))
             elif isinstance(col, ViewColumn):
-                d = self._upload_view_col(col, owned, keep)
+                d = self._upload_view_col(col, s, s.keep)
                 self.check(self.lib.acu_length_byte_view(self.h, op, C.byref(d), C.byref(out)))
             else:
-                d = self._upload_fsb(col, owned)
+                d = self._upload_fsb(col, s)
                 self.check(self.lib.acu_length_fixed_size_binary(self.h, col.width, op, C.byref(d), C.byref(out)))
-            res, out = self.download_out(out, I64 if wide else I32), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            for p in owned:
-                self.free(p)
+            return self._read_out(out, I64 if wide else I32)
 
     def length(self, col):
         """arrow_string::length::length of a Utf8Column, ViewColumn or FixedSizeBinaryColumn: an Int32 (Int64 for i64 offsets)
@@ -1311,81 +1144,39 @@ class Context:
     def bit_length(self, col):
         return self._length(abi.BIT_LENGTH, col)
 
-    def _substring_offsets(self, fn, col, data_capacity):
-        """Two-phase byte-array substring: the sizing call (no data buffer), then the copy into `data_capacity` bytes
-        (default: exactly the size). fn(d_out_off, d_out_data, capacity, total_ref, out) calls the entry point."""
-        n, ob = col.length, col.offsets.dtype.itemsize
-        d_out_off = self.malloc((n + 1) * ob + 16)
-        out = self.alloc_out(0, n)
-        d_out_data = None
-        try:
-            total = C.c_int64(0)
-            self.check(fn(d_out_off, None, 0, C.byref(total), C.byref(out)))
-            cap = total.value if data_capacity is None else data_capacity
-            d_out_data = self.malloc(cap + 16)
-            self.check(fn(d_out_off, d_out_data, cap, C.byref(total), C.byref(out)))
-            o = self.d2h(d_out_off, (n + 1) * ob, col.offsets.dtype)
-            b = self.d2h(d_out_data, total.value)
-            validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-            return Utf8Column(o, b, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
-        finally:
-            self._free_out(out)
-            for p in (d_out_off, d_out_data):
-                self.free(p)
-
     def substring(self, col, start, length=None, is_utf8=True, data_capacity=None):
         """arrow_string::substring::substring(col, start, length) of a Utf8Column (is_utf8=False: Binary / LargeBinary),
         ViewColumn (is_utf8=False: BinaryView) or FixedSizeBinaryColumn. A view result shares the input's data buffers."""
-        owned, keep = [], []
         has_len, ln = (0, 0) if length is None else (1, int(length))
-        try:
+        n = col.length
+        with self._scope() as s:
             if isinstance(col, Utf8Column):
-                d = self._upload_bytes_col(col, owned)
+                d = self._upload_bytes_col(col, s)
                 ob = col.offsets.dtype.itemsize
-                return self._substring_offsets(
-                    lambda oo, od, cap, tot, out: self.lib.acu_substring_bytes(self.h, ob, int(is_utf8), int(start), has_len, ln, C.byref(d),
-                                                                              col.data.nbytes, oo, od, cap, tot, out), col, data_capacity)
-            n = col.length
+                return self._bytes_out(s, lambda oo, od, cap, tot, out: self.lib.acu_substring_bytes(
+                    self.h, ob, int(is_utf8), int(start), has_len, ln, C.byref(d), col.data.nbytes, oo, od, cap, tot, out), n, ob, data_capacity)
             if isinstance(col, ViewColumn):
-                d = self._upload_view_col(col, owned, keep)
-                d_views = self.malloc(n * 16 + 16)
-                owned.append(d_views)
-                out = self.alloc_out(0, n)
-                try:
-                    self.check(self.lib.acu_substring_byte_view(self.h, int(is_utf8), int(start), has_len, ln, C.byref(d), d_views, C.byref(out)))
-                    views = self.d2h(d_views, n * 16).reshape(n, 16)
-                    validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-                finally:
-                    self._free_out(out)
-                nulls = HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0)
-                return ViewColumn(views, col.buffers, nulls)
-            d = self._upload_fsb(col, owned)
-            out = self.alloc_out(n * col.width, n)
-            try:
-                w = C.c_int32(0)
-                self.check(self.lib.acu_substring_fixed_size_binary(self.h, col.width, int(start), has_len, ln, C.byref(d), C.byref(w), C.byref(out)))
-                vals = self.d2h(out.values, n * w.value).reshape(n, w.value)
-                validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-            finally:
-                self._free_out(out)
-            return FixedSizeBinaryColumn(vals, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
-        finally:
-            for p in owned:
-                self.free(p)
+                d = self._upload_view_col(col, s, s.keep)
+                d_views = s.malloc(n * 16 + 16)
+                out = s.out(0, n)
+                self.check(self.lib.acu_substring_byte_view(self.h, int(is_utf8), int(start), has_len, ln, C.byref(d), d_views, C.byref(out)))
+                views = self.d2h(d_views, n * 16).reshape(n, 16)
+                return ViewColumn(views, col.buffers, self._nulls_out(out, n))
+            d = self._upload_fsb(col, s)
+            out = s.out(n * col.width, n)
+            w = C.c_int32(0)
+            self.check(self.lib.acu_substring_fixed_size_binary(self.h, col.width, int(start), has_len, ln, C.byref(d), C.byref(w), C.byref(out)))
+            vals = self.d2h(out.values, n * w.value).reshape(n, w.value)
+            return FixedSizeBinaryColumn(vals, self._nulls_out(out, n))
 
     def substring_by_char(self, col, start, length=None, data_capacity=None):
         """arrow_string::substring::substring_by_char of a Utf8Column (Utf8 / LargeUtf8)."""
-        owned = []
         has_len, ln = (0, 0) if length is None else (1, int(length))
-        try:
-            d = self._upload_bytes_col(col, owned)
+        with self._scope() as s:
+            d = self._upload_bytes_col(col, s)
             ob = col.offsets.dtype.itemsize
-            return self._substring_offsets(
-                lambda oo, od, cap, tot, out: self.lib.acu_substring_by_char(self.h, ob, int(start), has_len, ln, C.byref(d), oo, od, cap, tot, out),
-                col, data_capacity)
-        finally:
-            for p in owned:
-                self.free(p)
+            return self._bytes_out(s, lambda oo, od, cap, tot, out: self.lib.acu_substring_by_char(
+                self.h, ob, int(start), has_len, ln, C.byref(d), oo, od, cap, tot, out), col.length, ob, data_capacity)
 
     # -- concat_elements (arrow-string/src/concat_elements.rs) ------------------------------------------------------
     @staticmethod
@@ -1404,26 +1195,6 @@ class Context:
             return "Boolean"
         return abi.DTYPE_NAMES[col.dtype].capitalize().replace("Uint", "UInt")
 
-    def _concat_offsets(self, fn, n, ob, data_capacity):
-        """Two-phase byte-array concat, as _substring_offsets: fn(d_out_off, d_out_data, capacity, total_ref, out)."""
-        d_out_off = self.malloc((n + 1) * ob + 16)
-        out = self.alloc_out(0, n)
-        d_out_data = None
-        try:
-            total = C.c_int64(0)
-            self.check(fn(d_out_off, None, 0, C.byref(total), C.byref(out)))
-            cap = total.value if data_capacity is None else data_capacity
-            d_out_data = self.malloc(cap + 16)
-            self.check(fn(d_out_off, d_out_data, cap, C.byref(total), C.byref(out)))
-            o = self.d2h(d_out_off, (n + 1) * ob, np.int32 if ob == 4 else np.int64)
-            b = self.d2h(d_out_data, total.value)
-            validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-            return Utf8Column(o, b, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
-        finally:
-            self._free_out(out)
-            for p in (d_out_off, d_out_data):
-                self.free(p)
-
     def concat_elements(self, l, r, is_utf8=True, data_capacity=None):
         """arrow_string::concat_elements::concat_elements_dyn(l, r) of two Utf8Column (is_utf8=False: Binary / LargeBinary),
         ViewColumn (is_utf8=False: BinaryView) or FixedSizeBinaryColumn operands of one type. A view result has one new data
@@ -1434,152 +1205,82 @@ class Context:
             raise ArrowError(abi.ERR_COMPUTE, f"Compute error: Cannot concat arrays of different types: {lt} != {rt}")
         if not isinstance(l, (Utf8Column, ViewColumn, FixedSizeBinaryColumn)):
             raise ArrowError(abi.ERR_NOT_YET_IMPLEMENTED, f"Not yet implemented: concat not supported for {lt}")
-        owned, keep = [], []
         n = l.length
-        try:
+        with self._scope() as s:
             if isinstance(l, Utf8Column):
-                dl, dr = self._upload_bytes_col(l, owned), self._upload_bytes_col(r, owned)
+                dl, dr = self._upload_bytes_col(l, s), self._upload_bytes_col(r, s)
                 ob = l.offsets.dtype.itemsize
-                return self._concat_offsets(
-                    lambda oo, od, cap, tot, out: self.lib.acu_concat_elements_bytes(self.h, ob, C.byref(dl), C.byref(dr), oo, od, cap, tot, out),
-                    n, ob, data_capacity)
+                return self._bytes_out(s, lambda oo, od, cap, tot, out: self.lib.acu_concat_elements_bytes(
+                    self.h, ob, C.byref(dl), C.byref(dr), oo, od, cap, tot, out), n, ob, data_capacity)
             if isinstance(l, ViewColumn):
-                dl, dr = self._upload_view_col(l, owned, keep), self._upload_view_col(r, owned, keep)
-                d_views = self.malloc(n * 16 + 16)
-                owned.append(d_views)
-                out = self.alloc_out(0, n)
-                try:
-                    total = C.c_int64(0)
-                    self.check(self.lib.acu_concat_elements_byte_view(self.h, C.byref(dl), C.byref(dr), None, None, 0, C.byref(total), C.byref(out)))
-                    cap = total.value if data_capacity is None else data_capacity
-                    d_data = self.malloc(cap + 16)
-                    owned.append(d_data)
-                    self.check(self.lib.acu_concat_elements_byte_view(self.h, C.byref(dl), C.byref(dr), d_views, d_data, cap, C.byref(total),
+                dl, dr = self._upload_view_col(l, s, s.keep), self._upload_view_col(r, s, s.keep)
+                d_views = s.malloc(n * 16 + 16)
+                out = s.out(0, n)
+                total = C.c_int64(0)
+                self.check(self.lib.acu_concat_elements_byte_view(self.h, C.byref(dl), C.byref(dr), None, None, 0, C.byref(total), C.byref(out)))
+                cap = total.value if data_capacity is None else data_capacity
+                d_data = s.malloc(cap + 16)
+                self.check(self.lib.acu_concat_elements_byte_view(self.h, C.byref(dl), C.byref(dr), d_views, d_data, cap, C.byref(total),
+                                                                  C.byref(out)))
+                views = self.d2h(d_views, n * 16).reshape(n, 16)
+                buffers = [self.d2h(d_data, total.value)] if total.value else []
+                return ViewColumn(views, buffers, self._nulls_out(out, n))
+            dl, dr = self._upload_fsb(l, s), self._upload_fsb(r, s)
+            out = s.out(n * (l.width + r.width), n)
+            w = C.c_int32(0)
+            self.check(self.lib.acu_concat_elements_fixed_size_binary(self.h, l.width, C.byref(dl), r.width, C.byref(dr), C.byref(w),
                                                                       C.byref(out)))
-                    views = self.d2h(d_views, n * 16).reshape(n, 16)
-                    buffers = [self.d2h(d_data, total.value)] if total.value else []
-                    validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-                finally:
-                    self._free_out(out)
-                nulls = HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0)
-                return ViewColumn(views, buffers, nulls)
-            dl, dr = self._upload_fsb(l, owned), self._upload_fsb(r, owned)
-            out = self.alloc_out(n * (l.width + r.width), n)
-            try:
-                w = C.c_int32(0)
-                self.check(self.lib.acu_concat_elements_fixed_size_binary(self.h, l.width, C.byref(dl), r.width, C.byref(dr), C.byref(w),
-                                                                          C.byref(out)))
-                vals = self.d2h(out.values, n * w.value).reshape(n, w.value)
-                validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-            finally:
-                self._free_out(out)
-            return FixedSizeBinaryColumn(vals, HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0))
-        finally:
-            for p in owned:
-                self.free(p)
+            vals = self.d2h(out.values, n * w.value).reshape(n, w.value)
+            return FixedSizeBinaryColumn(vals, self._nulls_out(out, n))
 
     def concat_elements_utf8_many(self, cols, data_capacity=None):
         """arrow_string::concat_elements::concat_elements_utf8_many of Utf8Column operands with one offset width (the device
         path is the same for Binary / LargeBinary operands)."""
-        owned = []
-        try:
-            descs = (abi.BytesArray * max(len(cols), 1))(*[self._upload_bytes_col(c, owned) for c in cols])
+        with self._scope() as s:
+            descs = (abi.BytesArray * max(len(cols), 1))(*[self._upload_bytes_col(c, s) for c in cols])
             ob = cols[0].offsets.dtype.itemsize if cols else 4
             n = cols[0].length if cols else 0
-            return self._concat_offsets(
-                lambda oo, od, cap, tot, out: self.lib.acu_concat_elements_bytes_many(self.h, ob, len(cols), descs, oo, od, cap, tot, out),
-                n, ob, data_capacity)
-        finally:
-            for p in owned:
-                self.free(p)
+            return self._bytes_out(s, lambda oo, od, cap, tot, out: self.lib.acu_concat_elements_bytes_many(
+                self.h, ob, len(cols), descs, oo, od, cap, tot, out), n, ob, data_capacity)
 
     # -- fused compare -> filter (cmp.rs:220-382 feeding filter.rs:254-273) -------------------
     def filter_cmp(self, values, op, a, b):
         """filter(values, &cmp::op(a, b)?) with the predicate never materialised: the comparison writes the filter plan."""
         self.check_decimal_cmp(op, a, b)
         assert a.dtype == b.dtype
-        dv, da, db = self.upload(values), self.upload(a), self.upload(b)
-        plan = C.c_void_p()
-        out = None
-        try:
-            ad, bd = da.descriptor(), db.descriptor()
+        with self._scope() as s:
+            ad, bd = s.upload(a).descriptor(), s.upload(b).descriptor()
+            plan = s.plan()
             self.check(self.lib.acu_filter_plan_create_cmp(self.h, a.dtype, op, C.byref(ad), C.byref(bd), C.byref(plan)))
-            count = self.lib.acu_filter_plan_count(plan)
-            out = self.alloc_out(count * values.width(), count)
-            vd = dv.descriptor()
-            if values.dtype == BOOL:
-                self.check(self.lib.acu_filter_boolean(self.h, plan, C.byref(vd), C.byref(out)))
-            else:
-                self.check(self.lib.acu_filter_primitive(self.h, plan, values.width(), C.byref(vd), C.byref(out)))
-            strategy = self.lib.acu_filter_plan_strategy(plan)
-            res, out = self.download_out(out, values.dtype), None
-            return (values.like(res) if isinstance(values, DecimalArray) else res), (count, strategy)
-        finally:
-            if out is not None:
-                self._free_out(out)
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            dv.free()
-            da.free()
-            db.free()
+            res = self._filter_with_plan(values, plan)
+            return res, (self.lib.acu_filter_plan_count(plan), self.lib.acu_filter_plan_strategy(plan))
 
     # -- nullif / zip (arrow-select/src/nullif.rs, zip.rs) ------------------------------------
     def nullif(self, left, right):
         """arrow::compute::nullif(left, right): same values, validity &= !(right is Some(true))."""
-        dl, dr = self.upload(left), self.upload(right)
-        out = self.alloc_out(0, max(left.length, 1))
-        try:
-            ld, rd = dl.descriptor(), dr.descriptor()
+        with self._scope() as s:
+            ld, rd = s.upload(left).descriptor(), s.upload(right).descriptor()
+            out = s.out(0, max(left.length, 1))
             self.check(self.lib.acu_nullif(self.h, C.byref(ld), C.byref(rd), C.byref(out)))
             n = out.len
-            validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-            if n == 0:  # the array is returned as it is
-                return left
-            # the result shares left's value buffer (logical slice starting at row 0)
-            vals = left.values if left.dtype == BOOL else left.values[:n]
-            return HostArray(left.dtype, vals, n, validity, 0, left.values_offset if left.dtype == BOOL else 0,
-                             out.null_count if out.has_validity else 0)
-        finally:
-            self._free_out(out)
-            dl.free()
-            dr.free()
+            nulls = self._nulls_out(out, n)
+        if n == 0:  # the array is returned as it is
+            return left
+        # the result shares left's value buffer (logical slice starting at row 0)
+        vals = left.values if left.dtype == BOOL else left.values[:n]
+        return HostArray(left.dtype, vals, n, nulls.validity, 0, left.values_offset if left.dtype == BOOL else 0, nulls.null_count)
 
     def zip(self, mask, truthy, falsy):
         """arrow::compute::zip(mask, truthy, falsy) for primitive arrays / scalars."""
         assert truthy.dtype == falsy.dtype and truthy.dtype != BOOL
-        dm, dt, df = self.upload(mask), self.upload(truthy), self.upload(falsy)
         n = mask.length
-        out = self.alloc_out(n * truthy.width(), max(n, 1))
-        try:
-            md, td, fd = dm.descriptor(), dt.descriptor(), df.descriptor()
-            self.check(self.lib.acu_zip(self.h, truthy.width(), C.byref(md), C.byref(td), C.byref(fd), C.byref(out)))
-            res, out = self.download_out(out, truthy.dtype), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            dm.free()
-            dt.free()
-            df.free()
+        return self._call_out((mask, truthy, falsy), n * truthy.width(), max(n, 1),
+                              lambda md, td, fd, out: self.lib.acu_zip(self.h, truthy.width(), md, td, fd, out), truthy.dtype)
 
     # -- boolean (arrow-arith/src/boolean.rs) -------------------------------------------------
     def boolean(self, op, a, b=None):
-        da = self.upload(a)
-        db = self.upload(b) if b is not None else None
         n = max(a.length, 1)
-        out = self.alloc_out(bitmap_bytes(n), n)
-        try:
-            ad = da.descriptor()
-            bd = db.descriptor() if db is not None else None
-            self.check(self.lib.acu_boolean(self.h, op, C.byref(ad), C.byref(bd) if bd is not None else None, C.byref(out)))
-            res, out = self.download_out(out, BOOL), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
-            if db is not None:
-                db.free()
+        return self._call_out((a, b), bitmap_bytes(n), n, lambda ad, bd, out: self.lib.acu_boolean(self.h, op, ad, bd, out), BOOL)
 
     def and_(self, a, b): return self.boolean(abi.BOOL_AND, a, b)
     def or_(self, a, b): return self.boolean(abi.BOOL_OR, a, b)
@@ -1601,79 +1302,52 @@ class Context:
 
     # -- cast (arrow-cast/src/cast/mod.rs) -----------------------------------------------------
     def cast(self, a, to_dtype, safe=True):
-        da = self.upload(a)
-        out = self.alloc_out(a.length * abi.DTYPE_SIZE[to_dtype], a.length)
-        try:
-            ad = da.descriptor()
-            self.check(self.lib.acu_cast_numeric(self.h, a.dtype, to_dtype, int(safe), C.byref(ad), C.byref(out)))
-            res, out = self.download_out(out, to_dtype), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
+        return self._call_out((a,), a.length * abi.DTYPE_SIZE[to_dtype], a.length,
+                              lambda ad, out: self.lib.acu_cast_numeric(self.h, a.dtype, to_dtype, int(safe), ad, out), to_dtype)
 
     # -- decimal casts (arrow-cast/src/cast/decimal.rs) -------------------------------------------
     def cast_decimal(self, a, byte_width, precision, scale, safe=True):
         """cast(DecimalArray, Decimal{32,64,128}(precision, scale)) -> DecimalArray."""
         ft, tt = abi.DecimalType(a.byte_width, a.precision, a.scale), abi.DecimalType(byte_width, precision, scale)
-        res = self._cast_call(a, byte_width, lambda ad, out: self.lib.acu_cast_decimal(self.h, C.byref(ft), C.byref(tt), int(safe),
-                                                                                     C.byref(ad), C.byref(out)), _DECIMAL_NATIVE[byte_width])
+        res = self._call_out((a,), a.length * byte_width, a.length, lambda ad, out: self.lib.acu_cast_decimal(
+            self.h, C.byref(ft), C.byref(tt), int(safe), ad, out), _DECIMAL_NATIVE[byte_width])
         return DecimalArray(byte_width, precision, scale, res.values, res.length, res.validity, res.validity_offset, res.null_count)
 
     def cast_to_decimal(self, a, byte_width, precision, scale, safe=True):
         """cast(Int8..UInt64 / Float32 / Float64 HostArray, Decimal{32,64,128}(precision, scale)) -> DecimalArray."""
         tt = abi.DecimalType(byte_width, precision, scale)
-        res = self._cast_call(a, byte_width, lambda ad, out: self.lib.acu_cast_to_decimal(self.h, a.dtype, C.byref(tt), int(safe),
-                                                                                        C.byref(ad), C.byref(out)), _DECIMAL_NATIVE[byte_width])
+        res = self._call_out((a,), a.length * byte_width, a.length, lambda ad, out: self.lib.acu_cast_to_decimal(
+            self.h, a.dtype, C.byref(tt), int(safe), ad, out), _DECIMAL_NATIVE[byte_width])
         return DecimalArray(byte_width, precision, scale, res.values, res.length, res.validity, res.validity_offset, res.null_count)
 
     def cast_from_decimal(self, a, to_dtype, safe=True):
         """cast(DecimalArray, Int8..UInt64 / Float32 / Float64) -> HostArray."""
         ft = abi.DecimalType(a.byte_width, a.precision, a.scale)
-        return self._cast_call(a, abi.DTYPE_SIZE[to_dtype], lambda ad, out: self.lib.acu_cast_from_decimal(
-            self.h, C.byref(ft), to_dtype, int(safe), C.byref(ad), C.byref(out)), to_dtype)
-
-    def _cast_call(self, a, out_width, call, out_dtype):
-        da = self.upload(a)
-        out = self.alloc_out(a.length * out_width, a.length)
-        try:
-            self.check(call(da.descriptor(), out))
-            res, out = self.download_out(out, out_dtype), None
-            return res
-        finally:
-            if out is not None:
-                self._free_out(out)
-            da.free()
+        return self._call_out((a,), a.length * abi.DTYPE_SIZE[to_dtype], a.length, lambda ad, out: self.lib.acu_cast_from_decimal(
+            self.h, C.byref(ft), to_dtype, int(safe), ad, out), to_dtype)
 
     # -- aggregate (arrow-arith/src/aggregate.rs) ----------------------------------------------
     def aggregate(self, op, a):
         if a.dtype == abi.I128:
             return self.aggregate_i128(op, a)
-        da = self.upload(a)
-        try:
-            bits, cnt = C.c_uint64(0), C.c_int64(0)
-            ad = da.descriptor()
+        bits, cnt = C.c_uint64(0), C.c_int64(0)
+        with self._scope() as s:
+            ad = s.upload(a).descriptor()
             self.check(self.lib.acu_aggregate(self.h, a.dtype, op, C.byref(ad), C.byref(bits), C.byref(cnt)))
-            if cnt.value == 0:
-                return None
-            return np.array([bits.value], dtype=np.uint64).view(NP_DTYPES[a.dtype])[0].item() if abi.DTYPE_SIZE[a.dtype] == 8 \
-                else np.array([bits.value], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[a.dtype]].view(NP_DTYPES[a.dtype])[0].item()
-        finally:
-            da.free()
+        if cnt.value == 0:
+            return None
+        return np.array([bits.value], dtype=np.uint64).view(NP_DTYPES[a.dtype])[0].item() if abi.DTYPE_SIZE[a.dtype] == 8 \
+            else np.array([bits.value], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[a.dtype]].view(NP_DTYPES[a.dtype])[0].item()
 
     def aggregate_i128(self, op, a):
         """sum (wrapping) / min / max of a Decimal128 column as a Python int, None without valid rows."""
-        da = self.upload(a)
-        try:
-            bits, cnt = (C.c_uint64 * 2)(), C.c_int64(0)
-            ad = da.descriptor()
+        bits, cnt = (C.c_uint64 * 2)(), C.c_int64(0)
+        with self._scope() as s:
+            ad = s.upload(a).descriptor()
             self.check(self.lib.acu_aggregate_i128(self.h, op, C.byref(ad), bits, C.byref(cnt)))
-            if cnt.value == 0:
-                return None
-            return halves_to_i128(np.array([[bits[0], bits[1]]], dtype=np.uint64))[0]
-        finally:
-            da.free()
+        if cnt.value == 0:
+            return None
+        return halves_to_i128(np.array([[bits[0], bits[1]]], dtype=np.uint64))[0]
 
     def sum_checked(self, a):
         """arrow::compute::sum_checked (aggregate.rs:897): the in-order checked fold; raises ArrowError on overflow."""
@@ -1685,17 +1359,14 @@ class Context:
         return self._checked_fold(self.lib.acu_product_checked, a)
 
     def _checked_fold(self, fn, a):
-        da = self.upload(a)
-        try:
-            bits, cnt = C.c_uint64(0), C.c_int64(0)
-            ad = da.descriptor()
+        bits, cnt = C.c_uint64(0), C.c_int64(0)
+        with self._scope() as s:
+            ad = s.upload(a).descriptor()
             self.check(fn(self.h, a.dtype, C.byref(ad), C.byref(bits), C.byref(cnt)))
-            if cnt.value == 0:
-                return None
-            raw = np.array([bits.value], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[a.dtype]]
-            return raw.view(NP_DTYPES[a.dtype])[0].item()
-        finally:
-            da.free()
+        if cnt.value == 0:
+            return None
+        raw = np.array([bits.value], dtype=np.uint64).view(np.uint8)[: abi.DTYPE_SIZE[a.dtype]]
+        return raw.view(NP_DTYPES[a.dtype])[0].item()
 
     def sum(self, a): return self.aggregate(SUM, a)
     def min(self, a): return self.aggregate(MIN, a)
@@ -1709,27 +1380,18 @@ class Context:
     def min_max_row(self, op, col):
         """(row, valid_count): the lowest logical row holding the minimum (op = MIN) / maximum (MAX) of a Utf8Column,
         ViewColumn or FixedSizeBinaryColumn, -1 when there is none."""
-        owned, keep = [], []
         row, cnt = C.c_int64(0), C.c_int64(0)
-        try:
+        with self._scope() as s:
             if isinstance(col, Utf8Column):
-                d = self._upload_bytes_col(col, owned)
+                d = self._upload_bytes_col(col, s)
                 self.check(self.lib.acu_aggregate_bytes(self.h, col.offsets.dtype.itemsize, op, C.byref(d), C.byref(row), C.byref(cnt)))
             elif isinstance(col, ViewColumn):
-                d = self._upload_view_col(col, owned, keep)
+                d = self._upload_view_col(col, s, s.keep)
                 self.check(self.lib.acu_aggregate_byte_view(self.h, op, C.byref(d), C.byref(row), C.byref(cnt)))
             else:
-                d = self._upload_nulls(col.nulls, owned)
-                dv = self.malloc(col.values.nbytes + 16)
-                owned.append(dv)
-                if col.values.nbytes:
-                    self.h2d(dv, col.values)
-                d.values = dv
+                d = self._upload_fsb(col, s)
                 self.check(self.lib.acu_aggregate_fixed_size_binary(self.h, col.width, op, C.byref(d), C.byref(row), C.byref(cnt)))
-            return row.value, cnt.value
-        finally:
-            for p in owned:
-                self.free(p)
+        return row.value, cnt.value
 
     def _min_max_value(self, op, col, as_str):
         row, _ = self.min_max_row(op, col)
@@ -1751,14 +1413,11 @@ class Context:
 
     def aggregate_boolean(self, op, a):
         """(value, valid_count) of min_boolean (op = MIN) / max_boolean (MAX): value 0 | 1, -1 = None."""
-        da = self.upload(a)
-        try:
-            val, cnt = C.c_int32(0), C.c_int64(0)
-            ad = da.descriptor()
+        val, cnt = C.c_int32(0), C.c_int64(0)
+        with self._scope() as s:
+            ad = s.upload(a).descriptor()
             self.check(self.lib.acu_aggregate_boolean(self.h, op, C.byref(ad), C.byref(val), C.byref(cnt)))
-            return val.value, cnt.value
-        finally:
-            da.free()
+        return val.value, cnt.value
 
     def _boolean_value(self, op, a):
         v, _ = self.aggregate_boolean(op, a)
@@ -1773,109 +1432,68 @@ class Context:
     # -- List / LargeList / FixedSizeList (filter.rs:535-625, take.rs:646-795) -----------------
     # One C call per level: the list call returns the child's plan / row map, and the child is filtered / taken with it
     # through the entry point of its own type (the list calls again for a nested list).
-    def _list_descriptor(self, col, owned):
+    def _list_descriptor(self, col, s):
         d = abi.ListArray()
         if isinstance(col, FixedSizeListColumn):
             d.kind, d.list_size = abi.FIXED_SIZE_LIST, col.size
         else:
             d.kind = abi.LARGE_LIST if col.offsets.dtype == np.int64 else abi.LIST
-            off = np.ascontiguousarray(col.offsets)
-            d.offsets = self.malloc(off.nbytes + 16)
-            owned.append(d.offsets)
-            self.h2d(d.offsets, off)
-        d.nulls = self._upload_nulls(col.nulls, owned)
+            d.offsets = self._copy_in(col.offsets, s)
+        d.nulls = self._upload_nulls(col.nulls, s)
         d.child_len = col.child.length
         return d
 
-    def _nulls_out(self, out, n):
-        validity = self.d2h(out.validity, bitmap_bytes(n)) if out.has_validity else None
-        return HostArray(U8, np.zeros(0, np.uint8), n, validity, 0, 0, out.null_count if out.has_validity else 0)
-
     def filter_list(self, col, predicate):
         """arrow::compute::filter of a ListColumn / FixedSizeListColumn (any nesting of the supported children)."""
-        dp = self.upload(predicate)
-        plan = C.c_void_p()
-        try:
-            pd = dp.descriptor()
-            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
-            return self._filter_with_plan(col, plan)
-        finally:
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            dp.free()
+        return self.filter(col, predicate)
 
     def _filter_with_plan(self, col, plan, child_step=None):
-        """child_step: this level is the child of a list filtered with a plan that is not IterationStrategy::All (None at
+        """Filter any column this package filters with `plan`, one scope per nesting level.
+
+        child_step: this level is the child of a list filtered with a plan that is not IterationStrategy::All (None at
         the top). The reference then builds every level below it with MutableArrayData, whose freeze drops a NullBuffer
         without nulls (arrow-data/src/transform/mod.rs:936), also where the child's own plan selects every row."""
         count = self.lib.acu_filter_plan_count(plan)
-        owned, out = [], None
-        try:
+        with self._scope() as s:
             if isinstance(col, (ListColumn, FixedSizeListColumn)):
-                d = self._list_descriptor(col, owned)
+                d = self._list_descriptor(col, s)
                 fixed = isinstance(col, FixedSizeListColumn)
-                d_off = None if fixed else self.malloc((count + 1) * col.offsets.itemsize + 16)
-                if d_off:
-                    owned.append(d_off)
-                out = self.alloc_out(0, count)
-                child_plan = C.c_void_p()
-                self.check(self.lib.acu_filter_list(self.h, plan, C.byref(d), d_off, C.byref(out), C.byref(child_plan)))
-                # only the top level decides: under a top-level All the reference slices every level as it is
-                step = child_step if child_step is not None else count != self.lib.acu_filter_plan_len(plan)
-                try:
+                d_off = None if fixed else s.malloc((count + 1) * col.offsets.itemsize + 16)
+                out = s.out(0, count)
+                with self._scope() as cs:
+                    child_plan = cs.plan()
+                    self.check(self.lib.acu_filter_list(self.h, plan, C.byref(d), d_off, C.byref(out), C.byref(child_plan)))
+                    # only the top level decides: under a top-level All the reference slices every level as it is
+                    step = child_step if child_step is not None else count != self.lib.acu_filter_plan_len(plan)
                     child = self._filter_with_plan(col.child, child_plan, step)
-                finally:
-                    self.lib.acu_filter_plan_destroy(self.h, child_plan)
                 self._drop_empty_nulls(out, child_step)
                 nulls = self._nulls_out(out, count)
                 if fixed:
                     return FixedSizeListColumn(col.size, child, nulls)
                 return ListColumn(self.d2h(d_off, (count + 1) * col.offsets.itemsize, col.offsets.dtype), child, nulls)
             if isinstance(col, Utf8Column):
-                bd = self._upload_bytes_col(col, owned)
+                bd = self._upload_bytes_col(col, s)
                 ob = col.offsets.dtype.itemsize
-                d_off = self.malloc((count + 1) * ob + 16)
-                owned.append(d_off)
-                out = self.alloc_out(0, count)
-                total = C.c_int64(0)
-                self.check(self.lib.acu_filter_bytes(self.h, plan, ob, bd.offsets, bd.data, C.byref(bd.nulls), d_off, None, 0,
-                                                     C.byref(total), C.byref(out)))
-                d_data = self.malloc(total.value + 16)
-                owned.append(d_data)
-                self.check(self.lib.acu_filter_bytes(self.h, plan, ob, bd.offsets, bd.data, C.byref(bd.nulls), d_off, d_data,
-                                                     total.value, C.byref(total), C.byref(out)))
-                self._drop_empty_nulls(out, child_step)
-                return Utf8Column(self.d2h(d_off, (count + 1) * ob, col.offsets.dtype), self.d2h(d_data, total.value),
-                                  self._nulls_out(out, count))
+                return self._bytes_out(s, lambda oo, od, cap, tot, out: self.lib.acu_filter_bytes(
+                    self.h, plan, ob, bd.offsets, bd.data, C.byref(bd.nulls), oo, od, cap, tot, out), count, ob, child_step=child_step)
             if isinstance(col, ViewColumn):  # the views filter as 16-byte values; the data buffers are shared
-                keep = []
-                vd = self._upload_view_col(col, owned, keep)
+                vd = self._upload_view_col(col, s, s.keep)
                 arr = vd.nulls
                 arr.values = vd.views
-                out = self.alloc_out(count * 16, count)
+                out = s.out(count * 16, count)
                 self.check(self.lib.acu_filter_primitive(self.h, plan, 16, C.byref(arr), C.byref(out)))
                 self._drop_empty_nulls(out, child_step)
                 views = self.d2h(out.values, count * 16).reshape(-1, 16)
                 return ViewColumn(views, col.buffers, self._nulls_out(out, count))
-            dv = self.upload(col)
-            owned_arr = dv
-            try:
-                out = self.alloc_out(count * col.width(), count)
-                vd = dv.descriptor()
-                if col.dtype == BOOL:
-                    self.check(self.lib.acu_filter_boolean(self.h, plan, C.byref(vd), C.byref(out)))
-                else:
-                    self.check(self.lib.acu_filter_primitive(self.h, plan, col.width(), C.byref(vd), C.byref(out)))
-                self._drop_empty_nulls(out, child_step)
-                res, out = self.download_out(out, col.dtype), None
-                return col.like(res) if isinstance(col, DecimalArray) else res
-            finally:
-                owned_arr.free()
-        finally:
-            if out is not None:
-                self._free_out(out)
-            for p in owned:
-                self.free(p)
+            vd = s.upload(col).descriptor()
+            out = s.out(count * col.width(), count)
+            if col.dtype == BOOL:
+                self.check(self.lib.acu_filter_boolean(self.h, plan, C.byref(vd), C.byref(out)))
+            else:
+                self.check(self.lib.acu_filter_primitive(self.h, plan, col.width(), C.byref(vd), C.byref(out)))
+            self._drop_empty_nulls(out, child_step)
+            res = self._read_out(out, col.dtype)
+            return col.like(res) if isinstance(col, DecimalArray) else res
 
     @staticmethod
     def _drop_empty_nulls(out, child_step):
@@ -1884,14 +1502,9 @@ class Context:
 
     def take_list(self, col, indices, check_bounds=False):
         """arrow::compute::take of a ListColumn / FixedSizeListColumn by a HostArray of integer indices."""
-        di = self.upload(indices)
-        try:
-            idd = di.descriptor()
-            return self._take_level(col, idd, indices.dtype, check_bounds, False)
-        finally:
-            di.free()
+        return self.take(col, indices, check_bounds)
 
-    def _child_error_first(self, col, d, idd, index_dtype, row, owned):
+    def _child_error_first(self, col, d, idd, index_dtype, row, s):
         """The List `col` (descriptor d) passes i32::MAX at output row `row`. The reference extends the child of rows
         0 ..= row before it unwraps that row's offset, so the child's own offset overflow comes first: raise it if there is
         one (the caller then raises the panic)."""
@@ -1899,14 +1512,13 @@ class Context:
             return
         head = abi.Array.from_buffer_copy(idd)
         head.len = row
-        rmap, _, _, _, cdt, _, _ = self._row_map(d, head, index_dtype, False, False, row, owned)
+        rmap, _, _, _, cdt, _, _ = self._row_map(d, head, index_dtype, False, False, row, s)
         n0 = self._last_rows
         raw = self.d2h(idd.values + row * abi.DTYPE_SIZE[index_dtype], abi.DTYPE_SIZE[index_dtype], NP_DTYPES[index_dtype])
         ix = int(raw[0]) & (0xFFFFFFFF if index_dtype in (abi.I8, abi.I16, abi.I32) else 0xFFFFFFFFFFFFFFFF)
         w = abi.DTYPE_SIZE[cdt]
         extra = np.arange(int(col.offsets[ix]), int(col.offsets[ix + 1]), dtype=NP_DTYPES[cdt])
-        full = self.malloc((n0 + len(extra)) * w + 16)
-        owned.append(full)
+        full = s.malloc((n0 + len(extra)) * w + 16)
         if n0:
             self.check(self.lib.acu_memcpy_d2d(self.h, full, rmap, n0 * w))
         if len(extra):
@@ -1915,25 +1527,21 @@ class Context:
         cd.values, cd.len = full, n0 + len(extra)
         self._take_level(col.child, cd, cdt, False, True)
 
-    def _row_map(self, d, idd, index_dtype, check_bounds, keep, m, owned):
+    def _row_map(self, d, idd, index_dtype, check_bounds, keep, m, s):
         """acu_take_list both phases: (device row map, out ArrayOut of the list nulls, device offsets or None, child-index
         ArrayOut, row map dtype, offset width, a FixedSizeList's take_bits panic deferred behind its child)."""
         fixed = d.kind == abi.FIXED_SIZE_LIST
         ob = 0 if fixed else (8 if d.kind == abi.LARGE_LIST else 4)
-        d_off = self.malloc((m + 1) * max(ob, 1) + 16)
-        owned.append(d_off)
-        out = self.alloc_out(0, m)
-        owned += [out.values, out.validity]
+        d_off = s.malloc((m + 1) * max(ob, 1) + 16)
+        out = s.out(0, m)
         cdt = abi.U32 if fixed or d.child_len <= 0xFFFFFFFF else abi.U64
         rows = C.c_int64(0)
         cn = abi.ArrayOut()
         self.check(self.lib.acu_take_list(self.h, C.byref(d), C.byref(idd), index_dtype, int(check_bounds), int(keep), d_off, C.byref(out),
                                           cdt, None, 0, C.byref(rows), C.byref(cn)))
         n = rows.value
-        rmap = self.malloc(n * abi.DTYPE_SIZE[cdt] + 16)
-        owned.append(rmap)
-        cn.validity = self.malloc(bitmap_bytes(n) + 8)
-        owned.append(cn.validity)
+        rmap = s.malloc(n * abi.DTYPE_SIZE[cdt] + 16)
+        cn.validity = s.malloc(bitmap_bytes(n) + 8)
         deferred = None
         try:
             self.check(self.lib.acu_take_list(self.h, C.byref(d), C.byref(idd), index_dtype, int(check_bounds), int(keep), d_off,
@@ -1945,22 +1553,18 @@ class Context:
         self._last_rows = n
         return rmap, out, (d_off if ob else None), cn, cdt, ob, deferred
 
-    def _take_level(self, col, idd, index_dtype, check_bounds, keep, host_map=None):
-        """Take `col` by the device indices `idd` (or the host row map `host_map`). keep: this level is a child step of a
-        List / LargeList take (MutableArrayData::extend: every row keeps its range or bytes)."""
-        owned, dh = [], None
-        try:
-            if host_map is not None:
-                dh = self.upload(HostArray.from_numpy(index_dtype, host_map))
-                idd = dh.descriptor()
-            m = idd.len
+    def _take_level(self, col, idd, index_dtype, check_bounds, keep):
+        """Take any column this package takes by the device indices `idd`, one scope per nesting level. keep: this level is
+        a child step of a List / LargeList take (MutableArrayData::extend: every row keeps its range or bytes)."""
+        m = idd.len
+        with self._scope() as s:
             if isinstance(col, (ListColumn, FixedSizeListColumn)):
-                d = self._list_descriptor(col, owned)
+                d = self._list_descriptor(col, s)
                 try:
-                    rmap, out, d_off, cn, cdt, ob, deferred = self._row_map(d, idd, index_dtype, check_bounds, keep, m, owned)
+                    rmap, out, d_off, cn, cdt, ob, deferred = self._row_map(d, idd, index_dtype, check_bounds, keep, m, s)
                 except ArrowError as e:
                     if e.status == abi.ERR_PANIC_OUT_OF_BOUNDS and e.message.startswith("called `Option::unwrap()`"):
-                        self._child_error_first(col, d, idd, index_dtype, e.index, owned)
+                        self._child_error_first(col, d, idd, index_dtype, e.index, s)
                     raise
                 n = self._last_rows
                 cd = abi.Array()
@@ -1976,54 +1580,32 @@ class Context:
                     return FixedSizeListColumn(col.size, child, nulls)
                 return ListColumn(self.d2h(d_off, (m + 1) * ob, np.int32 if ob == 4 else np.int64), child, nulls)
             if isinstance(col, Utf8Column):
-                bd = self._upload_bytes_col(col, owned)
+                bd = self._upload_bytes_col(col, s)
                 ob = col.offsets.dtype.itemsize
-                d_off = self.malloc((m + 1) * ob + 16)
-                owned.append(d_off)
-                out = self.alloc_out(0, m)
-                owned += [out.values, out.validity]
-                total = C.c_int64(0)
 
-                def call(d_data, cap):
+                def call(oo, od, cap, tot, out):
                     if keep:
                         return self.lib.acu_take_bytes_extend(self.h, ob, bd.offsets, bd.data, C.byref(bd.nulls), C.byref(idd), index_dtype,
-                                                              d_off, d_data, cap, C.byref(total), C.byref(out))
+                                                              oo, od, cap, tot, out)
                     return self.lib.acu_take_bytes(self.h, ob, bd.offsets, bd.data, C.byref(bd.nulls), C.byref(idd), index_dtype,
-                                                   int(check_bounds), d_off, d_data, cap, C.byref(total), C.byref(out))
-                self.check(call(None, 0))
-                d_data = self.malloc(total.value + 16)
-                owned.append(d_data)
-                self.check(call(d_data, total.value))
-                return Utf8Column(self.d2h(d_off, (m + 1) * ob, col.offsets.dtype), self.d2h(d_data, total.value), self._nulls_out(out, m))
+                                                   int(check_bounds), oo, od, cap, tot, out)
+                return self._bytes_out(s, call, m, ob)
             if isinstance(col, ViewColumn):  # the views take as 16-byte values; the data buffers are shared
-                keep_tables = []
-                vd = self._upload_view_col(col, owned, keep_tables)
+                vd = self._upload_view_col(col, s, s.keep)
                 arr = vd.nulls
                 arr.values = vd.views
-                out = self.alloc_out(m * 16, m)
-                owned += [out.values, out.validity]
+                out = s.out(m * 16, m)
                 self.check(self.lib.acu_take_primitive(self.h, 16, C.byref(arr), C.byref(idd), index_dtype, int(check_bounds), C.byref(out)))
                 return ViewColumn(self.d2h(out.values, m * 16).reshape(-1, 16), col.buffers, self._nulls_out(out, m))
-            dv = self.upload(col)
-            try:
-                out = self.alloc_out(m * col.width(), m)
-                vd = dv.descriptor()
-                if col.dtype == BOOL:
-                    st = self.lib.acu_take_boolean(self.h, C.byref(vd), C.byref(idd), index_dtype, int(check_bounds), C.byref(out))
-                else:
-                    st = self.lib.acu_take_primitive(self.h, col.width(), C.byref(vd), C.byref(idd), index_dtype, int(check_bounds), C.byref(out))
-                if st != abi.OK:
-                    self._free_out(out)
-                    self.check(st)
-                res = self.download_out(out, col.dtype)
-                return col.like(res) if isinstance(col, DecimalArray) else res
-            finally:
-                dv.free()
-        finally:
-            for p in owned:
-                self.free(p)
-            if dh is not None:
-                dh.free()
+            vd = s.upload(col).descriptor()
+            out = s.out(m * col.width(), m)
+            if col.dtype == BOOL:
+                self.check(self.lib.acu_take_boolean(self.h, C.byref(vd), C.byref(idd), index_dtype, int(check_bounds), C.byref(out)))
+            else:
+                self.check(self.lib.acu_take_primitive(self.h, col.width(), C.byref(vd), C.byref(idd), index_dtype, int(check_bounds),
+                                                       C.byref(out)))
+            res = self._read_out(out, col.dtype)
+            return col.like(res) if isinstance(col, DecimalArray) else res
 
     # -- RunEndEncoded (filter_run_end_array filter.rs:628-677, take_run take.rs:948-995) ---------------------------
     # The run-end calls work on the run ends; the values child is filtered / taken with the plan / value indices they
@@ -2031,27 +1613,20 @@ class Context:
     def _run_descriptor(self, col, owned):
         d = abi.RunArray()
         d.run_end_dtype = {2: abi.I16, 4: abi.I32, 8: abi.I64}[col.run_ends.dtype.itemsize]
-        d.run_ends = self.malloc(col.run_ends.nbytes + 16)
-        owned.append(d.run_ends)
-        if col.run_ends.nbytes:
-            self.h2d(d.run_ends, col.run_ends)
+        d.run_ends = self._copy_in(col.run_ends, owned)
         d.n_runs, d.offset, d.len = len(col.run_ends), col.offset, col.length
         return d
 
     def filter_run_end(self, col, predicate):
         """arrow::compute::filter of a RunEndColumn: the run ends keep their type, the values child is any column this
         package filters."""
-        dp = self.upload(predicate)
-        plan, vplan, owned = C.c_void_p(), C.c_void_p(), []
-        try:
-            pd = dp.descriptor()
-            self.check(self.lib.acu_filter_plan_create(self.h, C.byref(pd), C.byref(plan)))
-            d = self._run_descriptor(col, owned)
+        with self._scope() as s:
+            plan = self._plan(s, predicate)
+            d = self._run_descriptor(col, s)
             count = self.lib.acu_filter_plan_count(plan)
             w = col.run_ends.itemsize
-            d_ends = self.malloc(max(min(count, len(col.run_ends)), 1) * w + 16)
-            owned.append(d_ends)
-            runs, vstart = C.c_int64(0), C.c_int64(0)
+            d_ends = s.malloc(max(min(count, len(col.run_ends)), 1) * w + 16)
+            runs, vstart, vplan = C.c_int64(0), C.c_int64(0), s.plan()
             self.check(self.lib.acu_filter_run_end(self.h, plan, C.byref(d), d_ends, C.byref(runs), C.byref(vstart), C.byref(vplan)))
             if not vplan:
                 if self.lib.acu_filter_plan_strategy(plan) == abi.FILTER_ALL:
@@ -2060,45 +1635,32 @@ class Context:
             values = self._filter_with_plan(slice_column(col.values, vstart.value, self.lib.acu_filter_plan_len(vplan)), vplan)
             ends = self.d2h(d_ends, runs.value * w, col.run_ends.dtype)
             return RunEndColumn(ends, values, 0, int(ends[-1]))
-        finally:
-            if vplan:
-                self.lib.acu_filter_plan_destroy(self.h, vplan)
-            if plan:
-                self.lib.acu_filter_plan_destroy(self.h, plan)
-            for p in owned:
-                self.free(p)
-            dp.free()
 
-    def _run_values(self, col, owned, keep):
-        """acu_run_values of a values child for take's run merge (uploads appended to owned / keep)."""
+    def _run_values(self, col, s):
+        """acu_run_values of a values child for take's run merge (the uploads belong to the scope s)."""
         v = abi.RunValues()
         if isinstance(col, (ListColumn, FixedSizeListColumn, RunEndColumn)):
             v.kind = abi.RUN_VALUES_NESTED
         elif isinstance(col, Utf8Column):
-            v.kind, v.width, v.bytes = abi.RUN_VALUES_BYTES, col.offsets.itemsize, self._upload_bytes_col(col, owned)
+            v.kind, v.width, v.bytes = abi.RUN_VALUES_BYTES, col.offsets.itemsize, self._upload_bytes_col(col, s)
         elif isinstance(col, ViewColumn):
-            v.kind, v.view = abi.RUN_VALUES_VIEW, self._upload_view_col(col, owned, keep)
+            v.kind, v.view = abi.RUN_VALUES_VIEW, self._upload_view_col(col, s, s.keep)
         else:
-            dv = self.upload(col)
-            keep.append(dv)
-            v.array = dv.descriptor()
+            v.array = s.upload(col).descriptor()
             v.kind, v.width = (abi.RUN_VALUES_BOOLEAN, 0) if col.dtype == BOOL else (abi.RUN_VALUES_FIXED, col.width())
         return v
 
     def take_run_end(self, col, indices, check_bounds=False):
         """arrow::compute::take of a RunEndColumn by a HostArray of integer indices (values: primitive, decimal, Boolean,
         Utf8 / Binary and view columns)."""
-        di = self.upload(indices)
-        owned, keep = [], []
-        try:
-            idd = di.descriptor()
-            d = self._run_descriptor(col, owned)
-            vd = self._run_values(col.values, owned, keep)
+        with self._scope() as s:
+            idd = s.upload(indices).descriptor()
+            d = self._run_descriptor(col, s)
+            vd = self._run_values(col.values, s)
             m = indices.length
             wide = indices.dtype in (abi.I64, abi.U64)
-            d_ends = self.malloc(max(m, 1) * col.run_ends.itemsize + 16)
-            d_vi = self.malloc(max(m, 1) * (8 if wide else 4) + 16)
-            owned += [d_ends, d_vi]
+            d_ends = s.malloc(max(m, 1) * col.run_ends.itemsize + 16)
+            d_vi = s.malloc(max(m, 1) * (8 if wide else 4) + 16)
             runs = C.c_int64(0)
             self.check(self.lib.acu_take_run_end(self.h, C.byref(d), C.byref(vd), C.byref(idd), indices.dtype, int(check_bounds), d_ends,
                                                  d_vi, C.byref(runs)))
@@ -2108,10 +1670,3 @@ class Context:
             cd.values, cd.len = d_vi, runs.value
             values = self._take_level(col.values, cd, abi.U64 if wide else abi.U32, False, False)
             return RunEndColumn(self.d2h(d_ends, runs.value * col.run_ends.itemsize, col.run_ends.dtype), values, 0, m)
-        finally:
-            for k in keep:
-                if isinstance(k, DeviceArray):
-                    k.free()
-            for p in owned:
-                self.free(p)
-            di.free()

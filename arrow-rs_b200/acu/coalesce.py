@@ -133,13 +133,12 @@ class BatchCoalescer:
         self.completed = deque()
 
     # -- device views of pushed columns -----------------------------------------------------------
-    def _upload(self, columns):
-        cols, owned = self.ctx._upload_columns(columns)
+    def _upload(self, columns, s):
         views = []
-        for c in cols:
+        for c in self.ctx._upload_columns(columns, s):
             views.append({"values": c.array.values, "values_offset": c.array.values_offset, "validity": c.array.validity,
                           "validity_offset": c.array.validity_offset, "null_count": c.array.null_count, "data": c.data})
-        return cols, owned, views
+        return views
 
     def _views_of_outs(self, columns, outs):
         views = []
@@ -156,58 +155,47 @@ class BatchCoalescer:
     def push_batch(self, columns):
         self._check_columns(columns)
         num_rows = columns[0].length if columns else 0
-        _, owned, views = self._upload(columns)
-        try:
-            self._push_device(views, num_rows)
-        finally:
-            self.ctx.sync()
-            self.ctx._free_columns(owned, None)
+        with self.ctx._scope() as s:
+            try:
+                self._push_device(self._upload(columns, s), num_rows)
+            finally:
+                self.ctx.sync()
 
     def push_batch_with_filter(self, columns, predicate):
         self._check_columns(columns)
         ctx = self.ctx
-        cols, owned = ctx._upload_columns(columns)
-        dp = ctx.upload(predicate)
-        plan = C.c_void_p()
-        outs = None
-        try:
-            pd = dp.descriptor()
-            ctx.check(ctx.lib.acu_filter_plan_create(ctx.h, C.byref(pd), C.byref(plan)))
-            count = ctx.lib.acu_filter_plan_count(plan)
-            caps = [int(c.data.nbytes) if isinstance(c, Utf8Column) else 0 for c in columns]
-            outs = ctx._alloc_column_outs(columns, count, caps)
-            ctx.check(ctx.lib.acu_filter_record_batch(ctx.h, plan, len(columns), cols, outs))
-            self._push_device(self._views_of_outs(columns, outs), count)
-        finally:
-            ctx.sync()
-            if plan:
-                ctx.lib.acu_filter_plan_destroy(ctx.h, plan)
-            ctx._free_columns(owned, outs)
-            dp.free()
+        with ctx._scope() as s:
+            try:
+                cols = ctx._upload_columns(columns, s)
+                plan = ctx._plan(s, predicate)
+                count = ctx.lib.acu_filter_plan_count(plan)
+                caps = [int(c.data.nbytes) if isinstance(c, Utf8Column) else 0 for c in columns]
+                outs = ctx._alloc_column_outs(columns, count, caps, s)
+                ctx.check(ctx.lib.acu_filter_record_batch(ctx.h, plan, len(columns), cols, outs))
+                self._push_device(self._views_of_outs(columns, outs), count)
+            finally:
+                ctx.sync()
 
     def push_batch_with_indices(self, columns, indices):
         self._check_columns(columns)
         ctx = self.ctx
-        cols, owned = ctx._upload_columns(columns)
-        di = ctx.upload(indices)
-        outs = None
-        try:
-            m = indices.length
-            caps = []
-            for c in columns:
-                if isinstance(c, Utf8Column):
-                    lens = np.diff(c.offsets.astype(np.int64)) if len(c.offsets) > 1 else np.zeros(0, np.int64)
-                    caps.append(int((lens.max() if lens.size else 0) * m))
-                else:
-                    caps.append(0)
-            outs = ctx._alloc_column_outs(columns, m, caps)
-            idd = di.descriptor()
-            ctx.check(ctx.lib.acu_take_record_batch(ctx.h, len(columns), cols, C.byref(idd), indices.dtype, 0, outs))
-            self._push_device(self._views_of_outs(columns, outs), m)
-        finally:
-            ctx.sync()
-            ctx._free_columns(owned, outs)
-            di.free()
+        with ctx._scope() as s:
+            try:
+                cols = ctx._upload_columns(columns, s)
+                idd = s.upload(indices).descriptor()
+                m = indices.length
+                caps = []
+                for c in columns:
+                    if isinstance(c, Utf8Column):
+                        lens = np.diff(c.offsets.astype(np.int64)) if len(c.offsets) > 1 else np.zeros(0, np.int64)
+                        caps.append(int((lens.max() if lens.size else 0) * m))
+                    else:
+                        caps.append(0)
+                outs = ctx._alloc_column_outs(columns, m, caps, s)
+                ctx.check(ctx.lib.acu_take_record_batch(ctx.h, len(columns), cols, C.byref(idd), indices.dtype, 0, outs))
+                self._push_device(self._views_of_outs(columns, outs), m)
+            finally:
+                ctx.sync()
 
     def _push_device(self, views, num_rows):
         """BatchCoalescer::push_batch (coalesce.rs:488-529) on device-resident columns."""
