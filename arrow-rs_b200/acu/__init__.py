@@ -403,9 +403,58 @@ class RunEndColumn:
         return RunEndColumn(self.run_ends, self.values, self.offset + offset, length)
 
 
+class StructColumn:
+    """A Struct column on the host (StructArray, arrow-array/src/array/struct_array.rs): `fields` are columns of the
+    struct's length starting at its logical row 0 (any column this package filters / takes; an empty list is a struct
+    without fields), `nulls` a HostArray carrying validity / length. Every field is treated as nullable."""
+
+    def __init__(self, fields, nulls):
+        self.fields, self.nulls = list(fields), nulls
+
+    @property
+    def length(self):
+        return self.nulls.length
+
+    def slice(self, offset, length):
+        """StructArray::slice: every field and the validity move together."""
+        nulls = self.nulls.slice(offset, length)
+        nulls.values = np.zeros(0, np.uint8)
+        return StructColumn([slice_column(f, offset, length) for f in self.fields], nulls)
+
+
+class UnionColumn:
+    """A sparse or dense Union column on the host (UnionArray, arrow-array/src/array/union_array.rs): `mode` is
+    abi.UNION_SPARSE or abi.UNION_DENSE, `field_type_ids` the fields' distinct type ids in [0, 127] in field order,
+    `children` one column per field, `type_ids` (np.int8) one per row and, for a dense union, `offsets` (np.int32) the
+    row's position in its child. A sparse union's children have the union's length; a union has no NullBuffer."""
+
+    def __init__(self, mode, field_type_ids, children, type_ids, offsets=None):
+        self.mode, self.field_type_ids, self.children = mode, [int(x) for x in field_type_ids], list(children)
+        self.type_ids = np.ascontiguousarray(type_ids, dtype=np.int8)
+        self.offsets = None if offsets is None else np.ascontiguousarray(offsets, dtype=np.int32)
+
+    @property
+    def dense(self):
+        return self.mode == abi.UNION_DENSE
+
+    @property
+    def length(self):
+        return len(self.type_ids)
+
+    def slice(self, offset, length):
+        """UnionArray::slice: the type ids (and offsets) move; a dense union keeps its children whole, a sparse one slices
+        them."""
+        tids = self.type_ids[offset:offset + length]
+        if self.dense:
+            return UnionColumn(self.mode, self.field_type_ids, self.children, tids, self.offsets[offset:offset + length])
+        return UnionColumn(self.mode, self.field_type_ids, [slice_column(c, offset, length) for c in self.children], tids)
+
+
 def slice_column(col, offset, length):
     """Array::slice of any host column: the same buffers, a new logical window."""
     if isinstance(col, HostArray):  # DecimalArray included
+        return col.slice(offset, length)
+    if isinstance(col, (StructColumn, UnionColumn)):
         return col.slice(offset, length)
     nulls = col.nulls.slice(offset, length)
     if isinstance(col, Utf8Column):
@@ -423,6 +472,11 @@ def slice_column(col, offset, length):
 
 def empty_column(col):
     """new_empty_array of col's type: no rows and no NullBuffer."""
+    if isinstance(col, StructColumn):
+        return StructColumn([empty_column(f) for f in col.fields], HostArray(abi.U8, np.zeros(0, np.uint8), 0, None, 0, 0, 0))
+    if isinstance(col, UnionColumn):
+        return UnionColumn(col.mode, col.field_type_ids, [empty_column(c) for c in col.children], np.zeros(0, np.int8),
+                           np.zeros(0, np.int32) if col.dense else None)
     e = slice_column(col, 0, 0)
     tgt = e if isinstance(e, HostArray) else (None if isinstance(e, RunEndColumn) else e.nulls)
     if tgt is not None:
@@ -1455,6 +1509,15 @@ class Context:
         without nulls (arrow-data/src/transform/mod.rs:936), also where the child's own plan selects every row."""
         count = self.lib.acu_filter_plan_count(plan)
         with self._scope() as s:
+            if isinstance(col, StructColumn):  # filter_struct (filter.rs:1010-1030): the fields, then filter_nulls
+                fields = [self._filter_with_plan(f, plan, child_step) for f in col.fields]
+                nd = self._upload_nulls(col.nulls, s)
+                out = s.out(0, count)
+                self.check(self.lib.acu_filter_nulls(self.h, plan, C.byref(nd), C.byref(out)))
+                self._drop_empty_nulls(out, child_step)
+                return StructColumn(fields, self._nulls_out(out, count))
+            if isinstance(col, UnionColumn):
+                return self._filter_union(col, plan, count, child_step, s)
             if isinstance(col, (ListColumn, FixedSizeListColumn)):
                 d = self._list_descriptor(col, s)
                 fixed = isinstance(col, FixedSizeListColumn)
@@ -1494,6 +1557,58 @@ class Context:
             self._drop_empty_nulls(out, child_step)
             res = self._read_out(out, col.dtype)
             return col.like(res) if isinstance(col, DecimalArray) else res
+
+    def _union_descriptor(self, col, s):
+        d = abi.UnionArray()
+        d.mode, d.n_fields, d.len = col.mode, len(col.field_type_ids), col.length
+        ids = (C.c_int8 * max(len(col.field_type_ids), 1))(*col.field_type_ids)
+        s.keep.append(ids)
+        d.field_type_ids = C.cast(ids, C.c_void_p)
+        d.type_ids = self._copy_in(col.type_ids, s)
+        if col.dense:
+            d.offsets = self._copy_in(col.offsets, s)
+        return d
+
+    def _union_out(self, col, m, s):
+        """Device buffers for acu_filter_union / acu_take_union of m output rows, and the host field starts."""
+        tids = s.malloc(m + 16)
+        offs = s.malloc(4 * m + 16) if col.dense else None
+        rows = s.malloc(4 * m + 16) if col.dense else None
+        return tids, offs, rows, (C.c_int64 * (len(col.children) + 1))()
+
+    def _union_children(self, col, rows, starts, keep):
+        """A dense union's children, child f taken / extended (keep) with rows [starts[f], starts[f + 1]) of the map."""
+        children = []
+        for f, child in enumerate(col.children):
+            cd = abi.Array()
+            cd.values, cd.len = rows + 4 * starts[f], starts[f + 1] - starts[f]
+            children.append(self._take_level(child, cd, abi.I32, False, keep))
+        return children
+
+    def _filter_union(self, col, plan, count, child_step, s):
+        """filter_sparse_union (filter.rs:1033-1054) / the dense MutableArrayData fallback (filter.rs:597-622,
+        build_extend_dense): a dense union's children are extended row by row, so every level below it is frozen."""
+        strategy = self.lib.acu_filter_plan_strategy(plan)
+        if col.dense and child_step and strategy == abi.FILTER_ALL:
+            # a list's child step extends every row even when its plan selects them all: the same rows as a take of 0..n
+            idx = HostArray.from_numpy(U64, np.arange(count, dtype=np.uint64))
+            return self._take_level(col, s.upload(idx).descriptor(), U64, False, True)
+        d = self._union_descriptor(col, s)
+        tids, offs, rows, starts = self._union_out(col, count, s)
+        self.check(self.lib.acu_filter_union(self.h, plan, C.byref(d), tids, offs, rows, starts))
+        if col.dense:
+            if strategy == abi.FILTER_NONE:
+                return empty_column(col)
+            if strategy == abi.FILTER_ALL:
+                return col.slice(0, count)  # values.slice(0, count): the children stay whole
+            return UnionColumn(col.mode, col.field_type_ids, self._union_children(col, rows, starts, True),
+                               self.d2h(tids, count, np.int8), self.d2h(offs, 4 * count, np.int32))
+        children = [self._filter_with_plan(c, plan, child_step) for c in col.children]
+        if strategy in (abi.FILTER_NONE, abi.FILTER_ALL):
+            tids_h = col.type_ids[:count].copy()
+        else:
+            tids_h = self.d2h(tids, count, np.int8)
+        return UnionColumn(col.mode, col.field_type_ids, children, tids_h)
 
     @staticmethod
     def _drop_empty_nulls(out, child_step):
@@ -1558,6 +1673,45 @@ class Context:
         a child step of a List / LargeList take (MutableArrayData::extend: every row keeps its range or bytes)."""
         m = idd.len
         with self._scope() as s:
+            if isinstance(col, StructColumn):
+                # take_impl's Struct arm (take.rs:270-298): the fields first, then the validity; check_bounds comes before
+                # both, BooleanBuffer::value's panic after the fields' own errors
+                nd = self._upload_nulls(col.nulls, s)
+                out = s.out(0, m)
+                deferred = None
+                try:
+                    self.check(self.lib.acu_take_nulls(self.h, C.byref(nd), C.byref(idd), index_dtype, int(check_bounds), C.byref(out)))
+                except ArrowError as e:
+                    if e.status != abi.ERR_PANIC_OUT_OF_BOUNDS:
+                        raise
+                    deferred = e
+                fields = [self._take_level(f, idd, index_dtype, False, keep) for f in col.fields]
+                if deferred is not None:
+                    raise deferred
+                nulls = self._nulls_out(out, m)
+                if not col.fields and not keep and nulls.validity is None:  # new_empty_fields keeps its NullBuffer
+                    nulls = HostArray(U8, np.zeros(0, np.uint8), m, pack_bits(np.ones(m, bool)), 0, 0, 0)
+                return StructColumn(fields, nulls)
+            if isinstance(col, UnionColumn):
+                d = self._union_descriptor(col, s)
+                tids, offs, rows, starts = self._union_out(col, m, s)
+                deferred = None
+                try:
+                    self.check(self.lib.acu_take_union(self.h, C.byref(d), C.byref(idd), index_dtype, int(check_bounds), tids, offs, rows,
+                                                       starts))
+                except ArrowError as e:  # UnionArray::try_new validates after the children are taken
+                    if not e.message.endswith(("Type Ids values must match one of the field type ids",
+                                               "Offsets must be non-negative and within the length of the Array")):
+                        raise
+                    deferred = e
+                if col.dense:
+                    children = self._union_children(col, rows, starts, keep)
+                else:
+                    children = [self._take_level(c, idd, index_dtype, False, keep) for c in col.children]
+                if deferred is not None:
+                    raise deferred
+                return UnionColumn(col.mode, col.field_type_ids, children, self.d2h(tids, m, np.int8),
+                                   self.d2h(offs, 4 * m, np.int32) if col.dense else None)
             if isinstance(col, (ListColumn, FixedSizeListColumn)):
                 d = self._list_descriptor(col, s)
                 try:
@@ -1639,7 +1793,7 @@ class Context:
     def _run_values(self, col, s):
         """acu_run_values of a values child for take's run merge (the uploads belong to the scope s)."""
         v = abi.RunValues()
-        if isinstance(col, (ListColumn, FixedSizeListColumn, RunEndColumn)):
+        if isinstance(col, (ListColumn, FixedSizeListColumn, RunEndColumn, StructColumn, UnionColumn)):
             v.kind = abi.RUN_VALUES_NESTED
         elif isinstance(col, Utf8Column):
             v.kind, v.width, v.bytes = abi.RUN_VALUES_BYTES, col.offsets.itemsize, self._upload_bytes_col(col, s)

@@ -125,6 +125,16 @@ class RunValues(C.Structure):
     _fields_ = [("kind", C.c_int32), ("width", C.c_int32), ("array", Array), ("bytes", BytesArray), ("view", ViewArray)]
 
 
+UNION_SPARSE, UNION_DENSE = range(2)
+UNION_MAX_FIELDS = 128
+
+
+class UnionArray(C.Structure):
+    """acu_union_array: one level of a sparse / dense Union column (the children are described separately)."""
+    _fields_ = [("mode", C.c_int32), ("n_fields", C.c_int32), ("field_type_ids", C.c_void_p), ("type_ids", C.c_void_p),
+                ("offsets", C.c_void_p), ("len", C.c_int64)]
+
+
 COL_PRIMITIVE, COL_BOOLEAN, COL_BYTES = range(3)
 BOOL_AND, BOOL_OR, BOOL_AND_NOT, BOOL_AND_KLEENE, BOOL_OR_KLEENE, BOOL_NOT, BOOL_IS_NULL, BOOL_IS_NOT_NULL = range(8)
 MAX_BATCH_COLUMNS = 64
@@ -238,6 +248,10 @@ PROTOTYPES = {
     "acu_take_list": (i32, [vp, P(ListArray), P(Array), i32, i32, i32, vp, P(ArrayOut), i32, vp, i64, P(i64), P(ArrayOut)]),
     "acu_filter_run_end": (i32, [vp, vp, P(RunArray), vp, P(i64), P(i64), P(vp)]),
     "acu_take_run_end": (i32, [vp, P(RunArray), P(RunValues), P(Array), i32, i32, vp, vp, P(i64)]),
+    "acu_filter_nulls": (i32, [vp, vp, P(Array), P(ArrayOut)]),
+    "acu_take_nulls": (i32, [vp, P(Array), P(Array), i32, i32, P(ArrayOut)]),
+    "acu_filter_union": (i32, [vp, vp, P(UnionArray), vp, vp, vp, P(i64)]),
+    "acu_take_union": (i32, [vp, P(UnionArray), P(Array), i32, i32, vp, vp, vp, P(i64)]),
     "acu_arith": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_bitwise": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_neg": (i32, [vp, i32, i32, P(Array), P(ArrayOut)]),

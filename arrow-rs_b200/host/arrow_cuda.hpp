@@ -143,7 +143,7 @@ inline std::vector<uint8_t> pack_bits(const std::vector<bool> &bits) {
 // DataType / native type traits (arrow-array/src/types.rs:67-80)
 // ---------------------------------------------------------------------------------------
 enum class DataType { Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Boolean, Utf8, Decimal32, Decimal64, Decimal128,
-                      List, LargeList, FixedSizeList, RunEndEncoded };
+                      List, LargeList, FixedSizeList, RunEndEncoded, Struct, Union };
 
 template <class T> struct NativeOf;
 #define ACU_NATIVE(T, DT, CODE) \
@@ -593,6 +593,103 @@ using Int16RunArray = RunArray<int16_t>;
 using Int32RunArray = RunArray<int32_t>;
 using Int64RunArray = RunArray<int64_t>;
 
+// StructArray (arrow-array/src/array/struct_array.rs): columns of the struct's length from its logical row 0, and the
+// nulls. Every field is nullable here.
+class StructArray : public Array {
+ public:
+  StructArray(std::vector<ArrayRef> columns, int64_t len, std::optional<NullBuffer> nulls) : columns_(std::move(columns)) {
+    len_ = len;
+    nulls_ = std::move(nulls);
+  }
+  // StructArray::new(fields, arrays, nulls): try_new drops a NullBuffer without nulls
+  static StructArray from(std::vector<ArrayRef> columns, const std::vector<bool> &valid = {}) {
+    const int64_t len = columns.at(0)->len();
+    return StructArray(std::move(columns), len, valid.empty() ? std::nullopt : nulls_from_mask(valid));
+  }
+  // StructArray::new_empty_fields(len, nulls): no columns, the NullBuffer kept as given
+  static StructArray new_empty_fields(int64_t len, const std::vector<bool> &valid = {}) {
+    return StructArray({}, len, valid.empty() ? std::nullopt : nulls_from_mask(valid, true));
+  }
+  DataType data_type() const override { return DataType::Struct; }
+  const std::vector<ArrayRef> &columns() const { return columns_; }
+  const ArrayRef &column(size_t i) const { return columns_.at(i); }
+  size_t num_columns() const { return columns_.size(); }
+ protected:
+  const void *values_ptr() const override { return nullptr; }
+ private:
+  std::vector<ArrayRef> columns_;
+};
+
+// UnionArray (arrow-array/src/array/union_array.rs): the fields' type ids in field order, one Int8 type id per row and, for
+// a dense union, one Int32 offset per row into the row's child. A sparse union's children have the union's length. A union
+// has no NullBuffer.
+class UnionArray : public Array {
+ public:
+  UnionArray(std::vector<int8_t> field_type_ids, Buffer type_ids, std::optional<Buffer> offsets, std::vector<ArrayRef> children, int64_t len)
+      : field_type_ids_(std::move(field_type_ids)), type_ids_(std::move(type_ids)), offsets_(std::move(offsets)), children_(std::move(children)) {
+    len_ = len;
+  }
+  // UnionArray::try_new (union_array.rs:177-242)
+  static Result<UnionArray> try_new(std::vector<int8_t> field_type_ids, const std::vector<int8_t> &type_ids,
+                                    std::optional<std::vector<int32_t>> offsets, std::vector<ArrayRef> children) {
+    auto fail = [](const char *m) { return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: ") + m}; };
+    if (field_type_ids.size() != children.size()) return fail("Union fields length must match child arrays length");
+    if (offsets && offsets->size() != type_ids.size()) return fail("Type Ids and Offsets lengths must match");
+    if (!offsets)
+      for (const auto &c : children)
+        if (c->len() != (int64_t)type_ids.size()) return fail("Sparse union child arrays must be equal in length to the length of the union");
+    std::map<int, int64_t> lens;
+    for (size_t f = 0; f < field_type_ids.size(); ++f) lens[field_type_ids[f]] = children[f]->len();
+    for (int8_t t : type_ids)
+      if (!lens.count(t)) return fail("Type Ids values must match one of the field type ids");
+    if (offsets)
+      for (size_t i = 0; i < type_ids.size(); ++i)
+        if ((*offsets)[i] < 0 || (*offsets)[i] >= lens[type_ids[i]]) return fail("Offsets must be non-negative and within the length of the Array");
+    std::optional<Buffer> ob;
+    if (offsets) ob = Buffer::from_host(offsets->data(), offsets->size() * 4);
+    return UnionArray(std::move(field_type_ids), Buffer::from_host(type_ids.data(), type_ids.size()), std::move(ob), std::move(children),
+                      (int64_t)type_ids.size());
+  }
+  DataType data_type() const override { return DataType::Union; }
+  bool is_dense() const { return offsets_.has_value(); }
+  const std::vector<int8_t> &field_type_ids() const { return field_type_ids_; }
+  const std::vector<ArrayRef> &children() const { return children_; }
+  const ArrayRef &child(int8_t type_id) const {
+    for (size_t f = 0; f < field_type_ids_.size(); ++f)
+      if (field_type_ids_[f] == type_id) return children_[f];
+    throw std::runtime_error("invalid union type id");
+  }
+  const Buffer &type_ids_buffer() const { return type_ids_; }
+  const std::optional<Buffer> &offsets_buffer() const { return offsets_; }
+  std::vector<int8_t> type_ids() const {
+    std::vector<int8_t> v((size_t)len_);
+    type_ids_.to_host(v.data(), v.size());
+    return v;
+  }
+  std::vector<int32_t> value_offsets() const {
+    std::vector<int32_t> v(offsets_ ? (size_t)len_ : 0);
+    if (offsets_) offsets_->to_host(v.data(), v.size() * 4);
+    return v;
+  }
+  acu_union_array union_view() const {
+    acu_union_array u{};
+    u.mode = offsets_ ? ACU_UNION_DENSE : ACU_UNION_SPARSE;
+    u.n_fields = (int32_t)field_type_ids_.size();
+    u.field_type_ids = field_type_ids_.data();
+    u.type_ids = static_cast<const int8_t *>(type_ids_.data());
+    u.offsets = offsets_ ? static_cast<const int32_t *>(offsets_->data()) : nullptr;
+    u.len = len_;
+    return u;
+  }
+ protected:
+  const void *values_ptr() const override { return nullptr; }
+ private:
+  std::vector<int8_t> field_type_ids_;
+  Buffer type_ids_;
+  std::optional<Buffer> offsets_;
+  std::vector<ArrayRef> children_;
+};
+
 // Datum (arrow-array/src/scalar.rs:78-152): an array, or a Scalar wrapping a 1-element array
 template <class A>
 struct Scalar {
@@ -680,7 +777,7 @@ inline ArrayRef make_primitive(DataType dt, Buffer values, int64_t len, std::opt
 }
 inline const char *dtype_display(DataType t) {
   static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64", "Boolean", "Utf8",
-                            "Decimal32", "Decimal64", "Decimal128", "List", "LargeList", "FixedSizeList", "RunEndEncoded"};
+                            "Decimal32", "Decimal64", "Decimal128", "List", "LargeList", "FixedSizeList", "RunEndEncoded", "Struct", "Union"};
   return n[(int)t];
 }
 template <class A> std::string type_text(const A &a) {
@@ -946,8 +1043,13 @@ inline ArrayRef list_like(const Array &a, Buffer offsets, ArrayRef child, int64_
 // child_step: `values` is a child of a list whose top level was filtered with a plan other than All (nullopt at the top).
 // The reference builds those levels with MutableArrayData (filter.rs:600), which drops a NullBuffer without nulls even
 // where the level's own plan selects every row; under a top-level All it slices every level as it is.
+inline Result<ArrayRef> filter_nested(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan, std::optional<bool> child_step);
+inline Result<ArrayRef> take_nested(const Array &values, const Array &indices, int cb, bool keep);
+inline bool is_nested(DataType t) { return t == DataType::Struct || t == DataType::Union; }
+
 inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan,
                                    std::optional<bool> child_step = std::nullopt) {
+  if (is_nested(values.data_type())) return filter_nested(values, pred, plan, child_step);
   if (!is_list(values.data_type())) {
     auto r = pred.filter(values);
     if (r.is_err() || !child_step.value_or(false)) return r;
@@ -1010,6 +1112,7 @@ inline Result<ArrayRef> take_list_level(const Array &values, const Array &indice
 
 inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool extend) {
   if (is_list(values.data_type())) return take_list_level(values, indices, cb, extend);
+  if (is_nested(values.data_type())) return take_nested(values, indices, cb, extend);
   if (!extend || values.data_type() != DataType::Utf8) return take(values, indices, TakeOptions{cb != 0});
   Context &c = Context::get();
   const auto &s = static_cast<const StringArray &>(values);
@@ -1097,6 +1200,11 @@ inline ArrayRef slice_any(const Array &a, int64_t off, int64_t len) {
       s.offsets().to_host(o.data(), o.size() * 4);
       return std::make_shared<StringArray>(Buffer::from_host(o.data() + off, (size_t)(len + 1) * 4), s.value_data(), len, nulls);
     }
+    case DataType::Struct: {
+      std::vector<ArrayRef> cols;
+      for (const auto &col : static_cast<const StructArray &>(a).columns()) cols.push_back(slice_any(*col, off, len));
+      return std::make_shared<StructArray>(std::move(cols), len, nulls);
+    }
     default: throw std::runtime_error(std::string("RunArray values of type ") + dtype_display(a.data_type()) + " are not supported by this mirror");
   }
 }
@@ -1171,7 +1279,9 @@ Result<ArrayRef> take(const RunArray<R> &values, const Array &indices, std::opti
       rv.bytes.nulls = vals.view();
       break;
     }
-    case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: rv.kind = ACU_RUN_VALUES_NESTED; break;
+    case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: case DataType::Struct: case DataType::Union:
+      rv.kind = ACU_RUN_VALUES_NESTED;
+      break;
     default:
       if (dtype_width(vals.data_type()) == 0)
         throw std::runtime_error(std::string("RunArray values of type ") + detail::dtype_display(vals.data_type()) + " are not supported by this mirror");
@@ -1194,6 +1304,165 @@ Result<ArrayRef> take(const RunArray<R> &values, const Array &indices, std::opti
   auto v = take(vals, *vix);
   if (v.is_err()) return v.unwrap_err();
   return ArrayRef(std::make_shared<RunArray<R>>(ends, runs, v.unwrap(), 0, m));
+}
+
+// ---- filter / take of Struct, sparse Union and dense Union (filter.rs:597-622, :1010-1054, take.rs:270-298, :334-382) ------
+// A struct's columns go through the entry points of their types and acu_filter_nulls / acu_take_nulls give its NullBuffer.
+// acu_filter_union / acu_take_union give a union's type ids and, for a dense union, its new offsets and a child row map
+// grouped by field; child f is then taken (take) or extended (filter, the child step of a list take) with its slice of the
+// map. Both nest under lists, structs and unions through filter_any / take_any.
+namespace detail {
+inline acu_array nulls_view(const Array &a) {
+  acu_array v = a.view();
+  v.values = nullptr;
+  return v;
+}
+inline ArrayRef i32_slice(const Buffer &map, int64_t start, int64_t len) {
+  return std::make_shared<PrimitiveArray<int32_t>>(map, len, std::nullopt, start);
+}
+// the first `len` rows of a union: the type ids (and offsets) move, a dense union keeps its children whole, a sparse one
+// slices them
+inline ArrayRef union_head(const UnionArray &u, int64_t len) {
+  std::vector<int8_t> t = u.type_ids();
+  std::optional<Buffer> ob;
+  std::vector<ArrayRef> children = u.children();
+  if (u.is_dense()) {
+    std::vector<int32_t> o = u.value_offsets();
+    ob = Buffer::from_host(o.data(), (size_t)len * 4);
+  } else {
+    for (auto &c : children) c = slice_any(*c, 0, len);
+  }
+  return std::make_shared<UnionArray>(u.field_type_ids(), Buffer::from_host(t.data(), (size_t)len), std::move(ob), std::move(children), len);
+}
+
+inline Result<ArrayRef> filter_nested(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan, std::optional<bool> child_step) {
+  Context &c = Context::get();
+  const int64_t n = pred.count();
+  acu_status st;
+  if (values.data_type() == DataType::Struct) {  // filter_struct: every column, then filter_nulls
+    const auto &sa = static_cast<const StructArray &>(values);
+    std::vector<ArrayRef> cols;
+    for (const auto &col : sa.columns()) {
+      auto r = filter_any(*col, pred, plan, child_step);
+      if (r.is_err()) return r.unwrap_err();
+      cols.push_back(r.unwrap());
+    }
+    const acu_array nv = nulls_view(values);
+    Buffer nb = Buffer::allocate(acu_bitmap_bytes(n));
+    acu_array_out o{};
+    o.validity = static_cast<uint8_t *>(nb.data());
+    if ((st = acu_filter_nulls(c.raw(), plan, &nv, &o)) != ACU_OK) return c.last_error(st);
+    if (child_step.value_or(false) && o.has_validity && o.null_count == 0) o.has_validity = 0;
+    return ArrayRef(std::make_shared<StructArray>(std::move(cols), n, out_nulls(o, nb)));
+  }
+  const auto &u = static_cast<const UnionArray &>(values);
+  const int32_t strategy = acu_filter_plan_strategy(plan);
+  if (u.is_dense() && child_step.value_or(false) && strategy == ACU_FILTER_ALL) {
+    // a list's child step extends every row even when its plan selects them all: the rows of a take of 0 .. n
+    std::vector<uint64_t> ids((size_t)n);
+    for (int64_t i = 0; i < n; ++i) ids[(size_t)i] = (uint64_t)i;
+    return take_nested(values, PrimitiveArray<uint64_t>::from(ids), 0, true);
+  }
+  const acu_union_array uv = u.union_view();
+  const size_t nf = u.field_type_ids().size();
+  Buffer tids = Buffer::allocate((size_t)n), offs = Buffer::allocate((size_t)n * 4), map = Buffer::allocate((size_t)n * 4);
+  std::vector<int64_t> starts(nf + 1, 0);
+  if ((st = acu_filter_union(c.raw(), plan, &uv, static_cast<int8_t *>(tids.data()), static_cast<int32_t *>(offs.data()),
+                             static_cast<int32_t *>(map.data()), starts.data())) != ACU_OK)
+    return c.last_error(st);
+  const bool whole = strategy == ACU_FILTER_NONE || strategy == ACU_FILTER_ALL;
+  std::vector<ArrayRef> children;
+  if (u.is_dense()) {
+    if (strategy == ACU_FILTER_ALL) return union_head(u, n);  // values.slice(0, count)
+    for (size_t f = 0; f < nf; ++f) {  // build_extend_dense: each child extended row by row
+      auto r = take_any(*u.children()[f], *i32_slice(map, starts[f], starts[f + 1] - starts[f]), 0, true);
+      if (r.is_err()) return r.unwrap_err();
+      children.push_back(r.unwrap());
+    }
+    return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, offs, std::move(children), n));
+  }
+  for (const auto &ch : u.children()) {
+    auto r = filter_any(*ch, pred, plan, child_step);
+    if (r.is_err()) return r.unwrap_err();
+    children.push_back(r.unwrap());
+  }
+  if (whole) {
+    std::vector<int8_t> t = u.type_ids();
+    tids = Buffer::from_host(t.data(), (size_t)n);
+  }
+  return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, std::nullopt, std::move(children), n));
+}
+
+inline Result<ArrayRef> take_nested(const Array &values, const Array &indices, int cb, bool keep) {
+  Context &c = Context::get();
+  const int64_t m = indices.len();
+  const acu_array ix = indices.view();
+  const acu_dtype it = (acu_dtype)dtype_code(indices.data_type());
+  acu_status st;
+  std::optional<ArrowError> deferred;
+  std::vector<ArrayRef> children;
+  if (values.data_type() == DataType::Struct) {
+    // take_impl's Struct arm: check_bounds first, then the columns, then the validity (whose panic comes after them)
+    const auto &sa = static_cast<const StructArray &>(values);
+    const acu_array nv = nulls_view(values);
+    Buffer nb = Buffer::allocate(acu_bitmap_bytes(m));
+    acu_array_out o{};
+    o.validity = static_cast<uint8_t *>(nb.data());
+    if ((st = acu_take_nulls(c.raw(), &nv, &ix, it, cb, &o)) != ACU_OK) {
+      if (st != ACU_ERR_PANIC_OUT_OF_BOUNDS) return c.last_error(st);
+      deferred = c.last_error(st);
+    }
+    for (const auto &col : sa.columns()) {
+      auto r = take_any(*col, indices, 0, keep);
+      if (r.is_err()) return r.unwrap_err();
+      children.push_back(r.unwrap());
+    }
+    if (deferred) return *deferred;
+    std::optional<NullBuffer> nulls = out_nulls(o, nb);
+    if (children.empty() && !keep && !nulls) nulls = nulls_from_mask(std::vector<bool>((size_t)m, true), true);  // new_empty_fields
+    return ArrayRef(std::make_shared<StructArray>(std::move(children), m, std::move(nulls)));
+  }
+  const auto &u = static_cast<const UnionArray &>(values);
+  const acu_union_array uv = u.union_view();
+  const size_t nf = u.field_type_ids().size();
+  Buffer tids = Buffer::allocate((size_t)m), offs = Buffer::allocate((size_t)m * 4), map = Buffer::allocate((size_t)m * 4);
+  std::vector<int64_t> starts(nf + 1, 0);
+  if ((st = acu_take_union(c.raw(), &uv, &ix, it, cb, static_cast<int8_t *>(tids.data()), static_cast<int32_t *>(offs.data()),
+                           static_cast<int32_t *>(map.data()), starts.data())) != ACU_OK) {
+    ArrowError e = c.last_error(st);
+    // UnionArray::try_new validates after the children are taken
+    if (e.message.find("Type Ids values must match one of the field type ids") == std::string::npos &&
+        e.message.find("Offsets must be non-negative and within the length of the Array") == std::string::npos)
+      return e;
+    deferred = e;
+  }
+  for (size_t f = 0; f < nf; ++f) {
+    auto r = u.is_dense() ? take_any(*u.children()[f], *i32_slice(map, starts[f], starts[f + 1] - starts[f]), 0, keep)
+                          : take_any(*u.children()[f], indices, 0, keep);
+    if (r.is_err()) return r.unwrap_err();
+    children.push_back(r.unwrap());
+  }
+  if (deferred) return *deferred;
+  std::optional<Buffer> ob;
+  if (u.is_dense()) ob = offs;
+  return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, std::move(ob), std::move(children), m));
+}
+
+inline Result<ArrayRef> take_nested_top(const Array &values, const Array &indices, std::optional<TakeOptions> options) {
+  const DataType it = indices.data_type();
+  if ((int)it > (int)DataType::UInt64)  // take.rs:103
+    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + dtype_display(it)};
+  return take_nested(values, indices, options && options->check_bounds ? 1 : 0, false);
+}
+}  // namespace detail
+
+inline Result<ArrayRef> filter(const StructArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
+inline Result<ArrayRef> filter(const UnionArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
+inline Result<ArrayRef> take(const StructArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+  return detail::take_nested_top(values, indices, options);
+}
+inline Result<ArrayRef> take(const UnionArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+  return detail::take_nested_top(values, indices, options);
 }
 
 // take.rs:1123-1133: every column gathered with the same indices, one synchronisation per (up to 64-column) call.

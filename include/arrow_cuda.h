@@ -607,6 +607,85 @@ acu_status acu_take_run_end(acu_ctx *ctx, const acu_run_array *ree, const acu_ru
                             int64_t *out_runs);
 
 /* ------------------------------------------------------------------------- */
+/* filter / take of Struct, sparse Union and dense Union columns             */
+/* ------------------------------------------------------------------------- */
+/* A struct's fields are filtered / taken one by one through the entry point of their type; these two calls produce the
+ * struct's own NullBuffer. `nulls_of` carries the struct's len / validity / validity_offset / null_count (`values` ignored).
+ *
+ * acu_filter_nulls: predicate.filter_nulls(array.nulls()) (filter_struct, arrow-select/src/filter.rs:1010-1030): out
+ * (capacity acu_bitmap_bytes(count)) holds the selected rows' validity, with a NullBuffer only when one of them is null;
+ * strategy ALL keeps the NullBuffer as it is (values.slice(0, count)), NONE has none. Predicate longer than the struct =>
+ * ACU_ERR_INVALID_ARGUMENT "Filter predicate of length {p} is larger than target array of length {n}". Synchronous; kernel
+ * time in ACU_K_FILTER.
+ *
+ * acu_take_nulls: the validity of take_impl's Struct arm (take.rs:270-298): row j is valid iff index j is valid and
+ * array.is_valid(index j). A NullBuffer only when a row is null (StructArray::try_new drops one without nulls; an
+ * empty-field struct keeps it, which is the caller's to build: out->validity is then written whenever the indices or the
+ * struct have a validity buffer). In order: a non-integer index type => ACU_ERR_INVALID_ARGUMENT "Take only supported for
+ * integers, got {type}"; check_bounds != 0 => ACU_ERR_COMPUTE "Array index out of bounds, cannot get item at index {i} from
+ * {len} entries"; then out is written. Unlike take_nulls, is_valid reads a validity buffer that has no null in the slice:
+ * when nulls_of has a validity buffer, a valid index >= len is BooleanBuffer::value's panic, ACU_ERR_PANIC_OUT_OF_BOUNDS
+ * "assertion failed: idx < self.bit_len" at the lowest such row. The reference takes the fields before it reads the
+ * validity, so that panic is returned after out is written: the caller takes the fields first and reports a field's own
+ * error ahead of it. Without a validity buffer no row is read. Synchronous; kernel time in ACU_K_TAKE. */
+acu_status acu_filter_nulls(acu_ctx *ctx, const acu_filter_plan *plan, const acu_array *nulls_of, acu_array_out *out);
+acu_status acu_take_nulls(acu_ctx *ctx, const acu_array *nulls_of, const acu_array *indices, acu_dtype index_dtype,
+                          int32_t check_bounds, acu_array_out *out);
+
+/* One level of a union column (UnionArray, arrow-array/src/array/union_array.rs). The children are NOT described here: the
+ * caller filters / takes each child through the entry point of its type, as for a list's child.
+ *   mode            ACU_UNION_SPARSE or ACU_UNION_DENSE;
+ *   n_fields        1..ACU_UNION_MAX_FIELDS;
+ *   field_type_ids  host array of n_fields distinct type ids in [0, 127], in field order;
+ *   type_ids        Int8, on the device, from logical row 0;
+ *   offsets         Int32, dense only, on the device, from logical row 0, 4-byte aligned;
+ *   len             logical rows.
+ * A type id that names no field, or a dense offset outside its child, is malformed input: the result is then unspecified,
+ * but no access leaves the buffers. A bad mode, field count, field type id or alignment => ACU_ERR_INVALID_ARGUMENT. */
+#define ACU_UNION_MAX_FIELDS 128
+typedef enum acu_union_mode { ACU_UNION_SPARSE = 0, ACU_UNION_DENSE = 1 } acu_union_mode;
+typedef struct acu_union_array {
+  int32_t mode;
+  int32_t n_fields;
+  const int8_t *field_type_ids;
+  const int8_t *type_ids;
+  const int32_t *offsets;
+  int64_t len;
+} acu_union_array;
+
+/* filter of a union. Sparse (filter_sparse_union, filter.rs:1033-1054): out_type_ids (count entries) = filter_primitive of
+ * the type ids; the caller filters every child with the same plan. Dense (the MutableArrayData fallback, filter.rs:597-622,
+ * build_extend_dense in arrow-data/src/transform/union.rs): out_type_ids as above; out_offsets (count entries) = for every
+ * selected row, the number of earlier selected rows of its type id; out_child_rows (capacity count Int32 entries) = the
+ * selected rows' source offsets grouped by field in field order, each group in output order; out_field_starts (host,
+ * n_fields + 1 entries): field f's rows are [starts[f], starts[f + 1]). The caller extends child f with those rows as ACU_I32
+ * indices (MutableArrayData::extend, the child step of a list take). Predicate longer than the union =>
+ * ACU_ERR_INVALID_ARGUMENT "Filter predicate of length {p} is larger than target array of length {n}". Strategy NONE / ALL:
+ * nothing is written (the reference returns new_empty_array / values.slice(0, count); a dense slice keeps its children
+ * whole, a sparse one slices them). Synchronous; the compaction counts in ACU_K_FILTER, the partition in ACU_K_FILTER_PLAN. */
+acu_status acu_filter_union(acu_ctx *ctx, const acu_filter_plan *plan, const acu_union_array *u, int8_t *out_type_ids,
+                            int32_t *out_offsets, int32_t *out_child_rows, int64_t *out_field_starts);
+
+/* take of a union (take.rs:334-382). In order:
+ *   - the index type, check_bounds and take_native's out-of-bounds panics exactly as acu_take_primitive (type ids first,
+ *     then the dense offsets); a null index gathers the type id / offset when it is in bounds and 0 when it is not;
+ *   - every output is written: out_type_ids (indices.len entries); for a dense union out_offsets (the running count per
+ *     type id), out_child_rows (capacity indices.len Int32 entries) and out_field_starts (host, n_fields + 1 entries), laid
+ *     out as in acu_filter_union; the caller takes child f with rows [starts[f], starts[f + 1]) as ACU_I32 indices (plain
+ *     take), or every child of a sparse union with the indices themselves;
+ *   - a taken type id that names no field (reachable: a null out-of-bounds index yields 0) => ACU_ERR_INVALID_ARGUMENT
+ *     "Type Ids values must match one of the field type ids" (UnionArray::try_new, union_array.rs:177-242), returned after
+ *     the outputs are written, so that the caller takes the children first and reports a child's error ahead of it;
+ *   - then, for a dense union, a field with more than i32::MAX output rows => ACU_ERR_INVALID_ARGUMENT "Offsets must be
+ *     non-negative and within the length of the Array", also after the outputs are written.
+ * The new offsets are i32: past i32::MAX rows of one field they wrap (two's complement), in acu_filter_union as well, as the
+ * reference's i32 running counts do in a release build.
+ * Synchronous; the gathers and the partition count in ACU_K_TAKE. */
+acu_status acu_take_union(acu_ctx *ctx, const acu_union_array *u, const acu_array *indices, acu_dtype index_dtype,
+                          int32_t check_bounds, int8_t *out_type_ids, int32_t *out_offsets, int32_t *out_child_rows,
+                          int64_t *out_field_starts);
+
+/* ------------------------------------------------------------------------- */
 /* like — arrow-string/src/like.rs                                           */
 /* ------------------------------------------------------------------------- */
 /* arrow-string/src/like.rs `enum Op` */

@@ -218,6 +218,19 @@ pub struct acu_run_values {
     pub bytes: acu_bytes_array,
     pub view: acu_view_array,
 }
+/// acu_union_array: one level of a sparse / dense Union column (the children are filtered / taken separately).
+pub const ACU_UNION_SPARSE: i32 = 0;
+pub const ACU_UNION_DENSE: i32 = 1;
+#[repr(C)]
+#[derive(Clone, Copy)]
+pub struct acu_union_array {
+    pub mode: i32,
+    pub n_fields: i32,
+    pub field_type_ids: *const i8,
+    pub type_ids: *const i8,
+    pub offsets: *const i32,
+    pub len: i64,
+}
 #[repr(C)]
 pub struct acu_ipc_stream { _private: [u8; 0] }
 
@@ -269,6 +282,13 @@ extern "C" {
     pub fn acu_take_run_end(ctx: *mut acu_ctx, ree: *const acu_run_array, values: *const acu_run_values, indices: *const acu_array,
                             index_dtype: i32, check_bounds: i32, out_run_ends: *mut c_void, out_value_indices: *mut c_void,
                             out_runs: *mut i64) -> acu_status;
+    pub fn acu_filter_nulls(ctx: *mut acu_ctx, plan: *const acu_filter_plan, nulls_of: *const acu_array, out: *mut acu_array_out) -> acu_status;
+    pub fn acu_take_nulls(ctx: *mut acu_ctx, nulls_of: *const acu_array, indices: *const acu_array, index_dtype: i32, check_bounds: i32,
+                          out: *mut acu_array_out) -> acu_status;
+    pub fn acu_filter_union(ctx: *mut acu_ctx, plan: *const acu_filter_plan, u: *const acu_union_array, out_type_ids: *mut i8,
+                            out_offsets: *mut i32, out_child_rows: *mut i32, out_field_starts: *mut i64) -> acu_status;
+    pub fn acu_take_union(ctx: *mut acu_ctx, u: *const acu_union_array, indices: *const acu_array, index_dtype: i32, check_bounds: i32,
+                          out_type_ids: *mut i8, out_offsets: *mut i32, out_child_rows: *mut i32, out_field_starts: *mut i64) -> acu_status;
     pub fn acu_arith(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_neg(ctx: *mut acu_ctx, dtype: i32, checked: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_decimal_arith(ctx: *mut acu_ctx, op: i32, lt: *const acu_decimal_type, a: *const acu_array, rt: *const acu_decimal_type,

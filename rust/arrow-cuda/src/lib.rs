@@ -298,6 +298,9 @@ pub mod compute {
             if let DataType::RunEndEncoded(_, _) = values.data_type() {
                 return run_end::filter(ctx, self.plan.raw, values);
             }
+            if let DataType::Struct(_) | DataType::Union(_, _) = values.data_type() {
+                return nested::filter(ctx, self.plan.raw, values, None);
+            }
             let v = DeviceArray::upload(ctx, values, false)?;
             let mut out = ColumnOut::new(ctx, values.data_type(), self.count(), v.data_bytes)?;
             let st = match kind_of(values.data_type())? {
@@ -361,6 +364,9 @@ pub mod compute {
         }
         if let DataType::RunEndEncoded(_, _) = values.data_type() {
             return run_end::take(&ctx, values, indices, idt, check);
+        }
+        if let DataType::Struct(_) | DataType::Union(_, _) = values.data_type() {
+            return nested::take(&ctx, values, indices, idt, check, false);
         }
         let (v, ix) = (DeviceArray::upload(&ctx, values, false)?, DeviceArray::upload(&ctx, indices, false)?);
         let m = indices.len();
@@ -460,7 +466,8 @@ pub mod compute {
             let vals = a.values();
             let mut rv: ffi::acu_run_values = unsafe { std::mem::zeroed() };
             let _up = match vals.data_type() {
-                DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) | DataType::RunEndEncoded(_, _) => {
+                DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) | DataType::RunEndEncoded(_, _)
+                | DataType::Struct(_) | DataType::Union(_, _) => {
                     rv.kind = ffi::ACU_RUN_VALUES_NESTED;
                     None
                 }
@@ -541,7 +548,7 @@ pub mod compute {
             make_array(unsafe { b.build_unchecked() })
         }
 
-        fn nulls_of(validity: &DeviceBuffer, o: &ffi::acu_array_out) -> Result<Option<NullBuffer>, ArrowError> {
+        pub(super) fn nulls_of(validity: &DeviceBuffer, o: &ffi::acu_array_out) -> Result<Option<NullBuffer>, ArrowError> {
             if o.has_validity == 0 { return Ok(None); }
             let bits = BooleanBuffer::new(validity.to_host(bitmap_bytes(o.len as usize))?, 0, o.len as usize);
             Ok(Some(unsafe { NullBuffer::new_unchecked(bits, o.null_count as usize) }))
@@ -564,6 +571,7 @@ pub mod compute {
             let step = child_step.unwrap_or(n != unsafe { ffi::acu_filter_plan_len(plan) } as usize);
             let child = match lv.child.data_type() {
                 DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) => filter(ctx, child_plan.raw, lv.child.as_ref(), Some(step))?,
+                DataType::Struct(_) | DataType::Union(_, _) => nested::filter(ctx, child_plan.raw, lv.child.as_ref(), Some(step))?,
                 _ => {
                     let c = FilterPredicate { plan: child_plan }.filter(lv.child.as_ref())?;
                     if step { drop_empty_nulls(c) } else { c }
@@ -612,9 +620,10 @@ pub mod compute {
             Ok(rebuild(values, offsets, child, m, nulls_of(&validity, &o)?))
         }
 
-        fn child_take(ctx: &Context, child: &dyn Array, map: &dyn Array, cdt: i32, extend: bool) -> Result<ArrayRef, ArrowError> {
+        pub(super) fn child_take(ctx: &Context, child: &dyn Array, map: &dyn Array, cdt: i32, extend: bool) -> Result<ArrayRef, ArrowError> {
             match child.data_type() {
                 DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) => take(ctx, child, map, cdt, 0, extend),
+                DataType::Struct(_) | DataType::Union(_, _) => nested::take(ctx, child, map, cdt, 0, extend),
                 DataType::Utf8 | DataType::Binary | DataType::LargeUtf8 | DataType::LargeBinary if extend => {
                     let ob = match kind_of(child.data_type())? { Kind::Bytes(ob) => ob, _ => unreachable!() };
                     let (v, ix) = (DeviceArray::upload(ctx, child, false)?, DeviceArray::upload(ctx, map, false)?);
@@ -635,6 +644,149 @@ pub mod compute {
                 }
                 _ => super::take(child, map, None),
             }
+        }
+    }
+
+    // ---- Struct, sparse Union, dense Union (filter.rs:597-622, :1010-1054, take.rs:270-298, :334-382) -----------------
+    /// A struct's columns go through filter / take of their own types and acu_filter_nulls / acu_take_nulls give its
+    /// NullBuffer. acu_filter_union / acu_take_union give a union's type ids and, for a dense union, its new offsets and a
+    /// child row map grouped by field; child f is then taken (take) or extended (filter: MutableArrayData, the child step of
+    /// a list take) with its slice of the map.
+    mod nested {
+        use super::*;
+        use arrow_array::types::{Int32Type, UInt64Type};
+        use arrow_array::{new_empty_array, Array, StructArray, UnionArray};
+        use super::list::nulls_of;
+        use arrow_buffer::ScalarBuffer;
+        use arrow_schema::UnionMode;
+
+        /// filter / take of a child with a borrowed plan (the caller owns it)
+        fn filter_child(ctx: &Context, plan: *mut ffi::acu_filter_plan, child: &dyn Array, child_step: Option<bool>) -> Result<ArrayRef, ArrowError> {
+            match child.data_type() {
+                DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) => list::filter(ctx, plan, child, child_step),
+                DataType::Struct(_) | DataType::Union(_, _) => filter(ctx, plan, child, child_step),
+                _ => {
+                    let p = std::mem::ManuallyDrop::new(FilterPredicate { plan: Plan { ctx: ctx.clone(), raw: plan } });
+                    let c = p.filter(child)?;
+                    if child_step == Some(true) && c.nulls().map_or(false, |n| n.null_count() == 0) {
+                        return Ok(make_array(unsafe { c.to_data().into_builder().nulls(None).build_unchecked() }));
+                    }
+                    Ok(c)
+                }
+            }
+        }
+
+        fn union_view(ctx: &Context, u: &UnionArray, ids: &[i8]) -> Result<(ffi::acu_union_array, Vec<DeviceBuffer>), ArrowError> {
+            let t = DeviceBuffer::from_host(ctx, u.type_ids().inner().as_slice())?;
+            let mut d = ffi::acu_union_array { mode: ffi::ACU_UNION_SPARSE, n_fields: ids.len() as i32, field_type_ids: ids.as_ptr(),
+                                               type_ids: t.as_ptr() as *const i8, offsets: std::ptr::null(), len: u.len() as i64 };
+            let mut bufs = vec![t];
+            if let Some(o) = u.offsets() {
+                let ob = DeviceBuffer::from_host(ctx, o.inner().as_slice())?;
+                d.mode = ffi::ACU_UNION_DENSE;
+                d.offsets = ob.as_ptr() as *const i32;
+                bufs.push(ob);
+            }
+            Ok((d, bufs))
+        }
+
+        fn finish_union(u: &UnionArray, tids: &DeviceBuffer, offs: Option<&DeviceBuffer>, n: usize, children: Vec<ArrayRef>) -> Result<ArrayRef, ArrowError> {
+            let DataType::Union(fields, _) = u.data_type() else { unreachable!() };
+            let t = ScalarBuffer::<i8>::new(tids.to_host(n)?, 0, n);
+            let o = match offs { Some(b) => Some(ScalarBuffer::<i32>::new(b.to_host(n * 4)?, 0, n)), None => None };
+            Ok(Arc::new(unsafe { UnionArray::new_unchecked(fields.clone(), t, o, children) }))
+        }
+
+        fn map_slice(map: &DeviceBuffer, starts: &[i64], f: usize, n: usize) -> Result<ArrayRef, ArrowError> {
+            let all = ScalarBuffer::<i32>::new(map.to_host(n * 4)?, 0, n);
+            let (a, b) = (starts[f] as usize, starts[f + 1] as usize);
+            Ok(Arc::new(PrimitiveArray::<Int32Type>::new(all.slice(a, b - a), None)))
+        }
+
+        pub(super) fn filter(ctx: &Context, plan: *mut ffi::acu_filter_plan, values: &dyn Array, child_step: Option<bool>) -> Result<ArrayRef, ArrowError> {
+            let n = unsafe { ffi::acu_filter_plan_count(plan) } as usize;
+            let strategy = unsafe { ffi::acu_filter_plan_strategy(plan) };
+            if let Some(s) = values.as_any().downcast_ref::<StructArray>() {  // filter_struct: every column, then filter_nulls
+                let cols = s.columns().iter().map(|c| filter_child(ctx, plan, c.as_ref(), child_step)).collect::<Result<Vec<_>, _>>()?;
+                let nv = DeviceArray::upload(ctx, &BooleanArray::new(BooleanBuffer::new_set(s.len()), s.nulls().cloned()), false)?;
+                let mut v = *nv.view();
+                v.values = std::ptr::null();
+                let validity = DeviceBuffer::allocate(ctx, bitmap_bytes(n.max(1)))?;
+                let mut o = ffi::acu_array_out { values: std::ptr::null_mut(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0, has_validity: 0, reserved: 0 };
+                ctx.check(unsafe { ffi::acu_filter_nulls(ctx.raw(), plan, &v, &mut o) })?;
+                if child_step == Some(true) && o.null_count == 0 { o.has_validity = 0; }
+                let DataType::Struct(fields) = s.data_type() else { unreachable!() };
+                return Ok(Arc::new(unsafe { StructArray::new_unchecked_with_length(fields.clone(), cols, nulls_of(&validity, &o)?, n) }));
+            }
+            let u = values.as_any().downcast_ref::<UnionArray>().unwrap();
+            let DataType::Union(fields, mode) = u.data_type() else { unreachable!() };
+            let dense = *mode == UnionMode::Dense;
+            if dense && child_step == Some(true) && strategy == 1 {
+                // a list's child step extends every row even when its plan selects them all: the rows of a take of 0 .. n
+                let ids = PrimitiveArray::<UInt64Type>::from_iter_values(0..n as u64);
+                return take(ctx, values, &ids, 7, 0, true);
+            }
+            let ids: Vec<i8> = fields.iter().map(|(t, _)| t).collect();
+            let (d, _bufs) = union_view(ctx, u, &ids)?;
+            let (tids, offs, map) = (DeviceBuffer::allocate(ctx, n.max(1))?, DeviceBuffer::allocate(ctx, n.max(1) * 4)?, DeviceBuffer::allocate(ctx, n.max(1) * 4)?);
+            let mut starts = vec![0i64; ids.len() + 1];
+            ctx.check(unsafe { ffi::acu_filter_union(ctx.raw(), plan, &d, tids.as_ptr() as *mut i8, offs.as_ptr() as *mut i32,
+                                                     map.as_ptr() as *mut i32, starts.as_mut_ptr()) })?;
+            if strategy == 1 { return Ok(u.slice(0, n)); }  // values.slice(0, count)
+            if dense {
+                let children = (0..ids.len()).map(|f| {
+                    let rows = map_slice(&map, &starts, f, n)?;
+                    list::child_take(ctx, u.child(ids[f]).as_ref(), rows.as_ref(), 2, true)  // ACU_I32, extended row by row
+                }).collect::<Result<Vec<_>, _>>()?;
+                return finish_union(u, &tids, Some(&offs), n, children);
+            }
+            let children = ids.iter().map(|&t| filter_child(ctx, plan, u.child(t).as_ref(), child_step)).collect::<Result<Vec<_>, _>>()?;
+            if strategy == 0 { return Ok(new_empty_array(u.data_type())); }
+            finish_union(u, &tids, None, n, children)
+        }
+
+        pub(super) fn take(ctx: &Context, values: &dyn Array, indices: &dyn Array, idt: i32, check: i32, keep: bool) -> Result<ArrayRef, ArrowError> {
+            let ix = DeviceArray::upload(ctx, indices, false)?;
+            let m = indices.len();
+            let child_take = |child: &dyn Array, rows: &dyn Array, cdt: i32| list::child_take(ctx, child, rows, cdt, keep);
+            if let Some(s) = values.as_any().downcast_ref::<StructArray>() {
+                // take_impl's Struct arm: check_bounds first, then the columns, then the validity (its panic after theirs)
+                let nv = DeviceArray::upload(ctx, &BooleanArray::new(BooleanBuffer::new_set(s.len()), s.nulls().cloned()), false)?;
+                let mut v = *nv.view();
+                v.values = std::ptr::null();
+                let validity = DeviceBuffer::allocate(ctx, bitmap_bytes(m.max(1)))?;
+                let mut o = ffi::acu_array_out { values: std::ptr::null_mut(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0, has_validity: 0, reserved: 0 };
+                let st = unsafe { ffi::acu_take_nulls(ctx.raw(), &v, ix.view(), idt, check, &mut o) };
+                let deferred = if st == ffi::ACU_ERR_PANIC_OUT_OF_BOUNDS { Some(ctx.check(st).unwrap_err()) } else { ctx.check(st).map(|_| None)? };
+                let cols = s.columns().iter().map(|c| child_take(c.as_ref(), indices, idt)).collect::<Result<Vec<_>, _>>()?;
+                if let Some(e) = deferred { return Err(e); }
+                let mut nulls = nulls_of(&validity, &o)?;
+                if cols.is_empty() && !keep && nulls.is_none() { nulls = Some(NullBuffer::new_valid(m)); }  // new_empty_fields
+                let DataType::Struct(fields) = s.data_type() else { unreachable!() };
+                return Ok(Arc::new(unsafe { StructArray::new_unchecked_with_length(fields.clone(), cols, nulls, m) }));
+            }
+            let u = values.as_any().downcast_ref::<UnionArray>().unwrap();
+            let DataType::Union(fields, mode) = u.data_type() else { unreachable!() };
+            let dense = *mode == UnionMode::Dense;
+            let ids: Vec<i8> = fields.iter().map(|(t, _)| t).collect();
+            let (d, _bufs) = union_view(ctx, u, &ids)?;
+            let (tids, offs, map) = (DeviceBuffer::allocate(ctx, m.max(1))?, DeviceBuffer::allocate(ctx, m.max(1) * 4)?, DeviceBuffer::allocate(ctx, m.max(1) * 4)?);
+            let mut starts = vec![0i64; ids.len() + 1];
+            let st = unsafe { ffi::acu_take_union(ctx.raw(), &d, ix.view(), idt, check, tids.as_ptr() as *mut i8, offs.as_ptr() as *mut i32,
+                                                  map.as_ptr() as *mut i32, starts.as_mut_ptr()) };
+            // UnionArray::try_new validates after the children are taken
+            let deferred = match ctx.check(st) {
+                Err(e) if e.to_string().ends_with("Type Ids values must match one of the field type ids")
+                    || e.to_string().ends_with("Offsets must be non-negative and within the length of the Array") => Some(e),
+                Err(e) => return Err(e),
+                Ok(()) => None,
+            };
+            let children = (0..ids.len()).map(|f| {
+                if dense { child_take(u.child(ids[f]).as_ref(), map_slice(&map, &starts, f, m)?.as_ref(), 2) }
+                else { child_take(u.child(ids[f]).as_ref(), indices, idt) }
+            }).collect::<Result<Vec<_>, _>>()?;
+            if let Some(e) = deferred { return Err(e); }
+            finish_union(u, &tids, if dense { Some(&offs) } else { None }, m, children)
         }
     }
 
