@@ -361,6 +361,12 @@ class FixedSizeBinaryColumn:
         nulls.values = np.zeros(0, np.uint8)
         return FixedSizeBinaryColumn(vals, nulls)
 
+    def slice(self, offset, length):
+        """FixedSizeBinaryArray::slice: the rows and the validity move together."""
+        nulls = self.nulls.slice(offset, length)
+        nulls.values = np.zeros(0, np.uint8)
+        return FixedSizeBinaryColumn(self.values[offset:offset + length], nulls)
+
 
 class ListColumn:
     """A List (np.int32 offsets) / LargeList (np.int64) column on the host (GenericListArray,
@@ -454,7 +460,7 @@ def slice_column(col, offset, length):
     """Array::slice of any host column: the same buffers, a new logical window."""
     if isinstance(col, HostArray):  # DecimalArray included
         return col.slice(offset, length)
-    if isinstance(col, (StructColumn, UnionColumn)):
+    if isinstance(col, (StructColumn, UnionColumn, FixedSizeBinaryColumn)):
         return col.slice(offset, length)
     nulls = col.nulls.slice(offset, length)
     if isinstance(col, Utf8Column):
@@ -863,6 +869,8 @@ class Context:
         """(acu_column kind, width) of a host column: a Utf8Column's width is its offset width."""
         if isinstance(col, Utf8Column):
             return abi.COL_BYTES, col.offsets.dtype.itemsize
+        if isinstance(col, FixedSizeBinaryColumn):
+            return abi.COL_FIXED_SIZE_BINARY, col.width
         return (abi.COL_BOOLEAN, 0) if col.dtype == BOOL else (abi.COL_PRIMITIVE, col.width())
 
     def _upload_columns(self, columns, s):
@@ -874,6 +882,8 @@ class Context:
                 cols[c].array = bd.nulls
                 cols[c].array.values = bd.offsets
                 cols[c].data = bd.data
+            elif isinstance(col, FixedSizeBinaryColumn):
+                cols[c].array = self._upload_fsb(col, s)
             else:
                 cols[c].array = s.upload(col).descriptor()
         return cols
@@ -893,6 +903,9 @@ class Context:
                 outs[c].array.validity = malloc(bitmap_bytes(rows) + 8)
                 outs[c].data = malloc(data_caps[c] + 16)
                 outs[c].data_capacity = data_caps[c]
+            elif isinstance(col, FixedSizeBinaryColumn):
+                outs[c].array.values = malloc(rows * col.width + 16)
+                outs[c].array.validity = malloc(bitmap_bytes(rows) + 8)
             else:
                 outs[c].array.values = malloc((bitmap_bytes(rows) if col.dtype == BOOL else rows * col.width()) + 16)
                 outs[c].array.validity = malloc(bitmap_bytes(rows) + 8)
@@ -908,7 +921,10 @@ class Context:
     def _read_column(self, kind, width, dtype, arr, data, data_len=None):
         """A column read back from the device buffers of an acu_column / acu_column_out: `arr` is an ArrayOut of its values
         (the offsets of a COL_BYTES column, `width` bytes each), validity and rows; `data` the bytes of a COL_BYTES column,
-        data_len of them (None: up to the last offset). Returns a Utf8Column, or a HostArray of `dtype`."""
+        data_len of them (None: up to the last offset). Returns a Utf8Column, a FixedSizeBinaryColumn of byte width `width`
+        (COL_FIXED_SIZE_BINARY), or a HostArray of `dtype`."""
+        if kind == abi.COL_FIXED_SIZE_BINARY:
+            return self._fsb_out(arr, arr.len, width)
         if kind != abi.COL_BYTES:
             return self._read_out(arr, BOOL if kind == abi.COL_BOOLEAN else dtype)
         n = arr.len
@@ -1139,6 +1155,10 @@ class Context:
         d = self._upload_nulls(col.nulls, owned)
         d.values = self._copy_in(col.values, owned)
         return d
+
+    def _fsb_out(self, out, n, width):
+        """The n-row FixedSizeBinary result `out` (an ArrayOut) read back; its buffers stay allocated."""
+        return FixedSizeBinaryColumn(self.d2h(out.values, n * width).reshape(n, width), self._nulls_out(out, n))
 
     def _bytes_predicate(self, a, b, call):
         """A boolean result of two Utf8Column or two ViewColumn operands (nulls.is_scalar marks a Datum scalar):
@@ -1534,6 +1554,13 @@ class Context:
                 if fixed:
                     return FixedSizeListColumn(col.size, child, nulls)
                 return ListColumn(self.d2h(d_off, (count + 1) * col.offsets.itemsize, col.offsets.dtype), child, nulls)
+            if isinstance(col, FixedSizeBinaryColumn):
+                d, w = self._upload_fsb(col, s), col.width
+                out = s.out(count * w, count)
+                self.check(self.lib.acu_filter_fixed_size_binary(self.h, plan, w, C.byref(d), C.byref(out)))
+                self._drop_empty_nulls(out, child_step)
+                # MutableArrayData keeps every extended row, also of width 0 (try_new's length rule is the top level's)
+                return self._fsb_out(out, count if child_step else out.len, w)
             if isinstance(col, Utf8Column):
                 bd = self._upload_bytes_col(col, s)
                 ob = col.offsets.dtype.itemsize
@@ -1733,6 +1760,12 @@ class Context:
                 if not ob:
                     return FixedSizeListColumn(col.size, child, nulls)
                 return ListColumn(self.d2h(d_off, (m + 1) * ob, np.int32 if ob == 4 else np.int64), child, nulls)
+            if isinstance(col, FixedSizeBinaryColumn):
+                d, w = self._upload_fsb(col, s), col.width
+                out = s.out(m * w, m)
+                self.check(self.lib.acu_take_fixed_size_binary(self.h, w, C.byref(d), C.byref(idd), index_dtype, int(check_bounds),
+                                                               C.byref(out)))
+                return self._fsb_out(out, m if keep else out.len, w)
             if isinstance(col, Utf8Column):
                 bd = self._upload_bytes_col(col, s)
                 ob = col.offsets.dtype.itemsize
@@ -1793,7 +1826,7 @@ class Context:
     def _run_values(self, col, s):
         """acu_run_values of a values child for take's run merge (the uploads belong to the scope s)."""
         v = abi.RunValues()
-        if isinstance(col, (ListColumn, FixedSizeListColumn, RunEndColumn, StructColumn, UnionColumn)):
+        if isinstance(col, (ListColumn, FixedSizeListColumn, RunEndColumn, StructColumn, UnionColumn, FixedSizeBinaryColumn)):
             v.kind = abi.RUN_VALUES_NESTED
         elif isinstance(col, Utf8Column):
             v.kind, v.width, v.bytes = abi.RUN_VALUES_BYTES, col.offsets.itemsize, self._upload_bytes_col(col, s)

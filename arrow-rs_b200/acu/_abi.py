@@ -135,7 +135,7 @@ class UnionArray(C.Structure):
                 ("offsets", C.c_void_p), ("len", C.c_int64)]
 
 
-COL_PRIMITIVE, COL_BOOLEAN, COL_BYTES = range(3)
+COL_PRIMITIVE, COL_BOOLEAN, COL_BYTES, COL_FIXED_SIZE_BINARY = range(4)
 BOOL_AND, BOOL_OR, BOOL_AND_NOT, BOOL_AND_KLEENE, BOOL_OR_KLEENE, BOOL_NOT, BOOL_IS_NULL, BOOL_IS_NOT_NULL = range(8)
 MAX_BATCH_COLUMNS = 64
 
@@ -252,6 +252,8 @@ PROTOTYPES = {
     "acu_take_nulls": (i32, [vp, P(Array), P(Array), i32, i32, P(ArrayOut)]),
     "acu_filter_union": (i32, [vp, vp, P(UnionArray), vp, vp, vp, P(i64)]),
     "acu_take_union": (i32, [vp, P(UnionArray), P(Array), i32, i32, vp, vp, vp, P(i64)]),
+    "acu_filter_fixed_size_binary": (i32, [vp, vp, i32, P(Array), P(ArrayOut)]),
+    "acu_take_fixed_size_binary": (i32, [vp, i32, P(Array), P(Array), i32, i32, P(ArrayOut)]),
     "acu_arith": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_bitwise": (i32, [vp, i32, i32, P(Array), P(Array), P(ArrayOut)]),
     "acu_neg": (i32, [vp, i32, i32, P(Array), P(ArrayOut)]),

@@ -69,6 +69,8 @@ extern "C" acu_status acu_export_column(acu_ctx *ctx, const acu_column *col, acu
                                         struct ArrowSchema *out_schema) {
   if (!col || !out_array) return ctx ? acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "export: NULL argument") : ACU_ERR_INVALID_ARGUMENT;
   out_array->array.release = nullptr;  // stays NULL on every error path: the caller of a failed export has nothing to release
+  if (col->kind == ACU_COL_FIXED_SIZE_BINARY)
+    return ctx ? acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "export: FixedSizeBinary columns are not supported") : ACU_ERR_INVALID_ARGUMENT;
   if (device_type != ARROW_DEVICE_CPU) {
     // a device column needs the ctx: no event is handed over (sync_event = NULL), so the data must be complete when this
     // returns — synchronise BEFORE anything is allocated or published

@@ -153,6 +153,8 @@ static acu_status concat_one_field(acu_ctx *ctx, int32_t n, const acu_column *co
                       "It is not possible to concatenate arrays of different data types (kind %d width %d, kind %d width %d).",
                       c0.kind, c0.width, c.kind, c.width);
   }
+  if (c0.kind == ACU_COL_FIXED_SIZE_BINARY)
+    return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, 0, "concat: FixedSizeBinary columns are not supported");
   if (c0.kind == ACU_COL_BYTES) ACU_TRY(acu_offset_width_check(ctx, c0.width));
   int64_t total = 0;
   bool any_nulls = false;

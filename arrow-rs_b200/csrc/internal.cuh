@@ -96,6 +96,20 @@ acu_status acu_filter_bytes_col_launch(acu_ctx *ctx, const acu_filter_plan *plan
 acu_status acu_filter_bytes_col_finalize(acu_ctx *ctx, const acu_bytes_col_state *st, const unsigned long long *hres,
                                          int64_t *out_data_len);
 
+// FixedSizeBinary columns (fixed_size_binary.cu) inside the record-batch drivers: the validity, and the values of the
+// widths the fixed-width kernels serve, go through acu_filter_cols_launch / acu_take_cols_launch with the kind / element
+// width given here; the other widths' values through the row gather the *_values_launch calls queue (errors in RES_ERR2).
+int acu_fsb_filter_kind(const acu_filter_plan *plan, int32_t w, const acu_array *values, const acu_array_out *out);  // 0 or 2
+acu_status acu_fsb_filter_values_launch(acu_ctx *ctx, const acu_filter_plan *plan, int32_t w, const acu_array *values, acu_array_out *out,
+                                        unsigned long long *res);
+void acu_fsb_filter_finalize(const acu_filter_plan *plan, int mode, int32_t w, const unsigned long long *hres, acu_array_out *out);
+int32_t acu_fsb_take_width(int32_t w, const acu_array *values, const acu_array_out *out);  // w when k_take serves the values, else 0
+acu_status acu_fsb_take_values_launch(acu_ctx *ctx, int32_t w, const acu_array *values, const acu_array *indices, acu_dtype index_dtype,
+                                      bool idx_nulls, acu_array_out *out, unsigned long long *res);
+// mode: acu_take_cols_launch's, -1 when no validity gather was queued
+acu_status acu_fsb_take_finalize(acu_ctx *ctx, int32_t w, const acu_array *values, const acu_array *indices, acu_dtype index_dtype,
+                                 bool val_nulls, int mode, const unsigned long long *hres, acu_array_out *out);
+
 // compare_op (arrow-ord/src/cmp.rs:220-382), elementwise.cu: the host-side decisions of every comparison, whatever the
 // operand type (primitive, Utf8 / Binary, view). The kernels compute is_lt(a, b) or is_eq(a, b) of the swapped operands
 // (a, b) at every slot, negate, then fold the validity into the values (distinct / not_distinct) or write it beside them.

@@ -24,6 +24,10 @@ acu_status bad_kind(acu_ctx *ctx, int32_t c, int32_t kind) {
   return ACU_ERR_INVALID_ARGUMENT;
 }
 
+acu_status bad_width(acu_ctx *ctx, int32_t c, int32_t width) {
+  return acu_fail(ctx, ACU_ERR_INVALID_ARGUMENT, -1, 0, 0, (uint64_t)c, "column %d: FixedSizeBinary byte width %d < 0", c, width);
+}
+
 // A failed launch may leave work queued: wait for it before returning the error (like the reference, the failing
 // column's own ArrowError).
 acu_status drain(acu_ctx *ctx, acu_status st) {
@@ -51,8 +55,10 @@ acu_status filter_columns(acu_ctx *ctx, const acu_filter_plan *plan, int32_t n_c
   std::vector<acu_bytes_col_state> bstate(n_columns);
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
-    if (col.kind != ACU_COL_PRIMITIVE && col.kind != ACU_COL_BOOLEAN && col.kind != ACU_COL_BYTES) return bad_kind(ctx, c, col.kind);
+    if (col.kind < ACU_COL_PRIMITIVE || col.kind > ACU_COL_FIXED_SIZE_BINARY) return bad_kind(ctx, c, col.kind);
+    if (col.kind == ACU_COL_FIXED_SIZE_BINARY && col.width < 0) return bad_width(ctx, c, col.width);
     kinds[c] = col.kind == ACU_COL_PRIMITIVE ? 0 : col.kind == ACU_COL_BOOLEAN ? 1 : 2;
+    if (col.kind == ACU_COL_FIXED_SIZE_BINARY) kinds[c] = acu_fsb_filter_kind(plan, col.width, &col.array, &outs[c].array);
     widths[c] = col.width;
     vals[c] = &col.array;
     outp[c] = &outs[c].array;
@@ -61,6 +67,11 @@ acu_status filter_columns(acu_ctx *ctx, const acu_filter_plan *plan, int32_t n_c
   ACU_TRY(acu_res_reset_n(ctx, n_columns));
   {  // values of fixed-width columns + every validity compaction, like columns sharing launches
     acu_status st = acu_filter_cols_launch(ctx, plan, n_columns, kinds.data(), widths.data(), vals.data(), outp.data(), resp.data(), mode.data());
+    if (st != ACU_OK) return drain(ctx, st);
+  }
+  for (int32_t c = 0; c < n_columns; ++c) {  // FixedSizeBinary values the fixed-width kernels do not serve
+    if (columns[c].kind != ACU_COL_FIXED_SIZE_BINARY || kinds[c] != 2) continue;
+    acu_status st = acu_fsb_filter_values_launch(ctx, plan, columns[c].width, &columns[c].array, &outs[c].array, acu_dres(ctx, c));
     if (st != ACU_OK) return drain(ctx, st);
   }
   size_t k = 0;
@@ -73,7 +84,8 @@ acu_status filter_columns(acu_ctx *ctx, const acu_filter_plan *plan, int32_t n_c
   }
   ACU_TRY(acu_res_fetch_n(ctx, n_columns));
   for (int32_t c = 0; c < n_columns; ++c) {
-    acu_filter_col_finalize(plan, mode[c], acu_hres(ctx, c), &outs[c].array);
+    if (columns[c].kind == ACU_COL_FIXED_SIZE_BINARY) acu_fsb_filter_finalize(plan, mode[c], columns[c].width, acu_hres(ctx, c), &outs[c].array);
+    else acu_filter_col_finalize(plan, mode[c], acu_hres(ctx, c), &outs[c].array);
     outs[c].data_len = 0;
     if (columns[c].kind == ACU_COL_BYTES) ACU_TRY(acu_filter_bytes_col_finalize(ctx, &bstate[c], acu_hres(ctx, c), &outs[c].data_len));
   }
@@ -119,9 +131,15 @@ acu_status take_columns(acu_ctx *ctx, int32_t n_columns, const acu_column *colum
   std::vector<int> who;
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
-    if (col.kind != ACU_COL_PRIMITIVE && col.kind != ACU_COL_BOOLEAN && col.kind != ACU_COL_BYTES) return bad_kind(ctx, c, col.kind);
+    if (col.kind < ACU_COL_PRIMITIVE || col.kind > ACU_COL_FIXED_SIZE_BINARY) return bad_kind(ctx, c, col.kind);
     if (col.kind == ACU_COL_BYTES && !val_nulls[c]) continue;  // nulls = indices.nulls().cloned(): queued with the bytes pass
-    eb.push_back(col.kind == ACU_COL_PRIMITIVE ? col.width : 0);
+    int32_t width = col.kind == ACU_COL_PRIMITIVE ? col.width : 0;
+    if (col.kind == ACU_COL_FIXED_SIZE_BINARY) {
+      if (col.width < 0) return bad_width(ctx, c, col.width);
+      width = acu_fsb_take_width(col.width, &col.array, &outs[c].array);
+      if (width == 0 && !val_nulls[c] && !indices->validity) continue;  // no validity to gather: the row gather alone
+    }
+    eb.push_back(width);
     vals.push_back(&col.array);
     isbool.push_back(col.kind == ACU_COL_BOOLEAN);
     vnulls.push_back(val_nulls[c]);
@@ -137,6 +155,11 @@ acu_status take_columns(acu_ctx *ctx, int32_t n_columns, const acu_column *colum
     if (st != ACU_OK) return drain(ctx, st);
     for (size_t i = 0; i < who.size(); ++i) mode[who[i]] = modes[i];
   }
+  for (int32_t c = 0; c < n_columns; ++c) {  // FixedSizeBinary values k_take does not serve
+    if (columns[c].kind != ACU_COL_FIXED_SIZE_BINARY) continue;
+    st = acu_fsb_take_values_launch(ctx, columns[c].width, &columns[c].array, indices, index_dtype, idx_nulls, &outs[c].array, acu_dres(ctx, c));
+    if (st != ACU_OK) return drain(ctx, st);
+  }
   size_t k = 0;
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
@@ -150,6 +173,10 @@ acu_status take_columns(acu_ctx *ctx, int32_t n_columns, const acu_column *colum
   for (int32_t c = 0; c < n_columns; ++c) {
     const acu_column &col = columns[c];
     outs[c].data_len = 0;
+    if (col.kind == ACU_COL_FIXED_SIZE_BINARY) {
+      ACU_TRY(acu_fsb_take_finalize(ctx, col.width, &col.array, indices, index_dtype, val_nulls[c], mode[c], acu_hres(ctx, c), &outs[c].array));
+      continue;
+    }
     if (mode[c] >= 0) ACU_TRY(acu_take_col_finalize(ctx, &col.array, indices, index_dtype, mode[c], acu_hres(ctx, c), &outs[c].array));
     if (col.kind == ACU_COL_BYTES)
       ACU_TRY(acu_take_bytes_col_finalize(ctx, &col.array, indices, index_dtype, &bstate[c], acu_hres(ctx, c), &outs[c].data_len, &outs[c].array));

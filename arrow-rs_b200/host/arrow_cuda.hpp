@@ -143,7 +143,7 @@ inline std::vector<uint8_t> pack_bits(const std::vector<bool> &bits) {
 // DataType / native type traits (arrow-array/src/types.rs:67-80)
 // ---------------------------------------------------------------------------------------
 enum class DataType { Int8, Int16, Int32, Int64, UInt8, UInt16, UInt32, UInt64, Float32, Float64, Boolean, Utf8, Decimal32, Decimal64, Decimal128,
-                      List, LargeList, FixedSizeList, RunEndEncoded, Struct, Union };
+                      List, LargeList, FixedSizeList, RunEndEncoded, Struct, Union, FixedSizeBinary };
 
 template <class T> struct NativeOf;
 #define ACU_NATIVE(T, DT, CODE) \
@@ -595,6 +595,71 @@ using Int64RunArray = RunArray<int64_t>;
 
 // StructArray (arrow-array/src/array/struct_array.rs): columns of the struct's length from its logical row 0, and the
 // nulls. Every field is nullable here.
+// FixedSizeBinaryArray (arrow-array/src/array/fixed_size_binary_array.rs): `value_length` bytes per row, the rows from
+// row `row_offset` of `values`.
+class FixedSizeBinaryArray : public Array {
+ public:
+  FixedSizeBinaryArray(int32_t value_length, Buffer values, int64_t len, std::optional<NullBuffer> nulls, int64_t row_offset = 0)
+      : value_length_(value_length), values_(std::move(values)), row_offset_(row_offset) {
+    len_ = len;
+    nulls_ = std::move(nulls);
+  }
+  // FixedSizeBinaryArray::try_new (:170-201): of width 0 the length comes from the NullBuffer (0 without one)
+  static Result<FixedSizeBinaryArray> try_new(int32_t value_length, Buffer values, std::optional<NullBuffer> nulls) {
+    if (value_length < 0)
+      return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: Value length cannot be negative, got " + std::to_string(value_length)};
+    int64_t len;
+    if (value_length == 0) {
+      if (values.len() != 0)
+        return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: Buffer cannot have non-zero length if the value length is zero"};
+      len = nulls ? nulls->len : 0;
+    } else {
+      len = (int64_t)values.len() / value_length;
+      if (nulls && nulls->len != len)
+        return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: Incorrect length of null buffer for FixedSizeBinaryArray, expected " +
+                                                        std::to_string(len) + " got " + std::to_string(nulls->len)};
+    }
+    return FixedSizeBinaryArray(value_length, std::move(values), len, std::move(nulls));
+  }
+  // try_from_sparse_iter_with_size: a null row's bytes are zero
+  static FixedSizeBinaryArray from(const std::vector<std::optional<std::vector<uint8_t>>> &rows, int32_t value_length) {
+    std::vector<uint8_t> bytes(rows.size() * (size_t)value_length, 0);
+    std::vector<bool> valid(rows.size(), true);
+    for (size_t i = 0; i < rows.size(); ++i) {
+      if (!rows[i]) { valid[i] = false; continue; }
+      if (rows[i]->size() != (size_t)value_length) throw std::invalid_argument("FixedSizeBinaryArray::from: a row of the wrong width");
+      std::copy(rows[i]->begin(), rows[i]->end(), bytes.begin() + i * value_length);
+    }
+    return FixedSizeBinaryArray(value_length, Buffer::from_host(bytes.data(), bytes.size()), (int64_t)rows.size(), nulls_from_mask(valid));
+  }
+  DataType data_type() const override { return DataType::FixedSizeBinary; }
+  int32_t value_length() const { return value_length_; }
+  std::vector<uint8_t> value(int64_t i) const {
+    if (i < 0 || i >= len_) throw std::out_of_range("FixedSizeBinaryArray::value: index out of bounds");
+    std::vector<uint8_t> v((size_t)value_length_);
+    if (value_length_)
+      acu_memcpy_d2h(Context::get().raw(), v.data(), static_cast<const uint8_t *>(values_ptr()) + (size_t)i * value_length_, v.size());
+    return v;
+  }
+  // Array::slice: zero copy
+  FixedSizeBinaryArray slice(int64_t offset, int64_t length) const {
+    FixedSizeBinaryArray out(value_length_, values_, length, nulls_, row_offset_ + offset);
+    if (out.nulls_) {
+      out.nulls_->offset += offset;
+      out.nulls_->len = length;
+      out.nulls_->null_count = -1;  // recounted on device on first use
+    }
+    return out;
+  }
+  const Buffer &values() const { return values_; }
+ protected:
+  const void *values_ptr() const override { return static_cast<const uint8_t *>(values_.data()) + (size_t)row_offset_ * value_length_; }
+ private:
+  int32_t value_length_ = 0;
+  Buffer values_;
+  int64_t row_offset_ = 0;
+};
+
 class StructArray : public Array {
  public:
   StructArray(std::vector<ArrayRef> columns, int64_t len, std::optional<NullBuffer> nulls) : columns_(std::move(columns)) {
@@ -777,7 +842,7 @@ inline ArrayRef make_primitive(DataType dt, Buffer values, int64_t len, std::opt
 }
 inline const char *dtype_display(DataType t) {
   static const char *n[] = {"Int8", "Int16", "Int32", "Int64", "UInt8", "UInt16", "UInt32", "UInt64", "Float32", "Float64", "Boolean", "Utf8",
-                            "Decimal32", "Decimal64", "Decimal128", "List", "LargeList", "FixedSizeList", "RunEndEncoded", "Struct", "Union"};
+                            "Decimal32", "Decimal64", "Decimal128", "List", "LargeList", "FixedSizeList", "RunEndEncoded", "Struct", "Union", "FixedSizeBinary"};
   return n[(int)t];
 }
 template <class A> std::string type_text(const A &a) {
@@ -797,6 +862,9 @@ inline acu_column column_view(const Array &a) {
     c.array.values = s.offsets().data();
     c.array.values_offset = 0;
     c.data = static_cast<const uint8_t *>(s.value_data().data());
+  } else if (a.data_type() == DataType::FixedSizeBinary) {
+    c.kind = ACU_COL_FIXED_SIZE_BINARY;
+    c.width = static_cast<const FixedSizeBinaryArray &>(a).value_length();
   } else {
     c.kind = ACU_COL_PRIMITIVE;
     c.width = dtype_width(a.data_type());
@@ -816,7 +884,8 @@ struct BatchOutputs {
     outs.assign(n, acu_column_out{});
     for (size_t i = 0; i < n; ++i) {
       const DataType dt = cols[i]->data_type();
-      const size_t vbytes = dt == DataType::Boolean ? acu_bitmap_bytes(rows) : dt == DataType::Utf8 ? (size_t)(rows + 1) * 4 : (size_t)rows * dtype_width(dt);
+      const size_t w = dt == DataType::FixedSizeBinary ? (size_t) static_cast<const FixedSizeBinaryArray &>(*cols[i]).value_length() : dtype_width(dt);
+      const size_t vbytes = dt == DataType::Boolean ? acu_bitmap_bytes(rows) : dt == DataType::Utf8 ? (size_t)(rows + 1) * 4 : (size_t)rows * w;
       values[i] = Buffer::allocate(vbytes);
       validity[i] = Buffer::allocate(acu_bitmap_bytes(rows));
       outs[i].array.values = values[i].data();
@@ -835,6 +904,9 @@ struct BatchOutputs {
       const acu_array_out &o = outs[i].array;
       if (dt == DataType::Boolean) res.push_back(std::make_shared<BooleanArray>(values[i], 0, o.len, out_nulls(o, validity[i])));
       else if (dt == DataType::Utf8) res.push_back(std::make_shared<StringArray>(values[i], data[i], o.len, out_nulls(o, validity[i])));
+      else if (dt == DataType::FixedSizeBinary)
+        res.push_back(std::make_shared<FixedSizeBinaryArray>(static_cast<const FixedSizeBinaryArray &>(*cols[i]).value_length(), values[i], o.len,
+                                                             out_nulls(o, validity[i])));
       else res.push_back(make_primitive(dt, values[i], o.len, out_nulls(o, validity[i])));
     }
     return res;
@@ -889,6 +961,12 @@ class FilterPredicate {
       if ((st = acu_filter_bytes(c.raw(), plan_.get(), 4, s.offsets().data(), static_cast<const uint8_t *>(s.value_data().data()), &v,
                                  offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o)) != ACU_OK) return c.last_error(st);
       return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, detail::out_nulls(o, nb)));
+    }
+    if (values.data_type() == DataType::FixedSizeBinary) {  // filter_fixed_size_binary (filter.rs:946-996)
+      const int32_t w = static_cast<const FixedSizeBinaryArray &>(values).value_length();
+      acu_array_out o = detail::make_out(vb, nb, (size_t)n * w, n);
+      if ((st = acu_filter_fixed_size_binary(c.raw(), plan_.get(), w, &v, &o)) != ACU_OK) return c.last_error(st);
+      return ArrayRef(std::make_shared<FixedSizeBinaryArray>(w, vb, o.len, detail::out_nulls(o, nb)));
     }
     const int w = dtype_width(values.data_type());
     acu_array_out o = detail::make_out(vb, nb, (size_t)n * w, n);
@@ -992,6 +1070,12 @@ inline Result<ArrayRef> take(const Array &values, const Array &indices, std::opt
       return c.last_error(st);
     return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, detail::out_nulls(o, nb)));
   }
+  if (values.data_type() == DataType::FixedSizeBinary) {  // take_fixed_size_binary (take.rs:802-862)
+    const int32_t w = static_cast<const FixedSizeBinaryArray &>(values).value_length();
+    acu_array_out o = detail::make_out(vb, nb, (size_t)m * w, m);
+    if ((st = acu_take_fixed_size_binary(c.raw(), w, &v, &ix, (acu_dtype)dtype_code(it), cb, &o)) != ACU_OK) return c.last_error(st);
+    return ArrayRef(std::make_shared<FixedSizeBinaryArray>(w, vb, o.len, detail::out_nulls(o, nb)));
+  }
   const int w = dtype_width(values.data_type());
   acu_array_out o = detail::make_out(vb, nb, (size_t)m * w, m);
   if ((st = acu_take_primitive(c.raw(), w, &v, &ix, (acu_dtype)dtype_code(it), cb, &o)) != ACU_OK) return c.last_error(st);
@@ -1047,6 +1131,14 @@ inline Result<ArrayRef> filter_nested(const Array &values, const FilterPredicate
 inline Result<ArrayRef> take_nested(const Array &values, const Array &indices, int cb, bool keep);
 inline bool is_nested(DataType t) { return t == DataType::Struct || t == DataType::Union; }
 
+// MutableArrayData keeps every extended row of a FixedSizeBinary(0) child (try_new's length rule is the top level's)
+inline ArrayRef keep_width0_rows(ArrayRef a, int64_t rows) {
+  if (a->data_type() != DataType::FixedSizeBinary) return a;
+  const auto &f = static_cast<const FixedSizeBinaryArray &>(*a);
+  if (f.value_length() != 0 || f.len() == rows) return a;
+  return std::make_shared<FixedSizeBinaryArray>(0, f.values(), rows, f.nulls());
+}
+
 inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan,
                                    std::optional<bool> child_step = std::nullopt) {
   if (is_nested(values.data_type())) return filter_nested(values, pred, plan, child_step);
@@ -1055,7 +1147,7 @@ inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &p
     if (r.is_err() || !child_step.value_or(false)) return r;
     ArrayRef a = r.unwrap();
     a->drop_empty_nulls();
-    return a;
+    return keep_width0_rows(a, pred.count());
   }
   Context &c = Context::get();
   const int64_t n = pred.count();
@@ -1113,6 +1205,11 @@ inline Result<ArrayRef> take_list_level(const Array &values, const Array &indice
 inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool extend) {
   if (is_list(values.data_type())) return take_list_level(values, indices, cb, extend);
   if (is_nested(values.data_type())) return take_nested(values, indices, cb, extend);
+  if (values.data_type() == DataType::FixedSizeBinary && extend) {
+    auto r = take(values, indices, TakeOptions{cb != 0});
+    if (r.is_err()) return r;
+    return keep_width0_rows(r.unwrap(), indices.len());
+  }
   if (!extend || values.data_type() != DataType::Utf8) return take(values, indices, TakeOptions{cb != 0});
   Context &c = Context::get();
   const auto &s = static_cast<const StringArray &>(values);
@@ -1200,6 +1297,8 @@ inline ArrayRef slice_any(const Array &a, int64_t off, int64_t len) {
       s.offsets().to_host(o.data(), o.size() * 4);
       return std::make_shared<StringArray>(Buffer::from_host(o.data() + off, (size_t)(len + 1) * 4), s.value_data(), len, nulls);
     }
+    case DataType::FixedSizeBinary:
+      return std::make_shared<FixedSizeBinaryArray>(static_cast<const FixedSizeBinaryArray &>(a).slice(off, len));
     case DataType::Struct: {
       std::vector<ArrayRef> cols;
       for (const auto &col : static_cast<const StructArray &>(a).columns()) cols.push_back(slice_any(*col, off, len));
@@ -1229,6 +1328,8 @@ inline ArrayRef empty_like(const Array &a) {
     case DataType::FixedSizeList:
       return std::make_shared<FixedSizeListArray>(static_cast<const FixedSizeListArray &>(a).value_length(), empty_like(*list_values(a)), 0,
                                                   std::nullopt);
+    case DataType::FixedSizeBinary:
+      return std::make_shared<FixedSizeBinaryArray>(static_cast<const FixedSizeBinaryArray &>(a).value_length(), Buffer::allocate(0), 0, std::nullopt);
     default: throw std::runtime_error(std::string("RunArray values of type ") + dtype_display(a.data_type()) + " are not supported by this mirror");
   }
 }
@@ -1280,6 +1381,7 @@ Result<ArrayRef> take(const RunArray<R> &values, const Array &indices, std::opti
       break;
     }
     case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: case DataType::Struct: case DataType::Union:
+    case DataType::FixedSizeBinary:  // the run merge would need a value_length-byte comparator
       rv.kind = ACU_RUN_VALUES_NESTED;
       break;
     default:

@@ -737,6 +737,32 @@ acu_status acu_length_bytes(acu_ctx *ctx, int32_t offset_bytes, acu_length_op op
 acu_status acu_length_byte_view(acu_ctx *ctx, acu_length_op op, const acu_view_array *a, acu_array_out *out);
 acu_status acu_length_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, acu_length_op op, const acu_array *a, acu_array_out *out);
 
+/* filter / take of a FixedSizeBinary(byte_width) column (filter_fixed_size_binary filter.rs:946-996, take_fixed_size_binary
+ * take.rs:802-862). `values->values` points at logical row 0 (values->len rows of byte_width bytes, any alignment);
+ * out->values has capacity (output rows) x byte_width bytes, any alignment; out->validity acu_bitmap_bytes(output rows) + 8.
+ * byte_width < 0 => ACU_ERR_INVALID_ARGUMENT.
+ *   - filter: the selected rows' bytes in row order, bytes under null slots included; the NullBuffer as for
+ *     acu_filter_primitive (FilterPredicate::filter_nulls; IterationStrategy::All keeps the input's).
+ *   - take: check_bounds and "Take only supported for integers" as for acu_take_primitive. Widths 1, 2, 4, 8 and 16 follow
+ *     take_fixed_size (take_native byte for byte): an in-bounds null index still gathers its row, an out-of-bounds null
+ *     index gives zeros, a valid out-of-bounds index is ACU_ERR_PANIC_OUT_OF_BOUNDS "Out-of-bounds index {index}". Every
+ *     other width (0 and 32 included) follows the dynamic-length path: a null index gives byte_width zero bytes and is never
+ *     read; a valid index reads values[index * byte_width .. + byte_width] in wrapping 64-bit arithmetic, so an index whose
+ *     product wraps into the buffer reads those bytes; a slice past the buffer or out of order is ACU_ERR_PANIC_OUT_OF_BOUNDS
+ *     at the lowest such row, checked in this order: "range start index {s} out of range for slice of length
+ *     {len * byte_width}", "range end index {e} out of range for slice of length {len * byte_width}", "slice index starts
+ *     at {s} but ends at {e}" (lhs_bits = s, rhs_bits = e). Then, when the values have a null, a valid index past them
+ *     is the validity gather's ACU_ERR_PANIC_OUT_OF_BOUNDS "assertion failed: idx < self.bit_len".
+ *     NullBuffer::union(take_nulls(values), indices.nulls()): has_validity = 1 only when the result has a null (unlike
+ *     acu_take_primitive, indices whose NullBuffer has no null give none).
+ *   - byte_width 0 (FixedSizeBinaryArray::try_new takes the length from the NullBuffer): a take, or a filter that is not
+ *     IterationStrategy::All, whose result has no NullBuffer has out->len = 0.
+ * Synchronous (refused inside a stream-ordered section); kernel time in ACU_K_FILTER / ACU_K_TAKE. */
+acu_status acu_filter_fixed_size_binary(acu_ctx *ctx, const acu_filter_plan *plan, int32_t byte_width, const acu_array *values,
+                                        acu_array_out *out);
+acu_status acu_take_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, const acu_array *values, const acu_array *indices,
+                                      acu_dtype index_dtype, int32_t check_bounds, acu_array_out *out);
+
 /* substring(array, start, length) (substring.rs:73-459): has_length = 0 is `None`, else `Some(length)`.
  *
  * acu_substring_bytes — byte_substring (:319-397) for Utf8 / LargeUtf8 (is_utf8 = 1) and Binary / LargeBinary (0).
@@ -1008,7 +1034,9 @@ acu_status acu_aggregate_boolean(acu_ctx *ctx, acu_agg_op op, const acu_array *a
  * bitmap; BYTES (Utf8/Binary/LargeUtf8/LargeBinary): `array.values` = the offsets
  * buffer (i32 if width == 4, i64 if width == 8, array.len + 1 entries), `data` = the
  * value bytes, `array.validity/len/null_count` the nulls. */
-typedef enum acu_column_kind { ACU_COL_PRIMITIVE = 0, ACU_COL_BOOLEAN = 1, ACU_COL_BYTES = 2 } acu_column_kind;
+/* FIXED_SIZE_BINARY (filter / take record-batch calls only): `array` as for acu_filter_fixed_size_binary with byte width
+ * `width`; acu_concat, acu_concat_batches and export refuse it with ACU_ERR_INVALID_ARGUMENT. */
+typedef enum acu_column_kind { ACU_COL_PRIMITIVE = 0, ACU_COL_BOOLEAN = 1, ACU_COL_BYTES = 2, ACU_COL_FIXED_SIZE_BINARY = 3 } acu_column_kind;
 
 typedef struct acu_column {
   int32_t kind;          /* acu_column_kind */

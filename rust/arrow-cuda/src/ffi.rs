@@ -88,6 +88,7 @@ pub const ACU_BOOL_IS_NOT_NULL: i32 = 7;
 pub const ACU_COL_PRIMITIVE: i32 = 0;
 pub const ACU_COL_BOOLEAN: i32 = 1;
 pub const ACU_COL_BYTES: i32 = 2;
+pub const ACU_COL_FIXED_SIZE_BINARY: i32 = 3;
 pub const ACU_MAX_BATCH_COLUMNS: usize = 64;
 
 #[repr(C)]
@@ -289,6 +290,10 @@ extern "C" {
                             out_offsets: *mut i32, out_child_rows: *mut i32, out_field_starts: *mut i64) -> acu_status;
     pub fn acu_take_union(ctx: *mut acu_ctx, u: *const acu_union_array, indices: *const acu_array, index_dtype: i32, check_bounds: i32,
                           out_type_ids: *mut i8, out_offsets: *mut i32, out_child_rows: *mut i32, out_field_starts: *mut i64) -> acu_status;
+    pub fn acu_filter_fixed_size_binary(ctx: *mut acu_ctx, plan: *const acu_filter_plan, byte_width: i32, values: *const acu_array,
+                                        out: *mut acu_array_out) -> acu_status;
+    pub fn acu_take_fixed_size_binary(ctx: *mut acu_ctx, byte_width: i32, values: *const acu_array, indices: *const acu_array,
+                                      index_dtype: i32, check_bounds: i32, out: *mut acu_array_out) -> acu_status;
     pub fn acu_arith(ctx: *mut acu_ctx, dtype: i32, op: i32, a: *const acu_array, b: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_neg(ctx: *mut acu_ctx, dtype: i32, checked: i32, a: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_decimal_arith(ctx: *mut acu_ctx, op: i32, lt: *const acu_decimal_type, a: *const acu_array, rt: *const acu_decimal_type,

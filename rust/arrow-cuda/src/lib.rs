@@ -144,12 +144,13 @@ fn decimal_type(t: &DataType) -> Option<ffi::acu_decimal_type> {
     Some(ffi::acu_decimal_type { byte_width, precision, scale, reserved: [0; 2] })
 }
 
-enum Kind { Primitive(usize), Boolean, Bytes(usize) }
+enum Kind { Primitive(usize), Boolean, Bytes(usize), FixedSizeBinary(usize) }
 fn kind_of(t: &DataType) -> Result<Kind, ArrowError> {
     match t {
         DataType::Boolean => Ok(Kind::Boolean),
         DataType::Utf8 | DataType::Binary => Ok(Kind::Bytes(4)),
         DataType::LargeUtf8 | DataType::LargeBinary => Ok(Kind::Bytes(8)),
+        DataType::FixedSizeBinary(w) if *w >= 0 => Ok(Kind::FixedSizeBinary(*w as usize)),
         // filter / take are type-agnostic copies: every fixed-width primitive goes by element width (SURVEY.md §8(a))
         t => t.primitive_width().map(Kind::Primitive).ok_or_else(|| ArrowError::NotYetImplemented(format!("arrow-cuda: data type {t}"))),
     }
@@ -207,6 +208,14 @@ impl DeviceArray {
                 col.kind = ffi::ACU_COL_BYTES;
                 col.width = ob as i32;
             }
+            Kind::FixedSizeBinary(w) => {  // values from logical row 0 (any alignment)
+                let bytes = &d.buffers()[0].as_slice()[d.offset() * w..(d.offset() + d.len()) * w];
+                let b = DeviceBuffer::from_host(ctx, bytes)?;
+                a.values = b.as_ptr();
+                bufs.push(b);
+                col.kind = ffi::ACU_COL_FIXED_SIZE_BINARY;
+                col.width = w as i32;
+            }
         }
         col.array = a;
         Ok(Self { _bufs: bufs, column: col, data_bytes })
@@ -222,6 +231,7 @@ impl ColumnOut {
             Kind::Primitive(w) => rows.max(1) * w,
             Kind::Boolean => bitmap_bytes(rows.max(1)),
             Kind::Bytes(ob) => (rows + 1) * ob,
+            Kind::FixedSizeBinary(w) => (rows * w).max(1),
         };
         let values = DeviceBuffer::allocate(ctx, vbytes)?;
         let validity = DeviceBuffer::allocate(ctx, bitmap_bytes(rows.max(1)))?;
@@ -246,6 +256,7 @@ impl ColumnOut {
         match kind_of(data_type)? {
             Kind::Primitive(w) => { b = b.add_buffer(self.values.to_host(len * w)?); }
             Kind::Boolean => { b = b.add_buffer(self.values.to_host(bitmap_bytes(len))?); }
+            Kind::FixedSizeBinary(w) => { b = b.add_buffer(self.values.to_host(len * w)?); }
             Kind::Bytes(ob) => {
                 b = b.add_buffer(self.values.to_host((len + 1) * ob)?);
                 b = b.add_buffer(self.data.as_ref().unwrap().to_host(self.out.data_len as usize)?);
@@ -306,6 +317,10 @@ pub mod compute {
             let st = match kind_of(values.data_type())? {
                 Kind::Primitive(w) => unsafe { ffi::acu_filter_primitive(ctx.raw(), self.plan.raw, w as i32, v.view(), out.array_out()) },
                 Kind::Boolean => unsafe { ffi::acu_filter_boolean(ctx.raw(), self.plan.raw, v.view(), out.array_out()) },
+                // filter_fixed_size_binary (filter.rs:946-996)
+                Kind::FixedSizeBinary(w) => unsafe {
+                    ffi::acu_filter_fixed_size_binary(ctx.raw(), self.plan.raw, w as i32, v.view(), out.array_out())
+                },
                 Kind::Bytes(ob) => unsafe {
                     ffi::acu_filter_bytes(ctx.raw(), self.plan.raw, ob as i32, v.view().values, v.column.data, v.view(), out.out.array.values,
                                           out.out.data, out.out.data_capacity, &mut out.out.data_len, &mut out.out.array)
@@ -380,6 +395,10 @@ pub mod compute {
             Kind::Boolean => {
                 out = ColumnOut::new(&ctx, values.data_type(), m, 0)?;
                 st = unsafe { ffi::acu_take_boolean(ctx.raw(), v.view(), ix.view(), idt, check, out.array_out()) };
+            }
+            Kind::FixedSizeBinary(w) => {  // take_fixed_size_binary (take.rs:802-862)
+                out = ColumnOut::new(&ctx, values.data_type(), m, 0)?;
+                st = unsafe { ffi::acu_take_fixed_size_binary(ctx.raw(), w as i32, v.view(), ix.view(), idt, check, out.array_out()) };
             }
             Kind::Bytes(ob) => {
                 // two-phase: offsets + required bytes first, then the copy (take_bytes computes the capacity first too, take.rs:520-523)
@@ -467,7 +486,7 @@ pub mod compute {
             let mut rv: ffi::acu_run_values = unsafe { std::mem::zeroed() };
             let _up = match vals.data_type() {
                 DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) | DataType::RunEndEncoded(_, _)
-                | DataType::Struct(_) | DataType::Union(_, _) => {
+                | DataType::Struct(_) | DataType::Union(_, _) | DataType::FixedSizeBinary(_) => {  // (the run merge compares values)
                     rv.kind = ffi::ACU_RUN_VALUES_NESTED;
                     None
                 }
@@ -476,6 +495,7 @@ pub mod compute {
                     match kind_of(t)? {
                         Kind::Primitive(w) => { rv.kind = ffi::ACU_RUN_VALUES_FIXED; rv.width = w as i32; rv.array = *u.view(); }
                         Kind::Boolean => { rv.kind = ffi::ACU_RUN_VALUES_BOOLEAN; rv.array = *u.view(); }
+                        Kind::FixedSizeBinary(_) => unreachable!(),
                         Kind::Bytes(ob) => {
                             rv.kind = ffi::ACU_RUN_VALUES_BYTES;
                             rv.width = ob as i32;
@@ -573,13 +593,20 @@ pub mod compute {
                 DataType::List(_) | DataType::LargeList(_) | DataType::FixedSizeList(_, _) => filter(ctx, child_plan.raw, lv.child.as_ref(), Some(step))?,
                 DataType::Struct(_) | DataType::Union(_, _) => nested::filter(ctx, child_plan.raw, lv.child.as_ref(), Some(step))?,
                 _ => {
+                    let rows = unsafe { ffi::acu_filter_plan_count(child_plan.raw) } as usize;
                     let c = FilterPredicate { plan: child_plan }.filter(lv.child.as_ref())?;
-                    if step { drop_empty_nulls(c) } else { c }
+                    if step { keep_width0_rows(drop_empty_nulls(c), rows) } else { c }
                 }
             };
             if child_step == Some(true) && o.null_count == 0 { o.has_validity = 0; }
             let offsets = if lv.ob > 0 { Some(offs.to_host((n + 1) * lv.ob)?) } else { None };
             Ok(rebuild(values, offsets, child, n, nulls_of(&validity, &o)?))
+        }
+
+        /// MutableArrayData keeps every extended row of a FixedSizeBinary(0) child (try_new's length rule is the top level's)
+        fn keep_width0_rows(a: ArrayRef, rows: usize) -> ArrayRef {
+            if a.data_type() != &DataType::FixedSizeBinary(0) || a.len() == rows { return a; }
+            make_array(unsafe { a.to_data().into_builder().len(rows).build_unchecked() })
         }
 
         fn drop_empty_nulls(a: ArrayRef) -> ArrayRef {
@@ -642,6 +669,7 @@ pub mod compute {
                     })?;
                     out.finish(child.data_type())
                 }
+                DataType::FixedSizeBinary(_) if extend => Ok(keep_width0_rows(super::take(child, map, None)?, map.len())),
                 _ => super::take(child, map, None),
             }
         }
@@ -1535,6 +1563,7 @@ pub mod compute {
                 let n = if l_s { r.len() } else { l.len() };
                 let mut out = ColumnOut::new(&ctx, &DataType::Boolean, n, 0)?;
                 let st = match kind_of(l.data_type())? {
+                    Kind::FixedSizeBinary(_) => return Err(ArrowError::NotYetImplemented(format!("arrow-cuda: data type {}", l.data_type()))),
                     Kind::Bytes(ob) => {
                         let (x, y) = (ffi::acu_bytes_array { offsets: a.view().values, data: a.column.data, nulls: *a.view() },
                                       ffi::acu_bytes_array { offsets: b.view().values, data: b.column.data, nulls: *b.view() });
