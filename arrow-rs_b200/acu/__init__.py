@@ -1344,12 +1344,59 @@ class Context:
         vals = left.values if left.dtype == BOOL else left.values[:n]
         return HostArray(left.dtype, vals, n, nulls.validity, 0, left.values_offset if left.dtype == BOOL else 0, nulls.null_count)
 
+    @staticmethod
+    def _zip_type(col):
+        """What zip compares for "the same data type": the column class plus its offset width / byte width / dtype."""
+        if isinstance(col, Utf8Column):
+            return ("bytes", col.offsets.dtype.itemsize)
+        if isinstance(col, ViewColumn):
+            return ("view",)
+        if isinstance(col, FixedSizeBinaryColumn):
+            return ("fsb", col.width)
+        return ("array", col.dtype)
+
     def zip(self, mask, truthy, falsy):
-        """arrow::compute::zip(mask, truthy, falsy) for primitive arrays / scalars."""
+        """arrow::compute::zip(mask, truthy, falsy) for primitive, Boolean (HostArray), Utf8 / Binary (Utf8Column), view
+        (ViewColumn) and FixedSizeBinary (FixedSizeBinaryColumn) operands; a scalar is a one-row operand marked is_scalar
+        (nulls.is_scalar for the column classes). A view result references truthy's data buffers, falsy's, both (truthy's
+        first) or none, as the reference decides."""
+        typed = (Utf8Column, ViewColumn, FixedSizeBinaryColumn)
+        if isinstance(truthy, typed) or isinstance(falsy, typed) or truthy.dtype == BOOL or falsy.dtype == BOOL:
+            return self._zip_columns(mask, truthy, falsy)
         assert truthy.dtype == falsy.dtype and truthy.dtype != BOOL
         n = mask.length
         return self._call_out((mask, truthy, falsy), n * truthy.width(), max(n, 1),
                               lambda md, td, fd, out: self.lib.acu_zip(self.h, truthy.width(), md, td, fd, out), truthy.dtype)
+
+    def _zip_columns(self, mask, truthy, falsy):
+        if self._zip_type(truthy) != self._zip_type(falsy):  # zip.rs:117-121 / ScalarZipper::try_new
+            raise ArrowError(abi.ERR_INVALID_ARGUMENT, "Invalid argument error: arguments need to have the same data type")
+        n = mask.length
+        with self._scope() as s:
+            md = s.upload(mask).descriptor()
+            if isinstance(truthy, Utf8Column):
+                dt, df = self._upload_bytes_col(truthy, s), self._upload_bytes_col(falsy, s)
+                ob = truthy.offsets.dtype.itemsize
+                return self._bytes_out(s, lambda oo, od, cap, tot, out: self.lib.acu_zip_bytes(
+                    self.h, ob, C.byref(md), C.byref(dt), C.byref(df), oo, od, cap, tot, out), n, ob)
+            if isinstance(truthy, ViewColumn):
+                dt, df = self._upload_view_col(truthy, s, s.keep), self._upload_view_col(falsy, s, s.keep)
+                d_views = s.malloc(n * 16 + 16)
+                out = s.out(0, n)
+                which = C.c_int32(-1)
+                self.check(self.lib.acu_zip_byte_view(self.h, C.byref(md), C.byref(dt), C.byref(df), d_views, C.byref(out), C.byref(which)))
+                buffers = {abi.ZIP_BUFFERS_NONE: [], abi.ZIP_BUFFERS_TRUTHY: list(truthy.buffers), abi.ZIP_BUFFERS_FALSY: list(falsy.buffers),
+                           abi.ZIP_BUFFERS_BOTH: list(truthy.buffers) + list(falsy.buffers)}[which.value]
+                return ViewColumn(self.d2h(d_views, n * 16).reshape(n, 16), buffers, self._nulls_out(out, n))
+            if isinstance(truthy, FixedSizeBinaryColumn):
+                dt, df = self._upload_fsb(truthy, s), self._upload_fsb(falsy, s)
+                out = s.out(n * truthy.width, n)
+                self.check(self.lib.acu_zip_fixed_size_binary(self.h, truthy.width, C.byref(md), C.byref(dt), C.byref(df), C.byref(out)))
+                return self._fsb_out(out, n, truthy.width)
+            dt, df = s.upload(truthy).descriptor(), s.upload(falsy).descriptor()
+            out = s.out(bitmap_bytes(n), n)
+            self.check(self.lib.acu_zip_boolean(self.h, C.byref(md), C.byref(dt), C.byref(df), C.byref(out)))
+            return self._read_out(out, BOOL)
 
     # -- boolean (arrow-arith/src/boolean.rs) -------------------------------------------------
     def boolean(self, op, a, b=None):

@@ -126,6 +126,7 @@ class RunValues(C.Structure):
 
 
 UNION_SPARSE, UNION_DENSE = range(2)
+ZIP_BUFFERS_NONE, ZIP_BUFFERS_TRUTHY, ZIP_BUFFERS_FALSY, ZIP_BUFFERS_BOTH = range(4)  # acu_zip_buffers
 UNION_MAX_FIELDS = 128
 
 
@@ -232,6 +233,10 @@ PROTOTYPES = {
     "acu_filter_plan_create_cmp": (i32, [vp, i32, i32, P(Array), P(Array), P(vp)]),
     "acu_nullif": (i32, [vp, P(Array), P(Array), P(ArrayOut)]),
     "acu_zip": (i32, [vp, i32, P(Array), P(Array), P(Array), P(ArrayOut)]),
+    "acu_zip_bytes": (i32, [vp, i32, P(Array), P(BytesArray), P(BytesArray), vp, vp, i64, P(i64), P(ArrayOut)]),
+    "acu_zip_byte_view": (i32, [vp, P(Array), P(ViewArray), P(ViewArray), vp, P(ArrayOut), P(i32)]),
+    "acu_zip_boolean": (i32, [vp, P(Array), P(Array), P(Array), P(ArrayOut)]),
+    "acu_zip_fixed_size_binary": (i32, [vp, i32, P(Array), P(Array), P(Array), P(ArrayOut)]),
     "acu_filter_plan_destroy": (None, [vp, vp]),
     "acu_filter_plan_indices": (i32, [vp, vp, i32, vp]),
     "acu_filter_plan_count": (i64, [vp]),

@@ -328,6 +328,22 @@ __global__ void __launch_bounds__(BY_THREADS, 2) k_bytes_offsets_copy(const R a,
   }
 }
 
+// p / w for every 64-bit p by one multiply-high (Granlund-Montgomery round-up multiplier), for the kernels that find the row
+// of a byte position in FixedSizeBinary(w) data (fixed_size_binary.cu, zip.cu): t = umulhi(magic, p), (t + ((p - t) >> sh1)) >> sh2.
+struct DivW {
+  uint64_t magic;
+  int sh1, sh2;
+};
+__device__ __forceinline__ uint64_t div_by(const DivW &d, uint64_t p) {
+  const uint64_t t = __umul64hi(d.magic, p);
+  return (t + ((p - t) >> d.sh1)) >> d.sh2;
+}
+inline DivW make_div_w(uint64_t w) {  // w >= 1
+  int l = 0;
+  while (l < 64 && (1ull << l) < w) ++l;
+  return DivW{(uint64_t)((((unsigned __int128)((l < 64 ? (1ull << l) : 0ull) - w)) << 64) / w) + 1, l < 1 ? l : 1, l > 1 ? l - 1 : 0};
+}
+
 // ---- host side: the launch sequence shared by substring.cu and concat_elements.cu ------------------------------------
 inline size_t align256(size_t b) { return (b + 255) & ~(size_t)255; }
 

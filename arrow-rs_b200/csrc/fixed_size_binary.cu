@@ -37,8 +37,7 @@ struct FsbArgs {
   uint64_t n_rows;        // values' rows
   uint64_t n_bytes;       // n_rows * w
   uint64_t w;             // >= 1
-  uint64_t magic;         // p / w = (t + ((p - t) >> sh1)) >> sh2, t = umulhi(magic, p)
-  int sh1, sh2;
+  DivW div;               // p / w (bytes_engine.cuh)
   const void *idx;        // ld_index kind `kind`
   int kind;
   const uint8_t *ivalid;  // validity of the indices when it holds a null, else NULL
@@ -51,11 +50,6 @@ struct FsbArgs {
 
 // Rows a 16-byte chunk can touch, and chunks per thread and round, by instantiation.
 template <int MAXR> struct FsbCfg { static constexpr int CHUNKS = MAXR <= 3 ? 4 : MAXR <= 5 ? 2 : 1; };
-
-__device__ __forceinline__ uint64_t div_w(const FsbArgs &a, uint64_t p) {
-  const uint64_t t = __umul64hi(a.magic, p);
-  return (t + ((p - t) >> a.sh1)) >> a.sh2;
-}
 
 // The source byte of row r's first byte, or ~0 when the row reads nothing (zeros); *err lowered on a panicking row.
 __device__ __forceinline__ uint64_t row_source(const FsbArgs &a, int64_t r, unsigned long long *err) {
@@ -97,7 +91,7 @@ __global__ void __launch_bounds__(FSB_THREADS) k_fsb_gather(const FsbArgs a) {
       const int64_t g = r0 + (int64_t)k * FSB_THREADS + threadIdx.x;
       const uint64_t p0 = (uint64_t)g * 16 - lead;  // may wrap below 0 for g == 0: only compared through pl
       const uint64_t pl = g == 0 ? 0 : p0, ph = (uint64_t)g * 16 + 16 - lead < total ? (uint64_t)g * 16 + 16 - lead : total;
-      row0[k] = g < n_chunks ? (int64_t)div_w(a, pl) : 0;
+      row0[k] = g < n_chunks ? (int64_t)div_by(a.div, pl) : 0;
 #pragma unroll
       for (int q = 0; q < MAXR; ++q) {
         const int64_t r = row0[k] + q;
@@ -140,15 +134,6 @@ __global__ void __launch_bounds__(FSB_THREADS) k_fsb_gather(const FsbArgs a) {
   if (err != ~0ull) atomicMin(a.res + RES_ERR2, err);
 }
 
-// div_w's constants for w (Granlund-Montgomery round-up multiplier: exact for every 64-bit p).
-void set_magic(FsbArgs *a, uint64_t w) {
-  int l = 0;
-  while (l < 64 && (1ull << l) < w) ++l;
-  a->magic = (uint64_t)((((unsigned __int128)((l < 64 ? (1ull << l) : 0ull) - w)) << 64) / w) + 1;
-  a->sh1 = l < 1 ? l : 1;
-  a->sh2 = l > 1 ? l - 1 : 0;
-}
-
 int max_rows(int64_t w) { return w >= 16 ? 2 : w >= 8 ? 3 : w >= 4 ? 5 : w >= 2 ? 9 : 17; }
 
 template <int MAXR>
@@ -169,7 +154,7 @@ acu_status launch_gather(acu_ctx *ctx, int cls, int64_t w, const acu_array *valu
   a.n_rows = (uint64_t)values->len;
   a.n_bytes = (uint64_t)values->len * (uint64_t)w;
   a.w = (uint64_t)w;
-  set_magic(&a, a.w);
+  a.div = make_div_w(a.w);
   a.idx = idx;
   a.kind = kind;
   a.ivalid = ivalid;

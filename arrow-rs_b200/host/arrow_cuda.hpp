@@ -2588,9 +2588,62 @@ inline Result<ArrayRef> nullif(const Array &left, const BooleanArray &right) {
   return detail::with_nulls(left, detail::out_nulls(o, nb));
 }
 
-// zip(mask, truthy, falsy) for primitive arrays / scalars of one type
+namespace detail {
+// zip of Utf8 (StringArray), Boolean and FixedSizeBinary operands: acu_zip_bytes / acu_zip_boolean / acu_zip_fixed_size_binary
+template <class A> struct zip_column : std::false_type {};
+template <> struct zip_column<StringArray> : std::true_type {};
+template <> struct zip_column<BooleanArray> : std::true_type {};
+template <> struct zip_column<FixedSizeBinaryArray> : std::true_type {};
+template <class D> using datum_array_t = std::decay_t<decltype(datum_array(std::declval<const D &>()))>;
+
+inline Result<ArrayRef> zip_column_impl(const BooleanArray &mask, const StringArray &t, bool ts, const StringArray &f, bool fs) {
+  const acu_bytes_array tb = kernels::cmp::bytes_view(t, ts), fb = kernels::cmp::bytes_view(f, fs);
+  const acu_array m = mask.view();
+  const int64_t n = mask.len();
+  Context &c = Context::get();
+  Buffer offs = Buffer::allocate((size_t)(n + 1) * 4), nb = Buffer::allocate(acu_bitmap_bytes(std::max<int64_t>(n, 1)));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  int64_t total = 0;
+  acu_status st = acu_zip_bytes(c.raw(), 4, &m, &tb, &fb, offs.data(), nullptr, 0, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  Buffer data = Buffer::allocate((size_t)std::max<int64_t>(total, 1));
+  st = acu_zip_bytes(c.raw(), 4, &m, &tb, &fb, offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, out_nulls(o, nb)));
+}
+
+inline Result<ArrayRef> zip_column_impl(const BooleanArray &mask, const BooleanArray &t, bool ts, const BooleanArray &f, bool fs) {
+  Context &c = Context::get();
+  const int64_t n = mask.len();
+  Buffer vb, nb;
+  acu_array m = mask.view(), tv = t.view(ts), fv = f.view(fs);
+  acu_array_out o = make_out(vb, nb, acu_bitmap_bytes(std::max<int64_t>(n, 1)), std::max<int64_t>(n, 1));
+  acu_status st = acu_zip_boolean(c.raw(), &m, &tv, &fv, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return ArrayRef(std::make_shared<BooleanArray>(vb, 0, o.len, out_nulls(o, nb)));
+}
+
+inline Result<ArrayRef> zip_column_impl(const BooleanArray &mask, const FixedSizeBinaryArray &t, bool ts, const FixedSizeBinaryArray &f,
+                                        bool fs) {
+  if (t.value_length() != f.value_length())  // FixedSizeBinary(4) vs (5): zip.rs:117-121
+    return ArrowError{ACU_ERR_INVALID_ARGUMENT, "Invalid argument error: arguments need to have the same data type"};
+  Context &c = Context::get();
+  const int64_t n = mask.len();
+  Buffer vb, nb;
+  acu_array m = mask.view(), tv = t.view(ts), fv = f.view(fs);
+  acu_array_out o = make_out(vb, nb, (size_t)std::max<int64_t>(n, 1) * t.value_length(), std::max<int64_t>(n, 1));
+  acu_status st = acu_zip_fixed_size_binary(c.raw(), t.value_length(), &m, &tv, &fv, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  return ArrayRef(std::make_shared<FixedSizeBinaryArray>(t.value_length(), vb, o.len, out_nulls(o, nb)));
+}
+}  // namespace detail
+
+// zip(mask, truthy, falsy) for arrays / scalars of one type: primitive, Utf8 (StringArray), Boolean or FixedSizeBinary
 template <class L, class R>
 Result<ArrayRef> zip(const BooleanArray &mask, const L &truthy, const R &falsy) {
+  if constexpr (detail::zip_column<detail::datum_array_t<L>>::value)
+    return detail::zip_column_impl(mask, datum_array(truthy), datum_is_scalar(truthy), datum_array(falsy), datum_is_scalar(falsy));
   const auto &t = datum_array(truthy);
   const auto &f = datum_array(falsy);
   if (t.data_type() != f.data_type())  // zip.rs:117-121
@@ -2603,6 +2656,46 @@ Result<ArrayRef> zip(const BooleanArray &mask, const L &truthy, const R &falsy) 
   acu_status st = acu_zip(c.raw(), dtype_width(t.data_type()), &m, &tv, &fv, &o);
   if (st != ACU_OK) return c.last_error(st);
   return detail::make_primitive(t.data_type(), vb, o.len, detail::out_nulls(o, nb));
+}
+
+// zip of Utf8View operands (StringViewArray, a data-buffer list of its own): the result references truthy's buffers,
+// falsy's, both (truthy's first) or none, as acu_zip_byte_view reports
+namespace detail {
+inline Result<StringViewArray> zip_views(const BooleanArray &mask, const StringViewArray &t, bool ts, const StringViewArray &f, bool fs) {
+  Context &c = Context::get();
+  const like::detail::ViewDesc tv(t, ts), fv(f, fs);
+  const acu_array m = mask.view();
+  const int64_t n = mask.len();
+  Buffer views = Buffer::allocate((size_t)std::max<int64_t>(n, 1) * 16), nb = Buffer::allocate(acu_bitmap_bytes(std::max<int64_t>(n, 1)));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(nb.data());
+  int32_t which = ACU_ZIP_BUFFERS_NONE;
+  const acu_status st = acu_zip_byte_view(c.raw(), &m, &tv.v, &fv.v, views.data(), &o, &which);
+  if (st != ACU_OK) return c.last_error(st);
+  std::vector<bool> valid((size_t)o.len, true);
+  if (o.has_validity) {
+    std::vector<uint8_t> bits(acu_bitmap_bytes(o.len));
+    nb.to_host(bits.data(), bits.size());
+    for (size_t i = 0; i < valid.size(); ++i) valid[i] = (bits[i >> 3] >> (i & 7)) & 1;
+  }
+  std::vector<ViewDataBuffer> bufs;
+  if (which == ACU_ZIP_BUFFERS_TRUTHY || which == ACU_ZIP_BUFFERS_BOTH) bufs = t.data_buffers();
+  if (which == ACU_ZIP_BUFFERS_FALSY || which == ACU_ZIP_BUFFERS_BOTH)
+    bufs.insert(bufs.end(), f.data_buffers().begin(), f.data_buffers().end());
+  return StringViewArray(views, 0, o.len, std::move(bufs), std::move(valid));
+}
+}  // namespace detail
+inline Result<StringViewArray> zip(const BooleanArray &mask, const StringViewArray &t, const StringViewArray &f) {
+  return detail::zip_views(mask, t, false, f, false);
+}
+inline Result<StringViewArray> zip(const BooleanArray &mask, const Scalar<StringViewArray> &t, const StringViewArray &f) {
+  return detail::zip_views(mask, t.array, true, f, false);
+}
+inline Result<StringViewArray> zip(const BooleanArray &mask, const StringViewArray &t, const Scalar<StringViewArray> &f) {
+  return detail::zip_views(mask, t, false, f.array, true);
+}
+inline Result<StringViewArray> zip(const BooleanArray &mask, const Scalar<StringViewArray> &t, const Scalar<StringViewArray> &f) {
+  return detail::zip_views(mask, t.array, true, f.array, true);
 }
 
 // ---- concat / concat_batches (arrow-select/src/concat.rs:495-640) -----------------------------------------------

@@ -310,6 +310,49 @@ acu_status acu_nullif(acu_ctx *ctx, const acu_array *left, const acu_array *righ
 acu_status acu_zip(acu_ctx *ctx, int32_t elem_bytes, const acu_array *mask /* boolean */, const acu_array *truthy,
                    const acu_array *falsy, acu_array_out *out);
 
+/* zip of Utf8 / Binary (offset_bytes 4), LargeUtf8 / LargeBinary (8), Utf8View / BinaryView, Boolean and
+ * FixedSizeBinary(byte_width) columns. Scalars, lengths, texts and mask nulls as acu_zip; masks, validity and operands may
+ * start at any bit offset or pointer alignment, with two exceptions: offsets are aligned to offset_bytes, as for the other
+ * byte calls, and views (truthy's, falsy's and out_views) to 16 bytes, the alignment of the u128 views buffer
+ * (ScalarBuffer<u128>); a misaligned views pointer => ACU_ERR_INVALID_ARGUMENT "views must be 16-byte aligned". The caller checks that
+ * both sides have one data type ("arguments need to have the same data type"). Three paths, as the reference:
+ *   - at least one side an array, and Boolean / FixedSizeBinary with two scalars (zip_impl over MutableArrayData,
+ *     zip.rs:148-210, FallbackImpl zip.rs:318-336): row i is row i of the chosen side (row 0 of a scalar), its bytes and bits
+ *     under nulls included; has_validity iff some input has a null and the result has one. Byte offsets are rebased on the
+ *     running total: an i32 end past i32::MAX is ACU_ERR_INVALID_ARGUMENT "offset overflow: data exceeds the capacity of the
+ *     offset type. ..." (try_extend_offsets) with detail.index = the first such row. A falsy view longer than 12 bytes gets
+ *     buffer_index += truthy->n_buffers (wrapping u32), nulls included, and *out_buffers = ACU_ZIP_BUFFERS_BOTH.
+ *   - two Utf8 / Binary scalars (BytesScalarImpl, zip.rs:439-660): both valid: no NullBuffer; one valid: its value where the
+ *     predicate (its negation for a valid falsy) holds, empty null rows elsewhere, has_validity = 1; both null: empty rows,
+ *     all null. An i32 overflow is the reference's panic, ACU_ERR_PANIC_OUT_OF_BOUNDS "offset overflow" (one value in every
+ *     row, or one valid scalar) or "overflow" (a mixed mask of two valid scalars), detail.index = -1.
+ *   - two view scalars (ByteViewScalarImpl, zip.rs:673-860): both valid: an all-true mask gives the truthy view and
+ *     buffers, an all-false one the falsy's, a mixed one the truthy buffers and, when falsy has any, falsy's after them, its
+ *     view's buffer index raised by truthy->n_buffers even when the view is inline; no NullBuffer. One valid: its view in
+ *     every row, its buffers, nulls = the predicate (negated for falsy), or zero views and no buffers when no row is
+ *     selected. Both null: zero views, no buffers, all null.
+ * acu_zip_bytes is two-phase like acu_filter_bytes: out_offsets (mask->len + 1 entries) always written, *out_data_len
+ * returned, bytes copied only when out_data != NULL; an offset overflow is reported by the sizing call already. acu_zip_byte_view
+ * writes mask->len views; of each side's data buffers it reads only n_buffers (neither `buffers` nor the bytes they point
+ * at, so a caller may pass buffers = NULL). Boolean results are a bitmap at bit offset 0; FixedSizeBinary
+ * results have mask->len x byte_width bytes at any alignment (byte_width < 0 => ACU_ERR_INVALID_ARGUMENT). Synchronous
+ * (refused inside a stream-ordered section); kernel time in ACU_K_BYTES (bytes, views) / ACU_K_ARITH (Boolean,
+ * FixedSizeBinary). */
+typedef enum acu_zip_buffers {  /* which data-buffer list a view zip result references */
+  ACU_ZIP_BUFFERS_NONE = 0, ACU_ZIP_BUFFERS_TRUTHY = 1, ACU_ZIP_BUFFERS_FALSY = 2, ACU_ZIP_BUFFERS_BOTH = 3
+} acu_zip_buffers;
+struct acu_bytes_array;
+struct acu_view_array;
+acu_status acu_zip_bytes(acu_ctx *ctx, int32_t offset_bytes, const acu_array *mask, const struct acu_bytes_array *truthy,
+                         const struct acu_bytes_array *falsy, void *out_offsets, uint8_t *out_data, int64_t out_data_capacity,
+                         int64_t *out_data_len, acu_array_out *out_nulls);
+acu_status acu_zip_byte_view(acu_ctx *ctx, const acu_array *mask, const struct acu_view_array *truthy,
+                             const struct acu_view_array *falsy, void *out_views, acu_array_out *out_nulls, int32_t *out_buffers);
+acu_status acu_zip_boolean(acu_ctx *ctx, const acu_array *mask, const acu_array *truthy, const acu_array *falsy,
+                           acu_array_out *out);
+acu_status acu_zip_fixed_size_binary(acu_ctx *ctx, int32_t byte_width, const acu_array *mask, const acu_array *truthy,
+                                     const acu_array *falsy, acu_array_out *out);
+
 /* ------------------------------------------------------------------------- */
 /* take — arrow-select/src/take.rs                                           */
 /* ------------------------------------------------------------------------- */

@@ -330,6 +330,15 @@ extern "C" {
     pub fn acu_nullif(ctx: *mut acu_ctx, left: *const acu_array, right: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_zip(ctx: *mut acu_ctx, elem_bytes: i32, mask: *const acu_array, truthy: *const acu_array, falsy: *const acu_array,
                    out: *mut acu_array_out) -> acu_status;
+    pub fn acu_zip_bytes(ctx: *mut acu_ctx, offset_bytes: i32, mask: *const acu_array, truthy: *const acu_bytes_array,
+                         falsy: *const acu_bytes_array, out_offsets: *mut c_void, out_data: *mut u8, out_data_capacity: i64,
+                         out_data_len: *mut i64, out_nulls: *mut acu_array_out) -> acu_status;
+    pub fn acu_zip_byte_view(ctx: *mut acu_ctx, mask: *const acu_array, truthy: *const acu_view_array, falsy: *const acu_view_array,
+                             out_views: *mut c_void, out_nulls: *mut acu_array_out, out_buffers: *mut i32) -> acu_status;
+    pub fn acu_zip_boolean(ctx: *mut acu_ctx, mask: *const acu_array, truthy: *const acu_array, falsy: *const acu_array,
+                           out: *mut acu_array_out) -> acu_status;
+    pub fn acu_zip_fixed_size_binary(ctx: *mut acu_ctx, byte_width: i32, mask: *const acu_array, truthy: *const acu_array,
+                                     falsy: *const acu_array, out: *mut acu_array_out) -> acu_status;
     pub fn acu_cmp_bytes(ctx: *mut acu_ctx, offset_bytes: i32, op: i32, l: *const acu_bytes_array, r: *const acu_bytes_array,
                          out: *mut acu_array_out) -> acu_status;
     pub fn acu_cmp_byte_view(ctx: *mut acu_ctx, op: i32, l: *const acu_view_array, r: *const acu_view_array, out: *mut acu_array_out) -> acu_status;

@@ -1429,17 +1429,108 @@ pub mod compute {
         Ok(make_array(unsafe { d.into_builder().nulls(nulls).build_unchecked() }))
     }
 
-    /// `arrow::compute::zip` (zip.rs:99) for primitive arrays / scalars.
+    /// `arrow::compute::zip` (zip.rs:99) for primitive, Boolean, Utf8 / Binary (and Large), Utf8View / BinaryView and
+    /// FixedSizeBinary arrays / scalars.
     pub fn zip(mask: &BooleanArray, truthy: &dyn Datum, falsy: &dyn Datum) -> Result<ArrayRef, ArrowError> {
         let (t, t_s) = truthy.get();
         let (f, f_s) = falsy.get();
         if t.data_type() != f.data_type() { return Err(ArrowError::InvalidArgumentError("arguments need to have the same data type".into())); }
+        match t.data_type() {
+            DataType::Boolean | DataType::FixedSizeBinary(_) | DataType::Utf8 | DataType::LargeUtf8 | DataType::Binary
+            | DataType::LargeBinary => return zip_column(mask, t, t_s, f, f_s),
+            DataType::Utf8View => return Ok(std::sync::Arc::new(zip_views(mask, arrow_array::cast::AsArray::as_string_view(t), t_s,
+                                                                   arrow_array::cast::AsArray::as_string_view(f), f_s)?)),
+            DataType::BinaryView => return Ok(std::sync::Arc::new(zip_views(mask, arrow_array::cast::AsArray::as_binary_view(t), t_s,
+                                                                     arrow_array::cast::AsArray::as_binary_view(f), f_s)?)),
+            _ => {}
+        }
         let w = t.data_type().primitive_width().ok_or_else(|| ArrowError::NotYetImplemented(format!("arrow-cuda zip: {}", t.data_type())))?;
         let ctx = Context::current()?;
         let (m, tv, fv) = (DeviceArray::upload(&ctx, mask, false)?, DeviceArray::upload(&ctx, t, t_s)?, DeviceArray::upload(&ctx, f, f_s)?);
         let mut out = ColumnOut::new(&ctx, t.data_type(), mask.len(), 0)?;
         ctx.check(unsafe { ffi::acu_zip(ctx.raw(), w as i32, m.view(), tv.view(), fv.view(), out.array_out()) })?;
         out.finish(t.data_type())
+    }
+
+    /// zip of Boolean, FixedSizeBinary and byte-array operands: acu_zip_boolean / acu_zip_fixed_size_binary / acu_zip_bytes
+    /// (two-phase: the offsets and the byte count, then the bytes).
+    fn zip_column(mask: &BooleanArray, t: &dyn Array, t_s: bool, f: &dyn Array, f_s: bool) -> Result<ArrayRef, ArrowError> {
+        let ctx = Context::current()?;
+        let dt = t.data_type();
+        let n = mask.len();
+        let (m, tv, fv) = (DeviceArray::upload(&ctx, mask, false)?, DeviceArray::upload(&ctx, t, t_s)?, DeviceArray::upload(&ctx, f, f_s)?);
+        match dt {
+            DataType::Boolean => {
+                let mut out = ColumnOut::new(&ctx, dt, n, 0)?;
+                ctx.check(unsafe { ffi::acu_zip_boolean(ctx.raw(), m.view(), tv.view(), fv.view(), out.array_out()) })?;
+                out.finish(dt)
+            }
+            DataType::FixedSizeBinary(w) => {
+                let mut out = ColumnOut::new(&ctx, dt, n, 0)?;
+                ctx.check(unsafe { ffi::acu_zip_fixed_size_binary(ctx.raw(), *w, m.view(), tv.view(), fv.view(), out.array_out()) })?;
+                out.finish(dt)
+            }
+            _ => {
+                let ob = if matches!(dt, DataType::LargeUtf8 | DataType::LargeBinary) { 8 } else { 4 };
+                let operand = |a: &DeviceArray| ffi::acu_bytes_array { offsets: a.view().values, data: a.column.data, nulls: *a.view() };
+                let (tb, fb) = (operand(&tv), operand(&fv));
+                let mut sizing = ColumnOut::new(&ctx, dt, n, 0)?;
+                let mut total = 0i64;
+                ctx.check(unsafe { ffi::acu_zip_bytes(ctx.raw(), ob, m.view(), &tb, &fb, sizing.out.array.values, std::ptr::null_mut(), 0,
+                                                      &mut total, &mut sizing.out.array) })?;
+                let mut out = ColumnOut::new(&ctx, dt, n, total as usize)?;
+                let (offs, data, cap) = (out.out.array.values, out.out.data, out.out.data_capacity);
+                ctx.check(unsafe { ffi::acu_zip_bytes(ctx.raw(), ob, m.view(), &tb, &fb, offs, data, cap, &mut out.out.data_len,
+                                                      &mut out.out.array) })?;
+                out.finish(dt)
+            }
+        }
+    }
+
+    /// zip of view operands: acu_zip_byte_view; the result references truthy's data buffers, falsy's, both or none.
+    fn zip_views<T: arrow_array::types::ByteViewType + ?Sized>(mask: &BooleanArray, t: &arrow_array::GenericByteViewArray<T>, t_s: bool,
+                                                               f: &arrow_array::GenericByteViewArray<T>, f_s: bool)
+                                                               -> Result<arrow_array::GenericByteViewArray<T>, ArrowError> {
+        let ctx = Context::current()?;
+        let n = mask.len();
+        let m = DeviceArray::upload(&ctx, mask, false)?;
+        // the views and the validity only: acu_zip_byte_view reads each side's buffer count, never the data buffers
+        fn operand<T: arrow_array::types::ByteViewType + ?Sized>(ctx: &Context, a: &arrow_array::GenericByteViewArray<T>, scalar: bool,
+                                                                 bufs: &mut Vec<DeviceBuffer>) -> Result<ffi::acu_view_array, ArrowError> {
+            let (validity, validity_offset, null_count) = match a.nulls() {
+                Some(n) => {
+                    let b = DeviceBuffer::from_host(ctx, n.buffer().as_slice())?;
+                    let p = b.as_ptr() as *const u8;
+                    bufs.push(b);
+                    (p, n.offset() as i64, n.null_count() as i64)
+                }
+                None => (std::ptr::null(), 0, 0),
+            };
+            let v = DeviceBuffer::from_host(ctx, a.views().inner().as_slice())?;
+            let views = v.as_ptr();
+            bufs.push(v);
+            let nulls = ffi::acu_array { values: std::ptr::null(), values_offset: 0, validity, validity_offset, len: a.len() as i64, null_count,
+                                         is_scalar: scalar as i32, reserved: 0 };
+            Ok(ffi::acu_view_array { views, buffers: std::ptr::null(), n_buffers: a.data_buffers().len() as i32, reserved: 0, nulls })
+        }
+        let mut bufs = Vec::new();
+        let tv = operand(&ctx, t, t_s, &mut bufs)?;
+        let fv = operand(&ctx, f, f_s, &mut bufs)?;
+        let views = DeviceBuffer::allocate(&ctx, n.max(1) * 16)?;
+        let validity = DeviceBuffer::allocate(&ctx, bitmap_bytes(n.max(1)))?;
+        let mut o = ffi::acu_array_out { values: std::ptr::null_mut(), validity: validity.as_ptr() as *mut u8, len: 0, null_count: 0,
+                                         has_validity: 0, reserved: 0 };
+        let mut which = 0i32;
+        ctx.check(unsafe { ffi::acu_zip_byte_view(ctx.raw(), m.view(), &tv, &fv, views.as_ptr(), &mut o, &mut which) })?;
+        let mut buffers: Vec<arrow_buffer::Buffer> = Vec::new();
+        if which == 1 || which == 3 { buffers.extend(t.data_buffers().iter().cloned()); }  // ACU_ZIP_BUFFERS_TRUTHY / _BOTH
+        if which == 2 || which == 3 { buffers.extend(f.data_buffers().iter().cloned()); }  // ACU_ZIP_BUFFERS_FALSY / _BOTH
+        let nulls = if o.has_validity == 0 { None } else {
+            let bits = arrow_buffer::BooleanBuffer::new(validity.to_host(bitmap_bytes(n))?, 0, n);
+            Some(unsafe { arrow_buffer::NullBuffer::new_unchecked(bits, o.null_count as usize) })
+        };
+        let v = arrow_buffer::ScalarBuffer::<u128>::new(views.to_host(n * 16)?, 0, n);
+        Ok(unsafe { GenericByteViewArray::<T>::new_unchecked(v, buffers, nulls) })
     }
 
     /// `arrow::compute::concat` (concat.rs:495).
