@@ -199,10 +199,6 @@ class Array {
   }
   bool is_null(int64_t i) const { return !valid_mask()[(size_t)i]; }
   bool is_valid(int64_t i) const { return !is_null(i); }
-  // MutableArrayData::freeze keeps a NullBuffer only if it has a null (arrow-data/src/transform/mod.rs:936)
-  void drop_empty_nulls() {
-    if (nulls_ && nulls_->null_count == 0) nulls_.reset();
-  }
  protected:
   virtual const void *values_ptr() const = 0;
   virtual int64_t values_bit_offset() const { return 0; }
@@ -816,8 +812,9 @@ inline acu_array_out make_out(Buffer &values, Buffer &validity, size_t value_byt
   o.validity = static_cast<uint8_t *>(validity.data());
   return o;
 }
-inline std::optional<NullBuffer> out_nulls(const acu_array_out &o, Buffer validity) {
-  if (!o.has_validity) return std::nullopt;
+// drop_empty_nulls: MutableArrayData::freeze keeps a NullBuffer only if it has a null (arrow-data/src/transform/mod.rs:936)
+inline std::optional<NullBuffer> out_nulls(const acu_array_out &o, Buffer validity, bool drop_empty_nulls = false) {
+  if (!o.has_validity || (drop_empty_nulls && o.null_count == 0)) return std::nullopt;
   return NullBuffer{std::move(validity), 0, o.len, o.null_count};
 }
 
@@ -920,6 +917,16 @@ class FilterPredicate {
  public:
   FilterPredicate() = default;
   explicit FilterPredicate(acu_filter_plan *p) : plan_(p, [](acu_filter_plan *q) { acu_filter_plan_destroy(Context::get().raw(), q); }) {}
+  // acu_filter_plan_create of a predicate (FilterBuilder::new(filter).build())
+  static Result<FilterPredicate> try_new(const BooleanArray &filter) {
+    Context &c = Context::get();
+    acu_array p = filter.view();
+    acu_filter_plan *plan = nullptr;
+    acu_status st = acu_filter_plan_create(c.raw(), &p, &plan);
+    if (st != ACU_OK) return c.last_error(st);
+    return FilterPredicate(plan);
+  }
+  acu_filter_plan *raw() const { return plan_.get(); }
   int64_t count() const { return acu_filter_plan_count(plan_.get()); }
   // IterationStrategy::Slices of FilterBuilder::optimize = SlicesIterator::new(&filter).collect() (filter.rs:44-77,285-298):
   // the runs of selected rows as [start, end), computed on the device
@@ -937,42 +944,8 @@ class FilterPredicate {
     for (int64_t k = 0; k < n; ++k) out[(size_t)k] = {(size_t)host[2 * k], (size_t)host[2 * k + 1]};
     return out;
   }
-  Result<ArrayRef> filter(const Array &values) const {
-    Context &c = Context::get();
-    const int64_t n = count();
-    Buffer vb, nb;
-    acu_array v = values.view();
-    acu_status st;
-    if (values.data_type() == DataType::Boolean) {
-      acu_array_out o = detail::make_out(vb, nb, acu_bitmap_bytes(n), n);
-      if ((st = acu_filter_boolean(c.raw(), plan_.get(), &v, &o)) != ACU_OK) return c.last_error(st);
-      return ArrayRef(std::make_shared<BooleanArray>(vb, 0, o.len, detail::out_nulls(o, nb)));
-    }
-    if (values.data_type() == DataType::Utf8) {
-      const auto &s = static_cast<const StringArray &>(values);
-      Buffer offs = Buffer::allocate((size_t)(n + 1) * 4), dummy;
-      acu_array_out o{};
-      nb = Buffer::allocate(acu_bitmap_bytes(n));
-      o.validity = static_cast<uint8_t *>(nb.data());
-      int64_t total = 0;
-      if ((st = acu_filter_bytes(c.raw(), plan_.get(), 4, s.offsets().data(), static_cast<const uint8_t *>(s.value_data().data()), &v,
-                                 offs.data(), nullptr, 0, &total, &o)) != ACU_OK) return c.last_error(st);
-      Buffer data = Buffer::allocate((size_t)total);
-      if ((st = acu_filter_bytes(c.raw(), plan_.get(), 4, s.offsets().data(), static_cast<const uint8_t *>(s.value_data().data()), &v,
-                                 offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o)) != ACU_OK) return c.last_error(st);
-      return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, detail::out_nulls(o, nb)));
-    }
-    if (values.data_type() == DataType::FixedSizeBinary) {  // filter_fixed_size_binary (filter.rs:946-996)
-      const int32_t w = static_cast<const FixedSizeBinaryArray &>(values).value_length();
-      acu_array_out o = detail::make_out(vb, nb, (size_t)n * w, n);
-      if ((st = acu_filter_fixed_size_binary(c.raw(), plan_.get(), w, &v, &o)) != ACU_OK) return c.last_error(st);
-      return ArrayRef(std::make_shared<FixedSizeBinaryArray>(w, vb, o.len, detail::out_nulls(o, nb)));
-    }
-    const int w = dtype_width(values.data_type());
-    acu_array_out o = detail::make_out(vb, nb, (size_t)n * w, n);
-    if ((st = acu_filter_primitive(c.raw(), plan_.get(), w, &v, &o)) != ACU_OK) return c.last_error(st);
-    return detail::make_primitive(values.data_type(), vb, o.len, detail::out_nulls(o, nb));
-  }
+  // FilterPredicate::filter (filter.rs:480-483): any array, at any nesting
+  Result<ArrayRef> filter(const Array &values) const;
   // FilterPredicate::filter_record_batch (filter.rs:459-478): one plan, every column, ONE synchronisation
   // (acu_filter_record_batch queues the kernels of all columns back to back).
   Result<RecordBatch> filter_record_batch(const RecordBatch &batch) const {
@@ -1003,11 +976,9 @@ class FilterPredicate {
 class FilterBuilder {  // filter.rs:254-324
  public:
   explicit FilterBuilder(const BooleanArray &filter) {
-    acu_array p = filter.view();
-    acu_filter_plan *plan = nullptr;
-    acu_status st = acu_filter_plan_create(Context::get().raw(), &p, &plan);
-    if (st != ACU_OK) throw std::runtime_error(Context::get().last_error(st).message);
-    pred_ = FilterPredicate(plan);
+    auto p = FilterPredicate::try_new(filter);
+    if (p.is_err()) throw std::runtime_error(p.unwrap_err().message);
+    pred_ = p.unwrap();
   }
   FilterBuilder &optimize() { return *this; }  // the device plan is always materialised
   FilterPredicate build() { return pred_; }
@@ -1030,65 +1001,52 @@ class FilterBuilder {  // filter.rs:254-324
   FilterPredicate pred_;
 };
 
-inline Result<ArrayRef> filter(const Array &values, const BooleanArray &predicate) {
-  return FilterBuilder(predicate).build().filter(values);
-}
-inline Result<RecordBatch> filter_record_batch(const RecordBatch &batch, const BooleanArray &predicate) {
-  return FilterBuilder(predicate).optimize().build().filter_record_batch(batch);
-}
-
 // ---- take (arrow-select/src/take.rs) ----------------------------------------------------
 struct TakeOptions { bool check_bounds = false; };  // take.rs:388-394
 
-inline Result<ArrayRef> take(const Array &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+// ---- filter / take of every array type (filter.rs:174-199, take.rs:89-105) ------------------------------------------
+// filter_any / take_any have one arm per DataType. A nested array makes one C call per level, which returns the plan or
+// row map of the level below, and each child goes through the arm of its own type:
+// - List / LargeList / FixedSizeList (filter.rs:535-625, take.rs:646-795): acu_filter_list / acu_take_list. A List's child
+//   is extended (MutableArrayData: a Utf8 child keeps the bytes under its null rows, acu_take_bytes_extend); a
+//   FixedSizeList's child is taken. Not reproduced here: when a List's i32 offsets and its child's both overflow, this
+//   mirror reports the List's unwrap panic (the Python layer reports the child's error first, as the reference does).
+// - Struct, sparse Union and dense Union (filter.rs:597-622, :1010-1054, take.rs:270-298, :334-382): a struct's columns,
+//   then acu_filter_nulls / acu_take_nulls for its NullBuffer. acu_filter_union / acu_take_union give a union's type ids
+//   and, for a dense union, its new offsets and a child row map grouped by field; child f is then taken (take) or extended
+//   (filter, the child step of a list take) with its slice of the map.
+// - RunEndEncoded (filter_run_end_array filter.rs:628-677, take_run take.rs:948-995), at the top level only:
+//   acu_filter_run_end / acu_take_run_end write the new run ends and return the values child's plan / value indices.
+//   Values: primitive, Boolean and Utf8 (and lists, filter only). As in the Python layer, a RunEndEncoded array below
+//   another level is refused (MutableArrayData does not extend one).
+namespace detail {
+// take.rs:103: the indices must be integers
+inline std::optional<ArrowError> index_type_error(DataType it) {
+  if ((int)it <= (int)DataType::UInt64) return std::nullopt;
+  return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + dtype_display(it)};
+}
+// an output of `rows` rows that receives a validity bitmap only
+inline acu_array_out validity_out(Buffer &validity, int64_t rows) {
+  validity = Buffer::allocate(acu_bitmap_bytes(rows));
+  acu_array_out o{};
+  o.validity = static_cast<uint8_t *>(validity.data());
+  return o;
+}
+// A Utf8 output of `rows` rows in two calls of `call(offsets, data, capacity, &total, &out)`: the first (no data buffer)
+// sizes the value bytes, the second writes them.
+template <class F>
+Result<ArrayRef> bytes_out(int64_t rows, bool drop_empty_nulls, F call) {
   Context &c = Context::get();
-  const DataType it = indices.data_type();
-  if ((int)it > (int)DataType::UInt64)  // take.rs:103
-    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + detail::dtype_display(it)};
-  const int cb = options && options->check_bounds ? 1 : 0;
-  const int64_t m = indices.len();
-  acu_array v = values.view(), ix = indices.view();
-  Buffer vb, nb;
-  acu_status st;
-  if (values.data_type() == DataType::Boolean) {
-    acu_array_out o = detail::make_out(vb, nb, acu_bitmap_bytes(m), m);
-    if ((st = acu_take_boolean(c.raw(), &v, &ix, (acu_dtype)dtype_code(it), cb, &o)) != ACU_OK) return c.last_error(st);
-    return ArrayRef(std::make_shared<BooleanArray>(vb, 0, o.len, detail::out_nulls(o, nb)));
-  }
-  if (values.data_type() == DataType::Utf8) {
-    const auto &s = static_cast<const StringArray &>(values);
-    Buffer offs = Buffer::allocate((size_t)(m + 1) * 4);
-    nb = Buffer::allocate(acu_bitmap_bytes(m));
-    acu_array_out o{};
-    o.validity = static_cast<uint8_t *>(nb.data());
-    int64_t total = 0;
-    if ((st = acu_take_bytes(c.raw(), 4, s.offsets().data(), static_cast<const uint8_t *>(s.value_data().data()), &v, &ix,
-                             (acu_dtype)dtype_code(it), cb, offs.data(), nullptr, 0, &total, &o)) != ACU_OK) return c.last_error(st);
-    Buffer data = Buffer::allocate((size_t)total);
-    if ((st = acu_take_bytes(c.raw(), 4, s.offsets().data(), static_cast<const uint8_t *>(s.value_data().data()), &v, &ix,
-                             (acu_dtype)dtype_code(it), cb, offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o)) != ACU_OK)
-      return c.last_error(st);
-    return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, detail::out_nulls(o, nb)));
-  }
-  if (values.data_type() == DataType::FixedSizeBinary) {  // take_fixed_size_binary (take.rs:802-862)
-    const int32_t w = static_cast<const FixedSizeBinaryArray &>(values).value_length();
-    acu_array_out o = detail::make_out(vb, nb, (size_t)m * w, m);
-    if ((st = acu_take_fixed_size_binary(c.raw(), w, &v, &ix, (acu_dtype)dtype_code(it), cb, &o)) != ACU_OK) return c.last_error(st);
-    return ArrayRef(std::make_shared<FixedSizeBinaryArray>(w, vb, o.len, detail::out_nulls(o, nb)));
-  }
-  const int w = dtype_width(values.data_type());
-  acu_array_out o = detail::make_out(vb, nb, (size_t)m * w, m);
-  if ((st = acu_take_primitive(c.raw(), w, &v, &ix, (acu_dtype)dtype_code(it), cb, &o)) != ACU_OK) return c.last_error(st);
-  return detail::make_primitive(values.data_type(), vb, o.len, detail::out_nulls(o, nb));
+  Buffer offs = Buffer::allocate((size_t)(rows + 1) * 4), nb;
+  acu_array_out o = validity_out(nb, rows);
+  int64_t total = 0;
+  acu_status st = call(offs.data(), nullptr, 0, &total, &o);
+  if (st != ACU_OK) return c.last_error(st);
+  Buffer data = Buffer::allocate((size_t)total);
+  if ((st = call(offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o)) != ACU_OK) return c.last_error(st);
+  return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, out_nulls(o, nb, drop_empty_nulls)));
 }
 
-// ---- filter / take of List, LargeList, FixedSizeList (filter.rs:535-625, take.rs:646-795) ---------------------------------
-// One C call per level: acu_filter_list / acu_take_list return the child's plan / row map, and the child goes through the
-// entry point of its own type (the list calls again for a nested list). A List's child is extended (MutableArrayData: a
-// Utf8 child keeps the bytes under its null rows, acu_take_bytes_extend); a FixedSizeList's child is taken.
-// Not reproduced here: when a List's i32 offsets and its child's both overflow, this mirror reports the List's unwrap panic
-// (the Python layer reports the child's error first, as the reference does).
-namespace detail {
 inline acu_list_array list_view(const Array &a) {
   acu_list_array l{};
   l.nulls = a.view();
@@ -1111,7 +1069,6 @@ inline acu_list_array list_view(const Array &a) {
   }
   return l;
 }
-inline bool is_list(DataType t) { return t == DataType::List || t == DataType::LargeList || t == DataType::FixedSizeList; }
 inline const ArrayRef &list_values(const Array &a) {
   if (a.data_type() == DataType::FixedSizeList) return static_cast<const FixedSizeListArray &>(a).values();
   if (a.data_type() == DataType::List) return static_cast<const ListArray &>(a).values();
@@ -1124,151 +1081,10 @@ inline ArrayRef list_like(const Array &a, Buffer offsets, ArrayRef child, int64_
   return std::make_shared<LargeListArray>(std::move(offsets), std::move(child), len, std::move(nulls));
 }
 
-// child_step: `values` is a child of a list whose top level was filtered with a plan other than All (nullopt at the top).
-// The reference builds those levels with MutableArrayData (filter.rs:600), which drops a NullBuffer without nulls even
-// where the level's own plan selects every row; under a top-level All it slices every level as it is.
-inline Result<ArrayRef> filter_nested(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan, std::optional<bool> child_step);
-inline Result<ArrayRef> take_nested(const Array &values, const Array &indices, int cb, bool keep);
-inline bool is_nested(DataType t) { return t == DataType::Struct || t == DataType::Union; }
-
-// MutableArrayData keeps every extended row of a FixedSizeBinary(0) child (try_new's length rule is the top level's)
-inline ArrayRef keep_width0_rows(ArrayRef a, int64_t rows) {
-  if (a->data_type() != DataType::FixedSizeBinary) return a;
-  const auto &f = static_cast<const FixedSizeBinaryArray &>(*a);
-  if (f.value_length() != 0 || f.len() == rows) return a;
-  return std::make_shared<FixedSizeBinaryArray>(0, f.values(), rows, f.nulls());
-}
-
-inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan,
-                                   std::optional<bool> child_step = std::nullopt) {
-  if (is_nested(values.data_type())) return filter_nested(values, pred, plan, child_step);
-  if (!is_list(values.data_type())) {
-    auto r = pred.filter(values);
-    if (r.is_err() || !child_step.value_or(false)) return r;
-    ArrayRef a = r.unwrap();
-    a->drop_empty_nulls();
-    return keep_width0_rows(a, pred.count());
-  }
-  Context &c = Context::get();
-  const int64_t n = pred.count();
-  const acu_list_array l = list_view(values);
-  const size_t ob = l.kind == ACU_LIST ? 4 : 8;
-  Buffer offs = Buffer::allocate((size_t)(n + 1) * ob), nb = Buffer::allocate(acu_bitmap_bytes(n));
-  acu_array_out o{};
-  o.validity = static_cast<uint8_t *>(nb.data());
-  acu_filter_plan *child_plan = nullptr;
-  acu_status st = acu_filter_list(c.raw(), plan, &l, offs.data(), &o, &child_plan);
-  if (st != ACU_OK) return c.last_error(st);
-  FilterPredicate cp(child_plan);
-  const bool step = child_step ? *child_step : n != acu_filter_plan_len(plan);
-  auto child = filter_any(*list_values(values), cp, child_plan, step);
-  if (child.is_err()) return child.unwrap_err();
-  if (child_step.value_or(false) && o.has_validity && o.null_count == 0) o.has_validity = 0;
-  return list_like(values, offs, child.unwrap(), o.len, out_nulls(o, nb));
-}
-
-inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool extend);
-
-inline Result<ArrayRef> take_list_level(const Array &values, const Array &indices, int cb, bool keep) {
-  Context &c = Context::get();
-  const int64_t m = indices.len();
-  const acu_list_array l = list_view(values);
-  const bool fixed = l.kind == ACU_FIXED_SIZE_LIST;
-  const size_t ob = l.kind == ACU_LIST ? 4 : 8;
-  const acu_dtype cdt = fixed || l.child_len <= (int64_t)UINT32_MAX ? ACU_U32 : ACU_U64;
-  const acu_array ix = indices.view();
-  const acu_dtype it = (acu_dtype)dtype_code(indices.data_type());
-  Buffer offs = Buffer::allocate((size_t)(m + 1) * ob), nb = Buffer::allocate(acu_bitmap_bytes(m));
-  acu_array_out o{}, cn{};
-  o.validity = static_cast<uint8_t *>(nb.data());
-  int64_t rows = 0;
-  acu_status st = acu_take_list(c.raw(), &l, &ix, it, cb, keep ? 1 : 0, offs.data(), &o, cdt, nullptr, 0, &rows, &cn);
-  if (st != ACU_OK) return c.last_error(st);
-  Buffer map = Buffer::allocate((size_t)rows * (cdt == ACU_U32 ? 4 : 8)), cnb = Buffer::allocate(acu_bitmap_bytes(rows));
-  cn.validity = static_cast<uint8_t *>(cnb.data());
-  st = acu_take_list(c.raw(), &l, &ix, it, cb, keep ? 1 : 0, offs.data(), &o, cdt, map.data(), rows, &rows, &cn);
-  std::optional<ArrowError> deferred;  // take_fixed_size_list: the child is taken before the list's validity is read
-  if (st != ACU_OK) {
-    if (!fixed || st != ACU_ERR_PANIC_OUT_OF_BOUNDS) return c.last_error(st);
-    deferred = c.last_error(st);
-  }
-  std::optional<NullBuffer> map_nulls;
-  if (cn.has_validity) map_nulls = NullBuffer{cnb, 0, rows, cn.null_count};
-  ArrayRef rm = cdt == ACU_U32 ? ArrayRef(std::make_shared<PrimitiveArray<uint32_t>>(map, rows, map_nulls))
-                               : ArrayRef(std::make_shared<PrimitiveArray<uint64_t>>(map, rows, map_nulls));
-  auto child = take_any(*list_values(values), *rm, 0, keep || !fixed);
-  if (child.is_err()) return child.unwrap_err();
-  if (deferred) return *deferred;
-  return list_like(values, offs, child.unwrap(), o.len, out_nulls(o, nb));
-}
-
-inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool extend) {
-  if (is_list(values.data_type())) return take_list_level(values, indices, cb, extend);
-  if (is_nested(values.data_type())) return take_nested(values, indices, cb, extend);
-  if (values.data_type() == DataType::FixedSizeBinary && extend) {
-    auto r = take(values, indices, TakeOptions{cb != 0});
-    if (r.is_err()) return r;
-    return keep_width0_rows(r.unwrap(), indices.len());
-  }
-  if (!extend || values.data_type() != DataType::Utf8) return take(values, indices, TakeOptions{cb != 0});
-  Context &c = Context::get();
-  const auto &s = static_cast<const StringArray &>(values);
-  const int64_t m = indices.len();
-  const acu_array v = values.view(), ix = indices.view();
-  const acu_dtype it = (acu_dtype)dtype_code(indices.data_type());
-  Buffer offs = Buffer::allocate((size_t)(m + 1) * 4), nb = Buffer::allocate(acu_bitmap_bytes(m));
-  acu_array_out o{};
-  o.validity = static_cast<uint8_t *>(nb.data());
-  int64_t total = 0;
-  const uint8_t *src = static_cast<const uint8_t *>(s.value_data().data());
-  acu_status st = acu_take_bytes_extend(c.raw(), 4, s.offsets().data(), src, &v, &ix, it, offs.data(), nullptr, 0, &total, &o);
-  if (st != ACU_OK) return c.last_error(st);
-  Buffer data = Buffer::allocate((size_t)total);
-  st = acu_take_bytes_extend(c.raw(), 4, s.offsets().data(), src, &v, &ix, it, offs.data(), static_cast<uint8_t *>(data.data()), total, &total, &o);
-  if (st != ACU_OK) return c.last_error(st);
-  return ArrayRef(std::make_shared<StringArray>(offs, data, o.len, out_nulls(o, nb)));
-}
-
-template <class L>
-Result<ArrayRef> filter_list(const L &values, const BooleanArray &predicate) {
-  acu_array p = predicate.view();
-  acu_filter_plan *plan = nullptr;
-  Context &c = Context::get();
-  acu_status st = acu_filter_plan_create(c.raw(), &p, &plan);
-  if (st != ACU_OK) return c.last_error(st);
-  FilterPredicate pred(plan);
-  return filter_any(values, pred, plan);
-}
-template <class L>
-Result<ArrayRef> take_list(const L &values, const Array &indices, std::optional<TakeOptions> options) {
-  const DataType it = indices.data_type();
-  if ((int)it > (int)DataType::UInt64)  // take.rs:103
-    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + dtype_display(it)};
-  return take_list_level(values, indices, options && options->check_bounds ? 1 : 0, false);
-}
-}  // namespace detail
-
-inline Result<ArrayRef> filter(const ListArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
-inline Result<ArrayRef> filter(const LargeListArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
-inline Result<ArrayRef> filter(const FixedSizeListArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
-inline Result<ArrayRef> take(const ListArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
-  return detail::take_list(values, indices, options);
-}
-inline Result<ArrayRef> take(const LargeListArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
-  return detail::take_list(values, indices, options);
-}
-inline Result<ArrayRef> take(const FixedSizeListArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
-  return detail::take_list(values, indices, options);
-}
-
-// ---- filter / take of RunEndEncoded (filter_run_end_array filter.rs:628-677, take_run take.rs:948-995) -------------------
-// acu_filter_run_end / acu_take_run_end write the new run ends and return the values child's plan / value indices; the
-// values child goes through the entry point of its own type. Values: primitive, Boolean and Utf8 (and lists, filter only).
-namespace detail {
 template <class T> ArrayRef slice_prim(const Array &a, int64_t off, int64_t len) {
   return std::make_shared<PrimitiveArray<T>>(static_cast<const PrimitiveArray<T> &>(a).slice(off, len));
 }
-// Array::slice of the value types above
+// Array::slice of the RunArray value types
 inline ArrayRef slice_any(const Array &a, int64_t off, int64_t len) {
   std::optional<NullBuffer> nulls = a.nulls();
   if (nulls) { nulls->offset += off; nulls->len = len; nulls->null_count = -1; }
@@ -1333,87 +1149,14 @@ inline ArrayRef empty_like(const Array &a) {
     default: throw std::runtime_error(std::string("RunArray values of type ") + dtype_display(a.data_type()) + " are not supported by this mirror");
   }
 }
-}  // namespace detail
-
-template <class R>
-Result<ArrayRef> filter(const RunArray<R> &values, const BooleanArray &predicate) {
-  Context &c = Context::get();
-  acu_array p = predicate.view();
-  acu_filter_plan *plan = nullptr;
-  acu_status st = acu_filter_plan_create(c.raw(), &p, &plan);
-  if (st != ACU_OK) return c.last_error(st);
-  FilterPredicate pred(plan);
-  const acu_run_array r = values.run_view();
-  const int64_t count = pred.count();
-  Buffer ends = Buffer::allocate((size_t)std::max<int64_t>(std::min(count, values.num_runs()), 1) * sizeof(R));
-  int64_t runs = 0, start = 0;
-  acu_filter_plan *vplan = nullptr;
-  if ((st = acu_filter_run_end(c.raw(), plan, &r, ends.data(), &runs, &start, &vplan)) != ACU_OK) return c.last_error(st);
-  if (!vplan) {
-    if (acu_filter_plan_strategy(plan) == ACU_FILTER_ALL) return ArrayRef(std::make_shared<RunArray<R>>(values.slice(0, count)));
-    return ArrayRef(std::make_shared<RunArray<R>>(Buffer::allocate(0), 0, detail::empty_like(*values.values()), 0, 0));
-  }
-  FilterPredicate vpred(vplan);
-  auto v = detail::filter_any(*detail::slice_any(*values.values(), start, acu_filter_plan_len(vplan)), vpred, vplan);
-  if (v.is_err()) return v.unwrap_err();
-  std::vector<R> host((size_t)runs);
-  ends.to_host(host.data(), host.size() * sizeof(R));
-  return ArrayRef(std::make_shared<RunArray<R>>(ends, runs, v.unwrap(), 0, (int64_t)host.back()));  // the last new run end
+// f(run) with the RunArray<R> behind a RunEndEncoded array
+template <class F>
+Result<ArrayRef> with_run_array(const Array &a, F f) {
+  if (const auto *r = dynamic_cast<const RunArray<int16_t> *>(&a)) return f(*r);
+  if (const auto *r = dynamic_cast<const RunArray<int32_t> *>(&a)) return f(*r);
+  return f(dynamic_cast<const RunArray<int64_t> &>(a));
 }
 
-template <class R>
-Result<ArrayRef> take(const RunArray<R> &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
-  Context &c = Context::get();
-  const DataType it = indices.data_type();
-  if ((int)it > (int)DataType::UInt64)  // take.rs:103
-    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + detail::dtype_display(it)};
-  const Array &vals = *values.values();
-  acu_run_values rv{};
-  switch (vals.data_type()) {
-    case DataType::Boolean: rv.kind = ACU_RUN_VALUES_BOOLEAN; rv.array = vals.view(); break;
-    case DataType::Utf8: {
-      const auto &s = static_cast<const StringArray &>(vals);
-      rv.kind = ACU_RUN_VALUES_BYTES;
-      rv.width = 4;
-      rv.bytes.offsets = s.offsets().data();
-      rv.bytes.data = static_cast<const uint8_t *>(s.value_data().data());
-      rv.bytes.nulls = vals.view();
-      break;
-    }
-    case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: case DataType::Struct: case DataType::Union:
-    case DataType::FixedSizeBinary:  // the run merge would need a value_length-byte comparator
-      rv.kind = ACU_RUN_VALUES_NESTED;
-      break;
-    default:
-      if (dtype_width(vals.data_type()) == 0)
-        throw std::runtime_error(std::string("RunArray values of type ") + detail::dtype_display(vals.data_type()) + " are not supported by this mirror");
-      rv.kind = ACU_RUN_VALUES_FIXED;
-      rv.width = dtype_width(vals.data_type());
-      rv.array = vals.view();
-  }
-  const int64_t m = indices.len();
-  const bool wide = it == DataType::Int64 || it == DataType::UInt64;  // ToIndices: UInt64 value indices
-  const acu_run_array r = values.run_view();
-  const acu_array ix = indices.view();
-  Buffer ends = Buffer::allocate((size_t)std::max<int64_t>(m, 1) * sizeof(R)), vi = Buffer::allocate((size_t)std::max<int64_t>(m, 1) * (wide ? 8 : 4));
-  int64_t runs = 0;
-  acu_status st = acu_take_run_end(c.raw(), &r, &rv, &ix, (acu_dtype)dtype_code(it), options && options->check_bounds ? 1 : 0, ends.data(),
-                                   vi.data(), &runs);
-  if (st != ACU_OK) return c.last_error(st);
-  if (m == 0) return ArrayRef(std::make_shared<RunArray<R>>(Buffer::allocate(0), 0, detail::empty_like(vals), 0, 0));
-  ArrayRef vix = wide ? ArrayRef(std::make_shared<PrimitiveArray<uint64_t>>(vi, runs, std::nullopt))
-                      : ArrayRef(std::make_shared<PrimitiveArray<uint32_t>>(vi, runs, std::nullopt));
-  auto v = take(vals, *vix);
-  if (v.is_err()) return v.unwrap_err();
-  return ArrayRef(std::make_shared<RunArray<R>>(ends, runs, v.unwrap(), 0, m));
-}
-
-// ---- filter / take of Struct, sparse Union and dense Union (filter.rs:597-622, :1010-1054, take.rs:270-298, :334-382) ------
-// A struct's columns go through the entry points of their types and acu_filter_nulls / acu_take_nulls give its NullBuffer.
-// acu_filter_union / acu_take_union give a union's type ids and, for a dense union, its new offsets and a child row map
-// grouped by field; child f is then taken (take) or extended (filter, the child step of a list take) with its slice of the
-// map. Both nest under lists, structs and unions through filter_any / take_any.
-namespace detail {
 inline acu_array nulls_view(const Array &a) {
   acu_array v = a.view();
   v.values = nullptr;
@@ -1437,134 +1180,311 @@ inline ArrayRef union_head(const UnionArray &u, int64_t len) {
   return std::make_shared<UnionArray>(u.field_type_ids(), Buffer::from_host(t.data(), (size_t)len), std::move(ob), std::move(children), len);
 }
 
-inline Result<ArrayRef> filter_nested(const Array &values, const FilterPredicate &pred, acu_filter_plan *plan, std::optional<bool> child_step) {
+// keep: `values` is the child step of a List take (MutableArrayData::extend: every row keeps its range or bytes).
+inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool keep);
+
+// child_step: `values` is a child of a list whose top level was filtered with a plan other than All (nullopt at the top).
+// The reference builds those levels with MutableArrayData (filter.rs:600), which drops a NullBuffer without nulls even
+// where the level's own plan selects every row; under a top-level All it slices every level as it is.
+inline Result<ArrayRef> filter_any(const Array &values, const FilterPredicate &pred, std::optional<bool> child_step = std::nullopt) {
   Context &c = Context::get();
+  acu_filter_plan *plan = pred.raw();
   const int64_t n = pred.count();
+  const bool step = child_step.value_or(false);
+  const acu_array v = values.view();
+  Buffer vb, nb;
   acu_status st;
-  if (values.data_type() == DataType::Struct) {  // filter_struct: every column, then filter_nulls
-    const auto &sa = static_cast<const StructArray &>(values);
-    std::vector<ArrayRef> cols;
-    for (const auto &col : sa.columns()) {
-      auto r = filter_any(*col, pred, plan, child_step);
-      if (r.is_err()) return r.unwrap_err();
-      cols.push_back(r.unwrap());
+  switch (values.data_type()) {
+    case DataType::Boolean: {
+      acu_array_out o = make_out(vb, nb, acu_bitmap_bytes(n), n);
+      if ((st = acu_filter_boolean(c.raw(), plan, &v, &o)) != ACU_OK) return c.last_error(st);
+      return ArrayRef(std::make_shared<BooleanArray>(vb, 0, o.len, out_nulls(o, nb, step)));
     }
-    const acu_array nv = nulls_view(values);
-    Buffer nb = Buffer::allocate(acu_bitmap_bytes(n));
-    acu_array_out o{};
-    o.validity = static_cast<uint8_t *>(nb.data());
-    if ((st = acu_filter_nulls(c.raw(), plan, &nv, &o)) != ACU_OK) return c.last_error(st);
-    if (child_step.value_or(false) && o.has_validity && o.null_count == 0) o.has_validity = 0;
-    return ArrayRef(std::make_shared<StructArray>(std::move(cols), n, out_nulls(o, nb)));
-  }
-  const auto &u = static_cast<const UnionArray &>(values);
-  const int32_t strategy = acu_filter_plan_strategy(plan);
-  if (u.is_dense() && child_step.value_or(false) && strategy == ACU_FILTER_ALL) {
-    // a list's child step extends every row even when its plan selects them all: the rows of a take of 0 .. n
-    std::vector<uint64_t> ids((size_t)n);
-    for (int64_t i = 0; i < n; ++i) ids[(size_t)i] = (uint64_t)i;
-    return take_nested(values, PrimitiveArray<uint64_t>::from(ids), 0, true);
-  }
-  const acu_union_array uv = u.union_view();
-  const size_t nf = u.field_type_ids().size();
-  Buffer tids = Buffer::allocate((size_t)n), offs = Buffer::allocate((size_t)n * 4), map = Buffer::allocate((size_t)n * 4);
-  std::vector<int64_t> starts(nf + 1, 0);
-  if ((st = acu_filter_union(c.raw(), plan, &uv, static_cast<int8_t *>(tids.data()), static_cast<int32_t *>(offs.data()),
-                             static_cast<int32_t *>(map.data()), starts.data())) != ACU_OK)
-    return c.last_error(st);
-  const bool whole = strategy == ACU_FILTER_NONE || strategy == ACU_FILTER_ALL;
-  std::vector<ArrayRef> children;
-  if (u.is_dense()) {
-    if (strategy == ACU_FILTER_ALL) return union_head(u, n);  // values.slice(0, count)
-    for (size_t f = 0; f < nf; ++f) {  // build_extend_dense: each child extended row by row
-      auto r = take_any(*u.children()[f], *i32_slice(map, starts[f], starts[f + 1] - starts[f]), 0, true);
-      if (r.is_err()) return r.unwrap_err();
-      children.push_back(r.unwrap());
+    case DataType::Utf8: {
+      const auto &s = static_cast<const StringArray &>(values);
+      return bytes_out(n, step, [&](void *offs, uint8_t *data, int64_t cap, int64_t *total, acu_array_out *o) {
+        return acu_filter_bytes(c.raw(), plan, 4, s.offsets().data(), static_cast<const uint8_t *>(s.value_data().data()), &v, offs, data, cap,
+                                total, o);
+      });
     }
-    return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, offs, std::move(children), n));
+    case DataType::FixedSizeBinary: {  // filter_fixed_size_binary (filter.rs:946-996)
+      const int32_t w = static_cast<const FixedSizeBinaryArray &>(values).value_length();
+      acu_array_out o = make_out(vb, nb, (size_t)n * w, n);
+      if ((st = acu_filter_fixed_size_binary(c.raw(), plan, w, &v, &o)) != ACU_OK) return c.last_error(st);
+      // MutableArrayData keeps every extended row of a FixedSizeBinary(0) child (try_new's length rule is the top level's)
+      return ArrayRef(std::make_shared<FixedSizeBinaryArray>(w, vb, step ? n : o.len, out_nulls(o, nb, step)));
+    }
+    case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: {
+      const acu_list_array l = list_view(values);
+      Buffer offs = Buffer::allocate((size_t)(n + 1) * (l.kind == ACU_LIST ? 4 : 8));
+      acu_array_out o = validity_out(nb, n);
+      acu_filter_plan *child_plan = nullptr;
+      if ((st = acu_filter_list(c.raw(), plan, &l, offs.data(), &o, &child_plan)) != ACU_OK) return c.last_error(st);
+      const FilterPredicate cp(child_plan);
+      auto child = filter_any(*list_values(values), cp, child_step ? *child_step : n != acu_filter_plan_len(plan));
+      if (child.is_err()) return child.unwrap_err();
+      return list_like(values, offs, child.unwrap(), o.len, out_nulls(o, nb, step));
+    }
+    case DataType::Struct: {  // filter_struct: every column, then filter_nulls
+      std::vector<ArrayRef> cols;
+      for (const auto &col : static_cast<const StructArray &>(values).columns()) {
+        auto r = filter_any(*col, pred, child_step);
+        if (r.is_err()) return r.unwrap_err();
+        cols.push_back(r.unwrap());
+      }
+      const acu_array nv = nulls_view(values);
+      acu_array_out o = validity_out(nb, n);
+      if ((st = acu_filter_nulls(c.raw(), plan, &nv, &o)) != ACU_OK) return c.last_error(st);
+      return ArrayRef(std::make_shared<StructArray>(std::move(cols), n, out_nulls(o, nb, step)));
+    }
+    case DataType::Union: {
+      const auto &u = static_cast<const UnionArray &>(values);
+      const int32_t strategy = acu_filter_plan_strategy(plan);
+      if (u.is_dense() && step && strategy == ACU_FILTER_ALL) {
+        // a list's child step extends every row even when its plan selects them all: the rows of a take of 0 .. n
+        std::vector<uint64_t> ids((size_t)n);
+        for (int64_t i = 0; i < n; ++i) ids[(size_t)i] = (uint64_t)i;
+        return take_any(values, PrimitiveArray<uint64_t>::from(ids), 0, true);
+      }
+      const acu_union_array uv = u.union_view();
+      const size_t nf = u.field_type_ids().size();
+      Buffer tids = Buffer::allocate((size_t)n), offs = Buffer::allocate((size_t)n * 4), map = Buffer::allocate((size_t)n * 4);
+      std::vector<int64_t> starts(nf + 1, 0);
+      if ((st = acu_filter_union(c.raw(), plan, &uv, static_cast<int8_t *>(tids.data()), static_cast<int32_t *>(offs.data()),
+                                 static_cast<int32_t *>(map.data()), starts.data())) != ACU_OK)
+        return c.last_error(st);
+      std::vector<ArrayRef> children;
+      if (u.is_dense()) {
+        if (strategy == ACU_FILTER_ALL) return union_head(u, n);  // values.slice(0, count)
+        for (size_t f = 0; f < nf; ++f) {  // build_extend_dense: each child extended row by row
+          auto r = take_any(*u.children()[f], *i32_slice(map, starts[f], starts[f + 1] - starts[f]), 0, true);
+          if (r.is_err()) return r.unwrap_err();
+          children.push_back(r.unwrap());
+        }
+        return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, offs, std::move(children), n));
+      }
+      for (const auto &ch : u.children()) {
+        auto r = filter_any(*ch, pred, child_step);
+        if (r.is_err()) return r.unwrap_err();
+        children.push_back(r.unwrap());
+      }
+      if (strategy == ACU_FILTER_NONE || strategy == ACU_FILTER_ALL) {
+        std::vector<int8_t> t = u.type_ids();
+        tids = Buffer::from_host(t.data(), (size_t)n);
+      }
+      return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, std::nullopt, std::move(children), n));
+    }
+    case DataType::RunEndEncoded:
+      return ArrowError{ACU_ERR_NOT_YET_IMPLEMENTED, "Not yet implemented: filter of a RunEndEncoded array below the top level"};
+    default: {
+      const int w = dtype_width(values.data_type());
+      acu_array_out o = make_out(vb, nb, (size_t)n * w, n);
+      if ((st = acu_filter_primitive(c.raw(), plan, w, &v, &o)) != ACU_OK) return c.last_error(st);
+      return make_primitive(values.data_type(), vb, o.len, out_nulls(o, nb, step));
+    }
   }
-  for (const auto &ch : u.children()) {
-    auto r = filter_any(*ch, pred, plan, child_step);
-    if (r.is_err()) return r.unwrap_err();
-    children.push_back(r.unwrap());
-  }
-  if (whole) {
-    std::vector<int8_t> t = u.type_ids();
-    tids = Buffer::from_host(t.data(), (size_t)n);
-  }
-  return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, std::nullopt, std::move(children), n));
 }
 
-inline Result<ArrayRef> take_nested(const Array &values, const Array &indices, int cb, bool keep) {
+inline Result<ArrayRef> take_any(const Array &values, const Array &indices, int cb, bool keep) {
   Context &c = Context::get();
   const int64_t m = indices.len();
-  const acu_array ix = indices.view();
+  const acu_array v = values.view(), ix = indices.view();
   const acu_dtype it = (acu_dtype)dtype_code(indices.data_type());
+  Buffer vb, nb;
   acu_status st;
   std::optional<ArrowError> deferred;
   std::vector<ArrayRef> children;
-  if (values.data_type() == DataType::Struct) {
-    // take_impl's Struct arm: check_bounds first, then the columns, then the validity (whose panic comes after them)
-    const auto &sa = static_cast<const StructArray &>(values);
-    const acu_array nv = nulls_view(values);
-    Buffer nb = Buffer::allocate(acu_bitmap_bytes(m));
-    acu_array_out o{};
-    o.validity = static_cast<uint8_t *>(nb.data());
-    if ((st = acu_take_nulls(c.raw(), &nv, &ix, it, cb, &o)) != ACU_OK) {
-      if (st != ACU_ERR_PANIC_OUT_OF_BOUNDS) return c.last_error(st);
-      deferred = c.last_error(st);
+  switch (values.data_type()) {
+    case DataType::Boolean: {
+      acu_array_out o = make_out(vb, nb, acu_bitmap_bytes(m), m);
+      if ((st = acu_take_boolean(c.raw(), &v, &ix, it, cb, &o)) != ACU_OK) return c.last_error(st);
+      return ArrayRef(std::make_shared<BooleanArray>(vb, 0, o.len, out_nulls(o, nb)));
     }
-    for (const auto &col : sa.columns()) {
-      auto r = take_any(*col, indices, 0, keep);
-      if (r.is_err()) return r.unwrap_err();
-      children.push_back(r.unwrap());
+    case DataType::Utf8: {
+      const auto &s = static_cast<const StringArray &>(values);
+      const uint8_t *src = static_cast<const uint8_t *>(s.value_data().data());
+      return bytes_out(m, false, [&](void *offs, uint8_t *data, int64_t cap, int64_t *total, acu_array_out *o) {
+        if (keep) return acu_take_bytes_extend(c.raw(), 4, s.offsets().data(), src, &v, &ix, it, offs, data, cap, total, o);
+        return acu_take_bytes(c.raw(), 4, s.offsets().data(), src, &v, &ix, it, cb, offs, data, cap, total, o);
+      });
     }
-    if (deferred) return *deferred;
-    std::optional<NullBuffer> nulls = out_nulls(o, nb);
-    if (children.empty() && !keep && !nulls) nulls = nulls_from_mask(std::vector<bool>((size_t)m, true), true);  // new_empty_fields
-    return ArrayRef(std::make_shared<StructArray>(std::move(children), m, std::move(nulls)));
+    case DataType::FixedSizeBinary: {  // take_fixed_size_binary (take.rs:802-862)
+      const int32_t w = static_cast<const FixedSizeBinaryArray &>(values).value_length();
+      acu_array_out o = make_out(vb, nb, (size_t)m * w, m);
+      if ((st = acu_take_fixed_size_binary(c.raw(), w, &v, &ix, it, cb, &o)) != ACU_OK) return c.last_error(st);
+      // MutableArrayData keeps every extended row of a FixedSizeBinary(0) child (try_new's length rule is the top level's)
+      return ArrayRef(std::make_shared<FixedSizeBinaryArray>(w, vb, keep ? m : o.len, out_nulls(o, nb)));
+    }
+    case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: {
+      const acu_list_array l = list_view(values);
+      const bool fixed = l.kind == ACU_FIXED_SIZE_LIST;
+      const acu_dtype cdt = fixed || l.child_len <= (int64_t)UINT32_MAX ? ACU_U32 : ACU_U64;
+      Buffer offs = Buffer::allocate((size_t)(m + 1) * (l.kind == ACU_LIST ? 4 : 8));
+      acu_array_out o = validity_out(nb, m), cn{};
+      int64_t rows = 0;
+      if ((st = acu_take_list(c.raw(), &l, &ix, it, cb, keep ? 1 : 0, offs.data(), &o, cdt, nullptr, 0, &rows, &cn)) != ACU_OK) return c.last_error(st);
+      Buffer map = Buffer::allocate((size_t)rows * (cdt == ACU_U32 ? 4 : 8)), cnb = Buffer::allocate(acu_bitmap_bytes(rows));
+      cn.validity = static_cast<uint8_t *>(cnb.data());
+      if ((st = acu_take_list(c.raw(), &l, &ix, it, cb, keep ? 1 : 0, offs.data(), &o, cdt, map.data(), rows, &rows, &cn)) != ACU_OK) {
+        // take_fixed_size_list: the child is taken before the list's validity is read
+        if (!fixed || st != ACU_ERR_PANIC_OUT_OF_BOUNDS) return c.last_error(st);
+        deferred = c.last_error(st);
+      }
+      std::optional<NullBuffer> map_nulls;
+      if (cn.has_validity) map_nulls = NullBuffer{cnb, 0, rows, cn.null_count};
+      ArrayRef rm = cdt == ACU_U32 ? ArrayRef(std::make_shared<PrimitiveArray<uint32_t>>(map, rows, map_nulls))
+                                   : ArrayRef(std::make_shared<PrimitiveArray<uint64_t>>(map, rows, map_nulls));
+      auto child = take_any(*list_values(values), *rm, 0, keep || !fixed);
+      if (child.is_err()) return child.unwrap_err();
+      if (deferred) return *deferred;
+      return list_like(values, offs, child.unwrap(), o.len, out_nulls(o, nb));
+    }
+    case DataType::Struct: {
+      // take_impl's Struct arm: check_bounds first, then the columns, then the validity (whose panic comes after them)
+      const acu_array nv = nulls_view(values);
+      acu_array_out o = validity_out(nb, m);
+      if ((st = acu_take_nulls(c.raw(), &nv, &ix, it, cb, &o)) != ACU_OK) {
+        if (st != ACU_ERR_PANIC_OUT_OF_BOUNDS) return c.last_error(st);
+        deferred = c.last_error(st);
+      }
+      for (const auto &col : static_cast<const StructArray &>(values).columns()) {
+        auto r = take_any(*col, indices, 0, keep);
+        if (r.is_err()) return r.unwrap_err();
+        children.push_back(r.unwrap());
+      }
+      if (deferred) return *deferred;
+      std::optional<NullBuffer> nulls = out_nulls(o, nb);
+      if (children.empty() && !keep && !nulls) nulls = nulls_from_mask(std::vector<bool>((size_t)m, true), true);  // new_empty_fields
+      return ArrayRef(std::make_shared<StructArray>(std::move(children), m, std::move(nulls)));
+    }
+    case DataType::Union: {
+      const auto &u = static_cast<const UnionArray &>(values);
+      const acu_union_array uv = u.union_view();
+      const size_t nf = u.field_type_ids().size();
+      Buffer tids = Buffer::allocate((size_t)m), offs = Buffer::allocate((size_t)m * 4), map = Buffer::allocate((size_t)m * 4);
+      std::vector<int64_t> starts(nf + 1, 0);
+      if ((st = acu_take_union(c.raw(), &uv, &ix, it, cb, static_cast<int8_t *>(tids.data()), static_cast<int32_t *>(offs.data()),
+                               static_cast<int32_t *>(map.data()), starts.data())) != ACU_OK) {
+        ArrowError e = c.last_error(st);
+        // UnionArray::try_new validates after the children are taken
+        if (e.message.find("Type Ids values must match one of the field type ids") == std::string::npos &&
+            e.message.find("Offsets must be non-negative and within the length of the Array") == std::string::npos)
+          return e;
+        deferred = e;
+      }
+      for (size_t f = 0; f < nf; ++f) {
+        auto r = u.is_dense() ? take_any(*u.children()[f], *i32_slice(map, starts[f], starts[f + 1] - starts[f]), 0, keep)
+                              : take_any(*u.children()[f], indices, 0, keep);
+        if (r.is_err()) return r.unwrap_err();
+        children.push_back(r.unwrap());
+      }
+      if (deferred) return *deferred;
+      std::optional<Buffer> ob;
+      if (u.is_dense()) ob = offs;
+      return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, std::move(ob), std::move(children), m));
+    }
+    case DataType::RunEndEncoded:
+      return ArrowError{ACU_ERR_NOT_YET_IMPLEMENTED, "Not yet implemented: take of a RunEndEncoded array below the top level"};
+    default: {
+      const int w = dtype_width(values.data_type());
+      acu_array_out o = make_out(vb, nb, (size_t)m * w, m);
+      if ((st = acu_take_primitive(c.raw(), w, &v, &ix, it, cb, &o)) != ACU_OK) return c.last_error(st);
+      return make_primitive(values.data_type(), vb, o.len, out_nulls(o, nb));
+    }
   }
-  const auto &u = static_cast<const UnionArray &>(values);
-  const acu_union_array uv = u.union_view();
-  const size_t nf = u.field_type_ids().size();
-  Buffer tids = Buffer::allocate((size_t)m), offs = Buffer::allocate((size_t)m * 4), map = Buffer::allocate((size_t)m * 4);
-  std::vector<int64_t> starts(nf + 1, 0);
-  if ((st = acu_take_union(c.raw(), &uv, &ix, it, cb, static_cast<int8_t *>(tids.data()), static_cast<int32_t *>(offs.data()),
-                           static_cast<int32_t *>(map.data()), starts.data())) != ACU_OK) {
-    ArrowError e = c.last_error(st);
-    // UnionArray::try_new validates after the children are taken
-    if (e.message.find("Type Ids values must match one of the field type ids") == std::string::npos &&
-        e.message.find("Offsets must be non-negative and within the length of the Array") == std::string::npos)
-      return e;
-    deferred = e;
-  }
-  for (size_t f = 0; f < nf; ++f) {
-    auto r = u.is_dense() ? take_any(*u.children()[f], *i32_slice(map, starts[f], starts[f + 1] - starts[f]), 0, keep)
-                          : take_any(*u.children()[f], indices, 0, keep);
-    if (r.is_err()) return r.unwrap_err();
-    children.push_back(r.unwrap());
-  }
-  if (deferred) return *deferred;
-  std::optional<Buffer> ob;
-  if (u.is_dense()) ob = offs;
-  return ArrayRef(std::make_shared<UnionArray>(u.field_type_ids(), tids, std::move(ob), std::move(children), m));
 }
 
-inline Result<ArrayRef> take_nested_top(const Array &values, const Array &indices, std::optional<TakeOptions> options) {
+template <class R>
+Result<ArrayRef> filter_run_end(const RunArray<R> &values, const FilterPredicate &pred) {
+  Context &c = Context::get();
+  acu_filter_plan *plan = pred.raw();
+  const acu_run_array r = values.run_view();
+  const int64_t count = pred.count();
+  Buffer ends = Buffer::allocate((size_t)std::max<int64_t>(std::min(count, values.num_runs()), 1) * sizeof(R));
+  int64_t runs = 0, start = 0;
+  acu_filter_plan *vplan = nullptr;
+  acu_status st = acu_filter_run_end(c.raw(), plan, &r, ends.data(), &runs, &start, &vplan);
+  if (st != ACU_OK) return c.last_error(st);
+  if (!vplan) {
+    if (acu_filter_plan_strategy(plan) == ACU_FILTER_ALL) return ArrayRef(std::make_shared<RunArray<R>>(values.slice(0, count)));
+    return ArrayRef(std::make_shared<RunArray<R>>(Buffer::allocate(0), 0, empty_like(*values.values()), 0, 0));
+  }
+  const FilterPredicate vpred(vplan);
+  auto v = filter_any(*slice_any(*values.values(), start, acu_filter_plan_len(vplan)), vpred);
+  if (v.is_err()) return v.unwrap_err();
+  std::vector<R> host((size_t)runs);
+  ends.to_host(host.data(), host.size() * sizeof(R));
+  return ArrayRef(std::make_shared<RunArray<R>>(ends, runs, v.unwrap(), 0, (int64_t)host.back()));  // the last new run end
+}
+
+template <class R>
+Result<ArrayRef> take_run_end(const RunArray<R> &values, const Array &indices, int cb) {
+  Context &c = Context::get();
   const DataType it = indices.data_type();
-  if ((int)it > (int)DataType::UInt64)  // take.rs:103
-    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + dtype_display(it)};
-  return take_nested(values, indices, options && options->check_bounds ? 1 : 0, false);
+  const Array &vals = *values.values();
+  acu_run_values rv{};
+  switch (vals.data_type()) {
+    case DataType::Boolean: rv.kind = ACU_RUN_VALUES_BOOLEAN; rv.array = vals.view(); break;
+    case DataType::Utf8: {
+      const auto &s = static_cast<const StringArray &>(vals);
+      rv.kind = ACU_RUN_VALUES_BYTES;
+      rv.width = 4;
+      rv.bytes.offsets = s.offsets().data();
+      rv.bytes.data = static_cast<const uint8_t *>(s.value_data().data());
+      rv.bytes.nulls = vals.view();
+      break;
+    }
+    case DataType::List: case DataType::LargeList: case DataType::FixedSizeList: case DataType::Struct: case DataType::Union:
+    case DataType::FixedSizeBinary:  // the run merge would need a value_length-byte comparator
+      rv.kind = ACU_RUN_VALUES_NESTED;
+      break;
+    default:
+      if (dtype_width(vals.data_type()) == 0)
+        throw std::runtime_error(std::string("RunArray values of type ") + dtype_display(vals.data_type()) + " are not supported by this mirror");
+      rv.kind = ACU_RUN_VALUES_FIXED;
+      rv.width = dtype_width(vals.data_type());
+      rv.array = vals.view();
+  }
+  const int64_t m = indices.len();
+  const bool wide = it == DataType::Int64 || it == DataType::UInt64;  // ToIndices: UInt64 value indices
+  const acu_run_array r = values.run_view();
+  const acu_array ix = indices.view();
+  Buffer ends = Buffer::allocate((size_t)std::max<int64_t>(m, 1) * sizeof(R)), vi = Buffer::allocate((size_t)std::max<int64_t>(m, 1) * (wide ? 8 : 4));
+  int64_t runs = 0;
+  acu_status st = acu_take_run_end(c.raw(), &r, &rv, &ix, (acu_dtype)dtype_code(it), cb, ends.data(), vi.data(), &runs);
+  if (st != ACU_OK) return c.last_error(st);
+  if (m == 0) return ArrayRef(std::make_shared<RunArray<R>>(Buffer::allocate(0), 0, empty_like(vals), 0, 0));
+  ArrayRef vix = wide ? ArrayRef(std::make_shared<PrimitiveArray<uint64_t>>(vi, runs, std::nullopt))
+                      : ArrayRef(std::make_shared<PrimitiveArray<uint32_t>>(vi, runs, std::nullopt));
+  auto v = take_any(vals, *vix, 0, false);
+  if (v.is_err()) return v.unwrap_err();
+  return ArrayRef(std::make_shared<RunArray<R>>(ends, runs, v.unwrap(), 0, m));
 }
 }  // namespace detail
 
-inline Result<ArrayRef> filter(const StructArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
-inline Result<ArrayRef> filter(const UnionArray &values, const BooleanArray &predicate) { return detail::filter_list(values, predicate); }
-inline Result<ArrayRef> take(const StructArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
-  return detail::take_nested_top(values, indices, options);
+inline Result<ArrayRef> FilterPredicate::filter(const Array &values) const {
+  if (values.data_type() == DataType::RunEndEncoded)
+    return detail::with_run_array(values, [&](const auto &run) { return detail::filter_run_end(run, *this); });
+  return detail::filter_any(values, *this);
 }
-inline Result<ArrayRef> take(const UnionArray &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
-  return detail::take_nested_top(values, indices, options);
+
+// arrow::compute::filter (filter.rs:201-213)
+inline Result<ArrayRef> filter(const Array &values, const BooleanArray &predicate) {
+  auto pred = FilterPredicate::try_new(predicate);
+  if (pred.is_err()) return pred.unwrap_err();
+  return pred.unwrap().filter(values);
+}
+inline Result<RecordBatch> filter_record_batch(const RecordBatch &batch, const BooleanArray &predicate) {
+  return FilterBuilder(predicate).optimize().build().filter_record_batch(batch);
+}
+
+// arrow::compute::take (take.rs:89-105)
+inline Result<ArrayRef> take(const Array &values, const Array &indices, std::optional<TakeOptions> options = std::nullopt) {
+  if (auto e = detail::index_type_error(indices.data_type())) return *e;
+  const int cb = options && options->check_bounds ? 1 : 0;
+  if (values.data_type() == DataType::RunEndEncoded)
+    return detail::with_run_array(values, [&](const auto &run) { return detail::take_run_end(run, indices, cb); });
+  return detail::take_any(values, indices, cb, false);
 }
 
 // take.rs:1123-1133: every column gathered with the same indices, one synchronisation per (up to 64-column) call.
@@ -1572,8 +1492,7 @@ inline Result<ArrayRef> take(const UnionArray &values, const Array &indices, std
 inline Result<RecordBatch> take_record_batch(const RecordBatch &batch, const Array &indices) {
   Context &c = Context::get();
   const DataType it = indices.data_type();
-  if (dtype_width(it) == 0 || it == DataType::Float32 || it == DataType::Float64)
-    return ArrowError{ACU_ERR_INVALID_ARGUMENT, std::string("Invalid argument error: Take only supported for integers, got ") + detail::dtype_display(it)};
+  if (auto e = detail::index_type_error(it)) return *e;
   const auto &cols = batch.columns();
   const int64_t m = indices.len();
   if (cols.empty()) return RecordBatch(batch.schema(), {}, m);

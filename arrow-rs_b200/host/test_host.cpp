@@ -671,6 +671,30 @@ static void test_slice_iterator() {
   CHECK_EQ(61 + 61 + 5, pred.count());
 }
 
+// Primitive, Boolean and Utf8 arrays reached through an ArrayRef (as RecordBatch::column returns them) give the results of
+// the concrete-type calls in filter, FilterPredicate::filter and take
+template <class A>
+static void check_array_ref(const A &a) {
+  const ArrayRef ref = std::make_shared<A>(a);
+  auto same = [](Result<ArrayRef> got, const ArrayRef &want) {
+    if (got.is_err()) return false;
+    const ArrayRef g = got.unwrap();
+    return g->data_type() == want->data_type() && static_cast<const A &>(*g).to_vec() == static_cast<const A &>(*want).to_vec();
+  };
+  const auto p = BooleanArray::from(std::vector<bool>{true, false, true, true});
+  const auto idx = Int64Array::from(std::vector<O<int64_t>>{3, N, 0, 0});
+  const ArrayRef f = filter(a, p).unwrap(), t = take(a, idx).unwrap();
+  CHECK(same(filter(*ref, p), f));
+  CHECK(same(FilterBuilder(p).build().filter(*ref), f));
+  CHECK(same(take(*ref, idx), t));
+}
+static void test_array_ref() {
+  check_array_ref(Int16Array::from(std::vector<O<int16_t>>{1, N, -3, 4}));
+  check_array_ref(Float64Array::from(std::vector<double>{1.5, 2.5, -3.5, 4.5}));
+  check_array_ref(BooleanArray::from(std::vector<O<bool>>{true, N, false, true}));
+  check_array_ref(StringArray::from(std::vector<O<std::string>>{"a", N, "ccc", ""}));
+}
+
 int main() {
   try {
     Context::get(0);
@@ -711,6 +735,7 @@ int main() {
       {"ipc_stream_reader", test_ipc_stream_reader},
       {"string_view_coalesce", test_string_view_coalesce},
       {"slice_iterator", test_slice_iterator},
+      {"array_ref", test_array_ref},
   };
   for (auto &t : tests) {
     int before = g_failed;

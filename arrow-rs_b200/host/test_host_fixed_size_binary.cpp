@@ -126,6 +126,33 @@ static void test_record_batches() {
   CHECK(t.num_rows() == 2 && fsb(t.column(0)).value(0) == Bytes(20, 3) && fsb(t.column(0)).value(1) == Bytes(20, 1) && !t.column(0)->nulls());
 }
 
+// FixedSizeBinary arrays of any width reached through an ArrayRef (as RecordBatch::column returns them) give the results of
+// the concrete-type calls in filter, FilterPredicate::filter and take
+static void test_array_ref() {
+  for (int32_t w : {0, 3, 16}) {
+    Rows rows;
+    for (uint8_t k = 1; k <= 4; ++k) rows.push_back(k == 2 ? std::nullopt : std::optional<Bytes>(Bytes((size_t)w, k)));
+    const auto a = FixedSizeBinaryArray::from(rows, w);
+    const ArrayRef ref = std::make_shared<FixedSizeBinaryArray>(a);
+    auto bytes = [](const ArrayRef &r) {
+      Rows out;
+      for (int64_t i = 0; i < r->len(); ++i) out.push_back(r->is_null(i) ? std::nullopt : std::optional<Bytes>(fsb(r).value(i)));
+      return out;
+    };
+    auto same = [&](Result<ArrayRef> got, const ArrayRef &want) {
+      if (got.is_err()) return false;
+      const ArrayRef g = got.unwrap();
+      return g->data_type() == DataType::FixedSizeBinary && fsb(g).value_length() == w && g->len() == want->len() && bytes(g) == bytes(want);
+    };
+    const auto p = pred({true, true, false, true});
+    const auto idx = UInt32Array::from(std::vector<uint32_t>{3, 1, 0});
+    const ArrayRef f = filter(a, p).unwrap(), t = take(a, idx).unwrap();
+    CHECK(same(filter(*ref, p), f));
+    CHECK(same(FilterBuilder(p).build().filter(*ref), f));
+    CHECK(same(take(*ref, idx), t));
+  }
+}
+
 int main() {
   try {
     Context::get();
@@ -140,6 +167,7 @@ int main() {
   test_take_panics_and_wrap();
   test_slice_and_nesting();
   test_record_batches();
+  test_array_ref();
   std::printf("%d checks, %d failed\n", g_checks, g_failed);
   return g_failed ? 1 : 0;
 }

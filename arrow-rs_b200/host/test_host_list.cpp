@@ -139,6 +139,29 @@ static void test_filter_child_plan_all() {
   CHECK(compute::detail::list_values(*r)->nulls().has_value());
 }
 
+// Every list type reached through an ArrayRef (as RecordBatch::column and every child accessor return it) takes the list
+// path in filter, FilterPredicate::filter and take, with the results of the concrete-type calls
+static bool same_list(Result<ArrayRef> got, const ArrayRef &want) {
+  if (got.is_err()) return false;
+  const ArrayRef g = got.unwrap();
+  return g->data_type() == want->data_type() && rows_of(*g) == rows_of(*want);
+}
+template <class L>
+static void check_array_ref(const L &a) {
+  const ArrayRef ref = std::make_shared<L>(a);
+  const auto p = BooleanArray::from(std::vector<bool>{true, false, true, true});
+  const auto idx = UInt32Array::from(std::vector<uint32_t>{3, 0, 0});
+  const ArrayRef f = filter(a, p).unwrap(), t = take(a, idx).unwrap();
+  CHECK(same_list(filter(*ref, p), f));
+  CHECK(same_list(FilterBuilder(p).build().filter(*ref), f));
+  CHECK(same_list(take(*ref, idx), t));
+}
+static void test_array_ref() {
+  check_array_ref(ListArray::from({0, 2, 2, 5, 6}, ints(iv({0, 1, 2, 3, 4, 5})), {true, false, true, true}));
+  check_array_ref(LargeListArray::from({0, 2, 2, 5, 6}, ints(iv({0, 1, 2, 3, 4, 5}))));
+  check_array_ref(FixedSizeListArray::from(2, ints(iv({0, 1, 2, 3, 4, 5, 6, 7}))));
+}
+
 int main() {
   try {
     Context::get();
@@ -155,6 +178,7 @@ int main() {
   test_take_sliced<ListArray>();
   test_take_sliced<LargeListArray>();
   test_take_fixed_size_list();
+  test_array_ref();
   std::printf("%d checks, %d failed\n", g_checks, g_failed);
   return g_failed ? 1 : 0;
 }

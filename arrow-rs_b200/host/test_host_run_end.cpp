@@ -227,6 +227,43 @@ static void test_take_errors() {
   CHECK(e.status == ACU_ERR_PANIC_OUT_OF_BOUNDS && e.message == "called `Option::unwrap()` on a `None` value");
 }
 
+// A RunArray of every run-end type reached through an ArrayRef (as RecordBatch::column and every child accessor return
+// it) takes the run-end path in filter, FilterPredicate::filter and take, with the results of the concrete-type calls
+template <class R>
+static void check_array_ref() {
+  const auto a = RunArray<R>::from({2, 3, 8}, prim<int32_t>({7, -2, 9}));
+  const ArrayRef ref = std::make_shared<RunArray<R>>(a);
+  auto same = [](Result<ArrayRef> got, const ArrayRef &want) {
+    if (got.is_err()) return false;
+    const ArrayRef g = got.unwrap();
+    return g->data_type() == DataType::RunEndEncoded && logical<R, int32_t>(as_run<R>(g)) == logical<R, int32_t>(as_run<R>(want));
+  };
+  const auto p = BooleanArray::from(std::vector<bool>{true, false, true, false, true, false, true, false});
+  const auto idx = UInt32Array::from(std::vector<uint32_t>{7, 2, 0, 0});
+  const ArrayRef f = filter(a, p).unwrap(), t = take(a, idx).unwrap();
+  CHECK(same(filter(*ref, p), f));
+  CHECK(same(FilterBuilder(p).build().filter(*ref), f));
+  CHECK(same(take(*ref, idx), t));
+}
+
+// RunEndEncoded is filtered and taken at the top level only: below a struct or a list it is refused
+static void test_nested_run_end_refused() {
+  const ArrayRef run = std::make_shared<Int32RunArray>(Int32RunArray::from({2, 3}, prim<int32_t>({1, 2})));
+  const auto p = BooleanArray::from(std::vector<bool>{true, false, true});
+  const auto idx = UInt32Array::from(std::vector<uint32_t>{2, 0});
+  const std::string f = "Not yet implemented: filter of a RunEndEncoded array below the top level";
+  const std::string t = "Not yet implemented: take of a RunEndEncoded array below the top level";
+  auto refused = [](Result<ArrayRef> r, const std::string &msg) {
+    return r.is_err() && r.unwrap_err().status == ACU_ERR_NOT_YET_IMPLEMENTED && r.unwrap_err().message == msg;
+  };
+  const auto s = StructArray::from({run});
+  CHECK(refused(filter(s, p), f));
+  CHECK(refused(take(s, idx), t));
+  const auto l = ListArray::from({0, 1, 3}, run);
+  CHECK(refused(filter(l, BooleanArray::from(std::vector<bool>{false, true})), f));
+  CHECK(refused(take(l, idx.slice(1, 1)), t));
+}
+
 int main() {
   try {
     Context::get();
@@ -249,6 +286,10 @@ int main() {
   test_take_mixed_runs();
   test_get_physical_indices();
   test_take_errors();
+  check_array_ref<int16_t>();
+  check_array_ref<int32_t>();
+  check_array_ref<int64_t>();
+  test_nested_run_end_refused();
   std::printf("%d checks, %d failed\n", g_checks, g_failed);
   return g_failed ? 1 : 0;
 }

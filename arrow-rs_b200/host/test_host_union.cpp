@@ -215,6 +215,34 @@ static void test_take_union_type_id_validation() {
   CHECK(UnionArray::try_new({0}, {1}, std::nullopt, {prim<int32_t>({1})}).is_err());
 }
 
+// Struct and Union arrays reached through an ArrayRef (as RecordBatch::column and every child accessor return them) take
+// their own paths in filter, FilterPredicate::filter and take, with the results of the concrete-type calls
+template <class A, class Rows>
+static void check_array_ref(const A &a, const BooleanArray &p, const UInt32Array &idx, Rows rows) {
+  const ArrayRef ref = std::make_shared<A>(a);
+  auto same = [&](Result<ArrayRef> got, const ArrayRef &want) {
+    if (got.is_err()) return false;
+    const ArrayRef g = got.unwrap();
+    return g->data_type() == a.data_type() && rows(g) == rows(want);
+  };
+  const ArrayRef f = filter(a, p).unwrap(), t = take(a, idx).unwrap();
+  CHECK(same(filter(*ref, p), f));
+  CHECK(same(FilterBuilder(p).build().filter(*ref), f));
+  CHECK(same(take(*ref, idx), t));
+}
+static void test_array_ref() {
+  const auto idx = UInt32Array::from(std::vector<uint32_t>{2, 0, 2});
+  for (bool dense : {true, false}) {
+    auto rows = [](const ArrayRef &r) {
+      std::vector<std::pair<int8_t, O<double>>> out;
+      for (const Row &x : union_rows(as_union(r))) out.push_back({x.t, x.v});
+      return out;
+    };
+    check_array_ref(ab_union({{0, 1}, {1, 3.2}, {0, 34}}, dense), pred({true, false, true}), idx, rows);
+  }
+  check_array_ref(test_struct(kStruct), pred({true, false, true, false, true}), idx, [](const ArrayRef &r) { return struct_rows(as_struct(r)); });
+}
+
 int main() {
   try {
     Context::get();
@@ -236,6 +264,7 @@ int main() {
   test_take_union_dense_using_builder();
   test_take_union_dense_all_match_issue_6206();
   test_take_union_type_id_validation();
+  test_array_ref();
   std::printf("%d checks, %d failed\n", g_checks, g_failed);
   return g_failed ? 1 : 0;
 }
