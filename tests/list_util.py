@@ -7,7 +7,7 @@ import numpy as np
 from acu import FixedSizeListColumn, HostArray, ListColumn
 from acu import _abi as abi
 
-import oracle_list as ol
+import oracle_filter_take as oft
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "list_vectors.json")
 DTYPES = {"u32": abi.U32, "i32": abi.I32, "i64": abi.I64, "u8": abi.U8, "u64": abi.U64}
@@ -56,8 +56,8 @@ def check(case, run, error_type):
         raise AssertionError(f"{case['name']}: no error")
     got = run()
     if exp is not None:
-        assert ol.to_pylist(got) == exp, case["name"]
+        assert oft.to_pylist(got) == exp, case["name"]
     if "expect_child" in case:
-        assert ol.to_pylist(got.child) == case["expect_child"], case["name"]
+        assert oft.to_pylist(got.child) == case["expect_child"], case["name"]
     if "expect_offsets" in case:
         assert [int(x) for x in got.offsets] == case["expect_offsets"]

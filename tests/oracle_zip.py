@@ -17,7 +17,7 @@ import numpy as np
 from acu import FixedSizeBinaryColumn, HostArray, Utf8Column, ViewColumn
 from acu import _abi as abi
 
-from oracle_list import EXTEND_OVERFLOW, OracleError
+from oracle_filter_take import EXTEND_OVERFLOW, OracleError
 
 I32_MAX = (1 << 31) - 1
 

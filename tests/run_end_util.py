@@ -7,7 +7,7 @@ import numpy as np
 from acu import HostArray, RunEndColumn, Utf8Column
 from acu import _abi as abi
 
-import oracle_run_end as ore
+import oracle_filter_take as oft
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "run_end_vectors.json")
 DTYPES = {"i8": abi.I8, "u8": abi.U8, "i16": abi.I16, "u16": abi.U16, "i32": abi.I32, "u32": abi.U32, "i64": abi.I64, "u64": abi.U64}
@@ -51,12 +51,12 @@ def check(case, got):
         assert [int(x) for x in got.run_ends] == case["expect_run_ends"], name
         assert got.offset == 0
     if "expect_values" in case:
-        vals = ore.ol.to_pylist(got.values)
+        vals = oft.to_pylist(got.values)
         if case["values_type"] == "utf8":
             vals = [v.decode() for v in vals]
         assert vals == case["expect_values"], name
     if "expect_logical" in case:
-        vals = ore.logical(got)
+        vals = oft.logical(got)
         if case["values_type"] == "utf8":
             vals = [v.decode() for v in vals]
         assert vals == case["expect_logical"], name

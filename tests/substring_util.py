@@ -8,6 +8,8 @@ import numpy as np
 from acu import FixedSizeBinaryColumn, HostArray, Utf8Column, ViewColumn, column_value
 from acu import _abi as abi
 
+from oracle_filter_take import nulls_of
+
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "substring_vectors.json")
 OFFSET_DTYPE = {"utf8": np.int32, "binary": np.int32, "large_utf8": np.int64, "large_binary": np.int64}
 
@@ -19,13 +21,6 @@ def golden_cases():
 
 def decode(items):
     return [None if x is None else bytes.fromhex(x) for x in items]
-
-
-def nulls_of(mask, force=False):
-    mask = np.asarray(mask, dtype=bool)
-    h = HostArray.from_list(abi.U8, [0 if m else None for m in mask], force_validity=force)
-    h.values = np.zeros(0, np.uint8)
-    return h
 
 
 def bytes_col(items, dtype, garbage=b""):

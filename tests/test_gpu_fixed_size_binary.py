@@ -1,4 +1,4 @@
-"""filter / take of FixedSizeBinary columns on the device against tests/oracle_fixed_size_binary.py, bit for bit: the value
+"""filter / take of FixedSizeBinary columns on the device against tests/oracle_filter_take.py, bit for bit: the value
 bytes (under null rows included), validity, null count, NullBuffer presence, length, and error status / text / row. Every
 case uses a fixed seed. The grid-round cases are sized from fixed_size_binary.cu's launch constants (checked against the
 source by test_fixed_size_binary_launch_constants.py)."""
@@ -11,9 +11,9 @@ import acu
 from acu import FixedSizeBinaryColumn, FixedSizeListColumn, HostArray, ListColumn, RunEndColumn, StructColumn, UnionColumn, Utf8Column
 from acu import _abi as abi
 
-import oracle_fixed_size_binary as of
-import oracle_list as ol
+import oracle_filter_take as oft
 import test_oracle_fixed_size_binary as tg
+from oracle_filter_take import nulls_of
 
 pytestmark = pytest.mark.gpu
 
@@ -39,13 +39,7 @@ def random_column(rng, n, w, null_p=0.2, bit_offset=0):
 
 
 def same(got, exp):
-    assert got.length == exp.length
-    assert got.values.shape == exp.values.shape
-    assert np.array_equal(got.values, exp.values)
-    assert of.has_buffer(got) == of.has_buffer(exp)
-    if of.has_buffer(exp):
-        assert np.array_equal(of.valid_mask(got), of.valid_mask(exp))
-        assert got.nulls.null_count == exp.nulls.null_count
+    assert oft.describe(got) == oft.describe(exp)
 
 
 def gpu_filter(gpu, col, pred):
@@ -53,14 +47,14 @@ def gpu_filter(gpu, col, pred):
 
 
 def oracle_filter(col, pred):
-    return of.filter(col, np.asarray(pred, bool))
+    return oft.filter(col, np.asarray(pred, bool))
 
 
 def run_both(gpu_fn, oracle_fn):
     """(result, None) or (None, error) for the device and the oracle; errors compared on status, text and row."""
     try:
         exp, eerr = oracle_fn(), None
-    except ol.OracleError as e:
+    except oft.OracleError as e:
         exp, eerr = None, e
     try:
         got, gerr = gpu_fn(), None
@@ -98,8 +92,8 @@ def test_filter_predicate_with_nulls(gpu, w):
     col = random_column(rng, n, w)
     for sel in (0.3, 0.95):
         pred = HostArray.bool_from_numpy(rng.random(n - 3) < sel, rng.random(n - 3) >= 0.2)
-        mask = ol.filter_mask(pred)
-        run_both(lambda: gpu.filter(col, pred), lambda: of.filter(col, mask))
+        mask = oft.filter_mask(pred)
+        run_both(lambda: gpu.filter(col, pred), lambda: oft.filter(col, mask))
 
 
 @pytest.mark.parametrize("w", WIDTHS)
@@ -112,9 +106,9 @@ def test_take_every_width(gpu, w):
     idx = rng.integers(0, min(n, np.iinfo(NP[dt]).max), m).astype(NP[dt])
     iv = rng.random(m) >= 0.15
     ix = HostArray.from_numpy(dt, idx, iv)
-    run_both(lambda: gpu.take(col, ix), lambda: of.take(col, idx, iv, True, dt))
+    run_both(lambda: gpu.take(col, ix), lambda: oft.take_host(col, ix))
     ixn = HostArray.from_numpy(dt, idx)
-    run_both(lambda: gpu.take(col, ixn, True), lambda: of.take(col, idx, None, False, dt, True))
+    run_both(lambda: gpu.take(col, ixn, True), lambda: oft.take_host(col, ixn, True))
 
 
 @pytest.mark.parametrize("dt", INDEX_DTYPES)
@@ -133,13 +127,13 @@ def test_take_index_types_nulls_and_errors(gpu, dt, w, check):
     if info.min < 0:
         idx[rng.integers(0, m, 2)] = -1
     idx = idx.astype(NP[dt])
-    for valid, buf in ((iv, True), (None, False)):
+    for valid in (iv, None):
         ix = HostArray.from_numpy(dt, idx, valid)
-        run_both(lambda: gpu.take(col, ix, check), lambda: of.take(col, idx, valid, buf, dt, check))
+        run_both(lambda: gpu.take(col, ix, check), lambda: oft.take_host(col, ix, check))
     # values without nulls: the take_bits panic cannot occur
     col2 = random_column(rng, n, w, null_p=0.0)
     ix = HostArray.from_numpy(dt, idx, iv)
-    run_both(lambda: gpu.take(col2, ix, check), lambda: of.take(col2, idx, iv, True, dt, check))
+    run_both(lambda: gpu.take(col2, ix, check), lambda: oft.take_host(col2, ix, check))
 
 
 @pytest.mark.parametrize("w", [3, 33, 20, 36])
@@ -155,7 +149,7 @@ def test_take_u64_indices_that_wrap_into_the_buffer(gpu, w):
         idx = np.array([(int(r) + int(c) * ((1 << 64) // tz)) % (1 << 64) for r, c in zip(rng.integers(0, n, 40), rng.integers(1, tz, 40))],
                        np.uint64)
     ix = HostArray.from_numpy(abi.U64, idx)
-    run_both(lambda: gpu.take(col, ix), lambda: of.take(col, idx, None, False, abi.U64))
+    run_both(lambda: gpu.take(col, ix), lambda: oft.take_host(col, ix))
 
 
 @pytest.mark.parametrize("w", [5, 20, 33])
@@ -171,7 +165,7 @@ def test_sliced_columns(gpu, w, bit_offset):
     idx = rng.integers(0, 300, 100).astype(np.uint32)
     iv = rng.random(100) >= 0.2
     ix = HostArray.from_numpy(abi.U32, idx, iv)
-    run_both(lambda: gpu.take(col, ix), lambda: of.take(col, idx, iv, True, abi.U32))
+    run_both(lambda: gpu.take(col, ix), lambda: oft.take_host(col, ix))
 
 
 # ---- the C ABI on raw device buffers: values at any alignment, outputs inside a sentinel-filled allocation --------------
@@ -229,7 +223,7 @@ def test_raw_alignment_and_sentinels(gpu, w, vshift, oshift):
         idd = s.upload(ix).descriptor()
         got = _raw(gpu, col, vshift, oshift, m, lambda a, o: gpu.check(gpu.lib.acu_take_fixed_size_binary(gpu.h, w, C.byref(a), C.byref(idd), abi.U32, 0,
                                                                                                          C.byref(o))))
-    same(got, of.take(col, idx, iv, True, abi.U32))
+    same(got, oft.take_host(col, ix))
 
 
 @pytest.mark.parametrize("w", [2, 4, 8, 16])
@@ -256,7 +250,7 @@ def test_raw_unaligned_native_width_out_of_bounds(gpu, w):
         idd = s.upload(ix).descriptor()
         got = _raw(gpu, col, 1, 3, m, lambda a, o: gpu.check(gpu.lib.acu_take_fixed_size_binary(gpu.h, w, C.byref(a), C.byref(idd), abi.U32, 0,
                                                                                                  C.byref(o))))
-    same(got, of.take(col, idx, iv, True, abi.U32))
+    same(got, oft.take_host(col, ix))
 
 
 # ---- byte positions past 2^32 ------------------------------------------------------------------------------------------
@@ -313,10 +307,10 @@ def test_take_past_one_grid_round_and_lowest_error_row(gpu, w):
     m = int(_round_chunks(gpu, w) * 16 * 1.3) // w + 11
     n = 5000
     vals = rng.integers(0, 256, (n, w), dtype=np.uint8)
-    col = of.column(vals, None)
+    col = FixedSizeBinaryColumn(vals, nulls_of(np.ones(n, bool)))
     idx = rng.integers(0, n, m).astype(np.uint32)
     got = gpu.take(col, HostArray.from_numpy(abi.U32, idx))
-    assert got.length == m and not of.has_buffer(got)
+    assert got.length == m and got.nulls.validity is None
     assert np.array_equal(got.values, vals[idx])
     # failing rows in two rounds: the lower one is reported
     one_round_rows = _round_chunks(gpu, w) * 16 // w
@@ -335,44 +329,37 @@ def test_filter_past_one_grid_round(gpu, w):
     n = int(k / 0.7)
     vals = rng.integers(0, 256, (n, w), dtype=np.uint8)
     mask = rng.random(n) >= 0.2
-    col = of.column(vals, mask)
+    col = FixedSizeBinaryColumn(vals, nulls_of(mask, force=True))
     pred = rng.random(n) < 0.7
     got = gpu_filter(gpu, col, pred)
     assert np.array_equal(got.values, vals[pred])
-    assert np.array_equal(of.valid_mask(got), mask[pred])
+    assert np.array_equal(oft.valid_mask(got), mask[pred])
 
 
 # ---- nesting and the record-batch calls ------------------------------------------------------------------------------
 def test_struct_field(gpu):
     rng = np.random.default_rng(9000)
     f = random_column(rng, 100, 20)
-    st = StructColumn([f, HostArray.from_numpy(abi.I64, rng.integers(0, 9, 100))], tg_nulls(rng.random(100) >= 0.1))
+    st = StructColumn([f, HostArray.from_numpy(abi.I64, rng.integers(0, 9, 100))], nulls_of(rng.random(100) >= 0.1))
     pred = rng.random(100) < 0.5
-    r = gpu_filter(gpu, st, pred)
-    same(r.fields[0], oracle_filter(f, pred))
-    idx = rng.integers(0, 100, 50).astype(np.int32)
-    r = gpu.take(st, HostArray.from_numpy(abi.I32, idx))
-    same(r.fields[0], of.take(f, idx, None, False, abi.I32))
-
-
-def tg_nulls(mask):
-    h = HostArray.from_list(abi.U8, [0 if v else None for v in mask])
-    h.values = np.zeros(0, np.uint8)
-    return h
+    same(gpu_filter(gpu, st, pred), oracle_filter(st, pred))
+    ix = HostArray.from_numpy(abi.I32, rng.integers(0, 100, 50).astype(np.int32))
+    same(gpu.take(st, ix), oft.take_host(st, ix))
 
 
 @pytest.mark.parametrize("w", [0, 7, 20])
 def test_list_child_step(gpu, w):
     rng = np.random.default_rng(9100 + w)
     child = random_column(rng, 60, w, null_p=0.0)
-    child.nulls = HostArray(abi.U8, np.zeros(0, np.uint8), 60, acu.pack_bits(np.ones(60, bool)), 0, 0, 0)  # a NullBuffer without nulls
+    child.nulls = nulls_of(np.ones(60, bool), force=True)  # a NullBuffer without nulls
     offs = np.arange(0, 61, 3, dtype=np.int32)
-    lst = ListColumn(offs, child, tg_nulls(np.ones(20, bool)))
+    lst = ListColumn(offs, child, nulls_of(np.ones(20, bool)))
     pred = np.zeros(20, bool)
     pred[[1, 4, 5]] = True
     r = gpu_filter(gpu, lst, pred)
+    same(r, oracle_filter(lst, pred))
     rows = np.concatenate([np.arange(3 * i, 3 * i + 3) for i in (1, 4, 5)])
-    assert r.child.length == 9 and not of.has_buffer(r.child)  # MutableArrayData: every row, an empty NullBuffer dropped
+    assert r.child.length == 9 and r.child.nulls.validity is None  # MutableArrayData: every row, an empty NullBuffer dropped
     assert np.array_equal(r.child.values, child.values[rows])
 
 
@@ -380,10 +367,11 @@ def test_list_child_step(gpu, w):
 def test_fixed_size_list_null_index(gpu, w, zeros):
     rng = np.random.default_rng(9200 + w)
     child = random_column(rng, 20, w, null_p=0.0)
-    fsl = FixedSizeListColumn(2, child, tg_nulls(np.ones(10, bool)))
+    fsl = FixedSizeListColumn(2, child, nulls_of(np.ones(10, bool)))
     ix = HostArray.from_list(abi.U32, [3, None, 1])
     ix.values[1] = 4
     r = gpu.take(fsl, ix)
+    same(r, oft.take_host(fsl, ix))
     vals = r.child.values
     assert np.array_equal(vals[0:2], child.values[6:8]) and np.array_equal(vals[4:6], child.values[2:4])
     # take_value_indices_from_fixed_size_list appends nulls (value 0) for a null index: W = 16 gathers child row 0 under them
@@ -395,21 +383,21 @@ def test_dense_union_child(gpu):
     a = random_column(rng, 6, 20)
     b = HostArray.from_numpy(abi.I32, np.arange(4, dtype=np.int32))
     u = UnionColumn(abi.UNION_DENSE, [0, 1], [a, b], [0, 1, 0, 0, 1, 0], [0, 0, 1, 2, 1, 5])
-    r = gpu.take(u, HostArray.from_list(abi.U32, [5, 0, 2]))
-    same(r.children[0], of.take(a, np.array([5, 0, 1]), None, False, abi.U32))
+    ix = HostArray.from_list(abi.U32, [5, 0, 2])
+    same(gpu.take(u, ix), oft.take_host(u, ix))
 
 
 def test_run_end_filter_and_take_refusal(gpu):
+    """FixedSizeBinary run values are filtered; take refuses them (the device does not merge their runs)."""
     rng = np.random.default_rng(9400)
     vals = random_column(rng, 4, 20)
     ree = RunEndColumn(np.array([3, 5, 9, 10], np.int32), vals)
     pred = np.array([True, False, False, True, False, True, True, False, False, True])
-    r = gpu.filter_run_end(ree, HostArray.bool_from_numpy(pred))
-    assert list(r.run_ends) == [1, 2, 4, 5]
-    assert r.values.length == 4 and np.array_equal(r.values.values, vals.values)
-    assert np.array_equal(of.valid_mask(r.values), of.valid_mask(vals))
+    run_both(lambda: gpu.filter_run_end(ree, HostArray.bool_from_numpy(pred)), lambda: oracle_filter(ree, pred))
+    ix = HostArray.from_list(abi.U32, [0, 4])
+    run_both(lambda: gpu.take_run_end(ree, ix), lambda: oft.take_host(ree, ix))
     with pytest.raises(acu.ArrowError) as e:
-        gpu.take_run_end(ree, HostArray.from_list(abi.U32, [0, 4]))
+        gpu.take_run_end(ree, ix)
     assert e.value.status == abi.ERR_NOT_YET_IMPLEMENTED
 
 
@@ -420,18 +408,17 @@ def test_record_batches(gpu):
     g = random_column(rng, n, 16)
     p = HostArray.from_numpy(abi.I64, rng.integers(0, 100, n), rng.random(n) >= 0.1)
     offs = np.arange(n + 1, dtype=np.int32)
-    u = Utf8Column(offs, rng.integers(97, 123, n).astype(np.uint8), tg_nulls(rng.random(n) >= 0.1))
+    u = Utf8Column(offs, rng.integers(97, 123, n).astype(np.uint8), nulls_of(rng.random(n) >= 0.1))
     pred = rng.random(n) < 0.4
-    out = gpu.filter_record_batch([p, f, u, g], HostArray.bool_from_numpy(pred))
-    same(out[1], oracle_filter(f, pred))
-    same(out[3], oracle_filter(g, pred))
-    assert out[0].to_list() == gpu.filter(p, HostArray.bool_from_numpy(pred)).to_list()
+    batch = [p, f, u, g]
+    out = gpu.filter_record_batch(batch, HostArray.bool_from_numpy(pred))
+    assert [oft.describe(c) for c in out] == [oft.describe(oracle_filter(c, pred)) for c in batch]
     idx = rng.integers(0, n, 300).astype(np.uint32)
     iv = rng.random(300) >= 0.1
     ix = HostArray.from_numpy(abi.U32, idx, iv)
-    out = gpu.take_record_batch([f, p, g, u], ix)
-    same(out[0], of.take(f, idx, iv, True, abi.U32))
-    same(out[2], of.take(g, idx, iv, True, abi.U32))
+    batch = [f, p, g, u]
+    out = gpu.take_record_batch(batch, ix)
+    assert [oft.describe(c) for c in out] == [oft.describe(oft.take_host(c, ix)) for c in batch]
     with pytest.raises(acu.ArrowError) as e:
         gpu.concat([f, f])
     assert e.value.status == abi.ERR_INVALID_ARGUMENT

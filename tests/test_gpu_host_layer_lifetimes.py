@@ -11,13 +11,9 @@ from acu import _abi as abi
 from acu import (BOOL, DecimalArray, FixedSizeBinaryColumn, FixedSizeListColumn, HostArray, ListColumn, RunEndColumn,
                  Utf8Column, ViewColumn)
 
+from oracle_filter_take import nulls_of
+
 pytestmark = pytest.mark.gpu
-
-
-def nulls_of(mask):
-    h = HostArray.from_list(abi.U8, [0 if m else None for m in mask])
-    h.values = np.zeros(0, np.uint8)
-    return h
 
 
 def utf8(items, dtype=np.int32):

@@ -1,4 +1,4 @@
-"""filter / take of List, LargeList and FixedSizeList columns on the device against tests/oracle_list.py, bit for bit:
+"""filter / take of List, LargeList and FixedSizeList columns on the device against tests/oracle_filter_take.py, bit for bit:
 offsets, child values (the bytes under null rows included) and NullBuffer presence at every level."""
 import numpy as np
 import pytest
@@ -7,17 +7,12 @@ import acu
 from acu import BOOL, DecimalArray, FixedSizeListColumn, HostArray, ListColumn, Utf8Column, ViewColumn
 from acu import _abi as abi
 
-import oracle_list as ol
+import oracle_filter_take as oft
+from oracle_filter_take import nulls_of
 
 pytestmark = pytest.mark.gpu
 
 INDEX_DTYPES = [abi.I8, abi.U8, abi.I16, abi.U16, abi.I32, abi.U32, abi.I64, abi.U64]
-
-
-def nulls_of(mask, bit_offset=0, force=False):
-    h = HostArray.from_list(abi.U8, [0 if v else None for v in mask], force_validity=force, bit_offset=bit_offset)
-    h.values = np.zeros(0, np.uint8)
-    return h
 
 
 def child_of(kind, n, rng, null_p=0.2):
@@ -89,22 +84,22 @@ def rand_idx(rng, n_src, m, dtype=abi.U32, null_p=0.1, oob_under_nulls=True):
 
 def check_filter(gpu, col, pred):
     got = gpu.filter_list(col, pred)
-    exp = ol.filter(col, ol.filter_mask(pred))
-    assert ol.describe(got) == ol.describe(exp)
+    exp = oft.filter(col, oft.filter_mask(pred))
+    assert oft.describe(got) == oft.describe(exp)
     return got
 
 
 def check_take(gpu, col, idx, check_bounds=False):
     got = gpu.take_list(col, idx, check_bounds)
-    exp = ol.take_host(col, idx, check_bounds)
-    assert ol.describe(got) == ol.describe(exp)
+    exp = oft.take_host(col, idx, check_bounds)
+    assert oft.describe(got) == oft.describe(exp)
     return got
 
 
 def check_error(fn, efn):
     with pytest.raises(acu.ArrowError) as g:
         fn()
-    with pytest.raises(ol.OracleError) as e:
+    with pytest.raises(oft.OracleError) as e:
         efn()
     assert (g.value.status, g.value.message) == (e.value.status, e.value.message)
     assert g.value.index == e.value.index
@@ -207,15 +202,15 @@ def test_errors(gpu):
     c = child_of("i32", 8, rng, null_p=0.0)
     col = ListColumn(np.array([0, 3, 6, 8], np.int32), c, nulls_of([True, True, True]))
     pred = HostArray.bool_from_numpy(np.ones(5, bool))
-    check_error(lambda: gpu.filter_list(col, pred), lambda: ol.filter(col, ol.filter_mask(pred)))
+    check_error(lambda: gpu.filter_list(col, pred), lambda: oft.filter(col, oft.filter_mask(pred)))
     for bad in (1000, 3):
         idx = HostArray.from_numpy(abi.U32, [0, bad])
-        e = check_error(lambda: gpu.take_list(col, idx), lambda: ol.take_host(col, idx))
+        e = check_error(lambda: gpu.take_list(col, idx), lambda: oft.take_host(col, idx))
         assert e.message == f"index out of bounds: the len is 4 but the index is {1000 if bad == 1000 else 4}"
-        check_error(lambda: gpu.take_list(col, idx, True), lambda: ol.take_host(col, idx, True))
+        check_error(lambda: gpu.take_list(col, idx, True), lambda: oft.take_host(col, idx, True))
     with_nulls = ListColumn(col.offsets, c, nulls_of([True, False, True]))
     idx = HostArray.from_numpy(abi.I64, [2, 0, 7])
-    e = check_error(lambda: gpu.take_list(with_nulls, idx), lambda: ol.take_host(with_nulls, idx))
+    e = check_error(lambda: gpu.take_list(with_nulls, idx), lambda: oft.take_host(with_nulls, idx))
     assert e.message == "assertion failed: idx < self.bit_len"
     # out-of-bounds values under null indices are never read
     idx = HostArray.from_numpy(abi.U32, [2, 99, 0], [True, False, True])
@@ -234,8 +229,8 @@ def test_skewed_row(gpu):
     pred = HostArray.bool_from_numpy(rng.random(len(lens)) < 0.5)
     pred.values = acu.pack_bits(np.asarray(pred.value_array()) | (np.arange(len(lens)) == 123_457))
     got = gpu.filter_list(col, pred)
-    exp = ol.filter(col, ol.filter_mask(pred))
-    assert ol.describe(got) == ol.describe(exp)
+    exp = oft.filter(col, oft.filter_mask(pred))
+    assert oft.describe(got) == oft.describe(exp)
     idx = HostArray.from_numpy(abi.U32, np.array([123_457, 0, 123_457, 17], np.uint32))
     check_take(gpu, col, idx)
 
@@ -247,7 +242,7 @@ def test_many_rows(gpu):
     n = col.length
     pred = rand_pred(rng, n, 0.3)
     got = gpu.filter_list(col, pred)
-    mask = ol.filter_mask(pred)
+    mask = oft.filter_mask(pred)
     rows = np.nonzero(mask)[0]
     lens = np.diff(col.offsets)[rows]
     assert np.array_equal(np.diff(got.offsets), lens)
@@ -272,7 +267,7 @@ def test_list_offset_overflow(gpu):
     idx = HostArray.from_numpy(abi.U32, np.zeros(2049, np.uint32))
     with pytest.raises(acu.ArrowError) as e:
         gpu.take_list(col, idx)
-    assert e.value.status == abi.ERR_PANIC_OUT_OF_BOUNDS and e.value.message == ol.UNWRAP_NONE
+    assert e.value.status == abi.ERR_PANIC_OUT_OF_BOUNDS and e.value.message == oft.UNWRAP_NONE
     assert e.value.index == 2047  # 2048 rows of 2^20 children end past i32::MAX
 
 
@@ -284,7 +279,7 @@ def test_child_byte_overflow(gpu):
     idx = HostArray.from_numpy(abi.U32, np.zeros(1025, np.uint32))
     with pytest.raises(acu.ArrowError) as e:
         gpu.take_list(col, idx)
-    assert e.value.status == abi.ERR_INVALID_ARGUMENT and e.value.message == "Invalid argument error: " + ol.EXTEND_OVERFLOW
+    assert e.value.status == abi.ERR_INVALID_ARGUMENT and e.value.message == "Invalid argument error: " + oft.EXTEND_OVERFLOW
     assert e.value.index == 1023  # 1024 strings of 2^21 bytes end past i32::MAX
 
 
@@ -300,10 +295,10 @@ def test_fixed_size_list_oob_child_first(gpu):
     c = HostArray.from_numpy(abi.I32, np.arange(9))
     col = FixedSizeListColumn(3, c, nulls_of([True, False, True]))
     idx = HostArray.from_numpy(abi.U32, [0, 5])
-    e = check_error(lambda: gpu.take_list(col, idx), lambda: ol.take_host(col, idx))
+    e = check_error(lambda: gpu.take_list(col, idx), lambda: oft.take_host(col, idx))
     assert e.message == "Out-of-bounds index 15"
     idx = HostArray.from_numpy(abi.U32, [0, 1431655766])  # * 3 = 2 (mod 2^32)
-    e = check_error(lambda: gpu.take_list(col, idx), lambda: ol.take_host(col, idx))
+    e = check_error(lambda: gpu.take_list(col, idx), lambda: oft.take_host(col, idx))
     assert e.message == "assertion failed: idx < self.bit_len"
 
 
@@ -319,5 +314,5 @@ def test_list_and_child_overflow(gpu, wrapped):
     idx = HostArray.from_numpy(abi.U32, np.zeros(2048, np.uint32))
     with pytest.raises(acu.ArrowError) as e:
         gpu.take_list(col, idx)
-    assert e.value.status == abi.ERR_INVALID_ARGUMENT and e.value.message == "Invalid argument error: " + ol.EXTEND_OVERFLOW
+    assert e.value.status == abi.ERR_INVALID_ARGUMENT and e.value.message == "Invalid argument error: " + oft.EXTEND_OVERFLOW
     assert e.value.index == (1 << 30) - 1

@@ -1,5 +1,5 @@
 """The List / LargeList / FixedSizeList kernels of csrc/list.cu where their code paths switch and past one grid-stride
-round, against a vectorised numpy restatement of one list level (checked against tests/oracle_list.py on small cases):
+round, against a vectorised numpy restatement of one list level (checked against tests/oracle_filter_take.py on small cases):
 
   k_list_expand    one thread per 64-bit child word: `base` and `child_end` mid-word and on word boundaries, rows that
                    start and end on words, a word of 64 one-row hops, words crossed by runs of empty rows (the binary
@@ -29,8 +29,8 @@ import acu
 from acu import FixedSizeListColumn, HostArray, ListColumn, Utf8Column, bitmap_bytes, pack_bits
 from acu import _abi as abi
 
-import oracle_list as ol
-from test_gpu_list import nulls_of
+import oracle_filter_take as oft
+from oracle_filter_take import nulls_of
 
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "arrow-rs_b200", "csrc")
 
@@ -96,7 +96,7 @@ def _bounds_error(vals, valid, dtype, n):
     if len(rows) == 0:
         return None
     j = int(rows[0])
-    return ol.OracleError(abi.ERR_COMPUTE, f"Array index out of bounds, cannot get item at index {int(vals[j])} from {n} entries", j)
+    return oft.OracleError(abi.ERR_COMPUTE, f"Array index out of bounds, cannot get item at index {int(vals[j])} from {n} entries", j)
 
 
 def ref_take_list(offsets, list_valid, vals, valid, dtype, check_bounds=False):
@@ -113,7 +113,7 @@ def ref_take_list(offsets, list_valid, vals, valid, dtype, check_bounds=False):
     inb = ix < np.uint64(n)
     oob_rows = np.flatnonzero(v & ~inb)
     if len(oob_rows) and not lv.all():
-        return None, None, None, ol.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, "assertion failed: idx < self.bit_len", int(oob_rows[0]))
+        return None, None, None, oft.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, "assertion failed: idx < self.bit_len", int(oob_rows[0]))
     ixs = np.where(inb, ix, 0).astype(np.int64)
     if n == 0:
         lv, offs = np.ones(1, bool), np.append(offs, offs[-1])  # every row is out of bounds or null
@@ -125,10 +125,10 @@ def ref_take_list(offsets, list_valid, vals, valid, dtype, check_bounds=False):
     ovf = int(ovf_rows[0]) if len(ovf_rows) else None
     if oob is not None and (ovf is None or oob < ovf):
         bad = int(ix[oob])
-        return None, None, None, ol.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS,
+        return None, None, None, oft.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS,
                                                 f"index out of bounds: the len is {n + 1} but the index is {bad + 1 if bad == n else bad}", oob)
     if ovf is not None:
-        return None, None, None, ol.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, ol.UNWRAP_NONE, ovf)
+        return None, None, None, oft.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, oft.UNWRAP_NONE, ovf)
     return np.concatenate([[0], ends]), lens, offs[ixs], None
 
 
@@ -160,11 +160,11 @@ def ref_take_fsl(n, list_valid, child_len, vals, valid, dtype, size, check_bound
     mp, vm, _ = ref_fsl_map(vals, valid, dtype, size)
     bad = np.flatnonzero((mp >= child_len) & (True if vm is None else vm))
     if len(bad):
-        return None, None, ol.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, f"Out-of-bounds index {int(mp[bad[0]])}", int(bad[0]))
+        return None, None, oft.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, f"Out-of-bounds index {int(mp[bad[0]])}", int(bad[0]))
     v = np.ones(len(vals), bool) if valid is None else np.asarray(valid, bool)
     if list_valid is not None and not np.all(list_valid) and (v & (to_index(vals, dtype) >= np.uint64(n))).any():
         j = int(np.flatnonzero(v & (to_index(vals, dtype) >= np.uint64(n)))[0])
-        return None, None, ol.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, "assertion failed: idx < self.bit_len", j)
+        return None, None, oft.OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, "assertion failed: idx < self.bit_len", j)
     return mp, vm, None
 
 
@@ -181,7 +181,7 @@ def _rand_index_values(rng, dtype, n, m):
 
 
 def test_reference_matches_oracle():
-    """The vectorised reference against tests/oracle_list.py on 360 small cases: all three kinds, the eight index dtypes
+    """The vectorised reference against tests/oracle_filter_take.py on 360 small cases: all three kinds, the eight index dtypes
     (negative i8 / i16 / i32 / i64 included), null indices, null lists, sliced lists, short predicates, check_bounds."""
     rng = np.random.default_rng(2024)
     seen = set()
@@ -215,8 +215,8 @@ def test_reference_matches_oracle():
         # filter
         plen = int(rng.integers(0, rows + 1))
         pred = HostArray.bool_from_numpy(rng.random(plen) < rng.random(), rng.random(plen) >= 0.1)
-        mask = ol.filter_mask(pred)
-        exp = ol.filter(col, mask)
+        mask = oft.filter_mask(pred)
+        exp = oft.filter(col, mask)
         cpred, new = ref_filter(offsets, col.size if offsets is None else 0, mask)
         assert np.array_equal(exp.child.value_array(), np.flatnonzero(cpred)), case
         if offsets is not None:
@@ -232,9 +232,9 @@ def test_reference_matches_oracle():
         seen.add(("index nulls", valid is not None and not valid.all()))
         idx_valid = [True] * m if valid is None else list(valid)
         try:
-            got = ol.take(col, list(vals), idx_valid, valid is not None, dtype, cb)
+            got = oft.take(col, list(vals), idx_valid, valid is not None, dtype, cb)
             err = None
-        except ol.OracleError as e:
+        except oft.OracleError as e:
             got, err = None, e
         if kind == abi.FIXED_SIZE_LIST:
             mp, vm, rerr = ref_take_fsl(rows, lmask, child_n, vals, valid, dtype, col.size, cb)
@@ -410,7 +410,7 @@ def check_filter_abi(gpu, kind, offsets, pred, size=0, n_rows=0, valid=None, wha
     finally:
         for p in owned:
             gpu.free(p)
-    mask = ol.filter_mask(pred)
+    mask = oft.filter_mask(pred)
     cpred, new = ref_filter(offsets, size, mask)
     exp_sel = np.flatnonzero(cpred)
     exp_len = int(offsets[len(mask)]) if offsets is not None else len(mask) * size
@@ -669,7 +669,7 @@ def test_row_map_u32_limit(gpu):
     offs = np.array([U32_MAX - 70, U32_MAX - 3, U32_MAX], np.int64)
     idx = HostArray.from_numpy(abi.U32, np.array([1, 0, 1], np.uint32))
     check_take_abi(gpu, abi.LARGE_LIST, offs, idx, abi.U32, child_len=U32_MAX)
-    err = ol.OracleError(abi.ERR_INVALID_ARGUMENT, f"child of {U32_MAX + 1} rows needs a UInt64 row map")
+    err = oft.OracleError(abi.ERR_INVALID_ARGUMENT, f"child of {U32_MAX + 1} rows needs a UInt64 row map")
     for kind, o in ((abi.LARGE_LIST, offs), (abi.LIST, np.array([0, 5, 9], np.int32))):
         owned = []
         try:
@@ -829,7 +829,7 @@ def test_engine_int32_max(gpu):
             v2, ok2 = vals.copy(), valid.copy()
             v2[extra], ok2[extra] = 2, True
             _, _, _, err = ref_take_list(ENGINE_SRC, None, v2, ok2, dtype)
-            assert err.message == ol.UNWRAP_NONE and err.index == extra
+            assert err.message == oft.UNWRAP_NONE and err.index == extra
             expect_error(lambda: abi_take(gpu, desc, HostArray.from_numpy(dtype, v2, ok2), abi.U32, write_map=False), err)
         finally:
             for p in owned:
@@ -871,7 +871,7 @@ def test_engine_error_rows(gpu, check_bounds):
                 _, _, _, err = ref_take_list(ENGINE_SRC, None, vals, valid, dtype, check_bounds)
                 first = oob_at if check_bounds else min(oob_at, ovf_at)
                 assert err is not None and err.index == first
-                assert (err.message == ol.UNWRAP_NONE) == (ovf_at < oob_at and not check_bounds)
+                assert (err.message == oft.UNWRAP_NONE) == (ovf_at < oob_at and not check_bounds)
                 expect_error(lambda: abi_take(gpu, desc, idx, abi.U32, check_bounds, write_map=False), err)
     finally:
         for p in owned:
@@ -905,7 +905,7 @@ def test_e2e_fsl_float32_768(gpu):
     assert np.array_equal(got.nulls.valid_mask(), ivalid & col.nulls.valid_mask()[vals])
     pred = HostArray.bool_from_numpy(rng.random(n) < 0.6)
     got = gpu.filter_list(col, pred)
-    cpred, _ = ref_filter(None, size, ol.filter_mask(pred))
+    cpred, _ = ref_filter(None, size, oft.filter_mask(pred))
     assert_flat(got.child, cvals[cpred], cvalid[cpred], "filter child")
 
 
@@ -949,7 +949,7 @@ def test_e2e_large_list_utf8_filter(gpu):
     col = ListColumn(offs, child, nulls_of(rng.random(len(lens)) >= 0.1))
     pred = HostArray.bool_from_numpy(rng.random(len(lens)) < 0.5, rng.random(len(lens)) >= 0.05)
     got = gpu.filter_list(col, pred)
-    cpred, new = ref_filter(offs, 0, ol.filter_mask(pred))
+    cpred, new = ref_filter(offs, 0, oft.filter_mask(pred))
     assert np.array_equal(got.offsets, new)
     rows = np.flatnonzero(cpred)
     rl = slens[rows]
@@ -995,12 +995,12 @@ def test_presence_oracle():
     filtered that way keeps a NullBuffer without nulls, even where its own plan selects every row. A top-level All
     slices, and every level keeps its NullBuffer."""
     for name, col, pred in presence_cases():
-        mask = ol.filter_mask(pred)
+        mask = oft.filter_mask(pred)
         cpred, _ = ref_filter(col.offsets, 0, mask)
         assert cpred.all() and not mask.all(), name
-        assert levels_present(ol.filter(col, mask)) == [False] * len(levels_present(col)), name
+        assert levels_present(oft.filter(col, mask)) == [False] * len(levels_present(col)), name
         all_pred = np.ones(col.length, bool)
-        assert levels_present(ol.filter(col, all_pred)) == levels_present(col) == [True] * len(levels_present(col)), name
+        assert levels_present(oft.filter(col, all_pred)) == levels_present(col) == [True] * len(levels_present(col)), name
 
 
 @pytest.mark.gpu
@@ -1008,7 +1008,7 @@ def test_presence_filter(gpu):
     """The device follows the same rule at every level (and keeps every NullBuffer under a top-level All)."""
     for name, col, pred in presence_cases():
         got = gpu.filter_list(col, pred)
-        assert ol.describe(got) == ol.describe(ol.filter(col, ol.filter_mask(pred))), name
+        assert oft.describe(got) == oft.describe(oft.filter(col, oft.filter_mask(pred))), name
         assert levels_present(got) == [False] * len(levels_present(col)), name
         got = gpu.filter_list(col, HostArray.bool_from_numpy(np.ones(col.length, bool)))
         assert levels_present(got) == [True] * len(levels_present(col)), name
@@ -1021,5 +1021,5 @@ def test_presence_take(gpu):
     for name, col, _ in presence_cases():
         idx = HostArray.from_numpy(abi.U32, np.arange(col.length)[::-1].copy())
         got = gpu.take_list(col, idx)
-        assert ol.describe(got) == ol.describe(ol.take_host(col, idx)), name
+        assert oft.describe(got) == oft.describe(oft.take_host(col, idx)), name
         assert levels_present(got) == [False] * len(levels_present(col)), name

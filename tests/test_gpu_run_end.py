@@ -1,4 +1,4 @@
-"""filter / take of RunEndEncoded columns on the device against tests/oracle_run_end.py, bit for bit: run ends and their
+"""filter / take of RunEndEncoded columns on the device against tests/oracle_filter_take.py, bit for bit: run ends and their
 type, the values child (the bytes under nulls included), NullBuffer presence, and status plus exact message."""
 import zlib
 
@@ -9,7 +9,8 @@ import acu
 from acu import DecimalArray, HostArray, ListColumn, RunEndColumn, Utf8Column, ViewColumn
 from acu import _abi as abi
 
-import oracle_run_end as ore
+import oracle_filter_take as oft
+from oracle_filter_take import nulls_of
 from run_end_util import check, golden_cases, run_case
 
 pytestmark = pytest.mark.gpu
@@ -17,12 +18,6 @@ pytestmark = pytest.mark.gpu
 INDEX_DTYPES = [abi.I8, abi.U8, abi.I16, abi.U16, abi.I32, abi.U32, abi.I64, abi.U64]
 R_TYPES = [np.int16, np.int32, np.int64]
 RE_THREADS, RE_PER_SM = 256, 8  # csrc/run_end.cu launch constants (pinned by test_run_end_launch_constants.py)
-
-
-def nulls_of(mask):
-    h = HostArray.from_list(abi.U8, [0 if v else None for v in mask])
-    h.values = np.zeros(0, np.uint8)
-    return h
 
 
 def values_of(kind, n, rng, null_p=0.2, distinct=3):
@@ -70,13 +65,13 @@ def ree_of(values, rng, r_dtype=np.int32, mean_run=8):
 def expect_same(run_dev, run_orc):
     try:
         exp = run_orc()
-    except ore.OracleError as e:
+    except oft.OracleError as e:
         with pytest.raises(acu.ArrowError) as got:
             run_dev()
         assert (got.value.status, got.value.message) == (e.status, e.message)
         return
     got = run_dev()
-    assert ore.describe(got) == ore.describe(exp)
+    assert oft.describe(got) == oft.describe(exp)
 
 
 def dev_filter(gpu, col, pred):
@@ -84,7 +79,7 @@ def dev_filter(gpu, col, pred):
 
 
 def orc_filter(col, pred):
-    return lambda: ore.filter(col, ore.ol.filter_mask(pred))
+    return lambda: oft.filter(col, oft.filter_mask(pred))
 
 
 def rand_pred(rng, n, p=0.5, null_p=0.1):
@@ -118,7 +113,7 @@ def test_take_types(gpu, kind, r_dtype):
     for ix in (rng.integers(0, n, 500), np.sort(rng.integers(0, n, 500)), np.sort(rng.integers(0, n, 500))[::-1],
                np.repeat(rng.integers(0, n, 50), 7)):
         idx = HostArray.from_numpy(abi.I64, ix, rng.random(len(ix)) >= 0.1)
-        expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+        expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
 
 
 def test_slices(gpu):
@@ -133,7 +128,7 @@ def test_slices(gpu):
             for pred in (rand_pred(rng, ln), rand_pred(rng, max(ln - 2, 0), p=0.9, null_p=0.0)):
                 expect_same(dev_filter(gpu, s, pred), orc_filter(s, pred))
             idx = HostArray.from_numpy(abi.U32, rng.integers(0, ln, 40))
-            expect_same(lambda: gpu.take_run_end(s, idx), lambda: ore.take(s, idx))
+            expect_same(lambda: gpu.take_run_end(s, idx), lambda: oft.take_host(s, idx))
 
 
 @pytest.mark.parametrize("mean_run", [1, 8, 10**6])
@@ -147,7 +142,7 @@ def test_run_lengths(gpu, mean_run):
                  HostArray.bool_from_numpy(np.ones(col.length, bool))):
         expect_same(dev_filter(gpu, col, pred), orc_filter(col, pred))
     idx = HostArray.from_numpy(abi.U64, rng.integers(0, col.length, 1000))
-    expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+    expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
 
 
 def test_filter_predicate_longer_than_array(gpu):
@@ -163,13 +158,13 @@ def test_take_index_dtypes(gpu, dtype):
     hi = min(col.length, 127)
     raw = rng.integers(0, hi, 300)
     idx = HostArray.from_numpy(dtype, raw, rng.random(300) >= 0.2)
-    expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+    expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
     for check_bounds in (False, True):
         bad = HostArray.from_numpy(dtype, raw, rng.random(300) >= 0.2)
         bad.values[7] = hi + 3 if hi + 3 <= 127 else 127  # valid out-of-bounds value
         if col.length > 127:
             bad.values[7] = 0
-        expect_same(lambda: gpu.take_run_end(col, bad, check_bounds), lambda: ore.take(col, bad, check_bounds))
+        expect_same(lambda: gpu.take_run_end(col, bad, check_bounds), lambda: oft.take_host(col, bad, check_bounds))
 
 
 @pytest.mark.parametrize("check_bounds", [False, True])
@@ -178,10 +173,10 @@ def test_take_null_over_out_of_bounds(gpu, check_bounds):
     col = RunEndColumn(np.array([3, 5, 9], np.int32), HostArray.from_list(abi.I64, [1, None, 3]))
     ok = HostArray.from_list(abi.U32, [0, None, 8, 4])
     ok.values[1] = 2
-    expect_same(lambda: gpu.take_run_end(col, ok, check_bounds), lambda: ore.take(col, ok, check_bounds))
+    expect_same(lambda: gpu.take_run_end(col, ok, check_bounds), lambda: oft.take_host(col, ok, check_bounds))
     bad = HostArray.from_list(abi.U32, [0, None, 8, 4])
     bad.values[1] = 9
-    expect_same(lambda: gpu.take_run_end(col, bad, check_bounds), lambda: ore.take(col, bad, check_bounds))
+    expect_same(lambda: gpu.take_run_end(col, bad, check_bounds), lambda: oft.take_host(col, bad, check_bounds))
 
 
 @pytest.mark.parametrize("dtype", [abi.I8, abi.I32])
@@ -189,7 +184,7 @@ def test_take_null_over_out_of_bounds(gpu, check_bounds):
 def test_take_negative_indices(gpu, dtype, check_bounds):
     col = RunEndColumn(np.array([3, 5, 9], np.int64), HostArray.from_list(abi.I64, [1, 2, 3]))
     idx = HostArray.from_list(dtype, [0, 4, -1, 2])
-    expect_same(lambda: gpu.take_run_end(col, idx, check_bounds), lambda: ore.take(col, idx, check_bounds))
+    expect_same(lambda: gpu.take_run_end(col, idx, check_bounds), lambda: oft.take_host(col, idx, check_bounds))
 
 
 def test_take_merges(gpu):
@@ -199,7 +194,7 @@ def test_take_merges(gpu):
     col = RunEndColumn(np.array([2, 4, 6, 8, 10, 12, 14], np.int32), vals)
     for ix in ([0, 5, 1, 2, 6, 10, 11, 7, 8], [4, 1, 6, 7, 10], [13, 12, 0, 4]):
         idx = HostArray.from_list(abi.U16, ix)
-        expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+        expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
     got = gpu.take_run_end(col, HostArray.from_list(abi.U16, [0, 5, 1, 2, 6, 10, 11, 7, 8]))
     assert [int(x) for x in got.run_ends] == [3, 4, 8, 9]  # 5 5 5 | 7 | null x4 | 7
 
@@ -210,7 +205,7 @@ def test_take_float_bits(gpu):
     v.view(np.uint64)[3] |= 1
     col = RunEndColumn(np.array([1, 2, 3, 4, 5], np.int64), HostArray.from_numpy(abi.F64, v))
     idx = HostArray.from_list(abi.U8, [0, 1, 2, 3, 3, 2, 0, 0])
-    expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+    expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
     assert [int(x) for x in gpu.take_run_end(col, idx).run_ends] == [1, 2, 3, 5, 6, 8]
 
 
@@ -218,19 +213,33 @@ def test_take_int16_unwrap(gpu):
     col = RunEndColumn(np.array([2, 5], np.int16), HostArray.from_list(abi.I8, [1, 2]))
     for m in (32767, 32768, 40000):
         idx = HostArray.from_numpy(abi.U16, np.arange(m) % 5)
-        expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+        expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
 
 
 def test_empty(gpu):
     col = RunEndColumn(np.array([2, 5], np.int32), HostArray.from_list(abi.I8, [1, 2]))
     idx = HostArray.from_numpy(abi.I32, np.zeros(0, np.int32))
-    expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+    expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
     empty = RunEndColumn(np.zeros(0, np.int32), HostArray.from_list(abi.I8, []))
-    expect_same(lambda: gpu.take_run_end(empty, idx), lambda: ore.take(empty, idx))
+    expect_same(lambda: gpu.take_run_end(empty, idx), lambda: oft.take_host(empty, idx))
     one = HostArray.from_numpy(abi.I32, np.zeros(1, np.int32))
-    expect_same(lambda: gpu.take_run_end(empty, one), lambda: ore.take(empty, one))
+    expect_same(lambda: gpu.take_run_end(empty, one), lambda: oft.take_host(empty, one))
     pred = HostArray.bool_from_numpy(np.zeros(0, bool))
     expect_same(dev_filter(gpu, empty, pred), orc_filter(empty, pred))
+
+
+def test_run_end_below_a_level(gpu):
+    """A RunEndEncoded field or list child fails as the oracle says: Context has a RunEndEncoded arm only at the top."""
+    ree = RunEndColumn(np.array([2, 3], np.int32), HostArray.from_list(abi.I32, [1, 2]))
+    st = acu.StructColumn([ree], nulls_of([True] * 3))
+    pred, idx = HostArray.bool_from_numpy(np.array([True, False, True])), HostArray.from_list(abi.U32, [2, 0])
+    for got, exp in ((lambda: gpu.filter(st, pred), lambda: oft.filter(st, oft.filter_mask(pred))),
+                     (lambda: gpu.take(st, idx), lambda: oft.take_host(st, idx))):
+        with pytest.raises(AttributeError) as g:
+            got()
+        with pytest.raises(AttributeError) as e:
+            exp()
+        assert str(g.value) == str(e.value)
 
 
 def test_take_nested_values_refused(gpu):
@@ -239,7 +248,7 @@ def test_take_nested_values_refused(gpu):
     # the refusal stands where take_run builds its comparator: empty indices and the bounds errors come first
     for idx, cb in ((HostArray.from_list(abi.U32, [0, 1]), False), (HostArray.from_numpy(abi.U32, np.zeros(0, np.uint32)), False),
                     (HostArray.from_list(abi.U32, [0, col.length]), False), (HostArray.from_list(abi.U32, [0, col.length]), True)):
-        expect_same(lambda: gpu.take_run_end(col, idx, cb), lambda: ore.take(col, idx, cb))
+        expect_same(lambda: gpu.take_run_end(col, idx, cb), lambda: oft.take_host(col, idx, cb))
 
 
 def _round(gpu):
@@ -266,6 +275,6 @@ def test_take_grid_rounds(gpu, kind):
     ix = np.sort(rng.integers(0, col.length - 1, m))
     ix[-5] = col.length - 1
     idx = HostArray.from_numpy(abi.U32, ix)
-    expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+    expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))
     ix[-2] = col.length  # out of bounds only in the last round
-    expect_same(lambda: gpu.take_run_end(col, idx), lambda: ore.take(col, idx))
+    expect_same(lambda: gpu.take_run_end(col, idx), lambda: oft.take_host(col, idx))

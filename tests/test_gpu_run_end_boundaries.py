@@ -1,6 +1,6 @@
 """The RunEndEncoded kernels of csrc/run_end.cu where their code paths switch, past one grid-stride round and past 2^32
 logical rows, against a vectorised numpy restatement of filter_run_end_array (filter.rs:628-677) and take_run
-(take.rs:948-995), itself checked against tests/oracle_run_end.py on small cases:
+(take.rs:948-995), itself checked against tests/oracle_filter_take.py on small cases:
 
   k_ree_take_map    one thread per index, grid-stride: the largest index (warp butterfly, then atomicMax from each
                     warp's lane 0) with a single out-of-bounds value at every lane 0-31 of an even and an odd warp, in
@@ -42,10 +42,9 @@ import acu
 from acu import BOOL, DecimalArray, HostArray, ListColumn, RunEndColumn, Utf8Column, ViewColumn
 from acu import _abi as abi
 
-import oracle_list as ol
-import oracle_run_end as ore
-from oracle_list import OracleError
-from test_gpu_list_boundaries import SIGNED, nulls_of, ref_strategy, to_index
+import oracle_filter_take as oft
+from oracle_filter_take import OracleError, nulls_of
+from test_gpu_list_boundaries import SIGNED, ref_strategy, to_index
 from test_gpu_run_end import RE_PER_SM, RE_THREADS, values_of
 
 CSRC = os.path.join(os.path.dirname(os.path.abspath(__file__)), "..", "arrow-rs_b200", "csrc")
@@ -55,7 +54,7 @@ TILE_WORDS = TILE_ROWS // 64
 INDEX_DTYPES = [abi.I8, abi.U8, abi.I16, abi.U16, abi.I32, abi.U32, abi.I64, abi.U64]
 R_TYPES = [np.int16, np.int32, np.int64]
 NAMES = {abi.I8: "i8", abi.U8: "u8", abi.I16: "i16", abi.U16: "u16", abi.I32: "i32", abi.U32: "u32", abi.I64: "i64", abi.U64: "u64"}
-SMALL = 4096           # values children up to this many rows are built by oracle_list, larger ones by a numpy gather
+SMALL = 4096           # values children up to this many rows are built by the oracle, larger ones by a numpy gather
 
 
 # ---- 1. the vectorised reference ------------------------------------------------------------------------------------
@@ -104,18 +103,18 @@ def gather(v, rows, keep_nulls=False):
 
 
 def ref_filter(col, mask):
-    """filter(col, predicate) with mask = oracle_list.filter_mask(predicate), as a RunEndColumn."""
+    """filter(col, predicate) with mask = oracle_filter_take.filter_mask(predicate), as a RunEndColumn."""
     mask = np.asarray(mask, bool)
     how, ends, rows = ref_filter_runs(col.run_ends, col.offset, col.length, len(mask), int(mask.sum()), mask_rank(mask))
     if how == "none":
-        return ore.empty(col)
+        return oft.empty_run_end(col)
     if how == "all":
         return col.slice(0, len(mask))
     s, e = physical_range(col.run_ends, col.offset, col.length)
     if e - s + 1 <= SMALL or not plain(col.values):
         keep = np.zeros(e - s + 1, bool)
         keep[rows - s] = True
-        values = ol.filter(acu.slice_column(col.values, s, e - s + 1), keep)
+        values = oft.filter(acu.slice_column(col.values, s, e - s + 1), keep)
     else:
         values = gather(col.values, rows, keep_nulls=len(rows) == e - s + 1)
     return RunEndColumn(ends, values, 0, int(ends[-1]))
@@ -125,7 +124,7 @@ def keys_of(v):
     """make_comparator classes of the physical values: equal keys iff is_eq (nulls one class, -1); None for nested."""
     if isinstance(v, (ListColumn, acu.FixedSizeListColumn, RunEndColumn)):
         return None
-    vm = ol.valid_mask(v)
+    vm = oft.valid_mask(v)
     if isinstance(v, (Utf8Column, ViewColumn)):
         items = [acu.column_value(v, i) if vm[i] else b"" for i in range(v.length)]  # views under nulls may be garbage
         ids = {}
@@ -141,7 +140,7 @@ def keys_of(v):
 
 def ref_bounds(n, vals, valid, dtype):
     """take's check_bounds (take.rs:167-209): skipped where the length exceeds the index type; the first bad row."""
-    if n > ore.INDEX_MAX[dtype]:
+    if n > oft.INDEX_MAX[dtype]:
         return
     allv = valid is None or bool(np.all(valid))
     raw = np.asarray(vals).astype(np.int64 if dtype in SIGNED else np.uint64)
@@ -167,9 +166,9 @@ def ref_take_runs(ends, offset, length, vals, valid, dtype, check_bounds, key):
         raise OracleError(abi.ERR_INVALID_ARGUMENT, f"Logical index {mx} is out of bounds for RunArray of length {length}")
     phys = np.searchsorted(np.asarray(ends).astype(np.int64), ix.astype(np.int64) + offset, "right")
     if key is None:
-        raise OracleError(abi.ERR_NOT_YET_IMPLEMENTED, "Not yet implemented: " + ore.NESTED_TEXT)
-    if m > ore.R_MAX[np.asarray(ends).itemsize]:
-        raise OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, ore.UNWRAP_NONE)
+        raise OracleError(abi.ERR_NOT_YET_IMPLEMENTED, "Not yet implemented: " + oft.NESTED_TEXT)
+    if m > oft.R_MAX[np.asarray(ends).itemsize]:
+        raise OracleError(abi.ERR_PANIC_OUT_OF_BOUNDS, oft.UNWRAP_NONE)
     k = key[phys]
     new = np.append(np.flatnonzero((phys[1:] != phys[:-1]) & (k[1:] != k[:-1])) + 1, m)
     return new.astype(np.asarray(ends).dtype), phys[new - 1]
@@ -180,10 +179,10 @@ def ref_take(col, idx, check_bounds=False):
     valid = idx.valid_mask() if idx.validity is not None else None
     ends, rows = ref_take_runs(col.run_ends, col.offset, col.length, idx.value_array(), valid, idx.dtype, check_bounds, keys_of(col.values))
     if ends is None:
-        return ore.empty(col)
+        return oft.empty_run_end(col)
     wide = idx.dtype in (abi.I64, abi.U64)
     if len(rows) <= SMALL or not plain(col.values):
-        values = ol.take(col.values, [int(r) for r in rows], [True] * len(rows), False, abi.U64 if wide else abi.U32)
+        values = oft.take(col.values, [int(r) for r in rows], [True] * len(rows), False, abi.U64 if wide else abi.U32)
     else:
         values = gather(col.values, rows)
     return RunEndColumn(ends, values, 0, idx.length)
@@ -199,7 +198,7 @@ def assert_same(got, exp, what=""):
         assert np.array_equal(np.asarray(g.values[:g.length]).view(np.uint8), np.asarray(e.values[:e.length]).view(np.uint8)), what
         assert np.array_equal(g.valid_mask(), e.valid_mask()), what
     else:
-        assert ol.describe(g) == ol.describe(e), what
+        assert oft.describe(g) == oft.describe(e), what
 
 
 def expect(run_dev, run_ref, what=""):
@@ -216,7 +215,7 @@ def expect(run_dev, run_ref, what=""):
 
 
 def check_filter(gpu, col, pred, what=""):
-    return expect(lambda: gpu.filter_run_end(col, pred), lambda: ref_filter(col, ol.filter_mask(pred)), what)
+    return expect(lambda: gpu.filter_run_end(col, pred), lambda: ref_filter(col, oft.filter_mask(pred)), what)
 
 
 def check_take(gpu, col, idx, check_bounds=False, what=""):
@@ -242,7 +241,7 @@ def _rand_indices(rng, dtype, n, m):
 
 
 def test_reference_matches_oracle():
-    """The reference against tests/oracle_run_end.py on 400 small random cases: every run-end type and value kind, slices,
+    """The reference against tests/oracle_filter_take.py on 400 small random cases: every run-end type and value kind, slices,
     short and null predicates, all eight index dtypes with nulls, negative and out-of-bounds values, check_bounds."""
     rng = np.random.default_rng(4242)
     kinds = ["i8", "i32", "i64", "f32", "f64", "bool", "dec128", "utf8", "lbin", "view", "list"]
@@ -253,13 +252,13 @@ def test_reference_matches_oracle():
         plen = col.length if rng.random() < 0.5 else int(rng.integers(0, col.length + 2))
         p = float(rng.choice([0.0, 0.05, 0.5, 0.95, 1.0]))
         pred = HostArray.bool_from_numpy(rng.random(plen) < p, rng.random(plen) >= 0.1 if rng.random() < 0.5 else None)
-        mask = ol.filter_mask(pred)
-        err = _same_as_oracle(lambda: ref_filter(col, mask), lambda: ore.filter(col, mask), case)
+        mask = oft.filter_mask(pred)
+        err = _same_as_oracle(lambda: ref_filter(col, mask), lambda: oft.filter(col, mask), case)
         seen.add(("filter error",) if err else ("filter", col.offset > 0, 0 < plen < col.length))
         dtype = INDEX_DTYPES[case % 8]
         idx = _rand_indices(rng, dtype, col.length, int(rng.integers(0, 30)))
         cb = case % 3 == 0
-        err = _same_as_oracle(lambda: ref_take(col, idx, cb), lambda: ore.take(col, idx, cb), case)
+        err = _same_as_oracle(lambda: ref_take(col, idx, cb), lambda: oft.take_host(col, idx, cb), case)
         seen.add(("take error", err.message.split(" ")[0]) if err else ("take", kind))
     for fact in [("filter error",), ("filter", True, True), ("filter", False, False), ("take error", "Compute"),
                  ("take error", "Invalid"), ("take error", "Not")] + [("take", k) for k in kinds[:-1]]:
@@ -275,7 +274,7 @@ def _same_as_oracle(run_ref, run_orc, case):
             run_ref()
         assert (g.value.status, g.value.message) == (e.status, e.message), case
         return e
-    assert ore.describe(run_ref()) == ore.describe(exp), case
+    assert oft.describe(run_ref()) == oft.describe(exp), case
     return None
 
 
@@ -399,7 +398,7 @@ def test_take_offsets_past_2_32(gpu, top, dtype):
     rows of every run in reach of the index type."""
     rng = np.random.default_rng(zlib.crc32(f"offsets {top} {dtype}".encode()))
     col = huge_column(rng, top)
-    imax = ore.INDEX_MAX[dtype]
+    imax = oft.INDEX_MAX[dtype]
     for off in (2**32, 2**32 + 1, 2**32 + 150, 2**40 + 3):
         if off >= top:
             continue

@@ -1,4 +1,4 @@
-"""filter / take of Struct, sparse Union and dense Union columns on the device against tests/oracle_union.py, bit for bit:
+"""filter / take of Struct, sparse Union and dense Union columns on the device against tests/oracle_filter_take.py, bit for bit:
 type ids, offsets, every child buffer (the bytes under null rows included), NullBuffer presence and error status / text /
 index. Every case uses a fixed seed. The partition's tile, warp and grid-round boundaries are sized from union.cu's
 launch constants (checked against the source by test_union_launch_constants.py) and compared with a vectorised numpy
@@ -10,8 +10,8 @@ import acu
 from acu import BOOL, DecimalArray, HostArray, ListColumn, StructColumn, UnionColumn, Utf8Column, ViewColumn
 from acu import _abi as abi
 
-import oracle_list as ol
-import oracle_union as ou
+import oracle_filter_take as oft
+from oracle_filter_take import nulls_of
 import union_util as uu
 
 pytestmark = pytest.mark.gpu
@@ -21,12 +21,6 @@ UN_TILE_ROWS = 4096
 UN_PER_SM = 8
 INDEX_DTYPES = [abi.I8, abi.U8, abi.I16, abi.U16, abi.I32, abi.U32, abi.I64, abi.U64]
 DENSE, SPARSE = abi.UNION_DENSE, abi.UNION_SPARSE
-
-
-def nulls_of(mask, bit_offset=0, force=False):
-    h = HostArray.from_list(abi.U8, [0 if v else None for v in mask], force_validity=force, bit_offset=bit_offset)
-    h.values = np.zeros(0, np.uint8)
-    return h
 
 
 def child_of(kind, n, rng, null_p=0.2):
@@ -94,25 +88,25 @@ def rand_idx(rng, n_src, m, dtype=abi.U32, null_p=0.1):
 def _run(fn):
     try:
         return fn(), None
-    except (acu.ArrowError, ou.OracleError) as e:
+    except (acu.ArrowError, oft.OracleError) as e:
         return None, (e.status, e.message, e.index)
 
 
 def check_filter(gpu, col, pred):
-    exp, eerr = _run(lambda: ou.filter(col, ol.filter_mask(pred)))
+    exp, eerr = _run(lambda: oft.filter(col, oft.filter_mask(pred)))
     got, gerr = _run(lambda: gpu.filter(col, pred))
     assert gerr == eerr
     if eerr is None:
-        assert ou.describe(got) == ou.describe(exp)
+        assert oft.describe(got) == oft.describe(exp)
     return got
 
 
 def check_take(gpu, col, idx, check_bounds=False):
-    exp, eerr = _run(lambda: ou.take_host(col, idx, check_bounds))
+    exp, eerr = _run(lambda: oft.take_host(col, idx, check_bounds))
     got, gerr = _run(lambda: gpu.take(col, idx, check_bounds))
     assert gerr == eerr
     if eerr is None:
-        assert ou.describe(got) == ou.describe(exp)
+        assert oft.describe(got) == oft.describe(exp)
     return got, gerr
 
 
@@ -125,8 +119,8 @@ def test_golden(gpu, i):
     case = CASES[i]
     got = uu.run_case(case, gpu.filter, gpu.take)
     uu.check(case, got)
-    exp = uu.run_case(case, lambda c, p: ou.filter(c, ol.filter_mask(p)), ou.take_host)
-    assert ou.describe(got) == ou.describe(exp)
+    exp = uu.run_case(case, lambda c, p: oft.filter(c, oft.filter_mask(p)), oft.take_host)
+    assert oft.describe(got) == oft.describe(exp)
 
 
 # ---- dense partition: field counts, ids, distributions -------------------------------------------------------------------
@@ -254,7 +248,7 @@ def test_null_out_of_bounds_index_fails_union_validation(gpu):
         idx = HostArray.from_list(abi.U32, [1, None, 2])
         idx.values[1] = 1000
         _, err = check_take(gpu, col, idx)
-        assert err[0] == abi.ERR_INVALID_ARGUMENT and err[1].endswith(ou.UNION_TYPE_IDS)
+        assert err[0] == abi.ERR_INVALID_ARGUMENT and err[1].endswith(oft.UNION_TYPE_IDS)
         col0 = (dense_union if mode == DENSE else sparse_union)(rng, [0, 7], 50, ["i64", "utf8"])
         check_take(gpu, col0, idx)  # type id 0 is a field: no error
 
@@ -269,7 +263,7 @@ def test_child_error_is_reported_ahead_of_the_validation(gpu):
     # a union whose ids do not include 0: the validation error
     col2 = UnionColumn(DENSE, [5], [HostArray.from_list(abi.I64, [1, 2])], [5, 5], [0, 1])
     _, err = check_take(gpu, col2, idx)
-    assert err[1].endswith(ou.UNION_TYPE_IDS)
+    assert err[1].endswith(oft.UNION_TYPE_IDS)
 
 
 def test_struct_validity_reads(gpu):

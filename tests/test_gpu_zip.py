@@ -14,7 +14,7 @@ from acu import _abi as abi
 
 import oracle_zip as oz
 import zip_util as zu
-from oracle_list import OracleError
+from oracle_filter_take import OracleError
 
 pytestmark = pytest.mark.gpu
 

@@ -8,7 +8,7 @@ from acu import _abi as abi
 
 import oracle_zip as oz
 import zip_util as zu
-from oracle_list import EXTEND_OVERFLOW, OracleError
+from oracle_filter_take import EXTEND_OVERFLOW, OracleError
 
 CASES = zu.golden_cases()
 

@@ -7,7 +7,8 @@ import numpy as np
 from acu import BOOL, HostArray, StructColumn, UnionColumn, Utf8Column
 from acu import _abi as abi
 
-import oracle_union as ou
+import oracle_filter_take as oft
+from oracle_filter_take import nulls_of
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "union_vectors.json")
 DTYPES = {"i32": abi.I32, "u32": abi.U32, "i64": abi.I64, "f64": abi.F64, "u8": abi.U8, "u64": abi.U64}
@@ -16,12 +17,6 @@ DTYPES = {"i32": abi.I32, "u32": abi.U32, "i64": abi.I64, "f64": abi.F64, "u8": 
 def golden_cases():
     with open(GOLDEN) as f:
         return json.load(f)
-
-
-def nulls_of(mask, force=False):
-    h = HostArray.from_list(abi.U8, [0 if v else None for v in mask], force_validity=force)
-    h.values = np.zeros(0, np.uint8)
-    return h
 
 
 def build(d):
@@ -64,7 +59,7 @@ def _plain(x):
 def check(case, got):
     name = case["name"]
     if "expect" in case:
-        assert _plain(ou.to_pylist(got)) == case["expect"], name
+        assert _plain(oft.to_pylist(got)) == case["expect"], name
     if "expect_len" in case:
         assert got.length == case["expect_len"], name
     if "expect_type_ids" in case:
@@ -74,9 +69,9 @@ def check(case, got):
     if "expect_children" in case:
         for c, exp in zip(got.children, case["expect_children"]):
             if exp is not None:
-                assert _plain(ou.to_pylist(c)) == exp, name
+                assert _plain(oft.to_pylist(c)) == exp, name
     if "expect_fields" in case:
-        assert [_plain(ou.to_pylist(f)) for f in got.fields] == case["expect_fields"], name
+        assert [_plain(oft.to_pylist(f)) for f in got.fields] == case["expect_fields"], name
     if "expect_nulls" in case:
         exp = case["expect_nulls"]
         assert (got.nulls.validity is None) == (exp is None), name
